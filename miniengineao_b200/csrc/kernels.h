@@ -7,18 +7,6 @@
 // atlas padding values itself (see render_ao.cu).
 #pragma once
 
-// Build switch: drop the per-pixel range test of the final division in the packed upsample path when the host has proved
-// it redundant from the two tolerances (blur_upsample.cu, bilateral2).  Shared by the kernel and the planner.  Off by default:
-// it only affects the MEAO_UPS_V2=0 form of that phase.
-#ifndef MEAO_UPS_STATIC_GUARD
-#define MEAO_UPS_STATIC_GUARD 0
-#endif
-// Build switch: the restructured bilateral-upsample phase (blur_upsample.cu, "phase-4 restructure"); it relies on the same
-// host-side proof as MEAO_UPS_STATIC_GUARD, so the planner applies the tighter tolerance bounds whenever either is on.
-#ifndef MEAO_UPS_V2
-#define MEAO_UPS_V2 1
-#endif
-
 #ifdef MEAO_EMULATE              // tests/emu only (see common.cuh)
 #include "cuda_emu.h"
 #else
@@ -117,12 +105,17 @@ struct UpsampleArgs {
     int out_vec_ok;         // out is 8B aligned and out_pitch % 8 == 0
     int hiw, hih;
     float noise_filter_strength, step_size, blur_tolerance, upsample_tolerance;
-    int fast_div_ok;        // upsample_tolerance and noise_filter_strength are positive normals in [2^-60, 2^60)
-                            // (built with MEAO_UPS_STATIC_GUARD: additionally tol >= 2^-55 and 2^-52 <= nfs < 2^59, see blur_upsample.cu)
+    int fast_div_ok;        // upsample_fast_div_ok(upsample_tolerance, noise_filter_strength); 0: every pixel takes the IEEE path
     int row0, row1;         // output rows (hi level) to produce
     uint32_t *tile_ctr;     // [0] next tile, [1] CTAs that have run out of tiles: device words owned by (context, level), zero between launches
     int tiles_x, tiles_y;   // tile grid (filled by launch_blur_upsample)
 };
+// The tolerances for which the upsample's fast divisions are proven exact: 2^-55 <= tol < 2^60 and 2^-52 <= nfs < 2^58.
+// Within them the final division needs no per-pixel range test (the proof is at bilateral2 in blur_upsample.cu).
+inline bool upsample_fast_div_ok(float tol, float nfs)
+{
+    return tol >= 2.7755575615628914e-17f && tol < 1152921504606846976.0f && nfs >= 2.220446049250313e-16f && nfs < 288230376151711744.0f;
+}
 // main_premin / main_premin_blendout (COMBINE_LOWER_RESOLUTIONS): the same arguments plus LoResAO2 = HighQuality<lo>
 struct UpsamplePreminArgs { UpsampleArgs base; const uint8_t *lo_ao2; int lo_a2pitch; };
 // lo_ao2 == nullptr: kernels main / main_blendout; otherwise the premin kernels (lo_ao2_map = its TMA descriptor).

@@ -517,15 +517,7 @@ int record_upsample(MeaoCtx *c, int lo, void *ao_out, cudaStream_t s)
     a.step_size = c->plan.step_size[lo];
     a.blur_tolerance = c->plan.blur_tolerance[lo];
     a.upsample_tolerance = c->plan.upsample_tolerance[lo];
-    {
-        auto safe = [](float x) { return x >= 8.673617379884035e-19f && x < 1152921504606846976.0f; };
-        a.fast_div_ok = safe(a.upsample_tolerance) && safe(a.noise_filter_strength);
-#if MEAO_UPS_STATIC_GUARD || MEAO_UPS_V2
-        // 2^-55, 2^-52, 2^59: with these bounds total / num of the final division are provably inside the fast-division range
-        a.fast_div_ok = a.fast_div_ok && a.upsample_tolerance >= 2.7755575615628914e-17f &&
-                        a.noise_filter_strength >= 2.220446049250313e-16f && a.noise_filter_strength < 288230376151711744.0f;
-#endif
-    }
+    a.fast_div_ok = upsample_fast_div_ok(a.upsample_tolerance, a.noise_filter_strength);
     a.row0 = c->need_c[hi].lo; a.row1 = c->need_c[hi].hi;
     a.tile_ctr = c->tile_ctr + 2 * (lo - 1);
     const uint8_t *lo_ao2 = hq_level(c, lo) ? c->hq[lo] : nullptr;                   // kernels main_premin / main_premin_blendout

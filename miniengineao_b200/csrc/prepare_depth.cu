@@ -30,7 +30,7 @@ __device__ __forceinline__ float linearize(float depth, float zbx, float zby)
     return dist;
 }
 
-// Eight pixels at once (MEAO_PACKED_RCP): the mad of DS1:40 is formed directly in negated form, nt = fma(-zbx, d, -zby) = -t
+// Eight pixels at once: the mad of DS1:40 is formed directly in negated form, nt = fma(-zbx, d, -zby) = -t
 // exactly (round-to-nearest is sign-symmetric), all eight range tests feed ONE branch, and the reciprocals run in pairs
 // (rcp2_fast_neg).  If any element is out of range (inf / NaN / zero / denormal / negative) the group takes the plain
 // per-element path of linearize() -- which recomputes t itself, so signed zeros behave exactly as before.
@@ -138,12 +138,7 @@ __global__ void __launch_bounds__(kPrepThreads) prepare_depth_kernel(const Prepa
         if (!rowok[p]) continue;
         const int y = ybase + warp + 8 * p;
         float d[8];
-#if MEAO_PACKED_RCP
         linearize8<RAW, REVERSED>(v[p], a.zbx, a.zby, d);
-#else
-#pragma unroll
-        for (int e = 0; e < 8; e++) d[e] = linearize<RAW, REVERSED>(v[p][e], a.zbx, a.zby);
-#endif
 
         __half *lin = a.lin + (size_t)y * a.lin_pitch + x;
         if (full) {

@@ -32,9 +32,6 @@ namespace meao {
 
 namespace {
 
-#ifndef MEAO_REN_THREADS
-#define MEAO_REN_THREADS 256
-#endif
 constexpr int kTW = 64;                     // outputs per CTA: 64 x TH, TH = 32 (least apron overhead), 16 or 8 for the latency-bound coarse
                                             // levels (kernels.h kRenderTileHs)
 // MODE 0 (main_interleaved): apron 4 slice texels x stride 4 = 16; MODE 1 (main, wide): apron 4 taps x stride 2 = 8
@@ -47,7 +44,7 @@ template <int MODE, int TH> struct Geo {
 #ifndef MEAO_REN_MINB
 #define MEAO_REN_MINB 6
 #endif
-constexpr int kThreads = MEAO_REN_THREADS;
+constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
 static_assert(Geo<0, 32>::kSW == kRenderBoxW && Geo<1, 32>::kSW == kRenderWideBoxW, "TMA box mismatch");
 static_assert(Geo<0, 32>::kSH == render_box_h(32, false) && Geo<1, 8>::kSH == render_box_h(8, true), "TMA box mismatch");
@@ -63,21 +60,10 @@ __device__ __forceinline__ float2 pair_eval2(float2 S1, float2 S2, float2 inv_ra
     const float2 d2 = ffma2(S2, inv_range, neg_front);             // REN:66
     const float p1x = __saturatef(__fmul_rn(rf, d1.x)), p1y = __saturatef(__fmul_rn(rf, d1.y));   // REN:68
     const float p2x = __saturatef(__fmul_rn(rf, d2.x)), p2y = __saturatef(__fmul_rn(rf, d2.y));   // REN:69
-    // clamp(d, p, 1): either max(saturate(d), p) (FADD.SAT on the FMA pipe + FMNMX) or the literal
+    // clamp(d, p, 1): c1 as max(saturate(d), p) (FADD.SAT on the FMA pipe + FMNMX), c2 as the literal
     // min(max(d, p), 1) (two FMNMX on the ALU pipe); both are exact, the mix balances the two pipes
-#ifndef MEAO_REN_CLAMP_MODE
-#define MEAO_REN_CLAMP_MODE 1
-#endif
-#if MEAO_REN_CLAMP_MODE == 0
-    const float2 c1 = make_float2(fmaxf(__saturatef(d1.x), p2x), fmaxf(__saturatef(d1.y), p2y));
-    const float2 c2 = make_float2(fmaxf(__saturatef(d2.x), p1x), fmaxf(__saturatef(d2.y), p1y));
-#elif MEAO_REN_CLAMP_MODE == 1
     const float2 c1 = make_float2(fmaxf(__saturatef(d1.x), p2x), fmaxf(__saturatef(d1.y), p2y));
     const float2 c2 = make_float2(fminf(fmaxf(d2.x, p1x), 1.0f), fminf(fmaxf(d2.y, p1y), 1.0f));
-#else
-    const float2 c1 = make_float2(fminf(fmaxf(d1.x, p2x), 1.0f), fminf(fmaxf(d1.y, p2y), 1.0f));
-    const float2 c2 = make_float2(fminf(fmaxf(d2.x, p1x), 1.0f), fminf(fmaxf(d2.y, p1y), 1.0f));
-#endif
     const float2 sum = fadd2(c1, c2);
     return make_float2(__saturatef(fmaf(-p1x, p2x, sum.x)), __saturatef(fmaf(-p1y, p2y, sum.y)));   // REN:71-74
 }
@@ -206,16 +192,12 @@ render_ao_kernel(const __grid_constant__ CUtensorMap low_map, const RenderArgs a
         if (oy < a.row0 || oy >= a.row1 || ox >= a.lw) continue;
         const float *c = tile + (row + kAp) * kSW + (px + kAp);
         const float2 ctr = *reinterpret_cast<const float2 *>(c);
-#if MEAO_PACKED_RCP
         float2 inv;                                                            // REN:140, both pixels under one range test
         {
             const float2 nctr = fmul2(ctr, make_float2(-1.0f, -1.0f));
             if (in_safe_range_neg(nctr.x) & in_safe_range_neg(nctr.y)) inv = rcp2_fast_neg(nctr);
             else inv = make_float2(1.0f / ctr.x, 1.0f / ctr.y);
         }
-#else
-        const float2 inv = make_float2(rcp_ieee(ctr.x), rcp_ieee(ctr.y));      // REN:140
-#endif
         float2 ao = make_float2(0.0f, 0.0f);                                   // REN:142
         if (!EXH) {
             // REN:162-168 -- the 36-sample checker pattern, in call order

@@ -13,34 +13,31 @@ KERNELS = ["prepare_depth.cu", "render_ao.cu", "blur_upsample.cu", "debug_view.c
 FLAGS = ["-std=c++17", "-O1", "-ffp-contract=off", "-fPIC", "-DMEAO_EMULATE", "-I", HERE, "-Wno-unknown-pragmas", "-Wno-unused-function"]
 
 
-def is_stale(lib: str = LIB) -> bool:
-    if not os.path.exists(lib):
+def is_stale() -> bool:
+    if not os.path.exists(LIB):
         return True
-    t = os.path.getmtime(lib)
+    t = os.path.getmtime(LIB)
     deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(HERE, f) for f in os.listdir(HERE) if f.endswith((".h", ".cpp", ".py"))]
     return any(os.path.getmtime(d) > t for d in deps)
 
 
-def build(force: bool = False, defs: list[str] | None = None) -> str:
-    """defs: extra -D switches (e.g. ["-DMEAO_UPS_STATIC_GUARD=1"]) -> a separately named library."""
-    lib = LIB if not defs else os.path.join(HERE, "libmeao_emu_" + "_".join(d.replace("-D", "").replace("=", "") for d in defs) + ".so")
-    if not force and not is_stale(lib):
-        return lib
+def build(force: bool = False) -> str:
+    if not force and not is_stale():
+        return LIB
     objs = []
-    tag = os.path.basename(lib)[:-3]
     for src, lang in [(os.path.join(HERE, "emu_runtime.cpp"), []), (os.path.join(HERE, "emu_driver.cpp"), [])] + \
                      [(os.path.join(CSRC, k), ["-x", "c++"]) for k in KERNELS]:
-        obj = os.path.join(HERE, f"{tag}_{os.path.basename(src)}.o")
-        cmd = ["g++"] + FLAGS + (defs or []) + lang + ["-c", src, "-o", obj]
+        obj = os.path.join(HERE, f"libmeao_emu_{os.path.basename(src)}.o")
+        cmd = ["g++"] + FLAGS + lang + ["-c", src, "-o", obj]
         p = subprocess.run(cmd, capture_output=True, text=True)
         if p.returncode != 0:
             sys.stderr.write(p.stdout + p.stderr)
             raise RuntimeError(f"emulator build failed: {os.path.basename(src)}")
         objs.append(obj)
-    subprocess.check_call(["g++", "-shared", "-o", lib] + objs)
+    subprocess.check_call(["g++", "-shared", "-o", LIB] + objs)
     for o in objs:
         os.remove(o)
-    return lib
+    return LIB
 
 
 if __name__ == "__main__":

@@ -15,13 +15,13 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 import build_emu  # noqa: E402
 
-_libs: dict[str, C.CDLL] = {}
+_lib: C.CDLL | None = None
 
 
-def lib(defs: tuple[str, ...] = ()) -> C.CDLL:
-    key = " ".join(defs)
-    if key not in _libs:
-        l = C.CDLL(build_emu.build(defs=list(defs) or None))
+def lib() -> C.CDLL:
+    global _lib
+    if _lib is None:
+        l = C.CDLL(build_emu.build())
         l.emu_create.restype = C.c_void_p
         l.emu_create.argtypes = [C.c_int, C.c_int]
         l.emu_destroy.argtypes = [C.c_void_p]
@@ -42,8 +42,8 @@ def lib(defs: tuple[str, ...] = ()) -> C.CDLL:
         l.emu_band_flags.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         l.emu_composite.argtypes = [C.c_void_p, C.c_void_p, C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_int]
         l.emu_composite_debug.argtypes = [C.c_void_p, C.c_void_p, C.c_longlong, C.c_int]
-        _libs[key] = l
-    return _libs[key]
+        _lib = l
+    return _lib
 
 
 def _aligned(a: np.ndarray) -> np.ndarray:
@@ -58,12 +58,12 @@ def _aligned(a: np.ndarray) -> np.ndarray:
 class EmulatedFrame:
     """One frame through the host-compiled kernels, planned by a plan-only libmeao context (device = -1)."""
 
-    def __init__(self, plan, *, linear: bool = False, defs: tuple[str, ...] = (), use_tma: bool = True, render_tile: int = -1):
+    def __init__(self, plan, *, linear: bool = False, use_tma: bool = True, render_tile: int = -1):
         """plan: miniengineao_b200.AmbientOcclusion(camera, device=-1) with parameters / variants already set.
         use_tma: interior tiles take the kernels' TMA path (emulated box loads) -- what runs on the GPU; False forces the
         gather path everywhere (libmeao's MEAO_DISABLE_TMA=1)."""
         from miniengineao_b200 import _native as N
-        self._lib = lib(defs)
+        self._lib = lib()
         plan.LateUpdate()
         self.plan = plan
         self.W, self.H = plan._width, plan._height
@@ -160,15 +160,15 @@ class EmulatedFrame:
         return out
 
 
-def composite(ao: np.ndarray, color: np.ndarray, *, rgb: bool, alpha: bool, one_minus: bool, defs: tuple[str, ...] = ()) -> np.ndarray:
+def composite(ao: np.ndarray, color: np.ndarray, *, rgb: bool, alpha: bool, one_minus: bool) -> np.ndarray:
     out = _aligned(np.ascontiguousarray(color))
     a = _aligned(np.ascontiguousarray(ao, np.uint8))
-    lib(defs).emu_composite(a.ctypes.data, out.ctypes.data, a.size, int(out.dtype == np.float16), int(rgb), int(alpha), int(one_minus))
+    lib().emu_composite(a.ctypes.data, out.ctypes.data, a.size, int(out.dtype == np.float16), int(rgb), int(alpha), int(one_minus))
     return out.copy()
 
 
-def composite_debug(view: np.ndarray, like: np.ndarray, defs: tuple[str, ...] = ()) -> np.ndarray:
+def composite_debug(view: np.ndarray, like: np.ndarray) -> np.ndarray:
     v = _aligned(np.ascontiguousarray(view, np.uint8))
     out = _aligned(np.zeros(v.shape + (4,), like.dtype))
-    lib(defs).emu_composite_debug(v.ctypes.data, out.ctypes.data, v.size, int(out.dtype == np.float16))
+    lib().emu_composite_debug(v.ctypes.data, out.ctypes.data, v.size, int(out.dtype == np.float16))
     return out.copy()

@@ -142,12 +142,7 @@ static void run_upsample(Emu *e, int lo)
     a.out_row_origin = 0; a.out_vec_ok = 1;
     a.hiw = e->lw[hi]; a.hih = e->lh[hi];
     a.noise_filter_strength = e->nfs[lo]; a.step_size = e->step[lo]; a.blur_tolerance = e->kblur[lo]; a.upsample_tolerance = e->tol[lo];
-    auto safe = [](float x) { return x >= 8.673617379884035e-19f && x < 1152921504606846976.0f; };
-    a.fast_div_ok = safe(a.upsample_tolerance) && safe(a.noise_filter_strength);
-#if MEAO_UPS_STATIC_GUARD || MEAO_UPS_V2
-    a.fast_div_ok = a.fast_div_ok && a.upsample_tolerance >= 2.7755575615628914e-17f && a.noise_filter_strength >= 2.220446049250313e-16f &&
-                    a.noise_filter_strength < 288230376151711744.0f;
-#endif
+    a.fast_div_ok = upsample_fast_div_ok(a.upsample_tolerance, a.noise_filter_strength);
     a.row0 = e->need_lo[hi]; a.row1 = e->need_hi[hi];
     a.tile_ctr = e->tile_ctr + 2 * (lo - 1);
     const bool premin = ((e->hq_mask >> (lo - 1)) & 1) != 0;
