@@ -52,6 +52,7 @@ namespace MiniEngineAO
         [DllImport(Lib)] public static extern int meao_set_variants(IntPtr ctx, ref MeaoVariants v);
         [DllImport(Lib)] public static extern int meao_set_camera(IntPtr ctx, ref MeaoCamera c);
         [DllImport(Lib)] public static extern int meao_resize(IntPtr ctx, int width, int height);
+        [DllImport(Lib)] public static extern int meao_set_layers(IntPtr ctx, int layers);   // layered frames: L views per frame, [L][H][W] buffers
         [DllImport(Lib)] public static extern int meao_render(IntPtr ctx, IntPtr depthDev, int depthKind, IntPtr aoOutDev, IntPtr stream);
         [DllImport(Lib)] public static extern int meao_render_host(IntPtr ctx, float[] depth, int depthKind, byte[] aoOut);
         [DllImport(Lib)] public static extern int meao_bind_event(IntPtr ctx, int eventId, IntPtr depthDev, int depthKind, IntPtr aoOutDev, IntPtr stream);
@@ -96,6 +97,10 @@ namespace MiniEngineAO
         // ---- not in the reference inspector: the shader variants Render.compute / Upsample.compute ship but AO.cs never selects ----
         [SerializeField] bool _sampleExhaustively;             // Render.compute:144-159, AmbientOcclusion.cs:709-715 (FIXME there)
         [SerializeField, Range(0, 15)] int _highQualityMask;   // bit k-1: Render kernel "main" on level k + Upsample "main_premin*"
+        // Layered frames (meao_set_layers): views per frame, rendered together -- 2 for the eye slices of a texture-array (instanced)
+        // stereo target, 6 for cube-map faces.  The depth and AO buffers the interop layer maps then hold Layers images each.
+        [SerializeField, Range(1, 65535)] int _layers = 1;
+        public int Layers { get { return _layers; } set { _layers = value; } }
         int _drawCountPerFrame;                                // AmbientOcclusion.cs:289, 349-355: single-pass stereo detection
         void OnPreRender() { _drawCountPerFrame++; }
         bool singlePassStereoEnabled                           // AmbientOcclusion.cs:392-401
@@ -149,6 +154,9 @@ namespace MiniEngineAO
                 single_scale = 0                                                             // BASELINE configs[0] plumbing mode; the component never selects it
             };
             rebuild |= MeaoNative.meao_set_variants(_ctx, ref variants) == 1;
+            var layered = MeaoNative.meao_set_layers(_ctx, _layers);
+            MeaoNative.Check(_ctx, layered);
+            rebuild |= layered == 1;
             rebuild |= MeaoNative.meao_resize(_ctx, _camera.pixelWidth * (stereo ? 2 : 1), _camera.pixelHeight) == 1;   // :338-341
             rebuild |= !Application.isPlaying;                                               // :345
             _drawCountPerFrame = 0;                                                          // :349

@@ -32,7 +32,8 @@ extern "C" {
 
 #define MEAO_ABI_VERSION 3   /* 2: + MeaoVariants, meao_stage_render_wide, meao_debug_view, meao_composite_debug, buffer ids 18..21
                               * 3: + MeaoVariants.single_scale, native peer halo exchange (meao_band_export / _connect / _step / _status),
-                              *      meao_bind_event takes the stream */
+                              *      meao_bind_event takes the stream
+                              *    + meao_set_layers (layered frames; additive, so the version stays 3) */
 
 typedef struct MeaoCtx MeaoCtx;
 
@@ -144,6 +145,21 @@ int meao_set_camera(MeaoCtx *ctx, const MeaoCamera *camera);
  * A size change RESETS the row band to the whole frame and drops the neighbour connections (meao_set_row_band,
  * meao_band_connect): a band host must set its band again after every call that returned 1. */
 int meao_resize(MeaoCtx *ctx, int32_t width, int32_t height);
+/* Layered frames: every frame holds `layers` independent views of width x height (texture-array stereo: 2 eye slices; cube-map
+ * AO: 6 faces; a batch of frames of one camera), rendered by ONE launch per stage.  Each layer's result is bit-identical to
+ * rendering that layer alone; one MeaoParams / MeaoCamera / MeaoVariants applies to all layers.  Layout rule: every image argument
+ * holds the L images stacked at a stride of one tight image -- depth is L*width*height elements of the depth kind, the AO output
+ * L*width*height bytes -- for meao_render, meao_render_host(_async), meao_bind_event, meao_profile_frame, the meao_stage_* calls,
+ * meao_debug_view (L images) and the meao_composite_* calls (L*width*height pixels).  meao_get_buffer / meao_set_buffer use
+ * [L][reference layout] (host_bytes = L x the single size; MeaoBufferDesc stays per layer).  meao_kernels_per_frame is unchanged
+ * (one layered launch is one kernel); meao_algorithmic_bytes scales by L.
+ * A plan input like meao_resize: default 1 (every entry point behaves as without layers); returns 1 if the value changed, 0 if
+ * not.  A change re-allocates the intermediates, drops the captured graphs, resets the row band to the whole frame and drops the
+ * neighbour connections.  layers must be in 1..65535 (the layer is a grid dimension of the layered kernels), else
+ * MEAO_ERR_INVALID; MEAO_ERR_NOMEM if the intermediates do not fit (the context keeps its previous layer count).
+ * Row bands and layers exclude each other: with layers > 1, meao_set_row_band, the halo calls (meao_halo_*, meao_render_band_*,
+ * meao_band_phase_a / _b) and the native exchange (meao_band_export / _connect / _step / _step_host) return MEAO_ERR_UNSUPPORTED. */
+int meao_set_layers(MeaoCtx *ctx, int32_t layers);
 
 /* ---- the frame ------------------------------------------------------------------------------- */
 /* replaces: replay of the "SSAO" command buffer, steps 1-10 of RebuildCommandBuffers (AO.cs:511-531):

@@ -59,6 +59,7 @@ SIGNATURES = {
     "meao_get_variants": (C.c_int, [C.c_void_p, C.POINTER(MeaoVariants)]),
     "meao_set_camera": (C.c_int, [C.c_void_p, C.POINTER(MeaoCamera)]),
     "meao_resize": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
+    "meao_set_layers": (C.c_int, [C.c_void_p, C.c_int32]),
     "meao_render": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "meao_render_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
     "meao_render_host_async": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32]),

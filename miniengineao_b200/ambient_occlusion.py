@@ -80,6 +80,7 @@ class AmbientOcclusion:
         self.sampleExhaustively = False     # Render.compute:144-159
         self.highQualityMask = 0            # bit k-1: Render.compute kernel "main" on level k + Upsample main_premin*
         self.singleScale = False            # BASELINE.json configs[0]: Downsample1 -> Render level 1 -> final-style Upsample only
+        self.layers = 1                     # views per frame (meao_set_layers): texture-array stereo 2, cube faces 6, frame batches
         self._band = None                   # (row0, row1) after set_row_band; reset by every re-allocation
         self._drawCountPerFrame = 0         # AO.cs:289: used to detect single-pass stereo
         self._stereo = False                # singlePassStereoEnabled as latched by the last LateUpdate
@@ -144,7 +145,9 @@ class AmbientOcclusion:
         v = N.MeaoVariants(int(stereo), int(self.sampleExhaustively), int(self.highQualityMask), int(self.singleScale))
         rebuild |= self._check(self._lib.meao_set_variants(self._ctx, C.byref(v))) == 1
         width = cam.pixelWidth * (2 if stereo else 1)                                                # AO.cs:338-341, 501-504
+        layered = self._check(self._lib.meao_set_layers(self._ctx, int(self.layers))) == 1           # re-allocates like a resize
         resized = self._check(self._lib.meao_resize(self._ctx, width, cam.pixelHeight)) == 1          # CheckBaseDimensions
+        resized |= layered
         self._width, self._height = width, cam.pixelHeight
         if resized:
             self._band = None       # meao_resize re-allocates: the C context is back to the whole frame and has dropped its neighbours
@@ -168,52 +171,63 @@ class AmbientOcclusion:
             return N.MEAO_DEPTH_RAW_D24S8
         raise ValueError(f"unsupported depth dtype {dtype_name}")
 
+    def _frame_shape(self) -> tuple:
+        """Shape of one frame's depth / AO: (rows, W), or (layers, H, W) for a layered context."""
+        if self.layers > 1:
+            return (self.layers, self._height, self._width)
+        return (self._band_rows(), self._width)
+
     def render(self, depth, out=None, *, linear: bool = False, stream=None):
-        """depth: CUDA tensor [H, W]: float32 raw camera depth (or linear if linear=True), uint16 D16_UNORM codes,
-        or int32 D24_UNORM_S8_UINT words.  Returns a CUDA uint8 tensor [H, W] -- the AmbientOcclusion R8 texture (AO.cs:475)."""
+        """depth: CUDA tensor [H, W] ([layers, H, W] when layers > 1): float32 raw camera depth (or linear if linear=True), uint16
+        D16_UNORM codes, or int32 D24_UNORM_S8_UINT words.  Returns a CUDA uint8 tensor of the same shape -- the AmbientOcclusion R8
+        texture (AO.cs:475), one per layer."""
         import torch
         self.LateUpdate()
         if not (depth.is_cuda and depth.is_contiguous()):
             raise ValueError("depth must be a contiguous CUDA tensor")
-        rows = self._band_rows()
-        if tuple(depth.shape) != (rows, self._width):
-            raise ValueError(f"depth shape {tuple(depth.shape)} != {(rows, self._width)}")
+        shape = self._frame_shape()
+        if tuple(depth.shape) != shape:
+            raise ValueError(f"depth shape {tuple(depth.shape)} != {shape}")
         if out is None:
-            out = torch.empty((rows, self._width), dtype=torch.uint8, device=depth.device)
+            out = torch.empty(shape, dtype=torch.uint8, device=depth.device)
+        elif tuple(out.shape) != shape or out.dtype != torch.uint8 or not out.is_contiguous():
+            raise ValueError(f"out must be a contiguous uint8 CUDA tensor {shape}")
         kind = self._kind(str(depth.dtype).replace("torch.", ""), linear)
         self._check(self._lib.meao_render(self._ctx, depth.data_ptr(), kind, out.data_ptr(), self._stream(stream)))
         return out
 
     def render_host(self, depth: np.ndarray, out: np.ndarray | None = None, *, linear: bool = False) -> np.ndarray:
-        """Host [H, W] depth (float32 / uint16 D16 codes / uint32 D24S8 words) in, host uint8 [H, W] out
-        (H2D + the kernels + D2H + sync)."""
+        """Host [H, W] depth ([layers, H, W] when layers > 1; float32 / uint16 D16 codes / uint32 D24S8 words) in, host uint8 of the
+        same shape out (H2D + the kernels + D2H + sync)."""
         self.LateUpdate()
-        rows = self._band_rows()
+        shape = self._frame_shape()
         d = np.ascontiguousarray(depth)
-        if d.shape != (rows, self._width):
-            raise ValueError(f"depth shape {d.shape} != {(rows, self._width)}")
+        if d.shape != shape:
+            raise ValueError(f"depth shape {d.shape} != {shape}")
         if out is None:
-            out = np.empty((rows, self._width), np.uint8)
+            out = np.empty(shape, np.uint8)
+        elif out.shape != shape or out.dtype != np.uint8 or not out.flags.c_contiguous:
+            raise ValueError(f"out must be a C-contiguous uint8 array {shape}")
         kind = self._kind(d.dtype.name, linear)
         self._check(self._lib.meao_render_host(self._ctx, d.ctypes.data, kind, out.ctypes.data))
         return out
 
     def render_host_batch(self, depths, outs, *, linear: bool = False) -> None:
-        """Frame stream with HOST buffers: depths[i] (float32, or uint16 D16_UNORM codes, [H, W]) -> outs[i] (uint8 [H, W]).  Frames alternate
+        """Frame stream with HOST buffers: depths[i] (float32, or uint16 D16_UNORM codes, [H, W] or [layers, H, W]) -> outs[i] (uint8, same shape).  Frames alternate
         over the two staging slots of the context, so the H2D copy of frame i+1 overlaps the kernels and the D2H
         copy of frame i.  Pass pinned arrays (meao_host_alloc) for real overlap; the arrays must stay alive and
         untouched until this call returns."""
         self.LateUpdate()
-        rows = self._band_rows()
+        shape = self._frame_shape()
         n = len(depths)
         assert len(outs) == n
         for i in range(n):
             d, o = depths[i], outs[i]
-            if d.dtype not in (np.float32, np.uint16) or not d.flags.c_contiguous or d.shape != (rows, self._width):
-                raise ValueError("depths[i] must be C-contiguous float32 (or uint16 D16 codes) [rows, W]")
+            if d.dtype not in (np.float32, np.uint16) or not d.flags.c_contiguous or d.shape != shape:
+                raise ValueError(f"depths[i] must be C-contiguous float32 (or uint16 D16 codes) {shape}")
             kind = self._kind(d.dtype.name, linear)
-            if o.dtype != np.uint8 or not o.flags.c_contiguous or o.shape != (rows, self._width):
-                raise ValueError("outs[i] must be C-contiguous uint8 [rows, W]")
+            if o.dtype != np.uint8 or not o.flags.c_contiguous or o.shape != shape:
+                raise ValueError(f"outs[i] must be C-contiguous uint8 {shape}")
             slot = i & 1
             if i >= 2:
                 self._check(self._lib.meao_host_wait(self._ctx, slot))
@@ -318,22 +332,27 @@ class AmbientOcclusion:
         self._check(self._lib.meao_buffer_desc(self._ctx, debug_id, C.byref(d)))
         return d
 
+    def _buffer_shape(self, d: N.MeaoBufferDesc) -> tuple:
+        shape = (d.slices, d.height, d.width) if d.slices > 1 else (d.height, d.width)
+        return (self.layers,) + shape if self.layers > 1 else shape
+
     def debug_buffer(self, debug_id: int) -> np.ndarray:
-        """Buffer <id> in the reference layout and native type: float16 / float32 / uint8 codes."""
+        """Buffer <id> in the reference layout and native type: float16 / float32 / uint8 codes (leading layer axis when layers > 1)."""
         d = self.buffer_desc(debug_id)
         dt = {1: np.uint8, 2: np.float16, 4: np.float32}[d.elem_bytes]
-        shape = (d.slices, d.height, d.width) if d.slices > 1 else (d.height, d.width)
+        shape = self._buffer_shape(d)
         a = np.empty(shape, dt)
         self._check(self._lib.meao_get_buffer(self._ctx, debug_id, a.ctypes.data, a.nbytes))
         return a
 
     def debug_view(self, debug_id: int, out=None, *, stream=None):
         """PushDebugBlitCommands (AO.cs:787-820): the W x H R8 image the `debug` property would put on screen for
-        buffer <debug_id>; returns a CUDA uint8 tensor [H, W]."""
+        buffer <debug_id>; returns a CUDA uint8 tensor [H, W] ([layers, H, W] when layers > 1)."""
         import torch
         self._update(False)
         if out is None:
-            out = torch.empty((self._height, self._width), dtype=torch.uint8, device=f"cuda:{self.device}")
+            shape = (self.layers, self._height, self._width) if self.layers > 1 else (self._height, self._width)
+            out = torch.empty(shape, dtype=torch.uint8, device=f"cuda:{self.device}")
         self._check(self._lib.meao_debug_view(self._ctx, debug_id, out.data_ptr(), self._stream(stream)))
         return out
 
@@ -350,7 +369,7 @@ class AmbientOcclusion:
         d = self.buffer_desc(debug_id)
         dt = {1: np.uint8, 2: np.float16, 4: np.float32}[d.elem_bytes]
         a = np.ascontiguousarray(values, dtype=dt)
-        assert a.shape == (d.height, d.width), (a.shape, d.height, d.width)
+        assert a.shape == self._buffer_shape(d), (a.shape, self._buffer_shape(d))
         self._check(self._lib.meao_set_buffer(self._ctx, debug_id, a.ctypes.data, a.nbytes))
 
     # ---- constants ----------------------------------------------------------------------------------

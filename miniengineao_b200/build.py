@@ -13,8 +13,10 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libmeao.so")
-SOURCES = ["meao_api.cu", "prepare_depth.cu", "render_ao.cu", "blur_upsample.cu", "selftest.cu", "halo.cu", "band_exchange.cu", "composite.cu", "debug_view.cu"]
-HEADERS = ["common.cuh", "kernels.h", "blur_upsample_kernel.inc", os.path.join("..", "..", "include", "meao.h")]
+SOURCES = ["meao_api.cu", "prepare_depth.cu", "render_ao.cu", "blur_upsample.cu", "selftest.cu", "halo.cu", "band_exchange.cu", "composite.cu", "debug_view.cu",
+           "prepare_depth_layered.cu", "render_ao_layered.cu", "blur_upsample_layered.cu"]
+HEADERS = ["common.cuh", "kernels.h", "prepare_depth_kernel.inc", "render_ao_kernel.inc", "blur_upsample_device.inc", "blur_upsample_kernel.inc",
+           os.path.join("..", "..", "include", "meao.h")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

@@ -111,7 +111,7 @@ struct UpsampleArgs {
     int tiles_x, tiles_y;   // tile grid (filled by launch_blur_upsample)
 };
 // The tolerances for which the upsample's fast divisions are proven exact: 2^-55 <= tol < 2^60 and 2^-52 <= nfs < 2^58.
-// Within them the final division needs no per-pixel range test (the proof is at bilateral2 in blur_upsample.cu).
+// Within them the final division needs no per-pixel range test (the proof is at bilateral2 in blur_upsample_device.inc).
 inline bool upsample_fast_div_ok(float tol, float nfs)
 {
     return tol >= 2.7755575615628914e-17f && tol < 1152921504606846976.0f && nfs >= 2.220446049250313e-16f && nfs < 288230376151711744.0f;
@@ -124,6 +124,18 @@ cudaError_t launch_blur_upsample(const CUtensorMap &lo_depth_map, const CUtensor
                                  const UpsampleArgs &a, const uint8_t *lo_ao2, int lo_a2pitch, int sm_count, cudaStream_t s);
 constexpr int kUpsDepthBoxW = 40, kUpsDepthBoxH = 22; // TMA boxes of the upsample kernel
 constexpr int kUpsAoBoxW = 64, kUpsAoBoxH = 22;
+
+// ---- layered frames (meao_set_layers): L same-size views through one launch per stage ------------------------------------
+// Every image is L images of the same pitch stored back to back ([L][h][pitch]; the caller's depth and AO: [L][H][W] tight), so
+// layer l of an image starts l x rows x pitch elements after layer 0.  The arguments are the single-image ones (row0 = 0,
+// row1 = the level's height, out_row_origin = 0) describing layer 0; the TMA maps span all layers (height L x h), and the kernels
+// fetch a box only when it lies inside one layer.  Separate kernels and translation units (*_layered.cu), so the single-image
+// kernels keep their code.  kMaxLayers: the prepare_depth / render_ao grids carry the layer in gridDim.z (at most 65535).
+constexpr int kMaxLayers = 65535;
+cudaError_t launch_prepare_depth_layered(const PrepareArgs &a, int layers, cudaStream_t s);
+cudaError_t launch_render_ao_layered(const CUtensorMap &low_map, bool use_tma, const RenderArgs &a, int layers, cudaStream_t s);
+cudaError_t launch_blur_upsample_layered(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
+                                         const UpsampleArgs &a, const uint8_t *lo_ao2, int lo_a2pitch, int layers, int sm_count, cudaStream_t s);
 
 // ---- debug: synthesise a TiledDepth<k> view (reference layout [16][sh][sw], f16 bits) ----------
 cudaError_t launch_synth_tiled(const float *low, int lw, int lh, int lpitch, int sw, int sh, float pad,
@@ -184,6 +196,9 @@ template <class K> inline cudaError_t preload_kernel(K kernel) { cudaFuncAttribu
 cudaError_t preload_prepare_depth();
 cudaError_t preload_render_ao();
 cudaError_t preload_blur_upsample();
+cudaError_t preload_prepare_depth_layered();
+cudaError_t preload_render_ao_layered();
+cudaError_t preload_blur_upsample_layered();
 cudaError_t preload_band_kernels();
 cudaError_t preload_aux_kernels();      // composite, debug views, self test
 #endif

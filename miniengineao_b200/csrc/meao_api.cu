@@ -78,6 +78,7 @@ struct MeaoCtx {
 
     int W = 0, H = 0;
     int lw[7] = {0}, lh[7] = {0};
+    int layers = 1;                         // meao_set_layers: every image holds `layers` same-size views stacked at a stride of one image
     // band (global L0 rows) + neighbours
     int band0 = 0, band1 = 0, prev0 = -1, next1 = -1;
 
@@ -92,8 +93,8 @@ struct MeaoCtx {
     uint8_t *result = nullptr; int result_pitch = 0;
     // staging for the host path: two slots so that the H2D copy of frame i+1 overlaps the kernels and the
     // D2H copy of frame i (meao_render_host_async)
-    float *depth_stage[2] = {nullptr, nullptr};     // device, W*H each
-    uint8_t *ao_stage[2] = {nullptr, nullptr};      // device, W*H each
+    float *depth_stage[2] = {nullptr, nullptr};     // device, layers*W*H each
+    uint8_t *ao_stage[2] = {nullptr, nullptr};      // device, layers*W*H each
     cudaStream_t slot_stream[2] = {nullptr, nullptr};
     cudaEvent_t slot_done[2] = {nullptr, nullptr};
     cudaEvent_t compute_done = nullptr;
@@ -151,6 +152,12 @@ int fail(MeaoCtx *c, int code, const char *fmt, ...)
     if (c) c->error = buf; else g_create_error = buf;
     return code;
 }
+// Row bands and layered frames exclude each other: a band's halo rows are whole rows of ONE image.
+int refuse_layered(MeaoCtx *c, const char *what)
+{
+    return fail(c, MEAO_ERR_UNSUPPORTED, "%s: row bands need a single-layer context (this one has %d layers, meao_set_layers)", what, c->layers);
+}
+#define LAYERS_GUARD(c, what) do { if ((c) && (c)->layers > 1) return refuse_layered((c), (what)); } while (0)
 #define CUDA_TRY(c, expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) \
     return fail((c), MEAO_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); } while (0)
 
@@ -341,23 +348,25 @@ int allocate(MeaoCtx *c)
     // pitches: rows start on 128-byte boundaries
     c->lin_pitch = align_up(c->lw[0], 64);
     c->result_pitch = align_up(c->lw[0], 128);
+    // every image: `layers` views of the same pitch, back to back ([L][h][pitch], kernels.h "layered frames")
+    const size_t L = (size_t)c->layers;
     size_t off = 0;
     auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 255) / 256 * 256; return o; };
     take(sizeof(BandFlags));            // offset 0 in EVERY context's arena (the neighbours address it through their peer mapping)
     const size_t o_ctr = take(8 * sizeof(uint32_t));
-    size_t o_lin = take((size_t)c->lin_pitch * c->lh[0] * sizeof(__half));
-    size_t o_res = take((size_t)c->result_pitch * c->lh[0]);
+    size_t o_lin = take(L * c->lin_pitch * c->lh[0] * sizeof(__half));
+    size_t o_res = take(L * c->result_pitch * c->lh[0]);
     size_t o_low[5], o_occ[5], o_comb[4], o_hq[5];
     for (int k = 1; k <= 4; k++) {
         c->low_pitch[k] = align_up(c->lw[k], 32);
         c->occ_pitch[k] = align_up(c->lw[k], 128);
-        o_low[k] = take((size_t)c->low_pitch[k] * c->lh[k] * sizeof(float));
-        o_occ[k] = take((size_t)c->occ_pitch[k] * c->lh[k]);
-        if (k <= 3) o_comb[k] = take((size_t)c->occ_pitch[k] * c->lh[k]);
-        o_hq[k] = take((size_t)c->occ_pitch[k] * c->lh[k]);
+        o_low[k] = take(L * c->low_pitch[k] * c->lh[k] * sizeof(float));
+        o_occ[k] = take(L * c->occ_pitch[k] * c->lh[k]);
+        if (k <= 3) o_comb[k] = take(L * c->occ_pitch[k] * c->lh[k]);
+        o_hq[k] = take(L * c->occ_pitch[k] * c->lh[k]);
     }
     size_t o_dst[2], o_ast[2];
-    for (int i = 0; i < 2; i++) { o_dst[i] = take((size_t)W * H * sizeof(float)); o_ast[i] = take((size_t)W * H); }
+    for (int i = 0; i < 2; i++) { o_dst[i] = take(L * W * H * sizeof(float)); o_ast[i] = take(L * W * H); }
     cudaError_t e = cudaMalloc(&c->arena, off);
     if (e != cudaSuccess) return fail(c, e == cudaErrorMemoryAllocation ? MEAO_ERR_NOMEM : MEAO_ERR_CUDA,
                                       "cudaMalloc(%zu) failed: %s", off, cudaGetErrorString(e));
@@ -385,17 +394,20 @@ int allocate(MeaoCtx *c)
     c->tma_ok = false;
     if (c->encode) {
         bool ok = true;
+        // one 2-D map over all layers: height L x lh (the kernels fetch a box only when it lies inside one layer); with one layer
+        // these are the single-image maps
         for (int k = 1; k <= 4 && ok; k++) {
+            const int mh = c->layers * c->lh[k];
             for (int t = 0; t < kRenderTileVariants; t++) {
-                ok &= make_map(c, &c->map_low_ren[t][k], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, c->low[k], c->lw[k], c->lh[k], c->low_pitch[k], kRenderBoxW, render_box_h(kRenderTileHs[t], false)) == 0;
-                ok &= make_map(c, &c->map_low_wide[t][k], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, c->low[k], c->lw[k], c->lh[k], c->low_pitch[k], kRenderWideBoxW, render_box_h(kRenderTileHs[t], true)) == 0;
+                ok &= make_map(c, &c->map_low_ren[t][k], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, c->low[k], c->lw[k], mh, c->low_pitch[k], kRenderBoxW, render_box_h(kRenderTileHs[t], false)) == 0;
+                ok &= make_map(c, &c->map_low_wide[t][k], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, c->low[k], c->lw[k], mh, c->low_pitch[k], kRenderWideBoxW, render_box_h(kRenderTileHs[t], true)) == 0;
             }
-            ok &= make_map(c, &c->map_low_ups[k], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, c->low[k], c->lw[k], c->lh[k], c->low_pitch[k], kUpsDepthBoxW, kUpsDepthBoxH) == 0;
+            ok &= make_map(c, &c->map_low_ups[k], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, c->low[k], c->lw[k], mh, c->low_pitch[k], kUpsDepthBoxW, kUpsDepthBoxH) == 0;
             uint8_t *ao = (k == 4) ? c->occ[4] : c->comb[k];
-            ok &= make_map(c, &c->map_ao_ups[k], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, ao, c->lw[k], c->lh[k], c->occ_pitch[k], kUpsAoBoxW, kUpsAoBoxH) == 0;
-            ok &= make_map(c, &c->map_hq_ups[k], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, c->hq[k], c->lw[k], c->lh[k], c->occ_pitch[k], kUpsAoBoxW, kUpsAoBoxH) == 0;
+            ok &= make_map(c, &c->map_ao_ups[k], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, ao, c->lw[k], mh, c->occ_pitch[k], kUpsAoBoxW, kUpsAoBoxH) == 0;
+            ok &= make_map(c, &c->map_hq_ups[k], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, c->hq[k], c->lw[k], mh, c->occ_pitch[k], kUpsAoBoxW, kUpsAoBoxH) == 0;
         }
-        ok &= make_map(c, &c->map_occ1_ups, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, c->occ[1], c->lw[1], c->lh[1], c->occ_pitch[1], kUpsAoBoxW, kUpsAoBoxH) == 0;
+        ok &= make_map(c, &c->map_occ1_ups, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, c->occ[1], c->lw[1], c->layers * c->lh[1], c->occ_pitch[1], kUpsAoBoxW, kUpsAoBoxH) == 0;
         c->tma_ok = ok;
     }
     if (!c->tma_ok) {
@@ -425,12 +437,13 @@ struct NvtxRange { explicit NvtxRange(const char *n) { nvtxRangePushA(n); } ~Nvt
 // Tile-height variant (index into kRenderTileHs = {32, 16, 8}) of a render launch.  The big levels keep the 64 x 32 tile
 // (least apron overhead: throughput); a level whose grid would not even put one CTA on every SM is latency-bound -- one
 // CTA's serial time IS the kernel time -- so it takes the tallest tile that still gives at least one CTA per SM, else 64 x 8.
+// A layered launch counts the CTAs of all its layers.
 int render_tile_variant(const MeaoCtx *c, int k, int rows)
 {
     const char *force = getenv("MEAO_REN_TILE");               // tuning aid: 0 / 1 / 2 forces a variant for every level
     if (force && force[0] >= '0' && force[0] < '0' + kRenderTileVariants) return force[0] - '0';
     for (int t = 0; t < kRenderTileVariants; t++) {
-        const int ctas = ((c->lw[k] + 63) / 64) * ((rows + kRenderTileHs[t] - 1) / kRenderTileHs[t]);
+        const long long ctas = (long long)c->layers * ((c->lw[k] + 63) / 64) * ((rows + kRenderTileHs[t] - 1) / kRenderTileHs[t]);
         if (ctas >= c->sm_count) return t;
     }
     return kRenderTileVariants - 1;
@@ -456,7 +469,8 @@ int record_downsample(MeaoCtx *c, const void *depth, int kind, cudaStream_t s)
     a.reversed_z = c->camera.reversed_z;
     a.vec_ok = (((uintptr_t)depth & 15) == 0) && (c->W % (a.in_format == 1 ? 8 : 4) == 0);
     c->last_kind = kind;
-    CUDA_TRY(c, launch_prepare_depth(a, s));
+    if (c->layers > 1) CUDA_TRY(c, launch_prepare_depth_layered(a, c->layers, s));
+    else CUDA_TRY(c, launch_prepare_depth(a, s));
     c->launches++;
     return 0;
 }
@@ -489,7 +503,9 @@ int record_render(MeaoCtx *c, int k, int kind, cudaStream_t s, bool wide = false
     a.exhaustive = exh ? 1 : 0;
     const int tv = render_tile_variant(c, k, a.row1 - (a.row0 & ~3));
     a.tile_h = kRenderTileHs[tv];
-    CUDA_TRY(c, launch_render_ao(wide ? c->map_low_wide[tv][k] : c->map_low_ren[tv][k], c->tma_ok, a, s));
+    const CUtensorMap &map = wide ? c->map_low_wide[tv][k] : c->map_low_ren[tv][k];
+    if (c->layers > 1) CUDA_TRY(c, launch_render_ao_layered(map, c->tma_ok, a, c->layers, s));
+    else CUDA_TRY(c, launch_render_ao(map, c->tma_ok, a, s));
     c->launches++;
     return 0;
 }
@@ -521,7 +537,10 @@ int record_upsample(MeaoCtx *c, int lo, void *ao_out, cudaStream_t s)
     a.row0 = c->need_c[hi].lo; a.row1 = c->need_c[hi].hi;
     a.tile_ctr = c->tile_ctr + 2 * (lo - 1);
     const uint8_t *lo_ao2 = hq_level(c, lo) ? c->hq[lo] : nullptr;                   // kernels main_premin / main_premin_blendout
-    CUDA_TRY(c, launch_blur_upsample(c->map_low_ups[lo], single ? c->map_occ1_ups : c->map_ao_ups[lo], &c->map_hq_ups[lo], c->tma_ok, a, lo_ao2, c->occ_pitch[lo], c->sm_count, s));
+    const CUtensorMap &ao_map = single ? c->map_occ1_ups : c->map_ao_ups[lo];
+    if (c->layers > 1)
+        CUDA_TRY(c, launch_blur_upsample_layered(c->map_low_ups[lo], ao_map, &c->map_hq_ups[lo], c->tma_ok, a, lo_ao2, c->occ_pitch[lo], c->layers, c->sm_count, s));
+    else CUDA_TRY(c, launch_blur_upsample(c->map_low_ups[lo], ao_map, &c->map_hq_ups[lo], c->tma_ok, a, lo_ao2, c->occ_pitch[lo], c->sm_count, s));
     c->launches++;
     return 0;
 }
@@ -710,6 +729,9 @@ int meao_create(const MeaoDeviceCfg *cfg, MeaoCtx **out)
             cudaError_t pe = preload_prepare_depth();
             if (pe == cudaSuccess) pe = preload_render_ao();
             if (pe == cudaSuccess) pe = preload_blur_upsample();
+            if (pe == cudaSuccess) pe = preload_prepare_depth_layered();
+            if (pe == cudaSuccess) pe = preload_render_ao_layered();
+            if (pe == cudaSuccess) pe = preload_blur_upsample_layered();
             if (pe == cudaSuccess) pe = preload_band_kernels();
             if (pe == cudaSuccess) pe = preload_aux_kernels();
             if (pe != cudaSuccess) { cudaGetLastError(); meao_destroy(c); return fail(nullptr, MEAO_ERR_CUDA, "loading the kernels failed: %s", cudaGetErrorString(pe)); }
@@ -813,9 +835,34 @@ int meao_resize(MeaoCtx *c, int32_t w, int32_t h)
     return 1;
 }
 
+int meao_set_layers(MeaoCtx *c, int32_t layers)
+{
+    if (!c) return MEAO_ERR_INVALID;
+    if (layers < 1 || layers > kMaxLayers)
+        return fail(c, MEAO_ERR_INVALID, "layers %d not in 1..%d (the layer is a grid dimension of the layered kernels)", layers, kMaxLayers);
+    if (layers == c->layers) return 0;
+    const int old = c->layers;
+    c->layers = layers;
+    if (c->W <= 0) return 1;                        // applied by the first meao_resize
+    if (!c->plan_only) {
+        CUDA_TRY(c, cudaSetDevice(c->device));
+        CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+    }
+    int rc = allocate(c);                           // like a size change: new arena, whole-frame band, no neighbours, no graphs
+    if (rc) {
+        const std::string err = c->error;
+        c->layers = old;
+        if (allocate(c)) { c->W = c->H = 0; }        // the previous arena could not be restored either: the context needs meao_resize
+        c->error = err;
+        return rc;
+    }
+    return 1;
+}
+
 int meao_set_row_band(MeaoCtx *c, int32_t row0, int32_t row1, int32_t prev_row0, int32_t next_row1)
 {
     if (!c || c->W <= 0) return MEAO_ERR_INVALID;
+    LAYERS_GUARD(c, "meao_set_row_band");
     if (row0 < 0 || row1 > c->H || row0 >= row1 || (row0 % 16) || ((row1 % 16) && row1 != c->H))
         return fail(c, MEAO_ERR_INVALID, "band [%d,%d) must be 16-row aligned inside [0,%d)", row0, row1, c->H);
     if ((prev_row0 >= 0 && (prev_row0 % 16 || prev_row0 >= row0)) || (next_row1 >= 0 && (next_row1 <= row1 || next_row1 > c->H)))
@@ -867,6 +914,7 @@ static void halo_ranges(MeaoCtx *c, int side, bool send, Range out[5])
 static int64_t halo_size(MeaoCtx *c, int side, bool send)
 {
     if (!c || c->W <= 0 || (side != 0 && side != 1)) return MEAO_ERR_INVALID;
+    LAYERS_GUARD(c, send ? "meao_halo_bytes" : "meao_halo_recv_bytes");
     Range r[5]; halo_ranges(c, side, send, r);
     int64_t bytes = 0;
     for (int k = 1; k <= 4; k++) bytes += (int64_t)(r[k].hi - r[k].lo) * c->lw[k] * 4;
@@ -876,6 +924,7 @@ int64_t meao_halo_bytes(MeaoCtx *c, int32_t side) { return halo_size(c, side, tr
 int meao_halo_rows(MeaoCtx *c, int32_t side, int32_t send, int32_t out8[8])
 {
     if (!c || c->W <= 0 || (side != 0 && side != 1) || !out8) return MEAO_ERR_INVALID;
+    LAYERS_GUARD(c, "meao_halo_rows");
     Range r[5]; halo_ranges(c, side, send != 0, r);
     for (int k = 1; k <= 4; k++) { out8[2 * (k - 1)] = r[k].lo; out8[2 * (k - 1) + 1] = r[k].hi; }
     return MEAO_OK;
@@ -894,6 +943,7 @@ int64_t meao_halo_recv_bytes(MeaoCtx *c, int32_t side) { return halo_size(c, sid
 
 static int halo_copy(MeaoCtx *c, int side, void *packed, bool pack, void *stream)
 {
+    LAYERS_GUARD(c, pack ? "meao_halo_pack" : "meao_halo_unpack");
     int rc = ensure_ready(c); if (rc) return rc;
     if (side != 0 && side != 1) return fail(c, MEAO_ERR_INVALID, "side must be 0 or 1");
     cudaStream_t s = (cudaStream_t)stream;
@@ -915,6 +965,7 @@ int meao_halo_unpack(MeaoCtx *c, int32_t side, const void *packed, void *stream)
 
 int meao_render_band_prepare(MeaoCtx *c, const void *depth, int32_t kind, void *stream)
 {
+    LAYERS_GUARD(c, "meao_render_band_prepare");
     int rc = ensure_ready(c); if (rc) return rc;
     if (!depth) return fail(c, MEAO_ERR_INVALID, "depth is NULL");
     return record_downsample(c, depth, kind, (cudaStream_t)stream);
@@ -922,6 +973,7 @@ int meao_render_band_prepare(MeaoCtx *c, const void *depth, int32_t kind, void *
 
 int meao_render_band_finish(MeaoCtx *c, void *ao_out, void *stream)
 {
+    LAYERS_GUARD(c, "meao_render_band_finish");
     int rc = ensure_ready(c); if (rc) return rc;
     cudaStream_t s = (cudaStream_t)stream;
     const int kind = c->last_kind;
@@ -1022,6 +1074,7 @@ static int launch_cached(MeaoCtx *c, const MeaoCtx::GraphKey &key, cudaStream_t 
 
 int meao_band_phase_a(MeaoCtx *c, const void *depth, int32_t kind, void *send_up, void *send_down, void *stream)
 {
+    LAYERS_GUARD(c, "meao_band_phase_a");
     int rc = ensure_ready(c); if (rc) return rc;
     if (!depth) return fail(c, MEAO_ERR_INVALID, "depth is NULL");
     c->last_kind = kind;
@@ -1037,6 +1090,7 @@ int meao_band_phase_a(MeaoCtx *c, const void *depth, int32_t kind, void *send_up
 
 int meao_band_phase_b(MeaoCtx *c, const void *recv_up, const void *recv_down, void *ao_out, void *stream)
 {
+    LAYERS_GUARD(c, "meao_band_phase_b");
     int rc = ensure_ready(c); if (rc) return rc;
     if (!ao_out) return fail(c, MEAO_ERR_INVALID, "ao_out is NULL");
     const int kind = c->last_kind;
@@ -1067,6 +1121,7 @@ constexpr uint32_t kPeerMagic = 0x4d45414fu;
 
 int meao_band_export(MeaoCtx *c, MeaoPeerHandle *out)
 {
+    LAYERS_GUARD(c, "meao_band_export");
     int rc = ensure_ready(c); if (rc) return rc;
     if (!out) return fail(c, MEAO_ERR_INVALID, "out is NULL");
     PeerHandlePod h{};
@@ -1081,6 +1136,7 @@ int meao_band_export(MeaoCtx *c, MeaoPeerHandle *out)
 
 int meao_band_connect(MeaoCtx *c, int32_t side, const MeaoPeerHandle *peer)
 {
+    LAYERS_GUARD(c, "meao_band_connect");
     int rc = ensure_ready(c); if (rc) return rc;
     if (side != 0 && side != 1) return fail(c, MEAO_ERR_INVALID, "side must be 0 (up) or 1 (down)");
     drop_graph(c);                                  // captured band steps carry the old peer pointers
@@ -1158,6 +1214,7 @@ static int record_exchange(MeaoCtx *c, cudaStream_t s)
 
 int meao_band_step(MeaoCtx *c, const void *depth, int32_t kind, void *ao_out, void *stream)
 {
+    LAYERS_GUARD(c, "meao_band_step");
     int rc = ensure_ready(c); if (rc) return rc;
     if (!depth || !ao_out) return fail(c, MEAO_ERR_INVALID, "depth / ao_out is NULL");
     if ((c->prev0 >= 0 && !c->peer_base[0]) || (c->next1 >= 0 && !c->peer_base[1]))
@@ -1180,6 +1237,7 @@ int meao_band_step(MeaoCtx *c, const void *depth, int32_t kind, void *ao_out, vo
 
 int meao_band_step_host(MeaoCtx *c, const void *depth_host, int32_t kind, uint8_t *ao_host)
 {
+    LAYERS_GUARD(c, "meao_band_step_host");
     int rc = ensure_ready(c); if (rc) return rc;
     if (!depth_host || !ao_host) return fail(c, MEAO_ERR_INVALID, "depth / ao_out is NULL");
     if (kind < MEAO_DEPTH_RAW_F32 || kind > MEAO_DEPTH_RAW_D24S8) return fail(c, MEAO_ERR_INVALID, "bad depth kind %d", kind);
@@ -1229,7 +1287,7 @@ int meao_render_host_async(MeaoCtx *c, const void *depth_host, int32_t kind, uin
     int rc = ensure_ready(c); if (rc) return rc;
     if (!depth_host || !ao_host) return fail(c, MEAO_ERR_INVALID, "depth / ao_out is NULL");
     if (slot != 0 && slot != 1) return fail(c, MEAO_ERR_INVALID, "slot must be 0 or 1");
-    const size_t rows = (size_t)(c->band1 - c->band0);
+    const size_t rows = (size_t)(c->band1 - c->band0) * c->layers;      // layered: L images of H rows (no band)
     cudaStream_t s = c->slot_stream[slot];
     const size_t esz = (kind == MEAO_DEPTH_RAW_D16_UNORM) ? 2 : 4;
     CUDA_TRY(c, cudaMemcpyAsync(c->depth_stage[slot], depth_host, rows * c->W * esz, cudaMemcpyHostToDevice, s));
@@ -1319,7 +1377,7 @@ int meao_get_buffer(MeaoCtx *c, int32_t id, void *host_out, size_t host_bytes)
     int rc = ensure_ready(c); if (rc) return rc;
     int lvl, slices, elem;
     if (!host_out || buffer_info(c, id, &lvl, &slices, &elem)) return fail(c, MEAO_ERR_INVALID, "bad buffer id %d", id);
-    const size_t need = (size_t)c->lw[lvl] * c->lh[lvl] * slices * elem;
+    const size_t one = (size_t)c->lw[lvl] * c->lh[lvl] * slices * elem, need = one * c->layers;     // [L][reference layout]
     if (host_bytes < need) return fail(c, MEAO_ERR_INVALID, "buffer %d needs %zu bytes, got %zu", id, need, host_bytes);
     CUDA_TRY(c, cudaDeviceSynchronize());     // debug path: frames may be in flight on any caller stream
     if (slices == 16) {
@@ -1327,7 +1385,10 @@ int meao_get_buffer(MeaoCtx *c, int32_t id, void *host_out, size_t host_bytes)
         __half *tmp = nullptr;
         CUDA_TRY(c, cudaMalloc(&tmp, need));
         const float pad = host_f16_round((c->last_kind != MEAO_DEPTH_LINEAR_F32) ? c->plan.pad[k] : 0.0f);
-        cudaError_t e = launch_synth_tiled(c->low[k], c->lw[k], c->lh[k], c->low_pitch[k], c->lw[k + 2], c->lh[k + 2], pad, tmp, c->stream);
+        cudaError_t e = cudaSuccess;
+        for (int l = 0; l < c->layers && e == cudaSuccess; l++)
+            e = launch_synth_tiled(c->low[k] + (size_t)l * c->lh[k] * c->low_pitch[k], c->lw[k], c->lh[k], c->low_pitch[k], c->lw[k + 2], c->lh[k + 2],
+                                   pad, (__half *)((char *)tmp + l * one), c->stream);
         if (e == cudaSuccess) e = cudaMemcpyAsync(host_out, tmp, need, cudaMemcpyDeviceToHost, c->stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
         cudaFree(tmp);
@@ -1344,7 +1405,7 @@ int meao_get_buffer(MeaoCtx *c, int32_t id, void *host_out, size_t host_bytes)
         if ((rc = record_upsample(c, 1, nullptr, c->stream))) return rc;
         c->launches = before;
     }
-    CUDA_TRY(c, cudaMemcpy2DAsync(host_out, wb, p, pitch, wb, c->lh[lvl], cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(c, cudaMemcpy2DAsync(host_out, wb, p, pitch, wb, (size_t)c->lh[lvl] * c->layers, cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     return MEAO_OK;
 }
@@ -1374,8 +1435,15 @@ int meao_debug_view(MeaoCtx *c, int32_t id, void *out, void *stream)
         buffer_ptr(c, id, &p, &pitch);
         a.src = p; a.elem = elem; a.spitch = (int)(pitch / elem); a.sw = c->lw[lvl]; a.sh = c->lh[lvl];
     }
-    CUDA_TRY(c, launch_debug_view(a, s));
-    c->launches++;
+    // layered: L images, each from its own layer of the source
+    const size_t src_layer = (slices == 16 ? (size_t)c->lh[id - 5] * c->low_pitch[id - 5] * 4 : (size_t)a.sh * a.spitch * a.elem);
+    for (int l = 0; l < c->layers; l++) {
+        DebugViewArgs al = a;
+        al.src = (const char *)a.src + l * src_layer;
+        al.out = a.out + (size_t)l * c->W * c->H;
+        CUDA_TRY(c, launch_debug_view(al, s));
+        c->launches++;
+    }
     return MEAO_OK;
 }
 
@@ -1385,13 +1453,13 @@ int meao_set_buffer(MeaoCtx *c, int32_t id, const void *host_in, size_t host_byt
     int lvl, slices, elem;
     if (!host_in || buffer_info(c, id, &lvl, &slices, &elem) || slices != 1)
         return fail(c, MEAO_ERR_INVALID, "buffer id %d cannot be set", id);
-    const size_t need = (size_t)c->lw[lvl] * c->lh[lvl] * elem;
+    const size_t need = (size_t)c->lw[lvl] * c->lh[lvl] * elem * c->layers;      // [L][h][w]
     if (host_bytes < need) return fail(c, MEAO_ERR_INVALID, "buffer %d needs %zu bytes, got %zu", id, need, host_bytes);
     void *p; size_t pitch;
     buffer_ptr(c, id, &p, &pitch);
     const size_t wb = (size_t)c->lw[lvl] * elem;
     CUDA_TRY(c, cudaDeviceSynchronize());
-    CUDA_TRY(c, cudaMemcpy2DAsync(p, pitch, host_in, wb, wb, c->lh[lvl], cudaMemcpyHostToDevice, c->stream));
+    CUDA_TRY(c, cudaMemcpy2DAsync(p, pitch, host_in, wb, wb, (size_t)c->lh[lvl] * c->layers, cudaMemcpyHostToDevice, c->stream));
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     return MEAO_OK;
 }
@@ -1453,7 +1521,7 @@ int meao_composite_framebuffer(MeaoCtx *c, const void *ao, void *color, int32_t 
 {
     int rc = ensure_ready(c); if (rc) return rc;
     if ((rc = composite_args(c, ao, color, fmt))) return rc;
-    const long long npix = (long long)c->W * (c->band1 - c->band0);
+    const long long npix = (long long)c->W * (c->band1 - c->band0) * c->layers;
     CUDA_TRY(c, launch_composite((const uint8_t *)ao, color, npix, fmt == MEAO_FMT_RGBA16_FLOAT, 1, 1, 0, (cudaStream_t)stream));
     c->launches++;
     return MEAO_OK;
@@ -1463,7 +1531,7 @@ int meao_composite_gbuffer(MeaoCtx *c, const void *ao, void *g0, void *g3, int32
 {
     int rc = ensure_ready(c); if (rc) return rc;
     if ((rc = composite_args(c, ao, g0, MEAO_FMT_RGBA8_UNORM)) || (rc = composite_args(c, ao, g3, fmt3))) return rc;
-    const long long npix = (long long)c->W * (c->band1 - c->band0);
+    const long long npix = (long long)c->W * (c->band1 - c->band0) * c->layers;
     CUDA_TRY(c, launch_composite((const uint8_t *)ao, g0, npix, 0, 0, 1, 1, (cudaStream_t)stream));                               // gbuffer0.a
     CUDA_TRY(c, launch_composite((const uint8_t *)ao, g3, npix, fmt3 == MEAO_FMT_RGBA16_FLOAT, 1, 0, 1, (cudaStream_t)stream));   // gbuffer3.rgb
     c->launches += 2;
@@ -1474,7 +1542,7 @@ int meao_composite_debug(MeaoCtx *c, const void *view, void *color, int32_t fmt,
 {
     int rc = ensure_ready(c); if (rc) return rc;
     if ((rc = composite_args(c, view, color, fmt))) return rc;
-    const long long npix = (long long)c->W * (c->band1 - c->band0);
+    const long long npix = (long long)c->W * (c->band1 - c->band0) * c->layers;
     CUDA_TRY(c, launch_debug_composite((const uint8_t *)view, color, npix, fmt == MEAO_FMT_RGBA16_FLOAT, (cudaStream_t)stream));
     c->launches++;
     return MEAO_OK;
@@ -1516,7 +1584,7 @@ int meao_kernels_per_frame(const MeaoCtx *c)
 int64_t meao_algorithmic_bytes(const MeaoCtx *c, int32_t stage)
 {
     if (!c || c->W <= 0) return MEAO_ERR_INVALID;
-    auto px = [&](int l) { return (int64_t)c->lw[l] * c->lh[l]; };
+    auto px = [&](int l) { return (int64_t)c->lw[l] * c->lh[l] * c->layers; };      // every layer moves the same bytes
     // SURVEY.md 8(d): every buffer of the reference data-flow read once per consuming stage, written once
     const int64_t ds1 = 6 * px(0) + 4 * px(1) + 4 * px(2) + 32 * px(3) + 32 * px(4);
     const int64_t ds2 = 4 * px(2) + 4 * px(3) + 4 * px(4) + 32 * px(5) + 32 * px(6);
