@@ -56,6 +56,10 @@ namespace MiniEngineAO
         [DllImport(Lib)] public static extern int meao_render(IntPtr ctx, IntPtr depthDev, int depthKind, IntPtr aoOutDev, IntPtr stream);
         [DllImport(Lib)] public static extern int meao_render_host(IntPtr ctx, float[] depth, int depthKind, byte[] aoOut);
         [DllImport(Lib)] public static extern int meao_bind_event(IntPtr ctx, int eventId, IntPtr depthDev, int depthKind, IntPtr aoOutDev, IntPtr stream);
+        // CUDA arrays (graphics interop: cudaGraphicsSubResourceGetMappedArray / level 0 of a Vulkan mipmapped array), no copies
+        [DllImport(Lib)] public static extern int meao_render_arrays(IntPtr ctx, IntPtr depthArray, int depthKind, IntPtr aoArray, IntPtr stream);
+        [DllImport(Lib)] public static extern int meao_bind_event_arrays(IntPtr ctx, int eventId, IntPtr depthArray, int depthKind, IntPtr aoArray, IntPtr stream);
+        [DllImport(Lib)] public static extern int meao_release_array(IntPtr ctx, IntPtr array);   // before the array is unmapped / unregistered / freed
         [DllImport(Lib)] public static extern IntPtr meao_get_render_event_func();
         [DllImport(Lib)] public static extern int meao_composite_framebuffer(IntPtr ctx, IntPtr aoDev, IntPtr colorDev, int colorFormat, IntPtr stream);
         [DllImport(Lib)] public static extern int meao_composite_gbuffer(IntPtr ctx, IntPtr aoDev, IntPtr gbuffer0Dev, IntPtr gbuffer3Dev, int gbuffer3Format, IntPtr stream);
@@ -114,6 +118,10 @@ namespace MiniEngineAO
         IntPtr _ctx = IntPtr.Zero;
         CommandBuffer _renderCommand;
         IntPtr _depthDev = IntPtr.Zero, _aoDev = IntPtr.Zero;   // mapped by the engine-specific interop layer
+        // ... or, when the interop layer maps the textures as CUDA arrays (cudaArray_t of the depth copy and the R8 AO target,
+        // registered with cudaGraphicsRegisterFlagsSurfaceLoadStore), those: the plugin event then reads and writes them directly
+        IntPtr _depthArray = IntPtr.Zero, _aoArray = IntPtr.Zero;
+        int _depthArrayKind = 0;                                // MEAO_DEPTH_RAW_F32 (R32_FLOAT copy) or 2 = RAW_D16_UNORM (R16 copy)
         IntPtr _stream = IntPtr.Zero;                           // cudaStream_t the plugin event renders on (ABI 3; Zero = legacy default stream)
 
         void LateUpdate()
@@ -169,11 +177,28 @@ namespace MiniEngineAO
             if (_renderCommand == null) _renderCommand = new CommandBuffer { name = "SSAO" };   // :481-482
             else _camera.RemoveCommandBuffer(CameraEvent.BeforeImageEffects, _renderCommand);
             _renderCommand.Clear();
-            // (engine-specific: map _CameraDepthTexture and the R8 AO render texture to _depthDev / _aoDev)
-            MeaoNative.Check(_ctx, MeaoNative.meao_bind_event(_ctx, kEventId, _depthDev, 0 /* MEAO_DEPTH_RAW_F32 */, _aoDev, _stream));
+            // (engine-specific: map _CameraDepthTexture and the R8 AO render texture to _depthDev / _aoDev, or to _depthArray / _aoArray)
+            if (_depthArray != IntPtr.Zero) BindEventArrays();
+            else MeaoNative.Check(_ctx, MeaoNative.meao_bind_event(_ctx, kEventId, _depthDev, 0 /* MEAO_DEPTH_RAW_F32 */, _aoDev, _stream));
             // one plugin event replaces the ten DispatchCompute calls recorded by :511-531
             _renderCommand.IssuePluginEvent(MeaoNative.meao_get_render_event_func(), kEventId);
             _camera.AddCommandBuffer(CameraEvent.BeforeImageEffects, _renderCommand);          // :421
+        }
+
+        // The array path of the plugin event: meao_render_arrays on the mapped arrays (checked here -- the event cannot report errors).
+        void BindEventArrays()
+        {
+            MeaoNative.Check(_ctx, MeaoNative.meao_bind_event_arrays(_ctx, kEventId, _depthArray, _depthArrayKind, _aoArray, _stream));
+        }
+
+        // The interop layer calls this before it unmaps, unregisters or re-creates a texture it handed over as an array: the plugin
+        // caches a surface object and graphs per array, and a new array may come back with the same handle.
+        public void ReleaseArrays()
+        {
+            if (_ctx == IntPtr.Zero) return;
+            if (_depthArray != IntPtr.Zero) MeaoNative.Check(_ctx, MeaoNative.meao_release_array(_ctx, _depthArray));
+            if (_aoArray != IntPtr.Zero) MeaoNative.Check(_ctx, MeaoNative.meao_release_array(_ctx, _aoArray));
+            _depthArray = _aoArray = IntPtr.Zero;
         }
 
         void OnDisable()

@@ -33,7 +33,8 @@ extern "C" {
 #define MEAO_ABI_VERSION 3   /* 2: + MeaoVariants, meao_stage_render_wide, meao_debug_view, meao_composite_debug, buffer ids 18..21
                               * 3: + MeaoVariants.single_scale, native peer halo exchange (meao_band_export / _connect / _step / _status),
                               *      meao_bind_event takes the stream
-                              *    + meao_set_layers (layered frames; additive, so the version stays 3) */
+                              *    + meao_set_layers (layered frames; additive, so the version stays 3)
+                              *    + meao_render_arrays / meao_bind_event_arrays / meao_release_array (CUDA-array I/O; additive) */
 
 typedef struct MeaoCtx MeaoCtx;
 
@@ -171,6 +172,33 @@ int meao_render(MeaoCtx *ctx, const void *depth_dev, int32_t depth_kind, void *a
 /* Same with HOST buffers: H2D copy of depth, the ten passes, D2H copy of the AO texture, then a
  * stream synchronise.  Use meao_host_alloc for pinned memory. */
 int meao_render_host(MeaoCtx *ctx, const void *depth_host, int32_t depth_kind, uint8_t *ao_out_host);
+/* ---- CUDA arrays -------------------------------------------------------------------------------------------------------------
+ * The frame of meao_render with the depth read from, and the AO written into, CUDA arrays -- what graphics interop hands out for a
+ * shared texture (D3D11 / D3D12 / GL: cudaGraphicsSubResourceGetMappedArray; Vulkan: cudaExternalMemoryGetMappedMipmappedArray, then
+ * level 0 through cudaGetMipmappedArrayLevel).  No copy to or from linear memory: the first and the last kernel of the frame access
+ * the arrays through surface objects.  Registering and mapping the resource stays with the host (it is graphics-API specific).
+ * depth_array / ao_array: cudaArray_t, passed as void *.  Checked on the host before anything is launched:
+ *   - depth_kind RAW_F32 / LINEAR_F32: one 32-bit float channel; RAW_D16_UNORM: one 16-bit unsigned channel (normalised or not);
+ *     RAW_D24S8 returns MEAO_ERR_UNSUPPORTED (no CUDA array holds a depth-stencil format).  ao_array: one 8-bit unsigned channel
+ *     (normalised or not; the R8 texture of AO.cs:475).
+ *   - width x height must be the context's; both arrays need cudaArraySurfaceLoadStore (interop: register the resource with
+ *     cudaGraphicsRegisterFlagsSurfaceLoadStore).
+ *   - layers: a 2-D array (or a cudaArrayLayered array of depth 1) has 1, a cudaArrayLayered array of depth n has n, a
+ *     cudaArrayCubemap array 6 (face f = layer f); each must equal meao_set_layers.  The two arrays may be of different shapes.
+ *     Cube-map arrays (cudaArrayCubemap | cudaArrayLayered) return MEAO_ERR_UNSUPPORTED.
+ *   - a context with a row band (meao_set_row_band) returns MEAO_ERR_UNSUPPORTED.
+ * A refused call returns MEAO_ERR_INVALID / MEAO_ERR_UNSUPPORTED with meao_last_error naming the field, and launches nothing.
+ * The result is bit-identical to meao_render on the same depth; graphs are captured and replayed per (depth_array, ao_array, kind)
+ * like meao_render's, and meao_get_buffer / meao_debug_view of the AO (id 17) regenerate the context's own copy as after a pointer
+ * frame.  meao_kernels_per_frame is unchanged.
+ * RELEASE CONTRACT: the context caches a surface object per array and the graphs that use it; both describe the array's MEMORY.
+ * Before freeing, unmapping or re-registering an array this context has rendered with (or bound with meao_bind_event_arrays), call
+ * meao_release_array(ctx, array): it synchronises the device, drops that array's graphs, surface object and event bindings.  A new
+ * array may come back with the same handle, and without the release the next frame would replay into freed memory.
+ * meao_destroy and every plan change (meao_resize, meao_set_layers, meao_set_params / _variants / _camera changes, meao_set_row_band)
+ * release all arrays.  Releasing an array this context never used returns MEAO_OK. */
+int meao_render_arrays(MeaoCtx *ctx, const void *depth_array, int32_t depth_kind, void *ao_array, void *stream);
+int meao_release_array(MeaoCtx *ctx, const void *array);
 /* Pipelined form of meao_render_host for frame streams: enqueues H2D + kernels + D2H of one frame on staging slot
  * `slot` (0 or 1) and returns; meao_host_wait(slot) blocks until that frame's AO is in ao_out_host.  Alternating the
  * two slots overlaps the H2D copy of frame i+1 with the kernels and the D2H copy of frame i (the kernels of
@@ -321,6 +349,10 @@ int meao_composite_debug(MeaoCtx *ctx, const void *view_r8_dev, void *color_dev,
 typedef void (*MeaoRenderEventFunc)(int event_id);
 /* stream: the cudaStream_t the plugin event renders on (ABI 3; NULL = the CUDA legacy default stream, as before). */
 int meao_bind_event(MeaoCtx *ctx, int32_t event_id, const void *depth_dev, int32_t depth_kind, void *ao_out_dev, void *stream);
+/* The array twin of meao_bind_event: the event renders meao_render_arrays(ctx, depth_array, depth_kind, ao_array, stream).  The arrays
+ * are checked now (the event cannot report an error), with the statuses of meao_render_arrays; both NULL unbinds.  An id holds one
+ * binding: binding it again, with either call, replaces it.  meao_release_array also removes the bindings that name the array. */
+int meao_bind_event_arrays(MeaoCtx *ctx, int32_t event_id, const void *depth_array, int32_t depth_kind, void *ao_array, void *stream);
 void meao_render_event(int event_id);
 MeaoRenderEventFunc meao_get_render_event_func(void);
 

@@ -196,6 +196,25 @@ class AmbientOcclusion:
         self._check(self._lib.meao_render(self._ctx, depth.data_ptr(), kind, out.data_ptr(), self._stream(stream)))
         return out
 
+    _ARRAY_KINDS = {"raw_f32": N.MEAO_DEPTH_RAW_F32, "linear_f32": N.MEAO_DEPTH_LINEAR_F32, "d16": N.MEAO_DEPTH_RAW_D16_UNORM,
+                    "d24s8": N.MEAO_DEPTH_RAW_D24S8}
+
+    def render_arrays(self, depth_array: int, ao_array: int, *, kind: str = "raw_f32", stream=None) -> None:
+        """The frame with the depth read from and the AO written into CUDA arrays (meao_render_arrays): integer cudaArray_t handles,
+        e.g. from graphics interop.  kind: "raw_f32", "linear_f32" or "d16" (the array's one channel: f32 / f32 / 16-bit unsigned).
+        The arrays must be W x H with the context's layer count (2-D: 1, layered: its depth, cube map: 6) and carry
+        cudaArraySurfaceLoadStore.  Call release_array before freeing an array this context has rendered with."""
+        if kind not in self._ARRAY_KINDS:
+            raise ValueError(f"kind must be one of {sorted(self._ARRAY_KINDS)}")
+        self.LateUpdate()
+        self._check(self._lib.meao_render_arrays(self._ctx, C.c_void_p(depth_array), self._ARRAY_KINDS[kind], C.c_void_p(ao_array),
+                                                 self._stream(stream)))
+
+    def release_array(self, handle: int) -> None:
+        """Drop the graphs, the surface object and the event bindings that refer to a CUDA array (meao_release_array; synchronises
+        the device).  Required before the array is freed or re-registered: a new array may come back with the same handle."""
+        self._check(self._lib.meao_release_array(self._ctx, C.c_void_p(handle)))
+
     def render_host(self, depth: np.ndarray, out: np.ndarray | None = None, *, linear: bool = False) -> np.ndarray:
         """Host [H, W] depth ([layers, H, W] when layers > 1; float32 / uint16 D16 codes / uint32 D24S8 words) in, host uint8 of the
         same shape out (H2D + the kernels + D2H + sync)."""

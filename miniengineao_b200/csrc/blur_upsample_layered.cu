@@ -13,23 +13,7 @@ namespace {
 
 #include "blur_upsample_device.inc"
 
-// The arguments of layer l: every image advances by whole pitched images of its level (rows x pitch).  out_row_origin is 0 in a
-// layered frame (no row band), so the output advances by hih rows like the other hi-res images.
-__device__ __forceinline__ UpsampleArgs layer_args(const UpsampleArgs &a, int l)
-{
-    UpsampleArgs r = a;
-    const size_t lo = (size_t)l * a.loh, hi = (size_t)l * a.hih;
-    r.lo_depth = a.lo_depth + lo * a.lo_dpitch;
-    r.lo_ao = a.lo_ao + lo * a.lo_apitch;
-    r.hi_depth = reinterpret_cast<const char *>(a.hi_depth) + hi * a.hi_dpitch * (a.hi_is_half ? 2 : 4);
-    r.hi_ao = a.hi_ao + hi * a.hi_apitch;          // hi_apitch == 0 when there is no hi-res AO (kernel "main")
-    r.out = a.out + hi * a.out_pitch;
-    return r;
-}
-__device__ __forceinline__ UpsamplePreminArgs layer_args(const UpsamplePreminArgs &pa, int l)
-{
-    return UpsamplePreminArgs{layer_args(pa.base, l), pa.lo_ao2 + (size_t)l * pa.base.loh * pa.lo_a2pitch, pa.lo_a2pitch};
-}
+#include "blur_upsample_layer_args.inc"
 
 #define MEAO_UPS_LAYERED 1
 #define MEAO_UPS_PREMIN 0

@@ -9,6 +9,7 @@
 
 #ifdef MEAO_EMULATE              // tests/emu only (see common.cuh)
 #include "cuda_emu.h"
+#include "cuda_emu_surface.h"     // cudaSurfaceObject_t and the surface calls of the CUDA-array kernels
 #else
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -137,6 +138,17 @@ cudaError_t launch_render_ao_layered(const CUtensorMap &low_map, bool use_tma, c
 cudaError_t launch_blur_upsample_layered(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
                                          const UpsampleArgs &a, const uint8_t *lo_ao2, int lo_a2pitch, int layers, int sm_count, cudaStream_t s);
 
+// ---- CUDA arrays (meao_render_arrays): the depth read from, the AO written into a 2-D / layered / cube-map array --------------------
+// The first and the last kernel of the frame in a form that reaches the array through a surface object (surface_io.cuh: kSurf2D /
+// kSurfLayered / kSurfCube); the arguments are the layered ones (layers >= 1, whole frame), the intermediates stay in the arena and the
+// other kernels are the existing ones.  prepare: in_format f32 or D16 (no CUDA array holds D24S8); upsample: the final level only
+// (hi_depth = LinearDepth, no hi_ao; a.out is unused).  Separate kernels and translation units (*_array.cu).
+enum { kSurf2D = 0, kSurfLayered = 1, kSurfCube = 2 };    // how a surface's layer coordinate is addressed (the array's shape)
+cudaError_t launch_prepare_depth_array(const PrepareArgs &a, cudaSurfaceObject_t depth, int surf_kind, int layers, cudaStream_t s);
+cudaError_t launch_blur_upsample_array(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
+                                       const UpsampleArgs &a, const uint8_t *lo_ao2, int lo_a2pitch, int layers, int sm_count,
+                                       cudaSurfaceObject_t out, int surf_kind, cudaStream_t s);
+
 // ---- debug: synthesise a TiledDepth<k> view (reference layout [16][sh][sw], f16 bits) ----------
 cudaError_t launch_synth_tiled(const float *low, int lw, int lh, int lpitch, int sw, int sh, float pad,
                                __half *out, cudaStream_t s);
@@ -199,6 +211,8 @@ cudaError_t preload_blur_upsample();
 cudaError_t preload_prepare_depth_layered();
 cudaError_t preload_render_ao_layered();
 cudaError_t preload_blur_upsample_layered();
+cudaError_t preload_prepare_depth_array();
+cudaError_t preload_blur_upsample_array();
 cudaError_t preload_band_kernels();
 cudaError_t preload_aux_kernels();      // composite, debug views, self test
 #endif

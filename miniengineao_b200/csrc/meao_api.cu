@@ -128,6 +128,8 @@ struct MeaoCtx {
     // CUDA graph cache: one instantiated graph per (depth, out, kind), LRU; when it is full the least recently used
     // executable graph is RE-TARGETED in place with cudaGraphExecUpdate (same topology, new pointers: no device
     // synchronisation, launches already enqueued are unaffected).  Dropped as a whole only when the plan changes.
+    // kind: the depth kind of a pointer frame; 100+ / 200+ / 300+ band graphs; kArrayGraphKind+ array frames (the key holds
+    // cudaArray_t handles, so a pointer equal to a handle value never finds an array frame's graph, nor the reverse).
     struct GraphKey { const void *p[4]; int kind; bool operator<(const GraphKey &o) const {
         for (int i = 0; i < 4; i++) if (p[i] != o.p[i]) return p[i] < o.p[i];
         return kind < o.kind; } };
@@ -136,7 +138,12 @@ struct MeaoCtx {
     std::vector<cudaGraphExec_t> retired;   // executable graphs replaced while possibly in flight: destroyed at the next drop_graph
     uint64_t graph_clock = 0;
     bool graphs_stale = false;              // set by the device-less getters: dropped by the next ensure_ready (on the right device)
-    void *last_out = nullptr;               // where the last final upsample wrote (nullptr: c->result)
+    void *last_out = nullptr;               // where the last final upsample wrote (nullptr: c->result; an array frame: its AO array)
+    // CUDA-array frames (meao_render_arrays): one surface object per cudaArray_t this context has rendered with, made on first use.
+    // A surface object describes the memory of its array, so it lives exactly as long as the graphs that launch with it: it is
+    // destroyed by meao_release_array (that array) and drop_graph (all), both after a device synchronise -- never while a launch
+    // that uses it may still be in flight.
+    std::map<const void *, cudaSurfaceObject_t> surfaces;
     int last_kind = MEAO_DEPTH_RAW_F32;     // ingest kind of the last downsample (selects the atlas padding value)
 
     std::vector<std::pair<std::string, float>> last_profile;
@@ -245,12 +252,14 @@ void build_plan(MeaoCtx *c)
 void drop_graph(MeaoCtx *c)
 {
     c->graphs_stale = false;
-    if (c->graphs.empty() && c->retired.empty()) return;
-    cudaDeviceSynchronize();            // a re-plan is rare; never destroy an executable graph that may still be in flight
+    if (c->graphs.empty() && c->retired.empty() && c->surfaces.empty()) return;
+    cudaDeviceSynchronize();            // a re-plan is rare; never destroy an executable graph (or surface) that may still be in flight
     for (auto &kv : c->graphs) cudaGraphExecDestroy(kv.second.exec);
     for (auto ge : c->retired) cudaGraphExecDestroy(ge);
+    for (auto &kv : c->surfaces) cudaDestroySurfaceObject(kv.second);
     c->graphs.clear();
     c->retired.clear();
+    c->surfaces.clear();
 }
 
 void disconnect_peers(MeaoCtx *c)
@@ -451,8 +460,11 @@ int render_tile_variant(const MeaoCtx *c, int k, int rows)
 
 // ---- the three recorders ---------------------------------------------------------------------
 
-// PushDownsampleCommands, AO.cs:604-658
-int record_downsample(MeaoCtx *c, const void *depth, int kind, cudaStream_t s)
+// A CUDA-array frame (meao_render_arrays): the surfaces of the depth and AO arrays and how their layers are addressed (surface_io.cuh).
+struct ArrayIO { cudaSurfaceObject_t depth, ao; int depth_surf, ao_surf; const void *ao_array; };
+
+// PushDownsampleCommands, AO.cs:604-658.  aio: read the depth from a CUDA array instead of `depth`.
+int record_downsample(MeaoCtx *c, const void *depth, int kind, cudaStream_t s, const ArrayIO *aio = nullptr)
 {
     if (kind < MEAO_DEPTH_RAW_F32 || kind > MEAO_DEPTH_RAW_D24S8) return fail(c, MEAO_ERR_INVALID, "bad depth kind %d", kind);
     NvtxRange nv("meao::prepare_depth");
@@ -469,7 +481,8 @@ int record_downsample(MeaoCtx *c, const void *depth, int kind, cudaStream_t s)
     a.reversed_z = c->camera.reversed_z;
     a.vec_ok = (((uintptr_t)depth & 15) == 0) && (c->W % (a.in_format == 1 ? 8 : 4) == 0);
     c->last_kind = kind;
-    if (c->layers > 1) CUDA_TRY(c, launch_prepare_depth_layered(a, c->layers, s));
+    if (aio) CUDA_TRY(c, launch_prepare_depth_array(a, aio->depth, aio->depth_surf, c->layers, s));
+    else if (c->layers > 1) CUDA_TRY(c, launch_prepare_depth_layered(a, c->layers, s));
     else CUDA_TRY(c, launch_prepare_depth(a, s));
     c->launches++;
     return 0;
@@ -511,8 +524,8 @@ int record_render(MeaoCtx *c, int k, int kind, cudaStream_t s, bool wide = false
 }
 inline bool hq_level(const MeaoCtx *c, int k) { return ((c->variants.high_quality_mask >> (k - 1)) & 1) != 0; }
 
-// PushUpsampleCommands with the wiring of AO.cs:528-531
-int record_upsample(MeaoCtx *c, int lo, void *ao_out, cudaStream_t s)
+// PushUpsampleCommands with the wiring of AO.cs:528-531.  aio (final level only): store the AO into a CUDA array instead of ao_out.
+int record_upsample(MeaoCtx *c, int lo, void *ao_out, cudaStream_t s, const ArrayIO *aio = nullptr)
 {
     const int hi = lo - 1;
     NvtxRange nv("meao::blur_upsample");
@@ -525,7 +538,7 @@ int record_upsample(MeaoCtx *c, int lo, void *ao_out, cudaStream_t s)
     if (hi == 0) {
         if (ao_out) { a.out = (uint8_t *)ao_out; a.out_pitch = c->W; a.out_row_origin = c->band0; }
         else { a.out = c->result; a.out_pitch = c->result_pitch; a.out_row_origin = 0; }
-        c->last_out = ao_out;
+        c->last_out = aio ? const_cast<void *>(aio->ao_array) : ao_out;
     } else { a.out = c->comb[hi]; a.out_pitch = c->occ_pitch[hi]; a.out_row_origin = 0; }
     a.out_vec_ok = (((uintptr_t)a.out & 7) == 0) && (a.out_pitch % 8 == 0);
     a.hiw = c->lw[hi]; a.hih = c->lh[hi];
@@ -538,7 +551,10 @@ int record_upsample(MeaoCtx *c, int lo, void *ao_out, cudaStream_t s)
     a.tile_ctr = c->tile_ctr + 2 * (lo - 1);
     const uint8_t *lo_ao2 = hq_level(c, lo) ? c->hq[lo] : nullptr;                   // kernels main_premin / main_premin_blendout
     const CUtensorMap &ao_map = single ? c->map_occ1_ups : c->map_ao_ups[lo];
-    if (c->layers > 1)
+    if (aio && hi == 0)
+        CUDA_TRY(c, launch_blur_upsample_array(c->map_low_ups[lo], ao_map, &c->map_hq_ups[lo], c->tma_ok, a, lo_ao2, c->occ_pitch[lo], c->layers, c->sm_count,
+                                               aio->ao, aio->ao_surf, s));
+    else if (c->layers > 1)
         CUDA_TRY(c, launch_blur_upsample_layered(c->map_low_ups[lo], ao_map, &c->map_hq_ups[lo], c->tma_ok, a, lo_ao2, c->occ_pitch[lo], c->layers, c->sm_count, s));
     else CUDA_TRY(c, launch_blur_upsample(c->map_low_ups[lo], ao_map, &c->map_hq_ups[lo], c->tma_ok, a, lo_ao2, c->occ_pitch[lo], c->sm_count, s));
     c->launches++;
@@ -555,18 +571,19 @@ struct PdlScope { bool prev; explicit PdlScope(bool on) : prev(g_launch_pdl) { g
 // the same stream; 2 = also on kernels that additionally wait for an event of another branch.  after_exchange: the node
 // before this DAG is the neighbour-exchange kernel, which spins on remote flags -- nothing may be scheduled "early" behind it
 // (a grid parked in griddepcontrol.wait holds SM resources that the neighbour band's kernels may need: see DESIGN.md 4).
+// aio: a CUDA-array frame -- the first and the last node read / write the arrays (depth and ao_out are unused).
 int record_frame_dag(MeaoCtx *c, const void *depth, int kind, void *ao_out, cudaStream_t s, bool do_prepare = true, int pdl = 0,
-                     bool after_exchange = false)
+                     bool after_exchange = false, const ArrayIO *aio = nullptr)
 {
     int rc;
     if (c->variants.single_scale) {     // BASELINE.json configs[0]: Downsample1 -> Render level 1 -> final-style Upsample on Occlusion1
-        if (do_prepare && (rc = record_downsample(c, depth, kind, s))) return rc;
+        if (do_prepare && (rc = record_downsample(c, depth, kind, s, aio))) return rc;
         { PdlScope p(pdl >= 1 && !after_exchange); if ((rc = record_render(c, 1, kind, s))) return rc; }
-        { PdlScope p(pdl >= 1); if ((rc = record_upsample(c, 1, ao_out, s))) return rc; }
+        { PdlScope p(pdl >= 1); if ((rc = record_upsample(c, 1, ao_out, s, aio))) return rc; }
         return 0;
     }
     cudaStream_t b1 = c->branch[0], b2 = c->branch[1], b3 = c->branch[2];
-    if (do_prepare && (rc = record_downsample(c, depth, kind, s))) return rc;
+    if (do_prepare && (rc = record_downsample(c, depth, kind, s, aio))) return rc;
     CUDA_TRY(c, cudaEventRecord(c->ev[0], s));
     CUDA_TRY(c, cudaStreamWaitEvent(b1, c->ev[0], 0));
     CUDA_TRY(c, cudaStreamWaitEvent(b2, c->ev[0], 0));
@@ -589,7 +606,7 @@ int record_frame_dag(MeaoCtx *c, const void *depth, int kind, void *ao_out, cuda
     CUDA_TRY(c, cudaEventRecord(c->ev[3], b3));
     CUDA_TRY(c, cudaStreamWaitEvent(s, c->ev[3], 0));
     { PdlScope p(pdl >= 2); if ((rc = record_upsample(c, 2, nullptr, s))) return rc; }
-    { PdlScope p(pdl >= 1); if ((rc = record_upsample(c, 1, ao_out, s))) return rc; }
+    { PdlScope p(pdl >= 1); if ((rc = record_upsample(c, 1, ao_out, s, aio))) return rc; }
     return 0;
 }
 
@@ -652,7 +669,7 @@ int buffer_ptr(MeaoCtx *c, int id, void **p, size_t *pitch_bytes)
 }
 
 std::mutex g_event_mutex;
-struct EventBinding { MeaoCtx *ctx; const void *depth; int kind; void *out; void *stream; };
+struct EventBinding { MeaoCtx *ctx; const void *depth; int kind; void *out; void *stream; bool arrays; };   // arrays: meao_bind_event_arrays
 std::map<int, EventBinding> g_events;
 
 }  // namespace
@@ -732,6 +749,8 @@ int meao_create(const MeaoDeviceCfg *cfg, MeaoCtx **out)
             if (pe == cudaSuccess) pe = preload_prepare_depth_layered();
             if (pe == cudaSuccess) pe = preload_render_ao_layered();
             if (pe == cudaSuccess) pe = preload_blur_upsample_layered();
+            if (pe == cudaSuccess) pe = preload_prepare_depth_array();
+            if (pe == cudaSuccess) pe = preload_blur_upsample_array();
             if (pe == cudaSuccess) pe = preload_band_kernels();
             if (pe == cudaSuccess) pe = preload_aux_kernels();
             if (pe != cudaSuccess) { cudaGetLastError(); meao_destroy(c); return fail(nullptr, MEAO_ERR_CUDA, "loading the kernels failed: %s", cudaGetErrorString(pe)); }
@@ -1282,6 +1301,122 @@ int meao_render(MeaoCtx *c, const void *depth, int32_t kind, void *ao_out, void 
     });
 }
 
+// ---- CUDA arrays (include/meao.h "CUDA arrays") ------------------------------------------------------------------------
+namespace {
+constexpr int kArrayGraphKind = 400;        // GraphKey.kind of an array frame: 400 + depth kind
+
+// What a cudaArray_t is, checked against the context on the host before anything is launched.  elem_bits / is_float: the one
+// channel the role needs.  Returns 0 and the layer addressing, or fails with a message naming the field.
+int check_array(MeaoCtx *c, const void *arr, const char *role, int elem_bits, bool is_float, int *surf_kind)
+{
+    cudaChannelFormatDesc d{};
+    cudaExtent e{};
+    unsigned int flags = 0;
+    const cudaError_t err = cudaArrayGetInfo(&d, &e, &flags, (cudaArray_t)arr);
+    if (err != cudaSuccess) { cudaGetLastError(); return fail(c, MEAO_ERR_INVALID, "%s: not a CUDA array (cudaArrayGetInfo: %s)", role, cudaGetErrorString(err)); }
+    const bool one_channel = d.x == elem_bits && d.y == 0 && d.z == 0 && d.w == 0;
+    bool kind_ok;
+    if (is_float) kind_ok = d.f == cudaChannelFormatKindFloat;
+    else kind_ok = d.f == cudaChannelFormatKindUnsigned ||
+                   (elem_bits == 8 && d.f == cudaChannelFormatKindUnsignedNormalized8X1) ||
+                   (elem_bits == 16 && d.f == cudaChannelFormatKindUnsignedNormalized16X1);
+    if (!one_channel || !kind_ok)
+        return fail(c, MEAO_ERR_INVALID, "%s: channel format (%d,%d,%d,%d bits, kind %d) is not one %d-bit %s channel", role, d.x, d.y, d.z, d.w, (int)d.f,
+                    elem_bits, is_float ? "float" : "unsigned (normalised or not)");
+    if ((int)e.width != c->W || (int)e.height != c->H || e.width != (size_t)c->W || e.height != (size_t)c->H)
+        return fail(c, MEAO_ERR_INVALID, "%s: extent %zux%zu differs from the context's %dx%d", role, e.width, e.height, c->W, c->H);
+    if (!(flags & cudaArraySurfaceLoadStore))
+        return fail(c, MEAO_ERR_INVALID, "%s: flags 0x%x lack cudaArraySurfaceLoadStore (register the resource with cudaGraphicsRegisterFlagsSurfaceLoadStore)", role, flags);
+    int layers;
+    if (flags & cudaArrayCubemap) {
+        if (flags & cudaArrayLayered) return fail(c, MEAO_ERR_UNSUPPORTED, "%s: cube-map arrays (cudaArrayCubemap | cudaArrayLayered) are not supported", role);
+        layers = 6; *surf_kind = kSurfCube;
+    } else if (flags & cudaArrayLayered) {
+        layers = e.depth > 0 ? (int)e.depth : 1; *surf_kind = kSurfLayered;
+    } else {
+        if (e.depth > 1) return fail(c, MEAO_ERR_INVALID, "%s: depth %zu: a 3-D array is not a 2-D or layered image", role, e.depth);
+        layers = 1; *surf_kind = kSurf2D;
+    }
+    if (layers != c->layers)
+        return fail(c, MEAO_ERR_INVALID, "%s: layer count %d differs from the context's %d (meao_set_layers)", role, layers, c->layers);
+    return 0;
+}
+
+int surface_of(MeaoCtx *c, const void *arr, cudaSurfaceObject_t *out)
+{
+    auto it = c->surfaces.find(arr);
+    if (it != c->surfaces.end()) { *out = it->second; return 0; }
+    cudaResourceDesc rd{};
+    rd.resType = cudaResourceTypeArray;
+    rd.res.array.array = (cudaArray_t)arr;
+    cudaSurfaceObject_t so = 0;
+    CUDA_TRY(c, cudaCreateSurfaceObject(&so, &rd));
+    c->surfaces.emplace(arr, so);
+    *out = so;
+    return 0;
+}
+
+// every check of meao_render_arrays / meao_bind_event_arrays; on success `io` holds the surfaces of a frame (made on first use)
+int prepare_arrays(MeaoCtx *c, const void *depth_array, int kind, const void *ao_array, ArrayIO *io)
+{
+    if (!depth_array || !ao_array) return fail(c, MEAO_ERR_INVALID, "depth_array / ao_array is NULL");
+    if (kind < MEAO_DEPTH_RAW_F32 || kind > MEAO_DEPTH_RAW_D24S8) return fail(c, MEAO_ERR_INVALID, "bad depth kind %d", kind);
+    if (kind == MEAO_DEPTH_RAW_D24S8) return fail(c, MEAO_ERR_UNSUPPORTED, "depth_kind RAW_D24S8: CUDA arrays have no depth-stencil format");
+    if (c->band0 != 0 || c->band1 != c->H) return fail(c, MEAO_ERR_UNSUPPORTED, "CUDA-array frames need a whole-frame context (no row band)");
+    int rc;
+    const bool d16 = kind == MEAO_DEPTH_RAW_D16_UNORM;
+    if ((rc = check_array(c, depth_array, "depth_array", d16 ? 16 : 32, !d16, &io->depth_surf))) return rc;
+    if ((rc = check_array(c, ao_array, "ao_array", 8, false, &io->ao_surf))) return rc;
+    if ((rc = surface_of(c, depth_array, &io->depth))) return rc;
+    if ((rc = surface_of(c, ao_array, &io->ao))) return rc;
+    io->ao_array = ao_array;
+    return 0;
+}
+}  // namespace
+
+int meao_render_arrays(MeaoCtx *c, const void *depth_array, int32_t kind, void *ao_array, void *stream)
+{
+    int rc = ensure_ready(c); if (rc) return rc;
+    ArrayIO io;
+    if ((rc = prepare_arrays(c, depth_array, kind, ao_array, &io))) return rc;
+    // the frame graph of meao_render with its first and last node reading / writing the arrays
+    NvtxRange nv("meao::frame_arrays");
+    const MeaoCtx::GraphKey key{{depth_array, ao_array, nullptr, nullptr}, kArrayGraphKind + kind};
+    c->last_kind = kind; c->last_out = ao_array;
+    return launch_cached(c, key, (cudaStream_t)stream, meao_kernels_per_frame(c), [&](cudaStream_t cs, int pdl) {
+        return record_frame_dag(c, nullptr, kind, nullptr, cs, true, pdl, false, &io);
+    });
+}
+
+int meao_release_array(MeaoCtx *c, const void *array)
+{
+    if (!c) return MEAO_ERR_INVALID;
+    if (c->plan_only) return fail(c, MEAO_ERR_CUDA, "plan-only context (device < 0): no CUDA device bound, and libmeao has no CPU fallback");
+    if (!array) return fail(c, MEAO_ERR_INVALID, "array is NULL");
+    {   // a plugin event bound to the array would re-create its surface after the array is freed
+        std::lock_guard<std::mutex> g(g_event_mutex);
+        for (auto it = g_events.begin(); it != g_events.end();) {
+            if (it->second.ctx == c && it->second.arrays && (it->second.depth == array || it->second.out == array)) it = g_events.erase(it); else ++it;
+        }
+    }
+    bool used = c->surfaces.count(array) != 0;
+    for (auto &kv : c->graphs) used |= kv.first.kind >= kArrayGraphKind && (kv.first.p[0] == array || kv.first.p[1] == array);
+    if (!used) return MEAO_OK;
+    CUDA_TRY(c, cudaSetDevice(c->device));
+    CUDA_TRY(c, cudaDeviceSynchronize());       // frames that use the array may be in flight on any stream
+    for (auto it = c->graphs.begin(); it != c->graphs.end();) {
+        if (it->first.kind >= kArrayGraphKind && (it->first.p[0] == array || it->first.p[1] == array)) {
+            cudaGraphExecDestroy(it->second.exec);
+            it = c->graphs.erase(it);
+        } else ++it;
+    }
+    for (auto ge : c->retired) cudaGraphExecDestroy(ge);      // a retired graph may be an array frame: none is in flight any more
+    c->retired.clear();
+    auto s = c->surfaces.find(array);
+    if (s != c->surfaces.end()) { cudaDestroySurfaceObject(s->second); c->surfaces.erase(s); }
+    return MEAO_OK;
+}
+
 int meao_render_host_async(MeaoCtx *c, const void *depth_host, int32_t kind, uint8_t *ao_host, int32_t slot)
 {
     int rc = ensure_ready(c); if (rc) return rc;
@@ -1553,7 +1688,24 @@ int meao_bind_event(MeaoCtx *c, int32_t event_id, const void *depth, int32_t kin
     if (!c) return MEAO_ERR_INVALID;
     std::lock_guard<std::mutex> g(g_event_mutex);
     if (!depth && !ao_out) { g_events.erase(event_id); return MEAO_OK; }
-    g_events[event_id] = EventBinding{c, depth, kind, ao_out, stream};
+    g_events[event_id] = EventBinding{c, depth, kind, ao_out, stream, false};
+    return MEAO_OK;
+}
+
+int meao_bind_event_arrays(MeaoCtx *c, int32_t event_id, const void *depth_array, int32_t kind, void *ao_array, void *stream)
+{
+    if (!c) return MEAO_ERR_INVALID;
+    if (!depth_array && !ao_array) {
+        std::lock_guard<std::mutex> g(g_event_mutex);
+        g_events.erase(event_id);
+        return MEAO_OK;
+    }
+    // checked now: the plugin event cannot report an error
+    int rc = ensure_ready(c); if (rc) return rc;
+    ArrayIO io;
+    if ((rc = prepare_arrays(c, depth_array, kind, ao_array, &io))) return rc;
+    std::lock_guard<std::mutex> g(g_event_mutex);
+    g_events[event_id] = EventBinding{c, depth_array, kind, ao_array, stream, true};
     return MEAO_OK;
 }
 
@@ -1566,7 +1718,8 @@ void meao_render_event(int event_id)
         if (it == g_events.end()) return;
         b = it->second;
     }
-    meao_render(b.ctx, b.depth, b.kind, b.out, b.stream);
+    if (b.arrays) meao_render_arrays(b.ctx, b.depth, b.kind, b.out, b.stream);
+    else meao_render(b.ctx, b.depth, b.kind, b.out, b.stream);
 }
 
 MeaoRenderEventFunc meao_get_render_event_func(void) { return meao_render_event; }
