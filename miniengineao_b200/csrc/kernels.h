@@ -61,7 +61,9 @@ struct PrepareArgs {
     int reversed_z;         // UNITY_REVERSED_Z (DS1:41-45)
     int vec_ok;             // depth pointer 16B aligned and rows stay 16B aligned (W % 4 == 0 for f32/u32, W % 8 == 0 for u16)
 };
-cudaError_t launch_prepare_depth(const PrepareArgs &a, cudaStream_t s);
+// low_only: write LowDepth1..4 only, loading the even rows alone (a.lin is not written); the frame's final upsample then
+// linearises its own pixels and writes LinearDepth (launch_blur_upsample_lin)
+cudaError_t launch_prepare_depth(const PrepareArgs &a, cudaStream_t s, bool low_only = false);
 
 // ---- stage 2: render_ao = Render.compute main_interleaved, one mip level -----------------------
 struct RenderArgs {
@@ -126,6 +128,23 @@ cudaError_t launch_blur_upsample(const CUtensorMap &lo_depth_map, const CUtensor
 constexpr int kUpsDepthBoxW = 40, kUpsDepthBoxH = 22; // TMA boxes of the upsample kernel
 constexpr int kUpsAoBoxW = 64, kUpsAoBoxH = 22;
 
+// The final upsample of a whole frame (L1 -> L0), reading the caller's raw depth instead of LinearDepth: each thread loads the
+// raw depth of its own eight pixels, linearises them with prepare_depth's arithmetic (depth_in.cuh), stores the f16 values to
+// LinearDepth (a.hi_depth, which must be the LinearDepth arena buffer) and upsamples with them -- so LinearDepth is still produced
+// every frame, and prepare_depth runs low_only.  A kernel parameter of its own: UpsampleArgs stays as it is (see
+// blur_upsample_kernel.inc).  layers > 1: the layered kernels (depth: L tight W x H images back to back).
+struct DepthIn {
+    const void *depth;      // rows [depth_row0, ...) of the frame, row pitch = hiw elements (PrepareArgs.depth)
+    int in_format;          // PrepareArgs.in_format
+    int depth_row0;         // global row of depth[0]
+    float zbx, zby;         // ZBufferParams.xy
+    int raw, reversed_z;    // as PrepareArgs
+    int vec_ok;             // as PrepareArgs
+};
+cudaError_t launch_blur_upsample_lin(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
+                                     const UpsampleArgs &a, const uint8_t *lo_ao2, int lo_a2pitch, const DepthIn &din, int layers, int sm_count,
+                                     cudaStream_t s);
+
 // ---- layered frames (meao_set_layers): L same-size views through one launch per stage ------------------------------------
 // Every image is L images of the same pitch stored back to back ([L][h][pitch]; the caller's depth and AO: [L][H][W] tight), so
 // layer l of an image starts l x rows x pitch elements after layer 0.  The arguments are the single-image ones (row0 = 0,
@@ -133,7 +152,7 @@ constexpr int kUpsAoBoxW = 64, kUpsAoBoxH = 22;
 // fetch a box only when it lies inside one layer.  Separate kernels and translation units (*_layered.cu), so the single-image
 // kernels keep their code.  kMaxLayers: the prepare_depth / render_ao grids carry the layer in gridDim.z (at most 65535).
 constexpr int kMaxLayers = 65535;
-cudaError_t launch_prepare_depth_layered(const PrepareArgs &a, int layers, cudaStream_t s);
+cudaError_t launch_prepare_depth_layered(const PrepareArgs &a, int layers, cudaStream_t s, bool low_only = false);
 cudaError_t launch_render_ao_layered(const CUtensorMap &low_map, bool use_tma, const RenderArgs &a, int layers, cudaStream_t s);
 cudaError_t launch_blur_upsample_layered(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
                                          const UpsampleArgs &a, const uint8_t *lo_ao2, int lo_a2pitch, int layers, int sm_count, cudaStream_t s);
@@ -213,6 +232,7 @@ cudaError_t preload_render_ao_layered();
 cudaError_t preload_blur_upsample_layered();
 cudaError_t preload_prepare_depth_array();
 cudaError_t preload_blur_upsample_array();
+cudaError_t preload_blur_upsample_lin();
 cudaError_t preload_band_kernels();
 cudaError_t preload_aux_kernels();      // composite, debug views, self test
 #endif

@@ -463,27 +463,43 @@ int render_tile_variant(const MeaoCtx *c, int k, int rows)
 // A CUDA-array frame (meao_render_arrays): the surfaces of the depth and AO arrays and how their layers are addressed (surface_io.cuh).
 struct ArrayIO { cudaSurfaceObject_t depth, ao; int depth_surf, ao_surf; const void *ao_array; };
 
-// PushDownsampleCommands, AO.cs:604-658.  aio: read the depth from a CUDA array instead of `depth`.
-int record_downsample(MeaoCtx *c, const void *depth, int kind, cudaStream_t s, const ArrayIO *aio = nullptr)
+// The caller's depth as the kernels read it: rows [band0, band1) of the frame (every layer's, back to back), tight rows of W elements.
+DepthIn depth_in(const MeaoCtx *c, const void *depth, int kind)
+{
+    DepthIn d{};
+    d.depth = depth;
+    d.in_format = (kind == MEAO_DEPTH_RAW_D16_UNORM) ? 1 : (kind == MEAO_DEPTH_RAW_D24S8 ? 2 : 0);
+    d.depth_row0 = c->band0;
+    d.zbx = c->plan.zb[0]; d.zby = c->plan.zb[1];
+    d.raw = (kind != MEAO_DEPTH_LINEAR_F32);
+    d.reversed_z = c->camera.reversed_z;
+    d.vec_ok = (((uintptr_t)depth & 15) == 0) && (c->W % (d.in_format == 1 ? 8 : 4) == 0);
+    return d;
+}
+
+// PushDownsampleCommands, AO.cs:604-658.  aio: read the depth from a CUDA array instead of `depth`.  low_only: LowDepth1..4 only --
+// the frame's final upsample is recorded with the same depth (record_upsample's `fused`) and writes LinearDepth itself.
+int record_downsample(MeaoCtx *c, const void *depth, int kind, cudaStream_t s, const ArrayIO *aio = nullptr, bool low_only = false)
 {
     if (kind < MEAO_DEPTH_RAW_F32 || kind > MEAO_DEPTH_RAW_D24S8) return fail(c, MEAO_ERR_INVALID, "bad depth kind %d", kind);
     NvtxRange nv("meao::prepare_depth");
+    const DepthIn d = depth_in(c, depth, kind);
     PrepareArgs a{};
     a.depth = depth;
-    a.in_format = (kind == MEAO_DEPTH_RAW_D16_UNORM) ? 1 : (kind == MEAO_DEPTH_RAW_D24S8 ? 2 : 0);
+    a.in_format = d.in_format;
     a.W = c->W; a.H = c->H;
-    a.depth_row0 = c->band0;
+    a.depth_row0 = d.depth_row0;
     a.row0 = c->band0; a.row1 = c->band1;
     a.lin = c->lin; a.lin_pitch = c->lin_pitch;
     for (int k = 1; k <= 4; k++) { a.low[k - 1] = c->low[k]; a.low_pitch[k - 1] = c->low_pitch[k]; }
-    a.zbx = c->plan.zb[0]; a.zby = c->plan.zb[1];
-    a.raw = (kind != MEAO_DEPTH_LINEAR_F32);
-    a.reversed_z = c->camera.reversed_z;
-    a.vec_ok = (((uintptr_t)depth & 15) == 0) && (c->W % (a.in_format == 1 ? 8 : 4) == 0);
+    a.zbx = d.zbx; a.zby = d.zby;
+    a.raw = d.raw;
+    a.reversed_z = d.reversed_z;
+    a.vec_ok = d.vec_ok;
     c->last_kind = kind;
     if (aio) CUDA_TRY(c, launch_prepare_depth_array(a, aio->depth, aio->depth_surf, c->layers, s));
-    else if (c->layers > 1) CUDA_TRY(c, launch_prepare_depth_layered(a, c->layers, s));
-    else CUDA_TRY(c, launch_prepare_depth(a, s));
+    else if (c->layers > 1) CUDA_TRY(c, launch_prepare_depth_layered(a, c->layers, s, low_only));
+    else CUDA_TRY(c, launch_prepare_depth(a, s, low_only));
     c->launches++;
     return 0;
 }
@@ -525,7 +541,9 @@ int record_render(MeaoCtx *c, int k, int kind, cudaStream_t s, bool wide = false
 inline bool hq_level(const MeaoCtx *c, int k) { return ((c->variants.high_quality_mask >> (k - 1)) & 1) != 0; }
 
 // PushUpsampleCommands with the wiring of AO.cs:528-531.  aio (final level only): store the AO into a CUDA array instead of ao_out.
-int record_upsample(MeaoCtx *c, int lo, void *ao_out, cudaStream_t s, const ArrayIO *aio = nullptr)
+// fused (final level only, with the frame's depth and kind): read and linearise the raw depth and write LinearDepth here, after a
+// low_only record_downsample of the same depth.
+int record_upsample(MeaoCtx *c, int lo, void *ao_out, cudaStream_t s, const ArrayIO *aio = nullptr, const DepthIn *fused = nullptr)
 {
     const int hi = lo - 1;
     NvtxRange nv("meao::blur_upsample");
@@ -551,7 +569,10 @@ int record_upsample(MeaoCtx *c, int lo, void *ao_out, cudaStream_t s, const Arra
     a.tile_ctr = c->tile_ctr + 2 * (lo - 1);
     const uint8_t *lo_ao2 = hq_level(c, lo) ? c->hq[lo] : nullptr;                   // kernels main_premin / main_premin_blendout
     const CUtensorMap &ao_map = single ? c->map_occ1_ups : c->map_ao_ups[lo];
-    if (aio && hi == 0)
+    if (fused && hi == 0)
+        CUDA_TRY(c, launch_blur_upsample_lin(c->map_low_ups[lo], ao_map, &c->map_hq_ups[lo], c->tma_ok, a, lo_ao2, c->occ_pitch[lo], *fused, c->layers,
+                                             c->sm_count, s));
+    else if (aio && hi == 0)
         CUDA_TRY(c, launch_blur_upsample_array(c->map_low_ups[lo], ao_map, &c->map_hq_ups[lo], c->tma_ok, a, lo_ao2, c->occ_pitch[lo], c->layers, c->sm_count,
                                                aio->ao, aio->ao_surf, s));
     else if (c->layers > 1)
@@ -572,18 +593,23 @@ struct PdlScope { bool prev; explicit PdlScope(bool on) : prev(g_launch_pdl) { g
 // before this DAG is the neighbour-exchange kernel, which spins on remote flags -- nothing may be scheduled "early" behind it
 // (a grid parked in griddepcontrol.wait holds SM resources that the neighbour band's kernels may need: see DESIGN.md 4).
 // aio: a CUDA-array frame -- the first and the last node read / write the arrays (depth and ao_out are unused).
+// depth != nullptr (not an array frame): the fused form -- prepare_depth runs low_only and the final upsample reads the raw depth and
+// writes LinearDepth; with do_prepare = false the caller has recorded that low_only prepare_depth of the same depth itself.
 int record_frame_dag(MeaoCtx *c, const void *depth, int kind, void *ao_out, cudaStream_t s, bool do_prepare = true, int pdl = 0,
                      bool after_exchange = false, const ArrayIO *aio = nullptr)
 {
     int rc;
+    const bool fused = depth && !aio;
+    const DepthIn din = depth_in(c, depth, kind);
+    const DepthIn *fin = fused ? &din : nullptr;
     if (c->variants.single_scale) {     // BASELINE.json configs[0]: Downsample1 -> Render level 1 -> final-style Upsample on Occlusion1
-        if (do_prepare && (rc = record_downsample(c, depth, kind, s, aio))) return rc;
+        if (do_prepare && (rc = record_downsample(c, depth, kind, s, aio, fused))) return rc;
         { PdlScope p(pdl >= 1 && !after_exchange); if ((rc = record_render(c, 1, kind, s))) return rc; }
-        { PdlScope p(pdl >= 1); if ((rc = record_upsample(c, 1, ao_out, s, aio))) return rc; }
+        { PdlScope p(pdl >= 1); if ((rc = record_upsample(c, 1, ao_out, s, aio, fin))) return rc; }
         return 0;
     }
     cudaStream_t b1 = c->branch[0], b2 = c->branch[1], b3 = c->branch[2];
-    if (do_prepare && (rc = record_downsample(c, depth, kind, s, aio))) return rc;
+    if (do_prepare && (rc = record_downsample(c, depth, kind, s, aio, fused))) return rc;
     CUDA_TRY(c, cudaEventRecord(c->ev[0], s));
     CUDA_TRY(c, cudaStreamWaitEvent(b1, c->ev[0], 0));
     CUDA_TRY(c, cudaStreamWaitEvent(b2, c->ev[0], 0));
@@ -606,7 +632,7 @@ int record_frame_dag(MeaoCtx *c, const void *depth, int kind, void *ao_out, cuda
     CUDA_TRY(c, cudaEventRecord(c->ev[3], b3));
     CUDA_TRY(c, cudaStreamWaitEvent(s, c->ev[3], 0));
     { PdlScope p(pdl >= 2); if ((rc = record_upsample(c, 2, nullptr, s))) return rc; }
-    { PdlScope p(pdl >= 1); if ((rc = record_upsample(c, 1, ao_out, s, aio))) return rc; }
+    { PdlScope p(pdl >= 1); if ((rc = record_upsample(c, 1, ao_out, s, aio, fin))) return rc; }
     return 0;
 }
 
@@ -622,13 +648,14 @@ int record_frame(MeaoCtx *c, const void *depth, int kind, void *ao_out, cudaStre
     const int reps = profile ? c->profile_repeats : 1;         // every kernel is idempotent (out of place), so repeating it is harmless
     int rc = 0;
     mark();
-    for (int r = 0; r < reps && !rc; r++) rc = record_downsample(c, depth, kind, s);
+    const DepthIn din = depth_in(c, depth, kind);          // the fused form of record_frame_dag
+    for (int r = 0; r < reps && !rc; r++) rc = record_downsample(c, depth, kind, s, nullptr, true);
     if (rc) return rc;
     names.push_back("prepare_depth"); mark();
     const int kmax = c->variants.single_scale ? 1 : 4;       // single-scale: Render level 1 + the final-style Upsample only
     for (int k = 1; k <= kmax; k++) { for (int r = 0; r < reps && !rc; r++) rc = record_render(c, k, kind, s); if (rc) return rc; names.push_back(ren_names[k]); mark(); }
     for (int k = 1; k <= kmax; k++) if (hq_level(c, k)) { for (int r = 0; r < reps && !rc; r++) rc = record_render(c, k, kind, s, true); if (rc) return rc; names.push_back(hq_names[k]); mark(); }
-    for (int lo = kmax; lo >= 1; lo--) { for (int r = 0; r < reps && !rc; r++) rc = record_upsample(c, lo, lo == 1 ? ao_out : nullptr, s); if (rc) return rc; names.push_back(ups_names[lo]); mark(); }
+    for (int lo = kmax; lo >= 1; lo--) { for (int r = 0; r < reps && !rc; r++) rc = record_upsample(c, lo, lo == 1 ? ao_out : nullptr, s, nullptr, lo == 1 ? &din : nullptr); if (rc) return rc; names.push_back(ups_names[lo]); mark(); }
     if (profile) {
         CUDA_TRY(c, cudaStreamSynchronize(s));
         c->last_profile.clear();
@@ -751,6 +778,7 @@ int meao_create(const MeaoDeviceCfg *cfg, MeaoCtx **out)
             if (pe == cudaSuccess) pe = preload_blur_upsample_layered();
             if (pe == cudaSuccess) pe = preload_prepare_depth_array();
             if (pe == cudaSuccess) pe = preload_blur_upsample_array();
+            if (pe == cudaSuccess) pe = preload_blur_upsample_lin();
             if (pe == cudaSuccess) pe = preload_band_kernels();
             if (pe == cudaSuccess) pe = preload_aux_kernels();
             if (pe != cudaSuccess) { cudaGetLastError(); meao_destroy(c); return fail(nullptr, MEAO_ERR_CUDA, "loading the kernels failed: %s", cudaGetErrorString(pe)); }
@@ -1247,10 +1275,10 @@ int meao_band_step(MeaoCtx *c, const void *depth, int32_t kind, void *ao_out, vo
     const bool has_peer = c->peer_base[0] || c->peer_base[1];
     const int nk = meao_kernels_per_frame(c) + (has_peer ? 1 : 0);
     return launch_cached(c, key, (cudaStream_t)stream, nk, [&](cudaStream_t s, int pdl) {
-        int r = record_downsample(c, depth, kind, s);
+        int r = record_downsample(c, depth, kind, s, nullptr, true);
         if (r) return r;
         { PdlScope p(pdl >= 1); if ((r = record_exchange(c, s))) return r; }
-        return record_frame_dag(c, nullptr, kind, ao_out, s, false, pdl, has_peer);
+        return record_frame_dag(c, depth, kind, ao_out, s, false, pdl, has_peer);
     });
 }
 

@@ -22,22 +22,24 @@ namespace {
 
 }  // namespace
 
-cudaError_t launch_prepare_depth(const PrepareArgs &a, cudaStream_t s)
+cudaError_t launch_prepare_depth(const PrepareArgs &a, cudaStream_t s, bool low_only)
 {
     if (a.row1 <= a.row0) return cudaSuccess;
-    dim3 grid(ceil_div(a.W, kPrepTileW), ceil_div(a.row1 - a.row0, kPrepTileH));
+    dim3 grid(ceil_div(a.W, kPrepTileW), ceil_div(a.row1 - a.row0, low_only ? kPrepLowTileH : kPrepTileH));
+#define MEAO_PREP_K(...) (low_only ? prepare_depth_low_kernel<__VA_ARGS__> : prepare_depth_kernel<__VA_ARGS__>)
     if (!a.raw) {
-        MEAO_LAUNCH((prepare_depth_kernel<false, true, IN_F32>), grid, kPrepThreads, 0, s, a);
+        MEAO_LAUNCH((MEAO_PREP_K(false, true, IN_F32)), grid, kPrepThreads, 0, s, a);
     } else if (a.in_format == IN_D16) {
-        if (a.reversed_z) MEAO_LAUNCH((prepare_depth_kernel<true, true, IN_D16>), grid, kPrepThreads, 0, s, a);
-        else              MEAO_LAUNCH((prepare_depth_kernel<true, false, IN_D16>), grid, kPrepThreads, 0, s, a);
+        if (a.reversed_z) MEAO_LAUNCH((MEAO_PREP_K(true, true, IN_D16)), grid, kPrepThreads, 0, s, a);
+        else              MEAO_LAUNCH((MEAO_PREP_K(true, false, IN_D16)), grid, kPrepThreads, 0, s, a);
     } else if (a.in_format == IN_D24S8) {
-        if (a.reversed_z) MEAO_LAUNCH((prepare_depth_kernel<true, true, IN_D24S8>), grid, kPrepThreads, 0, s, a);
-        else              MEAO_LAUNCH((prepare_depth_kernel<true, false, IN_D24S8>), grid, kPrepThreads, 0, s, a);
+        if (a.reversed_z) MEAO_LAUNCH((MEAO_PREP_K(true, true, IN_D24S8)), grid, kPrepThreads, 0, s, a);
+        else              MEAO_LAUNCH((MEAO_PREP_K(true, false, IN_D24S8)), grid, kPrepThreads, 0, s, a);
     } else {
-        if (a.reversed_z) MEAO_LAUNCH((prepare_depth_kernel<true, true, IN_F32>), grid, kPrepThreads, 0, s, a);
-        else              MEAO_LAUNCH((prepare_depth_kernel<true, false, IN_F32>), grid, kPrepThreads, 0, s, a);
+        if (a.reversed_z) MEAO_LAUNCH((MEAO_PREP_K(true, true, IN_F32)), grid, kPrepThreads, 0, s, a);
+        else              MEAO_LAUNCH((MEAO_PREP_K(true, false, IN_F32)), grid, kPrepThreads, 0, s, a);
     }
+#undef MEAO_PREP_K
     return cudaGetLastError();
 }
 
@@ -50,6 +52,10 @@ cudaError_t preload_prepare_depth()
     t(prepare_depth_kernel<true, true, IN_F32>); t(prepare_depth_kernel<true, false, IN_F32>);
     t(prepare_depth_kernel<true, true, IN_D16>); t(prepare_depth_kernel<true, false, IN_D16>);
     t(prepare_depth_kernel<true, true, IN_D24S8>); t(prepare_depth_kernel<true, false, IN_D24S8>);
+    t(prepare_depth_low_kernel<false, true, IN_F32>);
+    t(prepare_depth_low_kernel<true, true, IN_F32>); t(prepare_depth_low_kernel<true, false, IN_F32>);
+    t(prepare_depth_low_kernel<true, true, IN_D16>); t(prepare_depth_low_kernel<true, false, IN_D16>);
+    t(prepare_depth_low_kernel<true, true, IN_D24S8>); t(prepare_depth_low_kernel<true, false, IN_D24S8>);
     return e;
 }
 #endif

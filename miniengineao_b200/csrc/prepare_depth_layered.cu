@@ -15,23 +15,25 @@ namespace {
 
 }  // namespace
 
-cudaError_t launch_prepare_depth_layered(const PrepareArgs &a, int layers, cudaStream_t s)
+cudaError_t launch_prepare_depth_layered(const PrepareArgs &a, int layers, cudaStream_t s, bool low_only)
 {
     if (a.row1 <= a.row0) return cudaSuccess;
     if (layers < 1 || layers > kMaxLayers) return cudaErrorInvalidValue;
-    dim3 grid(ceil_div(a.W, kPrepTileW), ceil_div(a.row1 - a.row0, kPrepTileH), layers);
+    dim3 grid(ceil_div(a.W, kPrepTileW), ceil_div(a.row1 - a.row0, low_only ? kPrepLowTileH : kPrepTileH), layers);
+#define MEAO_PREP_K(...) (low_only ? prepare_depth_low_layered_kernel<__VA_ARGS__> : prepare_depth_layered_kernel<__VA_ARGS__>)
     if (!a.raw) {
-        MEAO_LAUNCH((prepare_depth_layered_kernel<false, true, IN_F32>), grid, kPrepThreads, 0, s, a);
+        MEAO_LAUNCH((MEAO_PREP_K(false, true, IN_F32)), grid, kPrepThreads, 0, s, a);
     } else if (a.in_format == IN_D16) {
-        if (a.reversed_z) MEAO_LAUNCH((prepare_depth_layered_kernel<true, true, IN_D16>), grid, kPrepThreads, 0, s, a);
-        else              MEAO_LAUNCH((prepare_depth_layered_kernel<true, false, IN_D16>), grid, kPrepThreads, 0, s, a);
+        if (a.reversed_z) MEAO_LAUNCH((MEAO_PREP_K(true, true, IN_D16)), grid, kPrepThreads, 0, s, a);
+        else              MEAO_LAUNCH((MEAO_PREP_K(true, false, IN_D16)), grid, kPrepThreads, 0, s, a);
     } else if (a.in_format == IN_D24S8) {
-        if (a.reversed_z) MEAO_LAUNCH((prepare_depth_layered_kernel<true, true, IN_D24S8>), grid, kPrepThreads, 0, s, a);
-        else              MEAO_LAUNCH((prepare_depth_layered_kernel<true, false, IN_D24S8>), grid, kPrepThreads, 0, s, a);
+        if (a.reversed_z) MEAO_LAUNCH((MEAO_PREP_K(true, true, IN_D24S8)), grid, kPrepThreads, 0, s, a);
+        else              MEAO_LAUNCH((MEAO_PREP_K(true, false, IN_D24S8)), grid, kPrepThreads, 0, s, a);
     } else {
-        if (a.reversed_z) MEAO_LAUNCH((prepare_depth_layered_kernel<true, true, IN_F32>), grid, kPrepThreads, 0, s, a);
-        else              MEAO_LAUNCH((prepare_depth_layered_kernel<true, false, IN_F32>), grid, kPrepThreads, 0, s, a);
+        if (a.reversed_z) MEAO_LAUNCH((MEAO_PREP_K(true, true, IN_F32)), grid, kPrepThreads, 0, s, a);
+        else              MEAO_LAUNCH((MEAO_PREP_K(true, false, IN_F32)), grid, kPrepThreads, 0, s, a);
     }
+#undef MEAO_PREP_K
     return cudaGetLastError();
 }
 
@@ -44,6 +46,10 @@ cudaError_t preload_prepare_depth_layered()
     t(prepare_depth_layered_kernel<true, true, IN_F32>); t(prepare_depth_layered_kernel<true, false, IN_F32>);
     t(prepare_depth_layered_kernel<true, true, IN_D16>); t(prepare_depth_layered_kernel<true, false, IN_D16>);
     t(prepare_depth_layered_kernel<true, true, IN_D24S8>); t(prepare_depth_layered_kernel<true, false, IN_D24S8>);
+    t(prepare_depth_low_layered_kernel<false, true, IN_F32>);
+    t(prepare_depth_low_layered_kernel<true, true, IN_F32>); t(prepare_depth_low_layered_kernel<true, false, IN_F32>);
+    t(prepare_depth_low_layered_kernel<true, true, IN_D16>); t(prepare_depth_low_layered_kernel<true, false, IN_D16>);
+    t(prepare_depth_low_layered_kernel<true, true, IN_D24S8>); t(prepare_depth_low_layered_kernel<true, false, IN_D24S8>);
     return e;
 }
 #endif
