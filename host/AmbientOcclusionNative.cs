@@ -60,6 +60,12 @@ namespace MiniEngineAO
         [DllImport(Lib)] public static extern int meao_render_arrays(IntPtr ctx, IntPtr depthArray, int depthKind, IntPtr aoArray, IntPtr stream);
         [DllImport(Lib)] public static extern int meao_bind_event_arrays(IntPtr ctx, int eventId, IntPtr depthArray, int depthKind, IntPtr aoArray, IntPtr stream);
         [DllImport(Lib)] public static extern int meao_release_array(IntPtr ctx, IntPtr array);   // before the array is unmapped / unregistered / freed
+        // Linear buffers with their own row and layer pitch, in bytes (D3D12 placed footprints, Vulkan buffers through external memory,
+        // cudaMallocPitch, a dynamic-resolution corner of a max-size target), no copies
+        [DllImport(Lib)] public static extern int meao_render_pitched(IntPtr ctx, IntPtr depthDev, long depthRowPitch, long depthLayerPitch, int depthKind,
+                                                                      IntPtr aoOutDev, long aoRowPitch, long aoLayerPitch, IntPtr stream);
+        [DllImport(Lib)] public static extern int meao_bind_event_pitched(IntPtr ctx, int eventId, IntPtr depthDev, long depthRowPitch, long depthLayerPitch,
+                                                                          int depthKind, IntPtr aoOutDev, long aoRowPitch, long aoLayerPitch, IntPtr stream);
         [DllImport(Lib)] public static extern IntPtr meao_get_render_event_func();
         [DllImport(Lib)] public static extern int meao_composite_framebuffer(IntPtr ctx, IntPtr aoDev, IntPtr colorDev, int colorFormat, IntPtr stream);
         [DllImport(Lib)] public static extern int meao_composite_gbuffer(IntPtr ctx, IntPtr aoDev, IntPtr gbuffer0Dev, IntPtr gbuffer3Dev, int gbuffer3Format, IntPtr stream);
@@ -122,6 +128,9 @@ namespace MiniEngineAO
         // registered with cudaGraphicsRegisterFlagsSurfaceLoadStore), those: the plugin event then reads and writes them directly
         IntPtr _depthArray = IntPtr.Zero, _aoArray = IntPtr.Zero;
         int _depthArrayKind = 0;                                // MEAO_DEPTH_RAW_F32 (R32_FLOAT copy) or 2 = RAW_D16_UNORM (R16 copy)
+        // ... or, when the interop layer maps linear buffers that keep the graphics API's row pitch (a D3D12 footprint rounds each row up
+        // to 256 bytes; a dynamic-resolution frame is the corner of a max-size target), their byte pitches; 0 = tight (meao_bind_event)
+        long _depthRowPitch, _depthLayerPitch, _aoRowPitch, _aoLayerPitch;
         IntPtr _stream = IntPtr.Zero;                           // cudaStream_t the plugin event renders on (ABI 3; Zero = legacy default stream)
 
         void LateUpdate()
@@ -179,6 +188,7 @@ namespace MiniEngineAO
             _renderCommand.Clear();
             // (engine-specific: map _CameraDepthTexture and the R8 AO render texture to _depthDev / _aoDev, or to _depthArray / _aoArray)
             if (_depthArray != IntPtr.Zero) BindEventArrays();
+            else if (_depthRowPitch != 0) BindEventPitched();
             else MeaoNative.Check(_ctx, MeaoNative.meao_bind_event(_ctx, kEventId, _depthDev, 0 /* MEAO_DEPTH_RAW_F32 */, _aoDev, _stream));
             // one plugin event replaces the ten DispatchCompute calls recorded by :511-531
             _renderCommand.IssuePluginEvent(MeaoNative.meao_get_render_event_func(), kEventId);
@@ -189,6 +199,14 @@ namespace MiniEngineAO
         void BindEventArrays()
         {
             MeaoNative.Check(_ctx, MeaoNative.meao_bind_event_arrays(_ctx, kEventId, _depthArray, _depthArrayKind, _aoArray, _stream));
+        }
+
+        // The pitched path of the plugin event: meao_render_pitched on the mapped buffers at their own pitches (checked here -- the
+        // event cannot report errors).  With one layer the layer pitches are not used.
+        void BindEventPitched()
+        {
+            MeaoNative.Check(_ctx, MeaoNative.meao_bind_event_pitched(_ctx, kEventId, _depthDev, _depthRowPitch, _depthLayerPitch, 0 /* MEAO_DEPTH_RAW_F32 */,
+                                                                     _aoDev, _aoRowPitch, _aoLayerPitch, _stream));
         }
 
         // The interop layer calls this before it unmaps, unregisters or re-creates a texture it handed over as an array: the plugin

@@ -34,7 +34,8 @@ extern "C" {
                               * 3: + MeaoVariants.single_scale, native peer halo exchange (meao_band_export / _connect / _step / _status),
                               *      meao_bind_event takes the stream
                               *    + meao_set_layers (layered frames; additive, so the version stays 3)
-                              *    + meao_render_arrays / meao_bind_event_arrays / meao_release_array (CUDA-array I/O; additive) */
+                              *    + meao_render_arrays / meao_bind_event_arrays / meao_release_array (CUDA-array I/O; additive)
+                              *    + meao_render_pitched / meao_bind_event_pitched (depth and AO with their own row and layer pitch; additive) */
 
 typedef struct MeaoCtx MeaoCtx;
 
@@ -169,6 +170,31 @@ int meao_set_layers(MeaoCtx *ctx, int32_t layers);
  * stream: a cudaStream_t, used as given (NULL = the CUDA legacy default stream).  Asynchronous.  Re-plans first if dirty
  * (LateUpdate, AO.cs:329-350). */
 int meao_render(MeaoCtx *ctx, const void *depth_dev, int32_t depth_kind, void *ao_out_dev, void *stream);
+/* ---- pitched views -----------------------------------------------------------------------------------------------------------
+ * meao_render with the depth and the AO as views inside larger allocations, every pitch in BYTES: a cudaMallocPitch / cudaMalloc3D
+ * image, a D3D12 / Vulkan buffer shared through external memory (rows keep the API's pitch, e.g. D3D12's 256-byte footprint rows),
+ * or the top-left width x height corner of a render target sized for a larger resolution (a sub-rectangle: the same view with a base
+ * offset).  Row r of layer l of the depth starts at depth_dev + l*depth_layer_pitch + r*depth_row_pitch, the AO likewise; r counts
+ * the rows meao_render reads (the band's rows with a row band, depth_row0 as there).  meao_render IS this call with the tight
+ * pitches (width*esize, rows*width*esize, width, rows*width; esize = 4 for RAW_F32 / LINEAR_F32 / RAW_D24S8, 2 for RAW_D16_UNORM).
+ * Everything else is meao_render's: whole frames, layered contexts and top / bottom row bands; graphs are captured and replayed per
+ * (depth, ao_out, kind, the four pitches); meao_get_buffer / meao_debug_view of the AO (id 17) regenerate the context's own copy;
+ * MEAO_FLAG_NO_GRAPH is honoured; the AO is bit-identical to meao_render on a tight copy of the same view.  Bytes outside the views
+ * are neither read nor written.  Refused with MEAO_ERR_INVALID (meao_last_error names the field; nothing is launched), besides
+ * meao_render's own refusals (NULL pointers, bad kind, interior row band):
+ *   - a negative pitch (bottom-up views are not supported), or a row pitch above INT32_MAX;
+ *   - depth_row_pitch below width*esize or not a multiple of esize; ao_row_pitch below width; depth_dev not aligned to esize;
+ *   - with layers > 1: a layer pitch below (rows - 1)*row pitch + width*esize (width for the AO): the layers would overlap; a depth
+ *     layer pitch that is not a multiple of esize.  With one layer the layer pitches are not used;
+ *   - depth and AO byte extents (first to last byte of each view) that intersect: the depth is read through the non-coherent cache,
+ *     so aliasing is undefined.  The test is conservative -- interleaved views that share no byte are refused as well.
+ * Speed: 128-bit depth loads need depth_dev 16-byte aligned and the row (layered: and layer) pitch a multiple of 16 bytes; 64-bit AO
+ * stores need ao_out_dev 8-byte aligned and the AO pitches multiples of 8.  Otherwise the affected pixels take the scalar path, with
+ * the same result.  Tight-only, unchanged: the stage API, meao_render_band_prepare / _finish, meao_band_phase_a / _b,
+ * meao_band_step(_host), the host-buffer calls, meao_profile_frame, the composites and the debug-view outputs. */
+int meao_render_pitched(MeaoCtx *ctx,
+                        const void *depth_dev, int64_t depth_row_pitch, int64_t depth_layer_pitch, int32_t depth_kind,
+                        void *ao_out_dev, int64_t ao_row_pitch, int64_t ao_layer_pitch, void *stream);
 /* Same with HOST buffers: H2D copy of depth, the ten passes, D2H copy of the AO texture, then a
  * stream synchronise.  Use meao_host_alloc for pinned memory. */
 int meao_render_host(MeaoCtx *ctx, const void *depth_host, int32_t depth_kind, uint8_t *ao_out_host);
@@ -353,6 +379,12 @@ int meao_bind_event(MeaoCtx *ctx, int32_t event_id, const void *depth_dev, int32
  * are checked now (the event cannot report an error), with the statuses of meao_render_arrays; both NULL unbinds.  An id holds one
  * binding: binding it again, with either call, replaces it.  meao_release_array also removes the bindings that name the array. */
 int meao_bind_event_arrays(MeaoCtx *ctx, int32_t event_id, const void *depth_array, int32_t depth_kind, void *ao_array, void *stream);
+/* The pitched twin of meao_bind_event: the event renders meao_render_pitched with these views.  The views are checked now, with the
+ * refusals of meao_render_pitched; both pointers NULL unbinds.  meao_bind_event binds the tight views of the context as it is when the
+ * event runs. */
+int meao_bind_event_pitched(MeaoCtx *ctx, int32_t event_id,
+                            const void *depth_dev, int64_t depth_row_pitch, int64_t depth_layer_pitch, int32_t depth_kind,
+                            void *ao_out_dev, int64_t ao_row_pitch, int64_t ao_layer_pitch, void *stream);
 void meao_render_event(int event_id);
 MeaoRenderEventFunc meao_get_render_event_func(void);
 

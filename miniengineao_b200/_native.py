@@ -61,6 +61,8 @@ SIGNATURES = {
     "meao_resize": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
     "meao_set_layers": (C.c_int, [C.c_void_p, C.c_int32]),
     "meao_render": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "meao_render_pitched": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_int64, C.c_int64,
+                                      C.c_void_p]),
     "meao_render_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
     "meao_render_arrays": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "meao_release_array": (C.c_int, [C.c_void_p, C.c_void_p]),
@@ -102,6 +104,8 @@ SIGNATURES = {
     "meao_band_status": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),
     "meao_bind_event": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "meao_bind_event_arrays": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "meao_bind_event_pitched": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_int64,
+                                          C.c_int64, C.c_void_p]),
     "meao_render_event": (None, [C.c_int]),
     "meao_get_render_event_func": (RENDER_EVENT_FUNC, []),
     "meao_launch_count": (C.c_int64, [C.c_void_p]),

@@ -180,21 +180,44 @@ class AmbientOcclusion:
     def render(self, depth, out=None, *, linear: bool = False, stream=None):
         """depth: CUDA tensor [H, W] ([layers, H, W] when layers > 1): float32 raw camera depth (or linear if linear=True), uint16
         D16_UNORM codes, or int32 D24_UNORM_S8_UINT words.  Returns a CUDA uint8 tensor of the same shape -- the AmbientOcclusion R8
-        texture (AO.cs:475), one per layer."""
+        texture (AO.cs:475), one per layer.
+        depth and out may be strided views -- last stride 1, the others positive, e.g. the corner rt[:h, :w] (rt[:, :h, :w]) of a
+        larger render target: their strides are the row and layer pitches of meao_render_pitched."""
         import torch
         self.LateUpdate()
-        if not (depth.is_cuda and depth.is_contiguous()):
-            raise ValueError("depth must be a contiguous CUDA tensor")
         shape = self._frame_shape()
+        if not depth.is_cuda:
+            raise ValueError("depth must be a CUDA tensor")
         if tuple(depth.shape) != shape:
             raise ValueError(f"depth shape {tuple(depth.shape)} != {shape}")
         if out is None:
             out = torch.empty(shape, dtype=torch.uint8, device=depth.device)
-        elif tuple(out.shape) != shape or out.dtype != torch.uint8 or not out.is_contiguous():
-            raise ValueError(f"out must be a contiguous uint8 CUDA tensor {shape}")
+        elif tuple(out.shape) != shape or out.dtype != torch.uint8 or not out.is_cuda:
+            raise ValueError(f"out must be a uint8 CUDA tensor {shape}")
         kind = self._kind(str(depth.dtype).replace("torch.", ""), linear)
-        self._check(self._lib.meao_render(self._ctx, depth.data_ptr(), kind, out.data_ptr(), self._stream(stream)))
+        if depth.is_contiguous() and out.is_contiguous():
+            # meao_render IS meao_render_pitched at the tight pitches; calling it spares a frame loop the per-call stride arithmetic
+            self._check(self._lib.meao_render(self._ctx, depth.data_ptr(), kind, out.data_ptr(), self._stream(stream)))
+            return out
+        dp, ap = self._pitches(depth, "depth"), self._pitches(out, "out")
+        self._check(self._lib.meao_render_pitched(self._ctx, depth.data_ptr(), dp[0], dp[1], kind, out.data_ptr(), ap[0], ap[1],
+                                                  self._stream(stream)))
         return out
+
+    def _pitches(self, t, name: str) -> tuple:
+        """(row pitch, layer pitch) in bytes of a [rows, W] / [layers, H, W] tensor view (one layer: the layer pitch is rows x row).
+        A dimension of size 1 is never stepped along, so its stride is taken as the tight one (as torch does for contiguity)."""
+        st = list(t.stride())
+        tight = 1
+        for i in range(t.dim() - 1, -1, -1):
+            if t.shape[i] == 1:
+                st[i] = tight
+            tight *= t.shape[i]
+        if st[-1] != 1 or any(s <= 0 for s in st[:-1]):
+            raise ValueError(f"{name} must have a last stride of 1 and positive other strides (got strides {tuple(st)})")
+        es = t.element_size()
+        row = st[-2] * es
+        return (row, st[0] * es) if t.dim() == 3 else (row, row * t.shape[0])
 
     _ARRAY_KINDS = {"raw_f32": N.MEAO_DEPTH_RAW_F32, "linear_f32": N.MEAO_DEPTH_LINEAR_F32, "d16": N.MEAO_DEPTH_RAW_D16_UNORM,
                     "d24s8": N.MEAO_DEPTH_RAW_D24S8}

@@ -31,9 +31,9 @@ namespace {
 template <int IN>
 __device__ __forceinline__ uint4 linearize_pixels8(const DepthIn &din, int layer, int py, int px0, int hiw, int hih, bool full, __half *lin)
 {
-    const void *depth = reinterpret_cast<const char *>(din.depth) + (size_t)layer * hiw * hih * (IN == IN_D16 ? 2 : 4);
+    const void *depth = reinterpret_cast<const char *>(din.depth) + (size_t)layer * din.depth_layer_pitch * (IN == IN_D16 ? 2 : 4);
     float v[8], d[8];
-    load8<IN>(depth, (size_t)(py - din.depth_row0) * hiw + px0, full && din.vec_ok, hiw - px0, v);
+    load8<IN>(depth, (size_t)(py - din.depth_row0) * din.depth_pitch + px0, full && din.vec_ok, hiw - px0, v);
     if (!din.raw) linearize8<false, true>(v, din.zbx, din.zby, d);
     else if (din.reversed_z) linearize8<true, true>(v, din.zbx, din.zby, d);
     else linearize8<true, false>(v, din.zbx, din.zby, d);
@@ -52,6 +52,21 @@ __device__ __forceinline__ uint4 linearize_pixels8(const DepthIn &din, int layer
         }
     }
     return pk;
+}
+
+// layer_args of the fused layered kernels: the caller's AO advances by its own layer pitch (DepthIn.ao_layer_pitch, bytes) instead of
+// hih x out_pitch, so a layered AO view keeps the layer pitch of the tensor or allocation it lives in
+__device__ __forceinline__ UpsampleArgs layer_args(const UpsampleArgs &a, int l, long long ao_layer_pitch)
+{
+    UpsampleArgs r = layer_args(a, l);
+    r.out = a.out + (size_t)l * ao_layer_pitch;
+    return r;
+}
+__device__ __forceinline__ UpsamplePreminArgs layer_args(const UpsamplePreminArgs &pa, int l, long long ao_layer_pitch)
+{
+    UpsamplePreminArgs r = layer_args(pa, l);
+    r.base.out = pa.base.out + (size_t)l * ao_layer_pitch;
+    return r;
 }
 
 #define MEAO_UPS_LIN 1
@@ -88,7 +103,7 @@ void launch_lin(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, c
 }  // namespace
 
 cudaError_t launch_blur_upsample_lin(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
-                                     const UpsampleArgs &a_in, const uint8_t *lo_ao2, int lo_a2pitch, const DepthIn &din, int layers, int sm_count,
+                                     const UpsampleArgs &a_in, const uint8_t *lo_ao2, int lo_a2pitch, const DepthIn &din_in, int layers, int sm_count,
                                      cudaStream_t s)
 {
     if (a_in.row1 <= a_in.row0) return cudaSuccess;
@@ -108,7 +123,11 @@ cudaError_t launch_blur_upsample_lin(const CUtensorMap &lo_depth_map, const CUte
     if (!persist) a.tile_ctr = nullptr;
     const dim3 grid(persist ? kWave : ntiles);
     const int t = use_tma ? 1 : 0;
-    if (din.in_format == IN_D16)        launch_lin<IN_D16>(lo_depth_map, lo_ao_map, lo_ao2_map, a, lo_ao2, lo_a2pitch, din, t, layers, grid, s);
+    DepthIn din = din_in;           // zero pitches: the tight values
+    if (!din.depth_pitch) din.depth_pitch = a.hiw;
+    if (!din.depth_layer_pitch) din.depth_layer_pitch = (long long)din.depth_pitch * a.hih;
+    if (!din.ao_layer_pitch) din.ao_layer_pitch = (long long)a.hih * a.out_pitch;
+    if (din.in_format == IN_D16)       launch_lin<IN_D16>(lo_depth_map, lo_ao_map, lo_ao2_map, a, lo_ao2, lo_a2pitch, din, t, layers, grid, s);
     else if (din.in_format == IN_D24S8) launch_lin<IN_D24S8>(lo_depth_map, lo_ao_map, lo_ao2_map, a, lo_ao2, lo_a2pitch, din, t, layers, grid, s);
     else                                launch_lin<IN_F32>(lo_depth_map, lo_ao_map, lo_ao2_map, a, lo_ao2, lo_a2pitch, din, t, layers, grid, s);
     return cudaGetLastError();

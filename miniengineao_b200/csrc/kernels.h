@@ -47,7 +47,7 @@ namespace meao {
 
 // ---- stage 1: prepare_depth = Downsample1.compute + Downsample2.compute fused ----------------
 struct PrepareArgs {
-    const void *depth;      // input rows [depth_row0, ...) of the frame, row pitch = W elements (f32 / u16 / u32)
+    const void *depth;      // input rows [depth_row0, ...) of the frame, row pitch = depth_pitch elements (f32 / u16 / u32)
     int in_format;          // 0 = f32, 1 = D16_UNORM codes (u16), 2 = D24_UNORM_S8_UINT words (u32, depth in the low 24 bits)
     int W, H;               // full-frame size
     int depth_row0;         // global row of depth[0]
@@ -59,8 +59,20 @@ struct PrepareArgs {
     float zbx, zby;         // ZBufferParams.xy (AmbientOcclusion.cs:561-568)
     int raw;                // 1: Linearize (DS1:37-48); 0: depth is already linear
     int reversed_z;         // UNITY_REVERSED_Z (DS1:41-45)
-    int vec_ok;             // depth pointer 16B aligned and rows stay 16B aligned (W % 4 == 0 for f32/u32, W % 8 == 0 for u16)
+    int vec_ok;             // depth pointer 16B aligned and rows (layered: and layers) stay 16B aligned: the depth_pitch (and
+                            //    depth_layer_pitch) bytes are multiples of 16 -- for a tight frame W % 4 == 0 (f32/u32), W % 8 == 0 (u16)
+    // appended last so that every field above keeps its parameter offset.  0 means tight (resolved by the launchers, so zero-filled
+    // argument blocks keep their meaning): depth_pitch = W, depth_layer_pitch = depth_pitch x H.
+    int depth_pitch;        // elements from one depth row to the next
+    long long depth_layer_pitch;    // layered: elements from one layer of `depth` to the next
 };
+// `a` with its zero pitches replaced by the tight values (what the prepare launchers pass to the kernels)
+inline PrepareArgs resolve_pitches(PrepareArgs a)
+{
+    if (!a.depth_pitch) a.depth_pitch = a.W;
+    if (!a.depth_layer_pitch) a.depth_layer_pitch = (long long)a.depth_pitch * a.H;
+    return a;
+}
 // low_only: write LowDepth1..4 only, loading the even rows alone (a.lin is not written); the frame's final upsample then
 // linearises its own pixels and writes LinearDepth (launch_blur_upsample_lin)
 cudaError_t launch_prepare_depth(const PrepareArgs &a, cudaStream_t s, bool low_only = false);
@@ -132,22 +144,27 @@ constexpr int kUpsAoBoxW = 64, kUpsAoBoxH = 22;
 // raw depth of its own eight pixels, linearises them with prepare_depth's arithmetic (depth_in.cuh), stores the f16 values to
 // LinearDepth (a.hi_depth, which must be the LinearDepth arena buffer) and upsamples with them -- so LinearDepth is still produced
 // every frame, and prepare_depth runs low_only.  A kernel parameter of its own: UpsampleArgs stays as it is (see
-// blur_upsample_kernel.inc).  layers > 1: the layered kernels (depth: L tight W x H images back to back).
+// blur_upsample_kernel.inc).  layers > 1: the layered kernels (depth: L images depth_layer_pitch elements apart, AO: L images
+// ao_layer_pitch bytes apart; the AO row pitch is UpsampleArgs.out_pitch).
 struct DepthIn {
-    const void *depth;      // rows [depth_row0, ...) of the frame, row pitch = hiw elements (PrepareArgs.depth)
+    const void *depth;      // rows [depth_row0, ...) of the frame, row pitch = depth_pitch elements (PrepareArgs.depth)
     int in_format;          // PrepareArgs.in_format
     int depth_row0;         // global row of depth[0]
     float zbx, zby;         // ZBufferParams.xy
     int raw, reversed_z;    // as PrepareArgs
     int vec_ok;             // as PrepareArgs
+    // appended last; 0 means tight (resolved by launch_blur_upsample_lin): hiw, depth_pitch x hih, hih x out_pitch
+    int depth_pitch;        // elements from one depth row to the next
+    long long depth_layer_pitch;    // layered: elements from one depth layer to the next
+    long long ao_layer_pitch;       // layered: bytes from one layer of UpsampleArgs.out to the next
 };
 cudaError_t launch_blur_upsample_lin(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
                                      const UpsampleArgs &a, const uint8_t *lo_ao2, int lo_a2pitch, const DepthIn &din, int layers, int sm_count,
                                      cudaStream_t s);
 
 // ---- layered frames (meao_set_layers): L same-size views through one launch per stage ------------------------------------
-// Every image is L images of the same pitch stored back to back ([L][h][pitch]; the caller's depth and AO: [L][H][W] tight), so
-// layer l of an image starts l x rows x pitch elements after layer 0.  The arguments are the single-image ones (row0 = 0,
+// Every image is L images of the same pitch stored back to back ([L][h][pitch]), so layer l of an image starts l x rows x pitch
+// elements after layer 0; the caller's depth and AO advance by their own layer pitches (PrepareArgs / DepthIn).  The arguments are the single-image ones (row0 = 0,
 // row1 = the level's height, out_row_origin = 0) describing layer 0; the TMA maps span all layers (height L x h), and the kernels
 // fetch a box only when it lies inside one layer.  Separate kernels and translation units (*_layered.cu), so the single-image
 // kernels keep their code.  kMaxLayers: the prepare_depth / render_ao grids carry the layer in gridDim.z (at most 65535).

@@ -130,9 +130,13 @@ struct MeaoCtx {
     // synchronisation, launches already enqueued are unaffected).  Dropped as a whole only when the plan changes.
     // kind: the depth kind of a pointer frame; 100+ / 200+ / 300+ band graphs; kArrayGraphKind+ array frames (the key holds
     // cudaArray_t handles, so a pointer equal to a handle value never finds an array frame's graph, nor the reverse).
-    struct GraphKey { const void *p[4]; int kind; bool operator<(const GraphKey &o) const {
+    // pitch: the byte pitches of a pointer frame's depth and AO views (meao_render_pitched; 0 for the other kinds) -- a frame at the
+    // same pointers with other pitches is another graph, never a replay that reads the wrong rows.
+    struct GraphKey { const void *p[4]; int kind; int64_t pitch[4] = {0, 0, 0, 0}; bool operator<(const GraphKey &o) const {
         for (int i = 0; i < 4; i++) if (p[i] != o.p[i]) return p[i] < o.p[i];
-        return kind < o.kind; } };
+        if (kind != o.kind) return kind < o.kind;
+        for (int i = 0; i < 4; i++) if (pitch[i] != o.pitch[i]) return pitch[i] < o.pitch[i];
+        return false; } };
     struct GraphEntry { cudaGraphExec_t exec; uint64_t last_use; };
     std::map<GraphKey, GraphEntry> graphs;
     std::vector<cudaGraphExec_t> retired;   // executable graphs replaced while possibly in flight: destroyed at the next drop_graph
@@ -463,9 +467,22 @@ int render_tile_variant(const MeaoCtx *c, int k, int rows)
 // A CUDA-array frame (meao_render_arrays): the surfaces of the depth and AO arrays and how their layers are addressed (surface_io.cuh).
 struct ArrayIO { cudaSurfaceObject_t depth, ao; int depth_surf, ao_surf; const void *ao_array; };
 
-// The caller's depth as the kernels read it: rows [band0, band1) of the frame (every layer's, back to back), tight rows of W elements.
-DepthIn depth_in(const MeaoCtx *c, const void *depth, int kind)
+// The byte pitches of the caller's depth and AO views (meao_render_pitched).  A view is `layers` images of rows [band0, band1) of
+// the frame, W pixels per row.
+struct ViewPitch { int64_t depth_row, depth_layer, ao_row, ao_layer; };
+inline int64_t depth_esize(int kind) { return kind == MEAO_DEPTH_RAW_D16_UNORM ? 2 : 4; }
+// meao_render's views: tight rows, tight layers
+ViewPitch tight_pitch(const MeaoCtx *c, int kind)
 {
+    const int64_t es = depth_esize(kind), rows = c->band1 - c->band0;
+    return ViewPitch{c->W * es, rows * c->W * es, c->W, rows * c->W};
+}
+
+// The caller's depth as the kernels read it: rows [band0, band1) of the frame of every layer, at the pitches of `vp` (nullptr: tight).
+DepthIn depth_in(const MeaoCtx *c, const void *depth, int kind, const ViewPitch *vp = nullptr)
+{
+    const ViewPitch p = vp ? *vp : tight_pitch(c, kind);
+    const int64_t es = depth_esize(kind);
     DepthIn d{};
     d.depth = depth;
     d.in_format = (kind == MEAO_DEPTH_RAW_D16_UNORM) ? 1 : (kind == MEAO_DEPTH_RAW_D24S8 ? 2 : 0);
@@ -473,17 +490,23 @@ DepthIn depth_in(const MeaoCtx *c, const void *depth, int kind)
     d.zbx = c->plan.zb[0]; d.zby = c->plan.zb[1];
     d.raw = (kind != MEAO_DEPTH_LINEAR_F32);
     d.reversed_z = c->camera.reversed_z;
-    d.vec_ok = (((uintptr_t)depth & 15) == 0) && (c->W % (d.in_format == 1 ? 8 : 4) == 0);
+    // 128-bit loads: every row (and layer) start 16-byte aligned.  Tight views: W % 4 == 0 (4-byte kinds), W % 8 == 0 (D16)
+    d.vec_ok = (((uintptr_t)depth & 15) == 0) && (p.depth_row % 16 == 0) && (c->layers == 1 || p.depth_layer % 16 == 0);
+    d.depth_pitch = (int)(p.depth_row / es);
+    d.depth_layer_pitch = p.depth_layer / es;
+    d.ao_layer_pitch = p.ao_layer;
     return d;
 }
 
 // PushDownsampleCommands, AO.cs:604-658.  aio: read the depth from a CUDA array instead of `depth`.  low_only: LowDepth1..4 only --
 // the frame's final upsample is recorded with the same depth (record_upsample's `fused`) and writes LinearDepth itself.
-int record_downsample(MeaoCtx *c, const void *depth, int kind, cudaStream_t s, const ArrayIO *aio = nullptr, bool low_only = false)
+// vp: the depth's pitches (nullptr: tight).
+int record_downsample(MeaoCtx *c, const void *depth, int kind, cudaStream_t s, const ArrayIO *aio = nullptr, bool low_only = false,
+                      const ViewPitch *vp = nullptr)
 {
     if (kind < MEAO_DEPTH_RAW_F32 || kind > MEAO_DEPTH_RAW_D24S8) return fail(c, MEAO_ERR_INVALID, "bad depth kind %d", kind);
     NvtxRange nv("meao::prepare_depth");
-    const DepthIn d = depth_in(c, depth, kind);
+    const DepthIn d = depth_in(c, depth, kind, vp);
     PrepareArgs a{};
     a.depth = depth;
     a.in_format = d.in_format;
@@ -496,6 +519,7 @@ int record_downsample(MeaoCtx *c, const void *depth, int kind, cudaStream_t s, c
     a.raw = d.raw;
     a.reversed_z = d.reversed_z;
     a.vec_ok = d.vec_ok;
+    a.depth_pitch = d.depth_pitch; a.depth_layer_pitch = d.depth_layer_pitch;
     c->last_kind = kind;
     if (aio) CUDA_TRY(c, launch_prepare_depth_array(a, aio->depth, aio->depth_surf, c->layers, s));
     else if (c->layers > 1) CUDA_TRY(c, launch_prepare_depth_layered(a, c->layers, s, low_only));
@@ -542,8 +566,9 @@ inline bool hq_level(const MeaoCtx *c, int k) { return ((c->variants.high_qualit
 
 // PushUpsampleCommands with the wiring of AO.cs:528-531.  aio (final level only): store the AO into a CUDA array instead of ao_out.
 // fused (final level only, with the frame's depth and kind): read and linearise the raw depth and write LinearDepth here, after a
-// low_only record_downsample of the same depth.
-int record_upsample(MeaoCtx *c, int lo, void *ao_out, cudaStream_t s, const ArrayIO *aio = nullptr, const DepthIn *fused = nullptr)
+// low_only record_downsample of the same depth (its ao_layer_pitch is the AO's).  vp: the pitches of ao_out (nullptr: tight).
+int record_upsample(MeaoCtx *c, int lo, void *ao_out, cudaStream_t s, const ArrayIO *aio = nullptr, const DepthIn *fused = nullptr,
+                    const ViewPitch *vp = nullptr)
 {
     const int hi = lo - 1;
     NvtxRange nv("meao::blur_upsample");
@@ -554,11 +579,12 @@ int record_upsample(MeaoCtx *c, int lo, void *ao_out, cudaStream_t s, const Arra
     if (hi == 0) { a.hi_depth = c->lin; a.hi_is_half = 1; a.hi_dpitch = c->lin_pitch; a.hi_ao = nullptr; a.hi_apitch = 0; }
     else { a.hi_depth = c->low[hi]; a.hi_is_half = 0; a.hi_dpitch = c->low_pitch[hi]; a.hi_ao = c->occ[hi]; a.hi_apitch = c->occ_pitch[hi]; }
     if (hi == 0) {
-        if (ao_out) { a.out = (uint8_t *)ao_out; a.out_pitch = c->W; a.out_row_origin = c->band0; }
+        if (ao_out) { a.out = (uint8_t *)ao_out; a.out_pitch = vp ? (int)vp->ao_row : c->W; a.out_row_origin = c->band0; }
         else { a.out = c->result; a.out_pitch = c->result_pitch; a.out_row_origin = 0; }
         c->last_out = aio ? const_cast<void *>(aio->ao_array) : ao_out;
     } else { a.out = c->comb[hi]; a.out_pitch = c->occ_pitch[hi]; a.out_row_origin = 0; }
-    a.out_vec_ok = (((uintptr_t)a.out & 7) == 0) && (a.out_pitch % 8 == 0);
+    // 64-bit stores: every row (and, in the caller's layered AO, layer) start 8-byte aligned.  A tight AO: W % 8 == 0
+    a.out_vec_ok = (((uintptr_t)a.out & 7) == 0) && (a.out_pitch % 8 == 0) && !(vp && ao_out && c->layers > 1 && vp->ao_layer % 8 != 0);
     a.hiw = c->lw[hi]; a.hih = c->lh[hi];
     a.noise_filter_strength = c->plan.noise_filter_strength[lo];
     a.step_size = c->plan.step_size[lo];
@@ -596,20 +622,20 @@ struct PdlScope { bool prev; explicit PdlScope(bool on) : prev(g_launch_pdl) { g
 // depth != nullptr (not an array frame): the fused form -- prepare_depth runs low_only and the final upsample reads the raw depth and
 // writes LinearDepth; with do_prepare = false the caller has recorded that low_only prepare_depth of the same depth itself.
 int record_frame_dag(MeaoCtx *c, const void *depth, int kind, void *ao_out, cudaStream_t s, bool do_prepare = true, int pdl = 0,
-                     bool after_exchange = false, const ArrayIO *aio = nullptr)
+                     bool after_exchange = false, const ArrayIO *aio = nullptr, const ViewPitch *vp = nullptr)
 {
     int rc;
     const bool fused = depth && !aio;
-    const DepthIn din = depth_in(c, depth, kind);
+    const DepthIn din = depth_in(c, depth, kind, vp);
     const DepthIn *fin = fused ? &din : nullptr;
     if (c->variants.single_scale) {     // BASELINE.json configs[0]: Downsample1 -> Render level 1 -> final-style Upsample on Occlusion1
-        if (do_prepare && (rc = record_downsample(c, depth, kind, s, aio, fused))) return rc;
+        if (do_prepare && (rc = record_downsample(c, depth, kind, s, aio, fused, vp))) return rc;
         { PdlScope p(pdl >= 1 && !after_exchange); if ((rc = record_render(c, 1, kind, s))) return rc; }
-        { PdlScope p(pdl >= 1); if ((rc = record_upsample(c, 1, ao_out, s, aio, fin))) return rc; }
+        { PdlScope p(pdl >= 1); if ((rc = record_upsample(c, 1, ao_out, s, aio, fin, vp))) return rc; }
         return 0;
     }
     cudaStream_t b1 = c->branch[0], b2 = c->branch[1], b3 = c->branch[2];
-    if (do_prepare && (rc = record_downsample(c, depth, kind, s, aio, fused))) return rc;
+    if (do_prepare && (rc = record_downsample(c, depth, kind, s, aio, fused, vp))) return rc;
     CUDA_TRY(c, cudaEventRecord(c->ev[0], s));
     CUDA_TRY(c, cudaStreamWaitEvent(b1, c->ev[0], 0));
     CUDA_TRY(c, cudaStreamWaitEvent(b2, c->ev[0], 0));
@@ -632,12 +658,12 @@ int record_frame_dag(MeaoCtx *c, const void *depth, int kind, void *ao_out, cuda
     CUDA_TRY(c, cudaEventRecord(c->ev[3], b3));
     CUDA_TRY(c, cudaStreamWaitEvent(s, c->ev[3], 0));
     { PdlScope p(pdl >= 2); if ((rc = record_upsample(c, 2, nullptr, s))) return rc; }
-    { PdlScope p(pdl >= 1); if ((rc = record_upsample(c, 1, ao_out, s, aio, fin))) return rc; }
+    { PdlScope p(pdl >= 1); if ((rc = record_upsample(c, 1, ao_out, s, aio, fin, vp))) return rc; }
     return 0;
 }
 
-// record order of RebuildCommandBuffers, AO.cs:511-531
-int record_frame(MeaoCtx *c, const void *depth, int kind, void *ao_out, cudaStream_t s, bool profile)
+// record order of RebuildCommandBuffers, AO.cs:511-531.  vp: the pitches of depth and ao_out (nullptr: tight).
+int record_frame(MeaoCtx *c, const void *depth, int kind, void *ao_out, cudaStream_t s, bool profile, const ViewPitch *vp = nullptr)
 {
     static const char *ren_names[5] = {"", "render_ao L1", "render_ao L2", "render_ao L3", "render_ao L4"};
     static const char *hq_names[5] = {"", "render_ao_wide L1", "render_ao_wide L2", "render_ao_wide L3", "render_ao_wide L4"};
@@ -648,14 +674,14 @@ int record_frame(MeaoCtx *c, const void *depth, int kind, void *ao_out, cudaStre
     const int reps = profile ? c->profile_repeats : 1;         // every kernel is idempotent (out of place), so repeating it is harmless
     int rc = 0;
     mark();
-    const DepthIn din = depth_in(c, depth, kind);          // the fused form of record_frame_dag
-    for (int r = 0; r < reps && !rc; r++) rc = record_downsample(c, depth, kind, s, nullptr, true);
+    const DepthIn din = depth_in(c, depth, kind, vp);      // the fused form of record_frame_dag
+    for (int r = 0; r < reps && !rc; r++) rc = record_downsample(c, depth, kind, s, nullptr, true, vp);
     if (rc) return rc;
     names.push_back("prepare_depth"); mark();
     const int kmax = c->variants.single_scale ? 1 : 4;       // single-scale: Render level 1 + the final-style Upsample only
     for (int k = 1; k <= kmax; k++) { for (int r = 0; r < reps && !rc; r++) rc = record_render(c, k, kind, s); if (rc) return rc; names.push_back(ren_names[k]); mark(); }
     for (int k = 1; k <= kmax; k++) if (hq_level(c, k)) { for (int r = 0; r < reps && !rc; r++) rc = record_render(c, k, kind, s, true); if (rc) return rc; names.push_back(hq_names[k]); mark(); }
-    for (int lo = kmax; lo >= 1; lo--) { for (int r = 0; r < reps && !rc; r++) rc = record_upsample(c, lo, lo == 1 ? ao_out : nullptr, s, nullptr, lo == 1 ? &din : nullptr); if (rc) return rc; names.push_back(ups_names[lo]); mark(); }
+    for (int lo = kmax; lo >= 1; lo--) { for (int r = 0; r < reps && !rc; r++) rc = record_upsample(c, lo, lo == 1 ? ao_out : nullptr, s, nullptr, lo == 1 ? &din : nullptr, vp); if (rc) return rc; names.push_back(ups_names[lo]); mark(); }
     if (profile) {
         CUDA_TRY(c, cudaStreamSynchronize(s));
         c->last_profile.clear();
@@ -696,7 +722,9 @@ int buffer_ptr(MeaoCtx *c, int id, void **p, size_t *pitch_bytes)
 }
 
 std::mutex g_event_mutex;
-struct EventBinding { MeaoCtx *ctx; const void *depth; int kind; void *out; void *stream; bool arrays; };   // arrays: meao_bind_event_arrays
+// arrays: meao_bind_event_arrays.  Otherwise a pointer frame at the pitches `pitch`, or, with tight (meao_bind_event), at the tight pitches
+// of the context when the event runs -- a meao_resize between binding and rendering keeps meaning what it meant before.
+struct EventBinding { MeaoCtx *ctx; const void *depth; int kind; void *out; void *stream; bool arrays; bool tight; ViewPitch pitch; };
 std::map<int, EventBinding> g_events;
 
 }  // namespace
@@ -1309,24 +1337,88 @@ int meao_band_status(MeaoCtx *c, int32_t out4[4])
     return MEAO_OK;
 }
 
-int meao_render(MeaoCtx *c, const void *depth, int32_t kind, void *ao_out, void *stream)
+namespace {
+// Every check of meao_render_pitched / meao_bind_event_pitched, on the host before anything is launched.  On success the layer pitches
+// of a single-layer context (unused) are replaced by the tight values, so that equivalent views share one cached graph.
+int check_views(MeaoCtx *c, const void *depth, int kind, const void *ao_out, ViewPitch *p)
 {
-    int rc = ensure_ready(c); if (rc) return rc;
     if (!depth || !ao_out) return fail(c, MEAO_ERR_INVALID, "depth / ao_out is NULL");
     if (kind < MEAO_DEPTH_RAW_F32 || kind > MEAO_DEPTH_RAW_D24S8) return fail(c, MEAO_ERR_INVALID, "bad depth kind %d", kind);
     if (c->need_low[1].lo < c->own_low[1].lo || c->need_low[1].hi > c->own_low[1].hi)
         return fail(c, MEAO_ERR_INVALID, "interior row band: use meao_render_band_prepare / halo exchange / meao_render_band_finish");
-    cudaStream_t s = (cudaStream_t)stream;
-    if (c->flags & MEAO_FLAG_NO_GRAPH) return record_frame(c, depth, kind, ao_out, s, false);
+    const int64_t es = depth_esize(kind), rows = c->band1 - c->band0, L = c->layers, W = c->W;
+    const struct { const char *name; int64_t v; } all[4] = {{"depth_row_pitch", p->depth_row}, {"depth_layer_pitch", p->depth_layer},
+                                                             {"ao_row_pitch", p->ao_row}, {"ao_layer_pitch", p->ao_layer}};
+    for (const auto &f : all)
+        if (f.v < 0) return fail(c, MEAO_ERR_INVALID, "%s %lld is negative (bottom-up views are not supported)", f.name, (long long)f.v);
+    if (p->depth_row > INT32_MAX) return fail(c, MEAO_ERR_INVALID, "depth_row_pitch %lld exceeds INT32_MAX", (long long)p->depth_row);
+    if (p->ao_row > INT32_MAX) return fail(c, MEAO_ERR_INVALID, "ao_row_pitch %lld exceeds INT32_MAX", (long long)p->ao_row);
+    if (p->depth_row < W * es || p->depth_row % es)
+        return fail(c, MEAO_ERR_INVALID, "depth_row_pitch %lld: must be at least width x %lld = %lld bytes and a multiple of %lld",
+                    (long long)p->depth_row, (long long)es, (long long)(W * es), (long long)es);
+    if (p->ao_row < W) return fail(c, MEAO_ERR_INVALID, "ao_row_pitch %lld is below the width %lld", (long long)p->ao_row, (long long)W);
+    if ((uintptr_t)depth % es) return fail(c, MEAO_ERR_INVALID, "depth_dev %p is not aligned to its %lld-byte element", depth, (long long)es);
+    if (L > 1) {
+        // layers must not overlap.  The extents below are then at most L x layer pitch: at most 2^16 x 2^63, which __int128 holds
+        const int64_t dmin = (rows - 1) * p->depth_row + W * es, amin = (rows - 1) * p->ao_row + W;
+        if (p->depth_layer < dmin)
+            return fail(c, MEAO_ERR_INVALID, "depth_layer_pitch %lld is below (rows - 1) x row pitch + width x %lld = %lld: layers would overlap",
+                        (long long)p->depth_layer, (long long)es, (long long)dmin);
+        // the kernels address the depth in elements: a layer pitch between two elements would read every layer after the first
+        // from misaligned bytes that start outside the view
+        if (p->depth_layer % es)
+            return fail(c, MEAO_ERR_INVALID, "depth_layer_pitch %lld is not a multiple of the %lld-byte element", (long long)p->depth_layer,
+                        (long long)es);
+        if (p->ao_layer < amin)
+            return fail(c, MEAO_ERR_INVALID, "ao_layer_pitch %lld is below (rows - 1) x row pitch + width = %lld: layers would overlap",
+                        (long long)p->ao_layer, (long long)amin);
+    } else {
+        const ViewPitch t = tight_pitch(c, kind);
+        p->depth_layer = t.depth_layer; p->ao_layer = t.ao_layer;
+    }
+    // The depth is read through the non-coherent path (ld.global.nc), so an AO view that shares bytes with it is undefined.  The test
+    // is conservative: it compares the byte ranges from each view's first to its last element, so two views that interleave without
+    // touching a common byte are refused as well.
+    using i128 = __int128;
+    const i128 d0 = (i128)(uintptr_t)depth, a0 = (i128)(uintptr_t)ao_out;
+    const i128 d1 = d0 + (i128)(L - 1) * p->depth_layer + (i128)(rows - 1) * p->depth_row + W * es;
+    const i128 a1 = a0 + (i128)(L - 1) * p->ao_layer + (i128)(rows - 1) * p->ao_row + W;
+    if (d0 < a1 && a0 < d1) return fail(c, MEAO_ERR_INVALID, "the byte extents of the depth view and the AO view (ao_out_dev) intersect");
+    return 0;
+}
+}  // namespace
 
-    // plan-once / replay: one captured graph per (depth, out, kind), like the reference's command buffer
+namespace {
+// The frame of meao_render / meao_render_pitched on a context that ensure_ready has prepared.
+int render_views(MeaoCtx *c, const void *depth, int kind, void *ao_out, ViewPitch p, void *stream)
+{
+    int rc;
+    if ((rc = check_views(c, depth, kind, ao_out, &p))) return rc;
+    cudaStream_t s = (cudaStream_t)stream;
+    if (c->flags & MEAO_FLAG_NO_GRAPH) return record_frame(c, depth, kind, ao_out, s, false, &p);
+
+    // plan-once / replay: one captured graph per (depth, out, kind, pitches), like the reference's command buffer
     // that is re-recorded only when something changed (AO.cs:334-347)
     NvtxRange nv("meao::frame");
-    const MeaoCtx::GraphKey key{{depth, ao_out, nullptr, nullptr}, kind};
+    const MeaoCtx::GraphKey key{{depth, ao_out, nullptr, nullptr}, kind, {p.depth_row, p.depth_layer, p.ao_row, p.ao_layer}};
     c->last_kind = kind; c->last_out = ao_out;
     return launch_cached(c, key, s, meao_kernels_per_frame(c), [&](cudaStream_t cs, int pdl) {
-        return record_frame_dag(c, depth, kind, ao_out, cs, true, pdl);
+        return record_frame_dag(c, depth, kind, ao_out, cs, true, pdl, false, nullptr, &p);
     });
+}
+}  // namespace
+
+int meao_render(MeaoCtx *c, const void *depth, int32_t kind, void *ao_out, void *stream)
+{
+    int rc = ensure_ready(c); if (rc) return rc;
+    return render_views(c, depth, kind, ao_out, tight_pitch(c, kind), stream);      // meao_render_pitched at the tight pitches
+}
+
+int meao_render_pitched(MeaoCtx *c, const void *depth, int64_t depth_row_pitch, int64_t depth_layer_pitch, int32_t kind,
+                        void *ao_out, int64_t ao_row_pitch, int64_t ao_layer_pitch, void *stream)
+{
+    int rc = ensure_ready(c); if (rc) return rc;
+    return render_views(c, depth, kind, ao_out, ViewPitch{depth_row_pitch, depth_layer_pitch, ao_row_pitch, ao_layer_pitch}, stream);
 }
 
 // ---- CUDA arrays (include/meao.h "CUDA arrays") ------------------------------------------------------------------------
@@ -1716,7 +1808,25 @@ int meao_bind_event(MeaoCtx *c, int32_t event_id, const void *depth, int32_t kin
     if (!c) return MEAO_ERR_INVALID;
     std::lock_guard<std::mutex> g(g_event_mutex);
     if (!depth && !ao_out) { g_events.erase(event_id); return MEAO_OK; }
-    g_events[event_id] = EventBinding{c, depth, kind, ao_out, stream, false};
+    g_events[event_id] = EventBinding{c, depth, kind, ao_out, stream, false, true, ViewPitch{}};
+    return MEAO_OK;
+}
+
+int meao_bind_event_pitched(MeaoCtx *c, int32_t event_id, const void *depth, int64_t depth_row_pitch, int64_t depth_layer_pitch, int32_t kind,
+                            void *ao_out, int64_t ao_row_pitch, int64_t ao_layer_pitch, void *stream)
+{
+    if (!c) return MEAO_ERR_INVALID;
+    if (!depth && !ao_out) {
+        std::lock_guard<std::mutex> g(g_event_mutex);
+        g_events.erase(event_id);
+        return MEAO_OK;
+    }
+    // checked now: the plugin event cannot report an error
+    int rc = ensure_ready(c); if (rc) return rc;
+    ViewPitch p{depth_row_pitch, depth_layer_pitch, ao_row_pitch, ao_layer_pitch};
+    if ((rc = check_views(c, depth, kind, ao_out, &p))) return rc;
+    std::lock_guard<std::mutex> g(g_event_mutex);
+    g_events[event_id] = EventBinding{c, depth, kind, ao_out, stream, false, false, p};
     return MEAO_OK;
 }
 
@@ -1733,7 +1843,7 @@ int meao_bind_event_arrays(MeaoCtx *c, int32_t event_id, const void *depth_array
     ArrayIO io;
     if ((rc = prepare_arrays(c, depth_array, kind, ao_array, &io))) return rc;
     std::lock_guard<std::mutex> g(g_event_mutex);
-    g_events[event_id] = EventBinding{c, depth_array, kind, ao_array, stream, true};
+    g_events[event_id] = EventBinding{c, depth_array, kind, ao_array, stream, true, false, ViewPitch{}};
     return MEAO_OK;
 }
 
@@ -1747,7 +1857,8 @@ void meao_render_event(int event_id)
         b = it->second;
     }
     if (b.arrays) meao_render_arrays(b.ctx, b.depth, b.kind, b.out, b.stream);
-    else meao_render(b.ctx, b.depth, b.kind, b.out, b.stream);
+    else if (b.tight) meao_render(b.ctx, b.depth, b.kind, b.out, b.stream);      // meao_render_pitched at the tight pitches of now
+    else meao_render_pitched(b.ctx, b.depth, b.pitch.depth_row, b.pitch.depth_layer, b.kind, b.out, b.pitch.ao_row, b.pitch.ao_layer, b.stream);
 }
 
 MeaoRenderEventFunc meao_get_render_event_func(void) { return meao_render_event; }

@@ -22,9 +22,10 @@ namespace {
 
 }  // namespace
 
-cudaError_t launch_prepare_depth(const PrepareArgs &a, cudaStream_t s, bool low_only)
+cudaError_t launch_prepare_depth(const PrepareArgs &a_in, cudaStream_t s, bool low_only)
 {
-    if (a.row1 <= a.row0) return cudaSuccess;
+    if (a_in.row1 <= a_in.row0) return cudaSuccess;
+    const PrepareArgs a = resolve_pitches(a_in);
     dim3 grid(ceil_div(a.W, kPrepTileW), ceil_div(a.row1 - a.row0, low_only ? kPrepLowTileH : kPrepTileH));
 #define MEAO_PREP_K(...) (low_only ? prepare_depth_low_kernel<__VA_ARGS__> : prepare_depth_kernel<__VA_ARGS__>)
     if (!a.raw) {

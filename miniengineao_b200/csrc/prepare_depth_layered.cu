@@ -1,5 +1,5 @@
 // prepare_depth_layered.cu -- stage 1 for a layered frame (meao_set_layers): L same-size depth images stacked at a stride of
-// one tight W x H image, ONE launch for all of them.  The kernel body is prepare_depth.cu's (prepare_depth_kernel.inc); the
+// PrepareArgs.depth_layer_pitch (tight: one W x H image), ONE launch for all of them.  The kernel body is prepare_depth.cu's (prepare_depth_kernel.inc); the
 // layer is blockIdx.z and selects the input image and the output images of every level (kernels.h "layered frames").
 // A translation unit of its own so that prepare_depth.cu compiles to exactly the code it did before.
 #include "common.cuh"
@@ -15,9 +15,10 @@ namespace {
 
 }  // namespace
 
-cudaError_t launch_prepare_depth_layered(const PrepareArgs &a, int layers, cudaStream_t s, bool low_only)
+cudaError_t launch_prepare_depth_layered(const PrepareArgs &a_in, int layers, cudaStream_t s, bool low_only)
 {
-    if (a.row1 <= a.row0) return cudaSuccess;
+    if (a_in.row1 <= a_in.row0) return cudaSuccess;
+    const PrepareArgs a = resolve_pitches(a_in);
     if (layers < 1 || layers > kMaxLayers) return cudaErrorInvalidValue;
     dim3 grid(ceil_div(a.W, kPrepTileW), ceil_div(a.row1 - a.row0, low_only ? kPrepLowTileH : kPrepTileH), layers);
 #define MEAO_PREP_K(...) (low_only ? prepare_depth_low_layered_kernel<__VA_ARGS__> : prepare_depth_layered_kernel<__VA_ARGS__>)
