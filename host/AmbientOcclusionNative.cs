@@ -53,6 +53,9 @@ namespace MiniEngineAO
         [DllImport(Lib)] public static extern int meao_set_camera(IntPtr ctx, ref MeaoCamera c);
         [DllImport(Lib)] public static extern int meao_resize(IntPtr ctx, int width, int height);
         [DllImport(Lib)] public static extern int meao_set_layers(IntPtr ctx, int layers);   // layered frames: L views per frame, [L][H][W] buffers
+        // one camera per layer (split-screen viewports, mirrors, batches from several cameras); null with count 0 clears the table
+        [DllImport(Lib)] public static extern int meao_set_layer_cameras(IntPtr ctx, [In] MeaoCamera[] cameras, int count);
+        [DllImport(Lib)] public static extern int meao_get_layer_cameras(IntPtr ctx, [Out] MeaoCamera[] cameras, int capacity);
         [DllImport(Lib)] public static extern int meao_render(IntPtr ctx, IntPtr depthDev, int depthKind, IntPtr aoOutDev, IntPtr stream);
         [DllImport(Lib)] public static extern int meao_render_host(IntPtr ctx, float[] depth, int depthKind, byte[] aoOut);
         [DllImport(Lib)] public static extern int meao_bind_event(IntPtr ctx, int eventId, IntPtr depthDev, int depthKind, IntPtr aoOutDev, IntPtr stream);
@@ -111,6 +114,10 @@ namespace MiniEngineAO
         // stereo target, 6 for cube-map faces.  The depth and AO buffers the interop layer maps then hold Layers images each.
         [SerializeField, Range(1, 65535)] int _layers = 1;
         public int Layers { get { return _layers; } set { _layers = value; } }
+        // One camera per layer (split-screen viewports, mirrors and portals, frames of several cameras in one batch); null: every layer
+        // renders with this component's camera.  Each must have this camera's pixel size; Length must equal Layers.
+        Camera[] _layerCameras;
+        public Camera[] LayerCameras { get { return _layerCameras; } set { _layerCameras = value; } }
         int _drawCountPerFrame;                                // AmbientOcclusion.cs:289, 349-355: single-pass stereo detection
         void OnPreRender() { _drawCountPerFrame++; }
         bool singlePassStereoEnabled                           // AmbientOcclusion.cs:392-401
@@ -174,11 +181,34 @@ namespace MiniEngineAO
             var layered = MeaoNative.meao_set_layers(_ctx, _layers);
             MeaoNative.Check(_ctx, layered);
             rebuild |= layered == 1;
+            rebuild |= SetLayerCameras() == 1;                                               // after meao_set_layers, which clears the table
             rebuild |= MeaoNative.meao_resize(_ctx, _camera.pixelWidth * (stereo ? 2 : 1), _camera.pixelHeight) == 1;   // :338-341
             rebuild |= !Application.isPlaying;                                               // :345
             _drawCountPerFrame = 0;                                                          // :349
 
             if (rebuild || _renderCommand == null) RebuildCommandBuffers();
+        }
+
+        // Hands LayerCameras to the plugin; returns 1 if it re-planned.  The same table again returns 0, so this runs every frame.
+        int SetLayerCameras()
+        {
+            if (_layerCameras == null) return MeaoNative.meao_set_layer_cameras(_ctx, null, 0);
+            var cams = new MeaoNative.MeaoCamera[_layerCameras.Length];
+            for (int i = 0; i < cams.Length; i++)
+            {
+                var c = _layerCameras[i];
+                if (c.pixelWidth != _camera.pixelWidth || c.pixelHeight != _camera.pixelHeight)
+                    throw new ArgumentException("LayerCameras[" + i + "] has another pixel size than the camera");
+                cams[i] = new MeaoNative.MeaoCamera
+                {
+                    near_clip = c.nearClipPlane, far_clip = c.farClipPlane,
+                    tan_half_fov_h = 1 / c.projectionMatrix[0, 0],
+                    reversed_z = SystemInfo.usesReversedZBuffer ? 1 : 0
+                };
+            }
+            var rc = MeaoNative.meao_set_layer_cameras(_ctx, cams, cams.Length);
+            MeaoNative.Check(_ctx, rc);
+            return rc;
         }
 
         void RebuildCommandBuffers()

@@ -149,7 +149,8 @@ int meao_set_camera(MeaoCtx *ctx, const MeaoCamera *camera);
 int meao_resize(MeaoCtx *ctx, int32_t width, int32_t height);
 /* Layered frames: every frame holds `layers` independent views of width x height (texture-array stereo: 2 eye slices; cube-map
  * AO: 6 faces; a batch of frames of one camera), rendered by ONE launch per stage.  Each layer's result is bit-identical to
- * rendering that layer alone; one MeaoParams / MeaoCamera / MeaoVariants applies to all layers.  Layout rule: every image argument
+ * rendering that layer alone; one MeaoParams / MeaoCamera / MeaoVariants applies to all layers unless meao_set_layer_cameras gives
+ * each layer its own camera.  Layout rule: every image argument
  * holds the L images stacked at a stride of one tight image -- depth is L*width*height elements of the depth kind, the AO output
  * L*width*height bytes -- for meao_render, meao_render_host(_async), meao_bind_event, meao_profile_frame, the meao_stage_* calls,
  * meao_debug_view (L images) and the meao_composite_* calls (L*width*height pixels).  meao_get_buffer / meao_set_buffer use
@@ -160,8 +161,24 @@ int meao_resize(MeaoCtx *ctx, int32_t width, int32_t height);
  * neighbour connections.  layers must be in 1..65535 (the layer is a grid dimension of the layered kernels), else
  * MEAO_ERR_INVALID; MEAO_ERR_NOMEM if the intermediates do not fit (the context keeps its previous layer count).
  * Row bands and layers exclude each other: with layers > 1, meao_set_row_band, the halo calls (meao_halo_*, meao_render_band_*,
- * meao_band_phase_a / _b) and the native exchange (meao_band_export / _connect / _step / _step_host) return MEAO_ERR_UNSUPPORTED. */
+ * meao_band_phase_a / _b) and the native exchange (meao_band_export / _connect / _step / _step_host) return MEAO_ERR_UNSUPPORTED.
+ * A change of the layer count also CLEARS the per-layer camera table (meao_set_layer_cameras): set it again after every call that
+ * returned 1. */
 int meao_set_layers(MeaoCtx *ctx, int32_t layers);
+/* Per-layer cameras for layered frames (split-screen viewports, mirrors and portals, batches of frames from several cameras): layer
+ * l is rendered with cameras[l] -- its near and far planes and field of view -- and is bit-identical to a single-layer meao_render
+ * of that layer's depth with meao_set_camera(cameras[l]), for the AO and every debug buffer.  MeaoParams, MeaoVariants and the
+ * size stay shared.  count must equal meao_set_layers; cameras == NULL with count == 0 clears the table, and every layer then uses
+ * the meao_set_camera camera again.  Each entry is validated like meao_set_camera, and all entries must have the same reversed_z
+ * (a platform property).  A refusal returns MEAO_ERR_INVALID, names the layer and field in meao_last_error, and changes nothing.
+ * A plan input like meao_set_camera: returns 1 if the plan was dirtied (the next frame re-plans and drops the captured graphs),
+ * 0 if the same table is set again -- so a host may call it every frame.  While a table is set it alone defines every layer's
+ * camera; meao_set_camera still records the shared camera, which takes effect when the table is cleared.  A change of the layer
+ * count clears the table.  Works on plan-only contexts (device < 0); with layers == 1 a table of one camera behaves exactly like
+ * meao_set_camera. */
+int meao_set_layer_cameras(MeaoCtx *ctx, const MeaoCamera *cameras, int32_t count);
+/* Copies the table into out (capacity entries; MEAO_ERR_INVALID if it does not fit) and returns its entry count (0 = no table). */
+int meao_get_layer_cameras(const MeaoCtx *ctx, MeaoCamera *out, int32_t capacity);
 
 /* ---- the frame ------------------------------------------------------------------------------- */
 /* replaces: replay of the "SSAO" command buffer, steps 1-10 of RebuildCommandBuffers (AO.cs:511-531):
@@ -276,6 +293,10 @@ int meao_render_constants_wide(MeaoCtx *ctx, int32_t level, float out28[28]);
 int meao_upsample_constants(MeaoCtx *ctx, int32_t lo_level, float out8[8]);
 /* out[0..3] ZBufferParams (AO.cs:561-568) */
 int meao_zbuffer_params(MeaoCtx *ctx, float out4[4]);
+/* The same per layer (0 .. layers-1) of a layered context: its own camera's values under meao_set_layer_cameras, the shared ones
+ * without a table.  The getters above return layer 0's.  wide: the layout of meao_render_constants_wide. */
+int meao_render_constants_layer(MeaoCtx *ctx, int32_t layer, int32_t level, int32_t wide, float out28[28]);
+int meao_zbuffer_params_layer(MeaoCtx *ctx, int32_t layer, float out4[4]);
 
 /* ---- row-band partitioning of one frame over several GPUs (new capability, SURVEY.md 8e) -------- */
 /* This context computes output rows [row0, row1) of the width x height frame set by meao_resize

@@ -60,6 +60,8 @@ SIGNATURES = {
     "meao_set_camera": (C.c_int, [C.c_void_p, C.POINTER(MeaoCamera)]),
     "meao_resize": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
     "meao_set_layers": (C.c_int, [C.c_void_p, C.c_int32]),
+    "meao_set_layer_cameras": (C.c_int, [C.c_void_p, C.POINTER(MeaoCamera), C.c_int32]),
+    "meao_get_layer_cameras": (C.c_int, [C.c_void_p, C.POINTER(MeaoCamera), C.c_int32]),
     "meao_render": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "meao_render_pitched": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_int64, C.c_int64,
                                       C.c_void_p]),
@@ -83,6 +85,8 @@ SIGNATURES = {
     "meao_debug_view": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "meao_upsample_constants": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_float)]),
     "meao_zbuffer_params": (C.c_int, [C.c_void_p, C.POINTER(C.c_float)]),
+    "meao_render_constants_layer": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_float)]),
+    "meao_zbuffer_params_layer": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_float)]),
     "meao_set_row_band": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "meao_halo_bytes": (C.c_int64, [C.c_void_p, C.c_int32]),
     "meao_halo_recv_bytes": (C.c_int64, [C.c_void_p, C.c_int32]),

@@ -81,6 +81,9 @@ class AmbientOcclusion:
         self.highQualityMask = 0            # bit k-1: Render.compute kernel "main" on level k + Upsample main_premin*
         self.singleScale = False            # BASELINE.json configs[0]: Downsample1 -> Render level 1 -> final-style Upsample only
         self.layers = 1                     # views per frame (meao_set_layers): texture-array stereo 2, cube faces 6, frame batches
+        # one Camera per layer (meao_set_layer_cameras): split-screen viewports, mirrors, batches from several cameras; None = every
+        # layer uses `camera`.  Each entry must match the main camera's pixelWidth, pixelHeight and usesReversedZBuffer.
+        self.layerCameras: list[Camera] | None = None
         self._band = None                   # (row0, row1) after set_row_band; reset by every re-allocation
         self._drawCountPerFrame = 0         # AO.cs:289: used to detect single-pass stereo
         self._stereo = False                # singlePassStereoEnabled as latched by the last LateUpdate
@@ -146,6 +149,7 @@ class AmbientOcclusion:
         rebuild |= self._check(self._lib.meao_set_variants(self._ctx, C.byref(v))) == 1
         width = cam.pixelWidth * (2 if stereo else 1)                                                # AO.cs:338-341, 501-504
         layered = self._check(self._lib.meao_set_layers(self._ctx, int(self.layers))) == 1           # re-allocates like a resize
+        rebuild |= self._apply_layer_cameras()
         resized = self._check(self._lib.meao_resize(self._ctx, width, cam.pixelHeight)) == 1          # CheckBaseDimensions
         resized |= layered
         self._width, self._height = width, cam.pixelHeight
@@ -156,6 +160,22 @@ class AmbientOcclusion:
         if frame:
             self._drawCountPerFrame = 0                                                              # AO.cs:349
         return rebuild or resized
+
+    def _apply_layer_cameras(self) -> bool:
+        """Hands layerCameras to meao_set_layer_cameras (after meao_set_layers, which clears the table); True if it re-planned."""
+        cams = self.layerCameras
+        if cams is None:
+            return self._check(self._lib.meao_set_layer_cameras(self._ctx, None, 0)) == 1
+        main = self._camera
+        for i, c in enumerate(cams):
+            for f in ("pixelWidth", "pixelHeight", "usesReversedZBuffer"):
+                if getattr(c, f) != getattr(main, f):
+                    raise ValueError(f"layerCameras[{i}].{f} = {getattr(c, f)!r} differs from the camera's {getattr(main, f)!r}")
+        if len(cams) != int(self.layers):
+            raise ValueError(f"layerCameras has {len(cams)} entries for {int(self.layers)} layers")
+        arr = (N.MeaoCamera * len(cams))(*[N.MeaoCamera(c.nearClipPlane, c.farClipPlane, 1.0 / c.projection00, int(c.usesReversedZBuffer))
+                                           for c in cams])
+        return self._check(self._lib.meao_set_layer_cameras(self._ctx, arr, len(cams))) == 1
 
     # ---- frame ----------------------------------------------------------------------------------
     @staticmethod

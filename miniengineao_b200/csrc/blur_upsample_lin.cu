@@ -28,15 +28,18 @@ namespace {
 // their raw depth, linearise it (DS1:37-48), round it to f16 and store it to LinearDepth at `lin` (this thread's first pixel; the
 // 16-byte store is aligned because px0 % 8 == 0 and rows are 128-byte pitched).  Returns the packed halves (pixel 0 in the low half
 // of .x): what the 128-bit LinearDepth load of the kernel that reads LinearDepth returns.
-template <int IN>
+// LAYERED: the layer's ZBufferParams come from din.layer_zb when it is set (per-layer cameras).
+template <int IN, bool LAYERED = false>
 __device__ __forceinline__ uint4 linearize_pixels8(const DepthIn &din, int layer, int py, int px0, int hiw, int hih, bool full, __half *lin)
 {
     const void *depth = reinterpret_cast<const char *>(din.depth) + (size_t)layer * din.depth_layer_pitch * (IN == IN_D16 ? 2 : 4);
     float v[8], d[8];
     load8<IN>(depth, (size_t)(py - din.depth_row0) * din.depth_pitch + px0, full && din.vec_ok, hiw - px0, v);
-    if (!din.raw) linearize8<false, true>(v, din.zbx, din.zby, d);
-    else if (din.reversed_z) linearize8<true, true>(v, din.zbx, din.zby, d);
-    else linearize8<true, false>(v, din.zbx, din.zby, d);
+    float zbx = din.zbx, zby = din.zby;
+    if (LAYERED && din.layer_zb) { zbx = __ldg(&din.layer_zb[layer].zbx); zby = __ldg(&din.layer_zb[layer].zby); }
+    if (!din.raw) linearize8<false, true>(v, zbx, zby, d);
+    else if (din.reversed_z) linearize8<true, true>(v, zbx, zby, d);
+    else linearize8<true, false>(v, zbx, zby, d);
     const __half2 h0 = __floats2half2_rn(d[0], d[1]), h1 = __floats2half2_rn(d[2], d[3]);
     const __half2 h2 = __floats2half2_rn(d[4], d[5]), h3 = __floats2half2_rn(d[6], d[7]);
     uint4 pk;

@@ -157,6 +157,8 @@ struct DepthIn {
     int depth_pitch;        // elements from one depth row to the next
     long long depth_layer_pitch;    // layered: elements from one depth layer to the next
     long long ao_layer_pitch;       // layered: bytes from one layer of UpsampleArgs.out to the next
+    // appended last: the layered kernels' per-layer ZBufferParams (LayerZ table below); nullptr: zbx / zby for every layer
+    const struct LayerZ *layer_zb;
 };
 cudaError_t launch_blur_upsample_lin(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
                                      const UpsampleArgs &a, const uint8_t *lo_ao2, int lo_a2pitch, const DepthIn &din, int layers, int sm_count,
@@ -169,8 +171,22 @@ cudaError_t launch_blur_upsample_lin(const CUtensorMap &lo_depth_map, const CUte
 // fetch a box only when it lies inside one layer.  Separate kernels and translation units (*_layered.cu), so the single-image
 // kernels keep their code.  kMaxLayers: the prepare_depth / render_ao grids carry the layer in gridDim.z (at most 65535).
 constexpr int kMaxLayers = 65535;
-cudaError_t launch_prepare_depth_layered(const PrepareArgs &a, int layers, cudaStream_t s, bool low_only = false);
-cudaError_t launch_render_ao_layered(const CUtensorMap &low_map, bool use_tma, const RenderArgs &a, int layers, cudaStream_t s);
+
+// Per-layer cameras (meao_set_layer_cameras): the camera-dependent constants of every layer, in tables in the context's arena (any
+// layer count up to kMaxLayers, so neither kernel parameters nor __constant__ memory).  The plan fills every entry alike when the
+// layers share one camera; the layered and array kernels read entry blockIdx.z (the fused upsample: its tile's layer).
+struct LayerZ { float zbx, zby; };              // ZBufferParams.xy of one layer
+struct LayerRender {                            // the camera-dependent RenderArgs fields of one layer at one render launch (level, wide)
+    float2 it_nf[12];                           // {inv_thickness[i], neg_front[i]} in CALL order (RenderArgs): one 8-byte read per sample group
+    float pad;                                  // raw ingest's atlas padding value of the level, f16-rounded (RenderArgs.pad)
+    float pad_[7];                              // to 128 bytes
+};
+static_assert(sizeof(LayerRender) == 128, "LayerRender is one 128-byte line");
+// layer_zb / layer_cam: the per-layer camera tables below, entry l = layer l (nullptr: the argument block's constants for every layer);
+// layer_pad: 1 = the entries' pad (raw ingest), 0 = RenderArgs.pad (linear ingest pads with 0)
+cudaError_t launch_prepare_depth_layered(const PrepareArgs &a, int layers, cudaStream_t s, bool low_only = false, const struct LayerZ *layer_zb = nullptr);
+cudaError_t launch_render_ao_layered(const CUtensorMap &low_map, bool use_tma, const RenderArgs &a, int layers, cudaStream_t s,
+                                     const struct LayerRender *layer_cam = nullptr, int layer_pad = 0);
 cudaError_t launch_blur_upsample_layered(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
                                          const UpsampleArgs &a, const uint8_t *lo_ao2, int lo_a2pitch, int layers, int sm_count, cudaStream_t s);
 
@@ -180,7 +196,8 @@ cudaError_t launch_blur_upsample_layered(const CUtensorMap &lo_depth_map, const 
 // other kernels are the existing ones.  prepare: in_format f32 or D16 (no CUDA array holds D24S8); upsample: the final level only
 // (hi_depth = LinearDepth, no hi_ao; a.out is unused).  Separate kernels and translation units (*_array.cu).
 enum { kSurf2D = 0, kSurfLayered = 1, kSurfCube = 2 };    // how a surface's layer coordinate is addressed (the array's shape)
-cudaError_t launch_prepare_depth_array(const PrepareArgs &a, cudaSurfaceObject_t depth, int surf_kind, int layers, cudaStream_t s);
+cudaError_t launch_prepare_depth_array(const PrepareArgs &a, cudaSurfaceObject_t depth, int surf_kind, int layers, cudaStream_t s,
+                                       const struct LayerZ *layer_zb = nullptr);
 cudaError_t launch_blur_upsample_array(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
                                        const UpsampleArgs &a, const uint8_t *lo_ao2, int lo_a2pitch, int layers, int sm_count,
                                        cudaSurfaceObject_t out, int surf_kind, cudaStream_t s);

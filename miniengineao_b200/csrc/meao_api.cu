@@ -57,6 +57,14 @@ struct Plan {
     float zb[4];
 };
 
+// The camera-dependent part of the plan, for one camera: ZBufferParams, both inv_thickness tables of every level and the atlas
+// padding value.  Plan holds it for the first layer; with per-layer cameras MeaoCtx::layer_consts holds it for every layer.
+struct CamConsts {
+    float zb[2];
+    float inv_thickness[5][12], inv_thickness_wide[5][12];
+    float pad[5];
+};
+
 }  // namespace
 
 struct MeaoCtx {
@@ -72,9 +80,12 @@ struct MeaoCtx {
 
     MeaoParams params;
     MeaoCamera camera;
+    std::vector<MeaoCamera> layer_cams;     // meao_set_layer_cameras: one camera per layer, or empty (every layer uses `camera`)
     MeaoVariants variants = {0, 0, 0, 0};
     bool plan_dirty = true;
     Plan plan;
+    std::vector<CamConsts> layer_consts;    // the plan's camera constants of every layer (all alike without a layer-camera table)
+    bool cam_table_stale = true;            // layer_consts changed since the device tables were written (ensure_ready uploads them)
 
     int W = 0, H = 0;
     int lw[7] = {0}, lh[7] = {0};
@@ -149,6 +160,9 @@ struct MeaoCtx {
     // that uses it may still be in flight.
     std::map<const void *, cudaSurfaceObject_t> surfaces;
     int last_kind = MEAO_DEPTH_RAW_F32;     // ingest kind of the last downsample (selects the atlas padding value)
+    // the per-layer camera tables in the arena (kernels.h LayerZ / LayerRender): layer_zb[l]; layer_ren[(2 (k - 1) + wide) L + l]
+    LayerZ *layer_zb = nullptr;
+    LayerRender *layer_ren = nullptr;
 
     std::vector<std::pair<std::string, float>> last_profile;
     int profile_repeats = 1;                // launches per kernel inside one event pair of meao_profile_frame
@@ -189,32 +203,70 @@ void sample_thickness(float t[12])
     t[10] = mathf_sqrt(1 - 0.4f * 0.4f - 0.8f * 0.8f);  t[11] = mathf_sqrt(1 - 0.6f * 0.6f - 0.6f * 0.6f);
 }
 
+// The camera-dependent constants of camera `cam` (the part of build_plan that reads the camera).
+void camera_consts(const MeaoCtx *c, const MeaoCamera &cam, CamConsts &p)
+{
+    // AO.cs:561-568
+    const float fpn = cam.far_clip / cam.near_clip;
+    if (cam.reversed_z) { p.zb[0] = fpn - 1; p.zb[1] = 1; } else { p.zb[0] = 1 - fpn; p.zb[1] = fpn; }
+
+    float thick[12];
+    sample_thickness(thick);
+    for (int k = 1; k <= 4; k++) {
+        const int src_w = c->lw[k + 2];
+        const float ScreenspaceDiameter = 10;                                                        // AO.cs:669
+        float ThicknessMultiplier = 2 * cam.tan_half_fov_h * ScreenspaceDiameter / src_w;           // AO.cs:678
+        if (c->variants.single_pass_stereo) ThicknessMultiplier *= 2;                                // AO.cs:680
+        float InverseRangeFactor = 1 / ThicknessMultiplier;                                          // AO.cs:683
+        for (int i = 0; i < 12; i++) p.inv_thickness[k][i] = InverseRangeFactor / thick[i];          // AO.cs:687-688
+        {   // the same recorder fed a non-tiled source (LowDepth<k>): kernel "main"
+            float tm = 2 * cam.tan_half_fov_h * ScreenspaceDiameter / c->lw[k];                     // AO.cs:678
+            tm *= 2;                                                                                 // AO.cs:679 (!source.isTiled)
+            if (c->variants.single_pass_stereo) tm *= 2;                                             // AO.cs:680
+            const float irf = 1 / tm;                                                                // AO.cs:683
+            for (int i = 0; i < 12; i++) p.inv_thickness_wide[k][i] = irf / thick[i];
+        }
+        // value of the atlas padding texels (SURVEY.md P3): Downsample1 writes Linearize(OOB load = 0),
+        // Downsample2 writes 0 (its OOB load of DS4x)
+        float pad = 0.0f;
+        if (k <= 2) {
+            // raw depth 0 through Linearize (DS1:40-45); linear ingest: 0
+            pad = cam.reversed_z ? 1e5f : 1.0f / std::fmaf(p.zb[0], 0.0f, p.zb[1]);
+        }
+        p.pad[k] = pad;   // the depth-kind dependent part (linear ingest -> 0) is applied at launch
+    }
+}
+
 // Rebuild the per-dispatch constants (the CPU half of RebuildCommandBuffers, AO.cs:496-540).
 void build_plan(MeaoCtx *c)
 {
     Plan &p = c->plan;
-    // AO.cs:561-568
-    const float fpn = c->camera.far_clip / c->camera.near_clip;
-    if (c->camera.reversed_z) { p.zb[0] = fpn - 1; p.zb[1] = 1; } else { p.zb[0] = 1 - fpn; p.zb[1] = fpn; }
+    // every layer's camera constants: one entry per distinct camera computed, copied to the layers that share it
+    const int L = c->layers;
+    c->layer_consts.resize(L);
+    if (c->layer_cams.empty()) {
+        camera_consts(c, c->camera, c->layer_consts[0]);
+        for (int l = 1; l < L; l++) c->layer_consts[l] = c->layer_consts[0];
+    } else {
+        for (int l = 0; l < L; l++) {
+            if (l > 0 && memcmp(&c->layer_cams[l], &c->layer_cams[l - 1], sizeof(MeaoCamera)) == 0) c->layer_consts[l] = c->layer_consts[l - 1];
+            else camera_consts(c, c->layer_cams[l], c->layer_consts[l]);
+        }
+    }
+    c->cam_table_stale = true;
+    // the Plan's own camera constants: the first layer's
+    const CamConsts &cc = c->layer_consts[0];
+    p.zb[0] = cc.zb[0]; p.zb[1] = cc.zb[1];
     p.zb[2] = p.zb[3] = 0;
+    memcpy(p.inv_thickness, cc.inv_thickness, sizeof p.inv_thickness);
+    memcpy(p.inv_thickness_wide, cc.inv_thickness_wide, sizeof p.inv_thickness_wide);
+    memcpy(p.pad, cc.pad, sizeof p.pad);
 
     float thick[12];
     sample_thickness(thick);
     for (int k = 1; k <= 4; k++) {
         const int src_w = c->lw[k + 2], src_h = c->lh[k + 2];
-        const float ScreenspaceDiameter = 10;                                                        // AO.cs:669
-        float ThicknessMultiplier = 2 * c->camera.tan_half_fov_h * ScreenspaceDiameter / src_w;     // AO.cs:678
-        if (c->variants.single_pass_stereo) ThicknessMultiplier *= 2;                                // AO.cs:680
-        float InverseRangeFactor = 1 / ThicknessMultiplier;                                          // AO.cs:683
-        for (int i = 0; i < 12; i++) p.inv_thickness[k][i] = InverseRangeFactor / thick[i];          // AO.cs:687-688
-        {   // the same recorder fed a non-tiled source (LowDepth<k>): kernel "main"
-            float tm = 2 * c->camera.tan_half_fov_h * ScreenspaceDiameter / c->lw[k];               // AO.cs:678
-            tm *= 2;                                                                                 // AO.cs:679 (!source.isTiled)
-            if (c->variants.single_pass_stereo) tm *= 2;                                             // AO.cs:680
-            const float irf = 1 / tm;                                                                // AO.cs:683
-            for (int i = 0; i < 12; i++) p.inv_thickness_wide[k][i] = irf / thick[i];
-            p.inv_slice_dim_wide[k][0] = 1.0f / c->lw[k]; p.inv_slice_dim_wide[k][1] = 1.0f / c->lh[k];
-        }
+        p.inv_slice_dim_wide[k][0] = 1.0f / c->lw[k]; p.inv_slice_dim_wide[k][1] = 1.0f / c->lh[k];
         static const float mult[12] = {4, 4, 4, 4, 4, 8, 8, 8, 4, 8, 8, 4};                          // AO.cs:696-707
         float *w = p.sample_weight[k];
         for (int i = 0; i < 12; i++) w[i] = mult[i] * thick[i];
@@ -223,14 +275,6 @@ void build_plan(MeaoCtx *c)
         for (int i = 0; i < 12; i++) total += w[i];                                                  // AO.cs:718-721
         for (int i = 0; i < 12; i++) w[i] /= total;                                                  // AO.cs:723-724
         p.inv_slice_dim[k][0] = 1.0f / src_w; p.inv_slice_dim[k][1] = 1.0f / src_h;                  // AO.cs:732
-        // value of the atlas padding texels (SURVEY.md P3): Downsample1 writes Linearize(OOB load = 0),
-        // Downsample2 writes 0 (its OOB load of DS4x)
-        float pad = 0.0f;
-        if (k <= 2) {
-            // raw depth 0 through Linearize (DS1:40-45); linear ingest: 0
-            pad = c->camera.reversed_z ? 1e5f : 1.0f / std::fmaf(p.zb[0], 0.0f, p.zb[1]);
-        }
-        p.pad[k] = pad;   // the depth-kind dependent part (linear ingest -> 0) is applied at launch
     }
     p.reject_fadeoff = -1 / c->params.thickness_modifier;                                            // AO.cs:733
     p.intensity = c->params.intensity;                                                               // AO.cs:734
@@ -380,6 +424,7 @@ int allocate(MeaoCtx *c)
     }
     size_t o_dst[2], o_ast[2];
     for (int i = 0; i < 2; i++) { o_dst[i] = take(L * W * H * sizeof(float)); o_ast[i] = take(L * W * H); }
+    const size_t o_lzb = take(L * sizeof(LayerZ)), o_lren = take(8 * L * sizeof(LayerRender));
     cudaError_t e = cudaMalloc(&c->arena, off);
     if (e != cudaSuccess) return fail(c, e == cudaErrorMemoryAllocation ? MEAO_ERR_NOMEM : MEAO_ERR_CUDA,
                                       "cudaMalloc(%zu) failed: %s", off, cudaGetErrorString(e));
@@ -403,6 +448,8 @@ int allocate(MeaoCtx *c)
         c->hq[k] = (uint8_t *)(b + o_hq[k]);
     }
     for (int i = 0; i < 2; i++) { c->depth_stage[i] = (float *)(b + o_dst[i]); c->ao_stage[i] = (uint8_t *)(b + o_ast[i]); }
+    c->layer_zb = (LayerZ *)(b + o_lzb);
+    c->layer_ren = (LayerRender *)(b + o_lren);     // written by the first ensure_ready (the plan is dirty)
 
     c->tma_ok = false;
     if (c->encode) {
@@ -434,6 +481,46 @@ int allocate(MeaoCtx *c)
     return setup_band(c);
 }
 
+// The call-order tables of record_render: Render.compute:162-168 (checker) and :148-159 (exhaustive) table slots
+const int kIdxChecker[7] = {1, 3, 4, 8, 11, 6, 10};
+const int kIdxExh[12] = {0, 1, 2, 3, 4, 8, 11, 5, 6, 7, 9, 10};
+
+// The LayerRender entry of camera constants `cc` at render level k (wide: kernel "main"): what record_render puts into RenderArgs
+LayerRender layer_render(const MeaoCtx *c, const CamConsts &cc, int k, bool wide)
+{
+    const bool exh = c->variants.sample_exhaustively != 0;
+    const int n = exh ? 12 : 7;
+    const int *idx = exh ? kIdxExh : kIdxChecker;
+    const float *it = wide ? cc.inv_thickness_wide[k] : cc.inv_thickness[k];
+    LayerRender r{};
+    for (int i = 0; i < n; i++) {
+        r.it_nf[i].x = it[idx[i]];
+        r.it_nf[i].y = -(r.it_nf[i].x - 0.5f);                                                      // Render.compute:85
+    }
+    r.pad = host_f16_round(cc.pad[k]);
+    return r;
+}
+
+// Write the per-layer camera tables to the arena.  Called by ensure_ready after a re-plan, once every frame that may read the old
+// tables has finished (a device synchronise: frames may be in flight on any caller stream).
+int upload_camera_tables(MeaoCtx *c)
+{
+    const int L = c->layers;
+    std::vector<LayerZ> zb(L);
+    std::vector<LayerRender> ren((size_t)8 * L);
+    for (int l = 0; l < L; l++) {
+        const CamConsts &cc = c->layer_consts[l];
+        zb[l] = LayerZ{cc.zb[0], cc.zb[1]};
+        for (int k = 1; k <= 4; k++)
+            for (int w = 0; w < 2; w++) ren[(size_t)(2 * (k - 1) + w) * L + l] = layer_render(c, cc, k, w != 0);
+    }
+    CUDA_TRY(c, cudaDeviceSynchronize());
+    CUDA_TRY(c, cudaMemcpy(c->layer_zb, zb.data(), zb.size() * sizeof(LayerZ), cudaMemcpyHostToDevice));
+    CUDA_TRY(c, cudaMemcpy(c->layer_ren, ren.data(), ren.size() * sizeof(LayerRender), cudaMemcpyHostToDevice));
+    c->cam_table_stale = false;
+    return 0;
+}
+
 int ensure_ready(MeaoCtx *c)
 {
     if (!c) return MEAO_ERR_INVALID;
@@ -442,7 +529,16 @@ int ensure_ready(MeaoCtx *c)
     CUDA_TRY(c, cudaSetDevice(c->device));
     if (c->plan_dirty) { build_plan(c); c->graphs_stale = true; }
     if (c->graphs_stale) drop_graph(c);
+    if (c->cam_table_stale) { int rc = upload_camera_tables(c); if (rc) return rc; }
     return 0;
+}
+
+// Z direction of the context's cameras (meao_set_layer_cameras requires one for all layers)
+inline int ctx_reversed_z(const MeaoCtx *c) { return c->layer_cams.empty() ? c->camera.reversed_z : c->layer_cams[0].reversed_z; }
+// The f16-rounded atlas padding value of layer l at render level k for depth kind `kind` (linear ingest pads with 0)
+inline float layer_pad(const MeaoCtx *c, int l, int k, int kind)
+{
+    return host_f16_round((kind != MEAO_DEPTH_LINEAR_F32) ? c->layer_consts[l].pad[k] : 0.0f);
 }
 
 struct NvtxRange { explicit NvtxRange(const char *n) { nvtxRangePushA(n); } ~NvtxRange() { nvtxRangePop(); } };
@@ -489,12 +585,13 @@ DepthIn depth_in(const MeaoCtx *c, const void *depth, int kind, const ViewPitch 
     d.depth_row0 = c->band0;
     d.zbx = c->plan.zb[0]; d.zby = c->plan.zb[1];
     d.raw = (kind != MEAO_DEPTH_LINEAR_F32);
-    d.reversed_z = c->camera.reversed_z;
+    d.reversed_z = ctx_reversed_z(c);
     // 128-bit loads: every row (and layer) start 16-byte aligned.  Tight views: W % 4 == 0 (4-byte kinds), W % 8 == 0 (D16)
     d.vec_ok = (((uintptr_t)depth & 15) == 0) && (p.depth_row % 16 == 0) && (c->layers == 1 || p.depth_layer % 16 == 0);
     d.depth_pitch = (int)(p.depth_row / es);
     d.depth_layer_pitch = p.depth_layer / es;
     d.ao_layer_pitch = p.ao_layer;
+    d.layer_zb = c->layer_zb;
     return d;
 }
 
@@ -521,8 +618,8 @@ int record_downsample(MeaoCtx *c, const void *depth, int kind, cudaStream_t s, c
     a.vec_ok = d.vec_ok;
     a.depth_pitch = d.depth_pitch; a.depth_layer_pitch = d.depth_layer_pitch;
     c->last_kind = kind;
-    if (aio) CUDA_TRY(c, launch_prepare_depth_array(a, aio->depth, aio->depth_surf, c->layers, s));
-    else if (c->layers > 1) CUDA_TRY(c, launch_prepare_depth_layered(a, c->layers, s, low_only));
+    if (aio) CUDA_TRY(c, launch_prepare_depth_array(a, aio->depth, aio->depth_surf, c->layers, s, d.layer_zb));
+    else if (c->layers > 1) CUDA_TRY(c, launch_prepare_depth_layered(a, c->layers, s, low_only, d.layer_zb));
     else CUDA_TRY(c, launch_prepare_depth(a, s, low_only));
     c->launches++;
     return 0;
@@ -532,11 +629,9 @@ int record_downsample(MeaoCtx *c, const void *depth, int kind, cudaStream_t s, c
 // wide = true: the same recorder for the non-tiled source LowDepth<k> (kernel main) -> HighQuality<k>.
 int record_render(MeaoCtx *c, int k, int kind, cudaStream_t s, bool wide = false)
 {
-    static const int idx_checker[7] = {1, 3, 4, 8, 11, 6, 10};                       // Render.compute:162-168 table slots, call order
-    static const int idx_exh[12] = {0, 1, 2, 3, 4, 8, 11, 5, 6, 7, 9, 10};           // Render.compute:148-159
     const bool exh = c->variants.sample_exhaustively != 0;
     const int n = exh ? 12 : 7;
-    const int *idx = exh ? idx_exh : idx_checker;
+    const int *idx = exh ? kIdxExh : kIdxChecker;
     NvtxRange nv(wide ? "meao::render_ao_wide" : "meao::render_ao");
     RenderArgs a{};
     a.low = c->low[k]; a.lw = c->lw[k]; a.lh = c->lh[k]; a.lpitch = c->low_pitch[k];
@@ -557,7 +652,9 @@ int record_render(MeaoCtx *c, int k, int kind, cudaStream_t s, bool wide = false
     const int tv = render_tile_variant(c, k, a.row1 - (a.row0 & ~3));
     a.tile_h = kRenderTileHs[tv];
     const CUtensorMap &map = wide ? c->map_low_wide[tv][k] : c->map_low_ren[tv][k];
-    if (c->layers > 1) CUDA_TRY(c, launch_render_ao_layered(map, c->tma_ok, a, c->layers, s));
+    if (c->layers > 1)
+        CUDA_TRY(c, launch_render_ao_layered(map, c->tma_ok, a, c->layers, s, c->layer_ren + (size_t)(2 * (k - 1) + (wide ? 1 : 0)) * c->layers,
+                                             kind != MEAO_DEPTH_LINEAR_F32 ? 1 : 0));
     else CUDA_TRY(c, launch_render_ao(map, c->tma_ok, a, s));
     c->launches++;
     return 0;
@@ -891,8 +988,47 @@ int meao_set_camera(MeaoCtx *c, const MeaoCamera *cam)
     if (!c || !cam) return MEAO_ERR_INVALID;
     if (!(cam->near_clip > 0) || !(cam->far_clip > cam->near_clip) || !(cam->tan_half_fov_h > 0))
         return fail(c, MEAO_ERR_INVALID, "bad camera (near %g far %g tanHalfFovH %g)", cam->near_clip, cam->far_clip, cam->tan_half_fov_h);
-    if (memcmp(&c->camera, cam, sizeof *cam) != 0) { c->camera = *cam; c->plan_dirty = true; }
+    if (memcmp(&c->camera, cam, sizeof *cam) != 0) {
+        c->camera = *cam;
+        if (c->layer_cams.empty()) c->plan_dirty = true;    // with a layer-camera table it takes effect when the table is cleared
+    }
     return MEAO_OK;
+}
+
+int meao_set_layer_cameras(MeaoCtx *c, const MeaoCamera *cams, int32_t count)
+{
+    if (!c) return MEAO_ERR_INVALID;
+    if (!cams && count == 0) {
+        if (c->layer_cams.empty()) return 0;
+        c->layer_cams.clear();
+        c->plan_dirty = true;
+        return 1;
+    }
+    if (!cams) return fail(c, MEAO_ERR_INVALID, "cameras is NULL with count %d (NULL clears the table only with count 0)", count);
+    if (count != c->layers) return fail(c, MEAO_ERR_INVALID, "count %d differs from the context's %d layers (meao_set_layers)", count, c->layers);
+    for (int l = 0; l < count; l++) {
+        const MeaoCamera &k = cams[l];
+        if (!(k.near_clip > 0)) return fail(c, MEAO_ERR_INVALID, "layer %d: bad camera near_clip %g (must be > 0)", l, k.near_clip);
+        if (!(k.far_clip > k.near_clip))
+            return fail(c, MEAO_ERR_INVALID, "layer %d: bad camera far_clip %g (must be > near_clip %g)", l, k.far_clip, k.near_clip);
+        if (!(k.tan_half_fov_h > 0)) return fail(c, MEAO_ERR_INVALID, "layer %d: bad camera tan_half_fov_h %g (must be > 0)", l, k.tan_half_fov_h);
+        if ((k.reversed_z != 0) != (cams[0].reversed_z != 0))
+            return fail(c, MEAO_ERR_INVALID, "layer %d: camera reversed_z %d differs from layer 0's %d (one Z direction for all layers)", l,
+                        k.reversed_z, cams[0].reversed_z);
+    }
+    if ((int)c->layer_cams.size() == count && memcmp(c->layer_cams.data(), cams, (size_t)count * sizeof(MeaoCamera)) == 0) return 0;
+    c->layer_cams.assign(cams, cams + count);
+    c->plan_dirty = true;
+    return 1;
+}
+
+int meao_get_layer_cameras(const MeaoCtx *c, MeaoCamera *out, int32_t capacity)
+{
+    if (!c) return MEAO_ERR_INVALID;
+    const int n = (int)c->layer_cams.size();
+    if (n && (!out || capacity < n)) return MEAO_ERR_INVALID;
+    if (n) memcpy(out, c->layer_cams.data(), (size_t)n * sizeof(MeaoCamera));
+    return n;
 }
 
 int meao_resize(MeaoCtx *c, int32_t w, int32_t h)
@@ -917,7 +1053,10 @@ int meao_set_layers(MeaoCtx *c, int32_t layers)
         return fail(c, MEAO_ERR_INVALID, "layers %d not in 1..%d (the layer is a grid dimension of the layered kernels)", layers, kMaxLayers);
     if (layers == c->layers) return 0;
     const int old = c->layers;
+    std::vector<MeaoCamera> old_cams;
+    old_cams.swap(c->layer_cams);                   // a table has one camera per layer: a new layer count clears it
     c->layers = layers;
+    c->plan_dirty = true;
     if (c->W <= 0) return 1;                        // applied by the first meao_resize
     if (!c->plan_only) {
         CUDA_TRY(c, cudaSetDevice(c->device));
@@ -927,6 +1066,7 @@ int meao_set_layers(MeaoCtx *c, int32_t layers)
     if (rc) {
         const std::string err = c->error;
         c->layers = old;
+        c->layer_cams.swap(old_cams);
         if (allocate(c)) { c->W = c->H = 0; }        // the previous arena could not be restored either: the context needs meao_resize
         c->error = err;
         return rc;
@@ -1639,11 +1779,10 @@ int meao_get_buffer(MeaoCtx *c, int32_t id, void *host_out, size_t host_bytes)
         const int k = id - 5;
         __half *tmp = nullptr;
         CUDA_TRY(c, cudaMalloc(&tmp, need));
-        const float pad = host_f16_round((c->last_kind != MEAO_DEPTH_LINEAR_F32) ? c->plan.pad[k] : 0.0f);
         cudaError_t e = cudaSuccess;
         for (int l = 0; l < c->layers && e == cudaSuccess; l++)
             e = launch_synth_tiled(c->low[k] + (size_t)l * c->lh[k] * c->low_pitch[k], c->lw[k], c->lh[k], c->low_pitch[k], c->lw[k + 2], c->lh[k + 2],
-                                   pad, (__half *)((char *)tmp + l * one), c->stream);
+                                   layer_pad(c, l, k, c->last_kind), (__half *)((char *)tmp + l * one), c->stream);
         if (e == cudaSuccess) e = cudaMemcpyAsync(host_out, tmp, need, cudaMemcpyDeviceToHost, c->stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
         cudaFree(tmp);
@@ -1678,7 +1817,7 @@ int meao_debug_view(MeaoCtx *c, int32_t id, void *out, void *stream)
         const int k = id - 5;
         a.tiled = 1; a.src = c->low[k]; a.elem = 4; a.spitch = c->low_pitch[k];
         a.sw = c->lw[k + 2]; a.sh = c->lh[k + 2]; a.lw = c->lw[k]; a.lh = c->lh[k];
-        a.pad = host_f16_round((c->last_kind != MEAO_DEPTH_LINEAR_F32) ? c->plan.pad[k] : 0.0f);
+        a.pad = layer_pad(c, 0, k, c->last_kind);
     } else {                                                        // AO.cs:815-819
         if (id == MEAO_BUF_AMBIENT_OCCLUSION && c->last_out) {
             // the last frame wrote the AO texture straight into the caller's buffer: regenerate the context's own copy
@@ -1696,6 +1835,7 @@ int meao_debug_view(MeaoCtx *c, int32_t id, void *out, void *stream)
         DebugViewArgs al = a;
         al.src = (const char *)a.src + l * src_layer;
         al.out = a.out + (size_t)l * c->W * c->H;
+        if (slices == 16) al.pad = layer_pad(c, l, id - 5, c->last_kind);     // the layer's camera
         CUDA_TRY(c, launch_debug_view(al, s));
         c->launches++;
     }
@@ -1761,6 +1901,24 @@ int meao_zbuffer_params(MeaoCtx *c, float out[4])
 {
     if (plan_only(c) || !out) return MEAO_ERR_INVALID;
     memcpy(out, c->plan.zb, 16);
+    return MEAO_OK;
+}
+
+int meao_render_constants_layer(MeaoCtx *c, int32_t layer, int32_t level, int32_t wide, float out[28])
+{
+    if (plan_only(c) || !out || level < 1 || level > 4 || layer < 0 || layer >= c->layers) return MEAO_ERR_INVALID;
+    int rc = wide ? meao_render_constants_wide(c, level, out) : meao_render_constants(c, level, out);
+    if (rc) return rc;
+    const CamConsts &cc = c->layer_consts[layer];
+    memcpy(out, wide ? cc.inv_thickness_wide[level] : cc.inv_thickness[level], 48);
+    return MEAO_OK;
+}
+
+int meao_zbuffer_params_layer(MeaoCtx *c, int32_t layer, float out[4])
+{
+    if (plan_only(c) || !out || layer < 0 || layer >= c->layers) return MEAO_ERR_INVALID;
+    const CamConsts &cc = c->layer_consts[layer];
+    out[0] = cc.zb[0]; out[1] = cc.zb[1]; out[2] = out[3] = 0.0f;
     return MEAO_OK;
 }
 

@@ -19,7 +19,8 @@ namespace {
 
 }  // namespace
 
-cudaError_t launch_prepare_depth_array(const PrepareArgs &a_in, cudaSurfaceObject_t depth, int surf_kind, int layers, cudaStream_t s)
+cudaError_t launch_prepare_depth_array(const PrepareArgs &a_in, cudaSurfaceObject_t depth, int surf_kind, int layers, cudaStream_t s,
+                                       const LayerZ *layer_zb)
 {
     if (a_in.row1 <= a_in.row0) return cudaSuccess;
     if (layers < 1 || layers > kMaxLayers || a_in.in_format == IN_D24S8) return cudaErrorInvalidValue;
@@ -28,13 +29,13 @@ cudaError_t launch_prepare_depth_array(const PrepareArgs &a_in, cudaSurfaceObjec
     a.vec_ok = 1;               // the input is read element by element; the intermediates' pitched rows keep the vector stores aligned
     dim3 grid(ceil_div(a.W, kPrepTileW), ceil_div(a.row1 - a.row0, kPrepTileH), layers);
     if (!a.raw) {
-        MEAO_LAUNCH((prepare_depth_array_kernel<false, true, IN_F32>), grid, kPrepThreads, 0, s, a, depth, surf_kind);
+        MEAO_LAUNCH((prepare_depth_array_kernel<false, true, IN_F32>), grid, kPrepThreads, 0, s, a, depth, surf_kind, layer_zb);
     } else if (a.in_format == IN_D16) {
-        if (a.reversed_z) MEAO_LAUNCH((prepare_depth_array_kernel<true, true, IN_D16>), grid, kPrepThreads, 0, s, a, depth, surf_kind);
-        else              MEAO_LAUNCH((prepare_depth_array_kernel<true, false, IN_D16>), grid, kPrepThreads, 0, s, a, depth, surf_kind);
+        if (a.reversed_z) MEAO_LAUNCH((prepare_depth_array_kernel<true, true, IN_D16>), grid, kPrepThreads, 0, s, a, depth, surf_kind, layer_zb);
+        else              MEAO_LAUNCH((prepare_depth_array_kernel<true, false, IN_D16>), grid, kPrepThreads, 0, s, a, depth, surf_kind, layer_zb);
     } else {
-        if (a.reversed_z) MEAO_LAUNCH((prepare_depth_array_kernel<true, true, IN_F32>), grid, kPrepThreads, 0, s, a, depth, surf_kind);
-        else              MEAO_LAUNCH((prepare_depth_array_kernel<true, false, IN_F32>), grid, kPrepThreads, 0, s, a, depth, surf_kind);
+        if (a.reversed_z) MEAO_LAUNCH((prepare_depth_array_kernel<true, true, IN_F32>), grid, kPrepThreads, 0, s, a, depth, surf_kind, layer_zb);
+        else              MEAO_LAUNCH((prepare_depth_array_kernel<true, false, IN_F32>), grid, kPrepThreads, 0, s, a, depth, surf_kind, layer_zb);
     }
     return cudaGetLastError();
 }

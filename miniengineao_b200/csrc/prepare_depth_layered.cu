@@ -15,7 +15,7 @@ namespace {
 
 }  // namespace
 
-cudaError_t launch_prepare_depth_layered(const PrepareArgs &a_in, int layers, cudaStream_t s, bool low_only)
+cudaError_t launch_prepare_depth_layered(const PrepareArgs &a_in, int layers, cudaStream_t s, bool low_only, const LayerZ *layer_zb)
 {
     if (a_in.row1 <= a_in.row0) return cudaSuccess;
     const PrepareArgs a = resolve_pitches(a_in);
@@ -23,16 +23,16 @@ cudaError_t launch_prepare_depth_layered(const PrepareArgs &a_in, int layers, cu
     dim3 grid(ceil_div(a.W, kPrepTileW), ceil_div(a.row1 - a.row0, low_only ? kPrepLowTileH : kPrepTileH), layers);
 #define MEAO_PREP_K(...) (low_only ? prepare_depth_low_layered_kernel<__VA_ARGS__> : prepare_depth_layered_kernel<__VA_ARGS__>)
     if (!a.raw) {
-        MEAO_LAUNCH((MEAO_PREP_K(false, true, IN_F32)), grid, kPrepThreads, 0, s, a);
+        MEAO_LAUNCH((MEAO_PREP_K(false, true, IN_F32)), grid, kPrepThreads, 0, s, a, layer_zb);
     } else if (a.in_format == IN_D16) {
-        if (a.reversed_z) MEAO_LAUNCH((MEAO_PREP_K(true, true, IN_D16)), grid, kPrepThreads, 0, s, a);
-        else              MEAO_LAUNCH((MEAO_PREP_K(true, false, IN_D16)), grid, kPrepThreads, 0, s, a);
+        if (a.reversed_z) MEAO_LAUNCH((MEAO_PREP_K(true, true, IN_D16)), grid, kPrepThreads, 0, s, a, layer_zb);
+        else              MEAO_LAUNCH((MEAO_PREP_K(true, false, IN_D16)), grid, kPrepThreads, 0, s, a, layer_zb);
     } else if (a.in_format == IN_D24S8) {
-        if (a.reversed_z) MEAO_LAUNCH((MEAO_PREP_K(true, true, IN_D24S8)), grid, kPrepThreads, 0, s, a);
-        else              MEAO_LAUNCH((MEAO_PREP_K(true, false, IN_D24S8)), grid, kPrepThreads, 0, s, a);
+        if (a.reversed_z) MEAO_LAUNCH((MEAO_PREP_K(true, true, IN_D24S8)), grid, kPrepThreads, 0, s, a, layer_zb);
+        else              MEAO_LAUNCH((MEAO_PREP_K(true, false, IN_D24S8)), grid, kPrepThreads, 0, s, a, layer_zb);
     } else {
-        if (a.reversed_z) MEAO_LAUNCH((MEAO_PREP_K(true, true, IN_F32)), grid, kPrepThreads, 0, s, a);
-        else              MEAO_LAUNCH((MEAO_PREP_K(true, false, IN_F32)), grid, kPrepThreads, 0, s, a);
+        if (a.reversed_z) MEAO_LAUNCH((MEAO_PREP_K(true, true, IN_F32)), grid, kPrepThreads, 0, s, a, layer_zb);
+        else              MEAO_LAUNCH((MEAO_PREP_K(true, false, IN_F32)), grid, kPrepThreads, 0, s, a, layer_zb);
     }
 #undef MEAO_PREP_K
     return cudaGetLastError();
