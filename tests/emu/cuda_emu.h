@@ -6,9 +6,10 @@
 // against the oracle without a GPU.  It is never built into, linked with or loaded by libmeao.so: the product has no CPU
 // path (include/meao.h), and nothing outside tests/ may use this directory.
 //
-// What is and is not emulated: fp32 arithmetic is IEEE on both sides, so results are bit-comparable; MUFU.RCP is replaced
-// by the correctly rounded reciprocal (the refinement steps that follow make the quotient exact from any start within an
-// ulp or two -- on the GPU that is what meao_selftest_div proves for the real MUFU); TMA box loads are emulated as synchronous copies with
+// What is and is not emulated: fp32 arithmetic is IEEE on both sides, so results are bit-comparable; MUFU.RCP keeps the
+// flush-to-zero behaviour of rcp.approx.ftz.f32 but returns the correctly rounded reciprocal in between (the refinement steps
+// that follow make the quotient exact from any start within an ulp or two -- on the GPU tests/test_fast_div_exhaustive_gpu.py
+// checks that for the real MUFU on every in-range operand); TMA box loads are emulated as synchronous copies with
 // zero fill (mbarriers become no-ops), so both the TMA path and the gather path of every kernel can be run; timing, occupancy and memory behaviour mean nothing here.
 #pragma once
 
@@ -86,7 +87,16 @@ using std::max;
 using std::min;
 
 namespace meao_emu {
-inline float rcp_approx(float x) { return (float)(1.0 / (double)x); }
+// rcp.approx.ftz.f32 (PTX ISA): a subnormal operand counts as a zero of its sign (so its reciprocal is +-inf), a subnormal
+// result flushes to a zero of its sign, +-inf -> +-0 and NaN -> NaN.  Between those edges the result here is correctly rounded;
+// the hardware's approximation error is not modelled -- the exhaustive fast-division test checks it on the GPU.  So a range
+// guard that lets a subnormal, zero or infinite operand into a fast path gives wrong results here as it does on the H100.
+inline float rcp_approx(float x)
+{
+    if (std::fpclassify(x) == FP_SUBNORMAL) x = std::copysign(0.0f, x);
+    const float r = (float)(1.0 / (double)x);
+    return std::fpclassify(r) == FP_SUBNORMAL ? std::copysign(0.0f, r) : r;
+}
 // cp.async.bulk.tensor.2d (tiled, no swizzle): box whose first element is (x, y); out-of-bounds elements are zero-filled.
 // Synchronous here: the issuing fiber (thread 0) runs before the others in every barrier phase, so the data is in place
 // when they pass the (no-op) mbarrier wait.  Like the hardware, refuse a start coordinate that is not 16-byte aligned

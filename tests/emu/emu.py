@@ -55,6 +55,13 @@ def _aligned(a: np.ndarray) -> np.ndarray:
     return out
 
 
+def linearize_zero(zb) -> float:
+    """Linearize(0) of a standard-Z camera, the value of the padding texels (DS1:40): 1 / fma(zbx, 0, zby), as libmeao forms it --
+    NaN when zbx is infinite (far / near overflowed f32), not 1 / zby."""
+    with np.errstate(invalid="ignore", divide="ignore"):
+        return float(np.float32(1) / (np.float32(zb[0]) * np.float32(0) + np.float32(zb[1])))
+
+
 class EmulatedFrame:
     """One frame through the host-compiled kernels, planned by a plan-only libmeao context (device = -1)."""
 
@@ -79,7 +86,7 @@ class EmulatedFrame:
         if linear:
             pad12 = 0.0
         else:       # Linearize(OOB load = 0): DS1:40-45
-            pad12 = 1e5 if rz else float(np.float32(1) / np.float32(zb[1]))
+            pad12 = 1e5 if rz else linearize_zero(zb)
         self._h = self._lib.emu_create(self.W, self.H)
         self._lib.emu_set_tma(self._h, int(use_tma))
         self._lib.emu_set_render_tile(self._h, int(render_tile))       # -1: the planner's rule; 0 / 1 / 2: force 64x32 / 64x16 / 64x8 tiles

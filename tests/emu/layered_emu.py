@@ -11,6 +11,7 @@ import numpy as np
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 import build_layered_emu  # noqa: E402
+from emu.emu import linearize_zero  # noqa: E402
 
 _lib: C.CDLL | None = None
 
@@ -39,6 +40,7 @@ def lib() -> C.CDLL:
     return _lib
 
 
+
 class LayeredFrame:
     """One layered frame through the host-compiled layered kernels, planned by a plan-only libmeao context (device = -1) whose
     `layers` property gives the layer count."""
@@ -59,7 +61,7 @@ class LayeredFrame:
             N.check(plan._ctx, nl.meao_upsample_constants(plan._ctx, k, C.cast(C.byref(uc, 32 * (k - 1)), C.POINTER(C.c_float))))
         N.check(plan._ctx, nl.meao_zbuffer_params(plan._ctx, zb))
         rz = bool(plan.camera.usesReversedZBuffer)
-        pad12 = 0.0 if linear else (1e5 if rz else float(np.float32(1) / np.float32(zb[1])))     # Linearize(OOB load = 0): DS1:40-45
+        pad12 = 0.0 if linear else (1e5 if rz else linearize_zero(zb))     # Linearize(OOB load = 0): DS1:40-45
         self._h = self._lib.lemu_create(self.W, self.H, self.layers)
         self._lib.lemu_set_constants(self._h, rc, rcw, uc, zb, pad12, int(not linear), int(rz), int(plan.highQualityMask),
                                      int(plan.sampleExhaustively), int(plan.singleScale), int(use_tma))

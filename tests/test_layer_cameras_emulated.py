@@ -19,6 +19,7 @@ from miniengineao_b200 import AmbientOcclusion, Camera, MeaoError
 from miniengineao_b200 import _native as N
 from oracle.oracle import Oracle
 
+from emu.emu import linearize_zero
 from test_layers_emulated import _raw, contrasting_layers
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -100,7 +101,7 @@ class CamFrame:
                 for wide, buf in ((0, lrc), (1, lrcw)):
                     N.check(ctx, nl.meao_render_constants_layer(ctx, l, k, wide, C.cast(C.byref(buf, 112 * (k - 1)), C.POINTER(C.c_float))))
             N.check(ctx, nl.meao_zbuffer_params_layer(ctx, l, lzb))
-            pad12 = 0.0 if linear else (1e5 if rz else float(np.float32(1) / np.float32(lzb[1])))     # Linearize(OOB load = 0)
+            pad12 = 0.0 if linear else (1e5 if rz else linearize_zero(lzb))     # Linearize(OOB load = 0)
             self._lib.lcemu_set_layer(self._h, l, lrc, lrcw, lzb, pad12)
         self._fused = int(fused)
         self._lib.lcemu_set_views(self._h, self._fused, 0, 0, None, 0, 0)

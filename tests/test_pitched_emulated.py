@@ -21,6 +21,7 @@ from miniengineao_b200 import _native as N
 from oracle.oracle import Oracle
 
 from emu import build_pitched_emu  # noqa: E402  (tests/ is on sys.path via conftest)
+from emu.emu import linearize_zero
 from test_fused_lin_emulated import _ingest, _raw_with_sky
 from test_layers_emulated import _compare_layer, _plan, contrasting_layers
 from miniengineao_b200 import synth
@@ -95,7 +96,7 @@ class PitchedFrame:
             N.check(plan._ctx, nl.meao_upsample_constants(plan._ctx, k, C.cast(C.byref(uc, 32 * (k - 1)), C.POINTER(C.c_float))))
         N.check(plan._ctx, nl.meao_zbuffer_params(plan._ctx, zb))
         rz = bool(plan.camera.usesReversedZBuffer)
-        pad12 = 0.0 if linear else (1e5 if rz else float(np.float32(1) / np.float32(zb[1])))
+        pad12 = 0.0 if linear else (1e5 if rz else linearize_zero(zb))
         self._h = self._lib.lemu_create(self.W, self.H, self.layers)
         self._lib.lemu_set_constants(self._h, rc, rcw, uc, zb, pad12, int(not linear), int(rz), int(plan.highQualityMask),
                                      int(plan.sampleExhaustively), int(plan.singleScale), 1)
