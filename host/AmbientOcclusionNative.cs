@@ -52,6 +52,16 @@ namespace MiniEngineAO
         [DllImport(Lib)] public static extern int meao_set_variants(IntPtr ctx, ref MeaoVariants v);
         [DllImport(Lib)] public static extern int meao_set_camera(IntPtr ctx, ref MeaoCamera c);
         [DllImport(Lib)] public static extern int meao_resize(IntPtr ctx, int width, int height);
+        // Dynamic resolution: what meao_reservation reports (meao.h MeaoReservation)
+        [StructLayout(LayoutKind.Sequential)]
+        public struct MeaoReservation
+        {
+            public int width, height;
+            public long arena_bytes, arena_bytes_needed, arena_allocations, graphs_held, graph_instantiations;
+        }
+        // lay the intermediates out once for the largest size; a resize inside it then allocates and synchronises nothing (0, 0 clears)
+        [DllImport(Lib)] public static extern int meao_reserve(IntPtr ctx, int maxWidth, int maxHeight);
+        [DllImport(Lib)] public static extern int meao_reservation(IntPtr ctx, out MeaoReservation r);
         [DllImport(Lib)] public static extern int meao_set_layers(IntPtr ctx, int layers);   // layered frames: L views per frame, [L][H][W] buffers
         // one camera per layer (split-screen viewports, mirrors, batches from several cameras); null with count 0 clears the table
         [DllImport(Lib)] public static extern int meao_set_layer_cameras(IntPtr ctx, [In] MeaoCamera[] cameras, int count);
@@ -118,6 +128,12 @@ namespace MiniEngineAO
         // renders with this component's camera.  Each must have this camera's pixel size; Length must equal Layers.
         Camera[] _layerCameras;
         public Camera[] LayerCameras { get { return _layerCameras; } set { _layerCameras = value; } }
+        // Dynamic resolution scaling: the largest camera pixel size the render size moves within (zero: none).  Reserved once
+        // (meao_reserve); a size change inside it then costs no allocation, device synchronise, graph teardown or event rebind.
+        Vector2Int _maxResolution;
+        public Vector2Int MaxResolution { get { return _maxResolution; } set { _maxResolution = value; } }
+        int _reservedW, _reservedH;                            // what meao_reserve was last given (doubled width under single-pass stereo)
+        int _width, _height;                                   // the size meao_resize was last given
         int _drawCountPerFrame;                                // AmbientOcclusion.cs:289, 349-355: single-pass stereo detection
         void OnPreRender() { _drawCountPerFrame++; }
         bool singlePassStereoEnabled                           // AmbientOcclusion.cs:392-401
@@ -182,11 +198,34 @@ namespace MiniEngineAO
             MeaoNative.Check(_ctx, layered);
             rebuild |= layered == 1;
             rebuild |= SetLayerCameras() == 1;                                               // after meao_set_layers, which clears the table
-            rebuild |= MeaoNative.meao_resize(_ctx, _camera.pixelWidth * (stereo ? 2 : 1), _camera.pixelHeight) == 1;   // :338-341
+            var width = _camera.pixelWidth * (stereo ? 2 : 1);
+            rebuild |= Reserve(width, _camera.pixelHeight, stereo);                          // before meao_resize, doubled like the width
+            var resized = MeaoNative.meao_resize(_ctx, width, _camera.pixelHeight);          // :338-341
+            MeaoNative.Check(_ctx, resized);
+            rebuild |= resized == 1 && _reservedW == 0;     // inside a reservation the bound event renders the new size as it is
+            _width = width; _height = _camera.pixelHeight;
             rebuild |= !Application.isPlaying;                                               // :345
             _drawCountPerFrame = 0;                                                          // :349
 
             if (rebuild || _renderCommand == null) RebuildCommandBuffers();
+        }
+
+        // Hands MaxResolution to meao_reserve; true if the arena was re-allocated.  When the current size does not fit the new
+        // reservation, the context first drops its reservation and takes the new size (meao_reserve refuses a reservation below it).
+        bool Reserve(int width, int height, bool stereo)
+        {
+            int w = _maxResolution.x * (stereo ? 2 : 1), h = _maxResolution.y;
+            if (_maxResolution.x <= 0 || _maxResolution.y <= 0) w = h = 0;
+            if (w == _reservedW && h == _reservedH) return false;
+            if (w != 0 && (_width > w || _height > h))
+            {
+                MeaoNative.Check(_ctx, MeaoNative.meao_reserve(_ctx, 0, 0));
+                _reservedW = _reservedH = 0;
+                MeaoNative.Check(_ctx, MeaoNative.meao_resize(_ctx, width, height));
+            }
+            MeaoNative.Check(_ctx, MeaoNative.meao_reserve(_ctx, w, h));
+            _reservedW = w; _reservedH = h;
+            return true;
         }
 
         // Hands LayerCameras to the plugin; returns 1 if it re-planned.  The same table again returns 0, so this runs every frame.

@@ -35,7 +35,8 @@ extern "C" {
                               *      meao_bind_event takes the stream
                               *    + meao_set_layers (layered frames; additive, so the version stays 3)
                               *    + meao_render_arrays / meao_bind_event_arrays / meao_release_array (CUDA-array I/O; additive)
-                              *    + meao_render_pitched / meao_bind_event_pitched (depth and AO with their own row and layer pitch; additive) */
+                              *    + meao_render_pitched / meao_bind_event_pitched (depth and AO with their own row and layer pitch; additive)
+                              *    + meao_reserve / meao_reservation (dynamic resolution; additive) */
 
 typedef struct MeaoCtx MeaoCtx;
 
@@ -147,6 +148,42 @@ int meao_set_camera(MeaoCtx *ctx, const MeaoCamera *camera);
  * A size change RESETS the row band to the whole frame and drops the neighbour connections (meao_set_row_band,
  * meao_band_connect): a band host must set its band again after every call that returned 1. */
 int meao_resize(MeaoCtx *ctx, int32_t width, int32_t height);
+/* ---- dynamic resolution ------------------------------------------------------------------------------------------------------
+ * meao_reserve lays the intermediates out ONCE for max_width x max_height at the context's layer count, so that meao_resize to any
+ * size inside the reservation is host bookkeeping: no allocation, free or memset, no stream or device synchronise, no graph
+ * destruction.  Every planned size keeps its plan, TMA maps and captured graphs: a return to a size used recently (the last 8,
+ * MEAO_SIZE_SLOTS) is a plain graph replay; a new size is planned on the host, its per-layer camera tables are written in stream order
+ * by its first frame, and its graph is captured and, once the graph cache is full, re-targets the least recently used executable graph.
+ * At most MEAO_MAX_GRAPHS_HELD executable graphs are alive at any time (MeaoReservation.graphs_held), whatever sizes a host visits.
+ *   - Returns 1 when the reservation changed (the arena was re-allocated: a synchronising plan change like a resize without one), 0
+ *     when the same reservation is set again.  Bounds as meao_resize (1..32768).  (0, 0) clears the reservation: the arena is then
+ *     re-allocated at the current size.
+ *   - Refused with MEAO_ERR_INVALID if the reservation is below the current size (meao_last_error names the dimension);
+ *     MEAO_ERR_NOMEM leaves the previous reservation and arena in place.
+ *   - meao_resize on a reserved context returns 1 when the size changed, as always; a size outside the reservation is refused with
+ *     MEAO_ERR_INVALID and changes nothing -- a dynamic-resolution host never gets a silent re-allocation.
+ *   - meao_set_layers re-allocates at the reservation x the new layer count.  A change of MeaoParams, MeaoVariants or a camera
+ *     re-plans with a device synchronise, as without a reservation, and forgets the other planned sizes; the arena stays.
+ *   - Row bands and reservations exclude each other: meao_reserve on a context with a row band, and meao_set_row_band, the halo calls
+ *     and the native exchange on a reserved context, return MEAO_ERR_UNSUPPORTED.
+ *   - After a size change the intermediates (meao_get_buffer, meao_debug_view) describe the new size; their contents are unspecified
+ *     until the first frame at that size (a fresh arena is zeroed; a reserved one holds whatever earlier sizes left there).
+ *   - Works on plan-only contexts (device < 0): the reservation is recorded and nothing is allocated.
+ * ORDERING CONTRACT (every context, reserved or not): the frames of one context run in the order they are issued -- they share the
+ * context's intermediates (and, reserved, its camera table slots).  Frames issued on one stream are ordered by it; a host that
+ * issues consecutive frames of one context on different streams orders them itself (an event, as meao_render_host_async does). */
+#define MEAO_SIZE_SLOTS 8
+#define MEAO_MAX_GRAPHS_HELD 72
+int meao_reserve(MeaoCtx *ctx, int32_t max_width, int32_t max_height);
+typedef struct {
+    int32_t width, height;              /* the reservation; 0 x 0 = none */
+    int64_t arena_bytes;                /* bytes of the arena (plan-only contexts: what it would allocate) */
+    int64_t arena_bytes_needed;         /* bytes the current size's layout needs (<= arena_bytes) */
+    int64_t arena_allocations;          /* arenas allocated since meao_create */
+    int64_t graphs_held;                /* executable graphs alive, retired ones waiting for their last launch included */
+    int64_t graph_instantiations;       /* cudaGraphInstantiate calls since meao_create */
+} MeaoReservation;
+int meao_reservation(const MeaoCtx *ctx, MeaoReservation *out);
 /* Layered frames: every frame holds `layers` independent views of width x height (texture-array stereo: 2 eye slices; cube-map
  * AO: 6 faces; a batch of frames of one camera), rendered by ONE launch per stage.  Each layer's result is bit-identical to
  * rendering that layer alone; one MeaoParams / MeaoCamera / MeaoVariants applies to all layers unless meao_set_layer_cameras gives

@@ -44,6 +44,15 @@ class MeaoBufferDesc(C.Structure):
     _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("slices", C.c_int32), ("elem_bytes", C.c_int32)]
 
 
+MEAO_SIZE_SLOTS = 8
+MEAO_MAX_GRAPHS_HELD = 72
+
+
+class MeaoReservation(C.Structure):
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("arena_bytes", C.c_int64), ("arena_bytes_needed", C.c_int64),
+                ("arena_allocations", C.c_int64), ("graphs_held", C.c_int64), ("graph_instantiations", C.c_int64)]
+
+
 RENDER_EVENT_FUNC = C.CFUNCTYPE(None, C.c_int)
 
 # name -> (restype, argtypes); every symbol include/meao.h declares
@@ -59,6 +68,8 @@ SIGNATURES = {
     "meao_get_variants": (C.c_int, [C.c_void_p, C.POINTER(MeaoVariants)]),
     "meao_set_camera": (C.c_int, [C.c_void_p, C.POINTER(MeaoCamera)]),
     "meao_resize": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
+    "meao_reserve": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
+    "meao_reservation": (C.c_int, [C.c_void_p, C.POINTER(MeaoReservation)]),
     "meao_set_layers": (C.c_int, [C.c_void_p, C.c_int32]),
     "meao_set_layer_cameras": (C.c_int, [C.c_void_p, C.POINTER(MeaoCamera), C.c_int32]),
     "meao_get_layer_cameras": (C.c_int, [C.c_void_p, C.POINTER(MeaoCamera), C.c_int32]),

@@ -84,6 +84,10 @@ class AmbientOcclusion:
         # one Camera per layer (meao_set_layer_cameras): split-screen viewports, mirrors, batches from several cameras; None = every
         # layer uses `camera`.  Each entry must match the main camera's pixelWidth, pixelHeight and usesReversedZBuffer.
         self.layerCameras: list[Camera] | None = None
+        # dynamic resolution: the largest (pixelWidth, pixelHeight) the camera will have, reserved once (meao_reserve) so that a size
+        # change inside it costs no allocation, device synchronise or graph teardown; None = every size change re-allocates
+        self.maxResolution: tuple[int, int] | None = None
+        self._reserved = (0, 0)             # what meao_reserve was last given (doubled width under single-pass stereo)
         self._band = None                   # (row0, row1) after set_row_band; reset by every re-allocation
         self._drawCountPerFrame = 0         # AO.cs:289: used to detect single-pass stereo
         self._stereo = False                # singlePassStereoEnabled as latched by the last LateUpdate
@@ -150,16 +154,41 @@ class AmbientOcclusion:
         width = cam.pixelWidth * (2 if stereo else 1)                                                # AO.cs:338-341, 501-504
         layered = self._check(self._lib.meao_set_layers(self._ctx, int(self.layers))) == 1           # re-allocates like a resize
         rebuild |= self._apply_layer_cameras()
+        reallocated = layered | self._apply_reservation(width, cam.pixelHeight, stereo)
         resized = self._check(self._lib.meao_resize(self._ctx, width, cam.pixelHeight)) == 1          # CheckBaseDimensions
-        resized |= layered
+        reallocated |= resized and self._reserved == (0, 0)       # inside a reservation a resize allocates nothing
+        resized |= reallocated
         self._width, self._height = width, cam.pixelHeight
-        if resized:
-            self._band = None       # meao_resize re-allocates: the C context is back to the whole frame and has dropped its neighbours
+        if reallocated:
+            self._band = None       # a re-allocation puts the C context back to the whole frame and drops its neighbours
         if rebuild or resized:
             self.rebuild_count += 1
         if frame:
             self._drawCountPerFrame = 0                                                              # AO.cs:349
         return rebuild or resized
+
+    def _apply_reservation(self, width: int, height: int, stereo: bool) -> bool:
+        """Hands maxResolution to meao_reserve before the frame's meao_resize (width doubled under single-pass stereo, like the size);
+        True if the arena was re-allocated.  When the context's current size does not fit the new reservation, the context first
+        drops its reservation and takes the new size, so that meao_reserve never sees a reservation below the current size."""
+        mr = self.maxResolution
+        want = (0, 0) if mr is None else (int(mr[0]) * (2 if stereo else 1), int(mr[1]))
+        if want == self._reserved:
+            return False
+        if want != (0, 0) and (self._width > want[0] or self._height > want[1]):
+            self._check(self._lib.meao_reserve(self._ctx, 0, 0))
+            self._reserved = (0, 0)
+            self._check(self._lib.meao_resize(self._ctx, width, height))
+        self._check(self._lib.meao_reserve(self._ctx, *want))
+        self._reserved = want
+        return True
+
+    def reservation(self) -> dict:
+        """meao_reservation: the reserved size, the arena's bytes and the bytes the current size needs, arenas allocated, executable
+        graphs held and graph instantiations since the context was created."""
+        r = N.MeaoReservation()
+        self._check(self._lib.meao_reservation(self._ctx, C.byref(r)))
+        return {f: getattr(r, f) for f, _ in N.MeaoReservation._fields_}
 
     def _apply_layer_cameras(self) -> bool:
         """Hands layerCameras to meao_set_layer_cameras (after meao_set_layers, which clears the table); True if it re-planned."""

@@ -17,7 +17,7 @@ SOURCES = ["meao_api.cu", "prepare_depth.cu", "render_ao.cu", "blur_upsample.cu"
            "prepare_depth_layered.cu", "render_ao_layered.cu", "blur_upsample_layered.cu", "prepare_depth_array.cu", "blur_upsample_array.cu",
            "blur_upsample_lin.cu"]
 HEADERS = ["common.cuh", "kernels.h", "prepare_depth_kernel.inc", "render_ao_kernel.inc", "blur_upsample_device.inc", "blur_upsample_kernel.inc",
-           "blur_upsample_layer_args.inc", "surface_io.cuh", "depth_in.cuh",
+           "blur_upsample_layer_args.inc", "surface_io.cuh", "depth_in.cuh", "arena_layout.h",
            os.path.join("..", "..", "include", "meao.h")]
 
 NVCC_FLAGS = [

@@ -24,6 +24,7 @@
 #include "../../include/meao.h"
 #include "common.cuh"
 #include "kernels.h"
+#include "arena_layout.h"
 
 using namespace meao;
 
@@ -33,7 +34,6 @@ thread_local std::string g_create_error;
 
 struct Range { int lo, hi; };   // [lo, hi)
 inline Range clampr(Range r, int n) { Range o{r.lo < 0 ? 0 : r.lo, r.hi > n ? n : r.hi}; if (o.hi < o.lo) o.hi = o.lo; return o; }
-inline int align_up(int x, int a) { return (x + a - 1) / a * a; }
 
 // cuTensorMapEncodeTiled is fetched through the runtime so libmeao.so has no link-time
 // dependency on libcuda (it must load on a machine without a driver for the ABI tests).
@@ -65,9 +65,50 @@ struct CamConsts {
     float pad[5];
 };
 
+// Everything of a context that depends on the frame size: the geometry, where the buffers of that size sit in the arena, the TMA maps,
+// the row ranges, the plan and the per-layer camera table slot.  A reserved context (meao_reserve) keeps one of these per recently used
+// size (MeaoCtx::size_slots) and swaps it in on a resize to that size, so a return to a planned size is host bookkeeping only.
+struct SizeState {
+    int W = 0, H = 0;
+    int lw[7] = {0}, lh[7] = {0};
+    // band (global L0 rows) + neighbours
+    int band0 = 0, band1 = 0, prev0 = -1, next1 = -1;
+
+    // device buffers (natural layout, pitched, global coordinates): arena_layout(W, H, layers)
+    __half *lin = nullptr; int lin_pitch = 0;
+    float *low[5] = {nullptr}; int low_pitch[5] = {0};
+    uint8_t *occ[5] = {nullptr}; int occ_pitch[5] = {0};
+    uint8_t *comb[4] = {nullptr};           // same pitch as occ of that level
+    uint8_t *hq[5] = {nullptr};             // HighQuality<k> (kernel "main" output), same pitch as occ of that level
+    uint8_t *result = nullptr; int result_pitch = 0;
+
+    bool tma_ok = false;
+    CUtensorMap map_low_ren[kRenderTileVariants][5];    // LowDepth<k> with the render box of tile height kRenderTileHs[t]
+    CUtensorMap map_low_ups[5];             // LowDepth<k> with the upsample depth box
+    CUtensorMap map_ao_ups[5];              // lo AO of upsample lo level k (Occlusion4 / Combined k)
+    CUtensorMap map_low_wide[kRenderTileVariants][5];   // LowDepth<k> with the wide-render box
+    CUtensorMap map_hq_ups[5];              // HighQuality<k> as LoResAO2 of upsample lo level k
+    CUtensorMap map_occ1_ups;               // Occlusion1 as LoResAO1 of the final upsample (MeaoVariants.single_scale)
+
+    // row ranges (per level) for this band
+    Range need_c[5];                        // rows of Occlusion<k>/Combined<k> to produce (k=1..4); [0] = final rows
+    Range need_low[5];                      // rows of LowDepth<k> required
+    Range own_low[5];                       // rows of LowDepth<k> this band produces
+
+    Plan plan;
+    std::vector<CamConsts> layer_consts;    // the plan's camera constants of every layer (all alike without a layer-camera table)
+    bool cam_table_stale = true;            // layer_consts changed since the device tables were written (ensure_ready uploads them)
+    // the per-layer camera tables of this size in arena slot `slot` (kernels.h LayerZ / LayerRender): layer_zb[l];
+    // layer_ren[(2 (k - 1) + wide) L + l]
+    int slot = 0;
+    LayerZ *layer_zb = nullptr;
+    LayerRender *layer_ren = nullptr;
+    bool table_pending = false;             // the slot's tables are not written yet: the next frame writes them on its own stream
+};
+
 }  // namespace
 
-struct MeaoCtx {
+struct MeaoCtx : SizeState {
     int device = 0;
     int sm_count = 132;                     // SMs of the device (set by meao_create; 132 = H100 SXM for plan-only contexts)
     bool plan_only = false;                 // device < 0: host-side planning only (no CUDA calls at all)
@@ -83,41 +124,27 @@ struct MeaoCtx {
     std::vector<MeaoCamera> layer_cams;     // meao_set_layer_cameras: one camera per layer, or empty (every layer uses `camera`)
     MeaoVariants variants = {0, 0, 0, 0};
     bool plan_dirty = true;
-    Plan plan;
-    std::vector<CamConsts> layer_consts;    // the plan's camera constants of every layer (all alike without a layer-camera table)
-    bool cam_table_stale = true;            // layer_consts changed since the device tables were written (ensure_ready uploads them)
 
-    int W = 0, H = 0;
-    int lw[7] = {0}, lh[7] = {0};
     int layers = 1;                         // meao_set_layers: every image holds `layers` same-size views stacked at a stride of one image
-    // band (global L0 rows) + neighbours
-    int band0 = 0, band1 = 0, prev0 = -1, next1 = -1;
 
-    // device buffers (natural layout, pitched, global coordinates)
+    // meao_reserve: the arena is laid out for res_w x res_h (0 x 0: for the current size) and every size inside it keeps its plan
+    int res_w = 0, res_h = 0;
+    struct SizeSlot { bool valid = false; uint64_t last_use = 0; SizeState s; };
+    SizeSlot size_slots[kSizeSlots];        // slot i: the parked state of a planned size whose camera tables live in arena slot i
+    uint64_t size_clock = 0;
+    int64_t arena_allocations = 0, graph_instantiations = 0;
+
     void *arena = nullptr;
     size_t arena_bytes = 0;
-    __half *lin = nullptr; int lin_pitch = 0;
-    float *low[5] = {nullptr}; int low_pitch[5] = {0};
-    uint8_t *occ[5] = {nullptr}; int occ_pitch[5] = {0};
-    uint8_t *comb[4] = {nullptr};           // same pitch as occ of that level
-    uint8_t *hq[5] = {nullptr};             // HighQuality<k> (kernel "main" output), same pitch as occ of that level
-    uint8_t *result = nullptr; int result_pitch = 0;
     // staging for the host path: two slots so that the H2D copy of frame i+1 overlaps the kernels and the
-    // D2H copy of frame i (meao_render_host_async)
+    // D2H copy of frame i (meao_render_host_async).  At the offsets of the arena's own size (the reservation's when reserved), so no
+    // size's intermediates ever share bytes with them.
     float *depth_stage[2] = {nullptr, nullptr};     // device, layers*W*H each
     uint8_t *ao_stage[2] = {nullptr, nullptr};      // device, layers*W*H each
     cudaStream_t slot_stream[2] = {nullptr, nullptr};
     cudaEvent_t slot_done[2] = {nullptr, nullptr};
     cudaEvent_t compute_done = nullptr;
     bool compute_done_valid = false;
-
-    bool tma_ok = false;
-    CUtensorMap map_low_ren[kRenderTileVariants][5];    // LowDepth<k> with the render box of tile height kRenderTileHs[t]
-    CUtensorMap map_low_ups[5];             // LowDepth<k> with the upsample depth box
-    CUtensorMap map_ao_ups[5];              // lo AO of upsample lo level k (Occlusion4 / Combined k)
-    CUtensorMap map_low_wide[kRenderTileVariants][5];   // LowDepth<k> with the wide-render box
-    CUtensorMap map_hq_ups[5];              // HighQuality<k> as LoResAO2 of upsample lo level k
-    CUtensorMap map_occ1_ups;               // Occlusion1 as LoResAO1 of the final upsample (MeaoVariants.single_scale)
 
     // native neighbour exchange (meao_band_export / _connect / _step)
     BandFlags *band_flags = nullptr;        // first 256 bytes of the arena
@@ -129,11 +156,6 @@ struct MeaoCtx {
     uint32_t *host_error_dev = nullptr;     // device alias of host_error
     int pdl_level = -1;                     // programmatic dependent launch in the captured graphs: -1 untried, 0 none, 1 plain chains, 2 all same-stream edges
 
-    // row ranges (per level) for this band
-    Range need_c[5];                        // rows of Occlusion<k>/Combined<k> to produce (k=1..4); [0] = final rows
-    Range need_low[5];                      // rows of LowDepth<k> required
-    Range own_low[5];                       // rows of LowDepth<k> this band produces
-
     int64_t launches = 0;
 
     // CUDA graph cache: one instantiated graph per (depth, out, kind), LRU; when it is full the least recently used
@@ -143,14 +165,21 @@ struct MeaoCtx {
     // cudaArray_t handles, so a pointer equal to a handle value never finds an array frame's graph, nor the reverse).
     // pitch: the byte pitches of a pointer frame's depth and AO views (meao_render_pitched; 0 for the other kinds) -- a frame at the
     // same pointers with other pitches is another graph, never a replay that reads the wrong rows.
-    struct GraphKey { const void *p[4]; int kind; int64_t pitch[4] = {0, 0, 0, 0}; bool operator<(const GraphKey &o) const {
+    // size: the frame size and camera table slot the graph was captured at (launch_cached fills it in) -- a reserved context keeps the
+    // graphs of every size it has visited, and a size re-planned into another slot never replays a graph that reads the old slot.
+    struct GraphKey { const void *p[4]; int kind; int64_t pitch[4] = {0, 0, 0, 0}; int size[3] = {0, 0, 0}; bool operator<(const GraphKey &o) const {
         for (int i = 0; i < 4; i++) if (p[i] != o.p[i]) return p[i] < o.p[i];
         if (kind != o.kind) return kind < o.kind;
         for (int i = 0; i < 4; i++) if (pitch[i] != o.pitch[i]) return pitch[i] < o.pitch[i];
+        for (int i = 0; i < 3; i++) if (size[i] != o.size[i]) return size[i] < o.size[i];
         return false; } };
     struct GraphEntry { cudaGraphExec_t exec; uint64_t last_use; };
     std::map<GraphKey, GraphEntry> graphs;
-    std::vector<cudaGraphExec_t> retired;   // executable graphs replaced while possibly in flight: destroyed at the next drop_graph
+    // executable graphs that cudaGraphExecUpdate could not re-target while they were possibly in flight; `done` is recorded after the
+    // frame that replaced them, so once it has completed (and, frames of a context running in order, every earlier frame) the graph
+    // is destroyed without a device synchronise (reclaim_retired)
+    struct Retired { cudaGraphExec_t exec; cudaEvent_t done; };
+    std::vector<Retired> retired;
     uint64_t graph_clock = 0;
     bool graphs_stale = false;              // set by the device-less getters: dropped by the next ensure_ready (on the right device)
     void *last_out = nullptr;               // where the last final upsample wrote (nullptr: c->result; an array frame: its AO array)
@@ -160,9 +189,6 @@ struct MeaoCtx {
     // that uses it may still be in flight.
     std::map<const void *, cudaSurfaceObject_t> surfaces;
     int last_kind = MEAO_DEPTH_RAW_F32;     // ingest kind of the last downsample (selects the atlas padding value)
-    // the per-layer camera tables in the arena (kernels.h LayerZ / LayerRender): layer_zb[l]; layer_ren[(2 (k - 1) + wide) L + l]
-    LayerZ *layer_zb = nullptr;
-    LayerRender *layer_ren = nullptr;
 
     std::vector<std::pair<std::string, float>> last_profile;
     int profile_repeats = 1;                // launches per kernel inside one event pair of meao_profile_frame
@@ -182,7 +208,13 @@ int refuse_layered(MeaoCtx *c, const char *what)
 {
     return fail(c, MEAO_ERR_UNSUPPORTED, "%s: row bands need a single-layer context (this one has %d layers, meao_set_layers)", what, c->layers);
 }
-#define LAYERS_GUARD(c, what) do { if ((c) && (c)->layers > 1) return refuse_layered((c), (what)); } while (0)
+// Row bands and reservations exclude each other too: every arena of one frame size must have one layout (DESIGN.md 4).
+int refuse_reserved(MeaoCtx *c, const char *what)
+{
+    return fail(c, MEAO_ERR_UNSUPPORTED, "%s: row bands need an unreserved context (this one reserves %dx%d, meao_reserve)", what, c->res_w, c->res_h);
+}
+#define BAND_GUARD(c, what) do { if ((c) && (c)->layers > 1) return refuse_layered((c), (what)); \
+    if ((c) && (c)->res_w > 0) return refuse_reserved((c), (what)); } while (0)
 #define CUDA_TRY(c, expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) \
     return fail((c), MEAO_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); } while (0)
 
@@ -303,7 +335,7 @@ void drop_graph(MeaoCtx *c)
     if (c->graphs.empty() && c->retired.empty() && c->surfaces.empty()) return;
     cudaDeviceSynchronize();            // a re-plan is rare; never destroy an executable graph (or surface) that may still be in flight
     for (auto &kv : c->graphs) cudaGraphExecDestroy(kv.second.exec);
-    for (auto ge : c->retired) cudaGraphExecDestroy(ge);
+    for (auto &r : c->retired) { cudaGraphExecDestroy(r.exec); cudaEventDestroy(r.done); }
     for (auto &kv : c->surfaces) cudaDestroySurfaceObject(kv.second);
     c->graphs.clear();
     c->retired.clear();
@@ -390,66 +422,34 @@ int setup_band(MeaoCtx *c)
     return 0;
 }
 
-int allocate(MeaoCtx *c)
+// The size the arena is laid out for: the reservation, or the current size
+inline int arena_w(const MeaoCtx *c) { return c->res_w > 0 ? c->res_w : c->W; }
+inline int arena_h(const MeaoCtx *c) { return c->res_w > 0 ? c->res_h : c->H; }
+
+// Places the buffers of the current size (c->W x c->H) in the arena, where a fresh context of that size has them, with its camera
+// tables in slot `slot`; encodes the TMA maps and resets the band to the whole frame.  Host work only: no allocation, no CUDA call.
+int place_size(MeaoCtx *c, int slot)
 {
-    const int W = c->W, H = c->H;
-    for (int l = 0; l < 7; l++) {                         // AO.cs:276-281
-        const int div = 1 << l;
-        c->lw[l] = (W + div - 1) / div;
-        c->lh[l] = (H + div - 1) / div;
-    }
-    c->band0 = 0; c->band1 = H; c->prev0 = -1; c->next1 = -1;
-    c->plan_dirty = true;
-    if (c->plan_only) return setup_band(c);
-    free_buffers(c);
-    // pitches: rows start on 128-byte boundaries
-    c->lin_pitch = align_up(c->lw[0], 64);
-    c->result_pitch = align_up(c->lw[0], 128);
-    // every image: `layers` views of the same pitch, back to back ([L][h][pitch], kernels.h "layered frames")
-    const size_t L = (size_t)c->layers;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 255) / 256 * 256; return o; };
-    take(sizeof(BandFlags));            // offset 0 in EVERY context's arena (the neighbours address it through their peer mapping)
-    const size_t o_ctr = take(8 * sizeof(uint32_t));
-    size_t o_lin = take(L * c->lin_pitch * c->lh[0] * sizeof(__half));
-    size_t o_res = take(L * c->result_pitch * c->lh[0]);
-    size_t o_low[5], o_occ[5], o_comb[4], o_hq[5];
-    for (int k = 1; k <= 4; k++) {
-        c->low_pitch[k] = align_up(c->lw[k], 32);
-        c->occ_pitch[k] = align_up(c->lw[k], 128);
-        o_low[k] = take(L * c->low_pitch[k] * c->lh[k] * sizeof(float));
-        o_occ[k] = take(L * c->occ_pitch[k] * c->lh[k]);
-        if (k <= 3) o_comb[k] = take(L * c->occ_pitch[k] * c->lh[k]);
-        o_hq[k] = take(L * c->occ_pitch[k] * c->lh[k]);
-    }
-    size_t o_dst[2], o_ast[2];
-    for (int i = 0; i < 2; i++) { o_dst[i] = take(L * W * H * sizeof(float)); o_ast[i] = take(L * W * H); }
-    const size_t o_lzb = take(L * sizeof(LayerZ)), o_lren = take(8 * L * sizeof(LayerRender));
-    cudaError_t e = cudaMalloc(&c->arena, off);
-    if (e != cudaSuccess) return fail(c, e == cudaErrorMemoryAllocation ? MEAO_ERR_NOMEM : MEAO_ERR_CUDA,
-                                      "cudaMalloc(%zu) failed: %s", off, cudaGetErrorString(e));
-    c->arena_bytes = off;
-    CUDA_TRY(c, cudaMemsetAsync(c->arena, 0, off, c->stream));
-    CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+    const ArenaLayout a = arena_layout(c->W, c->H, c->layers);
+    memcpy(c->lw, a.lw, sizeof c->lw);
+    memcpy(c->lh, a.lh, sizeof c->lh);
+    c->band0 = 0; c->band1 = c->H; c->prev0 = -1; c->next1 = -1;
+    c->slot = slot;
+    c->lin_pitch = a.lin_pitch;
+    c->result_pitch = a.result_pitch;
+    for (int k = 1; k <= 4; k++) { c->low_pitch[k] = a.low_pitch[k]; c->occ_pitch[k] = a.occ_pitch[k]; }
+    if (!c->arena) return setup_band(c);
     char *b = (char *)c->arena;
-    c->band_flags = (BandFlags *)b;
-    c->tile_ctr = (uint32_t *)(b + o_ctr);          // zeroed by the memset above
-    {
-        BandFlags init{}; init.epoch = 1;
-        CUDA_TRY(c, cudaMemcpy(c->band_flags, &init, sizeof init, cudaMemcpyHostToDevice));
-        if (c->host_error) *c->host_error = 0;
-    }
-    c->lin = (__half *)(b + o_lin);
-    c->result = (uint8_t *)(b + o_res);
+    c->lin = (__half *)(b + a.lin);
+    c->result = (uint8_t *)(b + a.result);
     for (int k = 1; k <= 4; k++) {
-        c->low[k] = (float *)(b + o_low[k]);
-        c->occ[k] = (uint8_t *)(b + o_occ[k]);
-        if (k <= 3) c->comb[k] = (uint8_t *)(b + o_comb[k]);
-        c->hq[k] = (uint8_t *)(b + o_hq[k]);
+        c->low[k] = (float *)(b + a.low[k]);
+        c->occ[k] = (uint8_t *)(b + a.occ[k]);
+        if (k <= 3) c->comb[k] = (uint8_t *)(b + a.comb[k]);
+        c->hq[k] = (uint8_t *)(b + a.hq[k]);
     }
-    for (int i = 0; i < 2; i++) { c->depth_stage[i] = (float *)(b + o_dst[i]); c->ao_stage[i] = (uint8_t *)(b + o_ast[i]); }
-    c->layer_zb = (LayerZ *)(b + o_lzb);
-    c->layer_ren = (LayerRender *)(b + o_lren);     // written by the first ensure_ready (the plan is dirty)
+    c->layer_zb = (LayerZ *)(b + a.table0 + (size_t)slot * a.table_stride);
+    c->layer_ren = (LayerRender *)((char *)c->layer_zb + a.table_ren);
 
     c->tma_ok = false;
     if (c->encode) {
@@ -481,6 +481,69 @@ int allocate(MeaoCtx *c)
     return setup_band(c);
 }
 
+// A new arena for arena_w x arena_h at the layer count, laid out by arena_layout; the current size (if any) is placed in it and
+// re-planned by the next ensure_ready.  keep_old: allocate before freeing the old arena, so that MEAO_ERR_NOMEM leaves the context as
+// it was (meao_reserve); otherwise the old arena goes first, as a resize always did.
+int allocate(MeaoCtx *c, bool keep_old = false)
+{
+    const ArenaLayout a = arena_layout(arena_w(c), arena_h(c), c->layers);
+    if (!c->plan_only) {
+        if (!keep_old) free_buffers(c);
+        void *arena = nullptr;
+        cudaError_t e = cudaMalloc(&arena, a.bytes);
+        if (e != cudaSuccess) return fail(c, e == cudaErrorMemoryAllocation ? MEAO_ERR_NOMEM : MEAO_ERR_CUDA,
+                                          "cudaMalloc(%zu) failed: %s", a.bytes, cudaGetErrorString(e));
+        if (keep_old) free_buffers(c);
+        c->arena = arena;
+        c->arena_bytes = a.bytes;
+        c->arena_allocations++;
+        CUDA_TRY(c, cudaMemsetAsync(c->arena, 0, a.bytes, c->stream));
+        CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+        char *b = (char *)c->arena;
+        c->band_flags = (BandFlags *)b;
+        c->tile_ctr = (uint32_t *)(b + a.ctr);          // zeroed by the memset above
+        {
+            BandFlags init{}; init.epoch = 1;
+            CUDA_TRY(c, cudaMemcpy(c->band_flags, &init, sizeof init, cudaMemcpyHostToDevice));
+            if (c->host_error) *c->host_error = 0;
+        }
+        for (int i = 0; i < 2; i++) { c->depth_stage[i] = (float *)(b + a.depth_stage[i]); c->ao_stage[i] = (uint8_t *)(b + a.ao_stage[i]); }
+    }
+    c->plan_dirty = true;                           // the camera tables are written by the first ensure_ready
+    for (auto &s : c->size_slots) s.valid = false;
+    if (c->W <= 0) return 0;
+    return place_size(c, 0);
+}
+
+// Reserved contexts: make w x h the current size without touching the device.  The current size is parked in its slot; a size parked
+// earlier is swapped back in as it was (plan, maps, camera tables); a new size takes a free slot or the least recently used one, and
+// is planned on the host -- its camera tables are written by its first frame, on that frame's stream (write_tables).
+int switch_size(MeaoCtx *c, int w, int h)
+{
+    SizeState &cur = *c;
+    if (c->W > 0) c->size_slots[c->slot] = MeaoCtx::SizeSlot{true, c->size_clock, cur};
+    int slot = -1;
+    for (int i = 0; i < kSizeSlots; i++) {
+        MeaoCtx::SizeSlot &s = c->size_slots[i];
+        if (s.valid && s.s.W == w && s.s.H == h) {
+            cur = s.s;
+            s.last_use = ++c->size_clock;
+            return 0;
+        }
+        if (slot < 0 || (c->size_slots[slot].valid && (!s.valid || s.last_use < c->size_slots[slot].last_use))) slot = i;
+    }
+    c->W = w; c->H = h;
+    int rc = place_size(c, slot);
+    if (rc) return rc;
+    if (!c->plan_dirty) {                           // else ensure_ready re-plans (and drops every other slot)
+        build_plan(c);
+        c->cam_table_stale = false;
+        c->table_pending = !c->plan_only;
+    }
+    c->size_slots[slot] = MeaoCtx::SizeSlot{true, ++c->size_clock, cur};
+    return 0;
+}
+
 // The call-order tables of record_render: Render.compute:162-168 (checker) and :148-159 (exhaustive) table slots
 const int kIdxChecker[7] = {1, 3, 4, 8, 11, 6, 10};
 const int kIdxExh[12] = {0, 1, 2, 3, 4, 8, 11, 5, 6, 7, 9, 10};
@@ -501,24 +564,57 @@ LayerRender layer_render(const MeaoCtx *c, const CamConsts &cc, int k, bool wide
     return r;
 }
 
-// Write the per-layer camera tables to the arena.  Called by ensure_ready after a re-plan, once every frame that may read the old
-// tables has finished (a device synchronise: frames may be in flight on any caller stream).
-int upload_camera_tables(MeaoCtx *c)
+// The per-layer camera tables of the current plan, as they go into the arena
+void camera_tables(const MeaoCtx *c, std::vector<LayerZ> &zb, std::vector<LayerRender> &ren)
 {
     const int L = c->layers;
-    std::vector<LayerZ> zb(L);
-    std::vector<LayerRender> ren((size_t)8 * L);
+    zb.resize(L);
+    ren.resize((size_t)8 * L);
     for (int l = 0; l < L; l++) {
         const CamConsts &cc = c->layer_consts[l];
         zb[l] = LayerZ{cc.zb[0], cc.zb[1]};
         for (int k = 1; k <= 4; k++)
             for (int w = 0; w < 2; w++) ren[(size_t)(2 * (k - 1) + w) * L + l] = layer_render(c, cc, k, w != 0);
     }
+}
+
+// Write the per-layer camera tables to the arena.  Called by ensure_ready after a re-plan, once every frame that may read the old
+// tables has finished (a device synchronise: frames may be in flight on any caller stream).
+int upload_camera_tables(MeaoCtx *c)
+{
+    std::vector<LayerZ> zb;
+    std::vector<LayerRender> ren;
+    camera_tables(c, zb, ren);
     CUDA_TRY(c, cudaDeviceSynchronize());
     CUDA_TRY(c, cudaMemcpy(c->layer_zb, zb.data(), zb.size() * sizeof(LayerZ), cudaMemcpyHostToDevice));
     CUDA_TRY(c, cudaMemcpy(c->layer_ren, ren.data(), ren.size() * sizeof(LayerRender), cudaMemcpyHostToDevice));
     c->cam_table_stale = false;
+    c->table_pending = false;
     return 0;
+}
+
+// The tables of a size newly planned by switch_size, written in stream order before the first frame that reads them, on that frame's
+// stream.  The slot may have held another size's tables: frames of one context run in the order they are issued (include/meao.h),
+// so every earlier frame that read it has completed before this copy lands.  The source is pageable, so the runtime stages it and
+// the vectors may go when the call returns.
+int write_tables(MeaoCtx *c, cudaStream_t s)
+{
+    if (!c->table_pending) return 0;
+    std::vector<LayerZ> zb;
+    std::vector<LayerRender> ren;
+    camera_tables(c, zb, ren);
+    CUDA_TRY(c, cudaMemcpyAsync(c->layer_zb, zb.data(), zb.size() * sizeof(LayerZ), cudaMemcpyHostToDevice, s));
+    CUDA_TRY(c, cudaMemcpyAsync(c->layer_ren, ren.data(), ren.size() * sizeof(LayerRender), cudaMemcpyHostToDevice, s));
+    c->table_pending = false;
+    return 0;
+}
+
+// A re-plan after a plan input changed: the parked sizes were planned with the old inputs, so they go (with the captured graphs).
+void replan(MeaoCtx *c)
+{
+    build_plan(c);
+    c->graphs_stale = true;
+    for (int i = 0; i < kSizeSlots; i++) if (i != c->slot) c->size_slots[i].valid = false;
 }
 
 int ensure_ready(MeaoCtx *c)
@@ -527,10 +623,17 @@ int ensure_ready(MeaoCtx *c)
     if (c->W <= 0) return fail(c, MEAO_ERR_INVALID, "meao_resize has not been called");
     if (c->plan_only) return fail(c, MEAO_ERR_CUDA, "plan-only context (device < 0): no CUDA device bound, and libmeao has no CPU fallback");
     CUDA_TRY(c, cudaSetDevice(c->device));
-    if (c->plan_dirty) { build_plan(c); c->graphs_stale = true; }
+    if (c->plan_dirty) replan(c);
     if (c->graphs_stale) drop_graph(c);
     if (c->cam_table_stale) { int rc = upload_camera_tables(c); if (rc) return rc; }
     return 0;
+}
+
+// ensure_ready for an entry point that issues work on stream s which may read the camera tables
+int frame_ready(MeaoCtx *c, cudaStream_t s)
+{
+    int rc = ensure_ready(c);
+    return rc ? rc : write_tables(c, s);
 }
 
 // Z direction of the context's cameras (meao_set_layer_cameras requires one for all layers)
@@ -1035,7 +1138,13 @@ int meao_resize(MeaoCtx *c, int32_t w, int32_t h)
 {
     if (!c) return MEAO_ERR_INVALID;
     if (w <= 0 || h <= 0 || w > 32768 || h > 32768) return fail(c, MEAO_ERR_INVALID, "bad size %dx%d", w, h);
+    if (c->res_w > 0 && (w > c->res_w || h > c->res_h))      // never a silent re-allocation for a dynamic-resolution host
+        return fail(c, MEAO_ERR_INVALID, "size %dx%d lies outside the reservation %dx%d (meao_reserve)", w, h, c->res_w, c->res_h);
     if (w == c->W && h == c->H && (c->arena || c->plan_only)) return 0;       // RTHandle.CheckBaseDimensions, AO.cs:145-148
+    if (c->res_w > 0 && (c->arena || c->plan_only)) {
+        const int rc = switch_size(c, w, h);        // no allocation, no synchronise, the other sizes' graphs stay
+        return rc ? rc : 1;
+    }
     if (!c->plan_only) {
         CUDA_TRY(c, cudaSetDevice(c->device));
         CUDA_TRY(c, cudaStreamSynchronize(c->stream));
@@ -1044,6 +1153,43 @@ int meao_resize(MeaoCtx *c, int32_t w, int32_t h)
     int rc = allocate(c);
     if (rc) { c->W = c->H = 0; return rc; }
     return 1;
+}
+
+int meao_reserve(MeaoCtx *c, int32_t max_w, int32_t max_h)
+{
+    if (!c) return MEAO_ERR_INVALID;
+    const bool clear = max_w == 0 && max_h == 0;
+    if (!clear && (max_w <= 0 || max_h <= 0 || max_w > 32768 || max_h > 32768))
+        return fail(c, MEAO_ERR_INVALID, "bad reservation %dx%d (each dimension in 1..32768, or 0x0 to clear)", max_w, max_h);
+    if (c->W > 0 && (c->band0 != 0 || c->band1 != c->H || c->prev0 >= 0 || c->next1 >= 0))
+        return fail(c, MEAO_ERR_UNSUPPORTED, "meao_reserve: this context has a row band (meao_set_row_band); row bands need an unreserved context");
+    if (!clear && c->W > 0 && max_w < c->W)
+        return fail(c, MEAO_ERR_INVALID, "reservation width %d is below the current width %d", max_w, c->W);
+    if (!clear && c->H > 0 && max_h < c->H)
+        return fail(c, MEAO_ERR_INVALID, "reservation height %d is below the current height %d", max_h, c->H);
+    if (max_w == c->res_w && max_h == c->res_h) return 0;
+    const int old_w = c->res_w, old_h = c->res_h;
+    c->res_w = max_w; c->res_h = max_h;
+    if (c->plan_only) return 1;                     // recorded; nothing to allocate
+    CUDA_TRY(c, cudaSetDevice(c->device));
+    CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+    if (clear && c->W <= 0) { free_buffers(c); return 1; }
+    const int rc = allocate(c, true);               // like a size change today, but the old arena stays until the new one exists
+    if (rc) { c->res_w = old_w; c->res_h = old_h; return rc; }
+    return 1;
+}
+
+int meao_reservation(const MeaoCtx *c, MeaoReservation *out)
+{
+    if (!c || !out) return MEAO_ERR_INVALID;
+    memset(out, 0, sizeof *out);
+    out->width = c->res_w; out->height = c->res_h;
+    if (arena_w(c) > 0) out->arena_bytes = c->plan_only ? (int64_t)arena_layout(arena_w(c), arena_h(c), c->layers).bytes : (int64_t)c->arena_bytes;
+    if (c->W > 0) out->arena_bytes_needed = (int64_t)arena_layout(c->W, c->H, c->layers).bytes;
+    out->arena_allocations = c->arena_allocations;
+    out->graphs_held = (int64_t)(c->graphs.size() + c->retired.size());
+    out->graph_instantiations = c->graph_instantiations;
+    return MEAO_OK;
 }
 
 int meao_set_layers(MeaoCtx *c, int32_t layers)
@@ -1057,7 +1203,7 @@ int meao_set_layers(MeaoCtx *c, int32_t layers)
     old_cams.swap(c->layer_cams);                   // a table has one camera per layer: a new layer count clears it
     c->layers = layers;
     c->plan_dirty = true;
-    if (c->W <= 0) return 1;                        // applied by the first meao_resize
+    if (c->W <= 0 && !c->arena) return 1;           // applied by the first meao_resize (a reserved arena is laid out again now)
     if (!c->plan_only) {
         CUDA_TRY(c, cudaSetDevice(c->device));
         CUDA_TRY(c, cudaStreamSynchronize(c->stream));
@@ -1077,7 +1223,7 @@ int meao_set_layers(MeaoCtx *c, int32_t layers)
 int meao_set_row_band(MeaoCtx *c, int32_t row0, int32_t row1, int32_t prev_row0, int32_t next_row1)
 {
     if (!c || c->W <= 0) return MEAO_ERR_INVALID;
-    LAYERS_GUARD(c, "meao_set_row_band");
+    BAND_GUARD(c, "meao_set_row_band");
     if (row0 < 0 || row1 > c->H || row0 >= row1 || (row0 % 16) || ((row1 % 16) && row1 != c->H))
         return fail(c, MEAO_ERR_INVALID, "band [%d,%d) must be 16-row aligned inside [0,%d)", row0, row1, c->H);
     if ((prev_row0 >= 0 && (prev_row0 % 16 || prev_row0 >= row0)) || (next_row1 >= 0 && (next_row1 <= row1 || next_row1 > c->H)))
@@ -1129,7 +1275,7 @@ static void halo_ranges(MeaoCtx *c, int side, bool send, Range out[5])
 static int64_t halo_size(MeaoCtx *c, int side, bool send)
 {
     if (!c || c->W <= 0 || (side != 0 && side != 1)) return MEAO_ERR_INVALID;
-    LAYERS_GUARD(c, send ? "meao_halo_bytes" : "meao_halo_recv_bytes");
+    BAND_GUARD(c, send ? "meao_halo_bytes" : "meao_halo_recv_bytes");
     Range r[5]; halo_ranges(c, side, send, r);
     int64_t bytes = 0;
     for (int k = 1; k <= 4; k++) bytes += (int64_t)(r[k].hi - r[k].lo) * c->lw[k] * 4;
@@ -1139,7 +1285,7 @@ int64_t meao_halo_bytes(MeaoCtx *c, int32_t side) { return halo_size(c, side, tr
 int meao_halo_rows(MeaoCtx *c, int32_t side, int32_t send, int32_t out8[8])
 {
     if (!c || c->W <= 0 || (side != 0 && side != 1) || !out8) return MEAO_ERR_INVALID;
-    LAYERS_GUARD(c, "meao_halo_rows");
+    BAND_GUARD(c, "meao_halo_rows");
     Range r[5]; halo_ranges(c, side, send != 0, r);
     for (int k = 1; k <= 4; k++) { out8[2 * (k - 1)] = r[k].lo; out8[2 * (k - 1) + 1] = r[k].hi; }
     return MEAO_OK;
@@ -1158,7 +1304,7 @@ int64_t meao_halo_recv_bytes(MeaoCtx *c, int32_t side) { return halo_size(c, sid
 
 static int halo_copy(MeaoCtx *c, int side, void *packed, bool pack, void *stream)
 {
-    LAYERS_GUARD(c, pack ? "meao_halo_pack" : "meao_halo_unpack");
+    BAND_GUARD(c, pack ? "meao_halo_pack" : "meao_halo_unpack");
     int rc = ensure_ready(c); if (rc) return rc;
     if (side != 0 && side != 1) return fail(c, MEAO_ERR_INVALID, "side must be 0 or 1");
     cudaStream_t s = (cudaStream_t)stream;
@@ -1180,7 +1326,7 @@ int meao_halo_unpack(MeaoCtx *c, int32_t side, const void *packed, void *stream)
 
 int meao_render_band_prepare(MeaoCtx *c, const void *depth, int32_t kind, void *stream)
 {
-    LAYERS_GUARD(c, "meao_render_band_prepare");
+    BAND_GUARD(c, "meao_render_band_prepare");
     int rc = ensure_ready(c); if (rc) return rc;
     if (!depth) return fail(c, MEAO_ERR_INVALID, "depth is NULL");
     return record_downsample(c, depth, kind, (cudaStream_t)stream);
@@ -1188,7 +1334,7 @@ int meao_render_band_prepare(MeaoCtx *c, const void *depth, int32_t kind, void *
 
 int meao_render_band_finish(MeaoCtx *c, void *ao_out, void *stream)
 {
-    LAYERS_GUARD(c, "meao_render_band_finish");
+    BAND_GUARD(c, "meao_render_band_finish");
     int rc = ensure_ready(c); if (rc) return rc;
     cudaStream_t s = (cudaStream_t)stream;
     const int kind = c->last_kind;
@@ -1247,24 +1393,55 @@ static int capture_graph(MeaoCtx *c, const std::function<int(cudaStream_t, int)>
     return fail(c, MEAO_ERR_CUDA, "graph capture failed");
 }
 
-static int launch_cached(MeaoCtx *c, const MeaoCtx::GraphKey &key, cudaStream_t s, int nk, const std::function<int(cudaStream_t, int)> &record)
+// The graph cache holds at most kMaxGraphs executable graphs; at most kMaxRetired more wait for their `done` event, so a context never
+// holds more than kMaxGraphs + kMaxRetired (include/meao.h MeaoReservation.graphs_held), whatever sequence of sizes and buffers it sees.
+constexpr size_t kMaxGraphs = 64, kMaxRetired = 8;
+static_assert(MEAO_SIZE_SLOTS == kSizeSlots && MEAO_MAX_GRAPHS_HELD == kMaxGraphs + kMaxRetired, "include/meao.h states these bounds");
+
+// Destroys the retired executable graphs whose `done` event has completed; with wait, first waits for the oldest (an event wait on
+// the host, not a device synchronise).
+static void reclaim_retired(MeaoCtx *c, bool wait)
+{
+    if (wait && !c->retired.empty()) cudaEventSynchronize(c->retired.front().done);
+    for (auto it = c->retired.begin(); it != c->retired.end();) {
+        const cudaError_t e = cudaEventQuery(it->done);
+        if (e == cudaErrorNotReady) { cudaGetLastError(); ++it; continue; }
+        cudaGetLastError();
+        cudaGraphExecDestroy(it->exec);
+        cudaEventDestroy(it->done);
+        it = c->retired.erase(it);
+    }
+}
+
+static int launch_cached(MeaoCtx *c, const MeaoCtx::GraphKey &key_in, cudaStream_t s, int nk, const std::function<int(cudaStream_t, int)> &record)
 {
     if (c->flags & MEAO_FLAG_NO_GRAPH) return record(s, 0);
-    constexpr size_t kMaxGraphs = 64;
+    MeaoCtx::GraphKey key = key_in;
+    key.size[0] = c->W; key.size[1] = c->H; key.size[2] = c->slot;
     auto it = c->graphs.find(key);
+    bool retiring = false;
     if (it == c->graphs.end()) {
+        if (!c->retired.empty()) reclaim_retired(c, c->retired.size() >= kMaxRetired);
         cudaGraph_t g = nullptr;
         int rc = capture_graph(c, record, &g);
         if (rc) return rc;
         cudaGraphExec_t ge = nullptr;
         if (c->graphs.size() >= kMaxGraphs) {
-            // a caller that rotates more buffers than the cache holds: re-target the least recently used executable graph
-            // (same topology, new kernel arguments) instead of synchronising the device and instantiating again
+            // a caller that rotates more buffers (or visits more frame sizes) than the cache holds: re-target the least recently used
+            // executable graph (same topology, new kernel arguments) instead of synchronising the device and instantiating again
             auto victim = c->graphs.begin();
             for (auto j = c->graphs.begin(); j != c->graphs.end(); ++j) if (j->second.last_use < victim->second.last_use) victim = j;
             cudaGraphExecUpdateResultInfo info;
             ge = victim->second.exec;
-            if (cudaGraphExecUpdate(ge, g, &info) != cudaSuccess) { cudaGetLastError(); c->retired.push_back(ge); ge = nullptr; }
+            if (cudaGraphExecUpdate(ge, g, &info) != cudaSuccess) {
+                cudaGetLastError();
+                cudaEvent_t done = nullptr;
+                if (cudaEventCreateWithFlags(&done, cudaEventDisableTiming) != cudaSuccess) { cudaGraphDestroy(g); return fail(c, MEAO_ERR_CUDA, "cudaEventCreate failed"); }
+                c->retired.push_back(MeaoCtx::Retired{ge, done});
+                cudaEventRecord(done, s);           // recorded again after the new launch below; this covers a launch that fails
+                retiring = true;
+                ge = nullptr;
+            }
             c->graphs.erase(victim);
         }
         if (!ge) {
@@ -1277,19 +1454,21 @@ static int launch_cached(MeaoCtx *c, const MeaoCtx::GraphKey &key, cudaStream_t 
                 e = cudaGraphInstantiate(&ge, g, 0);
             }
             if (e != cudaSuccess) { if (g) cudaGraphDestroy(g); return fail(c, MEAO_ERR_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(e)); }
+            c->graph_instantiations++;
         }
         cudaGraphDestroy(g);
         it = c->graphs.emplace(key, MeaoCtx::GraphEntry{ge, 0}).first;
     }
     it->second.last_use = ++c->graph_clock;
     CUDA_TRY(c, cudaGraphLaunch(it->second.exec, s));
+    if (retiring) CUDA_TRY(c, cudaEventRecord(c->retired.back().done, s));    // after the frame that replaced it
     c->launches += nk;
     return 0;
 }
 
 int meao_band_phase_a(MeaoCtx *c, const void *depth, int32_t kind, void *send_up, void *send_down, void *stream)
 {
-    LAYERS_GUARD(c, "meao_band_phase_a");
+    BAND_GUARD(c, "meao_band_phase_a");
     int rc = ensure_ready(c); if (rc) return rc;
     if (!depth) return fail(c, MEAO_ERR_INVALID, "depth is NULL");
     c->last_kind = kind;
@@ -1305,7 +1484,7 @@ int meao_band_phase_a(MeaoCtx *c, const void *depth, int32_t kind, void *send_up
 
 int meao_band_phase_b(MeaoCtx *c, const void *recv_up, const void *recv_down, void *ao_out, void *stream)
 {
-    LAYERS_GUARD(c, "meao_band_phase_b");
+    BAND_GUARD(c, "meao_band_phase_b");
     int rc = ensure_ready(c); if (rc) return rc;
     if (!ao_out) return fail(c, MEAO_ERR_INVALID, "ao_out is NULL");
     const int kind = c->last_kind;
@@ -1336,7 +1515,7 @@ constexpr uint32_t kPeerMagic = 0x4d45414fu;
 
 int meao_band_export(MeaoCtx *c, MeaoPeerHandle *out)
 {
-    LAYERS_GUARD(c, "meao_band_export");
+    BAND_GUARD(c, "meao_band_export");
     int rc = ensure_ready(c); if (rc) return rc;
     if (!out) return fail(c, MEAO_ERR_INVALID, "out is NULL");
     PeerHandlePod h{};
@@ -1351,7 +1530,7 @@ int meao_band_export(MeaoCtx *c, MeaoPeerHandle *out)
 
 int meao_band_connect(MeaoCtx *c, int32_t side, const MeaoPeerHandle *peer)
 {
-    LAYERS_GUARD(c, "meao_band_connect");
+    BAND_GUARD(c, "meao_band_connect");
     int rc = ensure_ready(c); if (rc) return rc;
     if (side != 0 && side != 1) return fail(c, MEAO_ERR_INVALID, "side must be 0 (up) or 1 (down)");
     drop_graph(c);                                  // captured band steps carry the old peer pointers
@@ -1429,7 +1608,7 @@ static int record_exchange(MeaoCtx *c, cudaStream_t s)
 
 int meao_band_step(MeaoCtx *c, const void *depth, int32_t kind, void *ao_out, void *stream)
 {
-    LAYERS_GUARD(c, "meao_band_step");
+    BAND_GUARD(c, "meao_band_step");
     int rc = ensure_ready(c); if (rc) return rc;
     if (!depth || !ao_out) return fail(c, MEAO_ERR_INVALID, "depth / ao_out is NULL");
     if ((c->prev0 >= 0 && !c->peer_base[0]) || (c->next1 >= 0 && !c->peer_base[1]))
@@ -1452,7 +1631,7 @@ int meao_band_step(MeaoCtx *c, const void *depth, int32_t kind, void *ao_out, vo
 
 int meao_band_step_host(MeaoCtx *c, const void *depth_host, int32_t kind, uint8_t *ao_host)
 {
-    LAYERS_GUARD(c, "meao_band_step_host");
+    BAND_GUARD(c, "meao_band_step_host");
     int rc = ensure_ready(c); if (rc) return rc;
     if (!depth_host || !ao_host) return fail(c, MEAO_ERR_INVALID, "depth / ao_out is NULL");
     if (kind < MEAO_DEPTH_RAW_F32 || kind > MEAO_DEPTH_RAW_D24S8) return fail(c, MEAO_ERR_INVALID, "bad depth kind %d", kind);
@@ -1550,14 +1729,14 @@ int render_views(MeaoCtx *c, const void *depth, int kind, void *ao_out, ViewPitc
 
 int meao_render(MeaoCtx *c, const void *depth, int32_t kind, void *ao_out, void *stream)
 {
-    int rc = ensure_ready(c); if (rc) return rc;
+    int rc = frame_ready(c, (cudaStream_t)stream); if (rc) return rc;
     return render_views(c, depth, kind, ao_out, tight_pitch(c, kind), stream);      // meao_render_pitched at the tight pitches
 }
 
 int meao_render_pitched(MeaoCtx *c, const void *depth, int64_t depth_row_pitch, int64_t depth_layer_pitch, int32_t kind,
                         void *ao_out, int64_t ao_row_pitch, int64_t ao_layer_pitch, void *stream)
 {
-    int rc = ensure_ready(c); if (rc) return rc;
+    int rc = frame_ready(c, (cudaStream_t)stream); if (rc) return rc;
     return render_views(c, depth, kind, ao_out, ViewPitch{depth_row_pitch, depth_layer_pitch, ao_row_pitch, ao_layer_pitch}, stream);
 }
 
@@ -1636,7 +1815,7 @@ int prepare_arrays(MeaoCtx *c, const void *depth_array, int kind, const void *ao
 
 int meao_render_arrays(MeaoCtx *c, const void *depth_array, int32_t kind, void *ao_array, void *stream)
 {
-    int rc = ensure_ready(c); if (rc) return rc;
+    int rc = frame_ready(c, (cudaStream_t)stream); if (rc) return rc;
     ArrayIO io;
     if ((rc = prepare_arrays(c, depth_array, kind, ao_array, &io))) return rc;
     // the frame graph of meao_render with its first and last node reading / writing the arrays
@@ -1670,7 +1849,7 @@ int meao_release_array(MeaoCtx *c, const void *array)
             it = c->graphs.erase(it);
         } else ++it;
     }
-    for (auto ge : c->retired) cudaGraphExecDestroy(ge);      // a retired graph may be an array frame: none is in flight any more
+    for (auto &r : c->retired) { cudaGraphExecDestroy(r.exec); cudaEventDestroy(r.done); }     // a retired graph may be an array frame: none is in flight any more
     c->retired.clear();
     auto s = c->surfaces.find(array);
     if (s != c->surfaces.end()) { cudaDestroySurfaceObject(s->second); c->surfaces.erase(s); }
@@ -1732,28 +1911,28 @@ void meao_host_free(void *p) { if (p) cudaFreeHost(p); }
 
 int meao_stage_downsample(MeaoCtx *c, const void *depth, int32_t kind, void *stream)
 {
-    int rc = ensure_ready(c); if (rc) return rc;
+    int rc = frame_ready(c, (cudaStream_t)stream); if (rc) return rc;
     if (!depth) return fail(c, MEAO_ERR_INVALID, "depth is NULL");
     return record_downsample(c, depth, kind, (cudaStream_t)stream);
 }
 
 int meao_stage_render(MeaoCtx *c, int32_t level, void *stream)
 {
-    int rc = ensure_ready(c); if (rc) return rc;
+    int rc = frame_ready(c, (cudaStream_t)stream); if (rc) return rc;
     if (level < 1 || level > 4) return fail(c, MEAO_ERR_INVALID, "render level %d not in 1..4", level);
     return record_render(c, level, c->last_kind, (cudaStream_t)stream);
 }
 
 int meao_stage_render_wide(MeaoCtx *c, int32_t level, void *stream)
 {
-    int rc = ensure_ready(c); if (rc) return rc;
+    int rc = frame_ready(c, (cudaStream_t)stream); if (rc) return rc;
     if (level < 1 || level > 4) return fail(c, MEAO_ERR_INVALID, "render level %d not in 1..4", level);
     return record_render(c, level, c->last_kind, (cudaStream_t)stream, true);
 }
 
 int meao_stage_upsample(MeaoCtx *c, int32_t lo_level, void *ao_out, void *stream)
 {
-    int rc = ensure_ready(c); if (rc) return rc;
+    int rc = frame_ready(c, (cudaStream_t)stream); if (rc) return rc;
     if (lo_level < 1 || lo_level > 4) return fail(c, MEAO_ERR_INVALID, "upsample lo level %d not in 1..4", lo_level);
     return record_upsample(c, lo_level, lo_level == 1 ? ao_out : nullptr, (cudaStream_t)stream);
 }
@@ -1769,7 +1948,7 @@ int meao_buffer_desc(const MeaoCtx *c, int32_t id, MeaoBufferDesc *out)
 
 int meao_get_buffer(MeaoCtx *c, int32_t id, void *host_out, size_t host_bytes)
 {
-    int rc = ensure_ready(c); if (rc) return rc;
+    int rc = frame_ready(c, c->stream); if (rc) return rc;
     int lvl, slices, elem;
     if (!host_out || buffer_info(c, id, &lvl, &slices, &elem)) return fail(c, MEAO_ERR_INVALID, "bad buffer id %d", id);
     const size_t one = (size_t)c->lw[lvl] * c->lh[lvl] * slices * elem, need = one * c->layers;     // [L][reference layout]
@@ -1806,7 +1985,7 @@ int meao_get_buffer(MeaoCtx *c, int32_t id, void *host_out, size_t host_bytes)
 
 int meao_debug_view(MeaoCtx *c, int32_t id, void *out, void *stream)
 {
-    int rc = ensure_ready(c); if (rc) return rc;
+    int rc = frame_ready(c, (cudaStream_t)stream); if (rc) return rc;
     int lvl, slices, elem;
     if (!out || buffer_info(c, id, &lvl, &slices, &elem)) return fail(c, MEAO_ERR_INVALID, "bad buffer id %d / out is NULL", id);
     if (c->band0 != 0 || c->band1 != c->H) return fail(c, MEAO_ERR_UNSUPPORTED, "debug views need a whole-frame context (no row band)");
@@ -1863,7 +2042,7 @@ int meao_set_buffer(MeaoCtx *c, int32_t id, const void *host_in, size_t host_byt
 static int plan_only(MeaoCtx *c)
 {
     if (!c || c->W <= 0) return MEAO_ERR_INVALID;
-    if (c->plan_dirty) { build_plan(c); c->graphs_stale = true; }    // the captured graphs are dropped by the next ensure_ready, on c->device
+    if (c->plan_dirty) replan(c);           // the captured graphs are dropped by the next ensure_ready, on c->device
     return 0;
 }
 
@@ -2083,7 +2262,7 @@ int meao_set_profile_repeats(MeaoCtx *c, int32_t n)
 
 int meao_profile_frame(MeaoCtx *c, const void *depth, int32_t kind, void *ao_out, float *ms_out, const char **names_out, int32_t capacity)
 {
-    int rc = ensure_ready(c); if (rc) return rc;
+    int rc = frame_ready(c, c->stream); if (rc) return rc;
     if (!depth || !ao_out) return fail(c, MEAO_ERR_INVALID, "depth / ao_out is NULL");
     CUDA_TRY(c, cudaDeviceSynchronize());
     if ((rc = record_frame(c, depth, kind, ao_out, c->stream, true))) return rc;
