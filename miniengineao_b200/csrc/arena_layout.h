@@ -1,6 +1,6 @@
 // arena_layout.h -- where every buffer of a context lives inside its one device allocation (the arena), as a pure function of the
-// frame size and the layer count.  meao_api.cu lays out an arena with it and tests/emu/drs_driver.cpp places its emulated buffers
-// with it, so both agree on every offset and pitch.
+// frame size and the layer count.  meao_api.cu lays out an arena with it and frame_record.h's place_frame places a frame's buffers
+// by it -- in libmeao and in the emulator (tests/emu/frame_driver.cpp) alike.
 //
 // Order: BandFlags (offset 0 in every arena: the neighbour bands address it through their peer mapping), the tile counters of the
 // persistent upsample grids, kSizeSlots per-layer camera table slots, LinearDepth, the AO result, LowDepth / Occlusion / Combined /

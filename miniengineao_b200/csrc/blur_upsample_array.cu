@@ -41,18 +41,8 @@ cudaError_t launch_blur_upsample_array(const CUtensorMap &lo_depth_map, const CU
     UpsampleArgs a = a_in;
     a.out = nullptr; a.out_pitch = 0; a.out_row_origin = 0;
     a.out_vec_ok = 1;               // surface stores have no alignment requirement
-    const int ybase = a.row0 & ~1;
-    a.tiles_x = ceil_div(a.hiw, kHW); a.tiles_y = ceil_div(a.row1 - ybase, kHH);
-    const long long ntiles_ll = (long long)a.tiles_x * a.tiles_y * layers;
-    if (ntiles_ll > 0x7fffffffLL) return cudaErrorInvalidValue;        // the tile index is a 32-bit int
-    const int ntiles = (int)ntiles_ll;
-    // the rule of launch_blur_upsample(_layered), on the tiles of all layers: the persistent tile loop from two tiles per CTA slot
-    const int kWave = sm_count * MEAO_UPS_MINB;
-    const char *force = getenv("MEAO_UPS_PERSIST_MIN_WAVES");
-    const double min_waves = force ? atof(force) : 2.0;
-    const bool persist = a.tile_ctr && ntiles >= (int)(min_waves * kWave);
-    if (!persist) a.tile_ctr = nullptr;
-    dim3 grid(persist ? kWave : ntiles);
+    dim3 grid;
+    if (!ups_tile_grid(a, layers, sm_count, &grid)) return cudaErrorInvalidValue;
     const int t = use_tma ? 1 : 0;
     if (!lo_ao2) {
         MEAO_LAUNCH((blur_upsample_array_kernel<false, true>), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, a, t, layers, out, surf_kind);

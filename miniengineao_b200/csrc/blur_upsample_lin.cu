@@ -113,18 +113,8 @@ cudaError_t launch_blur_upsample_lin(const CUtensorMap &lo_depth_map, const CUte
     if (layers < 1 || layers > kMaxLayers) return cudaErrorInvalidValue;
     if (!a_in.hi_is_half || a_in.hi_ao || (lo_ao2 && !lo_ao2_map)) return cudaErrorInvalidValue;      // the final level only
     UpsampleArgs a = a_in;
-    const int ybase = a.row0 & ~1;
-    a.tiles_x = ceil_div(a.hiw, kHW); a.tiles_y = ceil_div(a.row1 - ybase, kHH);
-    const long long ntiles_ll = (long long)a.tiles_x * a.tiles_y * layers;
-    if (ntiles_ll > 0x7fffffffLL) return cudaErrorInvalidValue;        // the tile index is a 32-bit int
-    const int ntiles = (int)ntiles_ll;
-    // the rule of launch_blur_upsample(_layered): the persistent tile loop from two tiles per CTA slot
-    const int kWave = sm_count * MEAO_UPS_MINB;
-    const char *force = getenv("MEAO_UPS_PERSIST_MIN_WAVES");
-    const double min_waves = force ? atof(force) : 2.0;
-    const bool persist = a.tile_ctr && ntiles >= (int)(min_waves * kWave);
-    if (!persist) a.tile_ctr = nullptr;
-    const dim3 grid(persist ? kWave : ntiles);
+    dim3 grid;
+    if (!ups_tile_grid(a, layers, sm_count, &grid)) return cudaErrorInvalidValue;
     const int t = use_tma ? 1 : 0;
     DepthIn din = din_in;           // zero pitches: the tight values
     if (!din.depth_pitch) din.depth_pitch = a.hiw;

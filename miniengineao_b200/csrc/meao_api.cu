@@ -25,6 +25,7 @@
 #include "common.cuh"
 #include "kernels.h"
 #include "arena_layout.h"
+#include "frame_record.h"
 
 using namespace meao;
 
@@ -32,7 +33,6 @@ namespace {
 
 thread_local std::string g_create_error;
 
-struct Range { int lo, hi; };   // [lo, hi)
 inline Range clampr(Range r, int n) { Range o{r.lo < 0 ? 0 : r.lo, r.hi > n ? n : r.hi}; if (o.hi < o.lo) o.hi = o.lo; return o; }
 
 // cuTensorMapEncodeTiled is fetched through the runtime so libmeao.so has no link-time
@@ -41,68 +41,15 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap *, CUtensorMapDataType, cuuint32
                                     const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
                                     CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-struct Plan {
-    // Render (per level 1..4) -- AO.cs:660-734
-    float inv_thickness[5][12];
-    float sample_weight[5][12];
-    float inv_slice_dim[5][2];
-    float reject_fadeoff;
-    float intensity;
-    float pad[5];
-    float inv_thickness_wide[5][12];       // the same for a NON-tiled source LowDepth<k> (kernel "main", AO.cs:679)
-    float inv_slice_dim_wide[5][2];
-    // Upsample (per lo level 1..4) -- AO.cs:750-771
-    float inv_low[5][2], inv_high[5][2];
-    float noise_filter_strength[5], step_size[5], blur_tolerance[5], upsample_tolerance[5];
-    float zb[4];
-};
-
-// The camera-dependent part of the plan, for one camera: ZBufferParams, both inv_thickness tables of every level and the atlas
-// padding value.  Plan holds it for the first layer; with per-layer cameras MeaoCtx::layer_consts holds it for every layer.
-struct CamConsts {
-    float zb[2];
-    float inv_thickness[5][12], inv_thickness_wide[5][12];
-    float pad[5];
-};
-
-// Everything of a context that depends on the frame size: the geometry, where the buffers of that size sit in the arena, the TMA maps,
-// the row ranges, the plan and the per-layer camera table slot.  A reserved context (meao_reserve) keeps one of these per recently used
-// size (MeaoCtx::size_slots) and swaps it in on a resize to that size, so a return to a planned size is host bookkeeping only.
-struct SizeState {
-    int W = 0, H = 0;
-    int lw[7] = {0}, lh[7] = {0};
-    // band (global L0 rows) + neighbours
-    int band0 = 0, band1 = 0, prev0 = -1, next1 = -1;
-
-    // device buffers (natural layout, pitched, global coordinates): arena_layout(W, H, layers)
-    __half *lin = nullptr; int lin_pitch = 0;
-    float *low[5] = {nullptr}; int low_pitch[5] = {0};
-    uint8_t *occ[5] = {nullptr}; int occ_pitch[5] = {0};
-    uint8_t *comb[4] = {nullptr};           // same pitch as occ of that level
-    uint8_t *hq[5] = {nullptr};             // HighQuality<k> (kernel "main" output), same pitch as occ of that level
-    uint8_t *result = nullptr; int result_pitch = 0;
-
-    bool tma_ok = false;
-    CUtensorMap map_low_ren[kRenderTileVariants][5];    // LowDepth<k> with the render box of tile height kRenderTileHs[t]
-    CUtensorMap map_low_ups[5];             // LowDepth<k> with the upsample depth box
-    CUtensorMap map_ao_ups[5];              // lo AO of upsample lo level k (Occlusion4 / Combined k)
-    CUtensorMap map_low_wide[kRenderTileVariants][5];   // LowDepth<k> with the wide-render box
-    CUtensorMap map_hq_ups[5];              // HighQuality<k> as LoResAO2 of upsample lo level k
-    CUtensorMap map_occ1_ups;               // Occlusion1 as LoResAO1 of the final upsample (MeaoVariants.single_scale)
-
-    // row ranges (per level) for this band
-    Range need_c[5];                        // rows of Occlusion<k>/Combined<k> to produce (k=1..4); [0] = final rows
-    Range need_low[5];                      // rows of LowDepth<k> required
+// Everything of a context that depends on the frame size: what the recorders read (frame_record.h FrameState) plus the band's
+// neighbours and row ranges and the state of the per-layer camera table slot.  A reserved context (meao_reserve) keeps one of these
+// per recently used size (MeaoCtx::size_slots) and swaps it in on a resize to that size, so a return to a planned size is host bookkeeping only.
+struct SizeState : FrameState {
+    int prev0 = -1, next1 = -1;             // the neighbour bands' extents (meao_set_row_band)
+    Range need_low[5];                      // rows of LowDepth<k> required by this band
     Range own_low[5];                       // rows of LowDepth<k> this band produces
-
-    Plan plan;
-    std::vector<CamConsts> layer_consts;    // the plan's camera constants of every layer (all alike without a layer-camera table)
     bool cam_table_stale = true;            // layer_consts changed since the device tables were written (ensure_ready uploads them)
-    // the per-layer camera tables of this size in arena slot `slot` (kernels.h LayerZ / LayerRender): layer_zb[l];
-    // layer_ren[(2 (k - 1) + wide) L + l]
-    int slot = 0;
-    LayerZ *layer_zb = nullptr;
-    LayerRender *layer_ren = nullptr;
+    int slot = 0;                           // the arena slot of this size's camera tables (FrameState::layer_zb / layer_ren)
     bool table_pending = false;             // the slot's tables are not written yet: the next frame writes them on its own stream
 };
 
@@ -110,7 +57,6 @@ struct SizeState {
 
 struct MeaoCtx : SizeState {
     int device = 0;
-    int sm_count = 132;                     // SMs of the device (set by meao_create; 132 = H100 SXM for plan-only contexts)
     bool plan_only = false;                 // device < 0: host-side planning only (no CUDA calls at all)
     uint32_t flags = 0;
     std::string error;
@@ -124,8 +70,6 @@ struct MeaoCtx : SizeState {
     std::vector<MeaoCamera> layer_cams;     // meao_set_layer_cameras: one camera per layer, or empty (every layer uses `camera`)
     MeaoVariants variants = {0, 0, 0, 0};
     bool plan_dirty = true;
-
-    int layers = 1;                         // meao_set_layers: every image holds `layers` same-size views stacked at a stride of one image
 
     // meao_reserve: the arena is laid out for res_w x res_h (0 x 0: for the current size) and every size inside it keeps its plan
     int res_w = 0, res_h = 0;
@@ -148,7 +92,6 @@ struct MeaoCtx : SizeState {
 
     // native neighbour exchange (meao_band_export / _connect / _step)
     BandFlags *band_flags = nullptr;        // first 256 bytes of the arena
-    uint32_t *tile_ctr = nullptr;           // 2 words per upsample level: tile cursor + finished-CTA count of the persistent blur_upsample grid (zero between launches)
     void *peer_base[2] = {nullptr, nullptr};    // the neighbours' arenas through a peer mapping (same layout as ours)
     bool peer_ipc[2] = {false, false};      // mapping came from cudaIpcOpenMemHandle (must be closed)
     unsigned long long band_timeout_ns = 2000000000ull;
@@ -222,8 +165,6 @@ int refuse_reserved(MeaoCtx *c, const char *what)
 float mathf_sqrt(float f) { return (float)std::sqrt((double)f); }
 float mathf_pow(float f, float p) { return (float)std::pow((double)f, (double)p); }
 
-float host_f16_round(float x) { return __half2float(__float2half_rn(x)); }
-
 // AO.cs:577-590
 void sample_thickness(float t[12])
 {
@@ -234,6 +175,9 @@ void sample_thickness(float t[12])
     t[8] = mathf_sqrt(1 - 0.4f * 0.4f - 0.4f * 0.4f);   t[9] = mathf_sqrt(1 - 0.4f * 0.4f - 0.6f * 0.6f);
     t[10] = mathf_sqrt(1 - 0.4f * 0.4f - 0.8f * 0.8f);  t[11] = mathf_sqrt(1 - 0.6f * 0.6f - 0.6f * 0.6f);
 }
+
+// Z direction of the context's cameras (meao_set_layer_cameras requires one for all layers)
+inline int ctx_reversed_z(const MeaoCtx *c) { return c->layer_cams.empty() ? c->camera.reversed_z : c->layer_cams[0].reversed_z; }
 
 // The camera-dependent constants of camera `cam` (the part of build_plan that reads the camera).
 void camera_consts(const MeaoCtx *c, const MeaoCamera &cam, CamConsts &p)
@@ -290,6 +234,8 @@ void build_plan(MeaoCtx *c)
     const CamConsts &cc = c->layer_consts[0];
     p.zb[0] = cc.zb[0]; p.zb[1] = cc.zb[1];
     p.zb[2] = p.zb[3] = 0;
+    p.variants = c->variants;
+    p.reversed_z = ctx_reversed_z(c);
     memcpy(p.inv_thickness, cc.inv_thickness, sizeof p.inv_thickness);
     memcpy(p.inv_thickness_wide, cc.inv_thickness_wide, sizeof p.inv_thickness_wide);
     memcpy(p.pad, cc.pad, sizeof p.pad);
@@ -430,54 +376,15 @@ inline int arena_h(const MeaoCtx *c) { return c->res_w > 0 ? c->res_h : c->H; }
 // tables in slot `slot`; encodes the TMA maps and resets the band to the whole frame.  Host work only: no allocation, no CUDA call.
 int place_size(MeaoCtx *c, int slot)
 {
-    const ArenaLayout a = arena_layout(c->W, c->H, c->layers);
-    memcpy(c->lw, a.lw, sizeof c->lw);
-    memcpy(c->lh, a.lh, sizeof c->lh);
     c->band0 = 0; c->band1 = c->H; c->prev0 = -1; c->next1 = -1;
     c->slot = slot;
-    c->lin_pitch = a.lin_pitch;
-    c->result_pitch = a.result_pitch;
-    for (int k = 1; k <= 4; k++) { c->low_pitch[k] = a.low_pitch[k]; c->occ_pitch[k] = a.occ_pitch[k]; }
+    place_frame(*c, arena_layout(c->W, c->H, c->layers), (char *)c->arena, slot);
     if (!c->arena) return setup_band(c);
-    char *b = (char *)c->arena;
-    c->lin = (__half *)(b + a.lin);
-    c->result = (uint8_t *)(b + a.result);
-    for (int k = 1; k <= 4; k++) {
-        c->low[k] = (float *)(b + a.low[k]);
-        c->occ[k] = (uint8_t *)(b + a.occ[k]);
-        if (k <= 3) c->comb[k] = (uint8_t *)(b + a.comb[k]);
-        c->hq[k] = (uint8_t *)(b + a.hq[k]);
-    }
-    c->layer_zb = (LayerZ *)(b + a.table0 + (size_t)slot * a.table_stride);
-    c->layer_ren = (LayerRender *)((char *)c->layer_zb + a.table_ren);
-
-    c->tma_ok = false;
-    if (c->encode) {
-        bool ok = true;
-        // one 2-D map over all layers: height L x lh (the kernels fetch a box only when it lies inside one layer); with one layer
-        // these are the single-image maps
-        for (int k = 1; k <= 4 && ok; k++) {
-            const int mh = c->layers * c->lh[k];
-            for (int t = 0; t < kRenderTileVariants; t++) {
-                ok &= make_map(c, &c->map_low_ren[t][k], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, c->low[k], c->lw[k], mh, c->low_pitch[k], kRenderBoxW, render_box_h(kRenderTileHs[t], false)) == 0;
-                ok &= make_map(c, &c->map_low_wide[t][k], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, c->low[k], c->lw[k], mh, c->low_pitch[k], kRenderWideBoxW, render_box_h(kRenderTileHs[t], true)) == 0;
-            }
-            ok &= make_map(c, &c->map_low_ups[k], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, c->low[k], c->lw[k], mh, c->low_pitch[k], kUpsDepthBoxW, kUpsDepthBoxH) == 0;
-            uint8_t *ao = (k == 4) ? c->occ[4] : c->comb[k];
-            ok &= make_map(c, &c->map_ao_ups[k], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, ao, c->lw[k], mh, c->occ_pitch[k], kUpsAoBoxW, kUpsAoBoxH) == 0;
-            ok &= make_map(c, &c->map_hq_ups[k], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, c->hq[k], c->lw[k], mh, c->occ_pitch[k], kUpsAoBoxW, kUpsAoBoxH) == 0;
-        }
-        ok &= make_map(c, &c->map_occ1_ups, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, c->occ[1], c->lw[1], c->layers * c->lh[1], c->occ_pitch[1], kUpsAoBoxW, kUpsAoBoxH) == 0;
-        c->tma_ok = ok;
-    }
-    if (!c->tma_ok) {
-        memset(&c->map_occ1_ups, 0, sizeof c->map_occ1_ups);
-        memset(c->map_low_ren, 0, sizeof c->map_low_ren);
-        memset(c->map_low_ups, 0, sizeof c->map_low_ups);
-        memset(c->map_ao_ups, 0, sizeof c->map_ao_ups);
-        memset(c->map_low_wide, 0, sizeof c->map_low_wide);
-        memset(c->map_hq_ups, 0, sizeof c->map_hq_ups);
-    }
+    c->tma_ok = c->encode && encode_maps(*c, [c](CUtensorMap &m, const MapSpec &sp) {
+        return make_map(c, &m, sp.elem == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT8, sp.elem, sp.base, sp.w, sp.h,
+                        sp.pitch_elems, sp.bw, sp.bh) == 0;
+    });
+    if (!c->tma_ok) memset(&c->maps, 0, sizeof c->maps);
     return setup_band(c);
 }
 
@@ -501,7 +408,6 @@ int allocate(MeaoCtx *c, bool keep_old = false)
         CUDA_TRY(c, cudaStreamSynchronize(c->stream));
         char *b = (char *)c->arena;
         c->band_flags = (BandFlags *)b;
-        c->tile_ctr = (uint32_t *)(b + a.ctr);          // zeroed by the memset above
         {
             BandFlags init{}; init.epoch = 1;
             CUDA_TRY(c, cudaMemcpy(c->band_flags, &init, sizeof init, cudaMemcpyHostToDevice));
@@ -544,47 +450,13 @@ int switch_size(MeaoCtx *c, int w, int h)
     return 0;
 }
 
-// The call-order tables of record_render: Render.compute:162-168 (checker) and :148-159 (exhaustive) table slots
-const int kIdxChecker[7] = {1, 3, 4, 8, 11, 6, 10};
-const int kIdxExh[12] = {0, 1, 2, 3, 4, 8, 11, 5, 6, 7, 9, 10};
-
-// The LayerRender entry of camera constants `cc` at render level k (wide: kernel "main"): what record_render puts into RenderArgs
-LayerRender layer_render(const MeaoCtx *c, const CamConsts &cc, int k, bool wide)
-{
-    const bool exh = c->variants.sample_exhaustively != 0;
-    const int n = exh ? 12 : 7;
-    const int *idx = exh ? kIdxExh : kIdxChecker;
-    const float *it = wide ? cc.inv_thickness_wide[k] : cc.inv_thickness[k];
-    LayerRender r{};
-    for (int i = 0; i < n; i++) {
-        r.it_nf[i].x = it[idx[i]];
-        r.it_nf[i].y = -(r.it_nf[i].x - 0.5f);                                                      // Render.compute:85
-    }
-    r.pad = host_f16_round(cc.pad[k]);
-    return r;
-}
-
-// The per-layer camera tables of the current plan, as they go into the arena
-void camera_tables(const MeaoCtx *c, std::vector<LayerZ> &zb, std::vector<LayerRender> &ren)
-{
-    const int L = c->layers;
-    zb.resize(L);
-    ren.resize((size_t)8 * L);
-    for (int l = 0; l < L; l++) {
-        const CamConsts &cc = c->layer_consts[l];
-        zb[l] = LayerZ{cc.zb[0], cc.zb[1]};
-        for (int k = 1; k <= 4; k++)
-            for (int w = 0; w < 2; w++) ren[(size_t)(2 * (k - 1) + w) * L + l] = layer_render(c, cc, k, w != 0);
-    }
-}
-
 // Write the per-layer camera tables to the arena.  Called by ensure_ready after a re-plan, once every frame that may read the old
 // tables has finished (a device synchronise: frames may be in flight on any caller stream).
 int upload_camera_tables(MeaoCtx *c)
 {
     std::vector<LayerZ> zb;
     std::vector<LayerRender> ren;
-    camera_tables(c, zb, ren);
+    camera_tables(*c, zb, ren);
     CUDA_TRY(c, cudaDeviceSynchronize());
     CUDA_TRY(c, cudaMemcpy(c->layer_zb, zb.data(), zb.size() * sizeof(LayerZ), cudaMemcpyHostToDevice));
     CUDA_TRY(c, cudaMemcpy(c->layer_ren, ren.data(), ren.size() * sizeof(LayerRender), cudaMemcpyHostToDevice));
@@ -602,7 +474,7 @@ int write_tables(MeaoCtx *c, cudaStream_t s)
     if (!c->table_pending) return 0;
     std::vector<LayerZ> zb;
     std::vector<LayerRender> ren;
-    camera_tables(c, zb, ren);
+    camera_tables(*c, zb, ren);
     CUDA_TRY(c, cudaMemcpyAsync(c->layer_zb, zb.data(), zb.size() * sizeof(LayerZ), cudaMemcpyHostToDevice, s));
     CUDA_TRY(c, cudaMemcpyAsync(c->layer_ren, ren.data(), ren.size() * sizeof(LayerRender), cudaMemcpyHostToDevice, s));
     c->table_pending = false;
@@ -636,67 +508,16 @@ int frame_ready(MeaoCtx *c, cudaStream_t s)
     return rc ? rc : write_tables(c, s);
 }
 
-// Z direction of the context's cameras (meao_set_layer_cameras requires one for all layers)
-inline int ctx_reversed_z(const MeaoCtx *c) { return c->layer_cams.empty() ? c->camera.reversed_z : c->layer_cams[0].reversed_z; }
-// The f16-rounded atlas padding value of layer l at render level k for depth kind `kind` (linear ingest pads with 0)
-inline float layer_pad(const MeaoCtx *c, int l, int k, int kind)
-{
-    return host_f16_round((kind != MEAO_DEPTH_LINEAR_F32) ? c->layer_consts[l].pad[k] : 0.0f);
-}
-
 struct NvtxRange { explicit NvtxRange(const char *n) { nvtxRangePushA(n); } ~NvtxRange() { nvtxRangePop(); } };
 
-// Tile-height variant (index into kRenderTileHs = {32, 16, 8}) of a render launch.  The big levels keep the 64 x 32 tile
-// (least apron overhead: throughput); a level whose grid would not even put one CTA on every SM is latency-bound -- one
-// CTA's serial time IS the kernel time -- so it takes the tallest tile that still gives at least one CTA per SM, else 64 x 8.
-// A layered launch counts the CTAs of all its layers.
-int render_tile_variant(const MeaoCtx *c, int k, int rows)
+// MEAO_REN_TILE = 0 / 1 / 2 forces a render tile variant for every level (a tuning aid); -1: the planner's rule
+int forced_render_tile()
 {
-    const char *force = getenv("MEAO_REN_TILE");               // tuning aid: 0 / 1 / 2 forces a variant for every level
-    if (force && force[0] >= '0' && force[0] < '0' + kRenderTileVariants) return force[0] - '0';
-    for (int t = 0; t < kRenderTileVariants; t++) {
-        const long long ctas = (long long)c->layers * ((c->lw[k] + 63) / 64) * ((rows + kRenderTileHs[t] - 1) / kRenderTileHs[t]);
-        if (ctas >= c->sm_count) return t;
-    }
-    return kRenderTileVariants - 1;
+    const char *force = getenv("MEAO_REN_TILE");
+    return (force && force[0] >= '0' && force[0] < '0' + kRenderTileVariants) ? force[0] - '0' : -1;
 }
 
-// ---- the three recorders ---------------------------------------------------------------------
-
-// A CUDA-array frame (meao_render_arrays): the surfaces of the depth and AO arrays and how their layers are addressed (surface_io.cuh).
-struct ArrayIO { cudaSurfaceObject_t depth, ao; int depth_surf, ao_surf; const void *ao_array; };
-
-// The byte pitches of the caller's depth and AO views (meao_render_pitched).  A view is `layers` images of rows [band0, band1) of
-// the frame, W pixels per row.
-struct ViewPitch { int64_t depth_row, depth_layer, ao_row, ao_layer; };
-inline int64_t depth_esize(int kind) { return kind == MEAO_DEPTH_RAW_D16_UNORM ? 2 : 4; }
-// meao_render's views: tight rows, tight layers
-ViewPitch tight_pitch(const MeaoCtx *c, int kind)
-{
-    const int64_t es = depth_esize(kind), rows = c->band1 - c->band0;
-    return ViewPitch{c->W * es, rows * c->W * es, c->W, rows * c->W};
-}
-
-// The caller's depth as the kernels read it: rows [band0, band1) of the frame of every layer, at the pitches of `vp` (nullptr: tight).
-DepthIn depth_in(const MeaoCtx *c, const void *depth, int kind, const ViewPitch *vp = nullptr)
-{
-    const ViewPitch p = vp ? *vp : tight_pitch(c, kind);
-    const int64_t es = depth_esize(kind);
-    DepthIn d{};
-    d.depth = depth;
-    d.in_format = (kind == MEAO_DEPTH_RAW_D16_UNORM) ? 1 : (kind == MEAO_DEPTH_RAW_D24S8 ? 2 : 0);
-    d.depth_row0 = c->band0;
-    d.zbx = c->plan.zb[0]; d.zby = c->plan.zb[1];
-    d.raw = (kind != MEAO_DEPTH_LINEAR_F32);
-    d.reversed_z = ctx_reversed_z(c);
-    // 128-bit loads: every row (and layer) start 16-byte aligned.  Tight views: W % 4 == 0 (4-byte kinds), W % 8 == 0 (D16)
-    d.vec_ok = (((uintptr_t)depth & 15) == 0) && (p.depth_row % 16 == 0) && (c->layers == 1 || p.depth_layer % 16 == 0);
-    d.depth_pitch = (int)(p.depth_row / es);
-    d.depth_layer_pitch = p.depth_layer / es;
-    d.ao_layer_pitch = p.ao_layer;
-    d.layer_zb = c->layer_zb;
-    return d;
-}
+// ---- the three recorders: frame_record.h's argument blocks and launcher choice, one launch each --------------------------------
 
 // PushDownsampleCommands, AO.cs:604-658.  aio: read the depth from a CUDA array instead of `depth`.  low_only: LowDepth1..4 only --
 // the frame's final upsample is recorded with the same depth (record_upsample's `fused`) and writes LinearDepth itself.
@@ -706,24 +527,8 @@ int record_downsample(MeaoCtx *c, const void *depth, int kind, cudaStream_t s, c
 {
     if (kind < MEAO_DEPTH_RAW_F32 || kind > MEAO_DEPTH_RAW_D24S8) return fail(c, MEAO_ERR_INVALID, "bad depth kind %d", kind);
     NvtxRange nv("meao::prepare_depth");
-    const DepthIn d = depth_in(c, depth, kind, vp);
-    PrepareArgs a{};
-    a.depth = depth;
-    a.in_format = d.in_format;
-    a.W = c->W; a.H = c->H;
-    a.depth_row0 = d.depth_row0;
-    a.row0 = c->band0; a.row1 = c->band1;
-    a.lin = c->lin; a.lin_pitch = c->lin_pitch;
-    for (int k = 1; k <= 4; k++) { a.low[k - 1] = c->low[k]; a.low_pitch[k - 1] = c->low_pitch[k]; }
-    a.zbx = d.zbx; a.zby = d.zby;
-    a.raw = d.raw;
-    a.reversed_z = d.reversed_z;
-    a.vec_ok = d.vec_ok;
-    a.depth_pitch = d.depth_pitch; a.depth_layer_pitch = d.depth_layer_pitch;
     c->last_kind = kind;
-    if (aio) CUDA_TRY(c, launch_prepare_depth_array(a, aio->depth, aio->depth_surf, c->layers, s, d.layer_zb));
-    else if (c->layers > 1) CUDA_TRY(c, launch_prepare_depth_layered(a, c->layers, s, low_only, d.layer_zb));
-    else CUDA_TRY(c, launch_prepare_depth(a, s, low_only));
+    CUDA_TRY(c, launch_prepare(*c, prepare_args(*c, depth_in(*c, depth, kind, vp)), aio, low_only, s));
     c->launches++;
     return 0;
 }
@@ -732,37 +537,11 @@ int record_downsample(MeaoCtx *c, const void *depth, int kind, cudaStream_t s, c
 // wide = true: the same recorder for the non-tiled source LowDepth<k> (kernel main) -> HighQuality<k>.
 int record_render(MeaoCtx *c, int k, int kind, cudaStream_t s, bool wide = false)
 {
-    const bool exh = c->variants.sample_exhaustively != 0;
-    const int n = exh ? 12 : 7;
-    const int *idx = exh ? kIdxExh : kIdxChecker;
     NvtxRange nv(wide ? "meao::render_ao_wide" : "meao::render_ao");
-    RenderArgs a{};
-    a.low = c->low[k]; a.lw = c->lw[k]; a.lh = c->lh[k]; a.lpitch = c->low_pitch[k];
-    a.occ = wide ? c->hq[k] : c->occ[k]; a.opitch = c->occ_pitch[k];
-    a.sw = c->lw[k + 2]; a.sh = c->lh[k + 2];
-    a.pad = host_f16_round((kind != MEAO_DEPTH_LINEAR_F32) ? c->plan.pad[k] : 0.0f);
-    const float *it = wide ? c->plan.inv_thickness_wide[k] : c->plan.inv_thickness[k];
-    for (int i = 0; i < n; i++) {
-        a.inv_thickness[i] = it[idx[i]];
-        a.neg_front[i] = -(a.inv_thickness[i] - 0.5f);                                               // Render.compute:85
-        a.weight[i] = c->plan.sample_weight[k][idx[i]];
-    }
-    a.reject_fadeoff = c->plan.reject_fadeoff;
-    a.intensity = c->plan.intensity;
-    a.row0 = c->need_c[k].lo; a.row1 = c->need_c[k].hi;
-    a.wide = wide ? 1 : 0;
-    a.exhaustive = exh ? 1 : 0;
-    const int tv = render_tile_variant(c, k, a.row1 - (a.row0 & ~3));
-    a.tile_h = kRenderTileHs[tv];
-    const CUtensorMap &map = wide ? c->map_low_wide[tv][k] : c->map_low_ren[tv][k];
-    if (c->layers > 1)
-        CUDA_TRY(c, launch_render_ao_layered(map, c->tma_ok, a, c->layers, s, c->layer_ren + (size_t)(2 * (k - 1) + (wide ? 1 : 0)) * c->layers,
-                                             kind != MEAO_DEPTH_LINEAR_F32 ? 1 : 0));
-    else CUDA_TRY(c, launch_render_ao(map, c->tma_ok, a, s));
+    CUDA_TRY(c, launch_render(*c, render_args(*c, k, kind, wide, forced_render_tile()), k, kind, s));
     c->launches++;
     return 0;
 }
-inline bool hq_level(const MeaoCtx *c, int k) { return ((c->variants.high_quality_mask >> (k - 1)) & 1) != 0; }
 
 // PushUpsampleCommands with the wiring of AO.cs:528-531.  aio (final level only): store the AO into a CUDA array instead of ao_out.
 // fused (final level only, with the frame's depth and kind): read and linearise the raw depth and write LinearDepth here, after a
@@ -770,40 +549,9 @@ inline bool hq_level(const MeaoCtx *c, int k) { return ((c->variants.high_qualit
 int record_upsample(MeaoCtx *c, int lo, void *ao_out, cudaStream_t s, const ArrayIO *aio = nullptr, const DepthIn *fused = nullptr,
                     const ViewPitch *vp = nullptr)
 {
-    const int hi = lo - 1;
     NvtxRange nv("meao::blur_upsample");
-    const bool single = c->variants.single_scale != 0 && lo == 1;      // LoResAO1 = Occlusion1: no coarser level contributes
-    UpsampleArgs a{};
-    a.lo_depth = c->low[lo]; a.low = c->lw[lo]; a.loh = c->lh[lo]; a.lo_dpitch = c->low_pitch[lo];
-    a.lo_ao = single ? c->occ[1] : (lo == 4) ? c->occ[4] : c->comb[lo]; a.lo_apitch = c->occ_pitch[lo];
-    if (hi == 0) { a.hi_depth = c->lin; a.hi_is_half = 1; a.hi_dpitch = c->lin_pitch; a.hi_ao = nullptr; a.hi_apitch = 0; }
-    else { a.hi_depth = c->low[hi]; a.hi_is_half = 0; a.hi_dpitch = c->low_pitch[hi]; a.hi_ao = c->occ[hi]; a.hi_apitch = c->occ_pitch[hi]; }
-    if (hi == 0) {
-        if (ao_out) { a.out = (uint8_t *)ao_out; a.out_pitch = vp ? (int)vp->ao_row : c->W; a.out_row_origin = c->band0; }
-        else { a.out = c->result; a.out_pitch = c->result_pitch; a.out_row_origin = 0; }
-        c->last_out = aio ? const_cast<void *>(aio->ao_array) : ao_out;
-    } else { a.out = c->comb[hi]; a.out_pitch = c->occ_pitch[hi]; a.out_row_origin = 0; }
-    // 64-bit stores: every row (and, in the caller's layered AO, layer) start 8-byte aligned.  A tight AO: W % 8 == 0
-    a.out_vec_ok = (((uintptr_t)a.out & 7) == 0) && (a.out_pitch % 8 == 0) && !(vp && ao_out && c->layers > 1 && vp->ao_layer % 8 != 0);
-    a.hiw = c->lw[hi]; a.hih = c->lh[hi];
-    a.noise_filter_strength = c->plan.noise_filter_strength[lo];
-    a.step_size = c->plan.step_size[lo];
-    a.blur_tolerance = c->plan.blur_tolerance[lo];
-    a.upsample_tolerance = c->plan.upsample_tolerance[lo];
-    a.fast_div_ok = upsample_fast_div_ok(a.upsample_tolerance, a.noise_filter_strength);
-    a.row0 = c->need_c[hi].lo; a.row1 = c->need_c[hi].hi;
-    a.tile_ctr = c->tile_ctr + 2 * (lo - 1);
-    const uint8_t *lo_ao2 = hq_level(c, lo) ? c->hq[lo] : nullptr;                   // kernels main_premin / main_premin_blendout
-    const CUtensorMap &ao_map = single ? c->map_occ1_ups : c->map_ao_ups[lo];
-    if (fused && hi == 0)
-        CUDA_TRY(c, launch_blur_upsample_lin(c->map_low_ups[lo], ao_map, &c->map_hq_ups[lo], c->tma_ok, a, lo_ao2, c->occ_pitch[lo], *fused, c->layers,
-                                             c->sm_count, s));
-    else if (aio && hi == 0)
-        CUDA_TRY(c, launch_blur_upsample_array(c->map_low_ups[lo], ao_map, &c->map_hq_ups[lo], c->tma_ok, a, lo_ao2, c->occ_pitch[lo], c->layers, c->sm_count,
-                                               aio->ao, aio->ao_surf, s));
-    else if (c->layers > 1)
-        CUDA_TRY(c, launch_blur_upsample_layered(c->map_low_ups[lo], ao_map, &c->map_hq_ups[lo], c->tma_ok, a, lo_ao2, c->occ_pitch[lo], c->layers, c->sm_count, s));
-    else CUDA_TRY(c, launch_blur_upsample(c->map_low_ups[lo], ao_map, &c->map_hq_ups[lo], c->tma_ok, a, lo_ao2, c->occ_pitch[lo], c->sm_count, s));
+    if (lo == 1) c->last_out = aio ? const_cast<void *>(aio->ao_array) : ao_out;
+    CUDA_TRY(c, launch_upsample(*c, lo, upsample_args(*c, lo, ao_out, vp), aio, fused, s));
     c->launches++;
     return 0;
 }
@@ -826,7 +574,7 @@ int record_frame_dag(MeaoCtx *c, const void *depth, int kind, void *ao_out, cuda
 {
     int rc;
     const bool fused = depth && !aio;
-    const DepthIn din = depth_in(c, depth, kind, vp);
+    const DepthIn din = depth_in(*c, depth, kind, vp);
     const DepthIn *fin = fused ? &din : nullptr;
     if (c->variants.single_scale) {     // BASELINE.json configs[0]: Downsample1 -> Render level 1 -> final-style Upsample on Occlusion1
         if (do_prepare && (rc = record_downsample(c, depth, kind, s, aio, fused, vp))) return rc;
@@ -842,15 +590,15 @@ int record_frame_dag(MeaoCtx *c, const void *depth, int kind, void *ao_out, cuda
     CUDA_TRY(c, cudaStreamWaitEvent(b3, c->ev[0], 0));
     // the optional high-quality render of a level (kernel "main") rides on the branch of that level's interleaved render
     { PdlScope p(pdl >= 1 && !after_exchange); if ((rc = record_render(c, 1, kind, s))) return rc; }
-    { PdlScope p(pdl >= 1); if (hq_level(c, 1) && (rc = record_render(c, 1, kind, s, true))) return rc; }
+    { PdlScope p(pdl >= 1); if (hq_level(*c, 1) && (rc = record_render(c, 1, kind, s, true))) return rc; }
     if ((rc = record_render(c, 2, kind, b1))) return rc;
-    { PdlScope p(pdl >= 1); if (hq_level(c, 2) && (rc = record_render(c, 2, kind, b1, true))) return rc; }
+    { PdlScope p(pdl >= 1); if (hq_level(*c, 2) && (rc = record_render(c, 2, kind, b1, true))) return rc; }
     CUDA_TRY(c, cudaEventRecord(c->ev[1], b1));
     if ((rc = record_render(c, 3, kind, b2))) return rc;
-    { PdlScope p(pdl >= 1); if (hq_level(c, 3) && (rc = record_render(c, 3, kind, b2, true))) return rc; }
+    { PdlScope p(pdl >= 1); if (hq_level(*c, 3) && (rc = record_render(c, 3, kind, b2, true))) return rc; }
     CUDA_TRY(c, cudaEventRecord(c->ev[2], b2));
     if ((rc = record_render(c, 4, kind, b3))) return rc;
-    { PdlScope p(pdl >= 1); if (hq_level(c, 4) && (rc = record_render(c, 4, kind, b3, true))) return rc; }
+    { PdlScope p(pdl >= 1); if (hq_level(*c, 4) && (rc = record_render(c, 4, kind, b3, true))) return rc; }
     CUDA_TRY(c, cudaStreamWaitEvent(b3, c->ev[2], 0));
     { PdlScope p(pdl >= 2); if ((rc = record_upsample(c, 4, nullptr, b3))) return rc; }
     CUDA_TRY(c, cudaStreamWaitEvent(b3, c->ev[1], 0));
@@ -874,13 +622,13 @@ int record_frame(MeaoCtx *c, const void *depth, int kind, void *ao_out, cudaStre
     const int reps = profile ? c->profile_repeats : 1;         // every kernel is idempotent (out of place), so repeating it is harmless
     int rc = 0;
     mark();
-    const DepthIn din = depth_in(c, depth, kind, vp);      // the fused form of record_frame_dag
+    const DepthIn din = depth_in(*c, depth, kind, vp);      // the fused form of record_frame_dag
     for (int r = 0; r < reps && !rc; r++) rc = record_downsample(c, depth, kind, s, nullptr, true, vp);
     if (rc) return rc;
     names.push_back("prepare_depth"); mark();
     const int kmax = c->variants.single_scale ? 1 : 4;       // single-scale: Render level 1 + the final-style Upsample only
     for (int k = 1; k <= kmax; k++) { for (int r = 0; r < reps && !rc; r++) rc = record_render(c, k, kind, s); if (rc) return rc; names.push_back(ren_names[k]); mark(); }
-    for (int k = 1; k <= kmax; k++) if (hq_level(c, k)) { for (int r = 0; r < reps && !rc; r++) rc = record_render(c, k, kind, s, true); if (rc) return rc; names.push_back(hq_names[k]); mark(); }
+    for (int k = 1; k <= kmax; k++) if (hq_level(*c, k)) { for (int r = 0; r < reps && !rc; r++) rc = record_render(c, k, kind, s, true); if (rc) return rc; names.push_back(hq_names[k]); mark(); }
     for (int lo = kmax; lo >= 1; lo--) { for (int r = 0; r < reps && !rc; r++) rc = record_upsample(c, lo, lo == 1 ? ao_out : nullptr, s, nullptr, lo == 1 ? &din : nullptr, vp); if (rc) return rc; names.push_back(ups_names[lo]); mark(); }
     if (profile) {
         CUDA_TRY(c, cudaStreamSynchronize(s));
@@ -1339,7 +1087,7 @@ int meao_render_band_finish(MeaoCtx *c, void *ao_out, void *stream)
     cudaStream_t s = (cudaStream_t)stream;
     const int kind = c->last_kind;
     for (int k = 1; k <= 4; k++) if ((rc = record_render(c, k, kind, s))) return rc;
-    for (int k = 1; k <= 4; k++) if (hq_level(c, k) && (rc = record_render(c, k, kind, s, true))) return rc;
+    for (int k = 1; k <= 4; k++) if (hq_level(*c, k) && (rc = record_render(c, k, kind, s, true))) return rc;
     for (int lo = 4; lo >= 1; lo--) if ((rc = record_upsample(c, lo, lo == 1 ? ao_out : nullptr, s))) return rc;
     return MEAO_OK;
 }
@@ -1692,7 +1440,7 @@ int check_views(MeaoCtx *c, const void *depth, int kind, const void *ao_out, Vie
             return fail(c, MEAO_ERR_INVALID, "ao_layer_pitch %lld is below (rows - 1) x row pitch + width = %lld: layers would overlap",
                         (long long)p->ao_layer, (long long)amin);
     } else {
-        const ViewPitch t = tight_pitch(c, kind);
+        const ViewPitch t = tight_pitch(*c, kind);
         p->depth_layer = t.depth_layer; p->ao_layer = t.ao_layer;
     }
     // The depth is read through the non-coherent path (ld.global.nc), so an AO view that shares bytes with it is undefined.  The test
@@ -1730,7 +1478,7 @@ int render_views(MeaoCtx *c, const void *depth, int kind, void *ao_out, ViewPitc
 int meao_render(MeaoCtx *c, const void *depth, int32_t kind, void *ao_out, void *stream)
 {
     int rc = frame_ready(c, (cudaStream_t)stream); if (rc) return rc;
-    return render_views(c, depth, kind, ao_out, tight_pitch(c, kind), stream);      // meao_render_pitched at the tight pitches
+    return render_views(c, depth, kind, ao_out, tight_pitch(*c, kind), stream);      // meao_render_pitched at the tight pitches
 }
 
 int meao_render_pitched(MeaoCtx *c, const void *depth, int64_t depth_row_pitch, int64_t depth_layer_pitch, int32_t kind,
@@ -1961,7 +1709,7 @@ int meao_get_buffer(MeaoCtx *c, int32_t id, void *host_out, size_t host_bytes)
         cudaError_t e = cudaSuccess;
         for (int l = 0; l < c->layers && e == cudaSuccess; l++)
             e = launch_synth_tiled(c->low[k] + (size_t)l * c->lh[k] * c->low_pitch[k], c->lw[k], c->lh[k], c->low_pitch[k], c->lw[k + 2], c->lh[k + 2],
-                                   layer_pad(c, l, k, c->last_kind), (__half *)((char *)tmp + l * one), c->stream);
+                                   layer_pad(*c, l, k, c->last_kind), (__half *)((char *)tmp + l * one), c->stream);
         if (e == cudaSuccess) e = cudaMemcpyAsync(host_out, tmp, need, cudaMemcpyDeviceToHost, c->stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
         cudaFree(tmp);
@@ -1996,7 +1744,7 @@ int meao_debug_view(MeaoCtx *c, int32_t id, void *out, void *stream)
         const int k = id - 5;
         a.tiled = 1; a.src = c->low[k]; a.elem = 4; a.spitch = c->low_pitch[k];
         a.sw = c->lw[k + 2]; a.sh = c->lh[k + 2]; a.lw = c->lw[k]; a.lh = c->lh[k];
-        a.pad = layer_pad(c, 0, k, c->last_kind);
+        a.pad = layer_pad(*c, 0, k, c->last_kind);
     } else {                                                        // AO.cs:815-819
         if (id == MEAO_BUF_AMBIENT_OCCLUSION && c->last_out) {
             // the last frame wrote the AO texture straight into the caller's buffer: regenerate the context's own copy
@@ -2014,7 +1762,7 @@ int meao_debug_view(MeaoCtx *c, int32_t id, void *out, void *stream)
         DebugViewArgs al = a;
         al.src = (const char *)a.src + l * src_layer;
         al.out = a.out + (size_t)l * c->W * c->H;
-        if (slices == 16) al.pad = layer_pad(c, l, id - 5, c->last_kind);     // the layer's camera
+        if (slices == 16) al.pad = layer_pad(*c, l, id - 5, c->last_kind);     // the layer's camera
         CUDA_TRY(c, launch_debug_view(al, s));
         c->launches++;
     }
@@ -2206,7 +1954,7 @@ int meao_kernels_per_frame(const MeaoCtx *c)
 {
     if (c && c->variants.single_scale) return 3;      // Downsample1 + Render level 1 + the final-style Upsample
     int n = 9;
-    if (c) for (int k = 1; k <= 4; k++) n += hq_level(c, k) ? 1 : 0;
+    if (c) for (int k = 1; k <= 4; k++) n += (c->variants.high_quality_mask >> (k - 1)) & 1;     // as set: the plan may not be rebuilt yet
     return n;
 }
 

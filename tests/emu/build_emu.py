@@ -1,15 +1,26 @@
-"""Builds tests/emu/libmeao_emu.so: the kernel SOURCES of miniengineao_b200/csrc compiled by g++ for the host
-(-DMEAO_EMULATE) plus the fiber runtime and the frame driver.  TEST INFRASTRUCTURE ONLY (see cuda_emu.h)."""
+"""Builds tests/emu/libmeao_emu.so: the kernel translation units libmeao.so is built from (miniengineao_b200/build.py SOURCES, less the
+context and the GPU self test) compiled by g++ for the host (-DMEAO_EMULATE), with the fiber runtime and the frame driver.  TEST
+INFRASTRUCTURE ONLY (see cuda_emu.h).
+
+The build goes through a private temporary directory and an atomic rename, so test processes that build it at the same time never
+see a half-written library."""
 from __future__ import annotations
 
 import os
+import shutil
 import subprocess
 import sys
+import tempfile
+from concurrent.futures import ThreadPoolExecutor
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-CSRC = os.path.join(os.path.dirname(os.path.dirname(HERE)), "miniengineao_b200", "csrc")
+ROOT = os.path.dirname(os.path.dirname(HERE))
+sys.path.insert(0, ROOT)
+from miniengineao_b200.build import SOURCES  # noqa: E402
+
+CSRC = os.path.join(ROOT, "miniengineao_b200", "csrc")
 LIB = os.path.join(HERE, "libmeao_emu.so")
-KERNELS = ["prepare_depth.cu", "render_ao.cu", "blur_upsample.cu", "debug_view.cu", "composite.cu", "halo.cu", "band_exchange.cu"]
+KERNELS = [s for s in SOURCES if s not in ("meao_api.cu", "selftest.cu")]
 FLAGS = ["-std=c++17", "-O1", "-ffp-contract=off", "-fPIC", "-DMEAO_EMULATE", "-I", HERE, "-Wno-unknown-pragmas", "-Wno-unused-function"]
 
 
@@ -24,19 +35,29 @@ def is_stale() -> bool:
 def build(force: bool = False) -> str:
     if not force and not is_stale():
         return LIB
-    objs = []
-    for src, lang in [(os.path.join(HERE, "emu_runtime.cpp"), []), (os.path.join(HERE, "emu_driver.cpp"), [])] + \
-                     [(os.path.join(CSRC, k), ["-x", "c++"]) for k in KERNELS]:
-        obj = os.path.join(HERE, f"libmeao_emu_{os.path.basename(src)}.o")
-        cmd = ["g++"] + FLAGS + lang + ["-c", src, "-o", obj]
-        p = subprocess.run(cmd, capture_output=True, text=True)
-        if p.returncode != 0:
-            sys.stderr.write(p.stdout + p.stderr)
-            raise RuntimeError(f"emulator build failed: {os.path.basename(src)}")
-        objs.append(obj)
-    subprocess.check_call(["g++", "-shared", "-o", LIB] + objs)
-    for o in objs:
-        os.remove(o)
+    tmp = tempfile.mkdtemp(prefix="meao_emu_")
+    try:
+        srcs = [(os.path.join(HERE, "emu_runtime.cpp"), []), (os.path.join(HERE, "frame_driver.cpp"), [])] + \
+               [(os.path.join(CSRC, k), ["-x", "c++"]) for k in KERNELS]
+
+        def compile_one(src_lang):
+            src, lang = src_lang
+            obj = os.path.join(tmp, os.path.basename(src) + ".o")
+            p = subprocess.run(["g++"] + FLAGS + lang + ["-c", src, "-o", obj], capture_output=True, text=True)
+            if p.returncode != 0:
+                sys.stderr.write(p.stdout + p.stderr)
+                raise RuntimeError(f"emulator build failed: {os.path.basename(src)}")
+            return obj
+
+        with ThreadPoolExecutor(max_workers=os.cpu_count() or 1) as pool:
+            objs = list(pool.map(compile_one, srcs))
+        out = os.path.join(tmp, "lib.so")
+        subprocess.check_call(["g++", "-shared", "-Wl,-Bsymbolic", "-o", out] + objs)
+        staged = f"{LIB}.tmp{os.getpid()}"
+        shutil.copyfile(out, staged)            # the temporary directory may be on another file system
+        os.replace(staged, LIB)
+    finally:
+        shutil.rmtree(tmp, ignore_errors=True)
     return LIB
 
 

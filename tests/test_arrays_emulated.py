@@ -1,7 +1,7 @@
 """CPU tests of CUDA-array frames (meao_render_arrays): the depth read from, the AO written into a 2-D, layered or cube-map CUDA array.
 
 The array kernel sources (csrc/prepare_depth_array.cu, csrc/blur_upsample_array.cu) run in the fiber emulator with emulated arrays and
-surface objects (tests/emu/arrays_emu.py); every layer's AO, LinearDepth and LowDepth1..4 must be bit-identical to the oracle run on
+surface objects (tests/emu/frame_driver.cpp); every layer's AO, LinearDepth and LowDepth1..4 must be bit-identical to the oracle run on
 that layer alone.  The emulated arrays have rows wider than the image with a marker in the spare bytes, and refuse any access that is
 not one element at an element boundary, of the wrong shape, or out of range in trap mode.  Also here: the packed-contraction audit of
 the array translation units and the plan-only contract of the three new entry points."""
@@ -17,7 +17,7 @@ import pytest
 from miniengineao_b200 import _native as N
 from oracle.oracle import Oracle
 
-from emu.arrays_emu import ArrayFrame  # noqa: E402  (tests/ is on sys.path via conftest)
+from emu.emu import Frame  # noqa: E402  (tests/ is on sys.path via conftest)
 from test_layers_emulated import _plan, _raw, contrasting_layers  # noqa: E402
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -31,7 +31,7 @@ def _d16(raw):
 
 def _run_arrays(W, H, depth, *, depth_shape, ao_shape=None, linear=False, single_scale=False, oracle_depth=None, **kw):
     L = depth.shape[0]
-    f = ArrayFrame(_plan(W, H, L, single_scale=single_scale, **kw), linear=linear)
+    f = Frame(_plan(W, H, L, single_scale=single_scale, **kw), linear=linear)
     n0 = f.surface_accesses()
     ao = f.run_arrays(depth, depth_shape, ao_shape)
     assert f.surface_accesses() - n0 >= 2 * L * W * H          # every depth element loaded, every AO byte stored
@@ -105,7 +105,7 @@ def test_interior_tiles_take_the_tma_path():
     """Big enough for TMA-fed interior tiles in the final level: the array kernel keeps the layered tile loop's box loads."""
     W, H = 640, 360
     depth = _raw(contrasting_layers(W, H, 2, seed=3))
-    f = ArrayFrame(_plan(W, H, 2))
+    f = Frame(_plan(W, H, 2))
     n0 = f.tma_box_loads()
     ao = f.run_arrays(depth, "layered")
     assert f.tma_box_loads() - n0 > 300

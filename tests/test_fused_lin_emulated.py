@@ -1,11 +1,10 @@
 """CPU tests of the fused frame: prepare_depth in its low-only form (LowDepth1..4 from the even depth rows, no LinearDepth) and the
 final blur_upsample reading the raw depth, linearising it and writing LinearDepth itself (csrc/blur_upsample_lin.cu).
 
-The kernel sources run in the fiber emulator (tests/emu/lin_driver.cpp) and every buffer must be bit-identical to the oracle's: the
+The kernel sources run in the fiber emulator (tests/emu/frame_driver.cpp) and every buffer must be bit-identical to the oracle's: the
 depth kinds, both Z directions, widths and depth pointers that rule out the 128-bit loads, sky patches (the grouped range test falls
 back), premin, single-scale, layered frames and a row band.  LinearDepth is poisoned with NaN first, so every element the frame does
 not write shows.  Also here: the packed-contraction audit of the new translation unit."""
-import ctypes as C
 import os
 import re
 import shutil
@@ -14,89 +13,21 @@ import subprocess
 import numpy as np
 import pytest
 
-from miniengineao_b200 import _native as N
 from miniengineao_b200 import synth
 from oracle.oracle import Oracle
 
-from emu import build_lin_emu  # noqa: E402  (tests/ is on sys.path via conftest)
-from emu.emu import linearize_zero
+from emu.emu import Frame  # noqa: E402  (tests/ is on sys.path via conftest)
 from test_layers_emulated import _compare_layer, _plan, contrasting_layers
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "miniengineao_b200", "csrc")
 
-_lib = None
 
-
-def lib():
-    global _lib
-    if _lib is None:
-        l = C.CDLL(build_lin_emu.build())
-        l.lemu_create.restype = C.c_void_p
-        l.lemu_create.argtypes = [C.c_int, C.c_int, C.c_int]
-        l.lemu_destroy.argtypes = [C.c_void_p]
-        l.lemu_set_constants.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float] + [C.c_int] * 6
-        l.lemu_get_buffer.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
-        l.femu_poison_lin.argtypes = [C.c_void_p]
-        l.femu_prepare_low.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
-        l.femu_run.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
-        _lib = l
-    return _lib
-
-
-class FusedFrame:
-    """One frame in the fused form, planned by a plan-only libmeao context (device = -1); the set-up of emu.layered_emu.LayeredFrame."""
-
-    def __init__(self, plan, *, linear=False):
-        self._lib = lib()
-        plan.LateUpdate()
-        self.plan = plan
-        self.W, self.H, self.layers = plan._width, plan._height, int(plan.layers)
-        nl = N.lib()
-        rc, rcw, uc, zb = (C.c_float * 112)(), (C.c_float * 112)(), (C.c_float * 32)(), (C.c_float * 4)()
-        for k in range(1, 5):
-            N.check(plan._ctx, nl.meao_render_constants(plan._ctx, k, C.cast(C.byref(rc, 112 * (k - 1)), C.POINTER(C.c_float))))
-            N.check(plan._ctx, nl.meao_render_constants_wide(plan._ctx, k, C.cast(C.byref(rcw, 112 * (k - 1)), C.POINTER(C.c_float))))
-            N.check(plan._ctx, nl.meao_upsample_constants(plan._ctx, k, C.cast(C.byref(uc, 32 * (k - 1)), C.POINTER(C.c_float))))
-        N.check(plan._ctx, nl.meao_zbuffer_params(plan._ctx, zb))
-        rz = bool(plan.camera.usesReversedZBuffer)
-        pad12 = 0.0 if linear else (1e5 if rz else linearize_zero(zb))
-        self._h = self._lib.lemu_create(self.W, self.H, self.layers)
-        self._lib.lemu_set_constants(self._h, rc, rcw, uc, zb, pad12, int(not linear), int(rz), int(plan.highQualityMask),
-                                     int(plan.sampleExhaustively), int(plan.singleScale), 1)
-        self._lib.femu_poison_lin(self._h)
-
-    def __del__(self):
-        if getattr(self, "_h", None):
-            self._lib.lemu_destroy(self._h)
-            self._h = None
-
-    @staticmethod
-    def _input(depth, offset):
-        """C-contiguous copy `offset` bytes past a 64-byte boundary (offset 4: the depth pointer is not 16-byte aligned)."""
-        raw = np.empty(depth.nbytes + 128, np.uint8)
-        off = (-raw.ctypes.data) % 64 + offset
-        out = raw[off:off + depth.nbytes].view(depth.dtype).reshape(depth.shape)
-        out[...] = depth
-        return out
-
-    def run(self, depth, *, offset=0, rows=(0, 0)):
-        fmt = {"float32": 0, "uint16": 1, "uint32": 2}[depth.dtype.name]
-        d = self._input(np.ascontiguousarray(depth), offset)
-        self._lib.femu_run(self._h, d.ctypes.data, fmt, rows[0], rows[1])
-
-    def prepare_low(self, depth):
-        fmt = {"float32": 0, "uint16": 1, "uint32": 2}[depth.dtype.name]
-        d = self._input(np.ascontiguousarray(depth), 0)
-        self._lib.femu_prepare_low(self._h, d.ctypes.data, fmt)
-
-    def buffer(self, bid, layer=0):
-        d = self.plan.buffer_desc(bid)
-        dt = {1: np.uint8, 2: np.float16, 4: np.float32}[d.elem_bytes]
-        shape = (d.slices, d.height, d.width) if d.slices > 1 else (d.height, d.width)
-        out = np.zeros(shape, dt)
-        assert self._lib.lemu_get_buffer(self._h, bid, layer, out.ctypes.data) == 0
-        return out
+def fused_frame(plan, **kw):
+    """A Frame whose LinearDepth is NaN first, so every element the fused frame does not write shows."""
+    f = Frame(plan, **kw)
+    f.poison_lin()
+    return f
 
 
 def _raw_with_sky(W, H, seed, reversed_z=True):
@@ -130,8 +61,8 @@ def test_fused_frame_equals_oracle(W, H, kind):
     rz = (W * H) % 2 == 1
     raw = synth.random_depth(W, H, seed=W + H).astype(np.float32) if kind == "linear" else _raw_with_sky(W, H, W + H, rz)
     depth, seen = _ingest(raw, kind)
-    f = FusedFrame(_plan(W, H, reversed_z=rz, intensity=1.1), linear=(kind == "linear"))
-    f.run(depth)
+    f = fused_frame(_plan(W, H, reversed_z=rz, intensity=1.1), linear=(kind == "linear"))
+    f.run_fused(depth)
     _check(f, seen, f"{kind} {W}x{H}", intensity=1.1, reversed_z=rz, depth_is_linear=(kind == "linear"))
 
 
@@ -140,8 +71,8 @@ def test_unaligned_depth_pointer(kind):
     """vec_ok false although W % 8 == 0: the depth pointer is 4 bytes past a 16-byte boundary."""
     W, H = 136, 72
     depth, seen = _ingest(_raw_with_sky(W, H, 2), kind)
-    f = FusedFrame(_plan(W, H, intensity=1.1))
-    f.run(depth, offset=4)
+    f = fused_frame(_plan(W, H, intensity=1.1))
+    f.run_fused(depth, offset=4)
     _check(f, seen, f"unaligned {kind}", intensity=1.1)
 
 
@@ -149,8 +80,8 @@ def test_unaligned_depth_pointer(kind):
 def test_fused_variants(kw):
     W, H = 250, 131
     raw = _raw_with_sky(W, H, 5)
-    f = FusedFrame(_plan(W, H, intensity=1.1, **kw))
-    f.run(raw)
+    f = fused_frame(_plan(W, H, intensity=1.1, **kw))
+    f.run_fused(raw)
     _check(f, raw, str(kw), intensity=1.1, **kw)
 
 
@@ -160,8 +91,8 @@ def test_fused_layered(layers):
     lin = contrasting_layers(W, H, layers, seed=layers)
     raw = np.stack([synth.lin01_to_raw(l) for l in lin]).astype(np.float32)
     raw[min(2, layers - 1), H // 4: H // 2, W // 5: W // 2] = 0.0
-    f = FusedFrame(_plan(W, H, layers, intensity=1.1, high_quality_mask=1))
-    f.run(raw)
+    f = fused_frame(_plan(W, H, layers, intensity=1.1, high_quality_mask=1))
+    f.run_fused(raw)
     for l in range(layers):
         _check(f, raw[l], f"layer {l}", layer=l, intensity=1.1, high_quality_mask=1)
 
@@ -170,8 +101,8 @@ def test_fused_row_band():
     """The final level's rows [32, 96) through the fused kernel with the band's own depth rows (depth_row0 = 32)."""
     W, H = 161, 130
     raw = _raw_with_sky(W, H, 8)
-    f = FusedFrame(_plan(W, H, intensity=1.1))
-    f.run(raw, rows=(32, 96))
+    f = fused_frame(_plan(W, H, intensity=1.1))
+    f.run_fused(raw, rows=(32, 96))
     ref = Oracle(W, H, threads=4, intensity=1.1).run(raw)
     assert np.array_equal(f.buffer(17)[32:96], ref[32:96])
 
@@ -183,14 +114,14 @@ def test_low_only_prepare_writes_no_linear_depth_and_reads_only_even_rows():
     raw = _raw_with_sky(W, H, 4)
     odd_nan = raw.copy()
     odd_nan[1::2] = np.nan
-    f = FusedFrame(_plan(W, H, intensity=1.1))
+    f = fused_frame(_plan(W, H, intensity=1.1))
     f.prepare_low(odd_nan)
     assert np.isnan(f.buffer(1).astype(np.float32)).all()
     orc = Oracle(W, H, threads=4, intensity=1.1)
     orc.run(raw)
     for bid in (2, 3, 4, 5):
         assert np.array_equal(f.buffer(bid).view(np.uint32), orc.buffer(bid).view(np.uint32)), bid
-    f.run(raw)
+    f.run_fused(raw)
     assert np.array_equal(f.buffer(1).view(np.uint16), orc.buffer(1).astype(np.float16).view(np.uint16))
 
 

@@ -15,12 +15,9 @@ from oracle import direct_formulation as DF
 from oracle.oracle import Oracle
 
 import hostile_cases as HC
-from emu.arrays_emu import ArrayFrame
-from emu.emu import EmulatedFrame
-from emu.layered_emu import LayeredFrame
-from test_fused_lin_emulated import FusedFrame
-from test_layer_cameras_emulated import CamFrame
-from test_pitched_emulated import SENTINEL, PitchedFrame, View
+from emu.emu import Frame
+from test_fused_lin_emulated import fused_frame
+from test_pitched_emulated import SENTINEL, View
 
 PARAMS = {"noise_filter_tolerance": "noiseFilterTolerance", "blur_tolerance": "blurTolerance", "upsample_tolerance": "upsampleTolerance",
           "thickness_modifier": "thicknessModifier", "intensity": "intensity"}
@@ -52,7 +49,7 @@ def _check(get, W, H, cam, seen, tag, *, linear=False, high_quality_mask=0, sing
 
 
 def _whole(cam, depth, seen, tag, *, linear=False, use_tma=True, **kw):
-    f = EmulatedFrame(_plan(cam, **kw), linear=linear, use_tma=use_tma)
+    f = Frame(_plan(cam, **kw), linear=linear, use_tma=use_tma)
     f.run(depth)
     _check(f.buffer, cam.pixelWidth, cam.pixelHeight, cam, seen, tag, linear=linear, **kw)
 
@@ -107,8 +104,8 @@ def test_fused_frame_hostile(kind):
         depth = seen = HC.hostile_raw(W0, H0, _zb(cam), rz, seed=7)
     else:
         depth, seen = HC.hostile_unorm(W0, H0, 16 if kind == "d16" else 24, rz, seed=7)
-    f = FusedFrame(_plan(cam), linear=kind == "linear")
-    f.run(depth)
+    f = fused_frame(_plan(cam), linear=kind == "linear")
+    f.run_fused(depth)
     _check(f.buffer, W0, H0, cam, seen, f"fused {kind}", linear=kind == "linear")
 
 
@@ -128,8 +125,8 @@ def test_extreme_camera_as_one_layer_of_a_batch(name):
     W, H = 136, 72
     cams = [Camera(W, H, nearClipPlane=0.1, farClipPlane=50.0), HC.camera(name, W, H, True), Camera(W, H, nearClipPlane=1.0, farClipPlane=1000.0)]
     depth = np.stack([HC.hostile_raw(W, H, _zb(c), True, seed=20 + l) for l, c in enumerate(cams)])
-    f = CamFrame(_plan(Camera(W, H), 3, layer_cameras=cams))
-    f.run(depth)
+    f = Frame(_plan(Camera(W, H), 3, layer_cameras=cams))
+    f.run_fused(depth)
     for l, c in enumerate(cams):
         _check(lambda bid: f.buffer(bid, l), W, H, c, depth[l], f"batch {name} layer {l}")
 
@@ -163,7 +160,7 @@ def test_variants_hostile(kw):
     if stereo:
         p.OnPreRender()                     # one draw for both eyes
     d = HC.hostile_linear(W, H, seed=17)
-    f = EmulatedFrame(p, linear=True)
+    f = Frame(p, linear=True)
     f.run(d)
     _check(f.buffer, W, H, cam, d, str(kw), linear=True, stereo=stereo, **kw)
 
@@ -176,7 +173,7 @@ def test_layered_frame_hostile(use_tma):
     d = np.stack([HC.hostile_raw(W, H, _zb(cam), True, seed=30), HC.salt(HC.hostile_raw(W, H, _zb(cam), True, seed=31), HC.LINEAR, 31),
                   HC.hostile_raw(W, H, _zb(cam), True, seed=32)])
     d[2, 16:64, 32:96] = np.nan
-    f = LayeredFrame(_plan(cam, 3), use_tma=use_tma)
+    f = Frame(_plan(cam, 3), use_tma=use_tma)
     f.run(d)
     for l in range(3):
         _check(lambda bid: f.buffer(bid, l), W, H, cam, d[l], f"layered layer {l}")
@@ -188,11 +185,11 @@ def test_pitched_view_hostile(linear):
     W, H = W0, H0
     cam = Camera(W, H)
     d = HC.hostile_linear(W, H, seed=40) if linear else HC.hostile_raw(W, H, _zb(cam), True, seed=40)
-    f = PitchedFrame(_plan(cam), linear=linear)
+    f = fused_frame(_plan(cam), linear=linear)
     dv = View((1, H, W), np.float32, 1024, 1024 * H)
     dv.arr[...] = d
     av = View((1, H, W), np.uint8, 256, 256 * H, fill=SENTINEL)
-    f.run(dv, av)
+    f.run_pitched(dv, av)
     assert (av.outside() == SENTINEL).all()
     _check(lambda bid: av.arr[0] if bid == 17 else f.buffer(bid), W, H, cam, d, f"pitched linear={linear}", linear=linear)
 
@@ -205,7 +202,7 @@ def test_array_frame_hostile(kind):
         depth, seen = HC.hostile_unorm(W, H, 16, True, seed=50)
     else:
         depth = seen = HC.hostile_raw(W, H, _zb(cam), True, seed=50)
-    f = ArrayFrame(_plan(cam))
+    f = Frame(_plan(cam))
     ao = f.run_arrays(depth[None])
     _check(lambda bid: ao[0] if bid == 17 else f.buffer(bid, 0), W, H, cam, seen, f"array {kind}")
 

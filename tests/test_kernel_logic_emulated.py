@@ -15,7 +15,7 @@ from miniengineao_b200 import AmbientOcclusion, Camera, synth
 from oracle import oracle as O
 from oracle.oracle import Oracle
 
-from emu.emu import EmulatedFrame, composite, composite_debug  # noqa: E402  (tests/ is on sys.path via conftest)
+from emu.emu import Frame, composite, composite_debug  # noqa: E402  (tests/ is on sys.path via conftest)
 
 
 def _plan(W, H, **kw):
@@ -51,7 +51,7 @@ def _run(W, H, seed=1, depth=None, use_tma=True, **kw):
     if depth is None:
         depth = synth.lin01_to_raw(synth.random_depth(W, H, seed=seed), reversed_z=kw.get("reversed_z", True))
     ref = orc.run(depth)
-    f = EmulatedFrame(_plan(W, H, **kw), use_tma=use_tma)
+    f = Frame(_plan(W, H, **kw), use_tma=use_tma)
     n0 = f.tma_box_loads()
     got = f.run(depth)
     f.tma_loads_in_run = f.tma_box_loads() - n0
@@ -129,7 +129,7 @@ def test_linear_and_native_depth_ingest():
     lin = synth.random_depth(W, H, seed=9)
     orc = Oracle(W, H, depth_is_linear=True)
     ref = orc.run(lin)
-    f = EmulatedFrame(_plan(W, H), linear=True)
+    f = Frame(_plan(W, H), linear=True)
     assert np.array_equal(f.run(lin), ref)
     _compare_all(f, orc, "linear ingest")
     raw = synth.lin01_to_raw(lin).astype(np.float64)
@@ -140,7 +140,7 @@ def test_linear_and_native_depth_ingest():
         orc = Oracle(W, H)
         ref = orc.run(as_float)
         words = codes.astype(np.uint16) if bits == 16 else (codes | (np.uint32(0xA5) << np.uint32(24)))
-        f = EmulatedFrame(_plan(W, H))
+        f = Frame(_plan(W, H))
         assert np.array_equal(f.run(words.astype(dt)), ref), bits
         _compare_all(f, orc, f"D{bits}")
 
@@ -192,7 +192,7 @@ def test_render_tile_height_variants(tile, use_tma):
     depth[100:140, 200:330] = 0.0
     orc = Oracle(W, H, threads=4, intensity=1.1, high_quality_mask=0b0011)
     ref = orc.run(depth)
-    f = EmulatedFrame(_plan(W, H, intensity=1.1, high_quality_mask=0b0011), use_tma=use_tma, render_tile=tile)
+    f = Frame(_plan(W, H, intensity=1.1, high_quality_mask=0b0011), use_tma=use_tma, render_tile=tile)
     n0 = f.tma_box_loads()
     assert np.array_equal(f.run(depth), ref)
     _compare_all(f, orc, f"tile variant {tile}", 0b0011)
@@ -208,7 +208,7 @@ def test_single_scale_plan(W, H):
     ref = orc.run(depth)
     plan = _plan(W, H, intensity=1.1)
     plan.singleScale = True
-    f = EmulatedFrame(plan)
+    f = Frame(plan)
     assert np.array_equal(f.run(depth), ref)
     for bid in (1, 2, 3, 4, 5, 10, 17):
         got = f.buffer(bid)
@@ -225,7 +225,7 @@ def _band_frames(W, H, nb, **kw):
     for i in range(nb):
         plan = _plan(W, H, **kw)
         plan.set_row_band(cuts[i], cuts[i + 1], *rowtile.neighbours(cuts, i))
-        f = EmulatedFrame(plan)
+        f = Frame(plan)
         f.use_plan_band()
         frames.append(f)
     return cuts, frames
@@ -245,7 +245,7 @@ def test_native_exchange_kernel_bands_equal_whole_frame(W, H, nb):
         want = ref if frame_no == 1 else Oracle(W, H, threads=4, intensity=1.1).run(d)
         for i, f in enumerate(frames):
             if frame_no == 2:
-                f._lib.emu_poison_low(f._h)
+                f.poison_low()
         for i, f in enumerate(frames):
             f.band_phase_a(d[cuts[i]:cuts[i + 1]])
         for i, f in enumerate(frames):
@@ -300,7 +300,7 @@ def test_persistent_tile_loop_forced_on_every_level(use_tma, monkeypatch):
     depth[100:130, 200:300] = 0.0                                   # sky: the out-of-line IEEE path inside the loop
     orc = Oracle(W, H, threads=4, intensity=1.1, high_quality_mask=0b0101)
     ref = orc.run(depth)
-    f = EmulatedFrame(_plan(W, H, intensity=1.1, high_quality_mask=0b0101), use_tma=use_tma)
+    f = Frame(_plan(W, H, intensity=1.1, high_quality_mask=0b0101), use_tma=use_tma)
     for frame in range(2):
         assert np.array_equal(f.run(depth), ref), frame
     _compare_all(f, orc, "tile loop", 0b0101)

@@ -1,7 +1,7 @@
 """CPU tests of per-layer cameras (meao_set_layer_cameras): every layer of a layered frame with its own near plane, far plane and field
 of view.
 
-The layered kernel sources run in the fiber emulator through their own driver (tests/emu/layer_cameras_driver.cpp), with each layer's
+The layered kernel sources run in the fiber emulator (tests/emu/frame_driver.cpp), with each layer's
 constants read from a plan-only libmeao context through the per-layer getters.  Layer l must be bit-identical to the oracle run on that
 layer alone with camera l -- the AO and every buffer.  Also here: the plan-only contract of meao_set_layer_cameras (return values,
 refusals, the per-layer getters against single-layer contexts), the Python property and the -Xptxas -v check of the changed kernels."""
@@ -10,7 +10,6 @@ import os
 import re
 import shutil
 import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -19,14 +18,10 @@ from miniengineao_b200 import AmbientOcclusion, Camera, MeaoError
 from miniengineao_b200 import _native as N
 from oracle.oracle import Oracle
 
-from emu.emu import linearize_zero
+from emu.emu import Frame
 from test_layers_emulated import _raw, contrasting_layers
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, os.path.join(HERE, "emu"))
-import build_layer_cameras_emu  # noqa: E402
-
-ROOT = os.path.dirname(HERE)
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "miniengineao_b200", "csrc")
 
 # visibly different cameras: near 0.1 / 0.3 / 1.0, far 50 / 100 / 1000, vertical FOV 40 / 60 / 90 degrees
@@ -34,25 +29,6 @@ CAMS = [(0.1, 50.0, 40.0), (0.3, 100.0, 60.0), (1.0, 1000.0, 90.0)]
 PARAMS = {"noise_filter_tolerance": "noiseFilterTolerance", "blur_tolerance": "blurTolerance", "upsample_tolerance": "upsampleTolerance",
           "thickness_modifier": "thicknessModifier", "intensity": "intensity", "sample_exhaustively": "sampleExhaustively",
           "high_quality_mask": "highQualityMask"}
-
-_lib = None
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        l = C.CDLL(build_layer_cameras_emu.build())
-        l.lcemu_create.restype = C.c_void_p
-        l.lcemu_create.argtypes = [C.c_int, C.c_int, C.c_int]
-        l.lcemu_destroy.argtypes = [C.c_void_p]
-        l.lcemu_set_constants.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float] + [C.c_int] * 6
-        l.lcemu_set_layer.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float]
-        l.lcemu_set_views.argtypes = [C.c_void_p, C.c_int, C.c_longlong, C.c_longlong, C.c_void_p, C.c_longlong, C.c_longlong]
-        l.lcemu_run.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
-        l.lcemu_get_buffer.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
-        l.lcemu_tma_box_loads.restype = C.c_longlong
-        _lib = l
-    return _lib
 
 
 def cameras(W, H, n, reversed_z=True):
@@ -75,61 +51,6 @@ def _aligned(nbytes):
     raw = np.zeros(nbytes + 128, np.uint8)
     off = (-raw.ctypes.data) % 64
     return raw[off:off + nbytes]
-
-
-class CamFrame:
-    """One layered frame with per-layer cameras through the host-compiled kernels, planned by a plan-only libmeao context."""
-
-    def __init__(self, plan, *, linear=False, use_tma=True, fused=True):
-        self._lib = lib()
-        plan.LateUpdate()
-        self.plan, self.W, self.H, self.L = plan, plan._width, plan._height, int(plan.layers)
-        nl, ctx = N.lib(), plan._ctx
-        rc, rcw, uc, zb = (C.c_float * 112)(), (C.c_float * 112)(), (C.c_float * 32)(), (C.c_float * 4)()
-        for k in range(1, 5):
-            N.check(ctx, nl.meao_render_constants(ctx, k, C.cast(C.byref(rc, 112 * (k - 1)), C.POINTER(C.c_float))))
-            N.check(ctx, nl.meao_render_constants_wide(ctx, k, C.cast(C.byref(rcw, 112 * (k - 1)), C.POINTER(C.c_float))))
-            N.check(ctx, nl.meao_upsample_constants(ctx, k, C.cast(C.byref(uc, 32 * (k - 1)), C.POINTER(C.c_float))))
-        N.check(ctx, nl.meao_zbuffer_params(ctx, zb))
-        rz = bool(plan.camera.usesReversedZBuffer)
-        self._h = self._lib.lcemu_create(self.W, self.H, self.L)
-        self._lib.lcemu_set_constants(self._h, rc, rcw, uc, zb, 0.0, int(not linear), int(rz), int(plan.highQualityMask),
-                                      int(plan.sampleExhaustively), int(plan.singleScale), int(use_tma))
-        for l in range(self.L):        # each layer's own constants, from the per-layer getters
-            lrc, lrcw, lzb = (C.c_float * 112)(), (C.c_float * 112)(), (C.c_float * 4)()
-            for k in range(1, 5):
-                for wide, buf in ((0, lrc), (1, lrcw)):
-                    N.check(ctx, nl.meao_render_constants_layer(ctx, l, k, wide, C.cast(C.byref(buf, 112 * (k - 1)), C.POINTER(C.c_float))))
-            N.check(ctx, nl.meao_zbuffer_params_layer(ctx, l, lzb))
-            pad12 = 0.0 if linear else (1e5 if rz else linearize_zero(lzb))     # Linearize(OOB load = 0)
-            self._lib.lcemu_set_layer(self._h, l, lrc, lrcw, lzb, pad12)
-        self._fused = int(fused)
-        self._lib.lcemu_set_views(self._h, self._fused, 0, 0, None, 0, 0)
-
-    def __del__(self):
-        if getattr(self, "_h", None):
-            self._lib.lcemu_destroy(self._h)
-            self._h = None
-
-    def run(self, depth, depth_row=0, depth_layer=0, ao=None, ao_row=0, ao_layer=0):
-        """depth: the [L, H, W] frame, or a flat aligned buffer holding it at the given element pitches; ao: a flat uint8 buffer."""
-        fmt = {"float32": 0, "uint16": 1, "uint32": 2}[depth.dtype.name]
-        if depth_row == 0:
-            buf = _aligned(depth.nbytes).view(depth.dtype)
-            buf[...] = depth.reshape(-1)
-            depth = buf
-        self._keep = (depth, ao)
-        self._lib.lcemu_set_views(self._h, self._fused, depth_row, depth_layer, None if ao is None else ao.ctypes.data, ao_row, ao_layer)
-        self.tma0 = self._lib.lcemu_tma_box_loads()
-        self._lib.lcemu_run(self._h, depth.ctypes.data, fmt)
-        self.tma_loads_in_run = self._lib.lcemu_tma_box_loads() - self.tma0
-
-    def buffer(self, bid, layer):
-        d = self.plan.buffer_desc(bid)
-        dt = {1: np.uint8, 2: np.float16, 4: np.float32}[d.elem_bytes]
-        out = np.zeros((d.slices, d.height, d.width) if d.slices > 1 else (d.height, d.width), dt)
-        assert self._lib.lcemu_get_buffer(self._h, bid, layer, out.ctypes.data) == 0
-        return out
 
 
 def _oracle(W, H, cam, **kw):
@@ -167,8 +88,8 @@ def _compare(f, W, H, depth, cams, *, linear=False, single_scale=False, oracle_d
 
 def _run(W, H, depth, *, use_tma=True, linear=False, single_scale=False, fused=True, oracle_depth=None, **kw):
     cams = cameras(W, H, depth.shape[0], kw.get("reversed_z", True))
-    f = CamFrame(_plan(W, H, cams, single_scale=single_scale, **kw), linear=linear, use_tma=use_tma, fused=fused)
-    f.run(depth)
+    f = Frame(_plan(W, H, cams, single_scale=single_scale, **kw), linear=linear, use_tma=use_tma)
+    (f.run_fused if fused else f.run)(depth)
     _compare(f, W, H, depth, cams, linear=linear, single_scale=single_scale, oracle_depth=oracle_depth, **kw)
     return f
 
@@ -233,8 +154,8 @@ def test_pitched_layered_corner():
     ao = _aligned(al * L)
     ao[:] = 0xA7
     cams = cameras(W, H, L)
-    f = CamFrame(_plan(W, H, cams), fused=True)
-    f.run(big, dr, dl, ao, ar, al)
+    f = Frame(_plan(W, H, cams))
+    f.run_fused(big, depth_row=dr, depth_layer=dl, ao=ao, ao_row=ar, ao_layer=al)
     view = lambda l: np.stack([ao[l * al + y * ar: l * al + y * ar + W] for y in range(H)])
     _compare(f, W, H, depth, cams, ao_of=view)
 

@@ -1,6 +1,6 @@
 """CPU tests of layered frames (meao_set_layers): L same-size views stacked at a stride of one image, one launch per stage.
 
-The layered kernel sources (csrc/*_layered.cu) run in the fiber emulator (tests/emu/layered_emu.py) and every layer must be bit-identical to the
+The layered kernel sources (csrc/*_layered.cu) run in the fiber emulator (tests/emu/frame_driver.cpp) and every layer must be bit-identical to the
 oracle run on that layer alone -- all 17 buffers and the AO.  Neighbouring layers are chosen to contrast (a corridor, constant
 depth, a frame with a sky patch, random depth) at sizes where no level is a multiple of 4, 16 or 64, so a read across a layer
 boundary changes bits.  Also here: the packed-contraction audit of the layered translation units and the plan-only contract of
@@ -18,7 +18,7 @@ from miniengineao_b200 import AmbientOcclusion, Camera, MeaoError, synth
 from miniengineao_b200 import _native as N
 from oracle.oracle import Oracle
 
-from emu.layered_emu import LayeredFrame  # noqa: E402  (tests/ is on sys.path via conftest)
+from emu.emu import Frame  # noqa: E402  (tests/ is on sys.path via conftest)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "miniengineao_b200", "csrc")
@@ -82,7 +82,7 @@ def _compare_layer(f, layer, orc, tag, mask=0, ids=None):
 def _run_layers(W, H, depth, *, use_tma=True, linear=False, single_scale=False, oracle_depth=None, **kw):
     """depth: [L, H, W] in the ingest format; oracle_depth: the float32 the oracle sees per layer (default: depth itself)."""
     L = depth.shape[0]
-    f = LayeredFrame(_plan(W, H, L, single_scale=single_scale, **kw), linear=linear, use_tma=use_tma)
+    f = Frame(_plan(W, H, L, single_scale=single_scale, **kw), linear=linear, use_tma=use_tma)
     n0 = f.tma_box_loads()
     f.run(depth)
     f.tma_loads_in_run = f.tma_box_loads() - n0
@@ -123,6 +123,24 @@ def test_layered_variants(kw):
     rz = kw.get("reversed_z", True)
     depth = _raw(contrasting_layers(W, H, 3, seed=7), reversed_z=rz)
     _run_layers(W, H, depth, intensity=1.2, **kw)
+
+
+def test_null_camera_tables_take_the_argument_block_constants():
+    """The layered and array kernels given no camera tables (a null table: every layer takes the argument block's constants).  libmeao
+    always passes its tables, so this pins the launchers' fallback on purpose: the stage frame, the fused frame and an array frame."""
+    W, H = 161, 93
+    depth = _raw(contrasting_layers(W, H, 3, seed=5))
+    f = Frame(_plan(W, H, 3, intensity=1.1), null_tables=True)
+    refs = [Oracle(W, H, threads=4, intensity=1.1) for _ in range(3)]
+    aos = [r.run(depth[l]) for l, r in enumerate(refs)]
+    f.run(depth)
+    for l in range(3):
+        _compare_layer(f, l, refs[l], "null tables")
+    f.run_fused(depth)
+    fused = [f.buffer(17, l) for l in range(3)]
+    ao = f.run_arrays(depth, "layered")
+    for l in range(3):
+        assert np.array_equal(fused[l], aos[l]) and np.array_equal(ao[l], aos[l]), l
 
 
 def test_layered_linear_and_native_ingest():

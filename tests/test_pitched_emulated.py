@@ -1,6 +1,6 @@
 """CPU tests of pitched frames (meao_render_pitched): the depth and the AO are views inside larger allocations, each with its own row and
-layer pitch.  The kernel sources of a fused frame run in the fiber emulator (tests/emu/pitched_driver.cpp) with the argument blocks
-meao_api.cu fills for such views.
+layer pitch.  The kernel sources of a fused frame run in the fiber emulator (tests/emu/frame_driver.cpp) with the argument blocks
+libmeao fills for such views.
 
 Every backing byte of the depth outside its view is 0xff (NaN as f32, the far-plane code as D16 / D24S8), so a bit-exact AO proves the
 padding is never read; every AO byte outside its view holds a sentinel that must survive.  AO, LinearDepth and LowDepth1..4 of every
@@ -8,7 +8,6 @@ layer must equal the oracle's on the tight depth, over the depth kinds, both Z d
 pitches, row pitches that rule out the 128-bit loads, a sub-rectangle at x0 = 1, a dynamic-resolution corner of a larger layered
 target, premin, single-scale and a row band.  Zero pitches in the argument blocks must keep meaning the tight views.  Also here: the
 packed-contraction audit of the changed translation units and a spill check of the fused final-level and prepare kernels."""
-import ctypes as C
 import os
 import re
 import shutil
@@ -17,36 +16,15 @@ import subprocess
 import numpy as np
 import pytest
 
-from miniengineao_b200 import _native as N
 from oracle.oracle import Oracle
 
-from emu import build_pitched_emu  # noqa: E402  (tests/ is on sys.path via conftest)
-from emu.emu import linearize_zero
-from test_fused_lin_emulated import _ingest, _raw_with_sky
+from test_fused_lin_emulated import _ingest, _raw_with_sky, fused_frame  # noqa: E402  (tests/ is on sys.path via conftest)
 from test_layers_emulated import _compare_layer, _plan, contrasting_layers
 from miniengineao_b200 import synth
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "miniengineao_b200", "csrc")
 SENTINEL = 0xA5
-
-_lib = None
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        l = C.CDLL(build_pitched_emu.build())
-        l.lemu_create.restype = C.c_void_p
-        l.lemu_create.argtypes = [C.c_int, C.c_int, C.c_int]
-        l.lemu_destroy.argtypes = [C.c_void_p]
-        l.lemu_set_constants.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float] + [C.c_int] * 6
-        l.lemu_get_buffer.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
-        l.femu_poison_lin.argtypes = [C.c_void_p]
-        l.pemu_run.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_longlong, C.c_longlong, C.c_void_p, C.c_longlong, C.c_longlong,
-                               C.c_int, C.c_int]
-        _lib = l
-    return _lib
 
 
 class View:
@@ -80,47 +58,6 @@ class View:
         return self.back[mask]
 
 
-class PitchedFrame:
-    """One fused frame on views, planned by a plan-only libmeao context (device = -1); the set-up of FusedFrame."""
-
-    def __init__(self, plan, *, linear=False):
-        self._lib = lib()
-        plan.LateUpdate()
-        self.plan = plan
-        self.W, self.H, self.layers = plan._width, plan._height, int(plan.layers)
-        nl = N.lib()
-        rc, rcw, uc, zb = (C.c_float * 112)(), (C.c_float * 112)(), (C.c_float * 32)(), (C.c_float * 4)()
-        for k in range(1, 5):
-            N.check(plan._ctx, nl.meao_render_constants(plan._ctx, k, C.cast(C.byref(rc, 112 * (k - 1)), C.POINTER(C.c_float))))
-            N.check(plan._ctx, nl.meao_render_constants_wide(plan._ctx, k, C.cast(C.byref(rcw, 112 * (k - 1)), C.POINTER(C.c_float))))
-            N.check(plan._ctx, nl.meao_upsample_constants(plan._ctx, k, C.cast(C.byref(uc, 32 * (k - 1)), C.POINTER(C.c_float))))
-        N.check(plan._ctx, nl.meao_zbuffer_params(plan._ctx, zb))
-        rz = bool(plan.camera.usesReversedZBuffer)
-        pad12 = 0.0 if linear else (1e5 if rz else linearize_zero(zb))
-        self._h = self._lib.lemu_create(self.W, self.H, self.layers)
-        self._lib.lemu_set_constants(self._h, rc, rcw, uc, zb, pad12, int(not linear), int(rz), int(plan.highQualityMask),
-                                     int(plan.sampleExhaustively), int(plan.singleScale), 1)
-        self._lib.femu_poison_lin(self._h)
-
-    def __del__(self):
-        if getattr(self, "_h", None):
-            self._lib.lemu_destroy(self._h)
-            self._h = None
-
-    def run(self, dv: View, av: View, rows=(0, 0), zero=False):
-        fmt = {"float32": 0, "uint16": 1, "uint32": 2}[dv.arr.dtype.name]
-        p = (0, 0, 0, 0) if zero else (dv.row, dv.layer, av.row, av.layer)
-        self._lib.pemu_run(self._h, dv.ptr, fmt, p[0], p[1], av.ptr, p[2], p[3], rows[0], rows[1])
-
-    def buffer(self, bid, layer=0):
-        d = self.plan.buffer_desc(bid)
-        dt = {1: np.uint8, 2: np.float16, 4: np.float32}[d.elem_bytes]
-        shape = (d.slices, d.height, d.width) if d.slices > 1 else (d.height, d.width)
-        out = np.zeros(shape, dt)
-        assert self._lib.lemu_get_buffer(self._h, bid, layer, out.ctypes.data) == 0
-        return out
-
-
 def _frame(depth, seen, *, drow=None, dlayer=None, dbase=0, arow=None, alayer=None, abase=0, linear=False, rz=True, rows=(0, 0),
            zero=False, **kw):
     """Run depth [L, H, W] (ingest format) through views with the given byte pitches (None: tight) and check every layer against the
@@ -131,13 +68,13 @@ def _frame(depth, seen, *, drow=None, dlayer=None, dbase=0, arow=None, alayer=No
     dlayer = dlayer or H * drow
     arow = arow or W
     alayer = alayer or H * arow
-    f = PitchedFrame(_plan(W, H, L, reversed_z=rz, intensity=1.1, **kw), linear=linear)
+    f = fused_frame(_plan(W, H, L, reversed_z=rz, intensity=1.1, **kw), linear=linear)
     band = rows[1] > rows[0]
     dv = View(depth.shape, depth.dtype, drow, dlayer, dbase)
     dv.arr[...] = depth
     ashape = (L, rows[1] - rows[0], W) if band else (L, H, W)
     av = View(ashape, np.uint8, arow, alayer, abase, fill=SENTINEL)
-    f.run(dv, av, rows, zero)
+    f.run_pitched(dv, av, rows, zero)
     assert (av.outside() == SENTINEL).all(), "a byte outside the AO view was written"
     assert (dv.outside() == 0xFF).all()
     okw = dict(intensity=1.1, reversed_z=rz, depth_is_linear=linear, **kw)
@@ -224,8 +161,8 @@ def test_pitched_row_band():
 
 @pytest.mark.parametrize("kind", ["f32", "d16"])
 def test_zero_pitches_in_the_argument_blocks_mean_tight(kind):
-    """The drivers written before the pitch fields zero-fill PrepareArgs / DepthIn: zero pitches on tight views give the tight
-    frame, for one layer and for a layered frame."""
+    """The launchers resolve zero pitches in PrepareArgs / DepthIn to the tight views (the blocks are built as libmeao builds them,
+    then their pitches zeroed): zero pitches on tight views give the tight frame, for one layer and for a layered frame."""
     W, H = 136, 72
     depth, seen = _one(W, H, kind, 11)
     _frame(depth, seen, zero=True)

@@ -129,7 +129,7 @@ def _worker_emulated(rank, world, port, W, H, q, mask):
     import torch.distributed as dist
     from miniengineao_b200 import AmbientOcclusion, Camera, rowtile, synth
     from oracle.oracle import Oracle
-    from emu.emu import EmulatedFrame
+    from emu.emu import Frame
 
     dist.init_process_group("gloo", init_method=f"tcp://127.0.0.1:{port}", rank=rank, world_size=world)
     try:
@@ -140,7 +140,7 @@ def _worker_emulated(rank, world, port, W, H, q, mask):
         plan = AmbientOcclusion(Camera(W, H), device=-1)
         plan.intensity, plan.highQualityMask = 1.1, mask
         plan.set_row_band(r0, r1, *rowtile.neighbours(cuts, rank))
-        f = EmulatedFrame(plan)
+        f = Frame(plan)
         f.use_plan_band()                                   # also poisons every LowDepth texel with NaN
         f.band_phase_a(depth[r0:r1])                        # this rank only ever sees its band of the depth buffer
         send = [torch.from_numpy(f.halo_pack(side).copy()) for side in (0, 1)]
