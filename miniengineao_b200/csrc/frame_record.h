@@ -6,6 +6,7 @@
 #define MEAO_FRAME_RECORD_H
 
 #include <stdint.h>
+#include <string>
 #include <vector>
 
 #include "../../include/meao.h"
@@ -328,6 +329,86 @@ inline cudaError_t launch_upsample(const FrameState &f, int lo, const UpsampleAr
         return launch_blur_upsample_array(dm, ao_map, hm, f.tma_ok, a, lo_ao2, f.occ_pitch[lo], f.layers, f.sm_count, aio->ao, aio->ao_surf, s);
     if (f.layers > 1) return launch_blur_upsample_layered(dm, ao_map, hm, f.tma_ok, a, lo_ao2, f.occ_pitch[lo], f.layers, f.sm_count, s);
     return launch_blur_upsample(dm, ao_map, hm, f.tma_ok, a, lo_ao2, f.occ_pitch[lo], f.sm_count, s);
+}
+
+// ---- the frame schedule: which kernels a frame launches, in what order, on which stream and after which other launch ----------
+enum FrameStage { kStagePrepare, kStageRender, kStageRenderWide, kStageUpsample };
+// PDL (DESIGN.md 2.5): a launch whose only predecessor is the launch before it on its stream carries the programmatic-dependent-launch
+// attribute from PDL level 1 on; one that also waits for another branch, from level 2; the first launch of a branch never.
+enum PdlClass { kPdlNever = 0, kPdlFrom1 = 1, kPdlFrom2 = 2 };
+
+struct FrameLaunch {
+    int stage;      // FrameStage
+    int level;      // render level k, or the upsample's lo level (1 = the final upsample); 0 for the prepare
+    int branch;     // 0: the caller's stream; 1..3: the context's forked streams
+    int wait;       // index of an earlier launch on another branch that this one waits for; -1: none
+    int pdl;        // PdlClass
+};
+
+inline bool pdl_on(const FrameLaunch &l, int pdl_level) { return l.pdl != kPdlNever && pdl_level >= l.pdl; }
+
+// The launches of one frame in serial order (RebuildCommandBuffers, AO.cs:511-531): prepare, render 1..k, the wide renders of the
+// high_quality_mask levels, upsamples k..1.  The branches make it a DAG: the four render levels are independent (SURVEY.md 3.2), a
+// level's wide render rides on its branch, the coarse upsample chain 4->3->2 only needs Occlusion2..4, and only the last two upsamples
+// wait for the big level-1 render.  single_scale (BASELINE.json configs[0]): prepare, render 1 and the final-style upsample on Occlusion1.
+inline std::vector<FrameLaunch> frame_schedule(const MeaoVariants &v)
+{
+    const int kmax = v.single_scale ? 1 : 4;
+    std::vector<FrameLaunch> s;
+    int last[4] = {0, 0, 0, 0};             // the last launch on each branch so far
+    auto add = [&](int stage, int level, int branch, int wait, int pdl) {
+        last[branch] = (int)s.size();
+        s.push_back(FrameLaunch{stage, level, branch, wait, pdl});
+    };
+    add(kStagePrepare, 0, 0, -1, kPdlNever);
+    for (int k = 1; k <= kmax; k++) add(kStageRender, k, k - 1, k == 1 ? -1 : 0, k == 1 ? kPdlFrom1 : kPdlNever);
+    for (int k = 1; k <= kmax; k++)
+        if ((v.high_quality_mask >> (k - 1)) & 1) add(kStageRenderWide, k, k - 1, -1, kPdlFrom1);
+    if (kmax == 4) {
+        add(kStageUpsample, 4, 3, last[2], kPdlFrom2);
+        add(kStageUpsample, 3, 3, last[1], kPdlFrom2);
+        add(kStageUpsample, 2, 0, last[3], kPdlFrom2);
+    }
+    add(kStageUpsample, 1, 0, -1, kPdlFrom1);
+    return s;
+}
+
+// The launch's name in meao_profile_frame: "prepare_depth", "render_ao L1", "render_ao_wide L1", "blur_upsample L2->L1"
+inline std::string launch_name(const FrameLaunch &l)
+{
+    const std::string k = std::to_string(l.level);
+    switch (l.stage) {
+        case kStagePrepare: return "prepare_depth";
+        case kStageRender: return "render_ao L" + k;
+        case kStageRenderWide: return "render_ao_wide L" + k;
+        default: return "blur_upsample L" + k + "->L" + std::to_string(l.level - 1);
+    }
+}
+
+// What a frame form puts into the first and the last launch of its schedule.
+struct FrameIO {
+    int kind = MEAO_DEPTH_RAW_F32;
+    DepthIn depth{};                    // the caller's depth (depth_in), read by the prepare and by a fused final upsample
+    const ArrayIO *aio = nullptr;       // read the depth from, and store the AO into, CUDA arrays
+    bool low_only = false;              // the prepare writes LowDepth1..4 only
+    bool fused = false;                 // the final upsample reads and linearises `depth` and writes LinearDepth
+    void *ao = nullptr;                 // the final upsample's AO at the pitches of vp (nullptr: tight); nullptr: the result buffer
+    const ViewPitch *vp = nullptr;
+};
+
+// Launches schedule entry l of a frame on stream s.  force_tile: render_tile_variant's force.
+inline cudaError_t launch_entry(const FrameState &f, const FrameLaunch &l, const FrameIO &io, int force_tile, cudaStream_t s)
+{
+    const bool final_level = l.stage == kStageUpsample && l.level == 1;
+    switch (l.stage) {
+        case kStagePrepare: return launch_prepare(f, prepare_args(f, io.depth), io.aio, io.low_only, s);
+        case kStageRender:
+        case kStageRenderWide:
+            return launch_render(f, render_args(f, l.level, io.kind, l.stage == kStageRenderWide, force_tile), l.level, io.kind, s);
+        default:
+            return launch_upsample(f, l.level, upsample_args(f, l.level, final_level ? io.ao : nullptr, final_level ? io.vp : nullptr),
+                                   io.aio, io.fused ? &io.depth : nullptr, s);
+    }
 }
 
 }  // namespace meao

@@ -116,7 +116,7 @@ struct MeaoCtx : SizeState {
         for (int i = 0; i < 4; i++) if (pitch[i] != o.pitch[i]) return pitch[i] < o.pitch[i];
         for (int i = 0; i < 3; i++) if (size[i] != o.size[i]) return size[i] < o.size[i];
         return false; } };
-    struct GraphEntry { cudaGraphExec_t exec; uint64_t last_use; };
+    struct GraphEntry { cudaGraphExec_t exec; uint64_t last_use; int launches; };     // launches: the kernels its capture recorded
     std::map<GraphKey, GraphEntry> graphs;
     // executable graphs that cudaGraphExecUpdate could not re-target while they were possibly in flight; `done` is recorded after the
     // frame that replaced them, so once it has completed (and, frames of a context running in order, every earlier frame) the graph
@@ -517,125 +517,113 @@ int forced_render_tile()
     return (force && force[0] >= '0' && force[0] < '0' + kRenderTileVariants) ? force[0] - '0' : -1;
 }
 
-// ---- the three recorders: frame_record.h's argument blocks and launcher choice, one launch each --------------------------------
+// ---- the recorders: frame_record.h's schedule, argument blocks and launcher choice -------------------------------------------
 
-// PushDownsampleCommands, AO.cs:604-658.  aio: read the depth from a CUDA array instead of `depth`.  low_only: LowDepth1..4 only --
-// the frame's final upsample is recorded with the same depth (record_upsample's `fused`) and writes LinearDepth itself.
-// vp: the depth's pitches (nullptr: tight).
-int record_downsample(MeaoCtx *c, const void *depth, int kind, cudaStream_t s, const ArrayIO *aio = nullptr, bool low_only = false,
-                      const ViewPitch *vp = nullptr)
+// One launch of the frame schedule on stream s, inside an NVTX range, counted.  io: the frame's depth and AO (FrameIO).  A prepare
+// goes through record_downsample, which checks the depth kind first.
+int record_launch(MeaoCtx *c, const FrameLaunch &l, const FrameIO &io, cudaStream_t s)
 {
-    if (kind < MEAO_DEPTH_RAW_F32 || kind > MEAO_DEPTH_RAW_D24S8) return fail(c, MEAO_ERR_INVALID, "bad depth kind %d", kind);
-    NvtxRange nv("meao::prepare_depth");
-    c->last_kind = kind;
-    CUDA_TRY(c, launch_prepare(*c, prepare_args(*c, depth_in(*c, depth, kind, vp)), aio, low_only, s));
+    static const char *nvtx[4] = {"meao::prepare_depth", "meao::render_ao", "meao::render_ao_wide", "meao::blur_upsample"};
+    if (l.stage == kStageUpsample && l.level == 1) c->last_out = io.aio ? const_cast<void *>(io.aio->ao_array) : io.ao;
+    NvtxRange nv(nvtx[l.stage]);
+    CUDA_TRY(c, launch_entry(*c, l, io, forced_render_tile(), s));
     c->launches++;
     return 0;
 }
 
+// The FrameIO of a pointer frame: its depth and AO at the pitches of vp (nullptr: tight).  fused: the prepare writes LowDepth1..4
+// only and the final upsample reads and linearises the same depth (what meao_render records).
+FrameIO frame_io(MeaoCtx *c, const void *depth, int kind, void *ao_out, bool fused, const ViewPitch *vp = nullptr)
+{
+    FrameIO io;
+    io.kind = kind; io.depth = depth_in(*c, depth, kind, vp); io.low_only = io.fused = fused; io.ao = ao_out; io.vp = vp;
+    return io;
+}
+
+// PushDownsampleCommands, AO.cs:604-658: the prepare_depth of every entry point, the first launch of the frame schedule.  io.low_only:
+// LowDepth1..4 only, for a frame whose final upsample reads the same depth; otherwise LinearDepth as well.
+int record_downsample(MeaoCtx *c, const FrameIO &io, cudaStream_t s)
+{
+    if (io.kind < MEAO_DEPTH_RAW_F32 || io.kind > MEAO_DEPTH_RAW_D24S8) return fail(c, MEAO_ERR_INVALID, "bad depth kind %d", io.kind);
+    c->last_kind = io.kind;
+    return record_launch(c, FrameLaunch{kStagePrepare, 0, 0, -1, kPdlNever}, io, s);
+}
+// One entry of the frame schedule: the prepare through record_downsample, every other launch through record_launch
+int record_entry(MeaoCtx *c, const FrameLaunch &l, const FrameIO &io, cudaStream_t s)
+{
+    return l.stage == kStagePrepare ? record_downsample(c, io, s) : record_launch(c, l, io, s);
+}
+
+// The stage API's recorders, one launch each: the prepare_depth of a pointer depth (tight rows), a render level, an upsample level.
+int record_downsample(MeaoCtx *c, const void *depth, int kind, cudaStream_t s, bool low_only = false)
+{
+    FrameIO io = frame_io(c, depth, kind, nullptr, false);
+    io.low_only = low_only;
+    return record_downsample(c, io, s);
+}
 // PushRenderCommands, AO.cs:660-748.  wide = false: the call AmbientOcclusion.cs makes (tiled source, kernel main_interleaved);
 // wide = true: the same recorder for the non-tiled source LowDepth<k> (kernel main) -> HighQuality<k>.
 int record_render(MeaoCtx *c, int k, int kind, cudaStream_t s, bool wide = false)
 {
-    NvtxRange nv(wide ? "meao::render_ao_wide" : "meao::render_ao");
-    CUDA_TRY(c, launch_render(*c, render_args(*c, k, kind, wide, forced_render_tile()), k, kind, s));
-    c->launches++;
-    return 0;
+    return record_launch(c, FrameLaunch{wide ? kStageRenderWide : kStageRender, k, 0, -1, kPdlNever}, frame_io(c, nullptr, kind, nullptr, false), s);
 }
-
-// PushUpsampleCommands with the wiring of AO.cs:528-531.  aio (final level only): store the AO into a CUDA array instead of ao_out.
-// fused (final level only, with the frame's depth and kind): read and linearise the raw depth and write LinearDepth here, after a
-// low_only record_downsample of the same depth (its ao_layer_pitch is the AO's).  vp: the pitches of ao_out (nullptr: tight).
-int record_upsample(MeaoCtx *c, int lo, void *ao_out, cudaStream_t s, const ArrayIO *aio = nullptr, const DepthIn *fused = nullptr,
-                    const ViewPitch *vp = nullptr)
+// PushUpsampleCommands with the wiring of AO.cs:528-531; the final level stores into ao_out (nullptr: the result buffer).
+int record_upsample(MeaoCtx *c, int lo, void *ao_out, cudaStream_t s)
 {
-    NvtxRange nv("meao::blur_upsample");
-    if (lo == 1) c->last_out = aio ? const_cast<void *>(aio->ao_array) : ao_out;
-    CUDA_TRY(c, launch_upsample(*c, lo, upsample_args(*c, lo, ao_out, vp), aio, fused, s));
-    c->launches++;
-    return 0;
+    return record_launch(c, FrameLaunch{kStageUpsample, lo, 0, -1, kPdlNever}, frame_io(c, nullptr, c->last_kind, ao_out, false), s);
 }
 
 // RAII: launches issued while one of these is alive (and `on`) carry the programmatic-dependent-launch attribute.
 struct PdlScope { bool prev; explicit PdlScope(bool on) : prev(g_launch_pdl) { g_launch_pdl = on; } ~PdlScope() { g_launch_pdl = prev; } };
 
-// The same nine launches as record_frame, recorded as a DAG on forked streams (for graph capture): the four
-// render levels are independent (SURVEY.md 3.2), the coarse upsample chain 4->3->2 only needs Occlusion2..4,
-// and only the last two upsamples wait for the big level-1 render.
-// pdl: 0 = plain edges; 1 = programmatic dependent launch on the kernels whose ONLY predecessor is the kernel before them in
-// the same stream; 2 = also on kernels that additionally wait for an event of another branch.  after_exchange: the node
-// before this DAG is the neighbour-exchange kernel, which spins on remote flags -- nothing may be scheduled "early" behind it
-// (a grid parked in griddepcontrol.wait holds SM resources that the neighbour band's kernels may need: see DESIGN.md 4).
-// aio: a CUDA-array frame -- the first and the last node read / write the arrays (depth and ao_out are unused).
-// depth != nullptr (not an array frame): the fused form -- prepare_depth runs low_only and the final upsample reads the raw depth and
-// writes LinearDepth; with do_prepare = false the caller has recorded that low_only prepare_depth of the same depth itself.
-int record_frame_dag(MeaoCtx *c, const void *depth, int kind, void *ao_out, cudaStream_t s, bool do_prepare = true, int pdl = 0,
-                     bool after_exchange = false, const ArrayIO *aio = nullptr, const ViewPitch *vp = nullptr)
+// The frame schedule from entry `first` on, recorded as a DAG on the caller's stream s and the forked streams (for graph capture):
+// an event is recorded after every launch a later one waits for.  first = 1: the caller has recorded the prepare, or a band's halo or
+// exchange kernel in its place; what waits for the prepare then waits for stream s as it stands here, so renders 2-4 still follow the
+// halo rows.  pdl: the level of frame_schedule's PDL classes.  after_exchange: the launch before this DAG is the neighbour-exchange
+// kernel, which spins on remote flags -- nothing may be scheduled "early" behind it (a grid parked in griddepcontrol.wait holds SM
+// resources that the neighbour band's kernels may need: see DESIGN.md 4), so the first launch goes without PDL.
+int record_frame_dag(MeaoCtx *c, const FrameIO &io, cudaStream_t s, size_t first, int pdl, bool after_exchange = false)
 {
-    int rc;
-    const bool fused = depth && !aio;
-    const DepthIn din = depth_in(*c, depth, kind, vp);
-    const DepthIn *fin = fused ? &din : nullptr;
-    if (c->variants.single_scale) {     // BASELINE.json configs[0]: Downsample1 -> Render level 1 -> final-style Upsample on Occlusion1
-        if (do_prepare && (rc = record_downsample(c, depth, kind, s, aio, fused, vp))) return rc;
-        { PdlScope p(pdl >= 1 && !after_exchange); if ((rc = record_render(c, 1, kind, s))) return rc; }
-        { PdlScope p(pdl >= 1); if ((rc = record_upsample(c, 1, ao_out, s, aio, fin, vp))) return rc; }
-        return 0;
+    const std::vector<FrameLaunch> sched = frame_schedule(c->plan.variants);
+    const cudaStream_t st[4] = {s, c->branch[0], c->branch[1], c->branch[2]};
+    std::vector<int> ev(sched.size(), -1);          // the event (of c->ev) recorded after launch i, if one waits for it: at most 4
+    int nev = 0;
+    for (const FrameLaunch &l : sched)
+        if (l.wait >= 0 && ev[l.wait] < 0) ev[l.wait] = nev++;
+    for (size_t i = 0; i < first; i++)
+        if (ev[i] >= 0) CUDA_TRY(c, cudaEventRecord(c->ev[ev[i]], st[sched[i].branch]));
+    for (size_t i = first; i < sched.size(); i++) {
+        const FrameLaunch &l = sched[i];
+        if (l.wait >= 0) CUDA_TRY(c, cudaStreamWaitEvent(st[l.branch], c->ev[ev[l.wait]], 0));
+        {
+            PdlScope p(pdl_on(l, pdl) && !(after_exchange && i == first));
+            int rc = record_entry(c, l, io, st[l.branch]);
+            if (rc) return rc;
+        }
+        if (ev[i] >= 0) CUDA_TRY(c, cudaEventRecord(c->ev[ev[i]], st[l.branch]));
     }
-    cudaStream_t b1 = c->branch[0], b2 = c->branch[1], b3 = c->branch[2];
-    if (do_prepare && (rc = record_downsample(c, depth, kind, s, aio, fused, vp))) return rc;
-    CUDA_TRY(c, cudaEventRecord(c->ev[0], s));
-    CUDA_TRY(c, cudaStreamWaitEvent(b1, c->ev[0], 0));
-    CUDA_TRY(c, cudaStreamWaitEvent(b2, c->ev[0], 0));
-    CUDA_TRY(c, cudaStreamWaitEvent(b3, c->ev[0], 0));
-    // the optional high-quality render of a level (kernel "main") rides on the branch of that level's interleaved render
-    { PdlScope p(pdl >= 1 && !after_exchange); if ((rc = record_render(c, 1, kind, s))) return rc; }
-    { PdlScope p(pdl >= 1); if (hq_level(*c, 1) && (rc = record_render(c, 1, kind, s, true))) return rc; }
-    if ((rc = record_render(c, 2, kind, b1))) return rc;
-    { PdlScope p(pdl >= 1); if (hq_level(*c, 2) && (rc = record_render(c, 2, kind, b1, true))) return rc; }
-    CUDA_TRY(c, cudaEventRecord(c->ev[1], b1));
-    if ((rc = record_render(c, 3, kind, b2))) return rc;
-    { PdlScope p(pdl >= 1); if (hq_level(*c, 3) && (rc = record_render(c, 3, kind, b2, true))) return rc; }
-    CUDA_TRY(c, cudaEventRecord(c->ev[2], b2));
-    if ((rc = record_render(c, 4, kind, b3))) return rc;
-    { PdlScope p(pdl >= 1); if (hq_level(*c, 4) && (rc = record_render(c, 4, kind, b3, true))) return rc; }
-    CUDA_TRY(c, cudaStreamWaitEvent(b3, c->ev[2], 0));
-    { PdlScope p(pdl >= 2); if ((rc = record_upsample(c, 4, nullptr, b3))) return rc; }
-    CUDA_TRY(c, cudaStreamWaitEvent(b3, c->ev[1], 0));
-    { PdlScope p(pdl >= 2); if ((rc = record_upsample(c, 3, nullptr, b3))) return rc; }
-    CUDA_TRY(c, cudaEventRecord(c->ev[3], b3));
-    CUDA_TRY(c, cudaStreamWaitEvent(s, c->ev[3], 0));
-    { PdlScope p(pdl >= 2); if ((rc = record_upsample(c, 2, nullptr, s))) return rc; }
-    { PdlScope p(pdl >= 1); if ((rc = record_upsample(c, 1, ao_out, s, aio, fin, vp))) return rc; }
     return 0;
 }
 
-// record order of RebuildCommandBuffers, AO.cs:511-531.  vp: the pitches of depth and ao_out (nullptr: tight).
-int record_frame(MeaoCtx *c, const void *depth, int kind, void *ao_out, cudaStream_t s, bool profile, const ViewPitch *vp = nullptr)
+// The frame schedule from entry `first` on, serially on stream s (MEAO_FLAG_NO_GRAPH, meao_render_band_finish).  profile: an event
+// pair around every launch (meao_profile_frame), each launched profile_repeats times.
+int record_frame(MeaoCtx *c, const FrameIO &io, cudaStream_t s, size_t first, bool profile)
 {
-    static const char *ren_names[5] = {"", "render_ao L1", "render_ao L2", "render_ao L3", "render_ao L4"};
-    static const char *hq_names[5] = {"", "render_ao_wide L1", "render_ao_wide L2", "render_ao_wide L3", "render_ao_wide L4"};
-    static const char *ups_names[5] = {"", "blur_upsample L1->L0", "blur_upsample L2->L1", "blur_upsample L3->L2", "blur_upsample L4->L3"};
-    std::vector<const char *> names;
+    const std::vector<FrameLaunch> sched = frame_schedule(c->plan.variants);
     std::vector<cudaEvent_t> ev;
     auto mark = [&]() { if (profile) { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, s); ev.push_back(e); } };
     const int reps = profile ? c->profile_repeats : 1;         // every kernel is idempotent (out of place), so repeating it is harmless
-    int rc = 0;
     mark();
-    const DepthIn din = depth_in(*c, depth, kind, vp);      // the fused form of record_frame_dag
-    for (int r = 0; r < reps && !rc; r++) rc = record_downsample(c, depth, kind, s, nullptr, true, vp);
-    if (rc) return rc;
-    names.push_back("prepare_depth"); mark();
-    const int kmax = c->variants.single_scale ? 1 : 4;       // single-scale: Render level 1 + the final-style Upsample only
-    for (int k = 1; k <= kmax; k++) { for (int r = 0; r < reps && !rc; r++) rc = record_render(c, k, kind, s); if (rc) return rc; names.push_back(ren_names[k]); mark(); }
-    for (int k = 1; k <= kmax; k++) if (hq_level(*c, k)) { for (int r = 0; r < reps && !rc; r++) rc = record_render(c, k, kind, s, true); if (rc) return rc; names.push_back(hq_names[k]); mark(); }
-    for (int lo = kmax; lo >= 1; lo--) { for (int r = 0; r < reps && !rc; r++) rc = record_upsample(c, lo, lo == 1 ? ao_out : nullptr, s, nullptr, lo == 1 ? &din : nullptr, vp); if (rc) return rc; names.push_back(ups_names[lo]); mark(); }
+    for (size_t i = first; i < sched.size(); i++) {
+        for (int r = 0; r < reps; r++) { int rc = record_entry(c, sched[i], io, s); if (rc) return rc; }
+        mark();
+    }
     if (profile) {
         CUDA_TRY(c, cudaStreamSynchronize(s));
         c->last_profile.clear();
         for (size_t i = 0; i + 1 < ev.size(); i++) {
             float ms = 0; cudaEventElapsedTime(&ms, ev[i], ev[i + 1]);
-            c->last_profile.push_back({names[i], ms / (float)reps});
+            c->last_profile.push_back({launch_name(sched[first + i]), ms / (float)reps});
         }
         for (auto e : ev) cudaEventDestroy(e);
     }
@@ -1084,12 +1072,7 @@ int meao_render_band_finish(MeaoCtx *c, void *ao_out, void *stream)
 {
     BAND_GUARD(c, "meao_render_band_finish");
     int rc = ensure_ready(c); if (rc) return rc;
-    cudaStream_t s = (cudaStream_t)stream;
-    const int kind = c->last_kind;
-    for (int k = 1; k <= 4; k++) if ((rc = record_render(c, k, kind, s))) return rc;
-    for (int k = 1; k <= 4; k++) if (hq_level(*c, k) && (rc = record_render(c, k, kind, s, true))) return rc;
-    for (int lo = 4; lo >= 1; lo--) if ((rc = record_upsample(c, lo, lo == 1 ? ao_out : nullptr, s))) return rc;
-    return MEAO_OK;
+    return record_frame(c, frame_io(c, nullptr, c->last_kind, ao_out, false), (cudaStream_t)stream, 1, false);
 }
 
 static int halo_kernel(MeaoCtx *c, void *up, void *down, bool pack, cudaStream_t s)
@@ -1117,8 +1100,8 @@ static int halo_kernel(MeaoCtx *c, void *up, void *down, bool pack, cudaStream_t
 
 // ---- graph cache ----------------------------------------------------------------------------------------------------
 // record(stream, pdl) issues the launches; it is captured into a graph, with the highest programmatic-dependent-launch
-// level the runtime accepts (tried once per context: 2, then 1, then 0 = plain edges).
-static int capture_graph(MeaoCtx *c, const std::function<int(cudaStream_t, int)> &record, cudaGraph_t *out)
+// level the runtime accepts (tried once per context: 2, then 1, then 0 = plain edges).  *launches: the kernels it recorded.
+static int capture_graph(MeaoCtx *c, const std::function<int(cudaStream_t, int)> &record, cudaGraph_t *out, int *launches)
 {
     const char *env = getenv("MEAO_PDL");                           // tuning / debugging aid: cap the level (0 disables)
     const int cap = (env && env[0] >= '0' && env[0] <= '2') ? env[0] - '0' : 2;
@@ -1127,6 +1110,7 @@ static int capture_graph(MeaoCtx *c, const std::function<int(cudaStream_t, int)>
         CUDA_TRY(c, cudaStreamBeginCapture(c->stream, cudaStreamCaptureModeThreadLocal));
         const int64_t before = c->launches;
         const int rc = record(c->stream, level);
+        *launches = (int)(c->launches - before);
         c->launches = before;
         const cudaError_t e = cudaStreamEndCapture(c->stream, &g);
         if (rc == 0 && e == cudaSuccess) { c->pdl_level = level; *out = g; return 0; }
@@ -1161,7 +1145,8 @@ static void reclaim_retired(MeaoCtx *c, bool wait)
     }
 }
 
-static int launch_cached(MeaoCtx *c, const MeaoCtx::GraphKey &key_in, cudaStream_t s, int nk, const std::function<int(cudaStream_t, int)> &record)
+// Replays the graph of `key`, captured from record(stream, pdl) on first use; a replay counts the launches its capture recorded.
+static int launch_cached(MeaoCtx *c, const MeaoCtx::GraphKey &key_in, cudaStream_t s, const std::function<int(cudaStream_t, int)> &record)
 {
     if (c->flags & MEAO_FLAG_NO_GRAPH) return record(s, 0);
     MeaoCtx::GraphKey key = key_in;
@@ -1171,7 +1156,8 @@ static int launch_cached(MeaoCtx *c, const MeaoCtx::GraphKey &key_in, cudaStream
     if (it == c->graphs.end()) {
         if (!c->retired.empty()) reclaim_retired(c, c->retired.size() >= kMaxRetired);
         cudaGraph_t g = nullptr;
-        int rc = capture_graph(c, record, &g);
+        int launches = 0;
+        int rc = capture_graph(c, record, &g, &launches);
         if (rc) return rc;
         cudaGraphExec_t ge = nullptr;
         if (c->graphs.size() >= kMaxGraphs) {
@@ -1198,19 +1184,19 @@ static int launch_cached(MeaoCtx *c, const MeaoCtx::GraphKey &key_in, cudaStream
                 cudaGetLastError();
                 cudaGraphDestroy(g); g = nullptr;
                 c->pdl_level = 0;
-                if ((rc = capture_graph(c, record, &g))) return rc;
+                if ((rc = capture_graph(c, record, &g, &launches))) return rc;
                 e = cudaGraphInstantiate(&ge, g, 0);
             }
             if (e != cudaSuccess) { if (g) cudaGraphDestroy(g); return fail(c, MEAO_ERR_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(e)); }
             c->graph_instantiations++;
         }
         cudaGraphDestroy(g);
-        it = c->graphs.emplace(key, MeaoCtx::GraphEntry{ge, 0}).first;
+        it = c->graphs.emplace(key, MeaoCtx::GraphEntry{ge, 0, launches}).first;
     }
     it->second.last_use = ++c->graph_clock;
     CUDA_TRY(c, cudaGraphLaunch(it->second.exec, s));
     if (retiring) CUDA_TRY(c, cudaEventRecord(c->retired.back().done, s));    // after the frame that replaced it
-    c->launches += nk;
+    c->launches += it->second.launches;
     return 0;
 }
 
@@ -1221,8 +1207,7 @@ int meao_band_phase_a(MeaoCtx *c, const void *depth, int32_t kind, void *send_up
     if (!depth) return fail(c, MEAO_ERR_INVALID, "depth is NULL");
     c->last_kind = kind;
     const MeaoCtx::GraphKey key{{depth, send_up, send_down, nullptr}, 100 + kind};
-    const int nk = 1 + ((send_up || send_down) ? 1 : 0);
-    return launch_cached(c, key, (cudaStream_t)stream, nk, [&](cudaStream_t s, int pdl) {
+    return launch_cached(c, key, (cudaStream_t)stream, [&](cudaStream_t s, int pdl) {
         int r = record_downsample(c, depth, kind, s);
         if (r) return r;
         PdlScope p(pdl >= 1);
@@ -1237,12 +1222,11 @@ int meao_band_phase_b(MeaoCtx *c, const void *recv_up, const void *recv_down, vo
     if (!ao_out) return fail(c, MEAO_ERR_INVALID, "ao_out is NULL");
     const int kind = c->last_kind;
     const MeaoCtx::GraphKey key{{recv_up, recv_down, ao_out, nullptr}, 200 + kind};
-    const int nk = meao_kernels_per_frame(c) - 1 + ((recv_up || recv_down) ? 1 : 0);
     c->last_out = ao_out;
-    return launch_cached(c, key, (cudaStream_t)stream, nk, [&](cudaStream_t s, int pdl) {
+    return launch_cached(c, key, (cudaStream_t)stream, [&](cudaStream_t s, int pdl) {
         int r = halo_kernel(c, (void *)recv_up, (void *)recv_down, false, s);
         if (r) return r;
-        return record_frame_dag(c, nullptr, kind, ao_out, s, false, pdl);
+        return record_frame_dag(c, frame_io(c, nullptr, kind, ao_out, false), s, 1, pdl);
     });
 }
 
@@ -1368,12 +1352,11 @@ int meao_band_step(MeaoCtx *c, const void *depth, int32_t kind, void *ao_out, vo
     c->last_kind = kind; c->last_out = ao_out;
     const MeaoCtx::GraphKey key{{depth, ao_out, c->peer_base[0], c->peer_base[1]}, 300 + kind};
     const bool has_peer = c->peer_base[0] || c->peer_base[1];
-    const int nk = meao_kernels_per_frame(c) + (has_peer ? 1 : 0);
-    return launch_cached(c, key, (cudaStream_t)stream, nk, [&](cudaStream_t s, int pdl) {
-        int r = record_downsample(c, depth, kind, s, nullptr, true);
+    return launch_cached(c, key, (cudaStream_t)stream, [&](cudaStream_t s, int pdl) {
+        int r = record_downsample(c, depth, kind, s, true);
         if (r) return r;
         { PdlScope p(pdl >= 1); if ((r = record_exchange(c, s))) return r; }
-        return record_frame_dag(c, depth, kind, ao_out, s, false, pdl, has_peer);
+        return record_frame_dag(c, frame_io(c, depth, kind, ao_out, true), s, 1, pdl, has_peer);
     });
 }
 
@@ -1462,15 +1445,15 @@ int render_views(MeaoCtx *c, const void *depth, int kind, void *ao_out, ViewPitc
     int rc;
     if ((rc = check_views(c, depth, kind, ao_out, &p))) return rc;
     cudaStream_t s = (cudaStream_t)stream;
-    if (c->flags & MEAO_FLAG_NO_GRAPH) return record_frame(c, depth, kind, ao_out, s, false, &p);
+    if (c->flags & MEAO_FLAG_NO_GRAPH) return record_frame(c, frame_io(c, depth, kind, ao_out, true, &p), s, 0, false);
 
     // plan-once / replay: one captured graph per (depth, out, kind, pitches), like the reference's command buffer
     // that is re-recorded only when something changed (AO.cs:334-347)
     NvtxRange nv("meao::frame");
     const MeaoCtx::GraphKey key{{depth, ao_out, nullptr, nullptr}, kind, {p.depth_row, p.depth_layer, p.ao_row, p.ao_layer}};
     c->last_kind = kind; c->last_out = ao_out;
-    return launch_cached(c, key, s, meao_kernels_per_frame(c), [&](cudaStream_t cs, int pdl) {
-        return record_frame_dag(c, depth, kind, ao_out, cs, true, pdl, false, nullptr, &p);
+    return launch_cached(c, key, s, [&](cudaStream_t cs, int pdl) {
+        return record_frame_dag(c, frame_io(c, depth, kind, ao_out, true, &p), cs, 0, pdl);
     });
 }
 }  // namespace
@@ -1570,8 +1553,10 @@ int meao_render_arrays(MeaoCtx *c, const void *depth_array, int32_t kind, void *
     NvtxRange nv("meao::frame_arrays");
     const MeaoCtx::GraphKey key{{depth_array, ao_array, nullptr, nullptr}, kArrayGraphKind + kind};
     c->last_kind = kind; c->last_out = ao_array;
-    return launch_cached(c, key, (cudaStream_t)stream, meao_kernels_per_frame(c), [&](cudaStream_t cs, int pdl) {
-        return record_frame_dag(c, nullptr, kind, nullptr, cs, true, pdl, false, &io);
+    return launch_cached(c, key, (cudaStream_t)stream, [&](cudaStream_t cs, int pdl) {
+        FrameIO fio = frame_io(c, nullptr, kind, nullptr, false);
+        fio.aio = &io;
+        return record_frame_dag(c, fio, cs, 0, pdl);
     });
 }
 
@@ -1952,10 +1937,7 @@ int64_t meao_launch_count(const MeaoCtx *c) { return c ? c->launches : 0; }
 int meao_pdl_level(const MeaoCtx *c) { return c ? c->pdl_level : -1; }
 int meao_kernels_per_frame(const MeaoCtx *c)
 {
-    if (c && c->variants.single_scale) return 3;      // Downsample1 + Render level 1 + the final-style Upsample
-    int n = 9;
-    if (c) for (int k = 1; k <= 4; k++) n += (c->variants.high_quality_mask >> (k - 1)) & 1;     // as set: the plan may not be rebuilt yet
-    return n;
+    return (int)frame_schedule(c ? c->variants : MeaoVariants{}).size();        // as set: the plan may not be rebuilt yet
 }
 
 int64_t meao_algorithmic_bytes(const MeaoCtx *c, int32_t stage)
@@ -2013,7 +1995,7 @@ int meao_profile_frame(MeaoCtx *c, const void *depth, int32_t kind, void *ao_out
     int rc = frame_ready(c, c->stream); if (rc) return rc;
     if (!depth || !ao_out) return fail(c, MEAO_ERR_INVALID, "depth / ao_out is NULL");
     CUDA_TRY(c, cudaDeviceSynchronize());
-    if ((rc = record_frame(c, depth, kind, ao_out, c->stream, true))) return rc;
+    if ((rc = record_frame(c, frame_io(c, depth, kind, ao_out, true), c->stream, 0, true))) return rc;
     const int n = (int)c->last_profile.size();
     for (int i = 0; i < n && i < capacity; i++) {
         if (ms_out) ms_out[i] = c->last_profile[i].second;

@@ -49,6 +49,7 @@ def lib() -> C.CDLL:
         l.frame_debug_view.argtypes = [P, I, P]
         l.frame_composite.argtypes = [P, P, LL, I, I, I, I]
         l.frame_composite_debug.argtypes = [P, P, LL, I]
+        l.frame_schedule_export.argtypes = [P, P, P, I]
         l.frame_tma_box_loads.restype = LL
         l.frame_surface_accesses.restype = LL
         _lib = l
@@ -273,6 +274,24 @@ class Frame:
         out = np.zeros((self.H, self.W), np.uint8)
         assert self._lib.frame_debug_view(self._h, bid, out.ctypes.data) == 0
         return out
+
+
+STAGES = ("prepare", "render", "render_wide", "upsample")    # frame_record.h FrameStage
+PDL = ("never", ">=1", ">=2")                                # frame_record.h PdlClass
+
+
+def schedule(variants=(0, 0, 0, 0)) -> list:
+    """frame_record.h frame_schedule of MeaoVariants (single_pass_stereo, sample_exhaustively, high_quality_mask, single_scale): one
+    (stage, level, branch, wait, pdl, name) per launch in serial order; wait is the index of the launch waited for, or None."""
+    cap = 32
+    out, names = (C.c_int * (5 * cap))(), C.create_string_buffer(32 * cap)
+    n = lib().frame_schedule_export((C.c_int * 4)(*variants), out, names, cap)
+    assert 0 < n <= cap
+    rows = []
+    for i in range(n):
+        stage, level, branch, wait, pdl = out[5 * i:5 * i + 5]
+        rows.append((STAGES[stage], level, branch, None if wait < 0 else wait, PDL[pdl], names.raw[32 * i:32 * (i + 1)].split(b"\0")[0].decode()))
+    return rows
 
 
 def composite(ao: np.ndarray, color: np.ndarray, *, rgb: bool, alpha: bool, one_minus: bool) -> np.ndarray:

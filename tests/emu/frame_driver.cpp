@@ -1,7 +1,9 @@
 // frame_driver.cpp -- runs frames through the HOST-compiled kernel sources (TEST INFRASTRUCTURE ONLY, see cuda_emu.h), launched the
-// way libmeao launches them: buffer placement, TMA maps, argument blocks and launcher choice all come from csrc/frame_record.h, the
-// code meao_api.cu records its frames with.  What this driver adds is a host arena, the plan (the constants a plan-only libmeao
-// context reports, handed in by the test) and the launch sequence of each frame form.
+// way libmeao launches them: buffer placement, TMA maps, the frame schedule, argument blocks and launcher choice all come from
+// csrc/frame_record.h, the code meao_api.cu records its frames with.  What this driver adds is a host arena, the plan (the constants a
+// plan-only libmeao context reports, handed in by the test) and what each frame form puts into its first and last launch.
+#include <algorithm>
+#include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <vector>
@@ -44,29 +46,23 @@ void whole_frame(Frame *f)
     for (int k = 0; k <= 4; k++) f->need_c[k] = Range{0, f->lh[k]};
 }
 
-void prepare(Frame *f, const void *depth, int kind, const ViewPitch *vp, const ArrayIO *aio, bool low_only)
+// The caller's depth (pitches vp, nullptr: tight) as the frame's first launch reads it
+FrameIO frame_io(Frame *f, const void *depth, int kind, const ViewPitch *vp = nullptr)
 {
-    f->kind = kind;
-    PrepareArgs a = prepare_args(*f, depth_in(*f, depth, kind, vp));
-    if (f->zero_pitches) { a.depth_pitch = 0; a.depth_layer_pitch = 0; }
-    launch_prepare(*f, a, aio, low_only, nullptr);
+    FrameIO io;
+    io.kind = kind; io.depth = depth_in(*f, depth, kind, vp);
+    if (f->zero_pitches) { io.depth.depth_pitch = 0; io.depth.depth_layer_pitch = 0; io.depth.ao_layer_pitch = 0; }
+    return io;
 }
 
-void render(Frame *f, int k, bool wide) { launch_render(*f, render_args(*f, k, f->kind, wide, f->ren_tile), k, f->kind, nullptr); }
-
-void upsample(Frame *f, int lo, void *ao = nullptr, const ViewPitch *vp = nullptr, const ArrayIO *aio = nullptr, const DepthIn *fused = nullptr)
+// Launches [first, end) of the frame schedule, serially, through the shared launcher
+void run_schedule(Frame *f, const FrameIO &io, size_t first, size_t end = SIZE_MAX)
 {
-    if (lo == 1) f->ao_elsewhere = ao || aio;
-    launch_upsample(*f, lo, upsample_args(*f, lo, ao, vp), aio, fused, nullptr);
-}
-
-// the launches of a frame between its prepare_depth and its final upsample, in meao_api.cu record_frame's order
-void levels(Frame *f)
-{
-    const int kmax = f->plan.variants.single_scale ? 1 : 4;
-    for (int k = 1; k <= kmax; k++) render(f, k, false);
-    for (int k = 1; k <= kmax; k++) if (hq_level(*f, k)) render(f, k, true);
-    for (int lo = kmax; lo >= 2; lo--) upsample(f, lo);
+    const std::vector<FrameLaunch> s = frame_schedule(f->plan.variants);
+    end = std::min(end, s.size());
+    if (first == 0) f->kind = io.kind;
+    if (end == s.size()) f->ao_elsewhere = io.ao || io.aio;
+    for (size_t i = first; i < end; i++) launch_entry(*f, s[i], io, f->ren_tile, nullptr);
 }
 
 }  // namespace
@@ -165,17 +161,15 @@ void frame_run(void *h, const void *depth, int kind, int fused, long long depth_
     Frame *f = F(h);
     whole_frame(f);
     const ViewPitch v{depth_row, depth_layer, ao_row, ao_layer}, *vp = depth_row ? &v : nullptr;
-    const bool band = row1 > row0;
-    prepare(f, depth, kind, vp, nullptr, fused && !band);
-    levels(f);
-    if (!fused) { upsample(f, 1, ao, vp); return; }
-    if (band) {
-        f->band0 = f->need_c[0].lo = row0; f->band1 = f->need_c[0].hi = row1;
-        depth = (const char *)depth + (size_t)row0 * (depth_row ? depth_row : f->W * depth_esize(kind));
-    }
-    DepthIn din = depth_in(*f, depth, kind, vp);
-    if (f->zero_pitches) { din.depth_pitch = 0; din.depth_layer_pitch = 0; din.ao_layer_pitch = 0; }
-    upsample(f, 1, ao, vp, nullptr, &din);
+    const bool band = fused && row1 > row0;
+    FrameIO io = frame_io(f, depth, kind, vp);
+    io.low_only = fused && !band; io.fused = fused != 0; io.ao = ao; io.vp = vp;
+    if (!band) { run_schedule(f, io, 0); return; }
+    const size_t n = frame_schedule(f->plan.variants).size();
+    run_schedule(f, io, 0, n - 1);
+    f->band0 = f->need_c[0].lo = row0; f->band1 = f->need_c[0].hi = row1;
+    io.depth = frame_io(f, (const char *)depth + (size_t)row0 * (depth_row ? depth_row : f->W * depth_esize(kind)), kind, vp).depth;
+    run_schedule(f, io, n - 1);
     whole_frame(f);
 }
 
@@ -183,7 +177,9 @@ void frame_run(void *h, const void *depth, int kind, int fused, long long depth_
 void frame_prepare_low(void *h, const void *depth, int kind)
 {
     whole_frame(F(h));
-    prepare(F(h), depth, kind, nullptr, nullptr, true);
+    FrameIO io = frame_io(F(h), depth, kind);
+    io.low_only = true;
+    run_schedule(F(h), io, 0, 1);
 }
 
 // A CUDA-array frame (meao_render_arrays): depth: `layers` images of W x H elements (4 bytes: f32, 2 bytes: D16 codes) with rows
@@ -197,9 +193,9 @@ void frame_run_arrays(void *h, void *depth, int kind, int depth_shape, long long
     // what meao_api.cu check_array derives from an array: how the kernels address its layers
     auto surf_kind = [](int shape) { return shape == meao_emu::SURF_2D ? kSurf2D : shape == meao_emu::SURF_LAYERED ? kSurfLayered : kSurfCube; };
     const ArrayIO aio{(cudaSurfaceObject_t)&ds, (cudaSurfaceObject_t)&as, surf_kind(depth_shape), surf_kind(ao_shape), ao};
-    prepare(f, nullptr, kind, nullptr, &aio, false);
-    levels(f);
-    upsample(f, 1, nullptr, nullptr, &aio);
+    FrameIO io = frame_io(f, nullptr, kind);
+    io.aio = &aio;
+    run_schedule(f, io, 0);
 }
 
 // ---- row bands: the two phases of meao_band_phase_a / _b around the neighbour exchange ----------------------------------
@@ -212,9 +208,10 @@ void frame_set_band(void *h, int row0, int row1, const int *produce10)
 }
 
 // depth_band: the band's rows only (row1 - row0 rows), like meao_render_band_prepare
-void frame_band_phase_a(void *h, const void *depth_band, int kind) { prepare(F(h), depth_band, kind, nullptr, nullptr, false); }
+void frame_band_phase_a(void *h, const void *depth_band, int kind) { run_schedule(F(h), frame_io(F(h), depth_band, kind), 0, 1); }
 
-void frame_band_phase_b(void *h) { levels(F(h)); upsample(F(h), 1); }
+// the launches after the prepare into the result buffer, like meao_band_phase_b and meao_render_band_finish
+void frame_band_phase_b(void *h) { run_schedule(F(h), frame_io(F(h), nullptr, F(h)->kind), 1); }
 
 // rows8 = meao_halo_rows(side, send): {lo1,hi1, ..., lo4,hi4}; packed message layout of meao_halo_pack (level 1 first, tight rows)
 void frame_halo(void *h, const int *rows8, float *packed, int pack)
@@ -293,7 +290,8 @@ int frame_get_buffer(void *h, int id, int layer, void *out)
 {
     Frame *f = F(h);
     if (layer < 0 || layer >= f->layers) return -1;
-    if (id == 17 && f->ao_elsewhere) upsample(f, 1);    // meao_get_buffer: the context's own copy of an AO stored elsewhere
+    if (id == 17 && f->ao_elsewhere)                    // meao_get_buffer: the context's own copy of an AO stored elsewhere
+        launch_entry(*f, frame_schedule(f->plan.variants).back(), FrameIO{}, f->ren_tile, nullptr);
     auto copy2d = [&](const void *src, size_t pitch_bytes, int w, int hgt, int elem) {
         src = (const char *)src + (size_t)layer * hgt * pitch_bytes;       // layer l starts l x rows x pitch after layer 0
         for (int y = 0; y < hgt; y++) memcpy((char *)out + (size_t)y * w * elem, (const char *)src + (size_t)y * pitch_bytes, (size_t)w * elem);
@@ -340,6 +338,22 @@ void frame_composite(const uint8_t *ao, void *color, long long npix, int half, i
 }
 
 void frame_composite_debug(const uint8_t *view, void *color, long long npix, int half) { launch_debug_composite(view, color, npix, half, nullptr); }
+
+// ---- the frame schedule ------------------------------------------------------------------------------------------------------------
+// frame_schedule of variants4 = MeaoVariants {single_pass_stereo, sample_exhaustively, high_quality_mask, single_scale}: launch i as
+// out5[5 i .. 5 i + 4] = stage, level, branch, wait, PDL class, and its meao_profile_frame name at names + 32 i.  Returns the count.
+int frame_schedule_export(const int *variants4, int *out5, char *names, int cap)
+{
+    const MeaoVariants v{variants4[0], variants4[1], variants4[2], variants4[3]};
+    const std::vector<FrameLaunch> s = frame_schedule(v);
+    for (size_t i = 0; i < s.size() && (int)i < cap; i++) {
+        const FrameLaunch &l = s[i];
+        const int row[5] = {l.stage, l.level, l.branch, l.wait, l.pdl};
+        memcpy(out5 + 5 * i, row, sizeof row);
+        snprintf(names + 32 * i, 32, "%s", launch_name(l).c_str());
+    }
+    return (int)s.size();
+}
 
 // ---- counters and self-checks -----------------------------------------------------------------------------------------------------
 long long frame_tma_box_loads() { return meao_emu::tma_box_loads; }

@@ -23,7 +23,7 @@ def _plan(W, H, **kw):
     p = AmbientOcclusion(cam, device=-1)
     for py, cs in (("noise_filter_tolerance", "noiseFilterTolerance"), ("blur_tolerance", "blurTolerance"), ("upsample_tolerance", "upsampleTolerance"),
                    ("thickness_modifier", "thicknessModifier"), ("intensity", "intensity"), ("sample_exhaustively", "sampleExhaustively"),
-                   ("high_quality_mask", "highQualityMask")):
+                   ("high_quality_mask", "highQualityMask"), ("single_scale", "singleScale")):
         if py in kw:
             setattr(p, cs, kw[py])
     return p
@@ -231,18 +231,21 @@ def _band_frames(W, H, nb, **kw):
     return cuts, frames
 
 
-@pytest.mark.parametrize("W,H,nb", [(200, 528, 2), (130, 1296, 3)])
-def test_native_exchange_kernel_bands_equal_whole_frame(W, H, nb):
+@pytest.mark.parametrize("W,H,nb,single_scale", [(200, 528, 2, False), (130, 1296, 3, False), (200, 528, 2, True)],
+                         ids=["200-528-2", "130-1296-3", "200-528-2-single_scale"])
+def test_native_exchange_kernel_bands_equal_whole_frame(W, H, nb, single_scale):
     """band_exchange_kernel (peer stores + epoch flags): each band pushes its border rows of LowDepth1..4 straight into the
     neighbours' buffers (NaN-poisoned beforehand); the union of the bands must equal the whole-frame oracle bit for bit.
     The fiber emulator runs one grid at a time, so the flags a CONCURRENT neighbour would have raised are preset for the band
-    that runs first; every later band finds them raised by the kernels that already ran."""
+    that runs first; every later band finds them raised by the kernels that already ran.  single_scale: phase b is render 1 and
+    the final-style upsample, as in libmeao's frame schedule."""
     depth = synth.lin01_to_raw(synth.random_depth(W, H, seed=3))
-    ref = Oracle(W, H, threads=4, intensity=1.1).run(depth)
+    okw = dict(threads=4, intensity=1.1, single_scale=single_scale)
+    ref = Oracle(W, H, **okw).run(depth)
     for frame_no in (1, 2):                                      # two epochs through the same flags
-        cuts, frames = (_band_frames(W, H, nb, intensity=1.1)) if frame_no == 1 else (cuts, frames)
+        cuts, frames = (_band_frames(W, H, nb, intensity=1.1, single_scale=single_scale)) if frame_no == 1 else (cuts, frames)
         d = depth if frame_no == 1 else depth[:, ::-1].copy()
-        want = ref if frame_no == 1 else Oracle(W, H, threads=4, intensity=1.1).run(d)
+        want = ref if frame_no == 1 else Oracle(W, H, **okw).run(d)
         for i, f in enumerate(frames):
             if frame_no == 2:
                 f.poison_low()
