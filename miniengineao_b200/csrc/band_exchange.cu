@@ -88,6 +88,8 @@ __global__ void __launch_bounds__(kXchgThreads) band_exchange_kernel(const XchgA
 #endif
 }
 
+const Kernel<XchgArgs> kKernels[] = {band_exchange_kernel};
+
 }  // namespace
 
 cudaError_t launch_band_exchange(const XchgArgs &a, cudaStream_t s)
@@ -98,8 +100,6 @@ cudaError_t launch_band_exchange(const XchgArgs &a, cudaStream_t s)
     return cudaGetLastError();
 }
 
-#ifndef MEAO_EMULATE
-cudaError_t preload_band_exchange_kernel() { return preload_kernel(band_exchange_kernel); }
-#endif
+const KernelUnit kBandExchangeUnit = {"band_exchange.cu", [](cudaError_t *load) { return walk_kernels(load, kKernels); }};
 
 }  // namespace meao

@@ -29,6 +29,11 @@ namespace {
 #undef MEAO_UPS_LAYERED
 #undef MEAO_UPS_ARRAY
 
+const struct {      // [upsample_slot]: the final level's slot only
+    Kernel<CUtensorMap, CUtensorMap, UpsampleArgs, int, int, cudaSurfaceObject_t, int> plain[kUpsampleSlots];
+    Kernel<CUtensorMap, CUtensorMap, CUtensorMap, UpsamplePreminArgs, int, int, cudaSurfaceObject_t, int> premin[kUpsampleSlots];
+} kKernels = {MEAO_UPSAMPLE_SLOTS(blur_upsample_array_kernel, MEAO_NO_SLOT), MEAO_UPSAMPLE_SLOTS(blur_upsample_premin_array_kernel, MEAO_NO_SLOT)};
+
 }  // namespace
 
 cudaError_t launch_blur_upsample_array(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
@@ -43,25 +48,18 @@ cudaError_t launch_blur_upsample_array(const CUtensorMap &lo_depth_map, const CU
     a.out_vec_ok = 1;               // surface stores have no alignment requirement
     dim3 grid;
     if (!ups_tile_grid(a, layers, sm_count, &grid)) return cudaErrorInvalidValue;
-    const int t = use_tma ? 1 : 0;
+    const int t = use_tma ? 1 : 0, k = upsample_slot(a);
     if (!lo_ao2) {
-        MEAO_LAUNCH((blur_upsample_array_kernel<false, true>), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, a, t, layers, out, surf_kind);
+        MEAO_LAUNCH((kKernels.plain[k]), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, a, t, layers, out, surf_kind);
     } else {        // main_premin
         if (!lo_ao2_map) return cudaErrorInvalidValue;
         const UpsamplePreminArgs pa{a, lo_ao2, lo_a2pitch};
-        MEAO_LAUNCH((blur_upsample_premin_array_kernel<false, true>), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, *lo_ao2_map, pa, t, layers, out, surf_kind);
+        MEAO_LAUNCH((kKernels.premin[k]), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, *lo_ao2_map, pa, t, layers, out, surf_kind);
     }
     return cudaGetLastError();
 }
 
-#ifndef MEAO_EMULATE
-cudaError_t preload_blur_upsample_array()
-{
-    cudaError_t e = cudaSuccess;
-    auto t = [&](auto k) { if (e == cudaSuccess) e = preload_kernel(k); };
-    t(blur_upsample_array_kernel<false, true>); t(blur_upsample_premin_array_kernel<false, true>);
-    return e;
-}
-#endif
+const KernelUnit kBlurUpsampleArrayUnit = {"blur_upsample_array.cu",
+                                           [](cudaError_t *load) { return walk_kernels(load, kKernels.plain, kKernels.premin); }};
 
 }  // namespace meao

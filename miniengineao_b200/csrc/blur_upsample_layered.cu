@@ -24,6 +24,11 @@ namespace {
 #undef MEAO_UPS_PREMIN
 #undef MEAO_UPS_LAYERED
 
+const struct {      // [upsample_slot]
+    Kernel<CUtensorMap, CUtensorMap, UpsampleArgs, int, int> plain[kUpsampleSlots];
+    Kernel<CUtensorMap, CUtensorMap, CUtensorMap, UpsamplePreminArgs, int, int> premin[kUpsampleSlots];
+} kKernels = {MEAO_UPSAMPLE_SLOTS(blur_upsample_layered_kernel, MEAO_SLOT), MEAO_UPSAMPLE_SLOTS(blur_upsample_premin_layered_kernel, MEAO_SLOT)};
+
 }  // namespace
 
 cudaError_t launch_blur_upsample_layered(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
@@ -34,40 +39,18 @@ cudaError_t launch_blur_upsample_layered(const CUtensorMap &lo_depth_map, const 
     UpsampleArgs a = a_in;
     dim3 grid;
     if (!ups_tile_grid(a, layers, sm_count, &grid)) return cudaErrorInvalidValue;
-    const int t = use_tma ? 1 : 0;
+    const int t = use_tma ? 1 : 0, k = upsample_slot(a);
     if (!lo_ao2) {
-        if (a.hi_ao) {
-            if (a.hi_is_half) MEAO_LAUNCH((blur_upsample_layered_kernel<true, true>), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, a, t, layers);
-            else              MEAO_LAUNCH((blur_upsample_layered_kernel<true, false>), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, a, t, layers);
-        } else {
-            if (a.hi_is_half) MEAO_LAUNCH((blur_upsample_layered_kernel<false, true>), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, a, t, layers);
-            else              MEAO_LAUNCH((blur_upsample_layered_kernel<false, false>), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, a, t, layers);
-        }
+        MEAO_LAUNCH((kKernels.plain[k]), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, a, t, layers);
     } else {        // main_premin / main_premin_blendout
         if (!lo_ao2_map) return cudaErrorInvalidValue;
         const UpsamplePreminArgs pa{a, lo_ao2, lo_a2pitch};
-        if (a.hi_ao) {
-            if (a.hi_is_half) MEAO_LAUNCH((blur_upsample_premin_layered_kernel<true, true>), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, *lo_ao2_map, pa, t, layers);
-            else              MEAO_LAUNCH((blur_upsample_premin_layered_kernel<true, false>), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, *lo_ao2_map, pa, t, layers);
-        } else {
-            if (a.hi_is_half) MEAO_LAUNCH((blur_upsample_premin_layered_kernel<false, true>), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, *lo_ao2_map, pa, t, layers);
-            else              MEAO_LAUNCH((blur_upsample_premin_layered_kernel<false, false>), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, *lo_ao2_map, pa, t, layers);
-        }
+        MEAO_LAUNCH((kKernels.premin[k]), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, *lo_ao2_map, pa, t, layers);
     }
     return cudaGetLastError();
 }
 
-#ifndef MEAO_EMULATE
-cudaError_t preload_blur_upsample_layered()
-{
-    cudaError_t e = cudaSuccess;
-    auto t = [&](auto k) { if (e == cudaSuccess) e = preload_kernel(k); };
-    t(blur_upsample_layered_kernel<true, true>); t(blur_upsample_layered_kernel<true, false>);
-    t(blur_upsample_layered_kernel<false, true>); t(blur_upsample_layered_kernel<false, false>);
-    t(blur_upsample_premin_layered_kernel<true, true>); t(blur_upsample_premin_layered_kernel<true, false>);
-    t(blur_upsample_premin_layered_kernel<false, true>); t(blur_upsample_premin_layered_kernel<false, false>);
-    return e;
-}
-#endif
+const KernelUnit kBlurUpsampleLayeredUnit = {"blur_upsample_layered.cu",
+                                             [](cudaError_t *load) { return walk_kernels(load, kKernels.plain, kKernels.premin); }};
 
 }  // namespace meao

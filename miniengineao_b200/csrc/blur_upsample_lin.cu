@@ -89,19 +89,13 @@ __device__ __forceinline__ UpsamplePreminArgs layer_args(const UpsamplePreminArg
 #undef MEAO_UPS_LAYERED
 #undef MEAO_UPS_LIN
 
-template <int IN>
-void launch_lin(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, const UpsampleArgs &a,
-                const uint8_t *lo_ao2, int lo_a2pitch, const DepthIn &din, int t, int layers, dim3 grid, cudaStream_t s)
-{
-    const UpsamplePreminArgs pa{a, lo_ao2, lo_a2pitch};
-    if (layers == 1) {
-        if (!lo_ao2) MEAO_LAUNCH((blur_upsample_lin_kernel<IN>), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, a, t, din);
-        else         MEAO_LAUNCH((blur_upsample_premin_lin_kernel<IN>), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, *lo_ao2_map, pa, t, din);
-    } else {
-        if (!lo_ao2) MEAO_LAUNCH((blur_upsample_lin_layered_kernel<IN>), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, a, t, layers, din);
-        else         MEAO_LAUNCH((blur_upsample_premin_lin_layered_kernel<IN>), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, *lo_ao2_map, pa, t, layers, din);
-    }
-}
+const struct {      // [depth_format_slot]
+    Kernel<CUtensorMap, CUtensorMap, UpsampleArgs, int, DepthIn> plain[kDepthFormatSlots];
+    Kernel<CUtensorMap, CUtensorMap, CUtensorMap, UpsamplePreminArgs, int, DepthIn> premin[kDepthFormatSlots];
+    Kernel<CUtensorMap, CUtensorMap, UpsampleArgs, int, int, DepthIn> layered[kDepthFormatSlots];
+    Kernel<CUtensorMap, CUtensorMap, CUtensorMap, UpsamplePreminArgs, int, int, DepthIn> premin_layered[kDepthFormatSlots];
+} kKernels = {MEAO_LIN_SLOTS(blur_upsample_lin_kernel), MEAO_LIN_SLOTS(blur_upsample_premin_lin_kernel),
+              MEAO_LIN_SLOTS(blur_upsample_lin_layered_kernel), MEAO_LIN_SLOTS(blur_upsample_premin_lin_layered_kernel)};
 
 }  // namespace
 
@@ -120,24 +114,20 @@ cudaError_t launch_blur_upsample_lin(const CUtensorMap &lo_depth_map, const CUte
     if (!din.depth_pitch) din.depth_pitch = a.hiw;
     if (!din.depth_layer_pitch) din.depth_layer_pitch = (long long)din.depth_pitch * a.hih;
     if (!din.ao_layer_pitch) din.ao_layer_pitch = (long long)a.hih * a.out_pitch;
-    if (din.in_format == IN_D16)       launch_lin<IN_D16>(lo_depth_map, lo_ao_map, lo_ao2_map, a, lo_ao2, lo_a2pitch, din, t, layers, grid, s);
-    else if (din.in_format == IN_D24S8) launch_lin<IN_D24S8>(lo_depth_map, lo_ao_map, lo_ao2_map, a, lo_ao2, lo_a2pitch, din, t, layers, grid, s);
-    else                                launch_lin<IN_F32>(lo_depth_map, lo_ao_map, lo_ao2_map, a, lo_ao2, lo_a2pitch, din, t, layers, grid, s);
+    const int k = depth_format_slot(din.in_format);
+    const UpsamplePreminArgs pa{a, lo_ao2, lo_a2pitch};
+    if (layers == 1) {
+        if (!lo_ao2) MEAO_LAUNCH((kKernels.plain[k]), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, a, t, din);
+        else         MEAO_LAUNCH((kKernels.premin[k]), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, *lo_ao2_map, pa, t, din);
+    } else {
+        if (!lo_ao2) MEAO_LAUNCH((kKernels.layered[k]), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, a, t, layers, din);
+        else         MEAO_LAUNCH((kKernels.premin_layered[k]), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, *lo_ao2_map, pa, t, layers, din);
+    }
     return cudaGetLastError();
 }
 
-#ifndef MEAO_EMULATE
-cudaError_t preload_blur_upsample_lin()
-{
-    cudaError_t e = cudaSuccess;
-    auto t = [&](auto k) { if (e == cudaSuccess) e = preload_kernel(k); };
-    t(blur_upsample_lin_kernel<IN_F32>); t(blur_upsample_lin_kernel<IN_D16>); t(blur_upsample_lin_kernel<IN_D24S8>);
-    t(blur_upsample_premin_lin_kernel<IN_F32>); t(blur_upsample_premin_lin_kernel<IN_D16>); t(blur_upsample_premin_lin_kernel<IN_D24S8>);
-    t(blur_upsample_lin_layered_kernel<IN_F32>); t(blur_upsample_lin_layered_kernel<IN_D16>); t(blur_upsample_lin_layered_kernel<IN_D24S8>);
-    t(blur_upsample_premin_lin_layered_kernel<IN_F32>); t(blur_upsample_premin_lin_layered_kernel<IN_D16>);
-    t(blur_upsample_premin_lin_layered_kernel<IN_D24S8>);
-    return e;
-}
-#endif
+const KernelUnit kBlurUpsampleLinUnit = {"blur_upsample_lin.cu", [](cudaError_t *load) {
+    return walk_kernels(load, kKernels.plain, kKernels.premin, kKernels.layered, kKernels.premin_layered);
+}};
 
 }  // namespace meao

@@ -85,6 +85,8 @@ composite_kernel(const uint8_t *__restrict__ ao, void *__restrict__ color, long 
 #endif
 }
 
+const Kernel<const uint8_t *, void *, long long, int, int, int> kKernels[2] = {composite_kernel<false>, composite_kernel<true>};    // [half]
+
 }  // namespace
 
 cudaError_t launch_composite(const uint8_t *ao, void *color, long long npix, int half, int rgb, int alpha, int one_minus, cudaStream_t s)
@@ -92,17 +94,10 @@ cudaError_t launch_composite(const uint8_t *ao, void *color, long long npix, int
     if (npix <= 0) return cudaSuccess;
     const long long groups = (npix + 3) / 4;
     const unsigned blocks = (unsigned)((groups + kCompThreads - 1) / kCompThreads);
-    if (half) MEAO_LAUNCH((composite_kernel<true>), blocks, kCompThreads, 0, s, ao, color, npix, rgb, alpha, one_minus);
-    else      MEAO_LAUNCH((composite_kernel<false>), blocks, kCompThreads, 0, s, ao, color, npix, rgb, alpha, one_minus);
+    MEAO_LAUNCH((kKernels[half ? 1 : 0]), blocks, kCompThreads, 0, s, ao, color, npix, rgb, alpha, one_minus);
     return cudaGetLastError();
 }
 
-#ifndef MEAO_EMULATE
-cudaError_t preload_composite_kernels()
-{
-    const cudaError_t e = preload_kernel(composite_kernel<false>);
-    return e != cudaSuccess ? e : preload_kernel(composite_kernel<true>);
-}
-#endif
+const KernelUnit kCompositeUnit = {"composite.cu", [](cudaError_t *load) { return walk_kernels(load, kKernels); }};
 
 }  // namespace meao

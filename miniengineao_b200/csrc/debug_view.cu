@@ -70,14 +70,18 @@ __global__ void __launch_bounds__(256) debug_composite_kernel(const uint8_t *__r
 #endif
 }
 
+const struct {
+    Kernel<DebugViewArgs> view;
+    Kernel<const uint8_t *, void *, long long> composite[2];       // [half]
+} kKernels = {debug_view_kernel, {debug_composite_kernel<false>, debug_composite_kernel<true>}};
+
 }  // namespace
 
 cudaError_t launch_debug_composite(const uint8_t *view, void *color, long long npix, int half, cudaStream_t s)
 {
     const int blocks = (int)((npix + 4 * 256 - 1) / (4 * 256));
     if (blocks <= 0) return cudaSuccess;
-    if (half) MEAO_LAUNCH((debug_composite_kernel<true>), blocks, 256, 0, s, view, color, npix);
-    else      MEAO_LAUNCH((debug_composite_kernel<false>), blocks, 256, 0, s, view, color, npix);
+    MEAO_LAUNCH((kKernels.composite[half ? 1 : 0]), blocks, 256, 0, s, view, color, npix);
     return cudaGetLastError();
 }
 
@@ -88,18 +92,6 @@ cudaError_t launch_debug_view(const DebugViewArgs &a, cudaStream_t s)
     return cudaGetLastError();
 }
 
-#ifndef MEAO_EMULATE
-cudaError_t preload_composite_kernels();
-cudaError_t preload_selftest_kernel();
-cudaError_t preload_aux_kernels()
-{
-    cudaError_t e = preload_kernel(debug_view_kernel);
-    if (e == cudaSuccess) e = preload_kernel(debug_composite_kernel<false>);
-    if (e == cudaSuccess) e = preload_kernel(debug_composite_kernel<true>);
-    if (e == cudaSuccess) e = preload_composite_kernels();
-    if (e == cudaSuccess) e = preload_selftest_kernel();
-    return e;
-}
-#endif
+const KernelUnit kDebugViewUnit = {"debug_view.cu", [](cudaError_t *load) { return walk_kernels(load, kKernels.view, kKernels.composite); }};
 
 }  // namespace meao

@@ -22,6 +22,8 @@ __global__ void __launch_bounds__(256) halo_copy_kernel(const HaloArgs a)
 #endif
 }
 
+const Kernel<HaloArgs> kKernels[] = {halo_copy_kernel};
+
 }  // namespace
 
 cudaError_t launch_halo_copy(const HaloArgs &a, cudaStream_t s)
@@ -34,13 +36,6 @@ cudaError_t launch_halo_copy(const HaloArgs &a, cudaStream_t s)
     return cudaGetLastError();
 }
 
-#ifndef MEAO_EMULATE
-cudaError_t preload_band_exchange_kernel();
-cudaError_t preload_band_kernels()
-{
-    const cudaError_t e = preload_kernel(halo_copy_kernel);
-    return e != cudaSuccess ? e : preload_band_exchange_kernel();
-}
-#endif
+const KernelUnit kHaloUnit = {"halo.cu", [](cudaError_t *load) { return walk_kernels(load, kKernels); }};
 
 }  // namespace meao

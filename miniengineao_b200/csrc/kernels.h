@@ -43,7 +43,17 @@ inline cudaError_t launch_ex(void (*kernel)(KArgs...), dim3 grid, dim3 block, si
 #define MEAO_LAUNCH(k, grid, block, smem, stream, ...) (void)meao::launch_ex(MEAO_UNPAREN k, (grid), (block), (smem), (stream), __VA_ARGS__)
 #endif
 
+// Kernel tables.  Every translation unit holds its __global__ instantiations in one static table of typed function pointers
+// (kKernels), laid out by the slot functions below; its launchers check their arguments, size the grid and launch
+// kKernels[...][slot].  The MEAO_*_SLOTS macros list one kernel template's instantiations in slot order, so each order is written
+// once, next to its slot function.  A slot a unit's form does not have holds nullptr: the macros' second argument is MEAO_SLOT, or
+// MEAO_NO_SLOT for the slots named in the macro's comment.
+#define MEAO_SLOT(...) __VA_ARGS__
+#define MEAO_NO_SLOT(...) nullptr
+
 namespace meao {
+
+template <class... P> using Kernel = void (*)(P...);
 
 // ---- stage 1: prepare_depth = Downsample1.compute + Downsample2.compute fused ----------------
 struct PrepareArgs {
@@ -73,6 +83,14 @@ inline PrepareArgs resolve_pitches(PrepareArgs a)
     if (!a.depth_layer_pitch) a.depth_layer_pitch = (long long)a.depth_pitch * a.H;
     return a;
 }
+// Raw depth format slot: 0 f32 (also any other code), 1 D16, 2 D24S8 -- PrepareArgs.in_format's codes, the IN_* of depth_in.cuh
+constexpr int kDepthFormatSlots = 3;
+inline int depth_format_slot(int in_format) { return in_format == 1 || in_format == 2 ? in_format : 0; }
+// prepare_depth<RAW, REVERSED, IN>: linear input (read as f32), then raw f32 / D16 / D24S8, reversed Z first.  D24S8: the last two.
+constexpr int kPrepareSlots = 7;
+inline int prepare_slot(const PrepareArgs &a) { return a.raw ? 1 + 2 * depth_format_slot(a.in_format) + (a.reversed_z ? 0 : 1) : 0; }
+#define MEAO_PREPARE_SLOTS(K, D24S8) {K<false, true, IN_F32>, K<true, true, IN_F32>, K<true, false, IN_F32>, K<true, true, IN_D16>, \
+                                      K<true, false, IN_D16>, D24S8(K<true, true, IN_D24S8>), D24S8(K<true, false, IN_D24S8>)}
 // low_only: write LowDepth1..4 only, loading the even rows alone (a.lin is not written); the frame's final upsample then
 // linearises its own pixels and writes LinearDepth (launch_blur_upsample_lin)
 cudaError_t launch_prepare_depth(const PrepareArgs &a, cudaStream_t s, bool low_only = false);
@@ -102,6 +120,18 @@ constexpr int kRenderTileVariants = 3;
 constexpr int kRenderTileHs[kRenderTileVariants] = {32, 16, 8};
 constexpr int kRenderBoxW = 96, kRenderWideBoxW = 80;               // TMA box widths of the render kernel (f32 elements): 64 + 2 x apron (16 / wide: 8)
 constexpr int render_box_h(int tile_h, bool wide) { return tile_h + (wide ? 16 : 32); }
+constexpr size_t render_smem_bytes(int tile_h, bool wide) { return (size_t)(wide ? kRenderWideBoxW : kRenderBoxW) * render_box_h(tile_h, wide) * sizeof(float); }
+// render_ao<MODE, EXH, TH>: wide, then exhaustive, then the tile variant (kRenderTileHs); -1: a tile height without a kernel
+constexpr int kRenderSlots = 4 * kRenderTileVariants;
+inline int render_slot(const RenderArgs &a)
+{
+    for (int t = 0; t < kRenderTileVariants; t++)
+        if (a.tile_h == kRenderTileHs[t]) return ((a.wide ? 2 : 0) + (a.exhaustive ? 1 : 0)) * kRenderTileVariants + t;
+    return -1;
+}
+#define MEAO_RENDER_SLOTS(K) {K<0, false, 32>, K<0, false, 16>, K<0, false, 8>, K<0, true, 32>, K<0, true, 16>, K<0, true, 8>, \
+                              K<1, false, 32>, K<1, false, 16>, K<1, false, 8>, K<1, true, 32>, K<1, true, 16>, K<1, true, 8>}
+static_assert(kRenderTileHs[0] == 32 && kRenderTileHs[1] == 16 && kRenderTileHs[2] == 8, "MEAO_RENDER_SLOTS lists the tile heights");
 
 // ---- stage 3: blur_upsample = Upsample.compute main / main_blendout, one level ----------------
 struct UpsampleArgs {
@@ -133,6 +163,11 @@ inline bool upsample_fast_div_ok(float tol, float nfs)
 }
 // main_premin / main_premin_blendout (COMBINE_LOWER_RESOLUTIONS): the same arguments plus LoResAO2 = HighQuality<lo>
 struct UpsamplePreminArgs { UpsampleArgs base; const uint8_t *lo_ao2; int lo_a2pitch; };
+// blur_upsample<BLEND, HI_HALF>: blend (a hi-res AO, kernel main_blendout), then hi-half (the hi-res depth is LinearDepth, f16).  The
+// premin kernels take other parameters: a unit lists them apart, in the same order.  MEAO_NO_SLOT: all but the final level's {0, 1}.
+constexpr int kUpsampleSlots = 4;
+inline int upsample_slot(const UpsampleArgs &a) { return (a.hi_ao ? 2 : 0) + (a.hi_is_half ? 1 : 0); }
+#define MEAO_UPSAMPLE_SLOTS(K, OTHER) {OTHER(K<false, false>), K<false, true>, OTHER(K<true, false>), OTHER(K<true, true>)}
 // lo_ao2 == nullptr: kernels main / main_blendout; otherwise the premin kernels (lo_ao2_map = its TMA descriptor).
 // sm_count: SMs of the device (sizes the one-wave grid of the persistent tile loop)
 cudaError_t launch_blur_upsample(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
@@ -163,6 +198,9 @@ struct DepthIn {
 cudaError_t launch_blur_upsample_lin(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
                                      const UpsampleArgs &a, const uint8_t *lo_ao2, int lo_a2pitch, const DepthIn &din, int layers, int sm_count,
                                      cudaStream_t s);
+// blur_upsample_lin<IN>: depth_format_slot(DepthIn.in_format).  The plain / premin and single-image / layered kernels take other
+// parameters: the unit lists each apart, in this order.
+#define MEAO_LIN_SLOTS(K) {K<IN_F32>, K<IN_D16>, K<IN_D24S8>}
 
 // ---- layered frames (meao_set_layers): L same-size views through one launch per stage ------------------------------------
 // Every image is L images of the same pitch stored back to back ([L][h][pitch]), so layer l of an image starts l x rows x pitch
@@ -255,21 +293,45 @@ cudaError_t launch_band_exchange(const XchgArgs &a, cudaStream_t s);
 // CUDA loads kernels lazily, on first launch, and that load can wait for kernels already RUNNING on the device.  A band's exchange
 // kernel spins until its neighbour has run -- if the neighbour's first launch then has to load a kernel on the same device, the two
 // wait for each other until the exchange times out (seen when the band tests ran first in a fresh process).  meao_create therefore
-// touches every kernel of the library once per device (cudaFuncGetAttributes forces the load).
+// touches every kernel of the library once per device (cudaFuncGetAttributes forces the load), walking every unit's kernel table.
+// A kernel that is launched is in its unit's table (the launchers take it from there), so it is loaded too; the test suite checks
+// that each table holds every kernel its unit compiles to.
+struct KernelUnit {
+    const char *file;                       // the translation unit (build.py SOURCES)
+    int (*walk)(cudaError_t *load);         // walk_kernels over the unit's table: its kernel count; load != nullptr: loads them too
+};
+// The number of kernels in a (nested) table, nullptr slots skipped.  load != nullptr: loads each one while *load is cudaSuccess and
+// keeps the first error there.
+template <class... P> inline int walk_kernels(cudaError_t *load, Kernel<P...> k)
+{
+    if (!k) return 0;
 #ifndef MEAO_EMULATE
-template <class K> inline cudaError_t preload_kernel(K kernel) { cudaFuncAttributes at; return cudaFuncGetAttributes(&at, (const void *)kernel); }
-cudaError_t preload_prepare_depth();
-cudaError_t preload_render_ao();
-cudaError_t preload_blur_upsample();
-cudaError_t preload_prepare_depth_layered();
-cudaError_t preload_render_ao_layered();
-cudaError_t preload_blur_upsample_layered();
-cudaError_t preload_prepare_depth_array();
-cudaError_t preload_blur_upsample_array();
-cudaError_t preload_blur_upsample_lin();
-cudaError_t preload_band_kernels();
-cudaError_t preload_aux_kernels();      // composite, debug views, self test
+    cudaFuncAttributes at;
+    if (load && *load == cudaSuccess) *load = cudaFuncGetAttributes(&at, (const void *)k);
 #endif
+    return 1;
+}
+template <class T, size_t N> inline int walk_kernels(cudaError_t *load, const T (&t)[N])
+{
+    int n = 0;
+    for (const T &e : t) n += walk_kernels(load, e);
+    return n;
+}
+template <class T, class U, class... R> inline int walk_kernels(cudaError_t *load, const T &t, const U &u, const R &...r)
+{
+    return walk_kernels(load, t) + walk_kernels(load, u, r...);
+}
+// Every kernel unit, in build.py SOURCES order.  The CPU emulator builds all but the GPU self test.
+extern const KernelUnit kPrepareDepthUnit, kRenderAoUnit, kBlurUpsampleUnit, kSelftestUnit, kHaloUnit, kBandExchangeUnit, kCompositeUnit,
+    kDebugViewUnit, kPrepareDepthLayeredUnit, kRenderAoLayeredUnit, kBlurUpsampleLayeredUnit, kPrepareDepthArrayUnit, kBlurUpsampleArrayUnit,
+    kBlurUpsampleLinUnit;
+inline const KernelUnit *const kKernelUnits[] = {
+    &kPrepareDepthUnit, &kRenderAoUnit, &kBlurUpsampleUnit,
+#ifndef MEAO_EMULATE
+    &kSelftestUnit,
+#endif
+    &kHaloUnit, &kBandExchangeUnit, &kCompositeUnit, &kDebugViewUnit, &kPrepareDepthLayeredUnit, &kRenderAoLayeredUnit,
+    &kBlurUpsampleLayeredUnit, &kPrepareDepthArrayUnit, &kBlurUpsampleArrayUnit, &kBlurUpsampleLinUnit};
 
 // ---- halo pack / unpack: row blocks of pitched buffers <-> contiguous staging, one launch ------
 struct HaloSeg { const float *src; float *dst; int src_pitch, dst_pitch, width, rows; };

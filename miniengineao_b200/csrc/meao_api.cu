@@ -734,17 +734,8 @@ int meao_create(const MeaoDeviceCfg *cfg, MeaoCtx **out)
         static std::map<int, bool> preloaded;
         std::lock_guard<std::mutex> g(preload_mutex);
         if (!preloaded[dev]) {
-            cudaError_t pe = preload_prepare_depth();
-            if (pe == cudaSuccess) pe = preload_render_ao();
-            if (pe == cudaSuccess) pe = preload_blur_upsample();
-            if (pe == cudaSuccess) pe = preload_prepare_depth_layered();
-            if (pe == cudaSuccess) pe = preload_render_ao_layered();
-            if (pe == cudaSuccess) pe = preload_blur_upsample_layered();
-            if (pe == cudaSuccess) pe = preload_prepare_depth_array();
-            if (pe == cudaSuccess) pe = preload_blur_upsample_array();
-            if (pe == cudaSuccess) pe = preload_blur_upsample_lin();
-            if (pe == cudaSuccess) pe = preload_band_kernels();
-            if (pe == cudaSuccess) pe = preload_aux_kernels();
+            cudaError_t pe = cudaSuccess;
+            for (const KernelUnit *u : kKernelUnits) u->walk(&pe);
             if (pe != cudaSuccess) { cudaGetLastError(); meao_destroy(c); return fail(nullptr, MEAO_ERR_CUDA, "loading the kernels failed: %s", cudaGetErrorString(pe)); }
             preloaded[dev] = true;
         }

@@ -20,6 +20,12 @@ namespace {
 #include "prepare_depth_kernel.inc"
 #undef MEAO_LAYERED
 
+static_assert(IN_D16 == 1 && IN_D24S8 == 2, "depth_format_slot takes the IN_* codes");
+
+// [low_only][prepare_slot]
+const Kernel<PrepareArgs> kKernels[2][kPrepareSlots] = {MEAO_PREPARE_SLOTS(prepare_depth_kernel, MEAO_SLOT),
+                                                        MEAO_PREPARE_SLOTS(prepare_depth_low_kernel, MEAO_SLOT)};
+
 }  // namespace
 
 cudaError_t launch_prepare_depth(const PrepareArgs &a_in, cudaStream_t s, bool low_only)
@@ -27,38 +33,10 @@ cudaError_t launch_prepare_depth(const PrepareArgs &a_in, cudaStream_t s, bool l
     if (a_in.row1 <= a_in.row0) return cudaSuccess;
     const PrepareArgs a = resolve_pitches(a_in);
     dim3 grid(ceil_div(a.W, kPrepTileW), ceil_div(a.row1 - a.row0, low_only ? kPrepLowTileH : kPrepTileH));
-#define MEAO_PREP_K(...) (low_only ? prepare_depth_low_kernel<__VA_ARGS__> : prepare_depth_kernel<__VA_ARGS__>)
-    if (!a.raw) {
-        MEAO_LAUNCH((MEAO_PREP_K(false, true, IN_F32)), grid, kPrepThreads, 0, s, a);
-    } else if (a.in_format == IN_D16) {
-        if (a.reversed_z) MEAO_LAUNCH((MEAO_PREP_K(true, true, IN_D16)), grid, kPrepThreads, 0, s, a);
-        else              MEAO_LAUNCH((MEAO_PREP_K(true, false, IN_D16)), grid, kPrepThreads, 0, s, a);
-    } else if (a.in_format == IN_D24S8) {
-        if (a.reversed_z) MEAO_LAUNCH((MEAO_PREP_K(true, true, IN_D24S8)), grid, kPrepThreads, 0, s, a);
-        else              MEAO_LAUNCH((MEAO_PREP_K(true, false, IN_D24S8)), grid, kPrepThreads, 0, s, a);
-    } else {
-        if (a.reversed_z) MEAO_LAUNCH((MEAO_PREP_K(true, true, IN_F32)), grid, kPrepThreads, 0, s, a);
-        else              MEAO_LAUNCH((MEAO_PREP_K(true, false, IN_F32)), grid, kPrepThreads, 0, s, a);
-    }
-#undef MEAO_PREP_K
+    MEAO_LAUNCH((kKernels[low_only][prepare_slot(a)]), grid, kPrepThreads, 0, s, a);
     return cudaGetLastError();
 }
 
-#ifndef MEAO_EMULATE
-cudaError_t preload_prepare_depth()
-{
-    cudaError_t e = cudaSuccess;
-    auto t = [&](auto k) { if (e == cudaSuccess) e = preload_kernel(k); };
-    t(prepare_depth_kernel<false, true, IN_F32>);
-    t(prepare_depth_kernel<true, true, IN_F32>); t(prepare_depth_kernel<true, false, IN_F32>);
-    t(prepare_depth_kernel<true, true, IN_D16>); t(prepare_depth_kernel<true, false, IN_D16>);
-    t(prepare_depth_kernel<true, true, IN_D24S8>); t(prepare_depth_kernel<true, false, IN_D24S8>);
-    t(prepare_depth_low_kernel<false, true, IN_F32>);
-    t(prepare_depth_low_kernel<true, true, IN_F32>); t(prepare_depth_low_kernel<true, false, IN_F32>);
-    t(prepare_depth_low_kernel<true, true, IN_D16>); t(prepare_depth_low_kernel<true, false, IN_D16>);
-    t(prepare_depth_low_kernel<true, true, IN_D24S8>); t(prepare_depth_low_kernel<true, false, IN_D24S8>);
-    return e;
-}
-#endif
+const KernelUnit kPrepareDepthUnit = {"prepare_depth.cu", [](cudaError_t *load) { return walk_kernels(load, kKernels); }};
 
 }  // namespace meao

@@ -17,6 +17,10 @@ namespace {
 #undef MEAO_ARRAY
 #undef MEAO_LAYERED
 
+// [prepare_slot]; no CUDA array holds D24S8
+const Kernel<PrepareArgs, cudaSurfaceObject_t, int, const LayerZ *> kKernels[kPrepareSlots] =
+    MEAO_PREPARE_SLOTS(prepare_depth_array_kernel, MEAO_NO_SLOT);
+
 }  // namespace
 
 cudaError_t launch_prepare_depth_array(const PrepareArgs &a_in, cudaSurfaceObject_t depth, int surf_kind, int layers, cudaStream_t s,
@@ -28,28 +32,10 @@ cudaError_t launch_prepare_depth_array(const PrepareArgs &a_in, cudaSurfaceObjec
     a.depth = nullptr;
     a.vec_ok = 1;               // the input is read element by element; the intermediates' pitched rows keep the vector stores aligned
     dim3 grid(ceil_div(a.W, kPrepTileW), ceil_div(a.row1 - a.row0, kPrepTileH), layers);
-    if (!a.raw) {
-        MEAO_LAUNCH((prepare_depth_array_kernel<false, true, IN_F32>), grid, kPrepThreads, 0, s, a, depth, surf_kind, layer_zb);
-    } else if (a.in_format == IN_D16) {
-        if (a.reversed_z) MEAO_LAUNCH((prepare_depth_array_kernel<true, true, IN_D16>), grid, kPrepThreads, 0, s, a, depth, surf_kind, layer_zb);
-        else              MEAO_LAUNCH((prepare_depth_array_kernel<true, false, IN_D16>), grid, kPrepThreads, 0, s, a, depth, surf_kind, layer_zb);
-    } else {
-        if (a.reversed_z) MEAO_LAUNCH((prepare_depth_array_kernel<true, true, IN_F32>), grid, kPrepThreads, 0, s, a, depth, surf_kind, layer_zb);
-        else              MEAO_LAUNCH((prepare_depth_array_kernel<true, false, IN_F32>), grid, kPrepThreads, 0, s, a, depth, surf_kind, layer_zb);
-    }
+    MEAO_LAUNCH((kKernels[prepare_slot(a)]), grid, kPrepThreads, 0, s, a, depth, surf_kind, layer_zb);
     return cudaGetLastError();
 }
 
-#ifndef MEAO_EMULATE
-cudaError_t preload_prepare_depth_array()
-{
-    cudaError_t e = cudaSuccess;
-    auto t = [&](auto k) { if (e == cudaSuccess) e = preload_kernel(k); };
-    t(prepare_depth_array_kernel<false, true, IN_F32>);
-    t(prepare_depth_array_kernel<true, true, IN_F32>); t(prepare_depth_array_kernel<true, false, IN_F32>);
-    t(prepare_depth_array_kernel<true, true, IN_D16>); t(prepare_depth_array_kernel<true, false, IN_D16>);
-    return e;
-}
-#endif
+const KernelUnit kPrepareDepthArrayUnit = {"prepare_depth_array.cu", [](cudaError_t *load) { return walk_kernels(load, kKernels); }};
 
 }  // namespace meao

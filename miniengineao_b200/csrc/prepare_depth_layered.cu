@@ -13,6 +13,10 @@ namespace {
 #include "prepare_depth_kernel.inc"
 #undef MEAO_LAYERED
 
+// [low_only][prepare_slot]
+const Kernel<PrepareArgs, const LayerZ *> kKernels[2][kPrepareSlots] = {MEAO_PREPARE_SLOTS(prepare_depth_layered_kernel, MEAO_SLOT),
+                                                                        MEAO_PREPARE_SLOTS(prepare_depth_low_layered_kernel, MEAO_SLOT)};
+
 }  // namespace
 
 cudaError_t launch_prepare_depth_layered(const PrepareArgs &a_in, int layers, cudaStream_t s, bool low_only, const LayerZ *layer_zb)
@@ -21,38 +25,10 @@ cudaError_t launch_prepare_depth_layered(const PrepareArgs &a_in, int layers, cu
     const PrepareArgs a = resolve_pitches(a_in);
     if (layers < 1 || layers > kMaxLayers) return cudaErrorInvalidValue;
     dim3 grid(ceil_div(a.W, kPrepTileW), ceil_div(a.row1 - a.row0, low_only ? kPrepLowTileH : kPrepTileH), layers);
-#define MEAO_PREP_K(...) (low_only ? prepare_depth_low_layered_kernel<__VA_ARGS__> : prepare_depth_layered_kernel<__VA_ARGS__>)
-    if (!a.raw) {
-        MEAO_LAUNCH((MEAO_PREP_K(false, true, IN_F32)), grid, kPrepThreads, 0, s, a, layer_zb);
-    } else if (a.in_format == IN_D16) {
-        if (a.reversed_z) MEAO_LAUNCH((MEAO_PREP_K(true, true, IN_D16)), grid, kPrepThreads, 0, s, a, layer_zb);
-        else              MEAO_LAUNCH((MEAO_PREP_K(true, false, IN_D16)), grid, kPrepThreads, 0, s, a, layer_zb);
-    } else if (a.in_format == IN_D24S8) {
-        if (a.reversed_z) MEAO_LAUNCH((MEAO_PREP_K(true, true, IN_D24S8)), grid, kPrepThreads, 0, s, a, layer_zb);
-        else              MEAO_LAUNCH((MEAO_PREP_K(true, false, IN_D24S8)), grid, kPrepThreads, 0, s, a, layer_zb);
-    } else {
-        if (a.reversed_z) MEAO_LAUNCH((MEAO_PREP_K(true, true, IN_F32)), grid, kPrepThreads, 0, s, a, layer_zb);
-        else              MEAO_LAUNCH((MEAO_PREP_K(true, false, IN_F32)), grid, kPrepThreads, 0, s, a, layer_zb);
-    }
-#undef MEAO_PREP_K
+    MEAO_LAUNCH((kKernels[low_only][prepare_slot(a)]), grid, kPrepThreads, 0, s, a, layer_zb);
     return cudaGetLastError();
 }
 
-#ifndef MEAO_EMULATE
-cudaError_t preload_prepare_depth_layered()
-{
-    cudaError_t e = cudaSuccess;
-    auto t = [&](auto k) { if (e == cudaSuccess) e = preload_kernel(k); };
-    t(prepare_depth_layered_kernel<false, true, IN_F32>);
-    t(prepare_depth_layered_kernel<true, true, IN_F32>); t(prepare_depth_layered_kernel<true, false, IN_F32>);
-    t(prepare_depth_layered_kernel<true, true, IN_D16>); t(prepare_depth_layered_kernel<true, false, IN_D16>);
-    t(prepare_depth_layered_kernel<true, true, IN_D24S8>); t(prepare_depth_layered_kernel<true, false, IN_D24S8>);
-    t(prepare_depth_low_layered_kernel<false, true, IN_F32>);
-    t(prepare_depth_low_layered_kernel<true, true, IN_F32>); t(prepare_depth_low_layered_kernel<true, false, IN_F32>);
-    t(prepare_depth_low_layered_kernel<true, true, IN_D16>); t(prepare_depth_low_layered_kernel<true, false, IN_D16>);
-    t(prepare_depth_low_layered_kernel<true, true, IN_D24S8>); t(prepare_depth_low_layered_kernel<true, false, IN_D24S8>);
-    return e;
-}
-#endif
+const KernelUnit kPrepareDepthLayeredUnit = {"prepare_depth_layered.cu", [](cudaError_t *load) { return walk_kernels(load, kKernels); }};
 
 }  // namespace meao

@@ -47,34 +47,22 @@ __global__ void synth_tiled_kernel(const float *low, int lw, int lh, int lpitch,
     out[((size_t)s * sh + j) * sw + i] = __float2half_rn(v);
 }
 
-}  // namespace
+const struct {
+    Kernel<CUtensorMap, RenderArgs, int> render[kRenderSlots];      // [render_slot]
+    Kernel<const float *, int, int, int, int, int, float, __half *> synth_tiled;
+} kKernels = {MEAO_RENDER_SLOTS(render_ao_kernel), synth_tiled_kernel};
 
-template <int MODE, bool EXH, int TH>
-static void launch_render_variant(const CUtensorMap &low_map, int t, const RenderArgs &a, dim3 grid, cudaStream_t s)
-{
-    const size_t smem = (size_t)Geo<MODE, TH>::kSW * Geo<MODE, TH>::kSH * sizeof(float);
-    MEAO_LAUNCH((render_ao_kernel<MODE, EXH, TH>), grid, kThreads, smem, s, low_map, a, t);
-}
-template <int MODE, bool EXH>
-static cudaError_t launch_render_th(const CUtensorMap &low_map, int t, const RenderArgs &a, int gx, int rows, cudaStream_t s)
-{
-    switch (a.tile_h) {
-        case kRenderTileHs[0]: launch_render_variant<MODE, EXH, kRenderTileHs[0]>(low_map, t, a, dim3(gx, ceil_div(rows, kRenderTileHs[0])), s); break;
-        case kRenderTileHs[1]: launch_render_variant<MODE, EXH, kRenderTileHs[1]>(low_map, t, a, dim3(gx, ceil_div(rows, kRenderTileHs[1])), s); break;
-        case kRenderTileHs[2]: launch_render_variant<MODE, EXH, kRenderTileHs[2]>(low_map, t, a, dim3(gx, ceil_div(rows, kRenderTileHs[2])), s); break;
-        default: return cudaErrorInvalidValue;
-    }
-    return cudaGetLastError();
-}
+}  // namespace
 
 cudaError_t launch_render_ao(const CUtensorMap &low_map, bool use_tma, const RenderArgs &a, cudaStream_t s)
 {
     if (a.row1 <= a.row0) return cudaSuccess;
+    const int k = render_slot(a);
+    if (k < 0) return cudaErrorInvalidValue;
     const int ybase = a.row0 & ~3;
-    const int gx = ceil_div(a.lw, kTW), rows = a.row1 - ybase;
-    const int t = use_tma ? 1 : 0;
-    if (!a.wide) return a.exhaustive ? launch_render_th<0, true>(low_map, t, a, gx, rows, s) : launch_render_th<0, false>(low_map, t, a, gx, rows, s);
-    return a.exhaustive ? launch_render_th<1, true>(low_map, t, a, gx, rows, s) : launch_render_th<1, false>(low_map, t, a, gx, rows, s);
+    const dim3 grid(ceil_div(a.lw, kTW), ceil_div(a.row1 - ybase, a.tile_h));
+    MEAO_LAUNCH((kKernels.render[k]), grid, kThreads, render_smem_bytes(a.tile_h, a.wide), s, low_map, a, use_tma ? 1 : 0);
+    return cudaGetLastError();
 }
 
 cudaError_t launch_synth_tiled(const float *low, int lw, int lh, int lpitch, int sw, int sh, float pad,
@@ -85,18 +73,6 @@ cudaError_t launch_synth_tiled(const float *low, int lw, int lh, int lpitch, int
     return cudaGetLastError();
 }
 
-#ifndef MEAO_EMULATE
-cudaError_t preload_render_ao()
-{
-    cudaError_t e = cudaSuccess;
-    auto t = [&](auto k) { if (e == cudaSuccess) e = preload_kernel(k); };
-    t(render_ao_kernel<0, false, 32>); t(render_ao_kernel<0, false, 16>); t(render_ao_kernel<0, false, 8>);
-    t(render_ao_kernel<0, true, 32>); t(render_ao_kernel<0, true, 16>); t(render_ao_kernel<0, true, 8>);
-    t(render_ao_kernel<1, false, 32>); t(render_ao_kernel<1, false, 16>); t(render_ao_kernel<1, false, 8>);
-    t(render_ao_kernel<1, true, 32>); t(render_ao_kernel<1, true, 16>); t(render_ao_kernel<1, true, 8>);
-    t(synth_tiled_kernel);
-    return e;
-}
-#endif
+const KernelUnit kRenderAoUnit = {"render_ao.cu", [](cudaError_t *load) { return walk_kernels(load, kKernels.render, kKernels.synth_tiled); }};
 
 }  // namespace meao

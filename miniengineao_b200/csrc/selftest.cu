@@ -48,6 +48,8 @@ __global__ void selftest_div_kernel(uint64_t n_per_thread, uint32_t seed, unsign
 #endif
 }
 
+const Kernel<uint64_t, uint32_t, unsigned long long *> kKernels[] = {selftest_div_kernel};
+
 }  // namespace
 
 cudaError_t launch_selftest_div(uint64_t n, uint32_t seed, unsigned long long *mismatch_dev, int sm_count, cudaStream_t s)
@@ -58,8 +60,6 @@ cudaError_t launch_selftest_div(uint64_t n, uint32_t seed, unsigned long long *m
     return cudaGetLastError();
 }
 
-#ifndef MEAO_EMULATE
-cudaError_t preload_selftest_kernel() { return preload_kernel(selftest_div_kernel); }
-#endif
+const KernelUnit kSelftestUnit = {"selftest.cu", [](cudaError_t *load) { return walk_kernels(load, kKernels); }};
 
 }  // namespace meao

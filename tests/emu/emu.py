@@ -50,6 +50,7 @@ def lib() -> C.CDLL:
         l.frame_composite.argtypes = [P, P, LL, I, I, I, I]
         l.frame_composite_debug.argtypes = [P, P, LL, I]
         l.frame_schedule_export.argtypes = [P, P, P, I]
+        l.frame_kernel_units.argtypes = [P, P, I]
         l.frame_tma_box_loads.restype = LL
         l.frame_surface_accesses.restype = LL
         _lib = l
@@ -292,6 +293,15 @@ def schedule(variants=(0, 0, 0, 0)) -> list:
         stage, level, branch, wait, pdl = out[5 * i:5 * i + 5]
         rows.append((STAGES[stage], level, branch, None if wait < 0 else wait, PDL[pdl], names.raw[32 * i:32 * (i + 1)].split(b"\0")[0].decode()))
     return rows
+
+
+def kernel_units() -> dict:
+    """kernels.h kKernelUnits as the emulator builds them: unit file -> the number of kernels in its table."""
+    cap = 32
+    names, counts = C.create_string_buffer(32 * cap), (C.c_int * cap)()
+    n = lib().frame_kernel_units(names, counts, cap)
+    assert 0 < n <= cap
+    return {names.raw[32 * i:32 * (i + 1)].split(b"\0")[0].decode(): counts[i] for i in range(n)}
 
 
 def composite(ao: np.ndarray, color: np.ndarray, *, rgb: bool, alpha: bool, one_minus: bool) -> np.ndarray:

@@ -355,6 +355,17 @@ int frame_schedule_export(const int *variants4, int *out5, char *names, int cap)
     return (int)s.size();
 }
 
+// ---- the kernel units (kernels.h kKernelUnits): unit i's file at names + 32 i, the kernel count of its table in counts[i] ----------
+int frame_kernel_units(char *names, int *counts, int cap)
+{
+    int n = 0;
+    for (const KernelUnit *u : kKernelUnits) {
+        if (n < cap) { snprintf(names + 32 * n, 32, "%s", u->file); counts[n] = u->walk(nullptr); }
+        n++;
+    }
+    return n;
+}
+
 // ---- counters and self-checks -----------------------------------------------------------------------------------------------------
 long long frame_tma_box_loads() { return meao_emu::tma_box_loads; }
 long long frame_surface_accesses() { return meao_emu::surface_accesses; }
