@@ -21,10 +21,15 @@
 // preprocessor).  CUDA build: cudaLaunchKernelEx, with the programmatic-dependent-launch attribute when the recorder asked
 // for it (meao::g_launch_pdl, set by meao_api.cu around the launches whose predecessor IN THE SAME STREAM is one of our
 // kernels): the dependent grid may then be scheduled while its predecessor drains, runs its prologue and blocks in
-// pdl_wait() (griddepcontrol.wait) until the predecessor has completed and flushed -- see common.cuh.
+// pdl_wait() (griddepcontrol.wait) until the predecessor has completed and flushed -- see common.cuh.  Emulated build: the kernel's
+// address is reported to the runtime before the launch, for its ledger of the kernels launched (tests/emu/emu_runtime.cpp).  The hook
+// is weak, so an emulator runtime without a ledger still links and launches as before.
 #define MEAO_UNPAREN(...) __VA_ARGS__
 #ifdef MEAO_EMULATE
-#define MEAO_LAUNCH(k, grid, block, smem, stream, ...) meao_emu::launch((grid), (block), (smem), [&]() { MEAO_UNPAREN k(__VA_ARGS__); })
+namespace meao_emu { __attribute__((weak)) void note_launch(const void *kernel); }
+#define MEAO_LAUNCH(k, grid, block, smem, stream, ...) \
+    ((meao_emu::note_launch ? meao_emu::note_launch(reinterpret_cast<const void *>(MEAO_UNPAREN k)) : (void)0), \
+     meao_emu::launch((grid), (block), (smem), [&]() { MEAO_UNPAREN k(__VA_ARGS__); }))
 #else
 namespace meao {
 inline thread_local bool g_launch_pdl = false;
@@ -164,10 +169,11 @@ inline bool upsample_fast_div_ok(float tol, float nfs)
 // main_premin / main_premin_blendout (COMBINE_LOWER_RESOLUTIONS): the same arguments plus LoResAO2 = HighQuality<lo>
 struct UpsamplePreminArgs { UpsampleArgs base; const uint8_t *lo_ao2; int lo_a2pitch; };
 // blur_upsample<BLEND, HI_HALF>: blend (a hi-res AO, kernel main_blendout), then hi-half (the hi-res depth is LinearDepth, f16).  The
-// premin kernels take other parameters: a unit lists them apart, in the same order.  MEAO_NO_SLOT: all but the final level's {0, 1}.
+// premin kernels take other parameters: a unit lists them apart, in the same order.  upsample_args blends exactly when the hi level is
+// not L0, so only two slots have a kernel: the final level's {0, 1} and the coarse levels' {1, 0}.  MEAO_NO_SLOT: the coarse levels'.
 constexpr int kUpsampleSlots = 4;
 inline int upsample_slot(const UpsampleArgs &a) { return (a.hi_ao ? 2 : 0) + (a.hi_is_half ? 1 : 0); }
-#define MEAO_UPSAMPLE_SLOTS(K, OTHER) {OTHER(K<false, false>), K<false, true>, OTHER(K<true, false>), OTHER(K<true, true>)}
+#define MEAO_UPSAMPLE_SLOTS(K, BLEND) {nullptr, K<false, true>, BLEND(K<true, false>), nullptr}
 // lo_ao2 == nullptr: kernels main / main_blendout; otherwise the premin kernels (lo_ao2_map = its TMA descriptor).
 // sm_count: SMs of the device (sizes the one-wave grid of the persistent tile loop)
 cudaError_t launch_blur_upsample(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,

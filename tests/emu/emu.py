@@ -7,6 +7,8 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import re
+import subprocess
 import sys
 
 import numpy as np
@@ -53,6 +55,7 @@ def lib() -> C.CDLL:
         l.frame_kernel_units.argtypes = [P, P, I]
         l.frame_tma_box_loads.restype = LL
         l.frame_surface_accesses.restype = LL
+        l.frame_ledger_read.argtypes = [P, P, P, I]
         _lib = l
     return _lib
 
@@ -302,6 +305,44 @@ def kernel_units() -> dict:
     n = lib().frame_kernel_units(names, counts, cap)
     assert 0 < n <= cap
     return {names.raw[32 * i:32 * (i + 1)].split(b"\0")[0].decode(): counts[i] for i in range(n)}
+
+
+_symbols: dict | None = None
+_KERNEL = re.compile(r"(?:void )?meao::\(anonymous namespace\)::(\w+_kernel(?:<[^()]*>)?)\([^()]*\)")
+
+
+def _kernel_symbols() -> dict:
+    """library-relative address -> 'name<template args>' of every kernel of the library (one nm run, cached).  The kernels are
+    meao::(anonymous namespace)::*_kernel functions: local symbols, in the symbol table but not among the dynamic ones."""
+    global _symbols
+    if _symbols is None:
+        out = subprocess.run(["nm", "-C", "--defined-only", build_emu.build()], capture_output=True, text=True, check=True).stdout
+        _symbols = {}
+        for line in out.splitlines():
+            parts = line.split(" ", 2)
+            m = _KERNEL.fullmatch(parts[2]) if len(parts) == 3 and parts[1] in "tT" else None
+            if m:
+                _symbols[int(parts[0], 16)] = m.group(1)
+    return _symbols
+
+
+def emulated_kernels() -> set:
+    """The name of every kernel the emulator builds ('render_ao_kernel<0, true, 32>', 'halo_copy_kernel')."""
+    return set(_kernel_symbols().values())
+
+
+def ledger_reset() -> None:
+    lib().frame_ledger_reset()
+
+
+def kernel_ledger() -> dict:
+    """The kernels launched since ledger_reset() in this process: {name: (launches, TMA box loads issued during them)}."""
+    cap = 256
+    off, n_launch, n_tma = (C.c_ulonglong * cap)(), (C.c_longlong * cap)(), (C.c_longlong * cap)()
+    n = lib().frame_ledger_read(off, n_launch, n_tma, cap)
+    assert 0 <= n <= cap
+    names = _kernel_symbols()
+    return {names.get(off[i], hex(off[i])): (n_launch[i], n_tma[i]) for i in range(n)}
 
 
 def composite(ao: np.ndarray, color: np.ndarray, *, rgb: bool, alpha: bool, one_minus: bool) -> np.ndarray:

@@ -3,7 +3,9 @@
 // or returns, so one sweep over the live fibers is one barrier phase.
 #include "cuda_emu.h"
 
+#include <dlfcn.h>
 #include <ucontext.h>
+#include <map>
 #include <vector>
 
 uint3 threadIdx, blockIdx;
@@ -19,6 +21,10 @@ ucontext_t g_sched;
 int g_current = -1;
 const std::function<void()> *g_body = nullptr;
 alignas(128) unsigned char g_dynamic_smem[64 * 1024];
+// the launch ledger: kernel address relative to its library's load base -> {launches, TMA box loads issued during them}.  The kernels
+// live in anonymous namespaces and have no dynamic symbols, so the test suite names them from the library's symbol table (nm).
+std::map<uintptr_t, std::pair<long long, long long>> g_ledger;
+uintptr_t g_next_kernel = 0;         // note_launch's kernel, the next launch's (0: none reported)
 
 void trampoline()
 {
@@ -42,8 +48,18 @@ void unsupported(const char *what)
     abort();
 }
 
+void note_launch(const void *kernel)
+{
+    Dl_info info{};
+    if (!kernel || !dladdr(kernel, &info) || !info.dli_fbase) unsupported("a launch of a kernel outside any loaded library");
+    g_next_kernel = (uintptr_t)kernel - (uintptr_t)info.dli_fbase;
+}
+
 void launch(dim3 grid, dim3 block, size_t dynamic_smem_bytes, const std::function<void()> &body)
 {
+    const uintptr_t kernel = g_next_kernel;
+    g_next_kernel = 0;
+    const long long tma0 = tma_box_loads;
     if (dynamic_smem_bytes > sizeof g_dynamic_smem) unsupported("more than 64 KB of dynamic shared memory");
     const int n = (int)(block.x * block.y * block.z);
     if ((int)g_fibers.size() < n) {
@@ -80,6 +96,23 @@ void launch(dim3 grid, dim3 block, size_t dynamic_smem_bytes, const std::functio
     }
     g_body = nullptr;
     g_current = -1;
+    if (kernel) {
+        auto &e = g_ledger[kernel];
+        e.first++;
+        e.second += tma_box_loads - tma0;
+    }
+}
+
+void ledger_reset() { g_ledger.clear(); }
+
+int ledger_read(unsigned long long *offset, long long *launches, long long *tma_loads, int cap)
+{
+    int n = 0;
+    for (const auto &kv : g_ledger) {
+        if (n < cap) { offset[n] = kv.first; launches[n] = kv.second.first; tma_loads[n] = kv.second.second; }
+        n++;
+    }
+    return n;
 }
 
 }  // namespace meao_emu

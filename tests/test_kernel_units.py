@@ -33,8 +33,8 @@ UNITS = [s for s in SOURCES if s != "meao_api.cu"]
 FMUL_SURPLUS = {
     "prepare_depth.cu": 0, "prepare_depth_layered.cu": 0, "prepare_depth_array.cu": 0,
     "render_ao.cu": 0, "render_ao_layered.cu": 0,
-    "blur_upsample.cu": 12, "blur_upsample_layered.cu": 12,
-    "blur_upsample_lin.cu": 22,     # its 12 kernels (blur_upsample.cu: 12 for 8)
+    "blur_upsample.cu": 6, "blur_upsample_layered.cu": 6,      # the premin kernels: 2 in the final level's, 4 in the blend levels'
+    "blur_upsample_lin.cu": 22,     # its 12 kernels
     "blur_upsample_array.cu": 2,    # the two final-level kernels
     "selftest.cu": 0, "halo.cu": 0, "band_exchange.cu": 0, "composite.cu": 0, "debug_view.cu": 0,
 }
@@ -44,7 +44,7 @@ NO_MUL = {"halo.cu", "band_exchange.cu"}        # copies only: no mul.rn.f32 to 
 ENTRIES = {
     "prepare_depth.cu": 14, "prepare_depth_layered.cu": 14, "prepare_depth_array.cu": 5,
     "render_ao.cu": 13, "render_ao_layered.cu": 12,
-    "blur_upsample.cu": 8, "blur_upsample_layered.cu": 8, "blur_upsample_array.cu": 2, "blur_upsample_lin.cu": 12,
+    "blur_upsample.cu": 4, "blur_upsample_layered.cu": 4, "blur_upsample_array.cu": 2, "blur_upsample_lin.cu": 12,
     "selftest.cu": 1, "halo.cu": 1, "band_exchange.cu": 1, "composite.cu": 2, "debug_view.cu": 3,
 }
 
