@@ -228,7 +228,7 @@ namespace MiniEngineAO
             return true;
         }
 
-        // Hands LayerCameras to the plugin; returns 1 if it re-planned.  The same table again returns 0, so this runs every frame.
+        // Hands LayerCameras to the plugin; returns 1 if a value changed (the next frame takes it without a re-plan).  The same table again returns 0, so this runs every frame.
         int SetLayerCameras()
         {
             if (_layerCameras == null) return MeaoNative.meao_set_layer_cameras(_ctx, null, 0);

@@ -132,16 +132,29 @@ void meao_destroy(MeaoCtx *ctx);
 const char *meao_last_error(const MeaoCtx *ctx);   /* ctx may be NULL: error of the last failed meao_create on this thread */
 int meao_abi_version(void);
 
-/* ---- parameters (plan inputs) ---------------------------------------------------------------- */
-/* replaces: the property setters AO.cs:22-66.  Marks the plan dirty iff a value changed
- * (CheckPropertiesChanged, AO.cs:104-113); returns 1 if the plan was dirtied, 0 if not. */
+/* ---- parameters (plan inputs) ----------------------------------------------------------------
+ * The plan inputs fall into two classes.
+ * FRAME CONSTANTS take effect at the next frame issued on the context, with no device or stream synchronise, no re-plan, no graph
+ * dropped or instantiated, no CUDA array released and no planned size forgotten (meao_reserve): the five floats of MeaoParams (and
+ * `debug`, which selects nothing), the near_clip, far_clip and tan_half_fov_h of a MeaoCamera, and the whole meao_set_layer_cameras
+ * table, clearing it included.  The host plans the new constants at once (the constant getters below return them), the next frame
+ * writes the per-layer camera tables on its own stream before its kernels, and each captured graph is re-targeted to the new kernel
+ * arguments (cudaGraphExecUpdate) at its next launch.  Under the ordering contract (meao_reserve) frame n sees the constants set
+ * before it was issued, and frame n-1, still in flight, keeps its own.  A host may therefore animate the camera and the
+ * parameters every frame.
+ * STRUCTURAL INPUTS re-plan with a device synchronise and drop the captured graphs: MeaoVariants, meao_set_layers, a resize without
+ * a reservation, meao_reserve, row bands, and a change of the cameras' reversed_z (it selects kernel instantiations; it is a
+ * platform property).
+ * A refused camera, table or parameter block leaves the context exactly as it was. */
+/* replaces: the property setters AO.cs:22-66 (CheckPropertiesChanged, AO.cs:104-113): returns 1 if a value changed, 0 if not. */
 int meao_set_params(MeaoCtx *ctx, const MeaoParams *params);
 int meao_get_params(const MeaoCtx *ctx, MeaoParams *out);
 void meao_default_params(MeaoParams *out);          /* AO.cs:20-68 defaults */
-/* Selects the undispatched shader variants above; returns 1 if the plan was dirtied, 0 if not. */
+/* Selects the undispatched shader variants above (a structural input); returns 1 if a value changed, 0 if not. */
 int meao_set_variants(MeaoCtx *ctx, const MeaoVariants *variants);
 int meao_get_variants(const MeaoCtx *ctx, MeaoVariants *out);
-/* replaces: CalculateZBufferParams / CalculateTanHalfFovHeight inputs (AO.cs:561-573). */
+/* replaces: CalculateZBufferParams / CalculateTanHalfFovHeight inputs (AO.cs:561-573).  A frame constant, except reversed_z;
+ * returns MEAO_OK. */
 int meao_set_camera(MeaoCtx *ctx, const MeaoCamera *camera);
 /* replaces: RTHandle.SetBaseDimensions + AllocateNow + the rebuild it triggers (AO.cs:338-341, 501-506).
  * Allocates the intermediates for width x height.  Returns 1 if dimensions changed, 0 if not.
@@ -162,8 +175,11 @@ int meao_resize(MeaoCtx *ctx, int32_t width, int32_t height);
  *     MEAO_ERR_NOMEM leaves the previous reservation and arena in place.
  *   - meao_resize on a reserved context returns 1 when the size changed, as always; a size outside the reservation is refused with
  *     MEAO_ERR_INVALID and changes nothing -- a dynamic-resolution host never gets a silent re-allocation.
- *   - meao_set_layers re-allocates at the reservation x the new layer count.  A change of MeaoParams, MeaoVariants or a camera
- *     re-plans with a device synchronise, as without a reservation, and forgets the other planned sizes; the arena stays.
+ *   - meao_set_layers re-allocates at the reservation x the new layer count.  A change of MeaoVariants or of the cameras' reversed_z
+ *     re-plans with a device synchronise, as without a reservation, and forgets the other planned sizes; the arena stays.  A change
+ *     of a frame constant (MeaoParams, a camera's planes and field of view, the layer-camera table) keeps every planned size: a size
+ *     parked with older constants is planned again on the host when it is swapped back in, and its graphs are re-targeted at their
+ *     first replay.
  *   - Row bands and reservations exclude each other: meao_reserve on a context with a row band, and meao_set_row_band, the halo calls
  *     and the native exchange on a reserved context, return MEAO_ERR_UNSUPPORTED.
  *   - After a size change the intermediates (meao_get_buffer, meao_debug_view) describe the new size; their contents are unspecified
@@ -208,8 +224,9 @@ int meao_set_layers(MeaoCtx *ctx, int32_t layers);
  * size stay shared.  count must equal meao_set_layers; cameras == NULL with count == 0 clears the table, and every layer then uses
  * the meao_set_camera camera again.  Each entry is validated like meao_set_camera, and all entries must have the same reversed_z
  * (a platform property).  A refusal returns MEAO_ERR_INVALID, names the layer and field in meao_last_error, and changes nothing.
- * A plan input like meao_set_camera: returns 1 if the plan was dirtied (the next frame re-plans and drops the captured graphs),
- * 0 if the same table is set again -- so a host may call it every frame.  While a table is set it alone defines every layer's
+ * A frame constant like meao_set_camera's planes and field of view: returns 1 if a value changed (the next frame takes the new table
+ * without a re-plan), 0 if the same table is set again -- so a host may call it every frame.  A table (or clearing one) that
+ * changes the Z direction in effect is a structural change and re-plans.  While a table is set it alone defines every layer's
  * camera; meao_set_camera still records the shared camera, which takes effect when the table is cleared.  A change of the layer
  * count clears the table.  Works on plan-only contexts (device < 0); with layers == 1 a table of one camera behaves exactly like
  * meao_set_camera. */
@@ -221,8 +238,8 @@ int meao_get_layer_cameras(const MeaoCtx *ctx, MeaoCamera *out, int32_t capacity
 /* replaces: replay of the "SSAO" command buffer, steps 1-10 of RebuildCommandBuffers (AO.cs:511-531):
  * Downsample1+2, Render x4, Upsample x4.  depth: device pointer, width*height f32, rows contiguous
  * (row pitch = width*4).  ao_out: device pointer, width*height bytes (R8, AO.cs:475).
- * stream: a cudaStream_t, used as given (NULL = the CUDA legacy default stream).  Asynchronous.  Re-plans first if dirty
- * (LateUpdate, AO.cs:329-350). */
+ * stream: a cudaStream_t, used as given (NULL = the CUDA legacy default stream).  Asynchronous.  Re-plans first after a structural
+ * change (LateUpdate, AO.cs:329-350); takes changed frame constants without one. */
 int meao_render(MeaoCtx *ctx, const void *depth_dev, int32_t depth_kind, void *ao_out_dev, void *stream);
 /* ---- pitched views -----------------------------------------------------------------------------------------------------------
  * meao_render with the depth and the AO as views inside larger allocations, every pitch in BYTES: a cudaMallocPitch / cudaMalloc3D
@@ -275,8 +292,9 @@ int meao_render_host(MeaoCtx *ctx, const void *depth_host, int32_t depth_kind, u
  * Before freeing, unmapping or re-registering an array this context has rendered with (or bound with meao_bind_event_arrays), call
  * meao_release_array(ctx, array): it synchronises the device, drops that array's graphs, surface object and event bindings.  A new
  * array may come back with the same handle, and without the release the next frame would replay into freed memory.
- * meao_destroy and every plan change (meao_resize, meao_set_layers, meao_set_params / _variants / _camera changes, meao_set_row_band)
- * release all arrays.  Releasing an array this context never used returns MEAO_OK. */
+ * meao_destroy and every structural plan change (meao_resize without a reservation, meao_reserve, meao_set_layers, meao_set_variants,
+ * a reversed_z change, meao_set_row_band) release all arrays; a frame-constant change (MeaoParams, the cameras' planes and fields of
+ * view) releases none.  Releasing an array this context never used returns MEAO_OK. */
 int meao_render_arrays(MeaoCtx *ctx, const void *depth_array, int32_t depth_kind, void *ao_array, void *stream);
 int meao_release_array(MeaoCtx *ctx, const void *array);
 /* Pipelined form of meao_render_host for frame streams: enqueues H2D + kernels + D2H of one frame on staging slot

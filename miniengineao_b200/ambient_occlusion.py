@@ -134,7 +134,8 @@ class AmbientOcclusion:
 
     # ---- LateUpdate: re-plan only when something changed (AO.cs:329-350) ---------------------------
     def LateUpdate(self) -> bool:
-        """Once per frame (AO.cs:329-350); render() / render_host() call it themselves.  Returns True when it re-planned."""
+        """Once per frame (AO.cs:329-350); render() / render_host() call it themselves.  Returns True when a plan input changed
+        (a changed parameter or layer-camera table is taken by the next frame without a re-plan; see include/meao.h)."""
         return self._update(True)
 
     def _update(self, frame: bool) -> bool:
@@ -191,7 +192,7 @@ class AmbientOcclusion:
         return {f: getattr(r, f) for f, _ in N.MeaoReservation._fields_}
 
     def _apply_layer_cameras(self) -> bool:
-        """Hands layerCameras to meao_set_layer_cameras (after meao_set_layers, which clears the table); True if it re-planned."""
+        """Hands layerCameras to meao_set_layer_cameras (after meao_set_layers, which clears the table); True if a value changed."""
         cams = self.layerCameras
         if cams is None:
             return self._check(self._lib.meao_set_layer_cameras(self._ctx, None, 0)) == 1

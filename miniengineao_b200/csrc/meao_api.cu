@@ -48,9 +48,10 @@ struct SizeState : FrameState {
     int prev0 = -1, next1 = -1;             // the neighbour bands' extents (meao_set_row_band)
     Range need_low[5];                      // rows of LowDepth<k> required by this band
     Range own_low[5];                       // rows of LowDepth<k> this band produces
-    bool cam_table_stale = true;            // layer_consts changed since the device tables were written (ensure_ready uploads them)
+    bool cam_table_stale = true;            // a structural re-plan changed layer_consts (ensure_ready uploads them after a device synchronise)
     int slot = 0;                           // the arena slot of this size's camera tables (FrameState::layer_zb / layer_ren)
     bool table_pending = false;             // the slot's tables are not written yet: the next frame writes them on its own stream
+    uint64_t plan_gen = 0;                  // the frame-constant generation (MeaoCtx::consts_gen) this size's plan was built at
 };
 
 }  // namespace
@@ -69,7 +70,10 @@ struct MeaoCtx : SizeState {
     MeaoCamera camera;
     std::vector<MeaoCamera> layer_cams;     // meao_set_layer_cameras: one camera per layer, or empty (every layer uses `camera`)
     MeaoVariants variants = {0, 0, 0, 0};
-    bool plan_dirty = true;
+    bool plan_dirty = true;                 // a structural input changed: the next frame re-plans (replan)
+    // Frame constants (include/meao.h): bumped by every change of MeaoParams or of a camera that keeps the Z direction.  A size whose
+    // plan_gen is older re-plans its constants on the host (refresh_constants); a graph captured at an older one re-targets (launch_cached).
+    uint64_t consts_gen = 0;
 
     // meao_reserve: the arena is laid out for res_w x res_h (0 x 0: for the current size) and every size inside it keeps its plan
     int res_w = 0, res_h = 0;
@@ -103,7 +107,8 @@ struct MeaoCtx : SizeState {
 
     // CUDA graph cache: one instantiated graph per (depth, out, kind), LRU; when it is full the least recently used
     // executable graph is RE-TARGETED in place with cudaGraphExecUpdate (same topology, new pointers: no device
-    // synchronisation, launches already enqueued are unaffected).  Dropped as a whole only when the plan changes.
+    // synchronisation, launches already enqueued are unaffected), and so is a graph captured before the frame constants last
+    // changed, at its next launch (new kernel arguments).  Dropped as a whole only when a structural plan input changes.
     // kind: the depth kind of a pointer frame; 100+ / 200+ / 300+ band graphs; kArrayGraphKind+ array frames (the key holds
     // cudaArray_t handles, so a pointer equal to a handle value never finds an array frame's graph, nor the reverse).
     // pitch: the byte pitches of a pointer frame's depth and AO views (meao_render_pitched; 0 for the other kinds) -- a frame at the
@@ -116,7 +121,8 @@ struct MeaoCtx : SizeState {
         for (int i = 0; i < 4; i++) if (pitch[i] != o.pitch[i]) return pitch[i] < o.pitch[i];
         for (int i = 0; i < 3; i++) if (size[i] != o.size[i]) return size[i] < o.size[i];
         return false; } };
-    struct GraphEntry { cudaGraphExec_t exec; uint64_t last_use; int launches; };     // launches: the kernels its capture recorded
+    // launches: the kernels its capture recorded; gen: the plan_gen of the constants it launches with
+    struct GraphEntry { cudaGraphExec_t exec; uint64_t last_use; int launches; uint64_t gen; };
     std::map<GraphKey, GraphEntry> graphs;
     // executable graphs that cudaGraphExecUpdate could not re-target while they were possibly in flight; `done` is recorded after the
     // frame that replaced them, so once it has completed (and, frames of a context running in order, every earlier frame) the graph
@@ -179,6 +185,14 @@ void sample_thickness(float t[12])
 // Z direction of the context's cameras (meao_set_layer_cameras requires one for all layers)
 inline int ctx_reversed_z(const MeaoCtx *c) { return c->layer_cams.empty() ? c->camera.reversed_z : c->layer_cams[0].reversed_z; }
 
+// A change of the cameras in effect.  Their near and far planes and fields of view are frame constants; their Z direction selects
+// kernel instantiations (prepare_slot), so a change of it re-plans like any structural input.
+void note_camera_change(MeaoCtx *c, int old_reversed_z, int new_reversed_z)
+{
+    if (old_reversed_z != new_reversed_z) c->plan_dirty = true;
+    else c->consts_gen++;
+}
+
 // The camera-dependent constants of camera `cam` (the part of build_plan that reads the camera).
 void camera_consts(const MeaoCtx *c, const MeaoCamera &cam, CamConsts &p)
 {
@@ -229,7 +243,6 @@ void build_plan(MeaoCtx *c)
             else camera_consts(c, c->layer_cams[l], c->layer_consts[l]);
         }
     }
-    c->cam_table_stale = true;
     // the Plan's own camera constants: the first layer's
     const CamConsts &cc = c->layer_consts[0];
     p.zb[0] = cc.zb[0]; p.zb[1] = cc.zb[1];
@@ -272,6 +285,7 @@ void build_plan(MeaoCtx *c)
         p.upsample_tolerance[lo] = upsampleTolerance;
     }
     c->plan_dirty = false;
+    c->plan_gen = c->consts_gen;
 }
 
 // Caller must have made c->device current (ensure_ready / meao_resize / meao_destroy do).
@@ -421,9 +435,22 @@ int allocate(MeaoCtx *c, bool keep_old = false)
     return place_size(c, 0);
 }
 
+// A frame-constant change (include/meao.h) since the current size was planned: its constants are planned again on the host, and its
+// camera tables are written by the next frame on that frame's stream (write_tables) -- no synchronise, no graph dropped; the graphs
+// re-target at their next launch (launch_cached).  A pending structural re-plan (plan_dirty) covers the constants itself.
+void refresh_constants(MeaoCtx *c)
+{
+    if (c->plan_dirty || c->W <= 0 || c->plan_gen == c->consts_gen) return;
+    build_plan(c);
+    c->table_pending = !c->plan_only;
+}
+
 // Reserved contexts: make w x h the current size without touching the device.  The current size is parked in its slot; a size parked
 // earlier is swapped back in as it was (plan, maps, camera tables); a new size takes a free slot or the least recently used one, and
 // is planned on the host -- its camera tables are written by its first frame, on that frame's stream (write_tables).
+// HAZARD: a parked size keeps the constants it was parked with.  Frame constants may have changed since, so a size swapped back in
+// re-plans its constants here (refresh_constants) before any frame or getter can read them, and its graphs re-target at their first
+// replay; it must never replay with the constants it was parked with.
 int switch_size(MeaoCtx *c, int w, int h)
 {
     SizeState &cur = *c;
@@ -434,6 +461,7 @@ int switch_size(MeaoCtx *c, int w, int h)
         if (s.valid && s.s.W == w && s.s.H == h) {
             cur = s.s;
             s.last_use = ++c->size_clock;
+            refresh_constants(c);
             return 0;
         }
         if (slot < 0 || (c->size_slots[slot].valid && (!s.valid || s.last_use < c->size_slots[slot].last_use))) slot = i;
@@ -450,8 +478,8 @@ int switch_size(MeaoCtx *c, int w, int h)
     return 0;
 }
 
-// Write the per-layer camera tables to the arena.  Called by ensure_ready after a re-plan, once every frame that may read the old
-// tables has finished (a device synchronise: frames may be in flight on any caller stream).
+// Write the per-layer camera tables to the arena.  Called by ensure_ready after a structural re-plan, once every frame that may read the
+// old tables has finished (a device synchronise: frames may be in flight on any caller stream).
 int upload_camera_tables(MeaoCtx *c)
 {
     std::vector<LayerZ> zb;
@@ -465,9 +493,10 @@ int upload_camera_tables(MeaoCtx *c)
     return 0;
 }
 
-// The tables of a size newly planned by switch_size, written in stream order before the first frame that reads them, on that frame's
-// stream.  The slot may have held another size's tables: frames of one context run in the order they are issued (include/meao.h),
-// so every earlier frame that read it has completed before this copy lands.  The source is pageable, so the runtime stages it and
+// The tables of a size newly planned by switch_size, or re-planned after a frame-constant change (refresh_constants), written in
+// stream order before the first frame that reads them, on that frame's stream.  The slot may have held another size's tables, or
+// this size's older ones: frames of one context run in the order they are issued (include/meao.h), so every earlier frame that
+// read it has completed before this copy lands.  The source is pageable, so the runtime stages it and
 // the vectors may go when the call returns.
 int write_tables(MeaoCtx *c, cudaStream_t s)
 {
@@ -481,10 +510,12 @@ int write_tables(MeaoCtx *c, cudaStream_t s)
     return 0;
 }
 
-// A re-plan after a plan input changed: the parked sizes were planned with the old inputs, so they go (with the captured graphs).
+// A re-plan after a structural plan input changed: the parked sizes were planned with the old inputs, so they go (with the captured
+// graphs), and the tables are uploaded after a device synchronise (upload_camera_tables).
 void replan(MeaoCtx *c)
 {
     build_plan(c);
+    c->cam_table_stale = true;
     c->graphs_stale = true;
     for (int i = 0; i < kSizeSlots; i++) if (i != c->slot) c->size_slots[i].valid = false;
 }
@@ -496,12 +527,14 @@ int ensure_ready(MeaoCtx *c)
     if (c->plan_only) return fail(c, MEAO_ERR_CUDA, "plan-only context (device < 0): no CUDA device bound, and libmeao has no CPU fallback");
     CUDA_TRY(c, cudaSetDevice(c->device));
     if (c->plan_dirty) replan(c);
+    refresh_constants(c);
     if (c->graphs_stale) drop_graph(c);
     if (c->cam_table_stale) { int rc = upload_camera_tables(c); if (rc) return rc; }
     return 0;
 }
 
-// ensure_ready for an entry point that issues work on stream s which may read the camera tables
+// ensure_ready for an entry point that issues work on stream s which may read the camera tables: every frame form, band phase and
+// stage call, so that each sees the tables of the constants set before it was issued
 int frame_ready(MeaoCtx *c, cudaStream_t s)
 {
     int rc = ensure_ready(c);
@@ -783,7 +816,7 @@ int meao_set_params(MeaoCtx *c, const MeaoParams *p)
                    c->params.intensity != p->intensity || c->params.debug != p->debug;
     if (!(p->thickness_modifier > 0.0f)) return fail(c, MEAO_ERR_INVALID, "thickness_modifier must be > 0");
     c->params = *p;
-    if (changed) c->plan_dirty = true;
+    if (changed) c->consts_gen++;                   // frame constants: the next frame takes them without a re-plan
     return changed ? 1 : 0;
 }
 
@@ -819,8 +852,9 @@ int meao_set_camera(MeaoCtx *c, const MeaoCamera *cam)
     if (!(cam->near_clip > 0) || !(cam->far_clip > cam->near_clip) || !(cam->tan_half_fov_h > 0))
         return fail(c, MEAO_ERR_INVALID, "bad camera (near %g far %g tanHalfFovH %g)", cam->near_clip, cam->far_clip, cam->tan_half_fov_h);
     if (memcmp(&c->camera, cam, sizeof *cam) != 0) {
+        const int old_z = c->camera.reversed_z;
         c->camera = *cam;
-        if (c->layer_cams.empty()) c->plan_dirty = true;    // with a layer-camera table it takes effect when the table is cleared
+        if (c->layer_cams.empty()) note_camera_change(c, old_z, cam->reversed_z);   // with a layer-camera table it takes effect when the table is cleared
     }
     return MEAO_OK;
 }
@@ -830,8 +864,9 @@ int meao_set_layer_cameras(MeaoCtx *c, const MeaoCamera *cams, int32_t count)
     if (!c) return MEAO_ERR_INVALID;
     if (!cams && count == 0) {
         if (c->layer_cams.empty()) return 0;
+        const int old_z = ctx_reversed_z(c);
         c->layer_cams.clear();
-        c->plan_dirty = true;
+        note_camera_change(c, old_z, c->camera.reversed_z);
         return 1;
     }
     if (!cams) return fail(c, MEAO_ERR_INVALID, "cameras is NULL with count %d (NULL clears the table only with count 0)", count);
@@ -847,8 +882,9 @@ int meao_set_layer_cameras(MeaoCtx *c, const MeaoCamera *cams, int32_t count)
                         k.reversed_z, cams[0].reversed_z);
     }
     if ((int)c->layer_cams.size() == count && memcmp(c->layer_cams.data(), cams, (size_t)count * sizeof(MeaoCamera)) == 0) return 0;
+    const int old_z = ctx_reversed_z(c);
     c->layer_cams.assign(cams, cams + count);
-    c->plan_dirty = true;
+    note_camera_change(c, old_z, cams[0].reversed_z);
     return 1;
 }
 
@@ -1054,7 +1090,7 @@ int meao_halo_unpack(MeaoCtx *c, int32_t side, const void *packed, void *stream)
 int meao_render_band_prepare(MeaoCtx *c, const void *depth, int32_t kind, void *stream)
 {
     BAND_GUARD(c, "meao_render_band_prepare");
-    int rc = ensure_ready(c); if (rc) return rc;
+    int rc = frame_ready(c, (cudaStream_t)stream); if (rc) return rc;
     if (!depth) return fail(c, MEAO_ERR_INVALID, "depth is NULL");
     return record_downsample(c, depth, kind, (cudaStream_t)stream);
 }
@@ -1062,7 +1098,7 @@ int meao_render_band_prepare(MeaoCtx *c, const void *depth, int32_t kind, void *
 int meao_render_band_finish(MeaoCtx *c, void *ao_out, void *stream)
 {
     BAND_GUARD(c, "meao_render_band_finish");
-    int rc = ensure_ready(c); if (rc) return rc;
+    int rc = frame_ready(c, (cudaStream_t)stream); if (rc) return rc;
     return record_frame(c, frame_io(c, nullptr, c->last_kind, ao_out, false), (cudaStream_t)stream, 1, false);
 }
 
@@ -1136,7 +1172,27 @@ static void reclaim_retired(MeaoCtx *c, bool wait)
     }
 }
 
-// Replays the graph of `key`, captured from record(stream, pdl) on first use; a replay counts the launches its capture recorded.
+// Re-targets the executable graph *ge to the freshly captured g with cudaGraphExecUpdate: new kernel arguments and pointers, no device
+// synchronise, launches already enqueued are unaffected.  When the update is refused (another topology), *ge is retired instead -- its
+// `done` event is recorded on s now and again after the frame that replaces it (*retiring) -- and *ge becomes nullptr: the caller
+// instantiates g.
+static int retarget(MeaoCtx *c, cudaGraphExec_t *ge, cudaGraph_t g, cudaStream_t s, bool *retiring)
+{
+    cudaGraphExecUpdateResultInfo info;
+    if (cudaGraphExecUpdate(*ge, g, &info) == cudaSuccess) return 0;
+    cudaGetLastError();
+    cudaEvent_t done = nullptr;
+    if (cudaEventCreateWithFlags(&done, cudaEventDisableTiming) != cudaSuccess) return fail(c, MEAO_ERR_CUDA, "cudaEventCreate failed");
+    c->retired.push_back(MeaoCtx::Retired{*ge, done});
+    cudaEventRecord(done, s);                       // recorded again after the new launch; this covers a launch that fails
+    *retiring = true;
+    *ge = nullptr;
+    return 0;
+}
+
+// Replays the graph of `key`, captured from record(stream, pdl) on first use; a replay counts the launches its capture recorded.  A
+// graph captured before the frame constants last changed (its gen) is captured again and re-targeted in place before it is launched:
+// lazily, so a change costs one capture + update per graph actually replayed, not one per cached graph.
 static int launch_cached(MeaoCtx *c, const MeaoCtx::GraphKey &key_in, cudaStream_t s, const std::function<int(cudaStream_t, int)> &record)
 {
     if (c->flags & MEAO_FLAG_NO_GRAPH) return record(s, 0);
@@ -1144,29 +1200,23 @@ static int launch_cached(MeaoCtx *c, const MeaoCtx::GraphKey &key_in, cudaStream
     key.size[0] = c->W; key.size[1] = c->H; key.size[2] = c->slot;
     auto it = c->graphs.find(key);
     bool retiring = false;
-    if (it == c->graphs.end()) {
+    if (it == c->graphs.end() || it->second.gen != c->plan_gen) {
         if (!c->retired.empty()) reclaim_retired(c, c->retired.size() >= kMaxRetired);
         cudaGraph_t g = nullptr;
         int launches = 0;
         int rc = capture_graph(c, record, &g, &launches);
         if (rc) return rc;
         cudaGraphExec_t ge = nullptr;
-        if (c->graphs.size() >= kMaxGraphs) {
+        auto victim = it;
+        if (victim == c->graphs.end() && c->graphs.size() >= kMaxGraphs) {
             // a caller that rotates more buffers (or visits more frame sizes) than the cache holds: re-target the least recently used
             // executable graph (same topology, new kernel arguments) instead of synchronising the device and instantiating again
-            auto victim = c->graphs.begin();
+            victim = c->graphs.begin();
             for (auto j = c->graphs.begin(); j != c->graphs.end(); ++j) if (j->second.last_use < victim->second.last_use) victim = j;
-            cudaGraphExecUpdateResultInfo info;
+        }
+        if (victim != c->graphs.end()) {
             ge = victim->second.exec;
-            if (cudaGraphExecUpdate(ge, g, &info) != cudaSuccess) {
-                cudaGetLastError();
-                cudaEvent_t done = nullptr;
-                if (cudaEventCreateWithFlags(&done, cudaEventDisableTiming) != cudaSuccess) { cudaGraphDestroy(g); return fail(c, MEAO_ERR_CUDA, "cudaEventCreate failed"); }
-                c->retired.push_back(MeaoCtx::Retired{ge, done});
-                cudaEventRecord(done, s);           // recorded again after the new launch below; this covers a launch that fails
-                retiring = true;
-                ge = nullptr;
-            }
+            if ((rc = retarget(c, &ge, g, s, &retiring))) { cudaGraphDestroy(g); return rc; }
             c->graphs.erase(victim);
         }
         if (!ge) {
@@ -1182,7 +1232,7 @@ static int launch_cached(MeaoCtx *c, const MeaoCtx::GraphKey &key_in, cudaStream
             c->graph_instantiations++;
         }
         cudaGraphDestroy(g);
-        it = c->graphs.emplace(key, MeaoCtx::GraphEntry{ge, 0, launches}).first;
+        it = c->graphs.emplace(key, MeaoCtx::GraphEntry{ge, 0, launches, c->plan_gen}).first;
     }
     it->second.last_use = ++c->graph_clock;
     CUDA_TRY(c, cudaGraphLaunch(it->second.exec, s));
@@ -1194,7 +1244,7 @@ static int launch_cached(MeaoCtx *c, const MeaoCtx::GraphKey &key_in, cudaStream
 int meao_band_phase_a(MeaoCtx *c, const void *depth, int32_t kind, void *send_up, void *send_down, void *stream)
 {
     BAND_GUARD(c, "meao_band_phase_a");
-    int rc = ensure_ready(c); if (rc) return rc;
+    int rc = frame_ready(c, (cudaStream_t)stream); if (rc) return rc;
     if (!depth) return fail(c, MEAO_ERR_INVALID, "depth is NULL");
     c->last_kind = kind;
     const MeaoCtx::GraphKey key{{depth, send_up, send_down, nullptr}, 100 + kind};
@@ -1209,7 +1259,7 @@ int meao_band_phase_a(MeaoCtx *c, const void *depth, int32_t kind, void *send_up
 int meao_band_phase_b(MeaoCtx *c, const void *recv_up, const void *recv_down, void *ao_out, void *stream)
 {
     BAND_GUARD(c, "meao_band_phase_b");
-    int rc = ensure_ready(c); if (rc) return rc;
+    int rc = frame_ready(c, (cudaStream_t)stream); if (rc) return rc;
     if (!ao_out) return fail(c, MEAO_ERR_INVALID, "ao_out is NULL");
     const int kind = c->last_kind;
     const MeaoCtx::GraphKey key{{recv_up, recv_down, ao_out, nullptr}, 200 + kind};
@@ -1332,7 +1382,7 @@ static int record_exchange(MeaoCtx *c, cudaStream_t s)
 int meao_band_step(MeaoCtx *c, const void *depth, int32_t kind, void *ao_out, void *stream)
 {
     BAND_GUARD(c, "meao_band_step");
-    int rc = ensure_ready(c); if (rc) return rc;
+    int rc = frame_ready(c, (cudaStream_t)stream); if (rc) return rc;
     if (!depth || !ao_out) return fail(c, MEAO_ERR_INVALID, "depth / ao_out is NULL");
     if ((c->prev0 >= 0 && !c->peer_base[0]) || (c->next1 >= 0 && !c->peer_base[1]))
         return fail(c, MEAO_ERR_INVALID, "meao_band_step: connect every neighbour first (meao_band_export / meao_band_connect)");
@@ -1767,6 +1817,7 @@ static int plan_only(MeaoCtx *c)
 {
     if (!c || c->W <= 0) return MEAO_ERR_INVALID;
     if (c->plan_dirty) replan(c);           // the captured graphs are dropped by the next ensure_ready, on c->device
+    refresh_constants(c);                   // the tables are written by the next frame, on its stream
     return 0;
 }
 
