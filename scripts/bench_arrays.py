@@ -36,7 +36,7 @@ def gpu_info() -> dict:
 
 
 def run_config(torch, rt, W, H, L, shape, frames, rounds):
-    from test_arrays_gpu import Array, Extent, Memcpy3DParms, PitchedPtr   # the ctypes CUDA-array helpers of the GPU tests
+    from gpu_harness import Array, Extent, Memcpy3DParms, PitchedPtr   # the ctypes CUDA-array helpers of the GPU tests
     from miniengineao_b200 import AmbientOcclusion, Camera, synth
     ao = AmbientOcclusion(Camera(W, H), device=0)
     ao.layers = L
@@ -114,15 +114,9 @@ def main():
     if not torch.cuda.is_available():
         sys.exit("bench_arrays.py needs a GPU")
     torch.cuda.init()
-    rt = C.CDLL("libcudart.so.12")
-    from test_arrays_gpu import ChannelDesc, Extent, Memcpy3DParms  # noqa: F401
-    rt.cudaMallocArray.argtypes = [C.POINTER(C.c_void_p), C.POINTER(ChannelDesc), C.c_size_t, C.c_size_t, C.c_uint]
-    rt.cudaMalloc3DArray.argtypes = [C.POINTER(C.c_void_p), C.POINTER(ChannelDesc), Extent, C.c_uint]
-    rt.cudaFreeArray.argtypes = [C.c_void_p]
-    rt.cudaMemcpy3D.argtypes = [C.POINTER(Memcpy3DParms)]
+    from gpu_harness import Memcpy3DParms, runtime
+    rt = runtime()
     rt.cudaMemcpy3DAsync.argtypes = [C.POINTER(Memcpy3DParms), C.c_void_p]
-    rt.cudaMemcpy2DToArray.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int]
-    rt.cudaMemcpy2DFromArray.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int]
     print(json.dumps({"gpu": gpu_info()}), flush=True)
     for cfg in args.configs.split(","):
         size, shape = cfg.split(":")

@@ -5,8 +5,8 @@ Every fast path in the kernels replaces IEEE division by a reciprocal that is on
 [2^-60, 2^60) and tests that range once for a whole group (eight pixels of linearize8, a render pair, four upsample texels, the
 bilateral pair sums); outside it the group must take the plain IEEE operators and give the oracle's bits.  So the values below sit at
 every lane of those groups, at tile seams, on the texels LowDepth1..4 sample, in solid blocks and in a checkerboard with ordinary
-depth.  The comparison helper treats two NaNs as equal whatever their sign or payload (the GPU returns the canonical NaN, the oracle
-keeps payloads) and everything else -- signed zeros and infinities included -- bit for bit."""
+depth.  The hostile-input tests compare with harness.n_diff(nan_equal=True): two NaNs match whatever their sign or payload (the GPU
+returns the canonical NaN, the oracle keeps payloads) and everything else -- signed zeros and infinities included -- bit for bit."""
 from __future__ import annotations
 
 import math
@@ -157,10 +157,6 @@ def camera(name: str, W: int, H: int, reversed_z: bool):
     return Camera(W, H, nearClipPlane=near, farClipPlane=far, usesReversedZBuffer=reversed_z, **kw)
 
 
-def oracle_camera_kw(cam) -> dict:
-    return dict(near=cam.nearClipPlane, far=cam.farClipPlane, tan_half_fov_h_=1.0 / cam.projection00, reversed_z=cam.usesReversedZBuffer)
-
-
 # ---- parameters ---------------------------------------------------------------------------------------------------------------
 # upsample_tolerance -16.55 / -16.56 put 10^x on either side of 2^-55; 0 and +20 (10^20 >= 2^60) on either side of the top;
 # noise_filter_tolerance 15.65 / 15.66 put noise_filter_strength on either side of 2^-52
@@ -184,36 +180,3 @@ def fast_div_sides(plan) -> set:
         uc = plan.upsample_constants(lo)
         out.add(fast_div_ok(float(uc["upsample_tolerance"]), float(uc["noise_filter_strength"])))
     return out
-
-
-# ---- comparison -----------------------------------------------------------------------------------------------------------------
-def n_diff(got: np.ndarray, ref: np.ndarray) -> int:
-    """Elements that differ: unorm8 codes exactly; f16 / f32 bit for bit, except that any two NaNs match."""
-    if got.dtype == np.uint8:
-        return int((got != ref).sum())
-    if got.dtype == np.float16:
-        with np.errstate(over="ignore", invalid="ignore"):
-            ref = np.asarray(ref).astype(np.float16)
-        same = got.view(np.uint16) == ref.view(np.uint16)
-    else:
-        ref = np.asarray(ref, np.float32)
-        same = got.view(np.uint32) == ref.view(np.uint32)
-    return int((~(same | (np.isnan(got) & np.isnan(ref)))).sum())
-
-
-def buffer_ids(high_quality_mask: int = 0, single_scale: bool = False) -> list:
-    if single_scale:
-        return [1, 2, 3, 4, 5, 10, 17]
-    return list(range(1, 18)) + [17 + k for k in range(1, 5) if (high_quality_mask >> (k - 1)) & 1]
-
-
-def compare_buffers(get, orc, tag: str, ids) -> None:
-    """get(bid) -> the kernel's buffer; orc: an Oracle that has run the same frame."""
-    bad = []
-    for bid in ids:
-        got = get(bid)
-        ref = orc.codes(bid) if got.dtype == np.uint8 else orc.buffer(bid)
-        n = n_diff(got, ref)
-        if n:
-            bad.append((bid, n, got.size))
-    assert not bad, f"{tag}: mismatching buffers (id, #diff, size): {bad}"

@@ -12,9 +12,7 @@ from __future__ import annotations
 
 from dataclasses import dataclass
 
-import numpy as np
-
-from test_layers_emulated import _raw, contrasting_layers  # noqa: E402  (tests/ is on sys.path via conftest)
+import harness  # noqa: E402  (tests/ is on sys.path via conftest)
 
 KINDS = ("linear", "f32", "d16", "d24s8")
 TILE_H = (32, 16, 8)                # forced render tile variant 0 / 1 / 2
@@ -64,9 +62,7 @@ class Case:
 
     def buffer_ids(self) -> list:
         """The intermediates a frame of this case produces (and the AO): debug ids 1-17, 18-21 for its high-quality levels."""
-        if self.single_scale:
-            return [1, 2, 3, 4, 5, 10, 17]
-        return list(range(1, 18)) + [17 + k for k in range(1, 5) if (self.hq >> (k - 1)) & 1]
+        return harness.buffer_ids(self.hq, self.single_scale)
 
 
 def _cases() -> list:
@@ -138,17 +134,10 @@ def depth(c: Case):
     """(depth in the case's ingest format, [layers, H, W]; the float32 the oracle sees per layer).  contrasting_layers with a sky patch
     in layer 2, and in layer 0 of a single-layer frame; native codes carry stencil bits."""
     W, H = c.size
-    lin = contrasting_layers(W, H, c.layers, seed=W + c.layers)
+    lin = harness.contrasting_layers(W, H, c.layers, seed=W + c.layers)
     if c.kind == "linear":
         return lin, lin
-    raw = _raw(lin, reversed_z=c.reversed_z)
+    raw = harness.raw(lin, reversed_z=c.reversed_z)
     if c.layers == 1:
         raw[0, H // 4: H // 2, W // 5: W // 2] = 0.0
-    if c.kind == "f32":
-        return raw, raw
-    bits = 16 if c.kind == "d16" else 24
-    full = (1 << bits) - 1
-    codes = np.clip(np.rint(raw.astype(np.float64) * full), 0, full).astype(np.uint32)
-    as_float = (codes.astype(np.float32) * np.float32(1.0 / full)).astype(np.float32)
-    words = codes.astype(np.uint16) if bits == 16 else codes | (np.uint32(0xA5) << np.uint32(24))
-    return words, as_float
+    return harness.ingest(raw, c.kind)

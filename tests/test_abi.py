@@ -13,6 +13,8 @@ from miniengineao_b200 import AmbientOcclusion, Camera, MeaoError
 from miniengineao_b200 import _native as N
 from oracle.oracle import Oracle
 
+import harness
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
@@ -137,18 +139,9 @@ def test_band_planning_halo_symmetry_and_limits():
         thin.set_row_band(100, 544, 0, 816)         # not 16-row aligned
 
 
-def _build_c_client(tmp_path):
-    exe = os.path.join(str(tmp_path), "meao_c_smoke")
-    libdir = os.path.dirname(N.LIB_PATH)
-    subprocess.check_call(["gcc", "-std=c99", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"),
-                           os.path.join(ROOT, "tests", "c_abi", "smoke.c"), "-o", exe,
-                           "-L", libdir, "-l:libmeao.so", f"-Wl,-rpath,{libdir}"])
-    return exe
-
-
 def test_pure_c_client_plans_without_gpu(tmp_path):
     """include/meao.h compiles as C99 and links against libmeao.so; the planner works and compute fails loudly."""
-    exe = _build_c_client(tmp_path)
+    exe = harness.build_c_client(tmp_path)
     r = subprocess.run([exe, "plan"], capture_output=True, text=True)
     assert r.returncode == 0 and "plan ok" in r.stdout, r.stderr
 

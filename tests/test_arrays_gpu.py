@@ -8,105 +8,10 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from test_layers_gpu import _ctx, _frames, _oracle  # noqa: E402  (tests/ is on sys.path via conftest)
+import harness
+from gpu_harness import KIND_UNORM8, KIND_UNORM16, LAYERED, Array, rt, torch_cuda  # noqa: F401  (the fixtures)
 
 pytestmark = pytest.mark.gpu
-
-LAYERED, SURFACE_LOAD_STORE, CUBEMAP = 0x01, 0x02, 0x04
-KIND_UNSIGNED, KIND_FLOAT, KIND_UNORM8, KIND_UNORM16 = 1, 2, 5, 8
-H2D, D2H = 1, 2
-
-
-class ChannelDesc(C.Structure):
-    _fields_ = [("x", C.c_int), ("y", C.c_int), ("z", C.c_int), ("w", C.c_int), ("f", C.c_int)]
-
-
-class Extent(C.Structure):
-    _fields_ = [("width", C.c_size_t), ("height", C.c_size_t), ("depth", C.c_size_t)]
-
-
-class Pos(C.Structure):
-    _fields_ = [("x", C.c_size_t), ("y", C.c_size_t), ("z", C.c_size_t)]
-
-
-class PitchedPtr(C.Structure):
-    _fields_ = [("ptr", C.c_void_p), ("pitch", C.c_size_t), ("xsize", C.c_size_t), ("ysize", C.c_size_t)]
-
-
-class Memcpy3DParms(C.Structure):
-    _fields_ = [("srcArray", C.c_void_p), ("srcPos", Pos), ("srcPtr", PitchedPtr), ("dstArray", C.c_void_p), ("dstPos", Pos),
-                ("dstPtr", PitchedPtr), ("extent", Extent), ("kind", C.c_int)]
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("GPU tests need a GPU")
-    torch.cuda.init()
-    return torch
-
-
-@pytest.fixture(scope="module")
-def rt(torch_cuda):
-    r = C.CDLL("libcudart.so.12")
-    r.cudaMallocArray.argtypes = [C.POINTER(C.c_void_p), C.POINTER(ChannelDesc), C.c_size_t, C.c_size_t, C.c_uint]
-    r.cudaMalloc3DArray.argtypes = [C.POINTER(C.c_void_p), C.POINTER(ChannelDesc), Extent, C.c_uint]
-    r.cudaFreeArray.argtypes = [C.c_void_p]
-    r.cudaMemcpy3D.argtypes = [C.POINTER(Memcpy3DParms)]
-    r.cudaMemcpy2DToArray.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int]
-    r.cudaMemcpy2DFromArray.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int]
-    return r
-
-
-class Array:
-    """A W x H CUDA array of `layers` layers: shape "2d" (layers 1), "layered" or "cube" (6), one channel of dtype."""
-    DT = {np.dtype(np.float32): (32, KIND_FLOAT), np.dtype(np.uint16): (16, KIND_UNSIGNED), np.dtype(np.uint8): (8, KIND_UNSIGNED)}
-
-    def __init__(self, rt, W, H, dtype, shape="2d", layers=1, flags=SURFACE_LOAD_STORE, kind=None, extra_flags=0):
-        self.rt, self.W, self.H, self.dtype, self.shape = rt, W, H, np.dtype(dtype), shape
-        self.layers = 6 if shape == "cube" else layers
-        bits, k = self.DT[self.dtype]
-        desc = ChannelDesc(bits, 0, 0, 0, k if kind is None else kind)
-        h = C.c_void_p()
-        if shape == "2d":
-            rc = rt.cudaMallocArray(C.byref(h), C.byref(desc), W, H, flags | extra_flags)
-        else:
-            f = flags | extra_flags | (CUBEMAP if shape == "cube" else LAYERED)
-            rc = rt.cudaMalloc3DArray(C.byref(h), C.byref(desc), Extent(W, H, self.layers), f)
-        assert rc == 0, f"array allocation failed ({rc})"
-        self.handle = h.value
-
-    def _copy(self, host, to_array):
-        if self.shape == "2d":
-            wb = self.W * self.dtype.itemsize
-            if to_array:
-                rc = self.rt.cudaMemcpy2DToArray(C.c_void_p(self.handle), 0, 0, C.c_void_p(host.ctypes.data), wb, wb, self.H, H2D)
-            else:
-                rc = self.rt.cudaMemcpy2DFromArray(C.c_void_p(host.ctypes.data), wb, C.c_void_p(self.handle), 0, 0, wb, self.H, D2H)
-        else:
-            p = Memcpy3DParms()
-            hp = PitchedPtr(host.ctypes.data, self.W * self.dtype.itemsize, self.W, self.H)
-            if to_array:
-                p.srcPtr, p.dstArray, p.kind = hp, self.handle, H2D
-            else:
-                p.srcArray, p.dstPtr, p.kind = self.handle, hp, D2H
-            p.extent = Extent(self.W, self.H, self.layers)
-            rc = self.rt.cudaMemcpy3D(C.byref(p))
-        assert rc == 0, f"array copy failed ({rc})"
-
-    def fill(self, img):
-        self._copy(np.ascontiguousarray(img.reshape(self.layers, self.H, self.W), dtype=self.dtype), True)
-
-    def read(self):
-        out = np.empty((self.layers, self.H, self.W), self.dtype)
-        self._copy(out, False)
-        return out
-
-    def free(self):
-        if self.handle:
-            assert self.rt.cudaFreeArray(C.c_void_p(self.handle)) == 0
-            self.handle = None
 
 
 def _pointer_frame(torch, ao, depth, linear=False):
@@ -119,10 +24,9 @@ def _stacked_buffers(ao, ids):
 
 
 def _depth_for(kind, W, H, L, seed=0, reversed_z=True):
-    raw = _frames(W, H, L, seed=seed, reversed_z=reversed_z)
+    raw = harness.frames(W, H, L, seed=seed, reversed_z=reversed_z)
     if kind == "d16":
-        codes = np.clip(np.rint(raw.astype(np.float64) * 65535), 0, 65535).astype(np.uint32)
-        return codes.astype(np.uint16), (codes.astype(np.float32) * np.float32(1.0 / 65535)).astype(np.float32)
+        return harness.ingest(raw, "d16")
     if kind == "linear_f32":
         from miniengineao_b200 import synth
         lin = np.stack([synth.random_depth(W, H, seed=seed + i) for i in range(L)]).astype(np.float32)
@@ -136,11 +40,10 @@ def _render_and_compare(torch, rt, W, H, L=1, *, kind="raw_f32", depth_shape=Non
     ao_shape = ao_shape or depth_shape
     rz = kw.get("reversed_z", True)
     depth, as_float = _depth_for(kind, W, H, L, seed=seed, reversed_z=rz)
-    ao = _ctx(W, H, L, **kw)
+    ao = harness.context(W, H, device=0, layers=L, **kw)
     linear = kind == "linear_f32"
     ptr = _pointer_frame(torch, ao, depth, linear=linear)
-    mask = kw.get("high_quality_mask", 0)
-    ids = [1, 2, 3, 4, 5, 10, 17] if kw.get("single_scale") else list(range(1, 18)) + [17 + k for k in range(1, 5) if (mask >> (k - 1)) & 1]
+    ids = harness.buffer_ids(kw.get("high_quality_mask", 0), kw.get("single_scale", False))
     ptr_bufs = _stacked_buffers(ao, ids) if buffers else None
     da = Array(rt, W, H, depth.dtype, depth_shape, L)
     aa = Array(rt, W, H, np.uint8, ao_shape, L)
@@ -161,7 +64,9 @@ def _render_and_compare(torch, rt, W, H, L=1, *, kind="raw_f32", depth_shape=Non
         if oracle:
             for l in range(L):
                 okw = {k: v for k, v in kw.items() if k != "stereo"}
-                ref = _oracle(W, H, stereo=kw.get("stereo", False), linear=linear, ao=ao, **okw).run(as_float[l])
+                if kw.get("stereo"):
+                    okw["tan_half_fov_h_"] = 1.0 / ao.camera.projection00
+                ref = harness.oracle(W, H, stereo=kw.get("stereo", False), linear=linear, threads=8, **okw).run(as_float[l])
                 assert np.array_equal(got[l], ref), f"{W}x{H} {kind} {kw}: layer {l} differs from the oracle"
     finally:
         ao.release_array(da.handle)
@@ -205,14 +110,14 @@ def test_mixed_shapes_and_normalised_formats(torch_cuda, rt):
     _render_and_compare(torch_cuda, rt, 65, 33, 1, depth_shape="2d", ao_shape="layered", buffers=False)
     W, H = 90, 50
     depth, as_float = _depth_for("d16", W, H, 1, seed=4)
-    ao = _ctx(W, H, 1)
+    ao = harness.context(W, H, device=0, layers=1)
     da = Array(rt, W, H, np.uint16, kind=KIND_UNORM16)
     aa = Array(rt, W, H, np.uint8, kind=KIND_UNORM8)
     try:
         da.fill(depth)
         ao.render_arrays(da.handle, aa.handle, kind="d16")
         torch_cuda.cuda.synchronize()
-        assert np.array_equal(aa.read()[0], _oracle(W, H).run(as_float[0]))
+        assert np.array_equal(aa.read()[0], harness.oracle(W, H, threads=8).run(as_float[0]))
     finally:
         ao.release_array(da.handle); ao.release_array(aa.handle)
         da.free(); aa.free()
@@ -220,7 +125,7 @@ def test_mixed_shapes_and_normalised_formats(torch_cuda, rt):
 
 def _replay_check(torch, rt, stream=None):
     W, H, L = 400, 240, 2
-    ao = _ctx(W, H, L)
+    ao = harness.context(W, H, device=0, layers=L)
     pairs = []
     for i in range(2):
         da, aa = Array(rt, W, H, np.float32, "layered", L), Array(rt, W, H, np.uint8, "layered", L)
@@ -231,8 +136,8 @@ def _replay_check(torch, rt, stream=None):
     try:
         for f in range(3):
             for i, (da, aa) in enumerate(pairs):
-                depth = _frames(W, H, L, seed=30 + 2 * f + i)
-                refs = [_oracle(W, H).run(depth[l]) for l in range(L)]
+                depth = harness.frames(W, H, L, seed=30 + 2 * f + i)
+                refs = [harness.oracle(W, H, threads=8).run(depth[l]) for l in range(L)]
                 da.fill(depth)
                 before = ao.launch_count
                 ao.render_arrays(da.handle, aa.handle, stream=stream)
@@ -265,16 +170,16 @@ def test_replay_on_a_non_default_stream(torch_cuda, rt):
 def test_release_then_free_and_reallocate(torch_cuda, rt):
     """After meao_release_array an array may be freed; a new one of the same shape (possibly the same handle) renders correctly."""
     W, H = 256, 144
-    ao = _ctx(W, H, 1)
+    ao = harness.context(W, H, device=0, layers=1)
     for round_ in range(3):
-        depth = _frames(W, H, 1, seed=50 + round_)
+        depth = harness.frames(W, H, 1, seed=50 + round_)
         da, aa = Array(rt, W, H, np.float32), Array(rt, W, H, np.uint8)
         try:
             da.fill(depth)
             ao.render_arrays(da.handle, aa.handle)
             ao.render_arrays(da.handle, aa.handle)          # replay
             torch_cuda.cuda.synchronize()
-            assert np.array_equal(aa.read()[0], _oracle(W, H).run(depth[0])), round_
+            assert np.array_equal(aa.read()[0], harness.oracle(W, H, threads=8).run(depth[0])), round_
         finally:
             ao.release_array(da.handle)
             ao.release_array(aa.handle)
@@ -285,10 +190,10 @@ def test_release_then_free_and_reallocate(torch_cuda, rt):
 def test_event_path_and_debug_buffer(torch_cuda, rt):
     from miniengineao_b200 import _native as N
     W, H = 300, 170
-    ao = _ctx(W, H, 1)
+    ao = harness.context(W, H, device=0, layers=1)
     ao.LateUpdate()
-    depth = _frames(W, H, 1, seed=60)
-    ref = _oracle(W, H).run(depth[0])
+    depth = harness.frames(W, H, 1, seed=60)
+    ref = harness.oracle(W, H, threads=8).run(depth[0])
     da, aa = Array(rt, W, H, np.float32), Array(rt, W, H, np.uint8)
     lib, ctx = N.lib(), ao._ctx
     try:
@@ -318,7 +223,7 @@ def test_event_path_and_debug_buffer(torch_cuda, rt):
 def test_refusals_launch_nothing(torch_cuda, rt):
     from miniengineao_b200 import _native as N
     W, H = 160, 96
-    ao = _ctx(W, H, 1)
+    ao = harness.context(W, H, device=0, layers=1)
     ao.LateUpdate()
     lib, ctx = N.lib(), ao._ctx
     made = []
@@ -329,7 +234,7 @@ def test_refusals_launch_nothing(torch_cuda, rt):
         return x
 
     good_d, good_o = arr(W, H, np.float32), arr(W, H, np.uint8)
-    depth = _frames(W, H, 1, seed=70)
+    depth = harness.frames(W, H, 1, seed=70)
     good_d.fill(depth)
     cases = [
         ("extent", arr(W + 1, H, np.float32), good_o, 0, N.MEAO_ERR_INVALID, b"extent"),
@@ -353,7 +258,7 @@ def test_refusals_launch_nothing(torch_cuda, rt):
             rc = lib.meao_bind_event_arrays(ctx, 5, C.c_void_p(d.handle if d else None), kind, C.c_void_p(o.handle if o else None), None)
             assert rc == want, (tag, "bind", rc)
         # a square context: a cube map needs 6 layers, a cube-map array is refused as such
-        sq = _ctx(64, 64, 6)
+        sq = harness.context(64, 64, device=0, layers=6)
         sq.LateUpdate()
         cube_d, cube_o = arr(64, 64, np.float32, "cube"), arr(64, 64, np.uint8, "cube")
         cube_arr = arr(64, 64, np.float32, "cube", extra_flags=LAYERED, layers=6)
@@ -376,7 +281,7 @@ def test_refusals_launch_nothing(torch_cuda, rt):
         # the context still renders correctly
         ao.render_arrays(good_d.handle, good_o.handle)
         torch_cuda.cuda.synchronize()
-        assert np.array_equal(good_o.read()[0], _oracle(W, H).run(depth[0]))
+        assert np.array_equal(good_o.read()[0], harness.oracle(W, H, threads=8).run(depth[0]))
         sq.release_array(cube_d.handle); sq.release_array(cube_o.handle); sq.release_array(cube_arr.handle)
     finally:
         for x in made:

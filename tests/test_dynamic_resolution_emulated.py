@@ -7,10 +7,9 @@ and layered frames, with and without the fused final level, and for the premin a
 import numpy as np
 import pytest
 
+import harness
 import hostile_cases as HC
 from emu.emu import Frame, lib  # noqa: E402  (tests/ is on sys.path via conftest)
-from oracle.oracle import Oracle
-from test_layers_emulated import _compare_layer, _plan, _raw, contrasting_layers
 
 MAX = (330, 190)
 SIZES = [(1, 1), (33, 17), (97, 61), (329, 189), (257, 131), (64, 32)]
@@ -19,7 +18,7 @@ SIZES = [(1, 1), (33, 17), (97, 61), (329, 189), (257, 131), (64, 32)]
 def test_layout_is_the_librarys():
     """The arena the driver allocates is the one meao_reserve reports for the same reservation and layer count."""
     for L in (1, 3):
-        p = _plan(64, 32, L)
+        p = harness.context(64, 32, layers=L)
         p.maxResolution = MAX
         p.LateUpdate()
         f = Frame(p, max_size=MAX)
@@ -44,19 +43,19 @@ CASES = {
 def test_smaller_frames_in_a_stale_arena_match_the_oracle(case, stale):
     kw = dict(CASES[case])
     L, fused = kw.pop("layers"), kw.pop("fused")
-    f = Frame(_plan(*MAX, L, intensity=1.1, **kw), max_size=MAX)
+    f = Frame(harness.context(*MAX, layers=L, intensity=1.1, **kw), max_size=MAX)
     run = f.run_fused if fused else f.run
     if stale == "max_frame":
         run(np.stack([HC.hostile_raw(*MAX, f.zb, True, seed=l) for l in range(L)]).astype(np.float32))
     else:
         f.fill()
-    ids = [1, 2, 3, 4, 5, 10, 17] if kw.get("single_scale") else None
+    ids = harness.buffer_ids(kw.get("high_quality_mask", 0), kw.get("single_scale", False))
     for i, (W, H) in enumerate(SIZES):
-        f.load(_plan(W, H, L, intensity=1.1, **kw))
-        depth = _raw(contrasting_layers(W, H, L, seed=i)).astype(np.float32)
+        f.load(harness.context(W, H, layers=L, intensity=1.1, **kw))
+        depth = harness.raw(harness.contrasting_layers(W, H, L, seed=i)).astype(np.float32)
         run(depth)
         for l in range(L):
-            orc = Oracle(W, H, threads=4, intensity=1.1, **kw)
+            orc = harness.oracle(W, H, intensity=1.1, **kw)
             ref = orc.run(depth[l])
             assert np.array_equal(f.buffer(17, l), ref), (case, stale, W, H, l)
-            _compare_layer(f, l, orc, f"{case} {stale} {W}x{H}", kw.get("high_quality_mask", 0), ids)
+            harness.compare_buffers(lambda bid: f.buffer(bid, l), orc, f"{case} {stale} {W}x{H} layer {l}", ids)

@@ -9,6 +9,8 @@ import pytest
 from miniengineao_b200 import AmbientOcclusion, Camera
 from miniengineao_b200 import _native as N
 
+import harness
+
 MAX = (3840, 2160)
 # ragged sizes: 1x1, odd, not multiples of 4 / 16 / 64, the reservation itself, and more distinct sizes than the context keeps planned
 SCHEDULE = [(3840, 2160), (3456, 1944), (2881, 1621), (1, 1), (17, 9), (1920, 1080), (3840, 2160), (2881, 1621), (63, 15), (1, 2160),
@@ -32,29 +34,6 @@ def _new(layers=1, cams=None, variants=None, params=None):
         arr = (N.MeaoCamera * len(cams))(*[N.MeaoCamera(*c) for c in cams])
         assert lib.meao_set_layer_cameras(h, arr, len(cams)) >= 0
     return h
-
-
-def _constants(h, layers):
-    """Every constant getter of the plan, as one byte string."""
-    lib = N.lib()
-    parts = []
-    for k in range(1, 5):
-        for getter, n in ((lib.meao_render_constants, 28), (lib.meao_render_constants_wide, 28), (lib.meao_upsample_constants, 8)):
-            out = (C.c_float * n)()
-            assert getter(h, k, out) == 0
-            parts.append(bytes(out))
-        for l in range(layers):
-            for wide in (0, 1):
-                out = (C.c_float * 28)()
-                assert lib.meao_render_constants_layer(h, l, k, wide, out) == 0
-                parts.append(bytes(out))
-    out = (C.c_float * 4)()
-    assert lib.meao_zbuffer_params(h, out) == 0
-    parts.append(bytes(out))
-    for l in range(layers):
-        assert lib.meao_zbuffer_params_layer(h, l, out) == 0
-        parts.append(bytes(out))
-    return b"".join(parts)
 
 
 def _reservation(h):
@@ -84,7 +63,7 @@ def test_constants_after_resizes_match_a_fresh_context(setup):
             f = _new(**kw)
             try:
                 assert lib.meao_resize(f, w, hh) == 1
-                assert _constants(h, kw["layers"]) == _constants(f, kw["layers"]), (w, hh)
+                assert harness.plan_constants(h, kw["layers"]) == harness.plan_constants(f, kw["layers"]), (w, hh)
             finally:
                 lib.meao_destroy(f)
     finally:
@@ -98,7 +77,7 @@ def test_param_change_between_resizes_replans_every_size():
     assert lib.meao_reserve(h, *MAX) == 1
     for w, hh in SCHEDULE[:6]:
         assert lib.meao_resize(h, w, hh) == 1
-        _constants(h, 3)
+        harness.plan_constants(h, 3)
     p = N.MeaoParams()
     lib.meao_default_params(C.byref(p))
     p.intensity, p.blur_tolerance = 1.7, -3.0
@@ -109,7 +88,7 @@ def test_param_change_between_resizes_replans_every_size():
         lib.meao_resize(h, w, hh)
         f = _new(layers=3, cams=list(reversed(CAMS3)), params=dict(intensity=1.7, blur_tolerance=-3.0))
         assert lib.meao_resize(f, w, hh) == 1
-        assert _constants(h, 3) == _constants(f, 3), (w, hh)
+        assert harness.plan_constants(h, 3) == harness.plan_constants(f, 3), (w, hh)
         lib.meao_destroy(f)
     lib.meao_destroy(h)
 
@@ -174,10 +153,10 @@ def test_refusals_change_nothing():
     h = _new(layers=2, cams=CAMS3[:2])
     assert lib.meao_reserve(h, 1920, 1080) == 1
     assert lib.meao_resize(h, 1001, 601) == 1
-    before = (_size(h), _constants(h, 2), bytes(_reservation(h)))
+    before = (_size(h), harness.plan_constants(h, 2), bytes(_reservation(h)))
 
     def unchanged():
-        assert (_size(h), _constants(h, 2), bytes(_reservation(h))) == before
+        assert (_size(h), harness.plan_constants(h, 2), bytes(_reservation(h))) == before
 
     for w, hh in ((1921, 1080), (1920, 1081), (4000, 3000)):
         assert lib.meao_resize(h, w, hh) == N.MEAO_ERR_INVALID

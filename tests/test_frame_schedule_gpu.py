@@ -4,26 +4,13 @@ counts exactly the launches its capture recorded."""
 import numpy as np
 import pytest
 
+import harness
+from gpu_harness import torch_cuda  # noqa: F401  (the fixture)
+
 pytestmark = pytest.mark.gpu
 
 VARIANTS = [dict(), dict(high_quality_mask=15), dict(single_scale=True)]
 IDS = ["default", "hq15", "single_scale"]
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("GPU tests need a GPU")
-    return torch
-
-
-def _ctx(W, H, *, use_graph=True, high_quality_mask=0, single_scale=False):
-    from miniengineao_b200 import AmbientOcclusion, Camera
-    ao = AmbientOcclusion(Camera(W, H), device=0, use_graph=use_graph)
-    ao.highQualityMask, ao.singleScale, ao.intensity = high_quality_mask, single_scale, 1.1
-    ao.LateUpdate()
-    return ao
 
 
 def _depth(torch, W, H):
@@ -31,20 +18,16 @@ def _depth(torch, W, H):
     return torch.from_numpy(synth.lin01_to_raw(synth.random_depth(W, H, seed=7))).cuda()
 
 
-def _oracle(W, H, depth, **kw):
-    from oracle.oracle import Oracle
-    return Oracle(W, H, threads=8, intensity=1.1, **kw).run(depth.cpu().numpy())
-
-
 @pytest.mark.parametrize("kw", VARIANTS, ids=IDS)
 def test_every_frame_form_launches_kernels_per_frame(torch_cuda, kw):
     torch = torch_cuda
     W, H = 320, 184
     d = _depth(torch, W, H)
-    ref = _oracle(W, H, d, **kw)
+    ref = harness.oracle(W, H, threads=8, intensity=1.1, **kw).run(d.cpu().numpy())
     kpf = 3 if kw.get("single_scale") else 9 + bin(kw.get("high_quality_mask", 0)).count("1")
     for use_graph in (True, False):
-        ao = _ctx(W, H, use_graph=use_graph, **kw)
+        ao = harness.context(W, H, device=0, use_graph=use_graph, intensity=1.1, **kw)
+        ao.LateUpdate()
         assert ao.kernels_per_frame == kpf
         out = torch.zeros((H, W), dtype=torch.uint8, device="cuda")
         for _ in range(2):                                  # with a graph: the capture, then a replay
@@ -68,8 +51,9 @@ def test_band_phases_count_the_launches_they_captured(torch_cuda):
     torch = torch_cuda
     W, H = 320, 184
     d = _depth(torch, W, H)
-    ref = _oracle(W, H, d)
-    ao = _ctx(W, H)
+    ref = harness.oracle(W, H, threads=8, intensity=1.1).run(d.cpu().numpy())
+    ao = harness.context(W, H, device=0, intensity=1.1)
+    ao.LateUpdate()
     assert ao.halo_bytes(0) == 0 and ao.halo_recv_bytes(0) == 0
     spare = torch.zeros(16, dtype=torch.uint8, device="cuda")
     out = torch.zeros((H, W), dtype=torch.uint8, device="cuda")

@@ -7,17 +7,10 @@ meao_band_step (the fused form on a row band) is checked against the oracle by t
 import numpy as np
 import pytest
 
-from test_parity_gpu import _compare_all, _mk
+import harness
+from gpu_harness import torch_cuda  # noqa: F401  (the fixture)
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("GPU tests need a GPU")
-    return torch
 
 
 def _depth(kind, W, H, seed, reversed_z=True):
@@ -29,15 +22,12 @@ def _depth(kind, W, H, seed, reversed_z=True):
     raw = raw.astype(np.float32)
     sky = np.float32(0.0 if reversed_z else 1.0)
     raw[: max(1, H // 7), : max(1, W // 5)] = sky
+    words, as_float = harness.ingest(raw, kind, stencil=0x5A)
     if kind in ("f32", "linear"):
         return torch.from_numpy(raw).cuda(), raw
-    bits = 16 if kind == "d16" else 24
-    full = (1 << bits) - 1
-    codes = np.clip(np.rint(raw.astype(np.float64) * full), 0, full).astype(np.uint32)
-    as_float = (codes.astype(np.float32) * np.float32(1.0 / full)).astype(np.float32)
-    if bits == 16:
-        return torch.from_numpy(codes.astype(np.uint16).view(np.int16)).cuda().view(torch.uint16), as_float
-    return torch.from_numpy((codes | (np.uint32(0x5A) << np.uint32(24))).view(np.int32)).cuda(), as_float
+    if kind == "d16":
+        return torch.from_numpy(words.view(np.int16)).cuda().view(torch.uint16), as_float
+    return torch.from_numpy(words.view(np.int32)).cuda(), as_float
 
 
 SIZES = [(1, 1), (3, 5), (161, 93), (250, 131), (37, 1000), (644, 362), (1920, 1080)]
@@ -47,44 +37,37 @@ SIZES = [(1, 1), (3, 5), (161, 93), (250, 131), (37, 1000), (644, 362), (1920, 1
 @pytest.mark.parametrize("W,H", SIZES)
 def test_fused_frame_matches_oracle(torch_cuda, kind, W, H):
     reversed_z = (W + H) % 2 == 0
-    ao, orc = _mk(W, H, intensity=1.1, reversed_z=reversed_z)
+    ao, orc = harness.context_and_oracle(W, H, intensity=1.1, reversed_z=reversed_z)
     d, seen = _depth(kind, W, H, seed=W * 3 + H, reversed_z=reversed_z)
-    from oracle.oracle import Oracle
     if kind == "linear":
-        orc = Oracle(W, H, threads=8, intensity=1.1, reversed_z=reversed_z, depth_is_linear=True)
+        orc = harness.oracle(W, H, threads=8, intensity=1.1, reversed_z=reversed_z, linear=True)
     ref = orc.run(seen)
     got = ao.render(d, linear=(kind == "linear")).cpu().numpy()
     assert np.array_equal(got, ref)
-    _compare_all(ao, orc, f"{kind} {W}x{H}")
+    harness.compare_buffers(ao.debug_buffer, orc, f"{kind} {W}x{H}", harness.buffer_ids())
 
 
 @pytest.mark.parametrize("variant", [dict(high_quality_mask=15), dict(high_quality_mask=1), dict(single_scale=True)])
 @pytest.mark.parametrize("W,H", [(250, 131), (1283, 721)])
 def test_fused_variants_match_oracle(torch_cuda, variant, W, H):
-    from oracle.oracle import Oracle
-    ao, orc = _mk(W, H, intensity=1.1, **{k: v for k, v in variant.items() if k != "single_scale"})
+    ao, orc = harness.context_and_oracle(W, H, intensity=1.1, **{k: v for k, v in variant.items() if k != "single_scale"})
     if variant.get("single_scale"):
         ao.singleScale = True
-        orc = Oracle(W, H, threads=8, intensity=1.1, single_scale=True)
+        orc = harness.oracle(W, H, threads=8, intensity=1.1, single_scale=True)
     d, seen = _depth("f32", W, H, seed=5)
     ref = orc.run(seen)
     assert np.array_equal(ao.render(d).cpu().numpy(), ref)
-    extra = [17 + k for k in range(1, 5) if (variant.get("high_quality_mask", 0) >> (k - 1)) & 1]
     if not variant.get("single_scale"):
-        _compare_all(ao, orc, str(variant), extra=extra)
+        harness.compare_buffers(ao.debug_buffer, orc, str(variant), harness.buffer_ids(variant.get("high_quality_mask", 0)))
 
 
 def test_fused_4k_matches_oracle(torch_cuda):
     from miniengineao_b200 import synth
-    from oracle.oracle import Oracle
     W, H = 3840, 2160
     depth = synth.lin01_to_raw(synth.corridor(W, H))
-    from miniengineao_b200 import AmbientOcclusion, Camera
-    ao = AmbientOcclusion(Camera(W, H), device=0)
-    ao.intensity = 1.1
-    ao.highQualityMask = 15
+    ao = harness.context(W, H, device=0, intensity=1.1, high_quality_mask=15)
     got = ao.render(torch_cuda.from_numpy(depth).cuda()).cpu().numpy()
-    ref = Oracle(W, H, threads=16, intensity=1.1, high_quality_mask=15).run(depth)
+    ref = harness.oracle(W, H, threads=16, intensity=1.1, high_quality_mask=15).run(depth)
     assert np.array_equal(got, ref)
 
 
@@ -92,7 +75,7 @@ def test_linear_depth_is_written_by_every_frame(torch_cuda):
     """LinearDepth poisoned with NaN before a frame: after it, every element equals the oracle's (the low-only prepare_depth does not
     write it; the fused final upsample writes each pixel once, partial rows included)."""
     W, H = 331, 187
-    ao, orc = _mk(W, H, intensity=1.1)
+    ao, orc = harness.context_and_oracle(W, H, intensity=1.1)
     d, seen = _depth("f32", W, H, seed=11)
     ref = orc.run(seen)
     ao.render(d)
@@ -108,7 +91,7 @@ def test_linear_depth_is_written_by_every_frame(torch_cuda):
 def test_host_batch_matches_oracle(torch_cuda):
     """meao_render_host_async: the staged depth is now read by the last kernel of the frame too."""
     W, H = 500, 284
-    ao, orc = _mk(W, H, intensity=1.1)
+    ao, orc = harness.context_and_oracle(W, H, intensity=1.1)
     ds = [_depth("f32", W, H, seed=40 + i)[1] for i in range(4)]
     outs = [np.zeros((H, W), np.uint8) for _ in ds]
     ao.render_host_batch(ds, outs)

@@ -10,52 +10,33 @@ except that two NaNs match.  Also here: the second restatement of the oracle (or
 import numpy as np
 import pytest
 
-from miniengineao_b200 import AmbientOcclusion, Camera
+from miniengineao_b200 import Camera
 from oracle import direct_formulation as DF
 from oracle.oracle import Oracle
 
+import harness
 import hostile_cases as HC
 from emu.emu import Frame
-from test_fused_lin_emulated import fused_frame
-from test_pitched_emulated import SENTINEL, View
+from harness import SENTINEL, View, fused_frame
 
-PARAMS = {"noise_filter_tolerance": "noiseFilterTolerance", "blur_tolerance": "blurTolerance", "upsample_tolerance": "upsampleTolerance",
-          "thickness_modifier": "thicknessModifier", "intensity": "intensity"}
 W0, H0 = 203, 97            # ragged: no level is a multiple of 4, 16 or 64, W % 8 == 3
-
-
-def _plan(cam, layers=1, *, high_quality_mask=0, sample_exhaustively=False, single_scale=False, layer_cameras=None, **params):
-    p = AmbientOcclusion(cam, device=-1)
-    for py, cs in PARAMS.items():
-        if py in params:
-            setattr(p, cs, params[py])
-    p.highQualityMask, p.sampleExhaustively, p.singleScale, p.layers = high_quality_mask, sample_exhaustively, single_scale, layers
-    p.layerCameras = layer_cameras
-    return p
-
-
-def _oracle(W, H, cam, *, linear=False, stereo=False, **kw):
-    okw = HC.oracle_camera_kw(cam)
-    if stereo:
-        okw["single_pass_stereo"] = True
-    return Oracle(W, H, threads=4, depth_is_linear=linear, **okw, **kw)
 
 
 def _check(get, W, H, cam, seen, tag, *, linear=False, high_quality_mask=0, single_scale=False, stereo=False, **kw):
     """get(bid) -> the kernel's buffer of this layer; seen: the float32 depth the oracle reads."""
-    orc = _oracle(W, H, cam, linear=linear, stereo=stereo, high_quality_mask=high_quality_mask, single_scale=single_scale, **kw)
+    orc = harness.oracle(W, H, camera=cam, linear=linear, stereo=stereo, high_quality_mask=high_quality_mask, single_scale=single_scale, **kw)
     orc.run(seen)
-    HC.compare_buffers(get, orc, tag, HC.buffer_ids(high_quality_mask, single_scale))
+    harness.compare_buffers(get, orc, tag, harness.buffer_ids(high_quality_mask, single_scale), nan_equal=True)
 
 
 def _whole(cam, depth, seen, tag, *, linear=False, use_tma=True, **kw):
-    f = Frame(_plan(cam, **kw), linear=linear, use_tma=use_tma)
+    f = Frame(harness.context(cam, **kw), linear=linear, use_tma=use_tma)
     f.run(depth)
     _check(f.buffer, cam.pixelWidth, cam.pixelHeight, cam, seen, tag, linear=linear, **kw)
 
 
 def _zb(cam):
-    return _plan(cam).zbuffer_params()
+    return harness.context(cam).zbuffer_params()
 
 
 # ---- depth values through the whole frame ---------------------------------------------------------------------------------------
@@ -104,7 +85,7 @@ def test_fused_frame_hostile(kind):
         depth = seen = HC.hostile_raw(W0, H0, _zb(cam), rz, seed=7)
     else:
         depth, seen = HC.hostile_unorm(W0, H0, 16 if kind == "d16" else 24, rz, seed=7)
-    f = fused_frame(_plan(cam), linear=kind == "linear")
+    f = fused_frame(harness.context(cam), linear=kind == "linear")
     f.run_fused(depth)
     _check(f.buffer, W0, H0, cam, seen, f"fused {kind}", linear=kind == "linear")
 
@@ -125,7 +106,7 @@ def test_extreme_camera_as_one_layer_of_a_batch(name):
     W, H = 136, 72
     cams = [Camera(W, H, nearClipPlane=0.1, farClipPlane=50.0), HC.camera(name, W, H, True), Camera(W, H, nearClipPlane=1.0, farClipPlane=1000.0)]
     depth = np.stack([HC.hostile_raw(W, H, _zb(c), True, seed=20 + l) for l, c in enumerate(cams)])
-    f = Frame(_plan(Camera(W, H), 3, layer_cameras=cams))
+    f = Frame(harness.context(Camera(W, H), layers=3, layer_cameras=cams))
     f.run_fused(depth)
     for l, c in enumerate(cams):
         _check(lambda bid: f.buffer(bid, l), W, H, c, depth[l], f"batch {name} layer {l}")
@@ -133,7 +114,7 @@ def test_extreme_camera_as_one_layer_of_a_batch(name):
 
 # ---- parameters ---------------------------------------------------------------------------------------------------------------
 def test_parameter_table_straddles_the_proven_final_division_range():
-    sides = [HC.fast_div_sides(_plan(Camera(W0, H0), **p)) for p in HC.PARAMS]
+    sides = [HC.fast_div_sides(harness.context(Camera(W0, H0), **p)) for p in HC.PARAMS]
     assert True in set.union(*sides) and False in set.union(*sides)
     by = {tuple(p.items()): s for p, s in zip(HC.PARAMS, sides)}
     assert by[(("upsample_tolerance", -16.55),)] == {True} and by[(("upsample_tolerance", -16.56),)] == {False}
@@ -156,7 +137,7 @@ def test_variants_hostile(kw):
     stereo = kw.pop("stereo", False)
     W, H = 2 * 68 if stereo else W0, H0
     cam = Camera(W // 2 if stereo else W, H, stereoEnabled=stereo)
-    p = _plan(cam, **kw)
+    p = harness.context(cam, **kw)
     if stereo:
         p.OnPreRender()                     # one draw for both eyes
     d = HC.hostile_linear(W, H, seed=17)
@@ -173,7 +154,7 @@ def test_layered_frame_hostile(use_tma):
     d = np.stack([HC.hostile_raw(W, H, _zb(cam), True, seed=30), HC.salt(HC.hostile_raw(W, H, _zb(cam), True, seed=31), HC.LINEAR, 31),
                   HC.hostile_raw(W, H, _zb(cam), True, seed=32)])
     d[2, 16:64, 32:96] = np.nan
-    f = Frame(_plan(cam, 3), use_tma=use_tma)
+    f = Frame(harness.context(cam, layers=3), use_tma=use_tma)
     f.run(d)
     for l in range(3):
         _check(lambda bid: f.buffer(bid, l), W, H, cam, d[l], f"layered layer {l}")
@@ -185,7 +166,7 @@ def test_pitched_view_hostile(linear):
     W, H = W0, H0
     cam = Camera(W, H)
     d = HC.hostile_linear(W, H, seed=40) if linear else HC.hostile_raw(W, H, _zb(cam), True, seed=40)
-    f = fused_frame(_plan(cam), linear=linear)
+    f = fused_frame(harness.context(cam), linear=linear)
     dv = View((1, H, W), np.float32, 1024, 1024 * H)
     dv.arr[...] = d
     av = View((1, H, W), np.uint8, 256, 256 * H, fill=SENTINEL)
@@ -202,7 +183,7 @@ def test_array_frame_hostile(kind):
         depth, seen = HC.hostile_unorm(W, H, 16, True, seed=50)
     else:
         depth = seen = HC.hostile_raw(W, H, _zb(cam), True, seed=50)
-    f = Frame(_plan(cam))
+    f = Frame(harness.context(cam))
     ao = f.run_arrays(depth[None])
     _check(lambda bid: ao[0] if bid == 17 else f.buffer(bid, 0), W, H, cam, seen, f"array {kind}")
 
@@ -223,12 +204,12 @@ def test_direct_formulation_agrees_on_hostile_frames(kind):
     uc = {k: o.upsample_constants(k) for k in range(1, 5)}
     with np.errstate(all="ignore"):
         r = DF.run(d, rc, uc, o.zbuffer_params(), reversed_z=rz, linear=linear, return_all=True)
-        assert HC.n_diff(np.asarray(r["linear"], np.float32).astype(np.float16), o.buffer(1)) == 0, "LinearDepth"
+        assert harness.n_diff(np.asarray(r["linear"], np.float32).astype(np.float16), o.buffer(1), nan_equal=True) == 0, "LinearDepth"
     dims = DF.level_dims(W, H)
     for k in range(1, 5):
-        assert HC.n_diff(np.asarray(r["low"][k], np.float32), o.buffer(1 + k)) == 0, f"LowDepth{k}"
+        assert harness.n_diff(np.asarray(r["low"][k], np.float32), o.buffer(1 + k), nan_equal=True) == 0, f"LowDepth{k}"
         tv = DF.tiled_view(r["low"][k], dims[k + 2][0], dims[k + 2][1], r["pad12"] if k <= 2 else np.float32(0))
-        assert HC.n_diff(np.asarray(tv, np.float32), o.buffer(5 + k)) == 0, f"TiledDepth{k}"
+        assert harness.n_diff(np.asarray(tv, np.float32), o.buffer(5 + k), nan_equal=True) == 0, f"TiledDepth{k}"
         assert np.array_equal(r["occ"][k], o.codes(9 + k)), f"Occlusion{k}"
     for k in range(1, 4):
         assert np.array_equal(r["comb"][k], o.codes(13 + k)), f"Combined{k}"

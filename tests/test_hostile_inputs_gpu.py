@@ -9,49 +9,25 @@ frame.  Every buffer must equal the oracle's: unorm8 codes exactly, f16 / f32 bi
 import numpy as np
 import pytest
 
+import harness
 import hostile_cases as HC
+from gpu_harness import Array, rt, torch_cuda  # noqa: F401  (the fixtures)
 
 pytestmark = pytest.mark.gpu
 
-PARAMS = {"noise_filter_tolerance": "noiseFilterTolerance", "blur_tolerance": "blurTolerance", "upsample_tolerance": "upsampleTolerance",
-          "thickness_modifier": "thicknessModifier", "intensity": "intensity"}
 W0, H0 = 643, 363           # ragged: W % 8 == 3, no level a multiple of 4, 16 or 64
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("GPU tests need a GPU")
-    return torch
-
-
-def _ctx(cam, layers=1, *, high_quality_mask=0, sample_exhaustively=False, single_scale=False, layer_cameras=None, **params):
-    from miniengineao_b200 import AmbientOcclusion
-    ao = AmbientOcclusion(cam, device=0)
-    for py, cs in PARAMS.items():
-        if py in params:
-            setattr(ao, cs, params[py])
-    ao.highQualityMask, ao.sampleExhaustively, ao.singleScale, ao.layers = high_quality_mask, sample_exhaustively, single_scale, layers
-    ao.layerCameras = layer_cameras
-    if cam.stereoEnabled:
-        ao.OnPreRender()                    # one draw for both eyes
-    return ao
 
 
 def _check(ao, cam, seen, tag, *, layer=None, got_ao=None, linear=False, high_quality_mask=0, single_scale=False, **kw):
     """Every buffer of `ao` (layer `layer` of a layered context) against the oracle run on `seen`, the float32 depth it reads."""
-    from oracle.oracle import Oracle
     H, W = seen.shape
-    okw = HC.oracle_camera_kw(cam)
-    if cam.stereoEnabled:
-        okw["single_pass_stereo"] = True
-    orc = Oracle(W, H, threads=8, depth_is_linear=linear, high_quality_mask=high_quality_mask, single_scale=single_scale, **okw, **kw)
+    orc = harness.oracle(W, H, camera=cam, linear=linear, stereo=cam.stereoEnabled, threads=8, high_quality_mask=high_quality_mask,
+                         single_scale=single_scale, **kw)
     ref = orc.run(seen)
     if got_ao is not None:
-        assert HC.n_diff(got_ao, ref) == 0, f"{tag}: AO differs from the oracle"
+        assert harness.n_diff(got_ao, ref, nan_equal=True) == 0, f"{tag}: AO differs from the oracle"
     get = (lambda bid: ao.debug_buffer(bid)) if layer is None else (lambda bid: ao.debug_buffer(bid)[layer])
-    HC.compare_buffers(get, orc, tag, HC.buffer_ids(high_quality_mask, single_scale))
+    harness.compare_buffers(get, orc, tag, harness.buffer_ids(high_quality_mask, single_scale), nan_equal=True)
 
 
 def _render(torch, ao, depth, linear=False):
@@ -59,8 +35,7 @@ def _render(torch, ao, depth, linear=False):
 
 
 def _zb(cam):
-    from miniengineao_b200 import AmbientOcclusion
-    return AmbientOcclusion(cam, device=-1).zbuffer_params()
+    return harness.context(cam).zbuffer_params()
 
 
 def _depth(kind, cam, seed):
@@ -82,7 +57,7 @@ def test_render_hostile(torch_cuda, kind, rz):
     from miniengineao_b200 import Camera
     cam = Camera(W0, H0, usesReversedZBuffer=rz)
     depth, seen, linear = _depth(kind, cam, seed=1)
-    ao = _ctx(cam)
+    ao = harness.context(cam, device=0)
     got = _render(torch_cuda, ao, depth, linear)
     _check(ao, cam, seen, f"render {kind} rz={rz}", got_ao=got, linear=linear)
 
@@ -94,7 +69,7 @@ def test_solid_hostile_linear_frame(torch_cuda, value):
     cam = Camera(W, H)
     d = HC.hostile_linear(W, H, seed=2)
     d[:576, :1088] = value
-    ao = _ctx(cam)
+    ao = harness.context(cam, device=0)
     got = _render(torch_cuda, ao, d, True)
     _check(ao, cam, d, f"solid {value!r}", got_ao=got, linear=True)
 
@@ -103,7 +78,7 @@ def test_render_host_hostile(torch_cuda):
     from miniengineao_b200 import Camera
     cam = Camera(321, 203)
     d = HC.hostile_raw(321, 203, _zb(cam), True, seed=3)
-    ao = _ctx(cam)
+    ao = harness.context(cam, device=0)
     got = ao.render_host(d)
     _check(ao, cam, d, "render_host", got_ao=got)
 
@@ -112,7 +87,7 @@ def test_4k_hostile(torch_cuda):
     from miniengineao_b200 import Camera
     cam = Camera(3840, 2160)
     d = HC.hostile_linear(3840, 2160, seed=4)
-    ao = _ctx(cam)
+    ao = harness.context(cam, device=0)
     got = _render(torch_cuda, ao, d, True)
     _check(ao, cam, d, "4K linear", got_ao=got, linear=True)
 
@@ -126,7 +101,7 @@ def test_pitched_view_hostile(torch_cuda):
     rt = torch.full((H0 + 37, 1024), float("nan"), dtype=torch.float32, device="cuda")
     rt[:H0, :W0] = torch.from_numpy(d).cuda()
     out = torch.full((H0 + 5, 768), 0xA5, dtype=torch.uint8, device="cuda")
-    ao = _ctx(cam)
+    ao = harness.context(cam, device=0)
     ao.render(rt[:H0, :W0], out[:H0, :W0])
     o = out.cpu().numpy()
     assert (o[:, W0:] == 0xA5).all() and (o[H0:] == 0xA5).all(), "a store outside the AO view"
@@ -141,27 +116,20 @@ def test_layered_frame_hostile(torch_cuda):
     d = np.stack([HC.hostile_raw(W0, H0, zb, True, seed=6), HC.salt(HC.hostile_raw(W0, H0, zb, True, seed=7), HC.LINEAR, 7),
                   HC.hostile_raw(W0, H0, zb, True, seed=8)])
     d[2, 64:256, 128:512] = np.nan
-    ao = _ctx(cam, 3)
+    ao = harness.context(cam, device=0, layers=3)
     got = _render(torch_cuda, ao, d)
     for l in range(3):
         _check(ao, cam, d[l], f"layered layer {l}", layer=l, got_ao=got[l])
 
 
 @pytest.mark.parametrize("kind", ["raw_f32", "d16"])
-def test_render_arrays_hostile(torch_cuda, kind):
-    import ctypes as C
+def test_render_arrays_hostile(torch_cuda, rt, kind):
     from miniengineao_b200 import Camera
-    import test_arrays_gpu as TA
-    r = C.CDLL("libcudart.so.12")             # the runtime set-up of test_arrays_gpu's `rt` fixture, for the 2-D arrays
-    r.cudaMallocArray.argtypes = [C.POINTER(C.c_void_p), C.POINTER(TA.ChannelDesc), C.c_size_t, C.c_size_t, C.c_uint]
-    r.cudaFreeArray.argtypes = [C.c_void_p]
-    r.cudaMemcpy2DToArray.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int]
-    r.cudaMemcpy2DFromArray.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int]
     W, H = 321, 203
     cam = Camera(W, H)
     depth, seen, _ = _depth("raw" if kind == "raw_f32" else "d16", cam, seed=9)
-    ao = _ctx(cam)
-    da, aa = TA.Array(r, W, H, depth.dtype), TA.Array(r, W, H, np.uint8)
+    ao = harness.context(cam, device=0)
+    da, aa = Array(rt, W, H, depth.dtype), Array(rt, W, H, np.uint8)
     try:
         da.fill(depth)
         aa.fill(np.full((1, H, W), 0x5A, np.uint8))
@@ -186,25 +154,24 @@ def test_variants_hostile(torch_cuda, kw):
     W, H = (2 * 322, H0) if stereo else (W0, H0)
     cam = Camera(W // 2 if stereo else W, H, stereoEnabled=stereo)
     d = HC.hostile_linear(W, H, seed=10)
-    ao = _ctx(cam, **kw)
+    ao = harness.context(cam, device=0, stereo=cam.stereoEnabled, **kw)
     got = _render(torch_cuda, ao, d, True)
     _check(ao, cam, d, f"{kw} stereo={stereo}", got_ao=got, linear=True, **kw)
 
 
 def test_two_band_row_split_with_hostile_rows_on_the_seam(torch_cuda):
-    from miniengineao_b200 import AmbientOcclusion, Camera
-    from oracle.oracle import Oracle
+    from miniengineao_b200 import Camera
     torch = torch_cuda
     W, H = 1280, 720
     cam = Camera(W, H)
     cut = 16 * (((H + 15) // 16) // 2)
     d = HC.hostile_raw(W, H, _zb(cam), True, seed=11)
     d[cut - 3:cut + 3] = HC.salt(d[cut - 3:cut + 3], HC.raw_values(_zb(cam)), 11)
-    ref = Oracle(W, H, threads=8).run(d)
+    ref = harness.oracle(W, H, threads=8).run(d)
     cuts = [0, cut, H]
     ctxs = []
     for i in range(2):
-        a = AmbientOcclusion(Camera(W, H), device=0)
+        a = harness.context(W, H, device=0)
         a.set_row_band(cuts[i], cuts[i + 1], cuts[i - 1] if i > 0 else -1, cuts[i + 2] if i + 2 <= 2 else -1)
         ctxs.append(a)
     for i, a in enumerate(ctxs):
@@ -223,7 +190,7 @@ def test_two_band_row_split_with_hostile_rows_on_the_seam(torch_cuda):
         a.band_finish(o)
         a.synchronize()
         got[cuts[i]:cuts[i + 1]] = o.cpu().numpy()
-    assert HC.n_diff(got, ref) == 0
+    assert harness.n_diff(got, ref, nan_equal=True) == 0
 
 
 # ---- cameras and parameters -----------------------------------------------------------------------------------------------------
@@ -232,7 +199,7 @@ def test_two_band_row_split_with_hostile_rows_on_the_seam(torch_cuda):
 def test_extreme_camera(torch_cuda, name, rz):
     cam = HC.camera(name, W0, H0, rz)
     d = HC.hostile_raw(W0, H0, _zb(cam), rz, seed=12)
-    ao = _ctx(cam)
+    ao = harness.context(cam, device=0)
     got = _render(torch_cuda, ao, d)
     _check(ao, cam, d, f"camera {name} rz={rz}", got_ao=got)
 
@@ -243,7 +210,7 @@ def test_extreme_camera_as_one_layer_of_a_batch(torch_cuda, name):
     cams = [Camera(W0, H0, nearClipPlane=0.1, farClipPlane=50.0), HC.camera(name, W0, H0, True),
             Camera(W0, H0, nearClipPlane=1.0, farClipPlane=1000.0)]
     d = np.stack([HC.hostile_raw(W0, H0, _zb(c), True, seed=13 + l) for l, c in enumerate(cams)])
-    ao = _ctx(Camera(W0, H0), 3, layer_cameras=cams)
+    ao = harness.context(Camera(W0, H0), device=0, layers=3, layer_cameras=cams)
     got = _render(torch_cuda, ao, d)
     for l, c in enumerate(cams):
         _check(ao, c, d[l], f"batch {name} layer {l}", layer=l, got_ao=got[l])
@@ -254,6 +221,6 @@ def test_extreme_parameters(torch_cuda, params):
     from miniengineao_b200 import Camera
     cam = Camera(W0, H0)
     d = HC.hostile_raw(W0, H0, _zb(cam), True, seed=14)
-    ao = _ctx(cam, **params)
+    ao = harness.context(cam, device=0, **params)
     got = _render(torch_cuda, ao, d)
     _check(ao, cam, d, str(params), got_ao=got, **params)

@@ -11,52 +11,25 @@ The emulator is test infrastructure: libmeao.so never contains it and still has 
 import numpy as np
 import pytest
 
-from miniengineao_b200 import AmbientOcclusion, Camera, synth
+from miniengineao_b200 import synth
 from oracle import oracle as O
-from oracle.oracle import Oracle
 
+import harness
 from emu.emu import Frame, composite, composite_debug  # noqa: E402  (tests/ is on sys.path via conftest)
-
-
-def _plan(W, H, **kw):
-    cam = Camera(W, H, usesReversedZBuffer=kw.get("reversed_z", True))
-    p = AmbientOcclusion(cam, device=-1)
-    for py, cs in (("noise_filter_tolerance", "noiseFilterTolerance"), ("blur_tolerance", "blurTolerance"), ("upsample_tolerance", "upsampleTolerance"),
-                   ("thickness_modifier", "thicknessModifier"), ("intensity", "intensity"), ("sample_exhaustively", "sampleExhaustively"),
-                   ("high_quality_mask", "highQualityMask"), ("single_scale", "singleScale")):
-        if py in kw:
-            setattr(p, cs, kw[py])
-    return p
-
-
-def _compare_all(f, orc, tag, mask=0):
-    bad = []
-    for bid in list(range(1, 18)) + [17 + k for k in range(1, 5) if (mask >> (k - 1)) & 1]:
-        got, ref = f.buffer(bid), orc.buffer(bid)
-        if got.dtype == np.uint8:
-            n = int((got != orc.codes(bid)).sum())
-        elif got.dtype == np.float16:
-            with np.errstate(over="ignore"):
-                n = int((got.view(np.uint16) != ref.astype(np.float16).view(np.uint16)).sum())
-        else:
-            n = int((got.view(np.uint32) != ref.view(np.uint32)).sum())
-        if n:
-            bad.append((bid, n, got.size))
-    assert not bad, f"{tag}: mismatching buffers (id, #diff, size): {bad}"
 
 
 def _run(W, H, seed=1, depth=None, use_tma=True, **kw):
     okw = {k: v for k, v in kw.items()}
-    orc = Oracle(W, H, threads=4, **okw)
+    orc = harness.oracle(W, H, **okw)
     if depth is None:
         depth = synth.lin01_to_raw(synth.random_depth(W, H, seed=seed), reversed_z=kw.get("reversed_z", True))
     ref = orc.run(depth)
-    f = Frame(_plan(W, H, **kw), use_tma=use_tma)
+    f = Frame(harness.context(W, H, **kw), use_tma=use_tma)
     n0 = f.tma_box_loads()
     got = f.run(depth)
     f.tma_loads_in_run = f.tma_box_loads() - n0
     assert int((got != ref).sum()) == 0, (W, H, kw)
-    _compare_all(f, orc, f"{W}x{H} {kw}", kw.get("high_quality_mask", 0))
+    harness.compare_buffers(f.buffer, orc, f"{W}x{H} {kw}", harness.buffer_ids(kw.get("high_quality_mask", 0)))
     return f, orc
 
 
@@ -127,22 +100,20 @@ def test_unaligned_tma_start_is_refused():
 def test_linear_and_native_depth_ingest():
     W, H = 250, 131
     lin = synth.random_depth(W, H, seed=9)
-    orc = Oracle(W, H, depth_is_linear=True)
+    orc = harness.oracle(W, H, linear=True, threads=1)
     ref = orc.run(lin)
-    f = Frame(_plan(W, H), linear=True)
+    f = Frame(harness.context(W, H), linear=True)
     assert np.array_equal(f.run(lin), ref)
-    _compare_all(f, orc, "linear ingest")
-    raw = synth.lin01_to_raw(lin).astype(np.float64)
-    for bits, dt in ((16, np.uint16), (24, np.uint32)):
-        full = (1 << bits) - 1
-        codes = np.clip(np.rint(raw * full), 1, full).astype(np.uint32)
-        as_float = (codes.astype(np.float32) * np.float32(1.0 / full)).astype(np.float32)
-        orc = Oracle(W, H)
+    harness.compare_buffers(f.buffer, orc, "linear ingest", harness.buffer_ids())
+    raw = synth.lin01_to_raw(lin)
+    assert np.rint(raw.astype(np.float64) * 65535).min() >= 1           # no code 0: the frame has no sky
+    for kind in ("d16", "d24s8"):
+        words, as_float = harness.ingest(raw, kind)
+        orc = harness.oracle(W, H, threads=1)
         ref = orc.run(as_float)
-        words = codes.astype(np.uint16) if bits == 16 else (codes | (np.uint32(0xA5) << np.uint32(24)))
-        f = Frame(_plan(W, H))
-        assert np.array_equal(f.run(words.astype(dt)), ref), bits
-        _compare_all(f, orc, f"D{bits}")
+        f = Frame(harness.context(W, H))
+        assert np.array_equal(f.run(words), ref), kind
+        harness.compare_buffers(f.buffer, orc, kind, harness.buffer_ids())
 
 
 def test_debug_views():
@@ -190,12 +161,12 @@ def test_render_tile_height_variants(tile, use_tma):
     W, H = 700, 420
     depth = synth.lin01_to_raw(synth.random_depth(W, H, seed=31))
     depth[100:140, 200:330] = 0.0
-    orc = Oracle(W, H, threads=4, intensity=1.1, high_quality_mask=0b0011)
+    orc = harness.oracle(W, H, intensity=1.1, high_quality_mask=0b0011)
     ref = orc.run(depth)
-    f = Frame(_plan(W, H, intensity=1.1, high_quality_mask=0b0011), use_tma=use_tma, render_tile=tile)
+    f = Frame(harness.context(W, H, intensity=1.1, high_quality_mask=0b0011), use_tma=use_tma, render_tile=tile)
     n0 = f.tma_box_loads()
     assert np.array_equal(f.run(depth), ref)
-    _compare_all(f, orc, f"tile variant {tile}", 0b0011)
+    harness.compare_buffers(f.buffer, orc, f"tile variant {tile}", harness.buffer_ids(0b0011))
     assert (f.tma_box_loads() - n0 > 50) if use_tma else (f.tma_box_loads() == n0)
 
 
@@ -204,9 +175,9 @@ def test_single_scale_plan(W, H):
     """BASELINE.json configs[0]: Downsample -> Render level 1 -> final-style Upsample on Occlusion1 (MeaoVariants.single_scale)."""
     lin = synth.flat_sphere(W, H) if (W, H) == (256, 256) else synth.random_depth(W, H, seed=W)
     depth = synth.lin01_to_raw(lin)
-    orc = Oracle(W, H, threads=4, intensity=1.1, single_scale=True)
+    orc = harness.oracle(W, H, intensity=1.1, single_scale=True)
     ref = orc.run(depth)
-    plan = _plan(W, H, intensity=1.1)
+    plan = harness.context(W, H, intensity=1.1)
     plan.singleScale = True
     f = Frame(plan)
     assert np.array_equal(f.run(depth), ref)
@@ -218,19 +189,6 @@ def test_single_scale_plan(W, H):
     assert plan.kernels_per_frame == 3
 
 
-def _band_frames(W, H, nb, **kw):
-    from miniengineao_b200 import rowtile
-    cuts = rowtile.partition(H, nb)
-    frames = []
-    for i in range(nb):
-        plan = _plan(W, H, **kw)
-        plan.set_row_band(cuts[i], cuts[i + 1], *rowtile.neighbours(cuts, i))
-        f = Frame(plan)
-        f.use_plan_band()
-        frames.append(f)
-    return cuts, frames
-
-
 @pytest.mark.parametrize("W,H,nb,single_scale", [(200, 528, 2, False), (130, 1296, 3, False), (200, 528, 2, True)],
                          ids=["200-528-2", "130-1296-3", "200-528-2-single_scale"])
 def test_native_exchange_kernel_bands_equal_whole_frame(W, H, nb, single_scale):
@@ -240,12 +198,12 @@ def test_native_exchange_kernel_bands_equal_whole_frame(W, H, nb, single_scale):
     that runs first; every later band finds them raised by the kernels that already ran.  single_scale: phase b is render 1 and
     the final-style upsample, as in libmeao's frame schedule."""
     depth = synth.lin01_to_raw(synth.random_depth(W, H, seed=3))
-    okw = dict(threads=4, intensity=1.1, single_scale=single_scale)
-    ref = Oracle(W, H, **okw).run(depth)
+    okw = dict(intensity=1.1, single_scale=single_scale)
+    ref = harness.oracle(W, H, **okw).run(depth)
     for frame_no in (1, 2):                                      # two epochs through the same flags
-        cuts, frames = (_band_frames(W, H, nb, intensity=1.1, single_scale=single_scale)) if frame_no == 1 else (cuts, frames)
+        cuts, frames = (harness.band_frames(W, H, nb, intensity=1.1, single_scale=single_scale)) if frame_no == 1 else (cuts, frames)
         d = depth if frame_no == 1 else depth[:, ::-1].copy()
-        want = ref if frame_no == 1 else Oracle(W, H, **okw).run(d)
+        want = ref if frame_no == 1 else harness.oracle(W, H, **okw).run(d)
         for i, f in enumerate(frames):
             if frame_no == 2:
                 f.poison_low()
@@ -270,7 +228,7 @@ def test_native_exchange_kernel_bands_equal_whole_frame(W, H, nb, single_scale):
 def test_native_exchange_times_out_instead_of_hanging():
     """A neighbour that never arrives: the kernel gives up after the time-out, sets the sticky error (1 = no ack, 2 = no rows),
     mirrors it to the host word, and later exchanges return immediately."""
-    cuts, frames = _band_frames(200, 528, 2, intensity=1.1)
+    cuts, frames = harness.band_frames(200, 528, 2, intensity=1.1)
     depth = synth.lin01_to_raw(synth.random_depth(200, 528, seed=3))
     a, b = frames
     a.band_phase_a(depth[cuts[0]:cuts[1]])
@@ -301,9 +259,9 @@ def test_persistent_tile_loop_forced_on_every_level(use_tma, monkeypatch):
     W, H = 640, 360
     depth = synth.lin01_to_raw(synth.corridor(W, H))
     depth[100:130, 200:300] = 0.0                                   # sky: the out-of-line IEEE path inside the loop
-    orc = Oracle(W, H, threads=4, intensity=1.1, high_quality_mask=0b0101)
+    orc = harness.oracle(W, H, intensity=1.1, high_quality_mask=0b0101)
     ref = orc.run(depth)
-    f = Frame(_plan(W, H, intensity=1.1, high_quality_mask=0b0101), use_tma=use_tma)
+    f = Frame(harness.context(W, H, intensity=1.1, high_quality_mask=0b0101), use_tma=use_tma)
     for frame in range(2):
         assert np.array_equal(f.run(depth), ref), frame
-    _compare_all(f, orc, "tile loop", 0b0101)
+    harness.compare_buffers(f.buffer, orc, "tile loop", harness.buffer_ids(0b0101))

@@ -10,13 +10,11 @@ import pytest
 
 from miniengineao_b200 import synth
 from oracle import oracle as O
-from oracle.oracle import Oracle
 
+import harness
 import kernel_matrix as km  # noqa: E402  (tests/ is on sys.path via conftest)
 from emu import emu  # noqa: E402
 from emu.emu import Frame, composite, composite_debug  # noqa: E402
-from test_kernel_logic_emulated import _band_frames  # noqa: E402
-from test_layers_emulated import _compare_layer, _plan  # noqa: E402
 
 
 def _ran(expected: set, tag: str) -> dict:
@@ -28,7 +26,7 @@ def _ran(expected: set, tag: str) -> dict:
 def _frame_case(c: km.Case) -> None:
     W, H = c.size
     depth, seen = km.depth(c)
-    plan = _plan(W, H, c.layers, single_scale=c.single_scale, reversed_z=c.reversed_z, intensity=1.1, high_quality_mask=c.hq,
+    plan = harness.context(W, H, layers=c.layers, single_scale=c.single_scale, reversed_z=c.reversed_z, intensity=1.1, high_quality_mask=c.hq,
                  sample_exhaustively=c.exhaustive)
     f = Frame(plan, linear=c.kind == "linear", render_tile=c.tile)
     ao = None
@@ -44,11 +42,11 @@ def _frame_case(c: km.Case) -> None:
         untouched = [k for k, (_, tma) in ledger.items() if k.startswith(("render_ao", "blur_upsample")) and tma == 0]
         assert not untouched, f"{c.id}: no TMA box loads in {untouched}"
     for l in range(c.layers):
-        orc = Oracle(W, H, threads=4, **c.oracle_kw())
+        orc = harness.oracle(W, H, **c.oracle_kw())
         ref = orc.run(seen[l])
         if ao is not None:
             assert np.array_equal(ao[l], ref), f"{c.id}: the AO array of layer {l} differs from the oracle"
-        _compare_layer(f, l, orc, c.id, c.hq, c.buffer_ids())
+        harness.compare_buffers(lambda bid: f.buffer(bid, l), orc, f"{c.id} layer {l}", c.buffer_ids())
 
 
 def _composite(c: km.Case) -> None:
@@ -78,9 +76,9 @@ def _debug_view(c: km.Case) -> None:
     itself (synth_tiled_kernel), after a frame."""
     W, H = c.size
     depth, seen = km.depth(c)
-    f = Frame(_plan(W, H, intensity=1.1))
+    f = Frame(harness.context(W, H, intensity=1.1))
     f.run(depth)
-    orc = Oracle(W, H, threads=4, **c.oracle_kw())
+    orc = harness.oracle(W, H, **c.oracle_kw())
     orc.run(seen[0])
     emu.ledger_reset()
     plain, tiled, atlas = f.debug_view(11), f.debug_view(7), f.buffer(7)
@@ -98,14 +96,14 @@ def _halo(c: km.Case) -> None:
     its rows of the whole-frame oracle."""
     W, H = 200, 528
     depth = _band_depth(W, H)
-    cuts, (a, b) = _band_frames(W, H, 2, intensity=1.1)
+    cuts, (a, b) = harness.band_frames(W, H, 2, intensity=1.1)
     a.band_phase_a(depth[cuts[0]:cuts[1]])
     b.band_phase_a(depth[cuts[1]:cuts[2]])
     emu.ledger_reset()
     b.halo_unpack(0, a.halo_pack(1))
     a.halo_unpack(1, b.halo_pack(0))
     _ran(km.expected_kernels(c), c.id)
-    ref = Oracle(W, H, threads=4, intensity=1.1).run(depth)
+    ref = harness.oracle(W, H, intensity=1.1).run(depth)
     for i, f in enumerate((a, b)):
         assert np.array_equal(f.band_phase_b(), ref[cuts[i]:cuts[i + 1]]), i
 
@@ -115,7 +113,7 @@ def _band_exchange(c: km.Case) -> None:
     time the first band runs are preset, as in test_kernel_logic_emulated.py."""
     W, H = 200, 528
     depth = _band_depth(W, H)
-    cuts, (a, b) = _band_frames(W, H, 2, intensity=1.1)
+    cuts, (a, b) = harness.band_frames(W, H, 2, intensity=1.1)
     a.band_phase_a(depth[cuts[0]:cuts[1]])
     b.band_phase_a(depth[cuts[1]:cuts[2]])
     emu.ledger_reset()
@@ -123,7 +121,7 @@ def _band_exchange(c: km.Case) -> None:
     a.flags(set_ready_ack=(fl["ready"][0], 1, fl["ack"][0], 1))
     assert a.exchange(None, b) == 0 and b.exchange(a, None) == 0
     _ran(km.expected_kernels(c), c.id)
-    ref = Oracle(W, H, threads=4, intensity=1.1).run(depth)
+    ref = harness.oracle(W, H, intensity=1.1).run(depth)
     for i, f in enumerate((a, b)):
         assert np.array_equal(f.band_phase_b(), ref[cuts[i]:cuts[i + 1]]), i
 

@@ -9,9 +9,9 @@ context per case, because MEAO_REN_TILE is read when a frame is recorded and a c
 import numpy as np
 import pytest
 
-import kernel_matrix as km  # noqa: E402  (tests/ is on sys.path via conftest)
-from test_arrays_gpu import Array, rt, torch_cuda  # noqa: E402,F401  (the fixtures)
-from test_layers_gpu import _ctx  # noqa: E402
+import harness  # noqa: E402  (tests/ is on sys.path via conftest)
+import kernel_matrix as km  # noqa: E402
+from gpu_harness import Array, rt, torch_cuda  # noqa: E402,F401  (the fixtures)
 
 pytestmark = pytest.mark.gpu
 
@@ -71,12 +71,11 @@ def _array_frame(torch, rt, ao, c, depth):
 
 @pytest.mark.parametrize("case", km.FRAME_CASES, ids=lambda c: c.id)
 def test_case_matches_the_oracle(torch_cuda, rt, case, monkeypatch):
-    from oracle.oracle import Oracle
     c = case
     monkeypatch.setenv("MEAO_REN_TILE", str(c.tile))
     W, H = c.size
     depth, seen = km.depth(c)
-    ao = _ctx(W, H, c.layers, reversed_z=c.reversed_z, sample_exhaustively=c.exhaustive, high_quality_mask=c.hq,
+    ao = harness.context(W, H, device=0, layers=c.layers, reversed_z=c.reversed_z, sample_exhaustively=c.exhaustive, high_quality_mask=c.hq,
               single_scale=c.single_scale, intensity=1.1)
     if c.form == "stage":
         got = _stage_frame(torch_cuda, ao, c, depth)
@@ -86,19 +85,7 @@ def test_case_matches_the_oracle(torch_cuda, rt, case, monkeypatch):
         got = _array_frame(torch_cuda, rt, ao, c, depth)
     bufs = {bid: ao.debug_buffer(bid) for bid in c.buffer_ids()}
     for l in range(c.layers):
-        orc = Oracle(W, H, threads=8, **c.oracle_kw())
+        orc = harness.oracle(W, H, threads=8, **c.oracle_kw())
         n = int((got[l] != orc.run(seen[l])).sum())
         assert n == 0, f"{c.id}: the AO of layer {l} differs from the oracle in {n} pixels"
-        bad = []
-        for bid, b in bufs.items():
-            g = b[l] if c.layers > 1 else b
-            if g.dtype == np.uint8:
-                n = int((g != orc.codes(bid)).sum())
-            elif g.dtype == np.float16:
-                with np.errstate(over="ignore"):
-                    n = int((g.view(np.uint16) != orc.buffer(bid).astype(np.float16).view(np.uint16)).sum())
-            else:
-                n = int((g.view(np.uint32) != orc.buffer(bid).view(np.uint32)).sum())
-            if n:
-                bad.append((bid, n))
-        assert not bad, f"{c.id} layer {l}: mismatching buffers (id, #diff) {bad}"
+        harness.compare_buffers(lambda bid: bufs[bid][l] if c.layers > 1 else bufs[bid], orc, f"{c.id} layer {l}", c.buffer_ids())

@@ -12,33 +12,16 @@ import pytest
 
 from miniengineao_b200 import AmbientOcclusion, Camera, MeaoError
 from miniengineao_b200 import _native as N
-from oracle.oracle import Oracle
 
+import harness
 from emu.emu import Frame
-from test_layers_emulated import _raw, contrasting_layers
 
 
 # visibly different cameras: near 0.1 / 0.3 / 1.0, far 50 / 100 / 1000, vertical FOV 40 / 60 / 90 degrees
 CAMS = [(0.1, 50.0, 40.0), (0.3, 100.0, 60.0), (1.0, 1000.0, 90.0)]
-PARAMS = {"noise_filter_tolerance": "noiseFilterTolerance", "blur_tolerance": "blurTolerance", "upsample_tolerance": "upsampleTolerance",
-          "thickness_modifier": "thicknessModifier", "intensity": "intensity", "sample_exhaustively": "sampleExhaustively",
-          "high_quality_mask": "highQualityMask"}
-
-
 def cameras(W, H, n, reversed_z=True):
     return [Camera(W, H, nearClipPlane=CAMS[i % 3][0], farClipPlane=CAMS[i % 3][1], fieldOfView=CAMS[i % 3][2], usesReversedZBuffer=reversed_z)
             for i in range(n)]
-
-
-def _plan(W, H, cams, single_scale=False, **kw):
-    p = AmbientOcclusion(Camera(W, H, usesReversedZBuffer=kw.get("reversed_z", True)), device=-1)
-    for py, cs in PARAMS.items():
-        if py in kw:
-            setattr(p, cs, kw[py])
-    p.singleScale = single_scale
-    p.layers = len(cams)
-    p.layerCameras = cams
-    return p
 
 
 def _aligned(nbytes):
@@ -47,42 +30,22 @@ def _aligned(nbytes):
     return raw[off:off + nbytes]
 
 
-def _oracle(W, H, cam, **kw):
-    return Oracle(W, H, threads=4, near=cam.nearClipPlane, far=cam.farClipPlane, tan_half_fov_h_=1.0 / cam.projection00,
-                  reversed_z=cam.usesReversedZBuffer, **kw)
-
-
 def _compare(f, W, H, depth, cams, *, linear=False, single_scale=False, oracle_depth=None, ao_of=None, **kw):
     okw = {k: v for k, v in kw.items() if k != "reversed_z"}
-    if linear:
-        okw["depth_is_linear"] = True
     if single_scale:
         okw["single_scale"] = True
-    mask = kw.get("high_quality_mask", 0)
-    ids = [1, 2, 3, 4, 5, 10, 17] if single_scale else list(range(1, 18)) + [17 + k for k in range(1, 5) if (mask >> (k - 1)) & 1]
+    ids = harness.buffer_ids(kw.get("high_quality_mask", 0), single_scale)
     for l, cam in enumerate(cams):
-        orc = _oracle(W, H, cam, **okw)
+        orc = harness.oracle(W, H, camera=cam, linear=linear, **okw)
         ref = orc.run(depth[l] if oracle_depth is None else oracle_depth[l])
         if ao_of is not None:
             assert np.array_equal(ao_of(l), ref), (W, H, l, "caller's AO view")
-        bad = []
-        for bid in ids:
-            got, want = f.buffer(bid, l), orc.buffer(bid)
-            if got.dtype == np.uint8:
-                n = int((got != orc.codes(bid)).sum())
-            elif got.dtype == np.float16:
-                with np.errstate(over="ignore"):
-                    n = int((got.view(np.uint16) != want.astype(np.float16).view(np.uint16)).sum())
-            else:
-                n = int((got.view(np.uint32) != want.view(np.uint32)).sum())
-            if n:
-                bad.append((bid, n, got.size))
-        assert not bad, f"{W}x{H} {kw} layer {l}: mismatching buffers (id, #diff, size): {bad}"
+        harness.compare_buffers(lambda bid: f.buffer(bid, l), orc, f"{W}x{H} {kw} layer {l}", ids)
 
 
 def _run(W, H, depth, *, use_tma=True, linear=False, single_scale=False, fused=True, oracle_depth=None, **kw):
     cams = cameras(W, H, depth.shape[0], kw.get("reversed_z", True))
-    f = Frame(_plan(W, H, cams, single_scale=single_scale, **kw), linear=linear, use_tma=use_tma)
+    f = Frame(harness.context(W, H, layers=len(cams), layer_cameras=cams, single_scale=single_scale, **kw), linear=linear, use_tma=use_tma)
     (f.run_fused if fused else f.run)(depth)
     _compare(f, W, H, depth, cams, linear=linear, single_scale=single_scale, oracle_depth=oracle_depth, **kw)
     return f
@@ -92,52 +55,49 @@ def _run(W, H, depth, *, use_tma=True, linear=False, single_scale=False, fused=T
 @pytest.mark.parametrize("use_tma", [True, False])
 @pytest.mark.parametrize("W,H", [(161, 93), (37, 300)])
 def test_ragged_layers_take_their_own_camera(W, H, use_tma):
-    f = _run(W, H, _raw(contrasting_layers(W, H, 3, seed=W)), use_tma=use_tma, intensity=1.1)
+    f = _run(W, H, harness.raw(harness.contrasting_layers(W, H, 3, seed=W)), use_tma=use_tma, intensity=1.1)
     if not use_tma:
         assert f.tma_loads_in_run == 0
 
 
 def test_interior_tiles_take_the_tma_path_with_layer_cameras():
     W, H = 640, 360
-    f = _run(W, H, _raw(contrasting_layers(W, H, 3, seed=3)), intensity=1.1, high_quality_mask=0b0011)
+    f = _run(W, H, harness.raw(harness.contrasting_layers(W, H, 3, seed=3)), intensity=1.1, high_quality_mask=0b0011)
     assert f.tma_loads_in_run > 300, f.tma_loads_in_run
 
 
 def test_forward_z_pads_each_layer_with_its_own_linearize0():
     """reversed_z = False: the atlas padding value Linearize(0) = near / far differs per layer."""
     W, H = 130, 70
-    _run(W, H, _raw(contrasting_layers(W, H, 3, seed=5), reversed_z=False), reversed_z=False, intensity=1.2)
+    _run(W, H, harness.raw(harness.contrasting_layers(W, H, 3, seed=5), reversed_z=False), reversed_z=False, intensity=1.2)
 
 
 @pytest.mark.parametrize("kw", [dict(high_quality_mask=15), dict(sample_exhaustively=True), dict(single_scale=True)])
 def test_layer_cameras_with_variants(kw):
     W, H = 130, 70
-    _run(W, H, _raw(contrasting_layers(W, H, 3, seed=7)), intensity=1.2, **kw)
+    _run(W, H, harness.raw(harness.contrasting_layers(W, H, 3, seed=7)), intensity=1.2, **kw)
 
 
 def test_prepare_then_layered_upsample_pair():
     """The pair prepare_depth -> LinearDepth -> layered upsample (stage API, array frames) with per-layer cameras."""
     W, H = 161, 93
-    _run(W, H, _raw(contrasting_layers(W, H, 3, seed=11)), fused=False, high_quality_mask=15)
+    _run(W, H, harness.raw(harness.contrasting_layers(W, H, 3, seed=11)), fused=False, high_quality_mask=15)
 
 
 def test_linear_and_native_ingest():
     W, H = 250, 131
-    lin = contrasting_layers(W, H, 3, seed=9)
+    lin = harness.contrasting_layers(W, H, 3, seed=9)
     _run(W, H, lin, linear=True)
-    raw = _raw(lin).astype(np.float64)
-    for bits, dt in ((16, np.uint16), (24, np.uint32)):
-        full = (1 << bits) - 1
-        codes = np.clip(np.rint(raw * full), 0, full).astype(np.uint32)
-        as_float = (codes.astype(np.float32) * np.float32(1.0 / full)).astype(np.float32)
-        words = codes.astype(np.uint16) if bits == 16 else (codes | (np.uint32(0xA5) << np.uint32(24)))
-        _run(W, H, words.astype(dt), oracle_depth=as_float)
+    raw = harness.raw(lin)
+    for kind in ("d16", "d24s8"):
+        words, as_float = harness.ingest(raw, kind)
+        _run(W, H, words, oracle_depth=as_float)
 
 
 def test_pitched_layered_corner():
     """The fused final level reading a layered depth corner of a larger buffer and writing into a padded AO view."""
     W, H, L = 150, 77, 3
-    depth = _raw(contrasting_layers(W, H, L, seed=13))
+    depth = harness.raw(harness.contrasting_layers(W, H, L, seed=13))
     dr, dl = 176, 176 * 90                     # element pitches of the depth view
     big = _aligned(dl * L * 4).view(np.float32)
     big[:] = np.nan
@@ -148,7 +108,7 @@ def test_pitched_layered_corner():
     ao = _aligned(al * L)
     ao[:] = 0xA7
     cams = cameras(W, H, L)
-    f = Frame(_plan(W, H, cams))
+    f = Frame(harness.context(W, H, layers=L, layer_cameras=cams))
     f.run_fused(big, depth_row=dr, depth_layer=dl, ao=ao, ao_row=ar, ao_layer=al)
     view = lambda l: np.stack([ao[l * al + y * ar: l * al + y * ar + W] for y in range(H)])
     _compare(f, W, H, depth, cams, ao_of=view)

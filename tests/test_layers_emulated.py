@@ -10,94 +10,36 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from miniengineao_b200 import AmbientOcclusion, Camera, MeaoError, synth
+from miniengineao_b200 import AmbientOcclusion, Camera, MeaoError
 from miniengineao_b200 import _native as N
-from oracle.oracle import Oracle
 
+import harness
 from emu.emu import Frame  # noqa: E402  (tests/ is on sys.path via conftest)
-
-
-PARAMS = {"noise_filter_tolerance": "noiseFilterTolerance", "blur_tolerance": "blurTolerance", "upsample_tolerance": "upsampleTolerance",
-          "thickness_modifier": "thicknessModifier", "intensity": "intensity", "sample_exhaustively": "sampleExhaustively",
-          "high_quality_mask": "highQualityMask"}
-
-
-def _plan(W, H, layers=1, single_scale=False, **kw):
-    p = AmbientOcclusion(Camera(W, H, usesReversedZBuffer=kw.get("reversed_z", True)), device=-1)
-    for py, cs in PARAMS.items():
-        if py in kw:
-            setattr(p, cs, kw[py])
-    p.singleScale = single_scale
-    p.layers = layers
-    return p
-
-
-def contrasting_layers(W, H, n, seed=0):
-    """Linear depth in [0, 1) of n layers that differ sharply at every boundary; layer 2 carries a sky patch (raw depth 0)."""
-    out = []
-    for i in range(n):
-        kind = i % 4
-        if kind == 0:
-            lin = synth.corridor(W, H, frame=i)
-        elif kind == 1:
-            lin = np.full((H, W), 0.37, np.float32)
-        elif kind == 2:
-            lin = synth.random_depth(W, H, seed=seed + 17 * i, lo=0.05, hi=0.6)
-        else:
-            lin = synth.random_depth(W, H, seed=seed + 31 * i)
-        out.append(lin.astype(np.float32))
-    return np.stack(out)
-
-
-def _raw(lin, reversed_z=True):
-    raw = np.stack([synth.lin01_to_raw(l, reversed_z=reversed_z) for l in lin])
-    if len(raw) > 2:
-        H, W = raw.shape[1:]
-        raw[2, H // 4: H // 2, W // 5: W // 2] = 0.0          # sky: raw 0 -> 1e5 -> inf in f16 -> NaN paths
-    return raw
-
-
-def _compare_layer(f, layer, orc, tag, mask=0, ids=None):
-    bad = []
-    for bid in ids or (list(range(1, 18)) + [17 + k for k in range(1, 5) if (mask >> (k - 1)) & 1]):
-        got, ref = f.buffer(bid, layer), orc.buffer(bid)
-        if got.dtype == np.uint8:
-            n = int((got != orc.codes(bid)).sum())
-        elif got.dtype == np.float16:
-            with np.errstate(over="ignore"):
-                n = int((got.view(np.uint16) != ref.astype(np.float16).view(np.uint16)).sum())
-        else:
-            n = int((got.view(np.uint32) != ref.view(np.uint32)).sum())
-        if n:
-            bad.append((bid, n, got.size))
-    assert not bad, f"{tag} layer {layer}: mismatching buffers (id, #diff, size): {bad}"
 
 
 def _run_layers(W, H, depth, *, use_tma=True, linear=False, single_scale=False, oracle_depth=None, **kw):
     """depth: [L, H, W] in the ingest format; oracle_depth: the float32 the oracle sees per layer (default: depth itself)."""
     L = depth.shape[0]
-    f = Frame(_plan(W, H, L, single_scale=single_scale, **kw), linear=linear, use_tma=use_tma)
+    f = Frame(harness.context(W, H, layers=L, single_scale=single_scale, **kw), linear=linear, use_tma=use_tma)
     n0 = f.tma_box_loads()
     f.run(depth)
     f.tma_loads_in_run = f.tma_box_loads() - n0
     okw = dict(kw)
-    if linear:
-        okw["depth_is_linear"] = True
     if single_scale:
         okw["single_scale"] = True
-    ids = [1, 2, 3, 4, 5, 10, 17] if single_scale else None
+    ids = harness.buffer_ids(kw.get("high_quality_mask", 0), single_scale)
     for l in range(L):
-        orc = Oracle(W, H, threads=4, **okw)
+        orc = harness.oracle(W, H, linear=linear, **okw)
         ref = orc.run(depth[l] if oracle_depth is None else oracle_depth[l])
         assert np.array_equal(f.buffer(17, l), ref), (W, H, l, kw)
-        _compare_layer(f, l, orc, f"{W}x{H} {kw}", kw.get("high_quality_mask", 0), ids)
+        harness.compare_buffers(lambda bid: f.buffer(bid, l), orc, f"{W}x{H} {kw} layer {l}", ids)
     return f
 
 
 @pytest.mark.parametrize("use_tma", [True, False])
 @pytest.mark.parametrize("W,H", [(161, 93), (37, 300), (250, 131)])
 def test_ragged_layers_equal_single_layer_oracle(W, H, use_tma):
-    depth = _raw(contrasting_layers(W, H, 3, seed=W))
+    depth = harness.raw(harness.contrasting_layers(W, H, 3, seed=W))
     f = _run_layers(W, H, depth, use_tma=use_tma, intensity=1.1)
     if not use_tma:
         assert f.tma_loads_in_run == 0
@@ -106,7 +48,7 @@ def test_ragged_layers_equal_single_layer_oracle(W, H, use_tma):
 def test_layered_interior_tiles_take_the_tma_path():
     """Big enough for interior (TMA-fed) tiles in every layer: the boxes are fetched at the layer's row offset of the stacked map."""
     W, H = 640, 360
-    depth = _raw(contrasting_layers(W, H, 3, seed=3))
+    depth = harness.raw(harness.contrasting_layers(W, H, 3, seed=3))
     f = _run_layers(W, H, depth, intensity=1.1, high_quality_mask=0b0011)
     assert f.tma_loads_in_run > 300, f.tma_loads_in_run
 
@@ -115,7 +57,7 @@ def test_layered_interior_tiles_take_the_tma_path():
 def test_layered_variants(kw):
     W, H = 130, 70
     rz = kw.get("reversed_z", True)
-    depth = _raw(contrasting_layers(W, H, 3, seed=7), reversed_z=rz)
+    depth = harness.raw(harness.contrasting_layers(W, H, 3, seed=7), reversed_z=rz)
     _run_layers(W, H, depth, intensity=1.2, **kw)
 
 
@@ -123,13 +65,13 @@ def test_null_camera_tables_take_the_argument_block_constants():
     """The layered and array kernels given no camera tables (a null table: every layer takes the argument block's constants).  libmeao
     always passes its tables, so this pins the launchers' fallback on purpose: the stage frame, the fused frame and an array frame."""
     W, H = 161, 93
-    depth = _raw(contrasting_layers(W, H, 3, seed=5))
-    f = Frame(_plan(W, H, 3, intensity=1.1), null_tables=True)
-    refs = [Oracle(W, H, threads=4, intensity=1.1) for _ in range(3)]
+    depth = harness.raw(harness.contrasting_layers(W, H, 3, seed=5))
+    f = Frame(harness.context(W, H, layers=3, intensity=1.1), null_tables=True)
+    refs = [harness.oracle(W, H, intensity=1.1) for _ in range(3)]
     aos = [r.run(depth[l]) for l, r in enumerate(refs)]
     f.run(depth)
     for l in range(3):
-        _compare_layer(f, l, refs[l], "null tables")
+        harness.compare_buffers(lambda bid: f.buffer(bid, l), refs[l], f"null tables layer {l}", harness.buffer_ids())
     f.run_fused(depth)
     fused = [f.buffer(17, l) for l in range(3)]
     ao = f.run_arrays(depth, "layered")
@@ -139,26 +81,22 @@ def test_null_camera_tables_take_the_argument_block_constants():
 
 def test_layered_linear_and_native_ingest():
     W, H = 250, 131
-    lin = contrasting_layers(W, H, 3, seed=9)
+    lin = harness.contrasting_layers(W, H, 3, seed=9)
     _run_layers(W, H, lin, linear=True)
-    raw = _raw(lin).astype(np.float64)
-    for bits, dt in ((16, np.uint16), (24, np.uint32)):
-        full = (1 << bits) - 1
-        codes = np.clip(np.rint(raw * full), 0, full).astype(np.uint32)
-        as_float = (codes.astype(np.float32) * np.float32(1.0 / full)).astype(np.float32)
-        words = codes.astype(np.uint16) if bits == 16 else (codes | (np.uint32(0xA5) << np.uint32(24)))
-        _run_layers(W, H, words.astype(dt), oracle_depth=as_float)
+    raw = harness.raw(lin)
+    for kind in ("d16", "d24s8"):
+        words, as_float = harness.ingest(raw, kind)
+        _run_layers(W, H, words, oracle_depth=as_float)
 
 
 def test_layered_vector_alignment_widths():
     """W % 8 == 0 keeps the 128-bit input loads in every layer (the layer stride W x H keeps the 16-byte alignment); W % 4 == 0
     with D16 input takes the per-element path.  Both must equal the oracle."""
     for W, H, dt in ((136, 40, np.uint16), (132, 44, np.uint16), (132, 44, np.float32)):
-        raw = _raw(contrasting_layers(W, H, 3, seed=W)).astype(np.float64)
+        raw = harness.raw(harness.contrasting_layers(W, H, 3, seed=W))
         if dt == np.uint16:
-            codes = np.clip(np.rint(raw * 65535), 0, 65535).astype(np.uint32)
-            as_float = (codes.astype(np.float32) * np.float32(1.0 / 65535)).astype(np.float32)
-            _run_layers(W, H, codes.astype(np.uint16), oracle_depth=as_float)
+            codes, as_float = harness.ingest(raw, "d16")
+            _run_layers(W, H, codes, oracle_depth=as_float)
         else:
             _run_layers(W, H, raw.astype(np.float32))
 

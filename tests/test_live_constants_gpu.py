@@ -8,16 +8,12 @@ import ctypes as C
 import numpy as np
 import pytest
 
+import harness
 import hostile_cases as HC
-from test_arrays_gpu import Array, rt, torch_cuda  # noqa: F401  (fixtures)
-from test_dynamic_resolution_gpu import SLEEP_CYCLES, _backlog, _depth
+from gpu_harness import SLEEP_CYCLES, Array, backlog, fresh_frame, native_bands, rt, torch_cuda  # noqa: F401  (the fixtures)
 
 pytestmark = pytest.mark.gpu
 
-# the Python property of each MeaoParams field, and the oracle's keyword for it
-PARAMS = {"noiseFilterTolerance": "noise_filter_tolerance", "blurTolerance": "blur_tolerance", "upsampleTolerance": "upsample_tolerance",
-          "thicknessModifier": "thickness_modifier", "intensity": "intensity"}
-SNAKE = {v: k for k, v in PARAMS.items()}
 # frame -> (hostile camera, hostile parameters): far/near at both extremes, fields of view at both extremes, upsample tolerances and
 # noise filter strengths on both sides of upsample_fast_div_ok, thickness and intensity far outside their ranges
 HOSTILE = {5: ("far_near_1e7", dict(upsample_tolerance=-16.56)), 9: ("tan_half_fov_1em6", dict(upsample_tolerance=-16.55)),
@@ -39,7 +35,7 @@ def _inputs(i, W, H, n=N_FRAMES):
         cam.update(nearClipPlane=near, farClipPlane=far)
         if tan is not None:
             cam["fieldOfView"] = HC.fov_for_tan_half_h(tan, W, H)
-        params.update({SNAKE[k]: v for k, v in hp.items()})
+        params.update({harness.PARAMS[k]: v for k, v in hp.items()})
     return cam, params
 
 
@@ -51,32 +47,14 @@ def _apply(ao, cam, params, cameras=None):
         setattr(ao, k, v)
 
 
-def _ao(W, H, cam=None, params=None, **kw):
-    from miniengineao_b200 import AmbientOcclusion, Camera
-    ao = AmbientOcclusion(Camera(W, H), device=0, use_graph=kw.pop("use_graph", True))
-    for k, v in kw.items():
-        setattr(ao, k, v)
-    _apply(ao, cam or {}, params or {})
-    return ao
-
-
 def _fresh(torch, W, H, depth, cam, params, layers=1, table=None):
     """The AO and every debug buffer of a fresh context given these inputs in one go."""
     from miniengineao_b200 import Camera
-    f = _ao(W, H, cam, params, layers=layers)
+    f = harness.context(W, H, device=0, layers=layers)
+    _apply(f, cam, params)
     if table is not None:
         f.layerCameras = [Camera(W, H, **c) for c in table]
-    out = f.render(torch.from_numpy(np.ascontiguousarray(depth)).cuda()).cpu().numpy()
-    bufs = {bid: f.debug_buffer(bid) for bid in HC.buffer_ids()}
-    f.close()
-    return out, bufs
-
-
-def _oracle(cam_obj, params, depth):
-    from oracle.oracle import Oracle
-    H, W = depth.shape
-    orc = Oracle(W, H, threads=8, **HC.oracle_camera_kw(cam_obj), **{PARAMS[k]: v for k, v in params.items()})
-    return orc, orc.run(depth)
+    return fresh_frame(torch, f, depth)
 
 
 def _res(ao):
@@ -86,24 +64,25 @@ def _res(ao):
 @pytest.mark.parametrize("W,H", [(1000, 563), (1920, 1080)])
 def test_animated_camera_and_parameters(torch_cuda, W, H):
     torch = torch_cuda
-    ao = _ao(W, H)
+    ao = harness.context(W, H, device=0)
     dd = torch.empty((H, W), device="cuda")                             # one depth and one AO buffer: one graph for every frame
     out = torch.empty((H, W), dtype=torch.uint8, device="cuda")
     r1 = None
     for i in range(N_FRAMES):
         cam, params = _inputs(i, W, H)
         _apply(ao, cam, params)
-        d = _depth(W, H, frame=i)
+        d = harness.corridor_depth(W, H, frame=i)
         dd.copy_(torch.from_numpy(d))
         got = ao.render(dd, out).cpu().numpy()
         ref, ref_bufs = _fresh(torch, W, H, d, cam, params)
-        assert HC.n_diff(got, ref) == 0, f"frame {i}: AO differs from a fresh context"
-        for bid in HC.buffer_ids():
-            assert HC.n_diff(ao.debug_buffer(bid), ref_bufs[bid]) == 0, f"frame {i}: buffer {bid} differs from a fresh context"
+        assert harness.n_diff(got, ref) == 0, f"frame {i}: AO differs from a fresh context"
+        for bid in harness.buffer_ids():
+            assert harness.n_diff(ao.debug_buffer(bid), ref_bufs[bid]) == 0, f"frame {i}: buffer {bid} differs from a fresh context"
         if i % 4 == 0 or i in HOSTILE:
-            orc, oref = _oracle(ao.camera, params, d)
-            assert HC.n_diff(got, oref) == 0, f"frame {i}: AO differs from the oracle"
-            HC.compare_buffers(ao.debug_buffer, orc, f"frame {i}", HC.buffer_ids())
+            orc = harness.oracle(W, H, camera=ao.camera, threads=8, **{harness.PROPERTIES[k]: v for k, v in params.items()})
+            oref = orc.run(d)
+            assert harness.n_diff(got, oref) == 0, f"frame {i}: AO differs from the oracle"
+            harness.compare_buffers(ao.debug_buffer, orc, f"frame {i}", harness.buffer_ids())
         r = _res(ao)
         if r1 is None:
             r1 = r
@@ -117,14 +96,14 @@ def test_camera_and_intensity_changes_do_not_wait(torch_cuda):
     torch = torch_cuda
     W, H = 1920, 1080
     s = torch.cuda.Stream()
-    ao = _ao(W, H)
-    d = torch.from_numpy(_depth(W, H)).cuda()
+    ao = harness.context(W, H, device=0)
+    d = torch.from_numpy(harness.corridor_depth(W, H)).cuda()
     outs = [torch.empty((H, W), dtype=torch.uint8, device="cuda") for _ in range(5)]
     for o in outs:                                                      # every output's graph: captured before the backlog
         ao.render(d, o, stream=s)
     torch.cuda.synchronize()
     inst = _res(ao)["graph_instantiations"]
-    e = _backlog(torch, s, ao, d, outs[0])
+    e = backlog(torch, s, ao, d, outs[0])
     frames = []
     for i in range(1, 5):
         cam, params = dict(fieldOfView=40.0 + 10.0 * i, nearClipPlane=0.1 * i), dict(intensity=0.5 + 0.3 * i)
@@ -134,11 +113,11 @@ def test_camera_and_intensity_changes_do_not_wait(torch_cuda):
     assert not e.query(), "a camera or parameter change waited for the GPU"
     torch.cuda.synchronize()
     assert _res(ao)["graph_instantiations"] == inst
-    dn = _depth(W, H)
+    dn = harness.corridor_depth(W, H)
     for cam, params, out in frames:
-        assert HC.n_diff(out.cpu().numpy(), _fresh(torch, W, H, dn, cam, params)[0]) == 0, (cam, params)
+        assert harness.n_diff(out.cpu().numpy(), _fresh(torch, W, H, dn, cam, params)[0]) == 0, (cam, params)
     # the control: a structural input (MeaoVariants) under the same backlog does drain the GPU -- the test observes what it claims
-    e = _backlog(torch, s, ao, d, outs[0])
+    e = backlog(torch, s, ao, d, outs[0])
     ao.sampleExhaustively = True
     ao.render(d, outs[1], stream=s)
     assert e.query(), "a variant change is expected to re-plan with a device synchronise"
@@ -164,10 +143,10 @@ def test_pitched_and_no_graph_frames(torch_cuda):
     W, H = 1000, 563
     s = torch.cuda.Stream()
     rtd = torch.zeros((H + 7, W + 24), device="cuda")
-    d = _depth(W, H)
+    d = harness.corridor_depth(W, H)
     rtd[3:3 + H, 5:5 + W].copy_(torch.from_numpy(d))
     for use_graph in (True, False):
-        ao = _ao(W, H, use_graph=use_graph)
+        ao = harness.context(W, H, device=0, use_graph=use_graph)
         big = [torch.zeros((H + 3, W + 40), dtype=torch.uint8, device="cuda") for _ in range(4)]
         for b in big:
             ao.render(rtd[3:3 + H, 5:5 + W], b[:H, 8:8 + W], stream=s)
@@ -184,7 +163,7 @@ def test_pitched_and_no_graph_frames(torch_cuda):
         torch.cuda.synchronize()
         assert _res(ao)["graph_instantiations"] == inst
         for cam, params, b in steps:
-            assert HC.n_diff(b[:H, 8:8 + W].cpu().numpy(), _fresh(torch, W, H, d, cam, params)[0]) == 0, (use_graph, cam, params)
+            assert harness.n_diff(b[:H, 8:8 + W].cpu().numpy(), _fresh(torch, W, H, d, cam, params)[0]) == 0, (use_graph, cam, params)
         ao.close()
 
 
@@ -192,8 +171,8 @@ def test_array_frames_keep_their_arrays(torch_cuda, rt):
     torch = torch_cuda
     W, H = 777, 431
     s = torch.cuda.Stream()
-    ao = _ao(W, H)
-    d = _depth(W, H)
+    ao = harness.context(W, H, device=0)
+    d = harness.corridor_depth(W, H)
     da = Array(rt, W, H, np.float32)
     da.fill(d)
     aas = [Array(rt, W, H, np.uint8) for _ in range(4)]
@@ -213,7 +192,7 @@ def test_array_frames_keep_their_arrays(torch_cuda, rt):
     torch.cuda.synchronize()
     assert _res(ao)["graph_instantiations"] == inst, "a constants change released the arrays' graphs"
     for cam, params, a in steps:
-        assert HC.n_diff(a.read()[0], _fresh(torch, W, H, d, cam, params)[0]) == 0, (cam, params)
+        assert harness.n_diff(a.read()[0], _fresh(torch, W, H, d, cam, params)[0]) == 0, (cam, params)
     for a in [da] + aas:
         ao.release_array(a.handle)
         a.free()
@@ -225,9 +204,9 @@ def test_plugin_event_bound_once(torch_cuda):
     torch = torch_cuda
     W, H = 1280, 720
     s = torch.cuda.Stream()
-    ao = _ao(W, H)
+    ao = harness.context(W, H, device=0)
     ao.LateUpdate()
-    d = _depth(W, H)
+    d = harness.corridor_depth(W, H)
     dd = torch.from_numpy(d).cuda()
     out = torch.zeros((H, W), dtype=torch.uint8, device="cuda")
     lib = N.lib()
@@ -242,7 +221,7 @@ def test_plugin_event_bound_once(torch_cuda):
         lib.meao_render_event(91)
         assert not e.query(), "a constants change waited for the GPU"
         torch.cuda.synchronize()
-        assert HC.n_diff(out.cpu().numpy(), _fresh(torch, W, H, d, cam, params)[0]) == 0, (cam, params)
+        assert harness.n_diff(out.cpu().numpy(), _fresh(torch, W, H, d, cam, params)[0]) == 0, (cam, params)
     assert _res(ao)["graph_instantiations"] == 1
     lib.meao_bind_event(ao._ctx, 91, None, 0, None, None)
     ao.close()
@@ -251,9 +230,9 @@ def test_plugin_event_bound_once(torch_cuda):
 def test_host_async_slots_and_stage_api(torch_cuda):
     torch = torch_cuda
     W, H = 960, 540
-    ao = _ao(W, H)
+    ao = harness.context(W, H, device=0)
     lib = ao._lib
-    d = _depth(W, H)
+    d = harness.corridor_depth(W, H)
     dpin = torch.from_numpy(d).pin_memory()
     outs = [torch.zeros((H, W), dtype=torch.uint8).pin_memory() for _ in range(6)]
     ao.LateUpdate()
@@ -274,7 +253,7 @@ def test_host_async_slots_and_stage_api(torch_cuda):
     assert lib.meao_host_wait(ao._ctx, 0) == 0 and lib.meao_host_wait(ao._ctx, 1) == 0
     torch.cuda.synchronize()
     for cam, params, o in steps:
-        assert HC.n_diff(o.numpy(), _fresh(torch, W, H, d, cam, params)[0]) == 0, (cam, params)
+        assert harness.n_diff(o.numpy(), _fresh(torch, W, H, d, cam, params)[0]) == 0, (cam, params)
     # the stage API on a stream behind a backlog: each stage call takes the constants of now
     dd = torch.from_numpy(d).cuda()
     for i in range(6, 8):
@@ -290,8 +269,8 @@ def test_host_async_slots_and_stage_api(torch_cuda):
         assert not e.query(), "the stage API waited for the GPU after a constants change"
         torch.cuda.synchronize()
         _, ref_bufs = _fresh(torch, W, H, d, cam, params)
-        for bid in HC.buffer_ids():
-            assert HC.n_diff(ao.debug_buffer(bid), ref_bufs[bid]) == 0, f"stage API step {i}: buffer {bid}"
+        for bid in harness.buffer_ids():
+            assert harness.n_diff(ao.debug_buffer(bid), ref_bufs[bid]) == 0, f"stage API step {i}: buffer {bid}"
     ao.close()
 
 
@@ -306,9 +285,9 @@ def test_layered_tables_change_every_frame_back_to_back(torch_cuda):
         return [dict(fieldOfView=30.0 + 9.0 * l + 3.0 * i, nearClipPlane=0.05 + 0.1 * l + 0.02 * i, farClipPlane=50.0 + 200.0 * l + 17.0 * i)
                 for l in range(L)]
 
-    ao = _ao(W, H, layers=L)
+    ao = harness.context(W, H, device=0, layers=L)
     ao.layerCameras = [Camera(W, H, **c) for c in table(0)]
-    d = _depth(W, H, L=L)
+    d = harness.corridor_depth(W, H, L=L)
     dd = torch.from_numpy(d).cuda()
     s = torch.cuda.Stream()
     outs = [torch.empty((L, H, W), dtype=torch.uint8, device="cuda") for _ in range(6)]
@@ -328,7 +307,7 @@ def test_layered_tables_change_every_frame_back_to_back(torch_cuda):
     assert _res(ao)["graph_instantiations"] == inst
     for t, intensity, out in frames:
         ref, _ = _fresh(torch, W, H, d, {}, dict(intensity=intensity), layers=L, table=t)
-        assert HC.n_diff(out.cpu().numpy(), ref) == 0, "a back-to-back frame read another frame's camera table"
+        assert harness.n_diff(out.cpu().numpy(), ref) == 0, "a back-to-back frame read another frame's camera table"
     ao.close()
 
 
@@ -336,10 +315,10 @@ def test_reserved_context_with_an_aspect_following_camera(torch_cuda):
     """The default Camera's projection follows its pixel aspect, so every resize below is a camera change as well."""
     torch = torch_cuda
     M = (1920, 1080)
-    ao = _ao(*M, maxResolution=M)
+    ao = harness.context(*M, device=0, max_resolution=M)
     sizes = [(1920, 1080), (1601, 901), (1000, 563), (1777, 999), (1280, 720)]
     walk = sizes[1:] + sizes[:1] + sizes[2:]
-    depths = {sz: torch.from_numpy(_depth(*sz)).cuda() for sz in sizes}
+    depths = {sz: torch.from_numpy(harness.corridor_depth(*sz)).cuda() for sz in sizes}
     outs = [torch.empty((sz[1], sz[0]), dtype=torch.uint8, device="cuda") for sz in walk]
     for sz, o in zip(walk, outs):                                      # the first capture of every size and output
         ao.camera.pixelWidth, ao.camera.pixelHeight = sz
@@ -359,18 +338,17 @@ def test_reserved_context_with_an_aspect_following_camera(torch_cuda):
     assert r1["arena_allocations"] == r0["arena_allocations"] and r1["graph_instantiations"] == r0["graph_instantiations"], (r0, r1)
     for sz, intensity, out in frames:
         ref, _ = _fresh(torch, *sz, depths[sz].cpu().numpy(), {}, dict(intensity=intensity))
-        assert HC.n_diff(out.cpu().numpy(), ref) == 0, sz
+        assert harness.n_diff(out.cpu().numpy(), ref) == 0, sz
     ao.close()
 
 
 def test_row_bands_follow_the_camera(torch_cuda):
     """Two connected bands in one process (as the native-exchange tests run them): the camera changes between steps, the bands stay
     connected and the union of the bands equals the whole frame of a fresh context every step."""
-    from test_parity_gpu import _native_bands
     torch = torch_cuda
     W, H, bands = 1920, 1080, 2
-    cuts, ctxs, streams = _native_bands(torch, W, H, bands)
-    d = _depth(W, H)
+    cuts, ctxs, streams = native_bands(torch, W, H, bands)
+    d = harness.corridor_depth(W, H)
     bufs = [torch.from_numpy(np.ascontiguousarray(d[cuts[i]:cuts[i + 1]])).cuda() for i in range(bands)]
     outs = [torch.zeros((cuts[i + 1] - cuts[i], W), dtype=torch.uint8, device="cuda") for i in range(bands)]
     for step in range(4):
@@ -384,7 +362,7 @@ def test_row_bands_follow_the_camera(torch_cuda):
         assert [a.band_status()["error"] for a in ctxs] == [0] * bands, "a neighbour exchange timed out"
         assert [a.band_status()["epoch"] for a in ctxs] == [step + 2] * bands, "a constants change reset the band's epoch"
         got = np.concatenate([o.cpu().numpy() for o in outs], axis=0)
-        assert HC.n_diff(got, _fresh(torch, W, H, d, cam, params)[0]) == 0, f"step {step}: the bands differ from the whole frame"
+        assert harness.n_diff(got, _fresh(torch, W, H, d, cam, params)[0]) == 0, f"step {step}: the bands differ from the whole frame"
     assert all(_res(a)["graph_instantiations"] == 1 for a in ctxs)
     for a in ctxs:
         a.close()

@@ -9,9 +9,9 @@ import random
 
 import pytest
 
+import harness
 import hostile_cases as HC
 from miniengineao_b200 import _native as N
-from test_dynamic_resolution_plan import _constants
 
 MAX = (3840, 2160)
 # ten sizes for eight slots: a walk through them evicts, and comes back to sizes parked several constant changes ago
@@ -63,7 +63,7 @@ def _check_fresh(h, st, tag, size=None):
     lib = N.lib()
     f = st.fresh(size)
     try:
-        assert _constants(h, st.layers) == _constants(f, st.layers), tag
+        assert harness.plan_constants(h, st.layers) == harness.plan_constants(f, st.layers), tag
     finally:
         lib.meao_destroy(f)
 
@@ -166,7 +166,7 @@ def test_refused_inputs_change_nothing():
         p, got = N.MeaoParams(), (N.MeaoCamera * 3)()
         assert lib.meao_get_params(h, C.byref(p)) == 0
         assert lib.meao_get_layer_cameras(h, got, 3) == 3
-        return _constants(h, 3), _key(p), bytes(got)
+        return harness.plan_constants(h, 3), _key(p), bytes(got)
 
     before = snapshot()
     refusals = [

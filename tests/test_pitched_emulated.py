@@ -11,44 +11,10 @@ target, premin, single-scale and a row band.  Zero pitches in the argument block
 import numpy as np
 import pytest
 
-from oracle.oracle import Oracle
-
-from test_fused_lin_emulated import _ingest, _raw_with_sky, fused_frame  # noqa: E402  (tests/ is on sys.path via conftest)
-from test_layers_emulated import _compare_layer, _plan, contrasting_layers
 from miniengineao_b200 import synth
 
-SENTINEL = 0xA5
-
-
-class View:
-    """`shape` = (layers, rows, W) elements of `dtype` at byte pitches (row, layer), `base` bytes past a 256-byte boundary of a backing
-    allocation filled with `fill`."""
-
-    def __init__(self, shape, dtype, row, layer, base=0, fill=0xFF):
-        L, rows, W = shape
-        es = np.dtype(dtype).itemsize
-        self.extent = (L - 1) * layer + (rows - 1) * row + W * es
-        self.raw = np.empty(base + self.extent + 512, np.uint8)
-        off = (-self.raw.ctypes.data) % 256
-        self.back = self.raw[off:off + base + self.extent + 256]
-        self.back[...] = fill
-        self.base, self.row, self.layer = base, row, layer
-        self.arr = np.ndarray(shape, dtype, buffer=self.back, offset=base, strides=(layer, row, es))
-
-    @property
-    def ptr(self):
-        return self.back.ctypes.data + self.base
-
-    def outside(self):
-        """The backing bytes that are not part of the view."""
-        mask = np.ones(self.back.size, bool)
-        L, rows, W = self.arr.shape
-        es = self.arr.itemsize
-        for l in range(L):
-            for r in range(rows):
-                s = self.base + l * self.layer + r * self.row
-                mask[s:s + W * es] = False
-        return self.back[mask]
+import harness
+from harness import SENTINEL, View, fused_frame
 
 
 def _frame(depth, seen, *, drow=None, dlayer=None, dbase=0, arow=None, alayer=None, abase=0, linear=False, rz=True, rows=(0, 0),
@@ -61,7 +27,7 @@ def _frame(depth, seen, *, drow=None, dlayer=None, dbase=0, arow=None, alayer=No
     dlayer = dlayer or H * drow
     arow = arow or W
     alayer = alayer or H * arow
-    f = fused_frame(_plan(W, H, L, reversed_z=rz, intensity=1.1, **kw), linear=linear)
+    f = fused_frame(harness.context(W, H, layers=L, reversed_z=rz, intensity=1.1, **kw), linear=linear)
     band = rows[1] > rows[0]
     dv = View(depth.shape, depth.dtype, drow, dlayer, dbase)
     dv.arr[...] = depth
@@ -72,19 +38,19 @@ def _frame(depth, seen, *, drow=None, dlayer=None, dbase=0, arow=None, alayer=No
     assert (dv.outside() == 0xFF).all()
     okw = dict(intensity=1.1, reversed_z=rz, depth_is_linear=linear, **kw)
     for l in range(L):
-        orc = Oracle(W, H, threads=4, **okw)
+        orc = harness.oracle(W, H, **okw)
         ref = orc.run(seen[l])
         if band:
             assert np.array_equal(av.arr[l], ref[rows[0]:rows[1]]), f"band layer {l}"
             continue
         assert np.array_equal(av.arr[l], ref), f"AO view layer {l}"
-        _compare_layer(f, l, orc, f"layer {l}", ids=[1, 2, 3, 4, 5])       # LinearDepth, LowDepth1..4
+        harness.compare_buffers(lambda bid: f.buffer(bid, l), orc, f"layer {l}", [1, 2, 3, 4, 5])       # LinearDepth, LowDepth1..4
     return f
 
 
 def _one(W, H, kind, seed, rz=True):
-    raw = synth.random_depth(W, H, seed=seed).astype(np.float32) if kind == "linear" else _raw_with_sky(W, H, seed, rz)
-    depth, seen = _ingest(raw, kind)
+    raw = synth.random_depth(W, H, seed=seed).astype(np.float32) if kind == "linear" else harness.raw_with_sky(W, H, seed, rz)
+    depth, seen = harness.ingest(raw, kind)
     return depth[None], seen[None]
 
 
@@ -123,7 +89,7 @@ def test_sub_rectangle_at_x0_1():
 def test_dynamic_resolution_corner_of_a_layered_target(layers):
     """[L, Hmax, Wmax][:, :H, :W]: the layer pitch is the whole max-size image, larger than rows x row pitch; premin on level 1."""
     W, H, Wmax, Hmax = 130, 70, 200, 96
-    lin = contrasting_layers(W, H, layers, seed=layers)
+    lin = harness.contrasting_layers(W, H, layers, seed=layers)
     raw = np.stack([synth.lin01_to_raw(l) for l in lin]).astype(np.float32)
     raw[min(2, layers - 1), H // 4: H // 2, W // 5: W // 2] = 0.0
     _frame(raw, raw, drow=Wmax * 4, dlayer=Hmax * Wmax * 4, arow=Wmax, alayer=Hmax * Wmax, high_quality_mask=1)
@@ -132,8 +98,8 @@ def test_dynamic_resolution_corner_of_a_layered_target(layers):
 def test_layered_d16_layer_pitch_off_the_grid():
     """Layer pitches that are not multiples of 16 (depth) or 8 (AO) bytes although the rows are: the layered vector-path rule."""
     W, H, L = 64, 40, 3
-    raws = [_raw_with_sky(W, H, 20 + l) for l in range(L)]
-    pairs = [_ingest(r, "d16") for r in raws]
+    raws = [harness.raw_with_sky(W, H, 20 + l) for l in range(L)]
+    pairs = [harness.ingest(r, "d16") for r in raws]
     depth, seen = np.stack([p[0] for p in pairs]), np.stack([p[1] for p in pairs])
     _frame(depth, seen, drow=256, dlayer=256 * H + 2, arow=64, alayer=64 * H + 4)
 
@@ -159,8 +125,8 @@ def test_zero_pitches_in_the_argument_blocks_mean_tight(kind):
     W, H = 136, 72
     depth, seen = _one(W, H, kind, 11)
     _frame(depth, seen, zero=True)
-    raws = [_raw_with_sky(W, H, 30 + l) for l in range(2)]
-    pairs = [_ingest(r, kind) for r in raws]
+    raws = [harness.raw_with_sky(W, H, 30 + l) for l in range(2)]
+    pairs = [harness.ingest(r, kind) for r in raws]
     _frame(np.stack([p[0] for p in pairs]), np.stack([p[1] for p in pairs]), zero=True)
 
 

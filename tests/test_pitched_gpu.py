@@ -8,22 +8,13 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from test_fused_lin_emulated import _ingest  # noqa: E402  (tests/ is on sys.path via conftest)
-from test_layers_gpu import _ctx, _frames, _oracle
-from test_pitched_emulated import SENTINEL, View
+import harness
+from gpu_harness import torch_cuda  # noqa: F401  (the fixture)
+from harness import SENTINEL, View
 
 pytestmark = pytest.mark.gpu
 
 KINDS = {"f32": 0, "linear": 1, "d16": 2, "d24s8": 3}
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("GPU tests need a GPU")
-    torch.cuda.init()
-    return torch
 
 
 class DevView:
@@ -48,8 +39,8 @@ def _depth(kind, W, H, L, seed=0, rz=True):
         from miniengineao_b200 import synth
         lin = np.stack([synth.random_depth(W, H, seed=seed + i) for i in range(L)]).astype(np.float32)
         return lin, lin
-    raw = _frames(W, H, L, seed=seed, reversed_z=rz)
-    pairs = [_ingest(r, kind) for r in raw]
+    raw = harness.frames(W, H, L, seed=seed, reversed_z=rz)
+    pairs = [harness.ingest(r, kind) for r in raw]
     return np.stack([p[0] for p in pairs]), np.stack([p[1] for p in pairs])
 
 
@@ -100,7 +91,7 @@ def _check_frame(torch, ao, depth, seen, kind, d: DevView, a: DevView, oracle=Tr
     if oracle:
         L, H, W = depth.shape
         for l in range(L):
-            ref = _oracle(W, H, linear=(kind == "linear"), **params).run(seen[l])
+            ref = harness.oracle(W, H, linear=(kind == "linear"), threads=8, **params).run(seen[l])
             assert np.array_equal(got[l], ref), f"layer {l} differs from the oracle"
     return got
 
@@ -112,7 +103,7 @@ def test_pitched_equals_tight_and_oracle(torch_cuda, W, H, kind, pitch):
     """Padded rows: 256-byte multiples (D3D12 footprints: 1366 x 4 B rows are 5632 bytes apart), and a row pitch off the 16-byte grid."""
     rz = (W + H) % 2 == 0
     depth, seen = _depth(kind, W, H, 1, seed=W % 7, rz=rz)
-    ao = _ctx(W, H, 1, reversed_z=rz, intensity=1.1)
+    ao = harness.context(W, H, device=0, layers=1, reversed_z=rz, intensity=1.1)
     d, a = _views(torch_cuda, depth, drow=pitch, arow=_up(W, 256) + (3 if W == 250 else 0))
     _check_frame(torch_cuda, ao, depth, seen, kind, d, a, reversed_z=rz, intensity=1.1)
 
@@ -122,7 +113,7 @@ def test_sub_rectangle_and_no_graph(torch_cuda):
     W, H = 640, 360
     depth, seen = _depth("f32", W, H, 1, seed=3)
     for use_graph in (True, False):
-        ao = _ctx(W, H, 1, use_graph=use_graph)
+        ao = harness.context(W, H, device=0, layers=1, use_graph=use_graph)
         d, a = _views(torch_cuda, depth, drow=4096, dbase=4, arow=1024, abase=1)
         _check_frame(torch_cuda, ao, depth, seen, "f32", d, a)
 
@@ -132,7 +123,7 @@ def test_layered_dynamic_resolution_corner(torch_cuda, L):
     """[L, Hmax, Wmax][:, :H, :W]: the layer pitch is the max-size image; premin on level 1."""
     W, H, Wmax, Hmax = 600, 330, 800, 450
     depth, seen = _depth("f32", W, H, L, seed=L)
-    ao = _ctx(W, H, L, high_quality_mask=1)
+    ao = harness.context(W, H, device=0, layers=L, high_quality_mask=1)
     d, a = _views(torch_cuda, depth, drow=Wmax * 4, dlayer=Hmax * Wmax * 4, arow=Wmax, alayer=Hmax * Wmax)
     _check_frame(torch_cuda, ao, depth, seen, "f32", d, a, high_quality_mask=1)
 
@@ -140,7 +131,7 @@ def test_layered_dynamic_resolution_corner(torch_cuda, L):
 def test_layered_1080p_d16_odd_layer_pitch(torch_cuda):
     W, H = 1920, 1080
     depth, seen = _depth("d16", W, H, 2, seed=9)
-    ao = _ctx(W, H, 2)
+    ao = harness.context(W, H, device=0, layers=2)
     d, a = _views(torch_cuda, depth, drow=4096, dlayer=4096 * H + 2, arow=2048, alayer=2048 * H + 4)
     _check_frame(torch_cuda, ao, depth, seen, "d16", d, a, oracle=False)
 
@@ -151,12 +142,12 @@ def test_row_band_contexts(torch_cuda):
     lib = N.lib()
     W, H = 320, 240
     depth, seen = _depth("f32", W, H, 1, seed=5)
-    ao = _ctx(W, H, 1)
+    ao = harness.context(W, H, device=0, layers=1)
     ao.LateUpdate()
     ao.set_row_band(0, H, -1, -1)
     d, a = _views(torch_cuda, depth, drow=2048, arow=512)
     _check_frame(torch_cuda, ao, depth, seen, "f32", d, a)
-    big = _ctx(1280, 1088, 1)
+    big = harness.context(1280, 1088, device=0, layers=1)
     big.LateUpdate()
     big.set_row_band(0, 544, -1, 1088)
     dep, _ = _depth("f32", 1280, 544, 1)
@@ -175,8 +166,8 @@ def test_graph_key_holds_the_pitches(torch_cuda):
     torch = torch_cuda
     W, H = 128, 96
     depth, seen = _depth("f32", W, H, 1, seed=7)
-    ref = _oracle(W, H).run(seen[0])
-    ao = _ctx(W, H, 1)
+    ref = harness.oracle(W, H, threads=8).run(seen[0])
+    ao = harness.context(W, H, device=0, layers=1)
     ao.LateUpdate()
     maxp = W * 4 + 16 * 80
     dbuf = torch.full(((H - 1) * maxp // 4 + W + 64,), float("nan"), dtype=torch.float32, device="cuda")
@@ -204,8 +195,8 @@ def test_event_binding_and_debug_buffer(torch_cuda):
     lib = N.lib()
     W, H = 300, 170
     depth, seen = _depth("f32", W, H, 1, seed=60)
-    ref = _oracle(W, H).run(seen[0])
-    ao = _ctx(W, H, 1)
+    ref = harness.oracle(W, H, threads=8).run(seen[0])
+    ao = harness.context(W, H, device=0, layers=1)
     ao.LateUpdate()
     d, a = _views(torch_cuda, depth, drow=2048, arow=512)
     stream = C.c_void_p(torch_cuda.cuda.current_stream().cuda_stream)
@@ -233,7 +224,7 @@ def test_refusals_launch_nothing(torch_cuda):
     lib = N.lib()
     torch = torch_cuda
     W, H = 160, 96
-    ao = _ctx(W, H, 1)
+    ao = harness.context(W, H, device=0, layers=1)
     ao.LateUpdate()
     buf = torch.zeros(1 << 22, dtype=torch.uint8, device="cuda")
     p = buf.data_ptr()
@@ -272,7 +263,7 @@ def test_refusals_launch_nothing(torch_cuda):
     for c in cases:
         check(ao, *c)
     # layered: overlapping layers are refused; with one layer the layer pitches are unused (0 is fine)
-    lay = _ctx(W, H, 2)
+    lay = harness.context(W, H, device=0, layers=2)
     lay.LateUpdate()
     check(lay, "depth layers overlap", dp, 640, 640 * (H - 1) + 636, 0, ap, W, W * H, b"depth_layer_pitch")
     check(lay, "depth layer pitch between two elements", dp, 640, 640 * H + 2, 0, ap, W, W * H, b"depth_layer_pitch")
@@ -290,7 +281,7 @@ def test_python_render_accepts_corner_views(torch_cuda):
     W, H, Wmax, Hmax = 333, 200, 512, 256
     depth, seen = _depth("f32", W, H, 2, seed=2)
     for L in (1, 2):
-        ao = _ctx(W, H, L)
+        ao = harness.context(W, H, device=0, layers=L)
         rt = torch.full((L, Hmax, Wmax), float("nan"), dtype=torch.float32, device="cuda")
         rt[:, :H, :W] = torch.from_numpy(depth[:L]).cuda()
         out_rt = torch.full((L, Hmax, Wmax), SENTINEL, dtype=torch.uint8, device="cuda")
@@ -299,7 +290,7 @@ def test_python_render_accepts_corner_views(torch_cuda):
         assert r.data_ptr() == oview.data_ptr()
         got = out_rt.cpu().numpy()
         for l in range(L):
-            assert np.array_equal(got[l, :H, :W], _oracle(W, H).run(seen[l])), (L, l)
+            assert np.array_equal(got[l, :H, :W], harness.oracle(W, H, threads=8).run(seen[l])), (L, l)
         mask = np.ones(got.shape, bool)
         mask[:, :H, :W] = False
         assert (got[mask] == SENTINEL).all()
@@ -314,11 +305,11 @@ def test_python_render_one_pixel_wide_transposed_tensor(torch_cuda):
     torch = torch_cuda
     H = 48
     depth, seen = _depth("f32", 1, H, 1, seed=4)
-    ao = _ctx(1, H, 1)
+    ao = harness.context(1, H, device=0, layers=1)
     d = torch.empty(1, H, dtype=torch.float32, device="cuda")
     d.copy_(torch.from_numpy(np.ascontiguousarray(depth[0].T)))
     d = d.t()                                                                 # (H, 1), strides (1, H)
     assert d.shape == (H, 1) and d.stride() == (1, H)
     out = torch.empty(1, H, dtype=torch.uint8, device="cuda").t()
     ao.render(d, out)
-    assert np.array_equal(out.cpu().numpy(), _oracle(1, H).run(seen[0]))
+    assert np.array_equal(out.cpu().numpy(), harness.oracle(1, H, threads=8).run(seen[0]))
