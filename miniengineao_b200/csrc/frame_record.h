@@ -1,5 +1,6 @@
 // frame_record.h -- what a frame's kernels are launched with: the frame state a recorder reads, where the buffers of a size sit in the
-// arena, the TMA maps over them, the argument blocks of the three stages and which launcher runs each stage.  Host code only, with no
+// arena, the TMA maps over them, the argument blocks of the three stages and which launcher runs each stage, and around the frame the
+// debug buffers' table and views and the segments a row band sends to its neighbours.  Host code only, with no
 // CUDA runtime call: meao_api.cu records its frames with it, and tests/emu/frame_driver.cpp runs the host-compiled kernels with it
 // (-DMEAO_EMULATE), so the CPU tests launch the kernels exactly as libmeao does.
 #ifndef MEAO_FRAME_RECORD_H
@@ -408,6 +409,79 @@ inline cudaError_t launch_entry(const FrameState &f, const FrameLaunch &l, const
         default:
             return launch_upsample(f, l.level, upsample_args(f, l.level, final_level ? io.ao : nullptr, final_level ? io.vp : nullptr),
                                    io.aio, io.fused ? &io.depth : nullptr, s);
+    }
+}
+
+// ---- the debug buffers (meao_get_buffer, meao_set_buffer, meao_debug_view) ---------------------------------------------------
+// Buffer `id` (include/meao.h MEAO_BUF_*, 1..21) of a frame: its reference layout (slices x lh[level] x lw[level] elements of elem
+// bytes per layer) and where layer 0 of it sits in the arena, every layer `layer` bytes after the one before.  TiledDepth<k> (16 slices
+// of level k + 2) exists only as a view of LowDepth<k>, so its base, pitch and layer are LowDepth<k>'s.  Without an arena: null base.
+struct BufferRef { int level, slices, elem; char *base; size_t pitch, layer; };
+
+inline bool buffer_ref(const FrameState &f, int id, BufferRef &b)
+{
+    auto ref = [&](int level, int slices, int elem, void *base, size_t pitch, int k) { b = BufferRef{level, slices, elem, (char *)base, pitch, pitch * f.lh[k]}; };
+    if (id == 1) ref(0, 1, 2, f.lin, (size_t)f.lin_pitch * 2, 0);
+    else if (id >= 2 && id <= 5) { const int k = id - 1; ref(k, 1, 4, f.low[k], (size_t)f.low_pitch[k] * 4, k); }
+    else if (id >= 6 && id <= 9) { const int k = id - 5; ref(k + 2, 16, 2, f.low[k], (size_t)f.low_pitch[k] * 4, k); }
+    else if (id >= 10 && id <= 13) { const int k = id - 9; ref(k, 1, 1, f.occ[k], f.occ_pitch[k], k); }
+    else if (id >= 14 && id <= 16) { const int k = id - 13; ref(k, 1, 1, f.comb[k], f.occ_pitch[k], k); }
+    else if (id == 17) ref(0, 1, 1, f.result, f.result_pitch, 0);
+    else if (id >= 18 && id <= 21) { const int k = id - 17; ref(k, 1, 1, f.hq[k], f.occ_pitch[k], k); }    // HighQuality1..4 (extension)
+    else return false;
+    return true;
+}
+
+// TiledDepth<k> of layer l in the reference layout (16 slices of lw[k + 2] x lh[k + 2] f16) into out, synthesised from LowDepth<k> with
+// the layer's atlas padding for depth kind `kind`
+inline cudaError_t launch_tiled_atlas(const FrameState &f, int k, int l, int kind, __half *out, cudaStream_t s)
+{
+    return launch_synth_tiled(f.low[k] + (size_t)l * f.lh[k] * f.low_pitch[k], f.lw[k], f.lh[k], f.low_pitch[k], f.lw[k + 2], f.lh[k + 2],
+                              layer_pad(f, l, k, kind), out, s);
+}
+
+// The debug view of layer l of buffer `id` into the W x H R8 image at out: TiledDepth<k> through Blit.shader pass 4 (AO.cs:810-814)
+// with the layer's atlas padding for depth kind `kind`, every other buffer point-sampled (AO.cs:815-819).  false: no such buffer.
+inline bool debug_view_args(const FrameState &f, int id, int l, int kind, uint8_t *out, DebugViewArgs &a)
+{
+    BufferRef b;
+    if (!buffer_ref(f, id, b)) return false;
+    a = DebugViewArgs{};
+    a.W = f.W; a.H = f.H; a.out = out; a.out_pitch = f.W;
+    a.src = b.base + (size_t)l * b.layer;
+    a.sw = f.lw[b.level]; a.sh = f.lh[b.level];
+    if (b.slices == 16) {
+        const int k = b.level - 2;
+        a.tiled = 1; a.elem = 4; a.spitch = f.low_pitch[k]; a.lw = f.lw[k]; a.lh = f.lh[k]; a.pad = layer_pad(f, l, k, kind);
+    } else {
+        a.elem = b.elem; a.spitch = (int)(b.pitch / b.elem);
+    }
+    return true;
+}
+
+// ---- row bands: what moves between neighbouring bands -------------------------------------------------------------------------
+// The halo message of one side (meao_halo_pack): rows[k] of LowDepth<k>, level 1 first, in tight rows from `packed` on.  Appends one
+// segment per non-empty level to a: pack copies the arena into the message, unpack the message into the arena.
+inline void halo_segments(const FrameState &f, const Range rows[5], float *packed, bool pack, HaloArgs &a)
+{
+    for (int k = 1; k <= 4; k++) {
+        const int n = rows[k].hi - rows[k].lo;
+        if (n <= 0) continue;
+        float *buf = f.low[k] + (size_t)rows[k].lo * f.low_pitch[k];
+        a.seg[a.nseg++] = pack ? HaloSeg{buf, packed, f.low_pitch[k], f.lw[k], f.lw[k], n} : HaloSeg{packed, buf, f.lw[k], f.low_pitch[k], f.lw[k], n};
+        packed += (size_t)n * f.lw[k];
+    }
+}
+
+// The neighbour exchange towards `side` (band_exchange_kernel): rows[k] of LowDepth<k> go to the same byte offset in the neighbour's
+// arena at `peer`, laid out like the local one at `arena`.  Whole pitched rows, so each level is one contiguous, 128-byte aligned copy.
+inline void exchange_segments(const FrameState &f, const char *arena, char *peer, int side, const Range rows[5], XchgArgs &a)
+{
+    for (int k = 1; k <= 4; k++) {
+        const int n = rows[k].hi - rows[k].lo;
+        if (n <= 0) continue;
+        const size_t off = (size_t)((const char *)(f.low[k] + (size_t)rows[k].lo * f.low_pitch[k]) - arena);
+        a.seg[a.nseg++] = XchgSeg{(const uint4 *)(arena + off), (uint4 *)(peer + off), (uint32_t)((size_t)n * f.low_pitch[k] * sizeof(float) / 16), side};
     }
 }
 

@@ -365,21 +365,24 @@ BandNeeds compute_needs(const MeaoCtx *c, int b0, int b1)
     return n;
 }
 
+// A band's LowDepth rows beyond its own come from its neighbours, so its halo may reach into the band above (starting at row prev0,
+// -1: none) and the band below (ending at row next1, -1: none) but not past them.
+int check_halo_reach(MeaoCtx *c, const BandNeeds &n, int prev0, int next1)
+{
+    for (int k = 1; k <= 4; k++) {
+        if (n.need_low[k].lo < n.own_low[k].lo && (prev0 < 0 || n.need_low[k].lo < (prev0 >> k)))
+            return fail(c, MEAO_ERR_UNSUPPORTED, "halo of level %d reaches beyond the band above", k);
+        if (n.need_low[k].hi > n.own_low[k].hi && (next1 < 0 || n.need_low[k].hi > ((next1 + (1 << k) - 1) >> k)))
+            return fail(c, MEAO_ERR_UNSUPPORTED, "halo of level %d reaches beyond the band below", k);
+    }
+    return 0;
+}
+
 int setup_band(MeaoCtx *c)
 {
     BandNeeds n = compute_needs(c, c->band0, c->band1);
     for (int k = 0; k <= 4; k++) { c->need_c[k] = n.need_c[k]; c->need_low[k] = n.need_low[k]; c->own_low[k] = n.own_low[k]; }
-    for (int k = 1; k <= 4; k++) {
-        if (c->need_low[k].lo < c->own_low[k].lo) {
-            if (c->prev0 < 0 || c->need_low[k].lo < (c->prev0 >> k))
-                return fail(c, MEAO_ERR_UNSUPPORTED, "halo of level %d reaches beyond the band above", k);
-        }
-        if (c->need_low[k].hi > c->own_low[k].hi) {
-            if (c->next1 < 0 || c->need_low[k].hi > ((c->next1 + (1 << k) - 1) >> k))
-                return fail(c, MEAO_ERR_UNSUPPORTED, "halo of level %d reaches beyond the band below", k);
-        }
-    }
-    return 0;
+    return check_halo_reach(c, n, c->prev0, c->next1);
 }
 
 // The size the arena is laid out for: the reservation, or the current size
@@ -663,31 +666,16 @@ int record_frame(MeaoCtx *c, const FrameIO &io, cudaStream_t s, size_t first, bo
     return 0;
 }
 
-int buffer_info(const MeaoCtx *c, int id, int *lvl, int *slices, int *elem)
+// Before a debug read of buffer `id` on stream s: when the last frame stored its AO elsewhere (the caller's buffer or array), the
+// context's own AO texture is regenerated from the still resident Combined1 / LowDepth1 / LinearDepth with the same kernel.  A debug
+// read is not a frame: the launch count stays.
+int own_ao(MeaoCtx *c, int id, cudaStream_t s)
 {
-    if (id == 1) { *lvl = 0; *slices = 1; *elem = 2; }
-    else if (id >= 2 && id <= 5) { *lvl = id - 1; *slices = 1; *elem = 4; }
-    else if (id >= 6 && id <= 9) { *lvl = id - 5 + 2; *slices = 16; *elem = 2; }
-    else if (id >= 10 && id <= 13) { *lvl = id - 9; *slices = 1; *elem = 1; }
-    else if (id >= 14 && id <= 16) { *lvl = id - 13; *slices = 1; *elem = 1; }
-    else if (id == 17) { *lvl = 0; *slices = 1; *elem = 1; }
-    else if (id >= 18 && id <= 21) { *lvl = id - 17; *slices = 1; *elem = 1; }      // HighQuality1..4 (extension)
-    else return -1;
-    (void)c;
-    return 0;
-}
-
-// device pointer + pitch (bytes) of a non-tiled buffer
-int buffer_ptr(MeaoCtx *c, int id, void **p, size_t *pitch_bytes)
-{
-    if (id == 1) { *p = c->lin; *pitch_bytes = (size_t)c->lin_pitch * 2; }
-    else if (id >= 2 && id <= 5) { *p = c->low[id - 1]; *pitch_bytes = (size_t)c->low_pitch[id - 1] * 4; }
-    else if (id >= 10 && id <= 13) { *p = c->occ[id - 9]; *pitch_bytes = c->occ_pitch[id - 9]; }
-    else if (id >= 14 && id <= 16) { *p = c->comb[id - 13]; *pitch_bytes = c->occ_pitch[id - 13]; }
-    else if (id == 17) { *p = c->result; *pitch_bytes = c->result_pitch; }
-    else if (id >= 18 && id <= 21) { *p = c->hq[id - 17]; *pitch_bytes = c->occ_pitch[id - 17]; }
-    else return -1;
-    return 0;
+    if (id != MEAO_BUF_AMBIENT_OCCLUSION || !c->last_out) return 0;
+    const int64_t before = c->launches;
+    const int rc = record_upsample(c, 1, nullptr, s);
+    c->launches = before;
+    return rc;
 }
 
 std::mutex g_event_mutex;
@@ -993,16 +981,9 @@ int meao_set_row_band(MeaoCtx *c, int32_t row0, int32_t row1, int32_t prev_row0,
         return fail(c, MEAO_ERR_INVALID, "bad neighbour extents");
     if ((row0 > 0) != (prev_row0 >= 0) || (row1 < c->H) != (next_row1 >= 0))
         return fail(c, MEAO_ERR_INVALID, "neighbour extents must be given exactly where the band is interior");
-    // validate against temporaries; the context keeps its old band when the new one is refused
-    {
-        const BandNeeds n = compute_needs(c, row0, row1);
-        for (int k = 1; k <= 4; k++) {
-            if (n.need_low[k].lo < n.own_low[k].lo && (prev_row0 < 0 || n.need_low[k].lo < (prev_row0 >> k)))
-                return fail(c, MEAO_ERR_UNSUPPORTED, "halo of level %d reaches beyond the band above", k);
-            if (n.need_low[k].hi > n.own_low[k].hi && (next_row1 < 0 || n.need_low[k].hi > ((next_row1 + (1 << k) - 1) >> k)))
-                return fail(c, MEAO_ERR_UNSUPPORTED, "halo of level %d reaches beyond the band below", k);
-        }
-    }
+    // validated before anything changes: the context keeps its old band when the new one is refused
+    int rc = check_halo_reach(c, compute_needs(c, row0, row1), prev_row0, next_row1);
+    if (rc) return rc;
     if (!c->plan_only) {
         CUDA_TRY(c, cudaSetDevice(c->device));
         drop_graph(c);
@@ -1072,15 +1053,12 @@ static int halo_copy(MeaoCtx *c, int side, void *packed, bool pack, void *stream
     if (side != 0 && side != 1) return fail(c, MEAO_ERR_INVALID, "side must be 0 or 1");
     cudaStream_t s = (cudaStream_t)stream;
     Range r[5]; halo_ranges(c, side, pack, r);
-    char *p = (char *)packed;
-    for (int k = 1; k <= 4; k++) {
-        const int rows = r[k].hi - r[k].lo;
-        if (rows <= 0) continue;
-        const size_t wb = (size_t)c->lw[k] * 4, pb = (size_t)c->low_pitch[k] * 4;
-        char *buf = (char *)(c->low[k] + (size_t)r[k].lo * c->low_pitch[k]);
-        if (pack) CUDA_TRY(c, cudaMemcpy2DAsync(p, wb, buf, pb, wb, rows, cudaMemcpyDeviceToDevice, s));
-        else      CUDA_TRY(c, cudaMemcpy2DAsync(buf, pb, p, wb, wb, rows, cudaMemcpyDeviceToDevice, s));
-        p += wb * rows;
+    HaloArgs a{};
+    halo_segments(*c, r, (float *)packed, pack, a);
+    for (int i = 0; i < a.nseg; i++) {                  // copies, not halo_copy_kernel: no kernel launch
+        const HaloSeg &g = a.seg[i];
+        CUDA_TRY(c, cudaMemcpy2DAsync(g.dst, (size_t)g.dst_pitch * sizeof(float), g.src, (size_t)g.src_pitch * sizeof(float),
+                                      (size_t)g.width * sizeof(float), g.rows, cudaMemcpyDeviceToDevice, s));
     }
     return MEAO_OK;
 }
@@ -1104,21 +1082,12 @@ int meao_render_band_finish(MeaoCtx *c, void *ao_out, void *stream)
 
 static int halo_kernel(MeaoCtx *c, void *up, void *down, bool pack, cudaStream_t s)
 {
-    HaloArgs a{}; a.nseg = 0;
+    HaloArgs a{};
     void *bufs[2] = {up, down};
     for (int side = 0; side < 2; side++) {
         if (!bufs[side]) continue;
         Range r[5]; halo_ranges(c, side, pack, r);
-        float *p = (float *)bufs[side];
-        for (int k = 1; k <= 4; k++) {
-            const int rows = r[k].hi - r[k].lo;
-            if (rows <= 0) continue;
-            float *buf = c->low[k] + (size_t)r[k].lo * c->low_pitch[k];
-            HaloSeg &g = a.seg[a.nseg++];
-            if (pack) g = HaloSeg{buf, p, c->low_pitch[k], c->lw[k], c->lw[k], rows};
-            else      g = HaloSeg{p, buf, c->lw[k], c->low_pitch[k], c->lw[k], rows};
-            p += (size_t)rows * c->lw[k];
-        }
+        halo_segments(*c, r, (float *)bufs[side], pack, a);
     }
     CUDA_TRY(c, launch_halo_copy(a, s));
     if (a.nseg) c->launches++;
@@ -1354,7 +1323,7 @@ int meao_band_connect(MeaoCtx *c, int32_t side, const MeaoPeerHandle *peer)
 static int record_exchange(MeaoCtx *c, cudaStream_t s)
 {
     NvtxRange nv("meao::band_exchange");
-    XchgArgs a{}; a.nseg = 0;
+    XchgArgs a{};
     a.local = c->band_flags;
     a.host_error = c->host_error_dev;
     a.timeout_ns = c->band_timeout_ns;
@@ -1362,16 +1331,7 @@ static int record_exchange(MeaoCtx *c, cudaStream_t s)
         a.peer[side] = (BandFlags *)c->peer_base[side];                 // BandFlags sit at offset 0 of every arena
         if (!c->peer_base[side]) continue;
         Range r[5]; halo_ranges(c, side, true, r);
-        for (int k = 1; k <= 4; k++) {
-            const int rows = r[k].hi - r[k].lo;
-            if (rows <= 0) continue;
-            const size_t off = (size_t)((char *)(c->low[k] + (size_t)r[k].lo * c->low_pitch[k]) - (char *)c->arena);
-            const size_t bytes = (size_t)rows * c->low_pitch[k] * sizeof(float);          // whole pitched rows: contiguous, 128 B aligned
-            XchgSeg &g = a.seg[a.nseg++];
-            g.src = (const uint4 *)((char *)c->arena + off);
-            g.dst = (uint4 *)((char *)c->peer_base[side] + off);
-            g.n16 = (uint32_t)(bytes / 16); g.side = side;
-        }
+        exchange_segments(*c, (const char *)c->arena, (char *)c->peer_base[side], side, r, a);
     }
     if (a.nseg == 0) return 0;
     CUDA_TRY(c, launch_band_exchange(a, s));
@@ -1409,8 +1369,7 @@ int meao_band_step_host(MeaoCtx *c, const void *depth_host, int32_t kind, uint8_
     if (kind < MEAO_DEPTH_RAW_F32 || kind > MEAO_DEPTH_RAW_D24S8) return fail(c, MEAO_ERR_INVALID, "bad depth kind %d", kind);
     const size_t rows = (size_t)(c->band1 - c->band0);
     cudaStream_t s = c->slot_stream[0];
-    const size_t esz = (kind == MEAO_DEPTH_RAW_D16_UNORM) ? 2 : 4;
-    CUDA_TRY(c, cudaMemcpyAsync(c->depth_stage[0], depth_host, rows * c->W * esz, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(c, cudaMemcpyAsync(c->depth_stage[0], depth_host, rows * c->W * depth_esize(kind), cudaMemcpyHostToDevice, s));
     if ((rc = meao_band_step(c, c->depth_stage[0], kind, c->ao_stage[0], s))) return rc;
     CUDA_TRY(c, cudaMemcpyAsync(ao_host, c->ao_stage[0], rows * c->W, cudaMemcpyDeviceToHost, s));
     return MEAO_OK;
@@ -1637,8 +1596,7 @@ int meao_render_host_async(MeaoCtx *c, const void *depth_host, int32_t kind, uin
     if (slot != 0 && slot != 1) return fail(c, MEAO_ERR_INVALID, "slot must be 0 or 1");
     const size_t rows = (size_t)(c->band1 - c->band0) * c->layers;      // layered: L images of H rows (no band)
     cudaStream_t s = c->slot_stream[slot];
-    const size_t esz = (kind == MEAO_DEPTH_RAW_D16_UNORM) ? 2 : 4;
-    CUDA_TRY(c, cudaMemcpyAsync(c->depth_stage[slot], depth_host, rows * c->W * esz, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(c, cudaMemcpyAsync(c->depth_stage[slot], depth_host, rows * c->W * depth_esize(kind), cudaMemcpyHostToDevice, s));
     // the two slots share the context's intermediates: kernels of consecutive frames are serialised, copies are not
     if (c->compute_done_valid) CUDA_TRY(c, cudaStreamWaitEvent(s, c->compute_done, 0));
     if ((rc = meao_render(c, c->depth_stage[slot], kind, c->ao_stage[slot], s))) return rc;
@@ -1714,45 +1672,34 @@ int meao_stage_upsample(MeaoCtx *c, int32_t lo_level, void *ao_out, void *stream
 int meao_buffer_desc(const MeaoCtx *c, int32_t id, MeaoBufferDesc *out)
 {
     if (!c || !out || c->W <= 0) return MEAO_ERR_INVALID;
-    int lvl, slices, elem;
-    if (buffer_info(c, id, &lvl, &slices, &elem)) return MEAO_ERR_INVALID;
-    out->width = c->lw[lvl]; out->height = c->lh[lvl]; out->slices = slices; out->elem_bytes = elem;
+    BufferRef b;
+    if (!buffer_ref(*c, id, b)) return MEAO_ERR_INVALID;
+    out->width = c->lw[b.level]; out->height = c->lh[b.level]; out->slices = b.slices; out->elem_bytes = b.elem;
     return MEAO_OK;
 }
 
 int meao_get_buffer(MeaoCtx *c, int32_t id, void *host_out, size_t host_bytes)
 {
     int rc = frame_ready(c, c->stream); if (rc) return rc;
-    int lvl, slices, elem;
-    if (!host_out || buffer_info(c, id, &lvl, &slices, &elem)) return fail(c, MEAO_ERR_INVALID, "bad buffer id %d", id);
-    const size_t one = (size_t)c->lw[lvl] * c->lh[lvl] * slices * elem, need = one * c->layers;     // [L][reference layout]
+    BufferRef b;
+    if (!host_out || !buffer_ref(*c, id, b)) return fail(c, MEAO_ERR_INVALID, "bad buffer id %d", id);
+    const size_t wb = (size_t)c->lw[b.level] * b.elem, one = wb * c->lh[b.level] * b.slices, need = one * c->layers;     // [L][reference layout]
     if (host_bytes < need) return fail(c, MEAO_ERR_INVALID, "buffer %d needs %zu bytes, got %zu", id, need, host_bytes);
     CUDA_TRY(c, cudaDeviceSynchronize());     // debug path: frames may be in flight on any caller stream
-    if (slices == 16) {
-        const int k = id - 5;
+    if (b.slices == 16) {
         __half *tmp = nullptr;
         CUDA_TRY(c, cudaMalloc(&tmp, need));
         cudaError_t e = cudaSuccess;
         for (int l = 0; l < c->layers && e == cudaSuccess; l++)
-            e = launch_synth_tiled(c->low[k] + (size_t)l * c->lh[k] * c->low_pitch[k], c->lw[k], c->lh[k], c->low_pitch[k], c->lw[k + 2], c->lh[k + 2],
-                                   layer_pad(*c, l, k, c->last_kind), (__half *)((char *)tmp + l * one), c->stream);
+            e = launch_tiled_atlas(*c, b.level - 2, l, c->last_kind, (__half *)((char *)tmp + l * one), c->stream);
         if (e == cudaSuccess) e = cudaMemcpyAsync(host_out, tmp, need, cudaMemcpyDeviceToHost, c->stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
         cudaFree(tmp);
         if (e != cudaSuccess) return fail(c, MEAO_ERR_CUDA, "tiled view: %s", cudaGetErrorString(e));
         return MEAO_OK;
     }
-    void *p; size_t pitch;
-    buffer_ptr(c, id, &p, &pitch);
-    const size_t wb = (size_t)c->lw[lvl] * elem;
-    if (id == MEAO_BUF_AMBIENT_OCCLUSION && c->last_out) {
-        // the last frame wrote the AO texture straight into the caller's buffer; regenerate the debug view
-        // from the (still resident) Combined1 / LowDepth1 / LinearDepth with the same kernel
-        const int64_t before = c->launches;
-        if ((rc = record_upsample(c, 1, nullptr, c->stream))) return rc;
-        c->launches = before;
-    }
-    CUDA_TRY(c, cudaMemcpy2DAsync(host_out, wb, p, pitch, wb, (size_t)c->lh[lvl] * c->layers, cudaMemcpyDeviceToHost, c->stream));
+    if ((rc = own_ao(c, id, c->stream))) return rc;
+    CUDA_TRY(c, cudaMemcpy2DAsync(host_out, wb, b.base, b.pitch, wb, (size_t)c->lh[b.level] * c->layers, cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     return MEAO_OK;
 }
@@ -1760,36 +1707,15 @@ int meao_get_buffer(MeaoCtx *c, int32_t id, void *host_out, size_t host_bytes)
 int meao_debug_view(MeaoCtx *c, int32_t id, void *out, void *stream)
 {
     int rc = frame_ready(c, (cudaStream_t)stream); if (rc) return rc;
-    int lvl, slices, elem;
-    if (!out || buffer_info(c, id, &lvl, &slices, &elem)) return fail(c, MEAO_ERR_INVALID, "bad buffer id %d / out is NULL", id);
+    BufferRef b;
+    if (!out || !buffer_ref(*c, id, b)) return fail(c, MEAO_ERR_INVALID, "bad buffer id %d / out is NULL", id);
     if (c->band0 != 0 || c->band1 != c->H) return fail(c, MEAO_ERR_UNSUPPORTED, "debug views need a whole-frame context (no row band)");
     cudaStream_t s = (cudaStream_t)stream;
-    DebugViewArgs a{};
-    a.W = c->W; a.H = c->H; a.out = (uint8_t *)out; a.out_pitch = c->W;
-    if (slices == 16) {                                             // AO.cs:810-814: Blit.shader pass 4
-        const int k = id - 5;
-        a.tiled = 1; a.src = c->low[k]; a.elem = 4; a.spitch = c->low_pitch[k];
-        a.sw = c->lw[k + 2]; a.sh = c->lh[k + 2]; a.lw = c->lw[k]; a.lh = c->lh[k];
-        a.pad = layer_pad(*c, 0, k, c->last_kind);
-    } else {                                                        // AO.cs:815-819
-        if (id == MEAO_BUF_AMBIENT_OCCLUSION && c->last_out) {
-            // the last frame wrote the AO texture straight into the caller's buffer: regenerate the context's own copy
-            const int64_t before = c->launches;
-            if ((rc = record_upsample(c, 1, nullptr, s))) return rc;
-            c->launches = before;
-        }
-        void *p; size_t pitch;
-        buffer_ptr(c, id, &p, &pitch);
-        a.src = p; a.elem = elem; a.spitch = (int)(pitch / elem); a.sw = c->lw[lvl]; a.sh = c->lh[lvl];
-    }
-    // layered: L images, each from its own layer of the source
-    const size_t src_layer = (slices == 16 ? (size_t)c->lh[id - 5] * c->low_pitch[id - 5] * 4 : (size_t)a.sh * a.spitch * a.elem);
-    for (int l = 0; l < c->layers; l++) {
-        DebugViewArgs al = a;
-        al.src = (const char *)a.src + l * src_layer;
-        al.out = a.out + (size_t)l * c->W * c->H;
-        if (slices == 16) al.pad = layer_pad(*c, l, id - 5, c->last_kind);     // the layer's camera
-        CUDA_TRY(c, launch_debug_view(al, s));
+    if ((rc = own_ao(c, id, s))) return rc;
+    for (int l = 0; l < c->layers; l++) {                           // layered: L images, each from its own layer of the source
+        DebugViewArgs a;
+        debug_view_args(*c, id, l, c->last_kind, (uint8_t *)out + (size_t)l * c->W * c->H, a);
+        CUDA_TRY(c, launch_debug_view(a, s));
         c->launches++;
     }
     return MEAO_OK;
@@ -1798,16 +1724,13 @@ int meao_debug_view(MeaoCtx *c, int32_t id, void *out, void *stream)
 int meao_set_buffer(MeaoCtx *c, int32_t id, const void *host_in, size_t host_bytes)
 {
     int rc = ensure_ready(c); if (rc) return rc;
-    int lvl, slices, elem;
-    if (!host_in || buffer_info(c, id, &lvl, &slices, &elem) || slices != 1)
+    BufferRef b;
+    if (!host_in || !buffer_ref(*c, id, b) || b.slices != 1)
         return fail(c, MEAO_ERR_INVALID, "buffer id %d cannot be set", id);
-    const size_t need = (size_t)c->lw[lvl] * c->lh[lvl] * elem * c->layers;      // [L][h][w]
+    const size_t wb = (size_t)c->lw[b.level] * b.elem, need = wb * c->lh[b.level] * c->layers;      // [L][h][w]
     if (host_bytes < need) return fail(c, MEAO_ERR_INVALID, "buffer %d needs %zu bytes, got %zu", id, need, host_bytes);
-    void *p; size_t pitch;
-    buffer_ptr(c, id, &p, &pitch);
-    const size_t wb = (size_t)c->lw[lvl] * elem;
     CUDA_TRY(c, cudaDeviceSynchronize());
-    CUDA_TRY(c, cudaMemcpy2DAsync(p, pitch, host_in, wb, wb, (size_t)c->lh[lvl] * c->layers, cudaMemcpyHostToDevice, c->stream));
+    CUDA_TRY(c, cudaMemcpy2DAsync(b.base, b.pitch, host_in, wb, wb, (size_t)c->lh[b.level] * c->layers, cudaMemcpyHostToDevice, c->stream));
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     return MEAO_OK;
 }

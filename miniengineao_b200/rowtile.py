@@ -138,13 +138,8 @@ class _null_ctx:
         return False
 
 
-def halo_slices(rows: list[tuple[int, int]], widths: list[int]) -> list[tuple[int, int, int]]:
-    """[(level, lo, hi)] with element offsets implied by order: level 1 first, rows tightly packed (the layout of
-    meao_halo_pack).  Used by the CPU (gloo) test to pack / unpack numpy buffers exactly like the C side."""
-    return [(k + 1, lo, hi) for k, (lo, hi) in enumerate(rows) if hi > lo and widths[k] > 0]
-
-
 def pack_rows(low: dict[int, np.ndarray], rows: list[tuple[int, int]]) -> np.ndarray:
+    """The message meao_halo_pack sends: rows[k - 1] of level k, level 1 first, rows tightly packed."""
     parts = [low[k + 1][lo:hi].reshape(-1) for k, (lo, hi) in enumerate(rows) if hi > lo]
     return np.concatenate(parts).astype(np.float32) if parts else np.zeros(0, np.float32)
 

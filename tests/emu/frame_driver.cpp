@@ -1,6 +1,7 @@
 // frame_driver.cpp -- runs frames through the HOST-compiled kernel sources (TEST INFRASTRUCTURE ONLY, see cuda_emu.h), launched the
-// way libmeao launches them: buffer placement, TMA maps, the frame schedule, argument blocks and launcher choice all come from
-// csrc/frame_record.h, the code meao_api.cu records its frames with.  What this driver adds is a host arena, the plan (the constants a
+// way libmeao launches them: buffer placement, TMA maps, the frame schedule, argument blocks and launcher choice, and the buffer
+// table, debug views, halo and exchange segments around the frame, all come from csrc/frame_record.h, the code meao_api.cu records
+// its frames and serves its debug reads and row bands with.  What this driver adds is a host arena, the plan (the constants a
 // plan-only libmeao context reports, handed in by the test) and what each frame form puts into its first and last launch.
 #include <algorithm>
 #include <cstdio>
@@ -213,47 +214,39 @@ void frame_band_phase_a(void *h, const void *depth_band, int kind) { run_schedul
 // the launches after the prepare into the result buffer, like meao_band_phase_b and meao_render_band_finish
 void frame_band_phase_b(void *h) { run_schedule(F(h), frame_io(F(h), nullptr, F(h)->kind), 1); }
 
-// rows8 = meao_halo_rows(side, send): {lo1,hi1, ..., lo4,hi4}; packed message layout of meao_halo_pack (level 1 first, tight rows)
+// rows8 = meao_halo_rows(side, send): {lo1,hi1, ..., lo4,hi4}, as the rows[k] of LowDepth<k> frame_record.h's segment builders take
+static void halo_rows(const int *rows8, Range rows[5])
+{
+    rows[0] = Range{0, 0};
+    for (int k = 1; k <= 4; k++) rows[k] = Range{rows8[2 * (k - 1)], rows8[2 * (k - 1) + 1]};
+}
+
+// meao_halo_pack / meao_halo_unpack of the side rows8 describes, through the segments of meao_band_phase_a / _b's halo_copy_kernel
 void frame_halo(void *h, const int *rows8, float *packed, int pack)
 {
-    Frame *f = F(h);
-    HaloArgs a{}; a.nseg = 0;
-    float *p = packed;
-    for (int k = 1; k <= 4; k++) {
-        const int lo = rows8[2 * (k - 1)], rows = rows8[2 * (k - 1) + 1] - lo;
-        if (rows <= 0) continue;
-        float *buf = f->low[k] + (size_t)lo * f->low_pitch[k];
-        HaloSeg &g = a.seg[a.nseg++];
-        if (pack) g = HaloSeg{buf, p, f->low_pitch[k], f->lw[k], f->lw[k], rows};
-        else      g = HaloSeg{p, buf, f->lw[k], f->low_pitch[k], f->lw[k], rows};
-        p += (size_t)rows * f->lw[k];
-    }
+    Range rows[5]; halo_rows(rows8, rows);
+    HaloArgs a{};
+    halo_segments(*F(h), rows, packed, pack != 0, a);
     launch_halo_copy(a, nullptr);
 }
 
-// ---- native neighbour exchange: band_exchange_kernel with the segments meao_api.cu's record_exchange builds (whole pitched rows
-// copied to the same position in the neighbour's LowDepth buffers).  up / down: the neighbours' handles (NULL = none);
-// rows_up8 / rows_down8 = meao_halo_rows(side, send = 1).  The fiber emulator runs one grid at a time, so the test presets the
-// flags a concurrently running neighbour would have written (frame_band_flags).  Returns the kernel's sticky error.
+// ---- native neighbour exchange: band_exchange_kernel with the segments meao_api.cu's record_exchange builds.  up / down: the
+// neighbours' handles (NULL = none), frames of the same size; rows_up8 / rows_down8 = meao_halo_rows(side, send = 1).  The fiber
+// emulator runs one grid at a time, so the test presets the flags a concurrently running neighbour would have written
+// (frame_band_flags).  Returns the kernel's sticky error.
 int frame_band_exchange(void *h, void *up, void *down, const int *rows_up8, const int *rows_down8, int timeout_polls)
 {
     Frame *f = F(h);
     Frame *peer[2] = {F(up), F(down)};
     const int *rows8[2] = {rows_up8, rows_down8};
-    XchgArgs a{}; a.nseg = 0;
+    XchgArgs a{};
     a.local = &f->flags(); a.host_error = &f->host_error;
     a.timeout_ns = (unsigned long long)timeout_polls * 1000ull;       // the emulated global timer advances 1000 "ns" per read
     for (int side = 0; side < 2; side++) {
         if (!peer[side]) continue;
         a.peer[side] = &peer[side]->flags();
-        for (int k = 1; k <= 4; k++) {
-            const int lo = rows8[side][2 * (k - 1)], rows = rows8[side][2 * (k - 1) + 1] - lo;
-            if (rows <= 0) continue;
-            XchgSeg &g = a.seg[a.nseg++];
-            g.src = (const uint4 *)(f->low[k] + (size_t)lo * f->low_pitch[k]);
-            g.dst = (uint4 *)(peer[side]->low[k] + (size_t)lo * f->low_pitch[k]);
-            g.n16 = (uint32_t)((size_t)rows * f->low_pitch[k] * sizeof(float) / 16); g.side = side;
-        }
+        Range rows[5]; halo_rows(rows8[side], rows);
+        exchange_segments(*f, f->arena, peer[side]->arena, side, rows, a);
     }
     launch_band_exchange(a, nullptr);
     return (int)f->flags().error;
@@ -289,44 +282,21 @@ void frame_poison(void *h, int what)
 int frame_get_buffer(void *h, int id, int layer, void *out)
 {
     Frame *f = F(h);
-    if (layer < 0 || layer >= f->layers) return -1;
+    BufferRef b;
+    if (layer < 0 || layer >= f->layers || !buffer_ref(*f, id, b)) return -1;
     if (id == 17 && f->ao_elsewhere)                    // meao_get_buffer: the context's own copy of an AO stored elsewhere
         launch_entry(*f, frame_schedule(f->plan.variants).back(), FrameIO{}, f->ren_tile, nullptr);
-    auto copy2d = [&](const void *src, size_t pitch_bytes, int w, int hgt, int elem) {
-        src = (const char *)src + (size_t)layer * hgt * pitch_bytes;       // layer l starts l x rows x pitch after layer 0
-        for (int y = 0; y < hgt; y++) memcpy((char *)out + (size_t)y * w * elem, (const char *)src + (size_t)y * pitch_bytes, (size_t)w * elem);
-    };
-    if (id == 1) copy2d(f->lin, (size_t)f->lin_pitch * 2, f->lw[0], f->lh[0], 2);
-    else if (id >= 2 && id <= 5) copy2d(f->low[id - 1], (size_t)f->low_pitch[id - 1] * 4, f->lw[id - 1], f->lh[id - 1], 4);
-    else if (id >= 6 && id <= 9) {
-        const int k = id - 5;
-        launch_synth_tiled(f->low[k] + (size_t)layer * f->lh[k] * f->low_pitch[k], f->lw[k], f->lh[k], f->low_pitch[k], f->lw[k + 2], f->lh[k + 2],
-                           layer_pad(*f, layer, k, f->kind), (__half *)out, nullptr);
-    }
-    else if (id >= 10 && id <= 13) copy2d(f->occ[id - 9], f->occ_pitch[id - 9], f->lw[id - 9], f->lh[id - 9], 1);
-    else if (id >= 14 && id <= 16) copy2d(f->comb[id - 13], f->occ_pitch[id - 13], f->lw[id - 13], f->lh[id - 13], 1);
-    else if (id == 17) copy2d(f->result, f->result_pitch, f->lw[0], f->lh[0], 1);
-    else if (id >= 18 && id <= 21) copy2d(f->hq[id - 17], f->occ_pitch[id - 17], f->lw[id - 17], f->lh[id - 17], 1);
-    else return -1;
+    if (b.slices == 16) { launch_tiled_atlas(*f, b.level - 2, layer, f->kind, (__half *)out, nullptr); return 0; }
+    const size_t wb = (size_t)f->lw[b.level] * b.elem;
+    for (int y = 0; y < f->lh[b.level]; y++) memcpy((char *)out + y * wb, b.base + layer * b.layer + y * b.pitch, wb);
     return 0;
 }
 
 // the debug view of buffer <id> of a single-layer frame (meao_debug_view) into out[W * H]
 int frame_debug_view(void *h, int id, uint8_t *out)
 {
-    Frame *f = F(h);
-    DebugViewArgs a{};
-    a.W = f->W; a.H = f->H; a.out = out; a.out_pitch = f->W;
-    if (id >= 6 && id <= 9) {
-        const int k = id - 5;
-        a.tiled = 1; a.src = f->low[k]; a.elem = 4; a.spitch = f->low_pitch[k]; a.sw = f->lw[k + 2]; a.sh = f->lh[k + 2]; a.lw = f->lw[k]; a.lh = f->lh[k];
-        a.pad = layer_pad(*f, 0, k, f->kind);
-    } else if (id == 1) { a.src = f->lin; a.elem = 2; a.spitch = f->lin_pitch; a.sw = f->lw[0]; a.sh = f->lh[0]; }
-    else if (id >= 2 && id <= 5) { a.src = f->low[id - 1]; a.elem = 4; a.spitch = f->low_pitch[id - 1]; a.sw = f->lw[id - 1]; a.sh = f->lh[id - 1]; }
-    else if (id >= 10 && id <= 13) { a.src = f->occ[id - 9]; a.elem = 1; a.spitch = f->occ_pitch[id - 9]; a.sw = f->lw[id - 9]; a.sh = f->lh[id - 9]; }
-    else if (id >= 14 && id <= 16) { a.src = f->comb[id - 13]; a.elem = 1; a.spitch = f->occ_pitch[id - 13]; a.sw = f->lw[id - 13]; a.sh = f->lh[id - 13]; }
-    else if (id == 17) { a.src = f->result; a.elem = 1; a.spitch = f->result_pitch; a.sw = f->lw[0]; a.sh = f->lh[0]; }
-    else return -1;
+    DebugViewArgs a;
+    if (!debug_view_args(*F(h), id, 0, F(h)->kind, out, a)) return -1;
     launch_debug_view(a, nullptr);
     return 0;
 }

@@ -119,7 +119,7 @@ def test_linear_and_native_depth_ingest():
 def test_debug_views():
     W, H = 130, 70
     f, orc = _run(W, H, seed=4, high_quality_mask=0b0101)
-    for bid in range(1, 18):
+    for bid in harness.buffer_ids(high_quality_mask=0b0101):
         assert np.array_equal(f.debug_view(bid), orc.debug_view(bid)), bid
 
 
