@@ -85,6 +85,8 @@ namespace MiniEngineAO
         [DllImport(Lib)] public static extern int meao_composite_debug(IntPtr ctx, IntPtr viewR8Dev, IntPtr colorDev, int colorFormat, IntPtr stream);   // AO.cs:826-829
         [DllImport(Lib)] public static extern int meao_get_buffer(IntPtr ctx, int bufferId, IntPtr hostOut, UIntPtr hostBytes);
         [DllImport(Lib)] public static extern int meao_debug_view(IntPtr ctx, int bufferId, IntPtr outR8Dev, IntPtr stream);   // AO.cs:787-820
+        // frames recorded into the host's own CUDA graph (a render called on a capturing stream) replay only while this is unchanged
+        [DllImport(Lib)] public static extern long meao_frame_generation(IntPtr ctx);
 
         public static void Check(IntPtr ctx, int rc)
         {
@@ -132,6 +134,9 @@ namespace MiniEngineAO
         // (meao_reserve); a size change inside it then costs no allocation, device synchronise, graph teardown or event rebind.
         Vector2Int _maxResolution;
         public Vector2Int MaxResolution { get { return _maxResolution; } set { _maxResolution = value; } }
+        // An engine that records the plugin's frame into a CUDA graph of its own (meao_render on a stream it captures) replays that
+        // graph only while this equals the value read right after the capture, and captures again when it changes (include/meao.h).
+        public long FrameGeneration { get { return _ctx == IntPtr.Zero ? -1 : MeaoNative.meao_frame_generation(_ctx); } }
         int _reservedW, _reservedH;                            // what meao_reserve was last given (doubled width under single-pass stereo)
         int _width, _height;                                   // the size meao_resize was last given
         int _drawCountPerFrame;                                // AmbientOcclusion.cs:289, 349-355: single-pass stereo detection

@@ -36,7 +36,8 @@ extern "C" {
                               *    + meao_set_layers (layered frames; additive, so the version stays 3)
                               *    + meao_render_arrays / meao_bind_event_arrays / meao_release_array (CUDA-array I/O; additive)
                               *    + meao_render_pitched / meao_bind_event_pitched (depth and AO with their own row and layer pitch; additive)
-                              *    + meao_reserve / meao_reservation (dynamic resolution; additive) */
+                              *    + meao_reserve / meao_reservation (dynamic resolution; additive)
+                              *    + meao_frame_generation (frames inside a caller's CUDA graph; additive) */
 
 typedef struct MeaoCtx MeaoCtx;
 
@@ -463,6 +464,42 @@ int meao_bind_event_pitched(MeaoCtx *ctx, int32_t event_id,
                             void *ao_out_dev, int64_t ao_row_pitch, int64_t ao_layer_pitch, void *stream);
 void meao_render_event(int event_id);
 MeaoRenderEventFunc meao_get_render_event_func(void);
+
+/* ---- frames inside a caller's graph ------------------------------------------------------------------------------------------
+ * When the stream an entry point is given is being captured (cudaStreamBeginCapture in any mode, torch.cuda.graph, the graph trees of
+ * torch.compile(mode="reduce-overhead")), the call records its kernel launches straight into that capture: the caller's graph then
+ * holds the frame, and every replay of it runs the frame.  No graph of the context is captured, instantiated or launched, and the
+ * graph cache is neither used nor changed.  A graph-path frame forks to the context's own streams and joins back inside the caller's
+ * capture (cross-stream dependencies of the caller's graph); a MEAO_FLAG_NO_GRAPH frame records its launches serially.  The launches
+ * carry programmatic dependent launch at the level an instantiation of this context has accepted (meao_pdl_level; none before the
+ * first), so a frame recorded into a caller's graph matches the context's own.  The capture status query is the only cost a frame
+ * outside a capture pays for this.
+ * Capturable: meao_render, meao_render_pitched, meao_render_arrays, meao_render_event (any binding), the meao_stage_* calls,
+ * meao_render_band_prepare / _finish, meao_band_phase_a / _b, meao_band_step, meao_halo_pack / _unpack, meao_debug_view and the three
+ * meao_composite_* calls.
+ * SETTLED CONTEXTS ONLY: inside a capture a call may issue nothing but kernel launches.  It is refused with MEAO_ERR_INVALID, records
+ * nothing and leaves the caller's capture valid (meao_last_error says why: "issue one frame outside the capture first") when
+ *   - a structural change is pending (a re-plan synchronises the device),
+ *   - the per-layer camera tables are still to be written: after a frame-constant change, or on the first frame at a size,
+ *   - or, for meao_render_arrays, the context has not rendered with one of the arrays yet (its surface object is made then).
+ * One frame of the same form issued outside the capture settles the context; torch's warm-up before torch.cuda.graph does that.
+ * A capture that has been invalidated returns MEAO_ERR_CUDA and records nothing.
+ * NOT capturable: the host-buffer calls (meao_render_host, _host_async, meao_host_wait, meao_band_step_host; they run on the
+ * context's own streams), meao_get_buffer, meao_set_buffer, meao_release_array, meao_synchronize, meao_band_connect, meao_band_status,
+ * meao_profile_frame and every structural setter (they may allocate or synchronise).  meao_profile_frame returns MEAO_ERR_UNSUPPORTED
+ * while a capture that holds a graph-path frame of this context is open; the others must not be called while one is.  While such a
+ * capture is open, issue this context's frames into that capture only.
+ * REPLAY CONTRACT: a recorded frame replays with the plan, size, buffers, arrays and frame constants it was recorded with -- the
+ * constants are baked into the caller's graph, as every kernel argument of a CUDA graph is (frame constants are live for frames the
+ * context issues itself, not inside a caller's graph).  meao_frame_generation changes whenever anything a recorded frame depends on
+ * changes: a frame constant, a switch of size or size slot (meao_resize), a structural re-plan, an arena re-allocation, a
+ * meao_release_array that released something, meao_band_connect or meao_set_row_band.  It does not change for a setter that changes
+ * nothing, for a refused call, for frames or for replays.  A host may replay a recorded frame only while meao_frame_generation equals
+ * the value it read right after recording; otherwise it re-captures (after one frame outside the capture).  Replaying after a
+ * re-allocation, a resize without a reservation or a release would read and write freed memory.
+ * Counting: meao_launch_count counts a recorded frame's kernels once, when it is recorded (replays of the caller's graph are
+ * invisible to the library); MeaoReservation.graph_instantiations does not move.  Works on plan-only contexts. */
+int64_t meao_frame_generation(const MeaoCtx *ctx);   /* >= 0; MEAO_ERR_INVALID for NULL */
 
 /* ---- introspection ------------------------------------------------------------------------------ */
 int64_t meao_launch_count(const MeaoCtx *ctx);       /* kernels launched (or replayed via graph) so far */

@@ -124,6 +124,7 @@ SIGNATURES = {
     "meao_render_event": (None, [C.c_int]),
     "meao_get_render_event_func": (RENDER_EVENT_FUNC, []),
     "meao_launch_count": (C.c_int64, [C.c_void_p]),
+    "meao_frame_generation": (C.c_int64, [C.c_void_p]),
     "meao_pdl_level": (C.c_int, [C.c_void_p]),
     "meao_kernels_per_frame": (C.c_int, [C.c_void_p]),
     "meao_algorithmic_bytes": (C.c_int64, [C.c_void_p, C.c_int32]),

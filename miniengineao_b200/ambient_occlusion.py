@@ -575,6 +575,15 @@ class AmbientOcclusion:
         return self._lib.meao_launch_count(self._ctx)
 
     @property
+    def frame_generation(self) -> int:
+        """meao_frame_generation, after the properties set so far have been applied: a frame recorded into a CUDA graph (render etc.
+        inside `with torch.cuda.graph(g):`) may be replayed only while this equals the value read right after the capture.  It changes
+        with every frame constant, size, re-plan, re-allocation, array release or band change; capture again (after one frame outside
+        the capture) when it does."""
+        self._update(False)
+        return self._lib.meao_frame_generation(self._ctx)
+
+    @property
     def pdl_level(self) -> int:
         """Programmatic-dependent-launch level the captured graphs use (-1 before the first capture)."""
         return self._lib.meao_pdl_level(self._ctx)

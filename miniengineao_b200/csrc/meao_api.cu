@@ -74,6 +74,8 @@ struct MeaoCtx : SizeState {
     // Frame constants (include/meao.h): bumped by every change of MeaoParams or of a camera that keeps the Z direction.  A size whose
     // plan_gen is older re-plans its constants on the host (refresh_constants); a graph captured at an older one re-targets (launch_cached).
     uint64_t consts_gen = 0;
+    // meao_frame_generation: bumped by every change a frame recorded into a caller's graph depends on (include/meao.h)
+    int64_t frame_gen = 0;
 
     // meao_reserve: the arena is laid out for res_w x res_h (0 x 0: for the current size) and every size inside it keeps its plan
     int res_w = 0, res_h = 0;
@@ -189,6 +191,7 @@ inline int ctx_reversed_z(const MeaoCtx *c) { return c->layer_cams.empty() ? c->
 // kernel instantiations (prepare_slot), so a change of it re-plans like any structural input.
 void note_camera_change(MeaoCtx *c, int old_reversed_z, int new_reversed_z)
 {
+    c->frame_gen++;
     if (old_reversed_z != new_reversed_z) c->plan_dirty = true;
     else c->consts_gen++;
 }
@@ -312,6 +315,7 @@ void disconnect_peers(MeaoCtx *c)
 
 void free_buffers(MeaoCtx *c)
 {
+    c->frame_gen++;                     // a recorded frame would touch freed memory
     drop_graph(c);
     disconnect_peers(c);
     c->band_flags = nullptr;
@@ -433,6 +437,7 @@ int allocate(MeaoCtx *c, bool keep_old = false)
         for (int i = 0; i < 2; i++) { c->depth_stage[i] = (float *)(b + a.depth_stage[i]); c->ao_stage[i] = (uint8_t *)(b + a.ao_stage[i]); }
     }
     c->plan_dirty = true;                           // the camera tables are written by the first ensure_ready
+    c->frame_gen++;
     for (auto &s : c->size_slots) s.valid = false;
     if (c->W <= 0) return 0;
     return place_size(c, 0);
@@ -456,6 +461,7 @@ void refresh_constants(MeaoCtx *c)
 // replay; it must never replay with the constants it was parked with.
 int switch_size(MeaoCtx *c, int w, int h)
 {
+    c->frame_gen++;
     SizeState &cur = *c;
     if (c->W > 0) c->size_slots[c->slot] = MeaoCtx::SizeSlot{true, c->size_clock, cur};
     int slot = -1;
@@ -523,12 +529,62 @@ void replan(MeaoCtx *c)
     for (int i = 0; i < kSizeSlots; i++) if (i != c->slot) c->size_slots[i].valid = false;
 }
 
-int ensure_ready(MeaoCtx *c)
+// ---- frames inside a caller's graph (include/meao.h) ------------------------------------------------------------------------
+// *active: the caller's stream s is being captured (cudaStreamBeginCapture, torch.cuda.graph), so the call records its launches into
+// that capture.  The legacy NULL stream is never captured; a query on cudaStreamLegacy while another stream captures may fail with
+// cudaErrorStreamCaptureImplicit, which means the same.  An invalidated capture is refused: nothing can be recorded into it.
+int stream_capturing(MeaoCtx *c, cudaStream_t s, bool *active)
+{
+    *active = false;
+    if (!s) return 0;
+    cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+    const cudaError_t e = cudaStreamGetCaptureInfo(s, &st);
+    if (e == cudaErrorStreamCaptureImplicit) { cudaGetLastError(); return 0; }
+    if (e == cudaErrorStreamCaptureInvalidated) { cudaGetLastError(); st = cudaStreamCaptureStatusInvalidated; }
+    else if (e != cudaSuccess) return fail(c, MEAO_ERR_CUDA, "cudaStreamGetCaptureInfo failed: %s", cudaGetErrorString(e));
+    if (st == cudaStreamCaptureStatusInvalidated)
+        return fail(c, MEAO_ERR_CUDA, "the stream's capture has been invalidated by an earlier error: nothing recorded");
+    *active = st == cudaStreamCaptureStatusActive;
+    return 0;
+}
+
+// Inside a caller's capture a call may issue nothing but kernel launches: a re-plan synchronises the device and uploads the camera
+// tables with blocking copies, and a table write is a pageable copy from a temporary.  Refused before any of them, so the caller's
+// capture stays valid.
+int refuse_unsettled(MeaoCtx *c)
+{
+    const char *why = nullptr;
+    if (c->plan_dirty || c->graphs_stale || c->cam_table_stale) why = "a structural change is pending (a re-plan synchronises the device)";
+    else if (c->table_pending || c->plan_gen != c->consts_gen) why = "the camera tables of new frame constants or of a new size are not written yet";
+    if (!why) return 0;
+    return fail(c, MEAO_ERR_INVALID, "cannot record into the stream's capture: %s; issue one frame outside the capture first", why);
+}
+
+// A capture that holds a graph-path frame of this context is still open: the forked streams that frame joined to it stay in it until
+// the caller ends the capture.
+bool in_open_capture(MeaoCtx *c)
+{
+    for (cudaStream_t b : c->branch) {
+        cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+        if (cudaStreamIsCapturing(b, &st) != cudaSuccess) { cudaGetLastError(); continue; }
+        if (st != cudaStreamCaptureStatusNone) return true;
+    }
+    return false;
+}
+
+// capturing: the call issues work on the caller's stream s; *capturing tells whether s is being captured, and a context that is not
+// settled (refuse_unsettled) is refused then.
+int ensure_ready(MeaoCtx *c, cudaStream_t s = nullptr, bool *capturing = nullptr)
 {
     if (!c) return MEAO_ERR_INVALID;
     if (c->W <= 0) return fail(c, MEAO_ERR_INVALID, "meao_resize has not been called");
     if (c->plan_only) return fail(c, MEAO_ERR_CUDA, "plan-only context (device < 0): no CUDA device bound, and libmeao has no CPU fallback");
     CUDA_TRY(c, cudaSetDevice(c->device));
+    if (capturing) {
+        int rc = stream_capturing(c, s, capturing);
+        if (!rc && *capturing) rc = refuse_unsettled(c);
+        if (rc) return rc;
+    }
     if (c->plan_dirty) replan(c);
     refresh_constants(c);
     if (c->graphs_stale) drop_graph(c);
@@ -537,10 +593,11 @@ int ensure_ready(MeaoCtx *c)
 }
 
 // ensure_ready for an entry point that issues work on stream s which may read the camera tables: every frame form, band phase and
-// stage call, so that each sees the tables of the constants set before it was issued
-int frame_ready(MeaoCtx *c, cudaStream_t s)
+// stage call, so that each sees the tables of the constants set before it was issued.  *capturing (optional): s is being captured.
+int frame_ready(MeaoCtx *c, cudaStream_t s, bool *capturing = nullptr)
 {
-    int rc = ensure_ready(c);
+    bool cap = false;
+    int rc = ensure_ready(c, s, capturing ? capturing : &cap);
     return rc ? rc : write_tables(c, s);
 }
 
@@ -804,7 +861,7 @@ int meao_set_params(MeaoCtx *c, const MeaoParams *p)
                    c->params.intensity != p->intensity || c->params.debug != p->debug;
     if (!(p->thickness_modifier > 0.0f)) return fail(c, MEAO_ERR_INVALID, "thickness_modifier must be > 0");
     c->params = *p;
-    if (changed) c->consts_gen++;                   // frame constants: the next frame takes them without a re-plan
+    if (changed) { c->consts_gen++; c->frame_gen++; }   // frame constants: the next frame takes them without a re-plan
     return changed ? 1 : 0;
 }
 
@@ -823,7 +880,7 @@ int meao_set_variants(MeaoCtx *c, const MeaoVariants *v)
     MeaoVariants n{v->single_pass_stereo ? 1 : 0, v->sample_exhaustively ? 1 : 0, v->high_quality_mask, v->single_scale ? 1 : 0};
     const bool changed = memcmp(&c->variants, &n, sizeof n) != 0;
     c->variants = n;
-    if (changed) c->plan_dirty = true;          // re-plan + drop the captured graphs (ensure_ready)
+    if (changed) { c->plan_dirty = true; c->frame_gen++; }      // re-plan + drop the captured graphs (ensure_ready)
     return changed ? 1 : 0;
 }
 
@@ -921,7 +978,7 @@ int meao_reserve(MeaoCtx *c, int32_t max_w, int32_t max_h)
     if (max_w == c->res_w && max_h == c->res_h) return 0;
     const int old_w = c->res_w, old_h = c->res_h;
     c->res_w = max_w; c->res_h = max_h;
-    if (c->plan_only) return 1;                     // recorded; nothing to allocate
+    if (c->plan_only) { c->frame_gen++; return 1; }     // recorded; nothing to allocate
     CUDA_TRY(c, cudaSetDevice(c->device));
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     if (clear && c->W <= 0) { free_buffers(c); return 1; }
@@ -950,6 +1007,7 @@ int meao_set_layers(MeaoCtx *c, int32_t layers)
         return fail(c, MEAO_ERR_INVALID, "layers %d not in 1..%d (the layer is a grid dimension of the layered kernels)", layers, kMaxLayers);
     if (layers == c->layers) return 0;
     const int old = c->layers;
+    c->frame_gen++;
     std::vector<MeaoCamera> old_cams;
     old_cams.swap(c->layer_cams);                   // a table has one camera per layer: a new layer count clears it
     c->layers = layers;
@@ -984,6 +1042,7 @@ int meao_set_row_band(MeaoCtx *c, int32_t row0, int32_t row1, int32_t prev_row0,
     // validated before anything changes: the context keeps its old band when the new one is refused
     int rc = check_halo_reach(c, compute_needs(c, row0, row1), prev_row0, next_row1);
     if (rc) return rc;
+    c->frame_gen++;
     if (!c->plan_only) {
         CUDA_TRY(c, cudaSetDevice(c->device));
         drop_graph(c);
@@ -1049,9 +1108,10 @@ int64_t meao_halo_recv_bytes(MeaoCtx *c, int32_t side) { return halo_size(c, sid
 static int halo_copy(MeaoCtx *c, int side, void *packed, bool pack, void *stream)
 {
     BAND_GUARD(c, pack ? "meao_halo_pack" : "meao_halo_unpack");
-    int rc = ensure_ready(c); if (rc) return rc;
-    if (side != 0 && side != 1) return fail(c, MEAO_ERR_INVALID, "side must be 0 or 1");
     cudaStream_t s = (cudaStream_t)stream;
+    bool capturing;
+    int rc = ensure_ready(c, s, &capturing); if (rc) return rc;
+    if (side != 0 && side != 1) return fail(c, MEAO_ERR_INVALID, "side must be 0 or 1");
     Range r[5]; halo_ranges(c, side, pack, r);
     HaloArgs a{};
     halo_segments(*c, r, (float *)packed, pack, a);
@@ -1162,9 +1222,14 @@ static int retarget(MeaoCtx *c, cudaGraphExec_t *ge, cudaGraph_t g, cudaStream_t
 // Replays the graph of `key`, captured from record(stream, pdl) on first use; a replay counts the launches its capture recorded.  A
 // graph captured before the frame constants last changed (its gen) is captured again and re-targeted in place before it is launched:
 // lazily, so a change costs one capture + update per graph actually replayed, not one per cached graph.
-static int launch_cached(MeaoCtx *c, const MeaoCtx::GraphKey &key_in, cudaStream_t s, const std::function<int(cudaStream_t, int)> &record)
+// capturing: s is being captured by the caller, whose graph then holds the launches themselves -- no graph of the context is captured,
+// instantiated, launched or evicted.  PDL at the level an instantiation of this context has accepted (0 before the first): a level
+// is never tried inside the caller's capture, where a refused attempt would invalidate it.
+static int launch_cached(MeaoCtx *c, const MeaoCtx::GraphKey &key_in, cudaStream_t s, bool capturing,
+                         const std::function<int(cudaStream_t, int)> &record)
 {
     if (c->flags & MEAO_FLAG_NO_GRAPH) return record(s, 0);
+    if (capturing) return record(s, c->pdl_level >= 0 ? c->pdl_level : 0);
     MeaoCtx::GraphKey key = key_in;
     key.size[0] = c->W; key.size[1] = c->H; key.size[2] = c->slot;
     auto it = c->graphs.find(key);
@@ -1213,11 +1278,12 @@ static int launch_cached(MeaoCtx *c, const MeaoCtx::GraphKey &key_in, cudaStream
 int meao_band_phase_a(MeaoCtx *c, const void *depth, int32_t kind, void *send_up, void *send_down, void *stream)
 {
     BAND_GUARD(c, "meao_band_phase_a");
-    int rc = frame_ready(c, (cudaStream_t)stream); if (rc) return rc;
+    bool capturing;
+    int rc = frame_ready(c, (cudaStream_t)stream, &capturing); if (rc) return rc;
     if (!depth) return fail(c, MEAO_ERR_INVALID, "depth is NULL");
     c->last_kind = kind;
     const MeaoCtx::GraphKey key{{depth, send_up, send_down, nullptr}, 100 + kind};
-    return launch_cached(c, key, (cudaStream_t)stream, [&](cudaStream_t s, int pdl) {
+    return launch_cached(c, key, (cudaStream_t)stream, capturing, [&](cudaStream_t s, int pdl) {
         int r = record_downsample(c, depth, kind, s);
         if (r) return r;
         PdlScope p(pdl >= 1);
@@ -1228,12 +1294,13 @@ int meao_band_phase_a(MeaoCtx *c, const void *depth, int32_t kind, void *send_up
 int meao_band_phase_b(MeaoCtx *c, const void *recv_up, const void *recv_down, void *ao_out, void *stream)
 {
     BAND_GUARD(c, "meao_band_phase_b");
-    int rc = frame_ready(c, (cudaStream_t)stream); if (rc) return rc;
+    bool capturing;
+    int rc = frame_ready(c, (cudaStream_t)stream, &capturing); if (rc) return rc;
     if (!ao_out) return fail(c, MEAO_ERR_INVALID, "ao_out is NULL");
     const int kind = c->last_kind;
     const MeaoCtx::GraphKey key{{recv_up, recv_down, ao_out, nullptr}, 200 + kind};
     c->last_out = ao_out;
-    return launch_cached(c, key, (cudaStream_t)stream, [&](cudaStream_t s, int pdl) {
+    return launch_cached(c, key, (cudaStream_t)stream, capturing, [&](cudaStream_t s, int pdl) {
         int r = halo_kernel(c, (void *)recv_up, (void *)recv_down, false, s);
         if (r) return r;
         return record_frame_dag(c, frame_io(c, nullptr, kind, ao_out, false), s, 1, pdl);
@@ -1276,6 +1343,7 @@ int meao_band_connect(MeaoCtx *c, int32_t side, const MeaoPeerHandle *peer)
     int rc = ensure_ready(c); if (rc) return rc;
     if (side != 0 && side != 1) return fail(c, MEAO_ERR_INVALID, "side must be 0 (up) or 1 (down)");
     drop_graph(c);                                  // captured band steps carry the old peer pointers
+    c->frame_gen++;
     if (c->peer_base[side] && c->peer_ipc[side]) cudaIpcCloseMemHandle(c->peer_base[side]);
     c->peer_base[side] = nullptr; c->peer_ipc[side] = false;
     if (!peer) return MEAO_OK;
@@ -1342,7 +1410,8 @@ static int record_exchange(MeaoCtx *c, cudaStream_t s)
 int meao_band_step(MeaoCtx *c, const void *depth, int32_t kind, void *ao_out, void *stream)
 {
     BAND_GUARD(c, "meao_band_step");
-    int rc = frame_ready(c, (cudaStream_t)stream); if (rc) return rc;
+    bool capturing;
+    int rc = frame_ready(c, (cudaStream_t)stream, &capturing); if (rc) return rc;
     if (!depth || !ao_out) return fail(c, MEAO_ERR_INVALID, "depth / ao_out is NULL");
     if ((c->prev0 >= 0 && !c->peer_base[0]) || (c->next1 >= 0 && !c->peer_base[1]))
         return fail(c, MEAO_ERR_INVALID, "meao_band_step: connect every neighbour first (meao_band_export / meao_band_connect)");
@@ -1353,7 +1422,7 @@ int meao_band_step(MeaoCtx *c, const void *depth, int32_t kind, void *ao_out, vo
     c->last_kind = kind; c->last_out = ao_out;
     const MeaoCtx::GraphKey key{{depth, ao_out, c->peer_base[0], c->peer_base[1]}, 300 + kind};
     const bool has_peer = c->peer_base[0] || c->peer_base[1];
-    return launch_cached(c, key, (cudaStream_t)stream, [&](cudaStream_t s, int pdl) {
+    return launch_cached(c, key, (cudaStream_t)stream, capturing, [&](cudaStream_t s, int pdl) {
         int r = record_downsample(c, depth, kind, s, true);
         if (r) return r;
         { PdlScope p(pdl >= 1); if ((r = record_exchange(c, s))) return r; }
@@ -1440,7 +1509,7 @@ int check_views(MeaoCtx *c, const void *depth, int kind, const void *ao_out, Vie
 
 namespace {
 // The frame of meao_render / meao_render_pitched on a context that ensure_ready has prepared.
-int render_views(MeaoCtx *c, const void *depth, int kind, void *ao_out, ViewPitch p, void *stream)
+int render_views(MeaoCtx *c, const void *depth, int kind, void *ao_out, ViewPitch p, void *stream, bool capturing)
 {
     int rc;
     if ((rc = check_views(c, depth, kind, ao_out, &p))) return rc;
@@ -1452,7 +1521,7 @@ int render_views(MeaoCtx *c, const void *depth, int kind, void *ao_out, ViewPitc
     NvtxRange nv("meao::frame");
     const MeaoCtx::GraphKey key{{depth, ao_out, nullptr, nullptr}, kind, {p.depth_row, p.depth_layer, p.ao_row, p.ao_layer}};
     c->last_kind = kind; c->last_out = ao_out;
-    return launch_cached(c, key, s, [&](cudaStream_t cs, int pdl) {
+    return launch_cached(c, key, s, capturing, [&](cudaStream_t cs, int pdl) {
         return record_frame_dag(c, frame_io(c, depth, kind, ao_out, true, &p), cs, 0, pdl);
     });
 }
@@ -1460,15 +1529,17 @@ int render_views(MeaoCtx *c, const void *depth, int kind, void *ao_out, ViewPitc
 
 int meao_render(MeaoCtx *c, const void *depth, int32_t kind, void *ao_out, void *stream)
 {
-    int rc = frame_ready(c, (cudaStream_t)stream); if (rc) return rc;
-    return render_views(c, depth, kind, ao_out, tight_pitch(*c, kind), stream);      // meao_render_pitched at the tight pitches
+    bool capturing;
+    int rc = frame_ready(c, (cudaStream_t)stream, &capturing); if (rc) return rc;
+    return render_views(c, depth, kind, ao_out, tight_pitch(*c, kind), stream, capturing);      // meao_render_pitched at the tight pitches
 }
 
 int meao_render_pitched(MeaoCtx *c, const void *depth, int64_t depth_row_pitch, int64_t depth_layer_pitch, int32_t kind,
                         void *ao_out, int64_t ao_row_pitch, int64_t ao_layer_pitch, void *stream)
 {
-    int rc = frame_ready(c, (cudaStream_t)stream); if (rc) return rc;
-    return render_views(c, depth, kind, ao_out, ViewPitch{depth_row_pitch, depth_layer_pitch, ao_row_pitch, ao_layer_pitch}, stream);
+    bool capturing;
+    int rc = frame_ready(c, (cudaStream_t)stream, &capturing); if (rc) return rc;
+    return render_views(c, depth, kind, ao_out, ViewPitch{depth_row_pitch, depth_layer_pitch, ao_row_pitch, ao_layer_pitch}, stream, capturing);
 }
 
 // ---- CUDA arrays (include/meao.h "CUDA arrays") ------------------------------------------------------------------------
@@ -1546,14 +1617,19 @@ int prepare_arrays(MeaoCtx *c, const void *depth_array, int kind, const void *ao
 
 int meao_render_arrays(MeaoCtx *c, const void *depth_array, int32_t kind, void *ao_array, void *stream)
 {
-    int rc = frame_ready(c, (cudaStream_t)stream); if (rc) return rc;
+    bool capturing;
+    int rc = frame_ready(c, (cudaStream_t)stream, &capturing); if (rc) return rc;
+    // a surface object is made on an array's first frame, which therefore cannot be recorded into a caller's capture
+    if (capturing && (!c->surfaces.count(depth_array) || !c->surfaces.count(ao_array)))
+        return fail(c, MEAO_ERR_INVALID, "cannot record into the stream's capture: an array this context has not rendered with needs a surface "
+                                         "object first; issue one frame with these arrays outside the capture first");
     ArrayIO io;
     if ((rc = prepare_arrays(c, depth_array, kind, ao_array, &io))) return rc;
     // the frame graph of meao_render with its first and last node reading / writing the arrays
     NvtxRange nv("meao::frame_arrays");
     const MeaoCtx::GraphKey key{{depth_array, ao_array, nullptr, nullptr}, kArrayGraphKind + kind};
     c->last_kind = kind; c->last_out = ao_array;
-    return launch_cached(c, key, (cudaStream_t)stream, [&](cudaStream_t cs, int pdl) {
+    return launch_cached(c, key, (cudaStream_t)stream, capturing, [&](cudaStream_t cs, int pdl) {
         FrameIO fio = frame_io(c, nullptr, kind, nullptr, false);
         fio.aio = &io;
         return record_frame_dag(c, fio, cs, 0, pdl);
@@ -1574,6 +1650,7 @@ int meao_release_array(MeaoCtx *c, const void *array)
     bool used = c->surfaces.count(array) != 0;
     for (auto &kv : c->graphs) used |= kv.first.kind >= kArrayGraphKind && (kv.first.p[0] == array || kv.first.p[1] == array);
     if (!used) return MEAO_OK;
+    c->frame_gen++;
     CUDA_TRY(c, cudaSetDevice(c->device));
     CUDA_TRY(c, cudaDeviceSynchronize());       // frames that use the array may be in flight on any stream
     for (auto it = c->graphs.begin(); it != c->graphs.end();) {
@@ -1809,7 +1886,8 @@ static int composite_args(MeaoCtx *c, const void *ao, const void *color, int fmt
 
 int meao_composite_framebuffer(MeaoCtx *c, const void *ao, void *color, int32_t fmt, void *stream)
 {
-    int rc = ensure_ready(c); if (rc) return rc;
+    bool capturing;
+    int rc = ensure_ready(c, (cudaStream_t)stream, &capturing); if (rc) return rc;
     if ((rc = composite_args(c, ao, color, fmt))) return rc;
     const long long npix = (long long)c->W * (c->band1 - c->band0) * c->layers;
     CUDA_TRY(c, launch_composite((const uint8_t *)ao, color, npix, fmt == MEAO_FMT_RGBA16_FLOAT, 1, 1, 0, (cudaStream_t)stream));
@@ -1819,7 +1897,8 @@ int meao_composite_framebuffer(MeaoCtx *c, const void *ao, void *color, int32_t 
 
 int meao_composite_gbuffer(MeaoCtx *c, const void *ao, void *g0, void *g3, int32_t fmt3, void *stream)
 {
-    int rc = ensure_ready(c); if (rc) return rc;
+    bool capturing;
+    int rc = ensure_ready(c, (cudaStream_t)stream, &capturing); if (rc) return rc;
     if ((rc = composite_args(c, ao, g0, MEAO_FMT_RGBA8_UNORM)) || (rc = composite_args(c, ao, g3, fmt3))) return rc;
     const long long npix = (long long)c->W * (c->band1 - c->band0) * c->layers;
     CUDA_TRY(c, launch_composite((const uint8_t *)ao, g0, npix, 0, 0, 1, 1, (cudaStream_t)stream));                               // gbuffer0.a
@@ -1830,7 +1909,8 @@ int meao_composite_gbuffer(MeaoCtx *c, const void *ao, void *g0, void *g3, int32
 
 int meao_composite_debug(MeaoCtx *c, const void *view, void *color, int32_t fmt, void *stream)
 {
-    int rc = ensure_ready(c); if (rc) return rc;
+    bool capturing;
+    int rc = ensure_ready(c, (cudaStream_t)stream, &capturing); if (rc) return rc;
     if ((rc = composite_args(c, view, color, fmt))) return rc;
     const long long npix = (long long)c->W * (c->band1 - c->band0) * c->layers;
     CUDA_TRY(c, launch_debug_composite((const uint8_t *)view, color, npix, fmt == MEAO_FMT_RGBA16_FLOAT, (cudaStream_t)stream));
@@ -1899,6 +1979,7 @@ void meao_render_event(int event_id)
 MeaoRenderEventFunc meao_get_render_event_func(void) { return meao_render_event; }
 
 int64_t meao_launch_count(const MeaoCtx *c) { return c ? c->launches : 0; }
+int64_t meao_frame_generation(const MeaoCtx *c) { return c ? c->frame_gen : MEAO_ERR_INVALID; }
 int meao_pdl_level(const MeaoCtx *c) { return c ? c->pdl_level : -1; }
 int meao_kernels_per_frame(const MeaoCtx *c)
 {
@@ -1957,6 +2038,8 @@ int meao_set_profile_repeats(MeaoCtx *c, int32_t n)
 
 int meao_profile_frame(MeaoCtx *c, const void *depth, int32_t kind, void *ao_out, float *ms_out, const char **names_out, int32_t capacity)
 {
+    if (c && !c->plan_only && in_open_capture(c))
+        return fail(c, MEAO_ERR_UNSUPPORTED, "meao_profile_frame synchronises the device: not while a capture that holds a frame of this context is open");
     int rc = frame_ready(c, c->stream); if (rc) return rc;
     if (!depth || !ao_out) return fail(c, MEAO_ERR_INVALID, "depth / ao_out is NULL");
     CUDA_TRY(c, cudaDeviceSynchronize());
