@@ -72,6 +72,12 @@ namespace MiniEngineAO
         // CUDA arrays (graphics interop: cudaGraphicsSubResourceGetMappedArray / level 0 of a Vulkan mipmapped array), no copies
         [DllImport(Lib)] public static extern int meao_render_arrays(IntPtr ctx, IntPtr depthArray, int depthKind, IntPtr aoArray, IntPtr stream);
         [DllImport(Lib)] public static extern int meao_bind_event_arrays(IntPtr ctx, int eventId, IntPtr depthArray, int depthKind, IntPtr aoArray, IntPtr stream);
+        // ... or a viewport of larger arrays: the frame's W x H texels at (depthX, depthY) and (aoX, aoY) -- max-size targets of a
+        // dynamic-resolution engine, one player's half of a split-screen texture
+        [DllImport(Lib)] public static extern int meao_render_arrays_at(IntPtr ctx, IntPtr depthArray, int depthX, int depthY, int depthKind,
+                                                                        IntPtr aoArray, int aoX, int aoY, IntPtr stream);
+        [DllImport(Lib)] public static extern int meao_bind_event_arrays_at(IntPtr ctx, int eventId, IntPtr depthArray, int depthX, int depthY, int depthKind,
+                                                                            IntPtr aoArray, int aoX, int aoY, IntPtr stream);
         [DllImport(Lib)] public static extern int meao_release_array(IntPtr ctx, IntPtr array);   // before the array is unmapped / unregistered / freed
         // Linear buffers with their own row and layer pitch, in bytes (D3D12 placed footprints, Vulkan buffers through external memory,
         // cudaMallocPitch, a dynamic-resolution corner of a max-size target), no copies
@@ -156,6 +162,8 @@ namespace MiniEngineAO
         // registered with cudaGraphicsRegisterFlagsSurfaceLoadStore), those: the plugin event then reads and writes them directly
         IntPtr _depthArray = IntPtr.Zero, _aoArray = IntPtr.Zero;
         int _depthArrayKind = 0;                                // MEAO_DEPTH_RAW_F32 (R32_FLOAT copy) or 2 = RAW_D16_UNORM (R16 copy)
+        // viewport origins in the arrays (BindEventArraysAt); null: the arrays are exactly the frame's size (meao_bind_event_arrays)
+        Vector2Int? _depthArrayOrigin, _aoArrayOrigin;
         // ... or, when the interop layer maps linear buffers that keep the graphics API's row pitch (a D3D12 footprint rounds each row up
         // to 256 bytes; a dynamic-resolution frame is the corner of a max-size target), their byte pitches; 0 = tight (meao_bind_event)
         long _depthRowPitch, _depthLayerPitch, _aoRowPitch, _aoLayerPitch;
@@ -269,10 +277,34 @@ namespace MiniEngineAO
             _camera.AddCommandBuffer(CameraEvent.BeforeImageEffects, _renderCommand);          // :421
         }
 
-        // The array path of the plugin event: meao_render_arrays on the mapped arrays (checked here -- the event cannot report errors).
+        // The array path of the plugin event: meao_render_arrays on the mapped arrays (checked here -- the event cannot report errors),
+        // or meao_render_arrays_at at the origins BindEventArraysAt set.
         void BindEventArrays()
         {
-            MeaoNative.Check(_ctx, MeaoNative.meao_bind_event_arrays(_ctx, kEventId, _depthArray, _depthArrayKind, _aoArray, _stream));
+            if (_depthArrayOrigin == null && _aoArrayOrigin == null)
+            {
+                MeaoNative.Check(_ctx, MeaoNative.meao_bind_event_arrays(_ctx, kEventId, _depthArray, _depthArrayKind, _aoArray, _stream));
+                return;
+            }
+            Vector2Int d = _depthArrayOrigin ?? Vector2Int.zero, a = _aoArrayOrigin ?? Vector2Int.zero;
+            MeaoNative.Check(_ctx, MeaoNative.meao_bind_event_arrays_at(_ctx, kEventId, _depthArray, d.x, d.y, _depthArrayKind, _aoArray, a.x, a.y, _stream));
+        }
+
+        // Dynamic resolution or split-screen on interop textures: the plugin event renders the frame's current W x H from the depth
+        // array's texels at depthOrigin into the AO array's at aoOrigin.  Register and map the textures once at their largest size and
+        // bind once: the event checks the viewport again at each frame's size, so a MaxResolution reservation needs no rebinding.
+        public void BindEventArraysAt(IntPtr depthArray, Vector2Int depthOrigin, IntPtr aoArray, Vector2Int aoOrigin, int depthKind = 0)
+        {
+            _depthArray = depthArray; _aoArray = aoArray; _depthArrayKind = depthKind;
+            _depthArrayOrigin = depthOrigin; _aoArrayOrigin = aoOrigin;
+            if (_ctx != IntPtr.Zero) BindEventArrays();
+        }
+
+        // One frame from and into viewports of the arrays, outside the command buffer (a second camera's half of a split-screen target).
+        public void RenderArraysAt(IntPtr depthArray, Vector2Int depthOrigin, IntPtr aoArray, Vector2Int aoOrigin, int depthKind = 0)
+        {
+            MeaoNative.Check(_ctx, MeaoNative.meao_render_arrays_at(_ctx, depthArray, depthOrigin.x, depthOrigin.y, depthKind, aoArray,
+                                                                    aoOrigin.x, aoOrigin.y, _stream));
         }
 
         // The pitched path of the plugin event: meao_render_pitched on the mapped buffers at their own pitches (checked here -- the
@@ -291,6 +323,7 @@ namespace MiniEngineAO
             if (_depthArray != IntPtr.Zero) MeaoNative.Check(_ctx, MeaoNative.meao_release_array(_ctx, _depthArray));
             if (_aoArray != IntPtr.Zero) MeaoNative.Check(_ctx, MeaoNative.meao_release_array(_ctx, _aoArray));
             _depthArray = _aoArray = IntPtr.Zero;
+            _depthArrayOrigin = _aoArrayOrigin = null;
         }
 
         void OnDisable()

@@ -37,7 +37,8 @@ extern "C" {
                               *    + meao_render_arrays / meao_bind_event_arrays / meao_release_array (CUDA-array I/O; additive)
                               *    + meao_render_pitched / meao_bind_event_pitched (depth and AO with their own row and layer pitch; additive)
                               *    + meao_reserve / meao_reservation (dynamic resolution; additive)
-                              *    + meao_frame_generation (frames inside a caller's CUDA graph; additive) */
+                              *    + meao_frame_generation (frames inside a caller's CUDA graph; additive)
+                              *    + meao_render_arrays_at / meao_bind_event_arrays_at (viewports of larger CUDA arrays; additive) */
 
 typedef struct MeaoCtx MeaoCtx;
 
@@ -297,6 +298,20 @@ int meao_render_host(MeaoCtx *ctx, const void *depth_host, int32_t depth_kind, u
  * a reversed_z change, meao_set_row_band) release all arrays; a frame-constant change (MeaoParams, the cameras' planes and fields of
  * view) releases none.  Releasing an array this context never used returns MEAO_OK. */
 int meao_render_arrays(MeaoCtx *ctx, const void *depth_array, int32_t depth_kind, void *ao_array, void *stream);
+/* Viewports: meao_render_arrays with the frame read from, and written into, a W x H rectangle of larger arrays -- render targets
+ * allocated (and registered) once at the largest size of a dynamic-resolution engine, or one player's half of a split-screen texture.
+ * The frame reads the context's current W x H (meao_resize, reserved or not) from the depth array's texels [depth_x, depth_x + W) x
+ * [depth_y, depth_y + H) and writes the AO into [ao_x, ao_x + W) x [ao_y, ao_y + H) of the AO array, in every layer or cube face.
+ * No texel outside the two rectangles is read or written.  The arrays may have different extents and origins (say an exact-size depth
+ * copy and a maximum-size AO target).  The checks are meao_render_arrays's, except the exact extent: instead each origin must be >= 0
+ * and the viewport must fit, x + W <= width and y + H <= height; a refusal returns MEAO_ERR_INVALID naming the array and the field
+ * (depth_x, depth_y, ao_x, ao_y) and launches nothing.  Everything else is meao_render_arrays's contract: layered and cube-map
+ * contexts, per-layer cameras, MEAO_FLAG_NO_GRAPH, the release contract, regeneration of id 17, recording into a caller's capture after
+ * one frame outside it.  The origins are arguments like the arrays: a graph is cached per (arrays, origins, kind), they do not move
+ * meao_frame_generation, and a frame recorded into a caller's graph replays at the origins it was recorded with.
+ * meao_render_arrays(ctx, d, kind, a, s) is meao_render_arrays_at(ctx, d, 0, 0, kind, a, 0, 0, s) on arrays of exactly W x H. */
+int meao_render_arrays_at(MeaoCtx *ctx, const void *depth_array, int32_t depth_x, int32_t depth_y, int32_t depth_kind,
+                          void *ao_array, int32_t ao_x, int32_t ao_y, void *stream);
 int meao_release_array(MeaoCtx *ctx, const void *array);
 /* Pipelined form of meao_render_host for frame streams: enqueues H2D + kernels + D2H of one frame on staging slot
  * `slot` (0 or 1) and returns; meao_host_wait(slot) blocks until that frame's AO is in ao_out_host.  Alternating the
@@ -456,6 +471,11 @@ int meao_bind_event(MeaoCtx *ctx, int32_t event_id, const void *depth_dev, int32
  * are checked now (the event cannot report an error), with the statuses of meao_render_arrays; both NULL unbinds.  An id holds one
  * binding: binding it again, with either call, replaces it.  meao_release_array also removes the bindings that name the array. */
 int meao_bind_event_arrays(MeaoCtx *ctx, int32_t event_id, const void *depth_array, int32_t depth_kind, void *ao_array, void *stream);
+/* The viewport twin: the event renders meao_render_arrays_at with these origins.  Checked now at the current size, and again at the
+ * size of the frame each time the event runs, so one binding to maximum-size arrays serves every size of a reservation; a viewport that
+ * no longer fits launches nothing and leaves the reason in meao_last_error. */
+int meao_bind_event_arrays_at(MeaoCtx *ctx, int32_t event_id, const void *depth_array, int32_t depth_x, int32_t depth_y,
+                              int32_t depth_kind, void *ao_array, int32_t ao_x, int32_t ao_y, void *stream);
 /* The pitched twin of meao_bind_event: the event renders meao_render_pitched with these views.  The views are checked now, with the
  * refusals of meao_render_pitched; both pointers NULL unbinds.  meao_bind_event binds the tight views of the context as it is when the
  * event runs. */
@@ -474,14 +494,14 @@ MeaoRenderEventFunc meao_get_render_event_func(void);
  * carry programmatic dependent launch at the level an instantiation of this context has accepted (meao_pdl_level; none before the
  * first), so a frame recorded into a caller's graph matches the context's own.  The capture status query is the only cost a frame
  * outside a capture pays for this.
- * Capturable: meao_render, meao_render_pitched, meao_render_arrays, meao_render_event (any binding), the meao_stage_* calls,
+ * Capturable: meao_render, meao_render_pitched, meao_render_arrays(_at), meao_render_event (any binding), the meao_stage_* calls,
  * meao_render_band_prepare / _finish, meao_band_phase_a / _b, meao_band_step, meao_halo_pack / _unpack, meao_debug_view and the three
  * meao_composite_* calls.
  * SETTLED CONTEXTS ONLY: inside a capture a call may issue nothing but kernel launches.  It is refused with MEAO_ERR_INVALID, records
  * nothing and leaves the caller's capture valid (meao_last_error says why: "issue one frame outside the capture first") when
  *   - a structural change is pending (a re-plan synchronises the device),
  *   - the per-layer camera tables are still to be written: after a frame-constant change, or on the first frame at a size,
- *   - or, for meao_render_arrays, the context has not rendered with one of the arrays yet (its surface object is made then).
+ *   - or, for meao_render_arrays(_at), the context has not rendered with one of the arrays yet (its surface object is made then).
  * One frame of the same form issued outside the capture settles the context; torch's warm-up before torch.cuda.graph does that.
  * A capture that has been invalidated returns MEAO_ERR_CUDA and records nothing.
  * NOT capturable: the host-buffer calls (meao_render_host, _host_async, meao_host_wait, meao_band_step_host; they run on the

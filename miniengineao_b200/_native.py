@@ -78,6 +78,7 @@ SIGNATURES = {
                                       C.c_void_p]),
     "meao_render_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
     "meao_render_arrays": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "meao_render_arrays_at": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
     "meao_release_array": (C.c_int, [C.c_void_p, C.c_void_p]),
     "meao_render_host_async": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32]),
     "meao_host_wait": (C.c_int, [C.c_void_p, C.c_int32]),
@@ -119,6 +120,8 @@ SIGNATURES = {
     "meao_band_status": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),
     "meao_bind_event": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "meao_bind_event_arrays": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "meao_bind_event_arrays_at": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32,
+                                            C.c_void_p]),
     "meao_bind_event_pitched": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_int64,
                                           C.c_int64, C.c_void_p]),
     "meao_render_event": (None, [C.c_int]),

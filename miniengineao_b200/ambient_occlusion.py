@@ -272,16 +272,24 @@ class AmbientOcclusion:
     _ARRAY_KINDS = {"raw_f32": N.MEAO_DEPTH_RAW_F32, "linear_f32": N.MEAO_DEPTH_LINEAR_F32, "d16": N.MEAO_DEPTH_RAW_D16_UNORM,
                     "d24s8": N.MEAO_DEPTH_RAW_D24S8}
 
-    def render_arrays(self, depth_array: int, ao_array: int, *, kind: str = "raw_f32", stream=None) -> None:
+    def render_arrays(self, depth_array: int, ao_array: int, *, kind: str = "raw_f32", stream=None, depth_origin=None,
+                      ao_origin=None) -> None:
         """The frame with the depth read from and the AO written into CUDA arrays (meao_render_arrays): integer cudaArray_t handles,
         e.g. from graphics interop.  kind: "raw_f32", "linear_f32" or "d16" (the array's one channel: f32 / f32 / 16-bit unsigned).
         The arrays must be W x H with the context's layer count (2-D: 1, layered: its depth, cube map: 6) and carry
-        cudaArraySurfaceLoadStore.  Call release_array before freeing an array this context has rendered with."""
+        cudaArraySurfaceLoadStore.  Call release_array before freeing an array this context has rendered with.
+        depth_origin / ao_origin: (x, y) of a W x H viewport in a larger array (meao_render_arrays_at; the other one defaults to
+        (0, 0)); the arrays may then be any size that holds the viewport."""
         if kind not in self._ARRAY_KINDS:
             raise ValueError(f"kind must be one of {sorted(self._ARRAY_KINDS)}")
         self.LateUpdate()
-        self._check(self._lib.meao_render_arrays(self._ctx, C.c_void_p(depth_array), self._ARRAY_KINDS[kind], C.c_void_p(ao_array),
-                                                 self._stream(stream)))
+        if depth_origin is None and ao_origin is None:
+            self._check(self._lib.meao_render_arrays(self._ctx, C.c_void_p(depth_array), self._ARRAY_KINDS[kind], C.c_void_p(ao_array),
+                                                     self._stream(stream)))
+            return
+        (dx, dy), (ax, ay) = depth_origin or (0, 0), ao_origin or (0, 0)
+        self._check(self._lib.meao_render_arrays_at(self._ctx, C.c_void_p(depth_array), int(dx), int(dy), self._ARRAY_KINDS[kind],
+                                                    C.c_void_p(ao_array), int(ax), int(ay), self._stream(stream)))
 
     def release_array(self, handle: int) -> None:
         """Drop the graphs, the surface object and the event bindings that refer to a CUDA array (meao_release_array; synchronises

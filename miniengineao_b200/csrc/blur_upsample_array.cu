@@ -2,7 +2,7 @@
 // AO) with the AO written into a CUDA array (meao_render_arrays): a 2-D, layered or cube-map array of L layers, one launch.  The
 // kernel bodies are blur_upsample.cu's in their layered tile-loop form (blur_upsample_kernel.inc with MEAO_UPS_LAYERED 1 and
 // MEAO_UPS_ARRAY 1): the 64-bit store of the fast path and the stores of upsample8_slow become one-byte surface stores at
-// (x, y, layer) (surface_io.cuh); everything else, including every read of the intermediates, is the existing code.  The coarse
+// (ao_x + x, ao_y + y, layer) (surface_io.cuh); everything else, including every read of the intermediates, is the existing code.  The coarse
 // levels run the existing kernels on the context's arena.  A translation unit of its own so that blur_upsample.cu and
 // blur_upsample_layered.cu compile to exactly the code they did before.
 #include <cstdlib>
@@ -30,18 +30,18 @@ namespace {
 #undef MEAO_UPS_ARRAY
 
 const struct {      // [upsample_slot]: the final level's slot only
-    Kernel<CUtensorMap, CUtensorMap, UpsampleArgs, int, int, cudaSurfaceObject_t, int> plain[kUpsampleSlots];
-    Kernel<CUtensorMap, CUtensorMap, CUtensorMap, UpsamplePreminArgs, int, int, cudaSurfaceObject_t, int> premin[kUpsampleSlots];
+    Kernel<CUtensorMap, CUtensorMap, UpsampleArgs, int, int, cudaSurfaceObject_t, int, int, int> plain[kUpsampleSlots];
+    Kernel<CUtensorMap, CUtensorMap, CUtensorMap, UpsamplePreminArgs, int, int, cudaSurfaceObject_t, int, int, int> premin[kUpsampleSlots];
 } kKernels = {MEAO_UPSAMPLE_SLOTS(blur_upsample_array_kernel, MEAO_NO_SLOT), MEAO_UPSAMPLE_SLOTS(blur_upsample_premin_array_kernel, MEAO_NO_SLOT)};
 
 }  // namespace
 
 cudaError_t launch_blur_upsample_array(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
                                        const UpsampleArgs &a_in, const uint8_t *lo_ao2, int lo_a2pitch, int layers, int sm_count,
-                                       cudaSurfaceObject_t out, int surf_kind, cudaStream_t s)
+                                       cudaSurfaceObject_t out, int surf_kind, int ao_x, int ao_y, cudaStream_t s)
 {
     if (a_in.row1 <= a_in.row0) return cudaSuccess;
-    if (layers < 1 || layers > kMaxLayers) return cudaErrorInvalidValue;
+    if (layers < 1 || layers > kMaxLayers || ao_x < 0 || ao_y < 0) return cudaErrorInvalidValue;
     if (a_in.hi_ao || !a_in.hi_is_half || a_in.row0 != 0 || a_in.row1 != a_in.hih) return cudaErrorInvalidValue;     // the final level, whole frame
     UpsampleArgs a = a_in;
     a.out = nullptr; a.out_pitch = 0; a.out_row_origin = 0;
@@ -50,11 +50,11 @@ cudaError_t launch_blur_upsample_array(const CUtensorMap &lo_depth_map, const CU
     if (!ups_tile_grid(a, layers, sm_count, &grid)) return cudaErrorInvalidValue;
     const int t = use_tma ? 1 : 0, k = upsample_slot(a);
     if (!lo_ao2) {
-        MEAO_LAUNCH((kKernels.plain[k]), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, a, t, layers, out, surf_kind);
+        MEAO_LAUNCH((kKernels.plain[k]), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, a, t, layers, out, surf_kind, ao_x, ao_y);
     } else {        // main_premin
         if (!lo_ao2_map) return cudaErrorInvalidValue;
         const UpsamplePreminArgs pa{a, lo_ao2, lo_a2pitch};
-        MEAO_LAUNCH((kKernels.premin[k]), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, *lo_ao2_map, pa, t, layers, out, surf_kind);
+        MEAO_LAUNCH((kKernels.premin[k]), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, *lo_ao2_map, pa, t, layers, out, surf_kind, ao_x, ao_y);
     }
     return cudaGetLastError();
 }

@@ -187,7 +187,9 @@ inline int render_tile_variant(const FrameState &f, int k, int rows, int force)
 }
 
 // A CUDA-array frame (meao_render_arrays): the surfaces of the depth and AO arrays and how their layers are addressed (surface_io.cuh).
-struct ArrayIO { cudaSurfaceObject_t depth, ao; int depth_surf, ao_surf; const void *ao_array; };
+// The frame reads the depth array's texels [depth_x, depth_x + W) x [depth_y, depth_y + H) and writes the AO array's at (ao_x, ao_y)
+// (meao_render_arrays_at; all 0 for meao_render_arrays).
+struct ArrayIO { cudaSurfaceObject_t depth, ao; int depth_surf, ao_surf; const void *ao_array; int depth_x = 0, depth_y = 0, ao_x = 0, ao_y = 0; };
 
 // The byte pitches of the caller's depth and AO views (meao_render_pitched).  A view is `layers` images of rows [band0, band1) of
 // the frame, W pixels per row.
@@ -244,7 +246,7 @@ inline PrepareArgs prepare_args(const FrameState &f, const DepthIn &d)
 // with the same depth (launch_upsample's `fused`) and writes LinearDepth itself.
 inline cudaError_t launch_prepare(const FrameState &f, const PrepareArgs &a, const ArrayIO *aio, bool low_only, cudaStream_t s)
 {
-    if (aio) return launch_prepare_depth_array(a, aio->depth, aio->depth_surf, f.layers, s, f.layer_zb);
+    if (aio) return launch_prepare_depth_array(a, aio->depth, aio->depth_surf, aio->depth_x, aio->depth_y, f.layers, s, f.layer_zb);
     if (f.layers > 1) return launch_prepare_depth_layered(a, f.layers, s, low_only, f.layer_zb);
     return launch_prepare_depth(a, s, low_only);
 }
@@ -327,7 +329,8 @@ inline cudaError_t launch_upsample(const FrameState &f, int lo, const UpsampleAr
     if (fused && final_level)
         return launch_blur_upsample_lin(dm, ao_map, hm, f.tma_ok, a, lo_ao2, f.occ_pitch[lo], *fused, f.layers, f.sm_count, s);
     if (aio && final_level)
-        return launch_blur_upsample_array(dm, ao_map, hm, f.tma_ok, a, lo_ao2, f.occ_pitch[lo], f.layers, f.sm_count, aio->ao, aio->ao_surf, s);
+        return launch_blur_upsample_array(dm, ao_map, hm, f.tma_ok, a, lo_ao2, f.occ_pitch[lo], f.layers, f.sm_count, aio->ao, aio->ao_surf,
+                                          aio->ao_x, aio->ao_y, s);
     if (f.layers > 1) return launch_blur_upsample_layered(dm, ao_map, hm, f.tma_ok, a, lo_ao2, f.occ_pitch[lo], f.layers, f.sm_count, s);
     return launch_blur_upsample(dm, ao_map, hm, f.tma_ok, a, lo_ao2, f.occ_pitch[lo], f.sm_count, s);
 }

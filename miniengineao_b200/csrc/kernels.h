@@ -238,13 +238,15 @@ cudaError_t launch_blur_upsample_layered(const CUtensorMap &lo_depth_map, const 
 // The first and the last kernel of the frame in a form that reaches the array through a surface object (surface_io.cuh: kSurf2D /
 // kSurfLayered / kSurfCube); the arguments are the layered ones (layers >= 1, whole frame), the intermediates stay in the arena and the
 // other kernels are the existing ones.  prepare: in_format f32 or D16 (no CUDA array holds D24S8); upsample: the final level only
-// (hi_depth = LinearDepth, no hi_ao; a.out is unused).  Separate kernels and translation units (*_array.cu).
+// (hi_depth = LinearDepth, no hi_ao; a.out is unused).  Frame pixel (x, y) is the depth array's texel (depth_x + x, depth_y + y) and
+// the AO array's (ao_x + x, ao_y + y): a viewport of a larger array (meao_render_arrays_at), whose fit the caller has checked.
+// Separate kernels and translation units (*_array.cu).
 enum { kSurf2D = 0, kSurfLayered = 1, kSurfCube = 2 };    // how a surface's layer coordinate is addressed (the array's shape)
-cudaError_t launch_prepare_depth_array(const PrepareArgs &a, cudaSurfaceObject_t depth, int surf_kind, int layers, cudaStream_t s,
-                                       const struct LayerZ *layer_zb = nullptr);
+cudaError_t launch_prepare_depth_array(const PrepareArgs &a, cudaSurfaceObject_t depth, int surf_kind, int depth_x, int depth_y, int layers,
+                                       cudaStream_t s, const struct LayerZ *layer_zb = nullptr);
 cudaError_t launch_blur_upsample_array(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
                                        const UpsampleArgs &a, const uint8_t *lo_ao2, int lo_a2pitch, int layers, int sm_count,
-                                       cudaSurfaceObject_t out, int surf_kind, cudaStream_t s);
+                                       cudaSurfaceObject_t out, int surf_kind, int ao_x, int ao_y, cudaStream_t s);
 
 // ---- debug: synthesise a TiledDepth<k> view (reference layout [16][sh][sw], f16 bits) ----------
 cudaError_t launch_synth_tiled(const float *low, int lw, int lh, int lpitch, int sw, int sh, float pad,

@@ -736,9 +736,12 @@ int own_ao(MeaoCtx *c, int id, cudaStream_t s)
 }
 
 std::mutex g_event_mutex;
-// arrays: meao_bind_event_arrays.  Otherwise a pointer frame at the pitches `pitch`, or, with tight (meao_bind_event), at the tight pitches
-// of the context when the event runs -- a meao_resize between binding and rendering keeps meaning what it meant before.
-struct EventBinding { MeaoCtx *ctx; const void *depth; int kind; void *out; void *stream; bool arrays; bool tight; ViewPitch pitch; };
+// arrays: meao_bind_event_arrays(_at), at the viewport origins `org` (depth x, y, AO x, y), checked again at the size of the frame
+// each time the event runs; exact: meao_bind_event_arrays (W x H arrays).  Otherwise a pointer frame at the pitches `pitch`, or, with
+// tight (meao_bind_event), at the tight pitches of the context when the event runs -- a meao_resize between binding and rendering keeps
+// meaning what it meant before.
+struct EventBinding { MeaoCtx *ctx; const void *depth; int kind; void *out; void *stream; bool arrays; bool tight; ViewPitch pitch;
+                      int org[4] = {0, 0, 0, 0}; bool exact = false; };
 std::map<int, EventBinding> g_events;
 
 }  // namespace
@@ -1546,15 +1549,17 @@ int meao_render_pitched(MeaoCtx *c, const void *depth, int64_t depth_row_pitch, 
 namespace {
 constexpr int kArrayGraphKind = 400;        // GraphKey.kind of an array frame: 400 + depth kind
 
-// What a cudaArray_t is, checked against the context on the host before anything is launched.  elem_bits / is_float: the one
-// channel the role needs.  Returns 0 and the layer addressing, or fails with a message naming the field.
-int check_array(MeaoCtx *c, const void *arr, const char *role, int elem_bits, bool is_float, int *surf_kind)
+// What a cudaArray_t is, checked against the context on the host before anything is launched.  role: "depth" or "ao", the prefix of
+// the fields named in a refusal (<role>_array, <role>_x, <role>_y).  elem_bits / is_float: the one channel the role needs.  exact: the
+// extent must be the context's W x H (meao_render_arrays); otherwise the W x H viewport at (x, y) must lie inside it.  Returns 0 and
+// the layer addressing, or fails with a message naming the field.
+int check_array(MeaoCtx *c, const void *arr, const char *role, int elem_bits, bool is_float, int x, int y, bool exact, int *surf_kind)
 {
     cudaChannelFormatDesc d{};
     cudaExtent e{};
     unsigned int flags = 0;
     const cudaError_t err = cudaArrayGetInfo(&d, &e, &flags, (cudaArray_t)arr);
-    if (err != cudaSuccess) { cudaGetLastError(); return fail(c, MEAO_ERR_INVALID, "%s: not a CUDA array (cudaArrayGetInfo: %s)", role, cudaGetErrorString(err)); }
+    if (err != cudaSuccess) { cudaGetLastError(); return fail(c, MEAO_ERR_INVALID, "%s_array: not a CUDA array (cudaArrayGetInfo: %s)", role, cudaGetErrorString(err)); }
     const bool one_channel = d.x == elem_bits && d.y == 0 && d.z == 0 && d.w == 0;
     bool kind_ok;
     if (is_float) kind_ok = d.f == cudaChannelFormatKindFloat;
@@ -1562,24 +1567,33 @@ int check_array(MeaoCtx *c, const void *arr, const char *role, int elem_bits, bo
                    (elem_bits == 8 && d.f == cudaChannelFormatKindUnsignedNormalized8X1) ||
                    (elem_bits == 16 && d.f == cudaChannelFormatKindUnsignedNormalized16X1);
     if (!one_channel || !kind_ok)
-        return fail(c, MEAO_ERR_INVALID, "%s: channel format (%d,%d,%d,%d bits, kind %d) is not one %d-bit %s channel", role, d.x, d.y, d.z, d.w, (int)d.f,
+        return fail(c, MEAO_ERR_INVALID, "%s_array: channel format (%d,%d,%d,%d bits, kind %d) is not one %d-bit %s channel", role, d.x, d.y, d.z, d.w, (int)d.f,
                     elem_bits, is_float ? "float" : "unsigned (normalised or not)");
-    if ((int)e.width != c->W || (int)e.height != c->H || e.width != (size_t)c->W || e.height != (size_t)c->H)
-        return fail(c, MEAO_ERR_INVALID, "%s: extent %zux%zu differs from the context's %dx%d", role, e.width, e.height, c->W, c->H);
+    if (exact) {
+        if ((int)e.width != c->W || (int)e.height != c->H || e.width != (size_t)c->W || e.height != (size_t)c->H)
+            return fail(c, MEAO_ERR_INVALID, "%s_array: extent %zux%zu differs from the context's %dx%d", role, e.width, e.height, c->W, c->H);
+    } else {
+        if (x < 0) return fail(c, MEAO_ERR_INVALID, "%s_x = %d: the viewport origin is negative", role, x);
+        if (y < 0) return fail(c, MEAO_ERR_INVALID, "%s_y = %d: the viewport origin is negative", role, y);
+        if ((size_t)x + (size_t)c->W > e.width)
+            return fail(c, MEAO_ERR_INVALID, "%s_x = %d: the %dx%d viewport overflows %s_array's width %zu", role, x, c->W, c->H, role, e.width);
+        if ((size_t)y + (size_t)c->H > e.height)
+            return fail(c, MEAO_ERR_INVALID, "%s_y = %d: the %dx%d viewport overflows %s_array's height %zu", role, y, c->W, c->H, role, e.height);
+    }
     if (!(flags & cudaArraySurfaceLoadStore))
-        return fail(c, MEAO_ERR_INVALID, "%s: flags 0x%x lack cudaArraySurfaceLoadStore (register the resource with cudaGraphicsRegisterFlagsSurfaceLoadStore)", role, flags);
+        return fail(c, MEAO_ERR_INVALID, "%s_array: flags 0x%x lack cudaArraySurfaceLoadStore (register the resource with cudaGraphicsRegisterFlagsSurfaceLoadStore)", role, flags);
     int layers;
     if (flags & cudaArrayCubemap) {
-        if (flags & cudaArrayLayered) return fail(c, MEAO_ERR_UNSUPPORTED, "%s: cube-map arrays (cudaArrayCubemap | cudaArrayLayered) are not supported", role);
+        if (flags & cudaArrayLayered) return fail(c, MEAO_ERR_UNSUPPORTED, "%s_array: cube-map arrays (cudaArrayCubemap | cudaArrayLayered) are not supported", role);
         layers = 6; *surf_kind = kSurfCube;
     } else if (flags & cudaArrayLayered) {
         layers = e.depth > 0 ? (int)e.depth : 1; *surf_kind = kSurfLayered;
     } else {
-        if (e.depth > 1) return fail(c, MEAO_ERR_INVALID, "%s: depth %zu: a 3-D array is not a 2-D or layered image", role, e.depth);
+        if (e.depth > 1) return fail(c, MEAO_ERR_INVALID, "%s_array: depth %zu: a 3-D array is not a 2-D or layered image", role, e.depth);
         layers = 1; *surf_kind = kSurf2D;
     }
     if (layers != c->layers)
-        return fail(c, MEAO_ERR_INVALID, "%s: layer count %d differs from the context's %d (meao_set_layers)", role, layers, c->layers);
+        return fail(c, MEAO_ERR_INVALID, "%s_array: layer count %d differs from the context's %d (meao_set_layers)", role, layers, c->layers);
     return 0;
 }
 
@@ -1597,8 +1611,9 @@ int surface_of(MeaoCtx *c, const void *arr, cudaSurfaceObject_t *out)
     return 0;
 }
 
-// every check of meao_render_arrays / meao_bind_event_arrays; on success `io` holds the surfaces of a frame (made on first use)
-int prepare_arrays(MeaoCtx *c, const void *depth_array, int kind, const void *ao_array, ArrayIO *io)
+// every check of meao_render_arrays(_at) / meao_bind_event_arrays(_at); on success `io` holds the surfaces of a frame (made on first use)
+// and its viewport origins.  exact: both arrays must be W x H, the origins are (0, 0) (the entry points without _at).
+int prepare_arrays(MeaoCtx *c, const void *depth_array, int dx, int dy, int kind, const void *ao_array, int ax, int ay, bool exact, ArrayIO *io)
 {
     if (!depth_array || !ao_array) return fail(c, MEAO_ERR_INVALID, "depth_array / ao_array is NULL");
     if (kind < MEAO_DEPTH_RAW_F32 || kind > MEAO_DEPTH_RAW_D24S8) return fail(c, MEAO_ERR_INVALID, "bad depth kind %d", kind);
@@ -1606,16 +1621,21 @@ int prepare_arrays(MeaoCtx *c, const void *depth_array, int kind, const void *ao
     if (c->band0 != 0 || c->band1 != c->H) return fail(c, MEAO_ERR_UNSUPPORTED, "CUDA-array frames need a whole-frame context (no row band)");
     int rc;
     const bool d16 = kind == MEAO_DEPTH_RAW_D16_UNORM;
-    if ((rc = check_array(c, depth_array, "depth_array", d16 ? 16 : 32, !d16, &io->depth_surf))) return rc;
-    if ((rc = check_array(c, ao_array, "ao_array", 8, false, &io->ao_surf))) return rc;
+    if ((rc = check_array(c, depth_array, "depth", d16 ? 16 : 32, !d16, dx, dy, exact, &io->depth_surf))) return rc;
+    if ((rc = check_array(c, ao_array, "ao", 8, false, ax, ay, exact, &io->ao_surf))) return rc;
     if ((rc = surface_of(c, depth_array, &io->depth))) return rc;
     if ((rc = surface_of(c, ao_array, &io->ao))) return rc;
     io->ao_array = ao_array;
+    io->depth_x = dx; io->depth_y = dy; io->ao_x = ax; io->ao_y = ay;
     return 0;
 }
-}  // namespace
 
-int meao_render_arrays(MeaoCtx *c, const void *depth_array, int32_t kind, void *ao_array, void *stream)
+// GraphKey.p[2] / p[3] of an array frame: a viewport origin, so that a frame at other origins never replays a graph recorded for these
+// ((0, 0) is nullptr: meao_render_arrays's key)
+const void *origin_key(int x, int y) { return (const void *)(uintptr_t)(((uint64_t)(uint32_t)x << 32) | (uint32_t)y); }
+
+// meao_render_arrays (exact) and meao_render_arrays_at: one path
+int render_arrays(MeaoCtx *c, const void *depth_array, int dx, int dy, int kind, void *ao_array, int ax, int ay, bool exact, void *stream)
 {
     bool capturing;
     int rc = frame_ready(c, (cudaStream_t)stream, &capturing); if (rc) return rc;
@@ -1624,16 +1644,28 @@ int meao_render_arrays(MeaoCtx *c, const void *depth_array, int32_t kind, void *
         return fail(c, MEAO_ERR_INVALID, "cannot record into the stream's capture: an array this context has not rendered with needs a surface "
                                          "object first; issue one frame with these arrays outside the capture first");
     ArrayIO io;
-    if ((rc = prepare_arrays(c, depth_array, kind, ao_array, &io))) return rc;
+    if ((rc = prepare_arrays(c, depth_array, dx, dy, kind, ao_array, ax, ay, exact, &io))) return rc;
     // the frame graph of meao_render with its first and last node reading / writing the arrays
     NvtxRange nv("meao::frame_arrays");
-    const MeaoCtx::GraphKey key{{depth_array, ao_array, nullptr, nullptr}, kArrayGraphKind + kind};
+    const MeaoCtx::GraphKey key{{depth_array, ao_array, origin_key(dx, dy), origin_key(ax, ay)}, kArrayGraphKind + kind};
     c->last_kind = kind; c->last_out = ao_array;
     return launch_cached(c, key, (cudaStream_t)stream, capturing, [&](cudaStream_t cs, int pdl) {
         FrameIO fio = frame_io(c, nullptr, kind, nullptr, false);
         fio.aio = &io;
         return record_frame_dag(c, fio, cs, 0, pdl);
     });
+}
+}  // namespace
+
+int meao_render_arrays(MeaoCtx *c, const void *depth_array, int32_t kind, void *ao_array, void *stream)
+{
+    return render_arrays(c, depth_array, 0, 0, kind, ao_array, 0, 0, true, stream);
+}
+
+int meao_render_arrays_at(MeaoCtx *c, const void *depth_array, int32_t depth_x, int32_t depth_y, int32_t kind, void *ao_array, int32_t ao_x,
+                          int32_t ao_y, void *stream)
+{
+    return render_arrays(c, depth_array, depth_x, depth_y, kind, ao_array, ao_x, ao_y, false, stream);
 }
 
 int meao_release_array(MeaoCtx *c, const void *array)
@@ -1945,7 +1977,9 @@ int meao_bind_event_pitched(MeaoCtx *c, int32_t event_id, const void *depth, int
     return MEAO_OK;
 }
 
-int meao_bind_event_arrays(MeaoCtx *c, int32_t event_id, const void *depth_array, int32_t kind, void *ao_array, void *stream)
+namespace {
+int bind_event_arrays(MeaoCtx *c, int32_t event_id, const void *depth_array, int dx, int dy, int kind, void *ao_array, int ax, int ay, bool exact,
+                      void *stream)
 {
     if (!c) return MEAO_ERR_INVALID;
     if (!depth_array && !ao_array) {
@@ -1956,10 +1990,22 @@ int meao_bind_event_arrays(MeaoCtx *c, int32_t event_id, const void *depth_array
     // checked now: the plugin event cannot report an error
     int rc = ensure_ready(c); if (rc) return rc;
     ArrayIO io;
-    if ((rc = prepare_arrays(c, depth_array, kind, ao_array, &io))) return rc;
+    if ((rc = prepare_arrays(c, depth_array, dx, dy, kind, ao_array, ax, ay, exact, &io))) return rc;
     std::lock_guard<std::mutex> g(g_event_mutex);
-    g_events[event_id] = EventBinding{c, depth_array, kind, ao_array, stream, true, false, ViewPitch{}};
+    g_events[event_id] = EventBinding{c, depth_array, kind, ao_array, stream, true, false, ViewPitch{}, {dx, dy, ax, ay}, exact};
     return MEAO_OK;
+}
+}  // namespace
+
+int meao_bind_event_arrays(MeaoCtx *c, int32_t event_id, const void *depth_array, int32_t kind, void *ao_array, void *stream)
+{
+    return bind_event_arrays(c, event_id, depth_array, 0, 0, kind, ao_array, 0, 0, true, stream);
+}
+
+int meao_bind_event_arrays_at(MeaoCtx *c, int32_t event_id, const void *depth_array, int32_t depth_x, int32_t depth_y, int32_t kind,
+                              void *ao_array, int32_t ao_x, int32_t ao_y, void *stream)
+{
+    return bind_event_arrays(c, event_id, depth_array, depth_x, depth_y, kind, ao_array, ao_x, ao_y, false, stream);
 }
 
 void meao_render_event(int event_id)
@@ -1971,7 +2017,7 @@ void meao_render_event(int event_id)
         if (it == g_events.end()) return;
         b = it->second;
     }
-    if (b.arrays) meao_render_arrays(b.ctx, b.depth, b.kind, b.out, b.stream);
+    if (b.arrays) render_arrays(b.ctx, b.depth, b.org[0], b.org[1], b.kind, b.out, b.org[2], b.org[3], b.exact, b.stream);
     else if (b.tight) meao_render(b.ctx, b.depth, b.kind, b.out, b.stream);      // meao_render_pitched at the tight pitches of now
     else meao_render_pitched(b.ctx, b.depth, b.pitch.depth_row, b.pitch.depth_layer, b.kind, b.out, b.pitch.ao_row, b.pitch.ao_layer, b.stream);
 }
