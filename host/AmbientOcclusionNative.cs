@@ -38,6 +38,14 @@ namespace MiniEngineAO
             public int reversed_z;
         }
 
+        // Where layer l of a CUDA-array frame reads its depth and writes its AO (meao.h: MeaoLayerViewport)
+        [StructLayout(LayoutKind.Sequential)]
+        public struct MeaoLayerViewport
+        {
+            public int depth_x, depth_y, depth_slice;
+            public int ao_x, ao_y, ao_slice;
+        }
+
         [StructLayout(LayoutKind.Sequential)]
         public struct MeaoDeviceCfg { public int device; public uint flags; }
 
@@ -66,6 +74,8 @@ namespace MiniEngineAO
         // one camera per layer (split-screen viewports, mirrors, batches from several cameras); null with count 0 clears the table
         [DllImport(Lib)] public static extern int meao_set_layer_cameras(IntPtr ctx, [In] MeaoCamera[] cameras, int count);
         [DllImport(Lib)] public static extern int meao_get_layer_cameras(IntPtr ctx, [Out] MeaoCamera[] cameras, int capacity);
+        [DllImport(Lib)] public static extern int meao_set_layer_viewports(IntPtr ctx, [In] MeaoLayerViewport[] views, int count);
+        [DllImport(Lib)] public static extern int meao_get_layer_viewports(IntPtr ctx, [Out] MeaoLayerViewport[] views, int capacity);
         [DllImport(Lib)] public static extern int meao_render(IntPtr ctx, IntPtr depthDev, int depthKind, IntPtr aoOutDev, IntPtr stream);
         [DllImport(Lib)] public static extern int meao_render_host(IntPtr ctx, float[] depth, int depthKind, byte[] aoOut);
         [DllImport(Lib)] public static extern int meao_bind_event(IntPtr ctx, int eventId, IntPtr depthDev, int depthKind, IntPtr aoOutDev, IntPtr stream);
@@ -136,6 +146,12 @@ namespace MiniEngineAO
         // renders with this component's camera.  Each must have this camera's pixel size; Length must equal Layers.
         Camera[] _layerCameras;
         public Camera[] LayerCameras { get { return _layerCameras; } set { _layerCameras = value; } }
+        // Where each layer lives in the depth and AO targets (split-screen players in one texture, a side-by-side stereo pair, cube faces
+        // in a 2-D atlas); null: every layer at the origin of its own slice.  Length must equal Layers.  Honoured by the frames of
+        // meao_render, meao_render_pitched and meao_render_arrays and the events bound to them; the host-buffer calls, the stage calls,
+        // the debug views and the composites keep the tight layer layout.
+        MeaoNative.MeaoLayerViewport[] _layerViewports;
+        public MeaoNative.MeaoLayerViewport[] LayerViewports { get { return _layerViewports; } set { _layerViewports = value; } }
         // Dynamic resolution scaling: the largest camera pixel size the render size moves within (zero: none).  Reserved once
         // (meao_reserve); a size change inside it then costs no allocation, device synchronise, graph teardown or event rebind.
         Vector2Int _maxResolution;
@@ -211,6 +227,10 @@ namespace MiniEngineAO
             MeaoNative.Check(_ctx, layered);
             rebuild |= layered == 1;
             rebuild |= SetLayerCameras() == 1;                                               // after meao_set_layers, which clears the table
+            var viewports = _layerViewports == null ? MeaoNative.meao_set_layer_viewports(_ctx, null, 0)
+                                                    : MeaoNative.meao_set_layer_viewports(_ctx, _layerViewports, _layerViewports.Length);
+            MeaoNative.Check(_ctx, viewports);
+            rebuild |= viewports == 1;                                                       // after meao_set_layers too
             var width = _camera.pixelWidth * (stereo ? 2 : 1);
             rebuild |= Reserve(width, _camera.pixelHeight, stereo);                          // before meao_resize, doubled like the width
             var resized = MeaoNative.meao_resize(_ctx, width, _camera.pixelHeight);          // :338-341

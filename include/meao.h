@@ -38,7 +38,9 @@ extern "C" {
                               *    + meao_render_pitched / meao_bind_event_pitched (depth and AO with their own row and layer pitch; additive)
                               *    + meao_reserve / meao_reservation (dynamic resolution; additive)
                               *    + meao_frame_generation (frames inside a caller's CUDA graph; additive)
-                              *    + meao_render_arrays_at / meao_bind_event_arrays_at (viewports of larger CUDA arrays; additive) */
+                              *    + meao_render_arrays_at / meao_bind_event_arrays_at (viewports of larger CUDA arrays; additive)
+                              *    + MeaoLayerViewport, meao_set_layer_viewports / meao_get_layer_viewports (each layer at its own
+                              *      viewport of shared CUDA arrays: split-screen, side-by-side stereo, cube atlases; additive) */
 
 typedef struct MeaoCtx MeaoCtx;
 
@@ -235,6 +237,43 @@ int meao_set_layers(MeaoCtx *ctx, int32_t layers);
 int meao_set_layer_cameras(MeaoCtx *ctx, const MeaoCamera *cameras, int32_t count);
 /* Copies the table into out (capacity entries; MEAO_ERR_INVALID if it does not fit) and returns its entry count (0 = no table). */
 int meao_get_layer_cameras(const MeaoCtx *ctx, MeaoCamera *out, int32_t capacity);
+/* Per-layer viewports for layered frames: where each layer of the frame lives in the caller's arrays or buffers, so that several views
+ * share one render target (2- and 4-player split-screen in one 2-D texture, a side-by-side stereo pair, the six faces of a cube into
+ * the cells of one 2-D atlas).  Layer l of a meao_render_arrays frame reads the depth texels [depth_x, depth_x + W) x [depth_y,
+ * depth_y + H) of the depth array's layer depth_slice and writes its AO into [ao_x, ao_x + W) x [ao_y, ao_y + H) of the AO array's layer
+ * ao_slice, W x H being the context's current size; it is bit-identical to a single-layer meao_render_arrays_at (meao_render_pitched)
+ * frame of that rectangle with that layer's camera.  No texel outside the rectangles is read or written.  With meao_set_layer_cameras each view also has its
+ * own camera.
+ * count must equal meao_set_layers; views == NULL with count == 0 clears the table.  Every coordinate must be >= 0; a refusal
+ * returns MEAO_ERR_INVALID, names the layer and field in meao_last_error and leaves the previous table in place.  A change of the
+ * layer count clears the table.
+ * A frame constant: changing the entries of a set table returns 1 and the next frame takes the new table without a re-plan, a device
+ * synchronise or a graph instantiation; setting the same table again returns 0.  Setting a table where there was none, or clearing
+ * one, switches kernels: it returns 1 and re-plans like a structural change.  meao_frame_generation moves with every change.  A frame
+ * whose new table is not written yet is refused inside a caller's capture, like new camera tables.  Works on plan-only contexts.
+ * Checked at every frame, against the current W x H (a reserved context may change size under a set table).  CUDA arrays: every
+ * rectangle fits its array (x + W <= width, y + H <= height) and every slice is below the array's layer count (1 for a 2-D array, n for a layered one,
+ * 6 for a cube map) -- the context's layer count no longer has to equal the arrays'; and no two layers' AO rectangles on one slice
+ * share a texel (depth rectangles may overlap: the depth is only read).  That test is linear in the layer count and runs once per
+ * (table, size), and not at all at a size no larger in either dimension than one that passed.  A refusal returns MEAO_ERR_INVALID naming the layer and field and launches nothing; so does a bound event.
+ * Pointer frames (meao_render_pitched, and meao_render at its tight pitches): slice s of a view starts s x layer pitch bytes in, and
+ * the rectangle's rows are the view's rows.  Every row of a rectangle must fit its row pitch ((x + W) x element size <= row pitch);
+ * when some slice is > 0, every rectangle must fit inside its slice (and the depth layer pitch be a whole number of elements); the
+ * depth and AO views' byte extents, from each base to the end of its last rectangle, must not intersect.  A layer whose
+ * rectangle starts misaligned for the vector accesses (16 bytes for the depth, 8 for the AO, with rows of such pitches) takes the
+ * element-wise path for its own pixels, with the same result.
+ * Which calls honour it: meao_render_arrays, meao_render_pitched, meao_render, and the events that render through them
+ * (meao_bind_event_arrays, meao_bind_event_pitched, meao_bind_event).  meao_render_arrays_at (and its event) names one origin for
+ * every layer and is refused with MEAO_ERR_INVALID while a table is set.  The host-buffer calls (meao_render_host(_async)), the
+ * stage API, meao_profile_frame, meao_debug_view and the composites keep the tight layer layout and ignore the table.  Row bands and
+ * tables exclude each other (MEAO_ERR_UNSUPPORTED). */
+typedef struct {
+    int32_t depth_x, depth_y, depth_slice;  /* layer l reads depth [x, x+W) x [y, y+H) of slice depth_slice */
+    int32_t ao_x, ao_y, ao_slice;           /* and writes its AO into [x, x+W) x [y, y+H) of slice ao_slice */
+} MeaoLayerViewport;
+int meao_set_layer_viewports(MeaoCtx *ctx, const MeaoLayerViewport *views, int32_t count);
+/* Copies the table into out (capacity entries; MEAO_ERR_INVALID if it does not fit) and returns its entry count (0 = no table). */
+int meao_get_layer_viewports(const MeaoCtx *ctx, MeaoLayerViewport *out, int32_t capacity);
 
 /* ---- the frame ------------------------------------------------------------------------------- */
 /* replaces: replay of the "SSAO" command buffer, steps 1-10 of RebuildCommandBuffers (AO.cs:511-531):
@@ -501,6 +540,7 @@ MeaoRenderEventFunc meao_get_render_event_func(void);
  * nothing and leaves the caller's capture valid (meao_last_error says why: "issue one frame outside the capture first") when
  *   - a structural change is pending (a re-plan synchronises the device),
  *   - the per-layer camera tables are still to be written: after a frame-constant change, or on the first frame at a size,
+ *   - a changed layer-viewport table (meao_set_layer_viewports) is still to be written,
  *   - or, for meao_render_arrays(_at), the context has not rendered with one of the arrays yet (its surface object is made then).
  * One frame of the same form issued outside the capture settles the context; torch's warm-up before torch.cuda.graph does that.
  * A capture that has been invalidated returns MEAO_ERR_CUDA and records nothing.

@@ -27,6 +27,11 @@ class MeaoCamera(C.Structure):
                 ("tan_half_fov_h", C.c_float), ("reversed_z", C.c_int32)]
 
 
+class MeaoLayerViewport(C.Structure):
+    _fields_ = [("depth_x", C.c_int32), ("depth_y", C.c_int32), ("depth_slice", C.c_int32),
+                ("ao_x", C.c_int32), ("ao_y", C.c_int32), ("ao_slice", C.c_int32)]
+
+
 class MeaoDeviceCfg(C.Structure):
     _fields_ = [("device", C.c_int32), ("flags", C.c_uint32)]
 
@@ -73,6 +78,8 @@ SIGNATURES = {
     "meao_set_layers": (C.c_int, [C.c_void_p, C.c_int32]),
     "meao_set_layer_cameras": (C.c_int, [C.c_void_p, C.POINTER(MeaoCamera), C.c_int32]),
     "meao_get_layer_cameras": (C.c_int, [C.c_void_p, C.POINTER(MeaoCamera), C.c_int32]),
+    "meao_set_layer_viewports": (C.c_int, [C.c_void_p, C.POINTER(MeaoLayerViewport), C.c_int32]),
+    "meao_get_layer_viewports": (C.c_int, [C.c_void_p, C.POINTER(MeaoLayerViewport), C.c_int32]),
     "meao_render": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "meao_render_pitched": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_int64, C.c_int64,
                                       C.c_void_p]),

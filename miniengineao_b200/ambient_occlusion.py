@@ -84,6 +84,11 @@ class AmbientOcclusion:
         # one Camera per layer (meao_set_layer_cameras): split-screen viewports, mirrors, batches from several cameras; None = every
         # layer uses `camera`.  Each entry must match the main camera's pixelWidth, pixelHeight and usesReversedZBuffer.
         self.layerCameras: list[Camera] | None = None
+        # where each layer lives in the caller's depth and AO (meao_set_layer_viewports): one (depth_x, depth_y, depth_slice, ao_x,
+        # ao_y, ao_slice) per layer -- split-screen players in one texture, a side-by-side stereo pair, cube faces in a 2-D atlas.  Honoured
+        # by render (and its plugin event), the pitched frames and render_arrays (not with origins); render_host, the stage calls, the
+        # debug views and the composites keep the tight layer layout.  None = every layer at (0, 0) of its own slice
+        self.layerViewports: list[tuple[int, int, int, int, int, int]] | None = None
         # dynamic resolution: the largest (pixelWidth, pixelHeight) the camera will have, reserved once (meao_reserve) so that a size
         # change inside it costs no allocation, device synchronise or graph teardown; None = every size change re-allocates
         self.maxResolution: tuple[int, int] | None = None
@@ -155,6 +160,7 @@ class AmbientOcclusion:
         width = cam.pixelWidth * (2 if stereo else 1)                                                # AO.cs:338-341, 501-504
         layered = self._check(self._lib.meao_set_layers(self._ctx, int(self.layers))) == 1           # re-allocates like a resize
         rebuild |= self._apply_layer_cameras()
+        rebuild |= self._apply_layer_viewports()
         reallocated = layered | self._apply_reservation(width, cam.pixelHeight, stereo)
         resized = self._check(self._lib.meao_resize(self._ctx, width, cam.pixelHeight)) == 1          # CheckBaseDimensions
         reallocated |= resized and self._reserved == (0, 0)       # inside a reservation a resize allocates nothing
@@ -206,6 +212,19 @@ class AmbientOcclusion:
         arr = (N.MeaoCamera * len(cams))(*[N.MeaoCamera(c.nearClipPlane, c.farClipPlane, 1.0 / c.projection00, int(c.usesReversedZBuffer))
                                            for c in cams])
         return self._check(self._lib.meao_set_layer_cameras(self._ctx, arr, len(cams))) == 1
+
+    def _apply_layer_viewports(self) -> bool:
+        """Hands layerViewports to meao_set_layer_viewports (after meao_set_layers, which clears the table); True if a value changed."""
+        views = self.layerViewports
+        if views is None:
+            return self._check(self._lib.meao_set_layer_viewports(self._ctx, None, 0)) == 1
+        if len(views) != int(self.layers):
+            raise ValueError(f"layerViewports has {len(views)} entries for {int(self.layers)} layers")
+        for i, v in enumerate(views):
+            if len(v) != 6:
+                raise ValueError(f"layerViewports[{i}] = {v!r}: (depth_x, depth_y, depth_slice, ao_x, ao_y, ao_slice) expected")
+        arr = (N.MeaoLayerViewport * len(views))(*[N.MeaoLayerViewport(*map(int, v)) for v in views])
+        return self._check(self._lib.meao_set_layer_viewports(self._ctx, arr, len(views))) == 1
 
     # ---- frame ----------------------------------------------------------------------------------
     @staticmethod

@@ -3,7 +3,7 @@
 // by it -- in libmeao and in the emulator (tests/emu/frame_driver.cpp) alike.
 //
 // Order: BandFlags (offset 0 in every arena: the neighbour bands address it through their peer mapping), the tile counters of the
-// persistent upsample grids, kSizeSlots per-layer camera table slots, LinearDepth, the AO result, LowDepth / Occlusion / Combined /
+// persistent upsample grids, kSizeSlots per-layer camera table slots, the layer-viewport table, LinearDepth, the AO result, LowDepth / Occlusion / Combined /
 // HighQuality of levels 1..4, and the two host-staging slots.  Every entry starts on a 256-byte boundary; rows start on 128-byte
 // boundaries (pitches below).  Every entry's size is monotone in W and H, so the entries of a W' x H' frame with W' <= W and H' <= H
 // lie inside the arena of W x H, each at an offset no larger than the W x H one (dynamic resolution, meao_reserve).
@@ -25,6 +25,7 @@ struct ArenaLayout {
     size_t ctr;                         // 8 words: cursor + finished-CTA count of each persistent blur_upsample grid
     size_t table0, table_stride;        // slot s: LayerZ[L] at table0 + s * table_stride, then LayerRender[8 L] at table_ren below
     size_t table_ren;                   // offset of the LayerRender table inside a slot
+    size_t views;                       // LayerView[L] (meao_set_layer_viewports): one table for every frame size
     size_t lin, result, low[5], occ[5], comb[4], hq[5];
     size_t depth_stage[2], ao_stage[2]; // L x W x H f32 (the largest depth element) and L x W x H bytes each
     size_t bytes;                       // the arena's size
@@ -52,6 +53,7 @@ inline ArenaLayout arena_layout(int W, int H, int L)
     a.table_ren = zb_bytes;
     a.table_stride = zb_bytes + (ren_bytes + 255) / 256 * 256;
     a.table0 = take(kSizeSlots * a.table_stride);
+    a.views = take(n * sizeof(LayerView));
     a.lin = take(n * a.lin_pitch * a.lh[0] * 2);
     a.result = take(n * a.result_pitch * a.lh[0]);
     for (int k = 1; k <= 4; k++) {

@@ -24,53 +24,7 @@ namespace {
 #include "blur_upsample_layer_args.inc"
 #include "depth_in.cuh"
 
-// The LinearDepth values of pixels px0 .. px0 + 7 of row py of layer `layer` (those inside the row: all eight when `full`): load
-// their raw depth, linearise it (DS1:37-48), round it to f16 and store it to LinearDepth at `lin` (this thread's first pixel; the
-// 16-byte store is aligned because px0 % 8 == 0 and rows are 128-byte pitched).  Returns the packed halves (pixel 0 in the low half
-// of .x): what the 128-bit LinearDepth load of the kernel that reads LinearDepth returns.
-// LAYERED: the layer's ZBufferParams come from din.layer_zb when it is set (per-layer cameras).
-template <int IN, bool LAYERED = false>
-__device__ __forceinline__ uint4 linearize_pixels8(const DepthIn &din, int layer, int py, int px0, int hiw, int hih, bool full, __half *lin)
-{
-    const void *depth = reinterpret_cast<const char *>(din.depth) + (size_t)layer * din.depth_layer_pitch * (IN == IN_D16 ? 2 : 4);
-    float v[8], d[8];
-    load8<IN>(depth, (size_t)(py - din.depth_row0) * din.depth_pitch + px0, full && din.vec_ok, hiw - px0, v);
-    float zbx = din.zbx, zby = din.zby;
-    if (LAYERED && din.layer_zb) { zbx = __ldg(&din.layer_zb[layer].zbx); zby = __ldg(&din.layer_zb[layer].zby); }
-    if (!din.raw) linearize8<false, true>(v, zbx, zby, d);
-    else if (din.reversed_z) linearize8<true, true>(v, zbx, zby, d);
-    else linearize8<true, false>(v, zbx, zby, d);
-    const __half2 h0 = __floats2half2_rn(d[0], d[1]), h1 = __floats2half2_rn(d[2], d[3]);
-    const __half2 h2 = __floats2half2_rn(d[4], d[5]), h3 = __floats2half2_rn(d[6], d[7]);
-    uint4 pk;
-    pk.x = *reinterpret_cast<const uint32_t *>(&h0); pk.y = *reinterpret_cast<const uint32_t *>(&h1);
-    pk.z = *reinterpret_cast<const uint32_t *>(&h2); pk.w = *reinterpret_cast<const uint32_t *>(&h3);
-    if (full) {
-        *reinterpret_cast<uint4 *>(lin) = pk;                                            // DS1:46
-    } else {
-#pragma unroll
-        for (int e = 0; e < 8; e++) {
-            if (px0 + e >= hiw) break;
-            lin[e] = __float2half_rn(d[e]);
-        }
-    }
-    return pk;
-}
-
-// layer_args of the fused layered kernels: the caller's AO advances by its own layer pitch (DepthIn.ao_layer_pitch, bytes) instead of
-// hih x out_pitch, so a layered AO view keeps the layer pitch of the tensor or allocation it lives in
-__device__ __forceinline__ UpsampleArgs layer_args(const UpsampleArgs &a, int l, long long ao_layer_pitch)
-{
-    UpsampleArgs r = layer_args(a, l);
-    r.out = a.out + (size_t)l * ao_layer_pitch;
-    return r;
-}
-__device__ __forceinline__ UpsamplePreminArgs layer_args(const UpsamplePreminArgs &pa, int l, long long ao_layer_pitch)
-{
-    UpsamplePreminArgs r = layer_args(pa, l);
-    r.base.out = pa.base.out + (size_t)l * ao_layer_pitch;
-    return r;
-}
+#include "blur_upsample_lin_device.inc"
 
 #define MEAO_UPS_LIN 1
 #define MEAO_UPS_PREMIN 0

@@ -75,6 +75,7 @@ struct FrameState {
     // the per-layer camera tables (kernels.h LayerZ / LayerRender): layer_zb[l]; layer_ren[(2 (k - 1) + wide) L + l]
     LayerZ *layer_zb = nullptr;
     LayerRender *layer_ren = nullptr;
+    LayerView *layer_views = nullptr;       // the layer-viewport table (meao_set_layer_viewports), read by the frames that have one set
 
     int sm_count = 132;                     // SMs of the device (132 = H100 SXM for plan-only contexts)
     bool tma_ok = false;
@@ -106,6 +107,7 @@ inline void place_frame(FrameState &f, const ArenaLayout &a, char *base, int slo
     f.tile_ctr = (uint32_t *)(base + a.ctr);
     f.layer_zb = (LayerZ *)(base + a.table0 + (size_t)slot * a.table_stride);
     f.layer_ren = (LayerRender *)((char *)f.layer_zb + a.table_ren);
+    f.layer_views = (LayerView *)(base + a.views);
 }
 
 // One TMA map: w x h elements of elem bytes (4: f32, 1: u8) at base, rows pitch_elems apart, box bw x bh
@@ -398,6 +400,7 @@ struct FrameIO {
     bool fused = false;                 // the final upsample reads and linearises `depth` and writes LinearDepth
     void *ao = nullptr;                 // the final upsample's AO at the pitches of vp (nullptr: tight); nullptr: the result buffer
     const ViewPitch *vp = nullptr;
+    const LayerView *views = nullptr;   // layer l reads and writes the rectangles and slices of views[l] (launch_entry_views)
 };
 
 // Launches schedule entry l of a frame on stream s.  force_tile: render_tile_variant's force.
@@ -413,6 +416,33 @@ inline cudaError_t launch_entry(const FrameState &f, const FrameLaunch &l, const
             return launch_upsample(f, l.level, upsample_args(f, l.level, final_level ? io.ao : nullptr, final_level ? io.vp : nullptr),
                                    io.aio, io.fused ? &io.depth : nullptr, s);
     }
+}
+
+// launch_entry for a frame that may have a layer-viewport table (FrameIO.views): its prepare and its final upsample are the table
+// kernels, every other launch is launch_entry's.  A CUDA-array frame (io.aio) or a fused pointer frame (what meao_render_pitched
+// records).  Apart from launch_entry so that a recorder that never sets a table does not link the table kernels.
+inline cudaError_t launch_entry_views(const FrameState &f, const FrameLaunch &l, const FrameIO &io, int force_tile, cudaStream_t s)
+{
+    const bool final_level = l.stage == kStageUpsample && l.level == 1;
+    if (!io.views || (l.stage != kStagePrepare && !final_level)) return launch_entry(f, l, io, force_tile, s);
+    // the vector accesses of a pointer frame: the host tests the rows (depth row pitch % 16, AO row pitch % 8), each layer its base
+    DepthIn d = io.depth;
+    d.vec_ok = (int64_t)d.depth_pitch * (d.in_format == 1 ? 2 : 4) % 16 == 0;
+    if (l.stage == kStagePrepare) {
+        PrepareArgs a = prepare_args(f, d);
+        if (io.aio) return launch_prepare_depth_array_views(a, io.aio->depth, io.aio->depth_surf, io.views, f.layers, s, f.layer_zb);
+        if (!io.fused) return cudaErrorInvalidValue;
+        return launch_prepare_depth_views(a, io.views, f.layers, s, f.layer_zb);
+    }
+    UpsampleArgs a = upsample_args(f, 1, io.aio ? nullptr : io.ao, io.aio ? nullptr : io.vp);
+    const uint8_t *lo_ao2 = hq_level(f, 1) ? f.hq[1] : nullptr;
+    const CUtensorMap &ao_map = f.plan.variants.single_scale != 0 ? f.maps.occ1_ups : f.maps.ao_ups[1];
+    if (io.aio)
+        return launch_blur_upsample_array_views(f.maps.low_ups[1], ao_map, &f.maps.hq_ups[1], f.tma_ok, a, lo_ao2, f.occ_pitch[1], f.layers,
+                                                f.sm_count, io.aio->ao, io.aio->ao_surf, io.views, s);
+    a.out_vec_ok = a.out_pitch % 8 == 0;
+    return launch_blur_upsample_lin_views(f.maps.low_ups[1], ao_map, &f.maps.hq_ups[1], f.tma_ok, a, lo_ao2, f.occ_pitch[1], d, f.layers,
+                                          f.sm_count, io.views, s);
 }
 
 // ---- the debug buffers (meao_get_buffer, meao_set_buffer, meao_debug_view) ---------------------------------------------------

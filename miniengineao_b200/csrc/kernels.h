@@ -247,6 +247,27 @@ cudaError_t launch_prepare_depth_array(const PrepareArgs &a, cudaSurfaceObject_t
 cudaError_t launch_blur_upsample_array(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
                                        const UpsampleArgs &a, const uint8_t *lo_ao2, int lo_a2pitch, int layers, int sm_count,
                                        cudaSurfaceObject_t out, int surf_kind, int ao_x, int ao_y, cudaStream_t s);
+// Layer viewports (meao_set_layer_viewports): layer l of a layered frame reads the depth texels [depth_x, depth_x + W) x [depth_y,
+// depth_y + H) of the depth array's layer depth_slice and writes its AO into the same rectangle at (ao_x, ao_y) of the AO array's layer
+// ao_slice -- entry l of a table in the context's arena (include/meao.h MeaoLayerViewport, field for field), read by the kernels at
+// their layer (blockIdx.z; the upsample: its tile's layer).  The fit of every rectangle and slice, and that no two AO rectangles share a
+// texel, the caller has checked.  Separate kernels and translation units (*_views.cu), so the existing kernels keep their code.
+struct LayerView { int depth_x, depth_y, depth_slice, ao_x, ao_y, ao_slice; };
+cudaError_t launch_prepare_depth_array_views(const PrepareArgs &a, cudaSurfaceObject_t depth, int surf_kind, const LayerView *views, int layers,
+                                             cudaStream_t s, const struct LayerZ *layer_zb = nullptr);
+cudaError_t launch_blur_upsample_array_views(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map,
+                                             bool use_tma, const UpsampleArgs &a, const uint8_t *lo_ao2, int lo_a2pitch, int layers, int sm_count,
+                                             cudaSurfaceObject_t out, int surf_kind, const LayerView *views, cudaStream_t s);
+// The fused pointer frame with a table (meao_render_pitched): the low-only prepare and the fused final upsample.  The caller's depth and
+// AO are slices of depth_layer_pitch elements / ao_layer_pitch bytes (DepthIn); layer l's rectangle starts at element
+// (depth_slice x depth_layer_pitch + depth_y x depth_pitch + depth_x) of the depth and at byte (ao_slice x ao_layer_pitch + ao_y x
+// out_pitch + ao_x) of the AO.  vec_ok / out_vec_ok hold the rows' alignment only (depth row pitch % 16, AO row pitch % 8); each
+// layer adds its own base's, so a misaligned layer takes the element-wise loads and stores for its own pixels only.
+cudaError_t launch_prepare_depth_views(const PrepareArgs &a, const LayerView *views, int layers, cudaStream_t s,
+                                       const struct LayerZ *layer_zb = nullptr);
+cudaError_t launch_blur_upsample_lin_views(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
+                                           const UpsampleArgs &a, const uint8_t *lo_ao2, int lo_a2pitch, const DepthIn &din, int layers,
+                                           int sm_count, const LayerView *views, cudaStream_t s);
 
 // ---- debug: synthesise a TiledDepth<k> view (reference layout [16][sh][sw], f16 bits) ----------
 cudaError_t launch_synth_tiled(const float *low, int lw, int lh, int lpitch, int sw, int sh, float pad,
@@ -340,6 +361,13 @@ inline const KernelUnit *const kKernelUnits[] = {
 #endif
     &kHaloUnit, &kBandExchangeUnit, &kCompositeUnit, &kDebugViewUnit, &kPrepareDepthLayeredUnit, &kRenderAoLayeredUnit,
     &kBlurUpsampleLayeredUnit, &kPrepareDepthArrayUnit, &kBlurUpsampleArrayUnit, &kBlurUpsampleLinUnit};
+// The layer-viewport units (build.py VIEW_SOURCES), loaded eagerly like the others.  The emulator builds them into a library of their
+// own (tests/emu/layer_views.py), so the emulator's unit list above stays the SOURCES one.
+extern const KernelUnit kPrepareDepthArrayViewsUnit, kBlurUpsampleArrayViewsUnit, kPrepareDepthViewsUnit, kBlurUpsampleLinViewsUnit;
+#ifndef MEAO_EMULATE
+inline const KernelUnit *const kViewKernelUnits[] = {&kPrepareDepthArrayViewsUnit, &kBlurUpsampleArrayViewsUnit, &kPrepareDepthViewsUnit,
+                                                     &kBlurUpsampleLinViewsUnit};
+#endif
 
 // ---- halo pack / unpack: row blocks of pitched buffers <-> contiguous staging, one launch ------
 struct HaloSeg { const float *src; float *dst; int src_pitch, dst_pitch, width, rows; };

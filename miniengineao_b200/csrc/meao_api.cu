@@ -7,7 +7,10 @@
 // "Plan once, replay per frame" maps to: constants + TMA descriptors are rebuilt only when a
 // parameter, the camera or the size changes; a frame is then ten kernel launches (or one CUDA
 // graph launch) on one stream.
+#include <algorithm>
+#include <array>
 #include <cstdarg>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -16,6 +19,8 @@
 #include <map>
 #include <mutex>
 #include <string>
+#include <tuple>
+#include <utility>
 #include <vector>
 #include <unistd.h>
 
@@ -69,6 +74,18 @@ struct MeaoCtx : SizeState {
     MeaoParams params;
     MeaoCamera camera;
     std::vector<MeaoCamera> layer_cams;     // meao_set_layer_cameras: one camera per layer, or empty (every layer uses `camera`)
+    // meao_set_layer_viewports: one viewport per layer, or empty (the tight layer layout).  views_pending: the arena's copy
+    // (FrameState::layer_views) is older than the table; the next frame writes it on its own stream (write_tables).  views_max[i]: the
+    // layer with the largest value of field i (depth_x .. ao_slice), for the per-frame fit tests of arrays.  views_last[r][0] / [1]: the
+    // layer whose rectangle ends last in (y, x) / (slice, y, x) order, for role r (0 depth, 1 AO) -- with every row inside its row pitch
+    // the one whose last byte lies furthest into its slice / into the view (check_view_pitches).  views_checked: the sizes at which the
+    // AO rectangles were found disjoint, none larger than another (a rectangle at a smaller size lies inside the larger one at the same
+    // origin), cleared with the table.
+    std::vector<MeaoLayerViewport> views;
+    bool views_pending = false;
+    int views_max[6] = {0, 0, 0, 0, 0, 0};
+    int views_last[2][2] = {{0, 0}, {0, 0}};
+    std::vector<std::pair<int, int>> views_checked;
     MeaoVariants variants = {0, 0, 0, 0};
     bool plan_dirty = true;                 // a structural input changed: the next frame re-plans (replan)
     // Frame constants (include/meao.h): bumped by every change of MeaoParams or of a camera that keeps the Z direction.  A size whose
@@ -497,8 +514,10 @@ int upload_camera_tables(MeaoCtx *c)
     CUDA_TRY(c, cudaDeviceSynchronize());
     CUDA_TRY(c, cudaMemcpy(c->layer_zb, zb.data(), zb.size() * sizeof(LayerZ), cudaMemcpyHostToDevice));
     CUDA_TRY(c, cudaMemcpy(c->layer_ren, ren.data(), ren.size() * sizeof(LayerRender), cudaMemcpyHostToDevice));
+    if (!c->views.empty()) CUDA_TRY(c, cudaMemcpy(c->layer_views, c->views.data(), c->views.size() * sizeof(LayerView), cudaMemcpyHostToDevice));
     c->cam_table_stale = false;
     c->table_pending = false;
+    c->views_pending = false;
     return 0;
 }
 
@@ -509,6 +528,10 @@ int upload_camera_tables(MeaoCtx *c)
 // the vectors may go when the call returns.
 int write_tables(MeaoCtx *c, cudaStream_t s)
 {
+    if (c->views_pending) {         // a changed layer-viewport table (one for every size): the same stream-order rule
+        CUDA_TRY(c, cudaMemcpyAsync(c->layer_views, c->views.data(), c->views.size() * sizeof(LayerView), cudaMemcpyHostToDevice, s));
+        c->views_pending = false;
+    }
     if (!c->table_pending) return 0;
     std::vector<LayerZ> zb;
     std::vector<LayerRender> ren;
@@ -556,6 +579,7 @@ int refuse_unsettled(MeaoCtx *c)
     const char *why = nullptr;
     if (c->plan_dirty || c->graphs_stale || c->cam_table_stale) why = "a structural change is pending (a re-plan synchronises the device)";
     else if (c->table_pending || c->plan_gen != c->consts_gen) why = "the camera tables of new frame constants or of a new size are not written yet";
+    else if (c->views_pending) why = "a changed layer-viewport table is not written yet";
     if (!why) return 0;
     return fail(c, MEAO_ERR_INVALID, "cannot record into the stream's capture: %s; issue one frame outside the capture first", why);
 }
@@ -619,7 +643,7 @@ int record_launch(MeaoCtx *c, const FrameLaunch &l, const FrameIO &io, cudaStrea
     static const char *nvtx[4] = {"meao::prepare_depth", "meao::render_ao", "meao::render_ao_wide", "meao::blur_upsample"};
     if (l.stage == kStageUpsample && l.level == 1) c->last_out = io.aio ? const_cast<void *>(io.aio->ao_array) : io.ao;
     NvtxRange nv(nvtx[l.stage]);
-    CUDA_TRY(c, launch_entry(*c, l, io, forced_render_tile(), s));
+    CUDA_TRY(c, launch_entry_views(*c, l, io, forced_render_tile(), s));
     c->launches++;
     return 0;
 }
@@ -817,6 +841,7 @@ int meao_create(const MeaoDeviceCfg *cfg, MeaoCtx **out)
         if (!preloaded[dev]) {
             cudaError_t pe = cudaSuccess;
             for (const KernelUnit *u : kKernelUnits) u->walk(&pe);
+            for (const KernelUnit *u : kViewKernelUnits) u->walk(&pe);
             if (pe != cudaSuccess) { cudaGetLastError(); meao_destroy(c); return fail(nullptr, MEAO_ERR_CUDA, "loading the kernels failed: %s", cudaGetErrorString(pe)); }
             preloaded[dev] = true;
         }
@@ -945,6 +970,64 @@ int meao_get_layer_cameras(const MeaoCtx *c, MeaoCamera *out, int32_t capacity)
     return n;
 }
 
+static_assert(sizeof(LayerView) == sizeof(MeaoLayerViewport) && offsetof(LayerView, ao_slice) == offsetof(MeaoLayerViewport, ao_slice),
+              "the arena's layer-viewport table is the public table, field for field");
+namespace {
+const char *const kViewField[6] = {"depth_x", "depth_y", "depth_slice", "ao_x", "ao_y", "ao_slice"};
+inline int view_field(const MeaoLayerViewport &v, int i) { return (&v.depth_x)[i]; }
+}  // namespace
+
+int meao_set_layer_viewports(MeaoCtx *c, const MeaoLayerViewport *views, int32_t count)
+{
+    if (!c) return MEAO_ERR_INVALID;
+    if (!views && count == 0) {
+        if (c->views.empty()) return 0;
+        c->views.clear();
+        c->views_pending = false;
+        c->plan_dirty = true;               // back to the array kernels without a table: a structural change
+        c->frame_gen++;
+        return 1;
+    }
+    if (!views) return fail(c, MEAO_ERR_INVALID, "views is NULL with count %d (NULL clears the table only with count 0)", count);
+    if (count != c->layers) return fail(c, MEAO_ERR_INVALID, "count %d differs from the context's %d layers (meao_set_layers)", count, c->layers);
+    for (int l = 0; l < count; l++)
+        for (int i = 0; i < 6; i++)
+            if (view_field(views[l], i) < 0)
+                return fail(c, MEAO_ERR_INVALID, "layer %d: %s = %d is negative", l, kViewField[i], view_field(views[l], i));
+    if ((int)c->views.size() == count && memcmp(c->views.data(), views, (size_t)count * sizeof(MeaoLayerViewport)) == 0) return 0;
+    if (c->views.empty()) c->plan_dirty = true;     // the table kernels replace the array kernels: a structural change
+    else c->views_pending = !c->plan_only;          // a frame constant: written by the next frame on its stream
+    c->views.assign(views, views + count);
+    for (int i = 0; i < 6; i++) {
+        int m = 0;
+        for (int l = 1; l < count; l++) if (view_field(views[l], i) > view_field(views[m], i)) m = l;
+        c->views_max[i] = m;
+    }
+    for (int r = 0; r < 2; r++) {
+        const int f = 3 * r;        // depth_x or ao_x; then y, slice
+        auto yx = [&](int l) { return std::make_pair(view_field(views[l], f + 1), view_field(views[l], f)); };
+        auto syx = [&](int l) { return std::make_tuple(view_field(views[l], f + 2), view_field(views[l], f + 1), view_field(views[l], f)); };
+        int a = 0, b = 0;
+        for (int l = 1; l < count; l++) {
+            if (yx(l) > yx(a)) a = l;
+            if (syx(l) > syx(b)) b = l;
+        }
+        c->views_last[r][0] = a; c->views_last[r][1] = b;
+    }
+    c->views_checked.clear();
+    c->frame_gen++;
+    return 1;
+}
+
+int meao_get_layer_viewports(const MeaoCtx *c, MeaoLayerViewport *out, int32_t capacity)
+{
+    if (!c) return MEAO_ERR_INVALID;
+    const int n = (int)c->views.size();
+    if (n && (!out || capacity < n)) return MEAO_ERR_INVALID;
+    if (n) memcpy(out, c->views.data(), (size_t)n * sizeof(MeaoLayerViewport));
+    return n;
+}
+
 int meao_resize(MeaoCtx *c, int32_t w, int32_t h)
 {
     if (!c) return MEAO_ERR_INVALID;
@@ -1013,6 +1096,10 @@ int meao_set_layers(MeaoCtx *c, int32_t layers)
     c->frame_gen++;
     std::vector<MeaoCamera> old_cams;
     old_cams.swap(c->layer_cams);                   // a table has one camera per layer: a new layer count clears it
+    std::vector<MeaoLayerViewport> old_views;       // and so does a viewport table
+    old_views.swap(c->views);
+    const bool old_views_pending = c->views_pending;
+    c->views_pending = false;
     c->layers = layers;
     c->plan_dirty = true;
     if (c->W <= 0 && !c->arena) return 1;           // applied by the first meao_resize (a reserved arena is laid out again now)
@@ -1025,6 +1112,8 @@ int meao_set_layers(MeaoCtx *c, int32_t layers)
         const std::string err = c->error;
         c->layers = old;
         c->layer_cams.swap(old_cams);
+        c->views.swap(old_views);
+        c->views_pending = old_views_pending;
         if (allocate(c)) { c->W = c->H = 0; }        // the previous arena could not be restored either: the context needs meao_resize
         c->error = err;
         return rc;
@@ -1460,9 +1549,62 @@ int meao_band_status(MeaoCtx *c, int32_t out4[4])
 }
 
 namespace {
+int check_ao_disjoint(MeaoCtx *c);
+
+// The layer-viewport table against the caller's pitched views (check_views, table set): the checks check_view_fit makes for arrays.
+// Every row of every rectangle fits its row pitch; when some slice is > 0, every rectangle fits inside its slice (so slices never
+// share a byte) and the depth layer pitch is a whole number of elements; no two AO rectangles share a byte (check_ao_disjoint: with
+// rows inside the row pitch and rectangles inside their slices, two share a byte exactly when they share a texel).  Constant time
+// (views_max, views_last), except check_ao_disjoint's once per (table, size).  Both the slice test and the extents are exact: once every
+// row fits its row pitch, a rectangle further down (or in a later slice) ends further in than any rectangle above it, whatever the x.
+int check_view_pitches(MeaoCtx *c, const void *depth, int64_t es, const void *ao_out, const ViewPitch &p)
+{
+    if (c->band0 != 0 || c->band1 != c->H) return fail(c, MEAO_ERR_UNSUPPORTED, "a layer-viewport table needs a whole-frame context (no row band)");
+    const int64_t W = c->W, H = c->H;
+    const struct { const char *role; int f0; int64_t es, row, layer; } views[2] = {{"depth", 0, es, p.depth_row, p.depth_layer},
+                                                                                    {"ao", 3, 1, p.ao_row, p.ao_layer}};
+    int64_t extent[2];
+    for (int i = 0; i < 2; i++) {
+        const auto &v = views[i];
+        const int lx = c->views_max[v.f0], ls = c->views_max[v.f0 + 2];
+        const int64_t x = view_field(c->views[lx], v.f0), sl = view_field(c->views[ls], v.f0 + 2);
+        if ((x + W) * v.es > v.row)
+            return fail(c, MEAO_ERR_INVALID, "layer %d: %s_x = %lld: a row of the %lldx%lld rectangle overflows %s_row_pitch %lld", lx, v.role,
+                        (long long)x, (long long)W, (long long)H, v.role, (long long)v.row);
+        // where a rectangle's last byte lies in its slice.  Slices at most 2^31 at a pitch of at most 2^63, rows at most 2^31 at a pitch
+        // of at most 2^31: every product below stays inside __int128
+        auto in_slice = [&](int l) {
+            const MeaoLayerViewport &e = c->views[l];
+            return (__int128)(view_field(e, v.f0 + 1) + H - 1) * v.row + (view_field(e, v.f0) + W) * v.es;
+        };
+        if (sl > 0) {
+            const int ly = c->views_last[i][0];
+            if (in_slice(ly) > v.layer)
+                return fail(c, MEAO_ERR_INVALID, "layer %d: %s_x, %s_y = %d, %d: the %lldx%lld rectangle overflows %s_layer_pitch %lld (its slice)",
+                            ly, v.role, v.role, view_field(c->views[ly], v.f0), view_field(c->views[ly], v.f0 + 1), (long long)W, (long long)H,
+                            v.role, (long long)v.layer);
+            if (v.layer % v.es)
+                return fail(c, MEAO_ERR_INVALID, "layer %d: %s_slice = %lld: %s_layer_pitch %lld is not a multiple of the %lld-byte element", ls,
+                            v.role, (long long)sl, v.role, (long long)v.layer, (long long)v.es);
+        }
+        const int le = c->views_last[i][1];
+        const __int128 end = (__int128)view_field(c->views[le], v.f0 + 2) * v.layer + in_slice(le);
+        if (end > INT64_MAX) return fail(c, MEAO_ERR_INVALID, "layer %d: %s_slice = %d: the view ends beyond 2^63 bytes", le, v.role,
+                                         view_field(c->views[le], v.f0 + 2));
+        extent[i] = (int64_t)end;
+    }
+    int rc = check_ao_disjoint(c);
+    if (rc) return rc;
+    // the existing extent test, from each view's base to the end of its last rectangle
+    const __int128 d0 = (__int128)(uintptr_t)depth, a0 = (__int128)(uintptr_t)ao_out;
+    if (d0 < a0 + extent[1] && a0 < d0 + extent[0])
+        return fail(c, MEAO_ERR_INVALID, "the byte extents of the depth view and the AO view (ao_out_dev) intersect");
+    return 0;
+}
+
 // Every check of meao_render_pitched / meao_bind_event_pitched, on the host before anything is launched.  On success the layer pitches
 // of a single-layer context (unused) are replaced by the tight values, so that equivalent views share one cached graph.
-int check_views(MeaoCtx *c, const void *depth, int kind, const void *ao_out, ViewPitch *p)
+int check_views(MeaoCtx *c, const void *depth, int kind, const void *ao_out, ViewPitch *p, bool table = true)
 {
     if (!depth || !ao_out) return fail(c, MEAO_ERR_INVALID, "depth / ao_out is NULL");
     if (kind < MEAO_DEPTH_RAW_F32 || kind > MEAO_DEPTH_RAW_D24S8) return fail(c, MEAO_ERR_INVALID, "bad depth kind %d", kind);
@@ -1480,6 +1622,7 @@ int check_views(MeaoCtx *c, const void *depth, int kind, const void *ao_out, Vie
                     (long long)p->depth_row, (long long)es, (long long)(W * es), (long long)es);
     if (p->ao_row < W) return fail(c, MEAO_ERR_INVALID, "ao_row_pitch %lld is below the width %lld", (long long)p->ao_row, (long long)W);
     if ((uintptr_t)depth % es) return fail(c, MEAO_ERR_INVALID, "depth_dev %p is not aligned to its %lld-byte element", depth, (long long)es);
+    if (table && !c->views.empty()) return check_view_pitches(c, depth, es, ao_out, *p);
     if (L > 1) {
         // layers must not overlap.  The extents below are then at most L x layer pitch: at most 2^16 x 2^63, which __int128 holds
         const int64_t dmin = (rows - 1) * p->depth_row + W * es, amin = (rows - 1) * p->ao_row + W;
@@ -1512,20 +1655,25 @@ int check_views(MeaoCtx *c, const void *depth, int kind, const void *ao_out, Vie
 
 namespace {
 // The frame of meao_render / meao_render_pitched on a context that ensure_ready has prepared.
-int render_views(MeaoCtx *c, const void *depth, int kind, void *ao_out, ViewPitch p, void *stream, bool capturing)
+// table: honour the layer-viewport table when one is set; false for the host-buffer calls, whose staging buffers hold the tight layout.
+int render_views(MeaoCtx *c, const void *depth, int kind, void *ao_out, ViewPitch p, void *stream, bool capturing, bool table = true)
 {
     int rc;
-    if ((rc = check_views(c, depth, kind, ao_out, &p))) return rc;
+    if ((rc = check_views(c, depth, kind, ao_out, &p, table))) return rc;
     cudaStream_t s = (cudaStream_t)stream;
-    if (c->flags & MEAO_FLAG_NO_GRAPH) return record_frame(c, frame_io(c, depth, kind, ao_out, true, &p), s, 0, false);
+    // a layer-viewport table: the rectangles of the arena's table; checked against these views by check_views
+    const LayerView *views = (!table || c->views.empty()) ? nullptr : c->layer_views;
+    auto io = [&]() { FrameIO fio = frame_io(c, depth, kind, ao_out, true, &p); fio.views = views; return fio; };
+    if (c->flags & MEAO_FLAG_NO_GRAPH) return record_frame(c, io(), s, 0, false);
 
     // plan-once / replay: one captured graph per (depth, out, kind, pitches), like the reference's command buffer
-    // that is re-recorded only when something changed (AO.cs:334-347)
+    // that is re-recorded only when something changed (AO.cs:334-347).  p[2]: the table a frame reads (nullptr: none), so a frame that
+    // ignores a set table never replays one recorded through it, nor the reverse
     NvtxRange nv("meao::frame");
-    const MeaoCtx::GraphKey key{{depth, ao_out, nullptr, nullptr}, kind, {p.depth_row, p.depth_layer, p.ao_row, p.ao_layer}};
+    const MeaoCtx::GraphKey key{{depth, ao_out, views, nullptr}, kind, {p.depth_row, p.depth_layer, p.ao_row, p.ao_layer}};
     c->last_kind = kind; c->last_out = ao_out;
     return launch_cached(c, key, s, capturing, [&](cudaStream_t cs, int pdl) {
-        return record_frame_dag(c, frame_io(c, depth, kind, ao_out, true, &p), cs, 0, pdl);
+        return record_frame_dag(c, io(), cs, 0, pdl);
     });
 }
 }  // namespace
@@ -1552,8 +1700,10 @@ constexpr int kArrayGraphKind = 400;        // GraphKey.kind of an array frame: 
 // What a cudaArray_t is, checked against the context on the host before anything is launched.  role: "depth" or "ao", the prefix of
 // the fields named in a refusal (<role>_array, <role>_x, <role>_y).  elem_bits / is_float: the one channel the role needs.  exact: the
 // extent must be the context's W x H (meao_render_arrays); otherwise the W x H viewport at (x, y) must lie inside it.  Returns 0 and
-// the layer addressing, or fails with a message naming the field.
-int check_array(MeaoCtx *c, const void *arr, const char *role, int elem_bits, bool is_float, int x, int y, bool exact, int *surf_kind)
+// the layer addressing, or fails with a message naming the field.  ext / layers_out (a layer-viewport table is set): no extent, origin
+// or layer-count test here; the array's extent and layer count are returned for check_view_fit instead.
+int check_array(MeaoCtx *c, const void *arr, const char *role, int elem_bits, bool is_float, int x, int y, bool exact, int *surf_kind,
+                cudaExtent *ext = nullptr, int *layers_out = nullptr)
 {
     cudaChannelFormatDesc d{};
     cudaExtent e{};
@@ -1569,7 +1719,9 @@ int check_array(MeaoCtx *c, const void *arr, const char *role, int elem_bits, bo
     if (!one_channel || !kind_ok)
         return fail(c, MEAO_ERR_INVALID, "%s_array: channel format (%d,%d,%d,%d bits, kind %d) is not one %d-bit %s channel", role, d.x, d.y, d.z, d.w, (int)d.f,
                     elem_bits, is_float ? "float" : "unsigned (normalised or not)");
-    if (exact) {
+    if (ext) {
+        *ext = e;
+    } else if (exact) {
         if ((int)e.width != c->W || (int)e.height != c->H || e.width != (size_t)c->W || e.height != (size_t)c->H)
             return fail(c, MEAO_ERR_INVALID, "%s_array: extent %zux%zu differs from the context's %dx%d", role, e.width, e.height, c->W, c->H);
     } else {
@@ -1592,8 +1744,57 @@ int check_array(MeaoCtx *c, const void *arr, const char *role, int elem_bits, bo
         if (e.depth > 1) return fail(c, MEAO_ERR_INVALID, "%s_array: depth %zu: a 3-D array is not a 2-D or layered image", role, e.depth);
         layers = 1; *surf_kind = kSurf2D;
     }
+    if (layers_out) { *layers_out = layers; return 0; }
     if (layers != c->layers)
         return fail(c, MEAO_ERR_INVALID, "%s_array: layer count %d differs from the context's %d (meao_set_layers)", role, layers, c->layers);
+    return 0;
+}
+
+// The layer-viewport table against one array at the current W x H: every rectangle inside the array's extent and every slice below
+// its layer count.  f0: the table's first field of the role (0: depth_x, 3: ao_x).  Constant time: views_max holds, per field, the layer
+// with the largest value.
+int check_view_fit(MeaoCtx *c, const char *role, const cudaExtent &e, int layers, int f0)
+{
+    const int lx = c->views_max[f0], ly = c->views_max[f0 + 1], ls = c->views_max[f0 + 2];
+    const int x = view_field(c->views[lx], f0), y = view_field(c->views[ly], f0 + 1), sl = view_field(c->views[ls], f0 + 2);
+    if ((size_t)x + (size_t)c->W > e.width)
+        return fail(c, MEAO_ERR_INVALID, "layer %d: %s_x = %d: the %dx%d rectangle overflows %s_array's width %zu", lx, role, x, c->W, c->H, role, e.width);
+    if ((size_t)y + (size_t)c->H > e.height)
+        return fail(c, MEAO_ERR_INVALID, "layer %d: %s_y = %d: the %dx%d rectangle overflows %s_array's height %zu", ly, role, y, c->W, c->H, role, e.height);
+    if (sl >= layers)
+        return fail(c, MEAO_ERR_INVALID, "layer %d: %s_slice = %d: %s_array has %d layer(s)", ls, role, sl, role, layers);
+    return 0;
+}
+
+// No two layers' AO rectangles on one slice share a texel, at the current W x H; once per (table, size), and not at all at a size no
+// larger in either dimension than one that passed.  Every rectangle is W x H, so
+// two overlap exactly when their origins are less than W apart in x and less than H apart in y.  The origins are binned into W x H
+// cells: an overlapping pair lies in the same or in neighbouring cells, and disjoint rectangles leave at most one origin per cell, so
+// the test takes L map lookups and insertions rather than L^2 comparisons.
+int check_ao_disjoint(MeaoCtx *c)
+{
+    const int W = c->W, H = c->H;
+    for (const auto &wh : c->views_checked)
+        if (W <= wh.first && H <= wh.second) return 0;
+    std::map<std::array<int, 3>, int> cells;
+    for (int l = 0; l < (int)c->views.size(); l++) {
+        const MeaoLayerViewport &v = c->views[l];
+        const int cx = v.ao_x / W, cy = v.ao_y / H;
+        for (int dy = -1; dy <= 1; dy++)
+            for (int dx = -1; dx <= 1; dx++) {
+                auto it = cells.find({v.ao_slice, cx + dx, cy + dy});
+                if (it == cells.end()) continue;
+                const MeaoLayerViewport &o = c->views[it->second];
+                if (std::abs(v.ao_x - o.ao_x) < W && std::abs(v.ao_y - o.ao_y) < H)
+                    return fail(c, MEAO_ERR_INVALID, "layer %d: ao_x, ao_y = %d, %d: its %dx%d AO rectangle shares texels with layer %d's at %d, %d "
+                                                     "(ao_slice %d)", l, v.ao_x, v.ao_y, W, H, it->second, o.ao_x, o.ao_y, v.ao_slice);
+            }
+        cells.emplace(std::array<int, 3>{v.ao_slice, cx, cy}, l);
+    }
+    // keep only the sizes no other passed size holds
+    auto held = [&](const std::pair<int, int> &wh) { return wh.first <= W && wh.second <= H; };
+    c->views_checked.erase(std::remove_if(c->views_checked.begin(), c->views_checked.end(), held), c->views_checked.end());
+    c->views_checked.emplace_back(W, H);
     return 0;
 }
 
@@ -1621,8 +1822,19 @@ int prepare_arrays(MeaoCtx *c, const void *depth_array, int dx, int dy, int kind
     if (c->band0 != 0 || c->band1 != c->H) return fail(c, MEAO_ERR_UNSUPPORTED, "CUDA-array frames need a whole-frame context (no row band)");
     int rc;
     const bool d16 = kind == MEAO_DEPTH_RAW_D16_UNORM;
-    if ((rc = check_array(c, depth_array, "depth", d16 ? 16 : 32, !d16, dx, dy, exact, &io->depth_surf))) return rc;
-    if ((rc = check_array(c, ao_array, "ao", 8, false, ax, ay, exact, &io->ao_surf))) return rc;
+    if (!c->views.empty()) {        // the table says where every layer goes (meao_set_layer_viewports)
+        if (!exact)
+            return fail(c, MEAO_ERR_INVALID, "a layer-viewport table is set (meao_set_layer_viewports): it places every layer, so the origins of "
+                                             "meao_render_arrays_at / meao_bind_event_arrays_at are refused; use meao_render_arrays");
+        cudaExtent de{}, ae{};
+        int dn = 0, an = 0;
+        if ((rc = check_array(c, depth_array, "depth", d16 ? 16 : 32, !d16, 0, 0, false, &io->depth_surf, &de, &dn))) return rc;
+        if ((rc = check_array(c, ao_array, "ao", 8, false, 0, 0, false, &io->ao_surf, &ae, &an))) return rc;
+        if ((rc = check_view_fit(c, "depth", de, dn, 0)) || (rc = check_view_fit(c, "ao", ae, an, 3)) || (rc = check_ao_disjoint(c))) return rc;
+    } else {
+        if ((rc = check_array(c, depth_array, "depth", d16 ? 16 : 32, !d16, dx, dy, exact, &io->depth_surf))) return rc;
+        if ((rc = check_array(c, ao_array, "ao", 8, false, ax, ay, exact, &io->ao_surf))) return rc;
+    }
     if ((rc = surface_of(c, depth_array, &io->depth))) return rc;
     if ((rc = surface_of(c, ao_array, &io->ao))) return rc;
     io->ao_array = ao_array;
@@ -1652,6 +1864,7 @@ int render_arrays(MeaoCtx *c, const void *depth_array, int dx, int dy, int kind,
     return launch_cached(c, key, (cudaStream_t)stream, capturing, [&](cudaStream_t cs, int pdl) {
         FrameIO fio = frame_io(c, nullptr, kind, nullptr, false);
         fio.aio = &io;
+        if (!c->views.empty()) fio.views = c->layer_views;
         return record_frame_dag(c, fio, cs, 0, pdl);
     });
 }
@@ -1708,7 +1921,10 @@ int meao_render_host_async(MeaoCtx *c, const void *depth_host, int32_t kind, uin
     CUDA_TRY(c, cudaMemcpyAsync(c->depth_stage[slot], depth_host, rows * c->W * depth_esize(kind), cudaMemcpyHostToDevice, s));
     // the two slots share the context's intermediates: kernels of consecutive frames are serialised, copies are not
     if (c->compute_done_valid) CUDA_TRY(c, cudaStreamWaitEvent(s, c->compute_done, 0));
-    if ((rc = meao_render(c, c->depth_stage[slot], kind, c->ao_stage[slot], s))) return rc;
+    // meao_render of the staging buffers, which hold the tight layout whether or not a layer-viewport table is set
+    bool capturing;
+    if ((rc = frame_ready(c, s, &capturing))) return rc;
+    if ((rc = render_views(c, c->depth_stage[slot], kind, c->ao_stage[slot], tight_pitch(*c, kind), s, capturing, false))) return rc;
     CUDA_TRY(c, cudaEventRecord(c->compute_done, s));
     c->compute_done_valid = true;
     CUDA_TRY(c, cudaMemcpyAsync(ao_host, c->ao_stage[slot], rows * c->W, cudaMemcpyDeviceToHost, s));
