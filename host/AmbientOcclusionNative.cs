@@ -103,6 +103,10 @@ namespace MiniEngineAO
         [DllImport(Lib)] public static extern int meao_debug_view(IntPtr ctx, int bufferId, IntPtr outR8Dev, IntPtr stream);   // AO.cs:787-820
         // frames recorded into the host's own CUDA graph (a render called on a capturing stream) replay only while this is unchanged
         [DllImport(Lib)] public static extern long meao_frame_generation(IntPtr ctx);
+        // MEAO_PROJECTION_PERSPECTIVE 0 / MEAO_PROJECTION_ORTHOGRAPHIC 1 (Camera.orthographic): a structural input, one per context.  Under
+        // an orthographic camera 1 / projectionMatrix[0,0] is the view volume's half-width, and LINEAR_F32 depth must be eye depth / far
+        [DllImport(Lib)] public static extern int meao_set_projection(IntPtr ctx, int projection);
+        [DllImport(Lib)] public static extern int meao_get_projection(IntPtr ctx);
 
         public static void Check(IntPtr ctx, int rc)
         {
@@ -215,6 +219,8 @@ namespace MiniEngineAO
                 reversed_z = SystemInfo.usesReversedZBuffer ? 1 : 0                          // :564
             };
             MeaoNative.Check(_ctx, MeaoNative.meao_set_camera(_ctx, ref cam));
+            // the projection excludes a layer-viewport table: back to perspective before a table is set, orthographic after it is cleared
+            if (!_camera.orthographic) rebuild |= SetProjection(0) == 1;
             var stereo = singlePassStereoEnabled;
             var variants = new MeaoNative.MeaoVariants
             {
@@ -231,6 +237,7 @@ namespace MiniEngineAO
                                                     : MeaoNative.meao_set_layer_viewports(_ctx, _layerViewports, _layerViewports.Length);
             MeaoNative.Check(_ctx, viewports);
             rebuild |= viewports == 1;                                                       // after meao_set_layers too
+            if (_camera.orthographic) rebuild |= SetProjection(1) == 1;
             var width = _camera.pixelWidth * (stereo ? 2 : 1);
             rebuild |= Reserve(width, _camera.pixelHeight, stereo);                          // before meao_resize, doubled like the width
             var resized = MeaoNative.meao_resize(_ctx, width, _camera.pixelHeight);          // :338-341
@@ -261,6 +268,14 @@ namespace MiniEngineAO
             return true;
         }
 
+        // Hands the projection to the plugin (0 perspective, 1 orthographic); returns 1 if it changed (a re-plan), 0 if not.
+        int SetProjection(int projection)
+        {
+            var rc = MeaoNative.meao_set_projection(_ctx, projection);
+            MeaoNative.Check(_ctx, rc);
+            return rc;
+        }
+
         // Hands LayerCameras to the plugin; returns 1 if a value changed (the next frame takes it without a re-plan).  The same table again returns 0, so this runs every frame.
         int SetLayerCameras()
         {
@@ -271,6 +286,8 @@ namespace MiniEngineAO
                 var c = _layerCameras[i];
                 if (c.pixelWidth != _camera.pixelWidth || c.pixelHeight != _camera.pixelHeight)
                     throw new ArgumentException("LayerCameras[" + i + "] has another pixel size than the camera");
+                if (c.orthographic != _camera.orthographic)
+                    throw new ArgumentException("LayerCameras[" + i + "] has another projection than the camera (one per context)");
                 cams[i] = new MeaoNative.MeaoCamera
                 {
                     near_clip = c.nearClipPlane, far_clip = c.farClipPlane,

@@ -40,7 +40,8 @@ extern "C" {
                               *    + meao_frame_generation (frames inside a caller's CUDA graph; additive)
                               *    + meao_render_arrays_at / meao_bind_event_arrays_at (viewports of larger CUDA arrays; additive)
                               *    + MeaoLayerViewport, meao_set_layer_viewports / meao_get_layer_viewports (each layer at its own
-                              *      viewport of shared CUDA arrays: split-screen, side-by-side stereo, cube atlases; additive) */
+                              *      viewport of shared CUDA arrays: split-screen, side-by-side stereo, cube atlases; additive)
+                              *    + MeaoProjection, meao_set_projection / meao_get_projection (orthographic cameras; additive) */
 
 typedef struct MeaoCtx MeaoCtx;
 
@@ -64,11 +65,11 @@ typedef struct {
     int32_t ambient_only;           /* default 1       AO.cs:62-68   (carried; composite is out of scope) */
 } MeaoParams;
 
-/* Camera inputs of the CPU-side constant math: AO.cs:561-573. */
+/* Camera inputs of the CPU-side constant math: AO.cs:561-573.  Their meaning under an orthographic projection: meao_set_projection. */
 typedef struct {
     float near_clip;        /* camera.nearClipPlane                         AO.cs:563 */
     float far_clip;         /* camera.farClipPlane                          AO.cs:563 */
-    float tan_half_fov_h;   /* 1 / camera.projectionMatrix[0,0]             AO.cs:570-573 */
+    float tan_half_fov_h;   /* 1 / camera.projectionMatrix[0,0]             AO.cs:570-573 (orthographic: the view volume's half-width) */
     int32_t reversed_z;     /* SystemInfo.usesReversedZBuffer (D3D11/12: 1) AO.cs:564, Downsample1.compute:41-45 */
 } MeaoCamera;
 
@@ -83,7 +84,8 @@ typedef struct {
 
 typedef enum {
     MEAO_DEPTH_RAW_F32 = 0,     /* camera depth, linearised by Downsample1.compute:37-48 (reference behaviour) */
-    MEAO_DEPTH_LINEAR_F32 = 1,  /* already-linear depth (Linearize becomes the identity; not in the reference) */
+    MEAO_DEPTH_LINEAR_F32 = 1,  /* already-linear depth (Linearize becomes the identity; not in the reference): eye depth / far_clip, the
+                                   values LinearDepth holds.  Perspective AO does not depend on the scale; orthographic AO does */
     /* native depth-buffer formats (what Blit.shader pass 0 :48-64 samples; SURVEY.md 8f.1): the UNORM code is
      * converted with the D3D rule (float)code * (1 / (2^n - 1)) and then linearised like RAW_F32 */
     MEAO_DEPTH_RAW_D16_UNORM = 2,   /* uint16 codes, 2 bytes / pixel */
@@ -147,8 +149,8 @@ int meao_abi_version(void);
  * before it was issued, and frame n-1, still in flight, keeps its own.  A host may therefore animate the camera and the
  * parameters every frame.
  * STRUCTURAL INPUTS re-plan with a device synchronise and drop the captured graphs: MeaoVariants, meao_set_layers, a resize without
- * a reservation, meao_reserve, row bands, and a change of the cameras' reversed_z (it selects kernel instantiations; it is a
- * platform property).
+ * a reservation, meao_reserve, row bands, a change of the cameras' reversed_z (it selects kernel instantiations; it is a
+ * platform property) and meao_set_projection.
  * A refused camera, table or parameter block leaves the context exactly as it was. */
 /* replaces: the property setters AO.cs:22-66 (CheckPropertiesChanged, AO.cs:104-113): returns 1 if a value changed, 0 if not. */
 int meao_set_params(MeaoCtx *ctx, const MeaoParams *params);
@@ -160,6 +162,33 @@ int meao_get_variants(const MeaoCtx *ctx, MeaoVariants *out);
 /* replaces: CalculateZBufferParams / CalculateTanHalfFovHeight inputs (AO.cs:561-573).  A frame constant, except reversed_z;
  * returns MEAO_OK. */
 int meao_set_camera(MeaoCtx *ctx, const MeaoCamera *camera);
+
+/* ---- projection ----------------------------------------------------------------------------------
+ * The projection model of the context's cameras, one for all layers (a batch that mixes projections needs two contexts).
+ * PERSPECTIVE (the default) is what the reference does.  ORTHOGRAPHIC (isometric and top-down views, CAD viewers, editor views):
+ *   - raw depth is affine in eye depth: with r = near_clip / far_clip, lin = fma(1 - r, d, r), reversed Z lin = fma(r - 1, d, 1) -- eye
+ *     depth / far_clip, LinearDepth's convention; d == 1 (reversed: d == 0) is sky, 1e5, as for perspective.  meao_zbuffer_params
+ *     returns {1 - r, r, 0, 0} (reversed: {r - 1, 1, 0, 0}), and the atlas padding of render levels 1-2 is r (reversed: 1e5).
+ *     MEAO_DEPTH_LINEAR_F32 input must follow the same convention, eye depth / far_clip: the sphere's thickness is absolute.
+ *   - the sampling sphere has a constant world size instead of growing with the centre depth: with the reference's ThicknessMultiplier
+ *     TM (AO.cs:671-683, from tan_half_fov_h and the source width), sample i has invRange = it_i = (far_clip / TM) / SampleThickness[i]
+ *     and frontDepth = centre x it_i - 0.5.  meao_render_constants return it_i in the gInvThicknessTable slots.
+ *   - tan_half_fov_h = 1 / projectionMatrix[0,0] (CalculateTanHalfFovHeight, AO.cs:570-573) is the half-width of the view volume in world
+ *     units (Unity: orthographicSize x aspect).  near_clip must be > 0 as for perspective, although Unity allows near <= 0 for an
+ *     orthographic camera: a linear depth of 0 would reach the upsample's 1 / depth.
+ *   - the planes and the half-width stay frame constants: an orthographic zoom takes effect at the next frame without a re-plan.
+ *   - the upsample and blur are the perspective ones (they work on the stored linear depth through 1 / depth, DESIGN.md 2.14).
+ * A change of projection is a structural input: it re-plans with a device synchronise, drops the captured graphs, moves
+ * meao_frame_generation and returns 1; the same value returns 0.  Not supported under ORTHOGRAPHIC, refused with MEAO_ERR_UNSUPPORTED in
+ * either order (setting the projection while one is set, or setting one under an orthographic projection), before anything changes:
+ * a layer-viewport table (meao_set_layer_viewports) and row bands with their halo and native-exchange calls.  An unknown value is
+ * MEAO_ERR_INVALID and changes nothing.  Both calls work on plan-only contexts. */
+typedef enum {
+    MEAO_PROJECTION_PERSPECTIVE = 0,
+    MEAO_PROJECTION_ORTHOGRAPHIC = 1
+} MeaoProjection;
+int meao_set_projection(MeaoCtx *ctx, int32_t projection);
+int meao_get_projection(const MeaoCtx *ctx);     /* MeaoProjection, or MEAO_ERR_INVALID for a NULL context */
 /* replaces: RTHandle.SetBaseDimensions + AllocateNow + the rebuild it triggers (AO.cs:338-341, 501-506).
  * Allocates the intermediates for width x height.  Returns 1 if dimensions changed, 0 if not.
  * A size change RESETS the row band to the whole frame and drops the neighbour connections (meao_set_row_band,
@@ -334,7 +363,7 @@ int meao_render_host(MeaoCtx *ctx, const void *depth_host, int32_t depth_kind, u
  * meao_release_array(ctx, array): it synchronises the device, drops that array's graphs, surface object and event bindings.  A new
  * array may come back with the same handle, and without the release the next frame would replay into freed memory.
  * meao_destroy and every structural plan change (meao_resize without a reservation, meao_reserve, meao_set_layers, meao_set_variants,
- * a reversed_z change, meao_set_row_band) release all arrays; a frame-constant change (MeaoParams, the cameras' planes and fields of
+ * a reversed_z change, meao_set_projection, meao_set_row_band) release all arrays; a frame-constant change (MeaoParams, the cameras' planes and fields of
  * view) releases none.  Releasing an array this context never used returns MEAO_OK. */
 int meao_render_arrays(MeaoCtx *ctx, const void *depth_array, int32_t depth_kind, void *ao_array, void *stream);
 /* Viewports: meao_render_arrays with the frame read from, and written into, a W x H rectangle of larger arrays -- render targets
@@ -538,7 +567,7 @@ MeaoRenderEventFunc meao_get_render_event_func(void);
  * meao_composite_* calls.
  * SETTLED CONTEXTS ONLY: inside a capture a call may issue nothing but kernel launches.  It is refused with MEAO_ERR_INVALID, records
  * nothing and leaves the caller's capture valid (meao_last_error says why: "issue one frame outside the capture first") when
- *   - a structural change is pending (a re-plan synchronises the device),
+ *   - a structural change is pending (a re-plan synchronises the device; meao_set_projection is one),
  *   - the per-layer camera tables are still to be written: after a frame-constant change, or on the first frame at a size,
  *   - a changed layer-viewport table (meao_set_layer_viewports) is still to be written,
  *   - or, for meao_render_arrays(_at), the context has not rendered with one of the arrays yet (its surface object is made then).

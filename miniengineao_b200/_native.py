@@ -13,6 +13,7 @@ MEAO_ABI_VERSION = 3
 MEAO_PEER_HANDLE_BYTES = 128
 MEAO_FLAG_NONE, MEAO_FLAG_NO_GRAPH = 0, 1
 MEAO_DEPTH_RAW_F32, MEAO_DEPTH_LINEAR_F32, MEAO_DEPTH_RAW_D16_UNORM, MEAO_DEPTH_RAW_D24S8 = 0, 1, 2, 3
+MEAO_PROJECTION_PERSPECTIVE, MEAO_PROJECTION_ORTHOGRAPHIC = 0, 1
 MEAO_FMT_RGBA8_UNORM, MEAO_FMT_RGBA16_FLOAT = 0, 1
 
 
@@ -135,6 +136,8 @@ SIGNATURES = {
     "meao_get_render_event_func": (RENDER_EVENT_FUNC, []),
     "meao_launch_count": (C.c_int64, [C.c_void_p]),
     "meao_frame_generation": (C.c_int64, [C.c_void_p]),
+    "meao_set_projection": (C.c_int, [C.c_void_p, C.c_int32]),
+    "meao_get_projection": (C.c_int, [C.c_void_p]),
     "meao_pdl_level": (C.c_int, [C.c_void_p]),
     "meao_kernels_per_frame": (C.c_int, [C.c_void_p]),
     "meao_algorithmic_bytes": (C.c_int64, [C.c_void_p, C.c_int32]),

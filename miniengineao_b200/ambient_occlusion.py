@@ -29,6 +29,8 @@ class Camera:
     targetTexture: object = None        # Camera.targetTexture (AO.cs:398)
     allowHDR: bool = True               # Camera.allowHDR (AO.cs:407)
     actualRenderingPath: str = "Forward"    # "Forward" | "DeferredShading" (AO.cs:408)
+    orthographic: bool = False          # Camera.orthographic: meao_set_projection(MEAO_PROJECTION_ORTHOGRAPHIC)
+    orthographicSize: float = 5.0       # Camera.orthographicSize: half the view volume's height, world units
 
     @property
     def aspect(self) -> float:
@@ -36,7 +38,9 @@ class Camera:
 
     @property
     def projection00(self) -> float:
-        """projectionMatrix[0,0] of a perspective camera."""
+        """projectionMatrix[0,0]: 1 / (aspect * tan(fieldOfView / 2)), orthographic 1 / (aspect * orthographicSize)."""
+        if self.orthographic:
+            return 1.0 / (self.aspect * self.orthographicSize)
         return 1.0 / (self.aspect * math.tan(math.radians(self.fieldOfView) / 2.0))
 
 
@@ -82,7 +86,7 @@ class AmbientOcclusion:
         self.singleScale = False            # BASELINE.json configs[0]: Downsample1 -> Render level 1 -> final-style Upsample only
         self.layers = 1                     # views per frame (meao_set_layers): texture-array stereo 2, cube faces 6, frame batches
         # one Camera per layer (meao_set_layer_cameras): split-screen viewports, mirrors, batches from several cameras; None = every
-        # layer uses `camera`.  Each entry must match the main camera's pixelWidth, pixelHeight and usesReversedZBuffer.
+        # layer uses `camera`.  Each entry must match the main camera's pixelWidth, pixelHeight, usesReversedZBuffer and orthographic.
         self.layerCameras: list[Camera] | None = None
         # where each layer lives in the caller's depth and AO (meao_set_layer_viewports): one (depth_x, depth_y, depth_slice, ao_x,
         # ao_y, ao_slice) per layer -- split-screen players in one texture, a side-by-side stereo pair, cube faces in a 2-D atlas.  Honoured
@@ -152,6 +156,10 @@ class AmbientOcclusion:
         rebuild = self._check(self._lib.meao_set_params(self._ctx, C.byref(p))) == 1      # CheckPropertiesChanged
         c = N.MeaoCamera(cam.nearClipPlane, cam.farClipPlane, 1.0 / cam.projection00, int(cam.usesReversedZBuffer))
         self._check(self._lib.meao_set_camera(self._ctx, C.byref(c)))
+        # the projection (a structural input: it re-plans) excludes a layer-viewport table, so it turns orthographic only after the
+        # table is cleared and back to perspective before a table is set
+        if not cam.orthographic:
+            rebuild |= self._check(self._lib.meao_set_projection(self._ctx, N.MEAO_PROJECTION_PERSPECTIVE)) == 1
         if frame:
             self._stereo = self.singlePassStereoEnabled       # evaluated once per frame, before the counter reset (AO.cs:338-349)
         stereo = self._stereo
@@ -161,6 +169,8 @@ class AmbientOcclusion:
         layered = self._check(self._lib.meao_set_layers(self._ctx, int(self.layers))) == 1           # re-allocates like a resize
         rebuild |= self._apply_layer_cameras()
         rebuild |= self._apply_layer_viewports()
+        if cam.orthographic:
+            rebuild |= self._check(self._lib.meao_set_projection(self._ctx, N.MEAO_PROJECTION_ORTHOGRAPHIC)) == 1
         reallocated = layered | self._apply_reservation(width, cam.pixelHeight, stereo)
         resized = self._check(self._lib.meao_resize(self._ctx, width, cam.pixelHeight)) == 1          # CheckBaseDimensions
         reallocated |= resized and self._reserved == (0, 0)       # inside a reservation a resize allocates nothing
@@ -204,7 +214,7 @@ class AmbientOcclusion:
             return self._check(self._lib.meao_set_layer_cameras(self._ctx, None, 0)) == 1
         main = self._camera
         for i, c in enumerate(cams):
-            for f in ("pixelWidth", "pixelHeight", "usesReversedZBuffer"):
+            for f in ("pixelWidth", "pixelHeight", "usesReversedZBuffer", "orthographic"):
                 if getattr(c, f) != getattr(main, f):
                     raise ValueError(f"layerCameras[{i}].{f} = {getattr(c, f)!r} differs from the camera's {getattr(main, f)!r}")
         if len(cams) != int(self.layers):

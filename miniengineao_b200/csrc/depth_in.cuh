@@ -2,6 +2,7 @@
 // stages that read it: prepare_depth (prepare_depth_kernel.inc) and the final upsample of a whole frame (blur_upsample_lin.cu),
 // which linearises its own pixels and writes LinearDepth itself.  Included inside an anonymous namespace.
 
+#if !MEAO_ORTHO
 template <bool RAW, bool REVERSED>
 __device__ __forceinline__ float linearize(float depth, float zbx, float zby)
 {
@@ -48,6 +49,41 @@ __device__ __forceinline__ void linearize8(const float (&v)[8], float zbx, float
         for (int e = 0; e < 8; e++) d[e] = linearize<RAW, REVERSED>(v[e], zbx, zby);
     }
 }
+#else
+// An orthographic projection (MEAO_ORTHO: the *_ortho kernels, meao_set_projection) stores depth that is affine in eye depth, so the
+// linear depth is one fused multiply-add: zb = {1 - n/f, n/f} (reversed: {n/f - 1, 1}) gives eye depth / far, LinearDepth's
+// convention.  The sky rule of DS1:41-44 is the perspective one.  No reciprocal, so no range test.
+template <bool RAW, bool REVERSED>
+__device__ __forceinline__ float linearize(float depth, float zbx, float zby)
+{
+    if (!RAW) return depth;
+    float dist = fmaf(zbx, depth, zby);
+    if (REVERSED) { if (depth == 0.0f) dist = 1e5f; }
+    else          { if (depth == 1.0f) dist = 1e5f; }
+    return dist;
+}
+
+template <bool RAW, bool REVERSED>
+__device__ __forceinline__ void linearize8(const float (&v)[8], float zbx, float zby, float (&d)[8])
+{
+    if (!RAW) {
+#pragma unroll
+        for (int e = 0; e < 8; e++) d[e] = v[e];
+        return;
+    }
+    const float2 zx = make_float2(zbx, zbx), zy = make_float2(zby, zby);
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+        const float2 r = ffma2(make_float2(v[2 * q], v[2 * q + 1]), zx, zy);
+        d[2 * q] = r.x; d[2 * q + 1] = r.y;
+    }
+#pragma unroll
+    for (int e = 0; e < 8; e++) {
+        if (REVERSED) { if (v[e] == 0.0f) d[e] = 1e5f; }
+        else          { if (v[e] == 1.0f) d[e] = 1e5f; }
+    }
+}
+#endif
 
 // native depth formats (SURVEY.md 8f.1): the camera depth texture read by Blit.shader pass 0 (:48-64) is a D32_FLOAT,
 // D24_UNORM_S8_UINT or D16_UNORM resource; SAMPLE_DEPTH_TEXTURE returns code / (2^n - 1) for the UNORM ones

@@ -35,6 +35,7 @@ struct Plan {
     // the plan inputs the recorders read besides the constants: the variants and the cameras' Z direction
     MeaoVariants variants;
     int reversed_z;
+    int orthographic;                       // MEAO_PROJECTION_ORTHOGRAPHIC: launch_entry_ortho's kernels
 };
 
 // The camera-dependent part of the plan, for one camera: ZBufferParams, both inv_thickness tables of every level and the atlas
@@ -281,15 +282,24 @@ inline RenderArgs render_args(const FrameState &f, int k, int kind, bool wide, i
     return a;
 }
 
-// The render launch of level k with the map of a.tile_h; a layered frame takes its layers' camera table entries
-inline cudaError_t launch_render(const FrameState &f, const RenderArgs &a, int k, int kind, cudaStream_t s)
+// The TMA map of render launch `a` of level k (its tile height and source) and its layers' camera table entries (nullptr: none)
+inline const CUtensorMap &render_map(const FrameState &f, const RenderArgs &a, int k)
 {
     int tv = 0;
     while (tv + 1 < kRenderTileVariants && kRenderTileHs[tv] != a.tile_h) tv++;
-    const CUtensorMap &map = a.wide ? f.maps.low_wide[tv][k] : f.maps.low_ren[tv][k];
+    return a.wide ? f.maps.low_wide[tv][k] : f.maps.low_ren[tv][k];
+}
+inline const LayerRender *render_layer_cams(const FrameState &f, const RenderArgs &a, int k)
+{
+    return f.layer_ren ? f.layer_ren + (size_t)(2 * (k - 1) + a.wide) * f.layers : nullptr;
+}
+
+// The render launch of level k with the map of a.tile_h; a layered frame takes its layers' camera table entries
+inline cudaError_t launch_render(const FrameState &f, const RenderArgs &a, int k, int kind, cudaStream_t s)
+{
+    const CUtensorMap &map = render_map(f, a, k);
     if (f.layers == 1) return launch_render_ao(map, f.tma_ok, a, s);
-    const LayerRender *ren = f.layer_ren ? f.layer_ren + (size_t)(2 * (k - 1) + a.wide) * f.layers : nullptr;
-    return launch_render_ao_layered(map, f.tma_ok, a, f.layers, s, ren, kind != MEAO_DEPTH_LINEAR_F32 ? 1 : 0);
+    return launch_render_ao_layered(map, f.tma_ok, a, f.layers, s, render_layer_cams(f, a, k), kind != MEAO_DEPTH_LINEAR_F32 ? 1 : 0);
 }
 
 // PushUpsampleCommands with the wiring of AO.cs:528-531, lo level `lo`.  ao_out (final level only): the caller's AO at the pitches
@@ -322,11 +332,19 @@ inline UpsampleArgs upsample_args(const FrameState &f, int lo, void *ao_out, con
 
 // The upsample launch of lo level `lo`.  aio (final level only): store the AO into a CUDA array.  fused (final level only): read and
 // linearise the raw depth and write LinearDepth, after a low_only prepare of the same depth.
+// The LoResAO1 map of the upsample of lo level `lo`, and its LoResAO2 (HighQuality<lo>: kernels main_premin / main_premin_blendout; nullptr:
+// main / main_blendout)
+inline const CUtensorMap &upsample_ao_map(const FrameState &f, int lo)
+{
+    return (f.plan.variants.single_scale != 0 && lo == 1) ? f.maps.occ1_ups : f.maps.ao_ups[lo];
+}
+inline const uint8_t *upsample_lo_ao2(const FrameState &f, int lo) { return hq_level(f, lo) ? f.hq[lo] : nullptr; }
+
 inline cudaError_t launch_upsample(const FrameState &f, int lo, const UpsampleArgs &a, const ArrayIO *aio, const DepthIn *fused, cudaStream_t s)
 {
     const bool final_level = lo == 1;
-    const uint8_t *lo_ao2 = hq_level(f, lo) ? f.hq[lo] : nullptr;                   // kernels main_premin / main_premin_blendout
-    const CUtensorMap &ao_map = (f.plan.variants.single_scale != 0 && final_level) ? f.maps.occ1_ups : f.maps.ao_ups[lo];
+    const uint8_t *lo_ao2 = upsample_lo_ao2(f, lo);
+    const CUtensorMap &ao_map = upsample_ao_map(f, lo);
     const CUtensorMap &dm = f.maps.low_ups[lo], *hm = &f.maps.hq_ups[lo];
     if (fused && final_level)
         return launch_blur_upsample_lin(dm, ao_map, hm, f.tma_ok, a, lo_ao2, f.occ_pitch[lo], *fused, f.layers, f.sm_count, s);
@@ -435,14 +453,42 @@ inline cudaError_t launch_entry_views(const FrameState &f, const FrameLaunch &l,
         return launch_prepare_depth_views(a, io.views, f.layers, s, f.layer_zb);
     }
     UpsampleArgs a = upsample_args(f, 1, io.aio ? nullptr : io.ao, io.aio ? nullptr : io.vp);
-    const uint8_t *lo_ao2 = hq_level(f, 1) ? f.hq[1] : nullptr;
-    const CUtensorMap &ao_map = f.plan.variants.single_scale != 0 ? f.maps.occ1_ups : f.maps.ao_ups[1];
+    const uint8_t *lo_ao2 = upsample_lo_ao2(f, 1);
+    const CUtensorMap &ao_map = upsample_ao_map(f, 1);
     if (io.aio)
         return launch_blur_upsample_array_views(f.maps.low_ups[1], ao_map, &f.maps.hq_ups[1], f.tma_ok, a, lo_ao2, f.occ_pitch[1], f.layers,
                                                 f.sm_count, io.aio->ao, io.aio->ao_surf, io.views, s);
     a.out_vec_ok = a.out_pitch % 8 == 0;
     return launch_blur_upsample_lin_views(f.maps.low_ups[1], ao_map, &f.maps.hq_ups[1], f.tma_ok, a, lo_ao2, f.occ_pitch[1], d, f.layers,
                                           f.sm_count, io.views, s);
+}
+
+// launch_entry for a frame under an orthographic projection (Plan.orthographic): the launches whose arithmetic depends on the projection
+// -- the prepare of raw depth, every render and the fused final upsample of raw depth -- are the orthographic kernels (kernels.h), every
+// other launch is launch_entry's.  No layer-viewport table and no row band go with an orthographic projection (meao_set_projection).
+// Apart from launch_entry so that a recorder that never sets the projection does not link the orthographic kernels.
+inline cudaError_t launch_entry_ortho(const FrameState &f, const FrameLaunch &l, const FrameIO &io, int force_tile, cudaStream_t s)
+{
+    if (!f.plan.orthographic || io.views) return cudaErrorInvalidValue;
+    if (l.stage == kStagePrepare) {
+        const PrepareArgs a = prepare_args(f, io.depth);
+        if (io.aio) return launch_prepare_depth_array_ortho(a, io.aio->depth, io.aio->depth_surf, io.aio->depth_x, io.aio->depth_y, f.layers, s, f.layer_zb);
+        if (f.layers > 1) return launch_prepare_depth_ortho_layered(a, f.layers, s, io.low_only, f.layer_zb);
+        return launch_prepare_depth_ortho(a, s, io.low_only);
+    }
+    if (l.stage == kStageRender || l.stage == kStageRenderWide) {
+        const RenderArgs a = render_args(f, l.level, io.kind, l.stage == kStageRenderWide, force_tile);
+        const CUtensorMap &map = render_map(f, a, l.level);
+        if (f.layers == 1) return launch_render_ao_ortho(map, f.tma_ok, a, s);
+        return launch_render_ao_ortho_layered(map, f.tma_ok, a, f.layers, s, render_layer_cams(f, a, l.level),
+                                              io.kind != MEAO_DEPTH_LINEAR_F32 ? 1 : 0);
+    }
+    if (l.level == 1 && io.fused) {
+        return launch_blur_upsample_lin_ortho(f.maps.low_ups[1], upsample_ao_map(f, 1), &f.maps.hq_ups[1], f.tma_ok,
+                                              upsample_args(f, 1, io.ao, io.vp), upsample_lo_ao2(f, 1), f.occ_pitch[1], io.depth, f.layers,
+                                              f.sm_count, s);
+    }
+    return launch_entry(f, l, io, force_tile, s);
 }
 
 // ---- the debug buffers (meao_get_buffer, meao_set_buffer, meao_debug_view) ---------------------------------------------------

@@ -96,6 +96,9 @@ constexpr int kPrepareSlots = 7;
 inline int prepare_slot(const PrepareArgs &a) { return a.raw ? 1 + 2 * depth_format_slot(a.in_format) + (a.reversed_z ? 0 : 1) : 0; }
 #define MEAO_PREPARE_SLOTS(K, D24S8) {K<false, true, IN_F32>, K<true, true, IN_F32>, K<true, false, IN_F32>, K<true, true, IN_D16>, \
                                       K<true, false, IN_D16>, D24S8(K<true, true, IN_D24S8>), D24S8(K<true, false, IN_D24S8>)}
+// the raw slots alone (slot 0, linear ingest, holds nullptr): the orthographic kernels, whose linear ingest is the perspective kernel's
+#define MEAO_PREPARE_SLOTS_RAW(K, D24S8) {nullptr, K<true, true, IN_F32>, K<true, false, IN_F32>, K<true, true, IN_D16>, \
+                                          K<true, false, IN_D16>, D24S8(K<true, true, IN_D24S8>), D24S8(K<true, false, IN_D24S8>)}
 // low_only: write LowDepth1..4 only, loading the even rows alone (a.lin is not written); the frame's final upsample then
 // linearises its own pixels and writes LinearDepth (launch_blur_upsample_lin)
 cudaError_t launch_prepare_depth(const PrepareArgs &a, cudaStream_t s, bool low_only = false);
@@ -269,6 +272,24 @@ cudaError_t launch_blur_upsample_lin_views(const CUtensorMap &lo_depth_map, cons
                                            const UpsampleArgs &a, const uint8_t *lo_ao2, int lo_a2pitch, const DepthIn &din, int layers,
                                            int sm_count, const LayerView *views, cudaStream_t s);
 
+// ---- orthographic projection (meao_set_projection): the launches whose arithmetic depends on the projection --------------------------
+// The prepare of raw depth (an affine linearisation, depth_in.cuh), every render (a sampling sphere of constant size: RenderArgs /
+// LayerRender inv_thickness carries it_i and neg_front is not read, render_ao_kernel.inc) and the fused final upsample of raw depth.  Same
+// arguments as the perspective launchers, which they call for linear ingest.  The PrepareArgs / DepthIn / LayerZ zbx, zby carry the
+// affine coefficients {1 - n/f, n/f} (reversed Z: {n/f - 1, 1}).  Separate kernels and translation units (*_ortho*.cu, build.py
+// ORTHO_SOURCES), so the existing kernels keep their code.
+cudaError_t launch_prepare_depth_ortho(const PrepareArgs &a, cudaStream_t s, bool low_only = false);
+cudaError_t launch_prepare_depth_ortho_layered(const PrepareArgs &a, int layers, cudaStream_t s, bool low_only = false,
+                                               const struct LayerZ *layer_zb = nullptr);
+cudaError_t launch_prepare_depth_array_ortho(const PrepareArgs &a, cudaSurfaceObject_t depth, int surf_kind, int depth_x, int depth_y, int layers,
+                                             cudaStream_t s, const struct LayerZ *layer_zb = nullptr);
+cudaError_t launch_render_ao_ortho(const CUtensorMap &low_map, bool use_tma, const RenderArgs &a, cudaStream_t s);
+cudaError_t launch_render_ao_ortho_layered(const CUtensorMap &low_map, bool use_tma, const RenderArgs &a, int layers, cudaStream_t s,
+                                           const struct LayerRender *layer_cam = nullptr, int layer_pad = 0);
+cudaError_t launch_blur_upsample_lin_ortho(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
+                                           const UpsampleArgs &a, const uint8_t *lo_ao2, int lo_a2pitch, const DepthIn &din, int layers,
+                                           int sm_count, cudaStream_t s);
+
 // ---- debug: synthesise a TiledDepth<k> view (reference layout [16][sh][sw], f16 bits) ----------
 cudaError_t launch_synth_tiled(const float *low, int lw, int lh, int lpitch, int sw, int sh, float pad,
                                __half *out, cudaStream_t s);
@@ -367,6 +388,13 @@ extern const KernelUnit kPrepareDepthArrayViewsUnit, kBlurUpsampleArrayViewsUnit
 #ifndef MEAO_EMULATE
 inline const KernelUnit *const kViewKernelUnits[] = {&kPrepareDepthArrayViewsUnit, &kBlurUpsampleArrayViewsUnit, &kPrepareDepthViewsUnit,
                                                      &kBlurUpsampleLinViewsUnit};
+#endif
+// The orthographic units (build.py ORTHO_SOURCES), loaded eagerly like the others and kept out of the emulator's unit list the same way.
+extern const KernelUnit kPrepareDepthOrthoUnit, kPrepareDepthOrthoLayeredUnit, kPrepareDepthArrayOrthoUnit, kRenderAoOrthoUnit,
+    kRenderAoOrthoLayeredUnit, kBlurUpsampleLinOrthoUnit;
+#ifndef MEAO_EMULATE
+inline const KernelUnit *const kOrthoKernelUnits[] = {&kPrepareDepthOrthoUnit, &kPrepareDepthOrthoLayeredUnit, &kPrepareDepthArrayOrthoUnit,
+                                                      &kRenderAoOrthoUnit, &kRenderAoOrthoLayeredUnit, &kBlurUpsampleLinOrthoUnit};
 #endif
 
 // ---- halo pack / unpack: row blocks of pitched buffers <-> contiguous staging, one launch ------

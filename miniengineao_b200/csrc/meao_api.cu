@@ -87,6 +87,7 @@ struct MeaoCtx : SizeState {
     int views_last[2][2] = {{0, 0}, {0, 0}};
     std::vector<std::pair<int, int>> views_checked;
     MeaoVariants variants = {0, 0, 0, 0};
+    int projection = MEAO_PROJECTION_PERSPECTIVE;  // meao_set_projection (a structural input: it selects the orthographic kernels)
     bool plan_dirty = true;                 // a structural input changed: the next frame re-plans (replan)
     // Frame constants (include/meao.h): bumped by every change of MeaoParams or of a camera that keeps the Z direction.  A size whose
     // plan_gen is older re-plans its constants on the host (refresh_constants); a graph captured at an older one re-targets (launch_cached).
@@ -181,8 +182,15 @@ int refuse_reserved(MeaoCtx *c, const char *what)
 {
     return fail(c, MEAO_ERR_UNSUPPORTED, "%s: row bands need an unreserved context (this one reserves %dx%d, meao_reserve)", what, c->res_w, c->res_h);
 }
+// Row bands and an orthographic projection exclude each other too: the band paths have no orthographic kernels.
+int refuse_ortho_band(MeaoCtx *c, const char *what)
+{
+    return fail(c, MEAO_ERR_UNSUPPORTED, "%s: row bands and the halo exchange are not supported under an orthographic projection "
+                "(meao_set_projection)", what);
+}
 #define BAND_GUARD(c, what) do { if ((c) && (c)->layers > 1) return refuse_layered((c), (what)); \
-    if ((c) && (c)->res_w > 0) return refuse_reserved((c), (what)); } while (0)
+    if ((c) && (c)->res_w > 0) return refuse_reserved((c), (what)); \
+    if ((c) && (c)->projection != MEAO_PROJECTION_PERSPECTIVE) return refuse_ortho_band((c), (what)); } while (0)
 #define CUDA_TRY(c, expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) \
     return fail((c), MEAO_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); } while (0)
 
@@ -214,11 +222,20 @@ void note_camera_change(MeaoCtx *c, int old_reversed_z, int new_reversed_z)
 }
 
 // The camera-dependent constants of camera `cam` (the part of build_plan that reads the camera).
+// Under an orthographic projection (include/meao.h meao_set_projection) ZBufferParams holds the affine linearisation {1 - n/f, n/f}
+// (reversed: {n/f - 1, 1}), the inv_thickness tables hold it_i = (far / ThicknessMultiplier) / SampleThickness[i] -- a sphere of constant
+// size, in units of LinearDepth (eye depth / far) -- and the padding value is the linearisation of raw depth 0.
 void camera_consts(const MeaoCtx *c, const MeaoCamera &cam, CamConsts &p)
 {
-    // AO.cs:561-568
-    const float fpn = cam.far_clip / cam.near_clip;
-    if (cam.reversed_z) { p.zb[0] = fpn - 1; p.zb[1] = 1; } else { p.zb[0] = 1 - fpn; p.zb[1] = fpn; }
+    const bool ortho = c->projection == MEAO_PROJECTION_ORTHOGRAPHIC;
+    if (!ortho) {
+        // AO.cs:561-568
+        const float fpn = cam.far_clip / cam.near_clip;
+        if (cam.reversed_z) { p.zb[0] = fpn - 1; p.zb[1] = 1; } else { p.zb[0] = 1 - fpn; p.zb[1] = fpn; }
+    } else {
+        const float r = cam.near_clip / cam.far_clip;
+        if (cam.reversed_z) { p.zb[0] = r - 1; p.zb[1] = 1; } else { p.zb[0] = 1 - r; p.zb[1] = r; }
+    }
 
     float thick[12];
     sample_thickness(thick);
@@ -227,13 +244,13 @@ void camera_consts(const MeaoCtx *c, const MeaoCamera &cam, CamConsts &p)
         const float ScreenspaceDiameter = 10;                                                        // AO.cs:669
         float ThicknessMultiplier = 2 * cam.tan_half_fov_h * ScreenspaceDiameter / src_w;           // AO.cs:678
         if (c->variants.single_pass_stereo) ThicknessMultiplier *= 2;                                // AO.cs:680
-        float InverseRangeFactor = 1 / ThicknessMultiplier;                                          // AO.cs:683
+        float InverseRangeFactor = ortho ? cam.far_clip / ThicknessMultiplier : 1 / ThicknessMultiplier;   // AO.cs:683
         for (int i = 0; i < 12; i++) p.inv_thickness[k][i] = InverseRangeFactor / thick[i];          // AO.cs:687-688
         {   // the same recorder fed a non-tiled source (LowDepth<k>): kernel "main"
             float tm = 2 * cam.tan_half_fov_h * ScreenspaceDiameter / c->lw[k];                     // AO.cs:678
             tm *= 2;                                                                                 // AO.cs:679 (!source.isTiled)
             if (c->variants.single_pass_stereo) tm *= 2;                                             // AO.cs:680
-            const float irf = 1 / tm;                                                                // AO.cs:683
+            const float irf = ortho ? cam.far_clip / tm : 1 / tm;                                    // AO.cs:683
             for (int i = 0; i < 12; i++) p.inv_thickness_wide[k][i] = irf / thick[i];
         }
         // value of the atlas padding texels (SURVEY.md P3): Downsample1 writes Linearize(OOB load = 0),
@@ -241,7 +258,8 @@ void camera_consts(const MeaoCtx *c, const MeaoCamera &cam, CamConsts &p)
         float pad = 0.0f;
         if (k <= 2) {
             // raw depth 0 through Linearize (DS1:40-45); linear ingest: 0
-            pad = cam.reversed_z ? 1e5f : 1.0f / std::fmaf(p.zb[0], 0.0f, p.zb[1]);
+            if (ortho) pad = cam.reversed_z ? 1e5f : std::fmaf(p.zb[0], 0.0f, p.zb[1]);
+            else pad = cam.reversed_z ? 1e5f : 1.0f / std::fmaf(p.zb[0], 0.0f, p.zb[1]);
         }
         p.pad[k] = pad;   // the depth-kind dependent part (linear ingest -> 0) is applied at launch
     }
@@ -269,6 +287,7 @@ void build_plan(MeaoCtx *c)
     p.zb[2] = p.zb[3] = 0;
     p.variants = c->variants;
     p.reversed_z = ctx_reversed_z(c);
+    p.orthographic = c->projection == MEAO_PROJECTION_ORTHOGRAPHIC;
     memcpy(p.inv_thickness, cc.inv_thickness, sizeof p.inv_thickness);
     memcpy(p.inv_thickness_wide, cc.inv_thickness_wide, sizeof p.inv_thickness_wide);
     memcpy(p.pad, cc.pad, sizeof p.pad);
@@ -643,7 +662,7 @@ int record_launch(MeaoCtx *c, const FrameLaunch &l, const FrameIO &io, cudaStrea
     static const char *nvtx[4] = {"meao::prepare_depth", "meao::render_ao", "meao::render_ao_wide", "meao::blur_upsample"};
     if (l.stage == kStageUpsample && l.level == 1) c->last_out = io.aio ? const_cast<void *>(io.aio->ao_array) : io.ao;
     NvtxRange nv(nvtx[l.stage]);
-    CUDA_TRY(c, launch_entry_views(*c, l, io, forced_render_tile(), s));
+    CUDA_TRY(c, c->plan.orthographic ? launch_entry_ortho(*c, l, io, forced_render_tile(), s) : launch_entry_views(*c, l, io, forced_render_tile(), s));
     c->launches++;
     return 0;
 }
@@ -842,6 +861,7 @@ int meao_create(const MeaoDeviceCfg *cfg, MeaoCtx **out)
             cudaError_t pe = cudaSuccess;
             for (const KernelUnit *u : kKernelUnits) u->walk(&pe);
             for (const KernelUnit *u : kViewKernelUnits) u->walk(&pe);
+            for (const KernelUnit *u : kOrthoKernelUnits) u->walk(&pe);
             if (pe != cudaSuccess) { cudaGetLastError(); meao_destroy(c); return fail(nullptr, MEAO_ERR_CUDA, "loading the kernels failed: %s", cudaGetErrorString(pe)); }
             preloaded[dev] = true;
         }
@@ -932,6 +952,27 @@ int meao_set_camera(MeaoCtx *c, const MeaoCamera *cam)
     return MEAO_OK;
 }
 
+int meao_set_projection(MeaoCtx *c, int32_t projection)
+{
+    if (!c) return MEAO_ERR_INVALID;
+    if (projection != MEAO_PROJECTION_PERSPECTIVE && projection != MEAO_PROJECTION_ORTHOGRAPHIC)
+        return fail(c, MEAO_ERR_INVALID, "projection %d is neither MEAO_PROJECTION_PERSPECTIVE (0) nor MEAO_PROJECTION_ORTHOGRAPHIC (1)", projection);
+    if (projection == c->projection) return 0;
+    if (projection == MEAO_PROJECTION_ORTHOGRAPHIC) {
+        if (!c->views.empty())
+            return fail(c, MEAO_ERR_UNSUPPORTED, "an orthographic projection is not supported with a layer-viewport table (meao_set_layer_viewports)");
+        if ((c->W > 0 && (c->band0 != 0 || c->band1 != c->H)) || c->peer_base[0] || c->peer_base[1])
+            return fail(c, MEAO_ERR_UNSUPPORTED, "an orthographic projection is not supported with a row band or a neighbour connection "
+                        "(meao_set_row_band, meao_band_connect)");
+    }
+    c->projection = projection;
+    c->plan_dirty = true;           // other kernels and other constants: re-plan + drop the captured graphs (ensure_ready)
+    c->frame_gen++;
+    return 1;
+}
+
+int meao_get_projection(const MeaoCtx *c) { return c ? c->projection : MEAO_ERR_INVALID; }
+
 int meao_set_layer_cameras(MeaoCtx *c, const MeaoCamera *cams, int32_t count)
 {
     if (!c) return MEAO_ERR_INVALID;
@@ -989,6 +1030,8 @@ int meao_set_layer_viewports(MeaoCtx *c, const MeaoLayerViewport *views, int32_t
         return 1;
     }
     if (!views) return fail(c, MEAO_ERR_INVALID, "views is NULL with count %d (NULL clears the table only with count 0)", count);
+    if (c->projection != MEAO_PROJECTION_PERSPECTIVE)
+        return fail(c, MEAO_ERR_UNSUPPORTED, "a layer-viewport table is not supported under an orthographic projection (meao_set_projection)");
     if (count != c->layers) return fail(c, MEAO_ERR_INVALID, "count %d differs from the context's %d layers (meao_set_layers)", count, c->layers);
     for (int l = 0; l < count; l++)
         for (int i = 0; i < 6; i++)
