@@ -89,6 +89,12 @@ namespace MiniEngineAO
         [DllImport(Lib)] public static extern int meao_bind_event_arrays_at(IntPtr ctx, int eventId, IntPtr depthArray, int depthX, int depthY, int depthKind,
                                                                             IntPtr aoArray, int aoX, int aoY, IntPtr stream);
         [DllImport(Lib)] public static extern int meao_release_array(IntPtr ctx, IntPtr array);   // before the array is unmapped / unregistered / freed
+        // Batches: layer l of a layered frame reads depthArrays[l] and writes aoArrays[l] -- several cameras, each with its own targets
+        // (count = meao_set_layers, at most MEAO_MAX_BATCH = 256; each array 2-D, at least W x H, the frame at its top-left corner)
+        [DllImport(Lib)] public static extern int meao_render_arrays_batch(IntPtr ctx, [In] IntPtr[] depthArrays, int depthKind, [In] IntPtr[] aoArrays,
+                                                                           int count, IntPtr stream);
+        [DllImport(Lib)] public static extern int meao_bind_event_arrays_batch(IntPtr ctx, int eventId, [In] IntPtr[] depthArrays, int depthKind,
+                                                                               [In] IntPtr[] aoArrays, int count, IntPtr stream);
         // Linear buffers with their own row and layer pitch, in bytes (D3D12 placed footprints, Vulkan buffers through external memory,
         // cudaMallocPitch, a dynamic-resolution corner of a max-size target), no copies
         [DllImport(Lib)] public static extern int meao_render_pitched(IntPtr ctx, IntPtr depthDev, long depthRowPitch, long depthLayerPitch, int depthKind,
@@ -342,6 +348,22 @@ namespace MiniEngineAO
         {
             MeaoNative.Check(_ctx, MeaoNative.meao_render_arrays_at(_ctx, depthArray, depthOrigin.x, depthOrigin.y, depthKind, aoArray,
                                                                     aoOrigin.x, aoOrigin.y, _stream));
+        }
+
+        // One frame of every camera of a batch, each layer from and into its own mapped arrays (meao_render_arrays_batch): the
+        // context's layer count must equal the list length.  Release each array with meao_release_array before it is unmapped.
+        public void RenderArraysBatch(IntPtr[] depthArrays, IntPtr[] aoArrays, int depthKind = 0)
+        {
+            if (depthArrays.Length != aoArrays.Length) throw new ArgumentException("one depth and one AO array per layer");
+            MeaoNative.Check(_ctx, MeaoNative.meao_render_arrays_batch(_ctx, depthArrays, depthKind, aoArrays, depthArrays.Length, _stream));
+        }
+
+        // The plugin event renders the batch: the library copies the lists and checks them now (the event cannot report errors).
+        public void BindEventArraysBatch(IntPtr[] depthArrays, IntPtr[] aoArrays, int depthKind = 0)
+        {
+            if (depthArrays.Length != aoArrays.Length) throw new ArgumentException("one depth and one AO array per layer");
+            MeaoNative.Check(_ctx, MeaoNative.meao_bind_event_arrays_batch(_ctx, kEventId, depthArrays, depthKind, aoArrays, depthArrays.Length,
+                                                                           _stream));
         }
 
         // The pitched path of the plugin event: meao_render_pitched on the mapped buffers at their own pitches (checked here -- the

@@ -41,7 +41,9 @@ extern "C" {
                               *    + meao_render_arrays_at / meao_bind_event_arrays_at (viewports of larger CUDA arrays; additive)
                               *    + MeaoLayerViewport, meao_set_layer_viewports / meao_get_layer_viewports (each layer at its own
                               *      viewport of shared CUDA arrays: split-screen, side-by-side stereo, cube atlases; additive)
-                              *    + MeaoProjection, meao_set_projection / meao_get_projection (orthographic cameras; additive) */
+                              *    + MeaoProjection, meao_set_projection / meao_get_projection (orthographic cameras; additive)
+                              *    + MEAO_MAX_BATCH, meao_render_arrays_batch / meao_render_batch / meao_bind_event_arrays_batch (each
+                              *      layer with its own depth and AO resources: several cameras, each with its own targets; additive) */
 
 typedef struct MeaoCtx MeaoCtx;
 
@@ -381,6 +383,42 @@ int meao_render_arrays(MeaoCtx *ctx, const void *depth_array, int32_t depth_kind
 int meao_render_arrays_at(MeaoCtx *ctx, const void *depth_array, int32_t depth_x, int32_t depth_y, int32_t depth_kind,
                           void *ao_array, int32_t ao_x, int32_t ao_y, void *stream);
 int meao_release_array(MeaoCtx *ctx, const void *array);
+/* ---- Batches: each layer with its own depth and AO --------------------------------------------------------------------------
+ * A layered frame (meao_set_layers L) whose layer l reads its own depth and writes its own AO: cameras that each render into their own
+ * targets (a Camera's own render textures, separate split-screen targets, one buffer per sensor, a list of tensors) in one frame of 9
+ * launches instead of L contexts or a copy into and out of one stacked allocation.  Only the frame's first and last kernel touch the
+ * caller's memory; they take the whole list as a kernel parameter.
+ *   - Bit-identical per layer: layer l is bit-identical, on the AO and on every debug buffer, to a single-layer frame of that layer's
+ *     depth with that layer's camera (meao_set_layer_cameras, or the context's camera for every layer).
+ *   - count must equal the layer count, and be at most MEAO_MAX_BATCH.
+ *   - Arrays (meao_render_arrays_batch): each entry is a 2-D array, or a cudaArrayLayered array of depth 1, with the formats and the
+ *     cudaArraySurfaceLoadStore flag meao_render_arrays requires (RAW_D24S8: MEAO_ERR_UNSUPPORTED).  Each must be AT LEAST W x H; the
+ *     frame sits at its top-left corner, so a dynamic-resolution host (meao_reserve) keeps per-camera targets at their maximum size.
+ *     No texel outside W x H is read or written.  No two layers may share an AO array; depth arrays may repeat.
+ *   - Pointers (meao_render_batch): layer l reads depth[l], rows depth_row_pitch[l] bytes apart, and writes ao[l], rows ao_row_pitch[l]
+ *     bytes apart (0 = tight: W x element size, W).  Per layer the checks of meao_render_pitched: pitches at least a row, at most
+ *     INT32_MAX, the depth pitch a multiple of the element size, depth[l] aligned to its element.  No two AO byte extents may
+ *     intersect, nor an AO extent any depth extent (an extent: first to last byte of a layer's view); depth entries may repeat.  The
+ *     check sorts the extents: O(L log L).  Each layer's vector loads and stores depend on its own base and pitch (16 bytes for the
+ *     depth, 8 for the AO); a misaligned layer takes the element-wise path for its own pixels only, with the same result.
+ *   - Refusals: MEAO_ERR_INVALID with the layer and field named in meao_last_error, and nothing launched, for a count that differs from
+ *     the layer count or exceeds MEAO_MAX_BATCH, a NULL list or entry, a shared AO array, intersecting extents, and every per-entry
+ *     check above.  A set layer-viewport table (meao_set_layer_viewports) is refused with MEAO_ERR_INVALID; an orthographic projection
+ *     and a row band with MEAO_ERR_UNSUPPORTED.
+ *   - Everything else is the layered frame's contract: per-layer cameras, the variants, MEAO_FLAG_NO_GRAPH, reservations, live frame
+ *     constants, and after a frame the regeneration of id 17 by meao_get_buffer / meao_debug_view.  meao_kernels_per_frame is unchanged.
+ *   - Graphs: one per (list, kind, size), the list compared in full; a host that rotates more lists than the cache holds re-targets
+ *     the least recently used graph like any other frame.  Capturable into a caller's graph: the list is baked into the recorded frame,
+ *     so a list, like an array or an origin, does not move meao_frame_generation.  An array batch is refused inside a capture for an
+ *     array this context has not rendered with yet (its surface object is made then).
+ *   - Release contract: meao_release_array(a) drops every cached graph and event binding whose list names a. */
+#define MEAO_MAX_BATCH 256
+/* Layer l of the frame reads depth_arrays[l] and writes ao_arrays[l]; count must equal meao_set_layers. */
+int meao_render_arrays_batch(MeaoCtx *ctx, const void *const *depth_arrays, int32_t depth_kind, void *const *ao_arrays, int32_t count,
+                             void *stream);
+/* Layer l reads depth[l] (row pitch depth_row_pitch[l] bytes, 0 = tight) and writes ao[l] (ao_row_pitch[l], 0 = tight). */
+int meao_render_batch(MeaoCtx *ctx, const void *const *depth, const int64_t *depth_row_pitch, int32_t depth_kind, void *const *ao,
+                      const int64_t *ao_row_pitch, int32_t count, void *stream);
 /* Pipelined form of meao_render_host for frame streams: enqueues H2D + kernels + D2H of one frame on staging slot
  * `slot` (0 or 1) and returns; meao_host_wait(slot) blocks until that frame's AO is in ao_out_host.  Alternating the
  * two slots overlaps the H2D copy of frame i+1 with the kernels and the D2H copy of frame i (the kernels of
@@ -550,6 +588,11 @@ int meao_bind_event_arrays_at(MeaoCtx *ctx, int32_t event_id, const void *depth_
 int meao_bind_event_pitched(MeaoCtx *ctx, int32_t event_id,
                             const void *depth_dev, int64_t depth_row_pitch, int64_t depth_layer_pitch, int32_t depth_kind,
                             void *ao_out_dev, int64_t ao_row_pitch, int64_t ao_layer_pitch, void *stream);
+/* The plugin-event twin of meao_render_arrays_batch: copies the lists and checks them now (with its refusals, and makes the surface
+ * objects, so the event may run inside a capture); both NULL unbinds.  meao_release_array removes the bindings whose lists name the
+ * array. */
+int meao_bind_event_arrays_batch(MeaoCtx *ctx, int32_t event_id, const void *const *depth_arrays, int32_t depth_kind,
+                                 void *const *ao_arrays, int32_t count, void *stream);
 void meao_render_event(int event_id);
 MeaoRenderEventFunc meao_get_render_event_func(void);
 
@@ -562,7 +605,8 @@ MeaoRenderEventFunc meao_get_render_event_func(void);
  * carry programmatic dependent launch at the level an instantiation of this context has accepted (meao_pdl_level; none before the
  * first), so a frame recorded into a caller's graph matches the context's own.  The capture status query is the only cost a frame
  * outside a capture pays for this.
- * Capturable: meao_render, meao_render_pitched, meao_render_arrays(_at), meao_render_event (any binding), the meao_stage_* calls,
+ * Capturable: meao_render, meao_render_pitched, meao_render_arrays(_at), meao_render_arrays_batch, meao_render_batch, meao_render_event
+ * (any binding), the meao_stage_* calls,
  * meao_render_band_prepare / _finish, meao_band_phase_a / _b, meao_band_step, meao_halo_pack / _unpack, meao_debug_view and the three
  * meao_composite_* calls.
  * SETTLED CONTEXTS ONLY: inside a capture a call may issue nothing but kernel launches.  It is refused with MEAO_ERR_INVALID, records
@@ -570,7 +614,8 @@ MeaoRenderEventFunc meao_get_render_event_func(void);
  *   - a structural change is pending (a re-plan synchronises the device; meao_set_projection is one),
  *   - the per-layer camera tables are still to be written: after a frame-constant change, or on the first frame at a size,
  *   - a changed layer-viewport table (meao_set_layer_viewports) is still to be written,
- *   - or, for meao_render_arrays(_at), the context has not rendered with one of the arrays yet (its surface object is made then).
+ *   - or, for meao_render_arrays(_at) and meao_render_arrays_batch, the context has not rendered with one of the arrays yet (its
+ *     surface object is made then).
  * One frame of the same form issued outside the capture settles the context; torch's warm-up before torch.cuda.graph does that.
  * A capture that has been invalidated returns MEAO_ERR_CUDA and records nothing.
  * NOT capturable: the host-buffer calls (meao_render_host, _host_async, meao_host_wait, meao_band_step_host; they run on the

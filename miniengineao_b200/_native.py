@@ -88,6 +88,9 @@ SIGNATURES = {
     "meao_render_arrays": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "meao_render_arrays_at": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
     "meao_release_array": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "meao_render_arrays_batch": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_int32, C.POINTER(C.c_void_p), C.c_int32, C.c_void_p]),
+    "meao_render_batch": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.c_int32, C.POINTER(C.c_void_p),
+                                    C.POINTER(C.c_int64), C.c_int32, C.c_void_p]),
     "meao_render_host_async": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32]),
     "meao_host_wait": (C.c_int, [C.c_void_p, C.c_int32]),
     "meao_synchronize": (C.c_int, [C.c_void_p]),
@@ -132,6 +135,8 @@ SIGNATURES = {
                                             C.c_void_p]),
     "meao_bind_event_pitched": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_int64,
                                           C.c_int64, C.c_void_p]),
+    "meao_bind_event_arrays_batch": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_void_p), C.c_int32, C.POINTER(C.c_void_p), C.c_int32,
+                                               C.c_void_p]),
     "meao_render_event": (None, [C.c_int]),
     "meao_get_render_event_func": (RENDER_EVENT_FUNC, []),
     "meao_launch_count": (C.c_int64, [C.c_void_p]),

@@ -320,6 +320,45 @@ class AmbientOcclusion:
         self._check(self._lib.meao_render_arrays_at(self._ctx, C.c_void_p(depth_array), int(dx), int(dy), self._ARRAY_KINDS[kind],
                                                     C.c_void_p(ao_array), int(ax), int(ay), self._stream(stream)))
 
+    def render_batch(self, depths, outs=None, *, linear: bool = False, stream=None) -> list:
+        """One layered frame over a list of separate CUDA tensors (meao_render_batch): layer l reads depths[l] and writes outs[l].
+        depths: one [H, W] CUDA tensor per layer (the context's layer count), all of one dtype (as render), each with its own row stride
+        (last stride 1).  outs: uint8 [H, W] CUDA tensors, or None for new ones.  Each layer is bit-identical to a single-layer frame of
+        its own depth.  Returns outs."""
+        import torch
+        self.LateUpdate()
+        shape = (self._height, self._width)
+        depths = list(depths)
+        if not depths or any(not d.is_cuda or tuple(d.shape) != shape for d in depths):
+            raise ValueError(f"depths must be a non-empty list of CUDA tensors {shape}")
+        if len({d.dtype for d in depths}) != 1:
+            raise ValueError("depths must share one dtype")
+        if outs is None:
+            outs = [torch.empty(shape, dtype=torch.uint8, device=d.device) for d in depths]
+        outs = list(outs)
+        if len(outs) != len(depths) or any(not o.is_cuda or o.dtype != torch.uint8 or tuple(o.shape) != shape for o in outs):
+            raise ValueError(f"outs must be {len(depths)} uint8 CUDA tensors {shape}")
+        kind = self._kind(str(depths[0].dtype).replace("torch.", ""), linear)
+        n = len(depths)
+        P, I64 = C.c_void_p * n, C.c_int64 * n
+        self._check(self._lib.meao_render_batch(self._ctx, P(*[d.data_ptr() for d in depths]), I64(*[self._pitches(d, "depth")[0] for d in depths]),
+                                                kind, P(*[o.data_ptr() for o in outs]), I64(*[self._pitches(o, "out")[0] for o in outs]), n,
+                                                self._stream(stream)))
+        return outs
+
+    def render_arrays_batch(self, depth_arrays, ao_arrays, *, kind: str = "raw_f32", stream=None) -> None:
+        """One layered frame over lists of CUDA arrays (meao_render_arrays_batch): layer l reads depth_arrays[l] and writes
+        ao_arrays[l] (integer cudaArray_t handles, one per layer).  Each array is 2-D (or layered of depth 1), at least W x H, with
+        cudaArraySurfaceLoadStore; the frame sits at its top-left corner.  kind: as render_arrays."""
+        if kind not in self._ARRAY_KINDS:
+            raise ValueError(f"kind must be one of {sorted(self._ARRAY_KINDS)}")
+        self.LateUpdate()
+        d, a = list(depth_arrays), list(ao_arrays)
+        if len(d) != len(a):
+            raise ValueError("depth_arrays and ao_arrays must have one entry per layer each")
+        P = C.c_void_p * len(d)
+        self._check(self._lib.meao_render_arrays_batch(self._ctx, P(*d), self._ARRAY_KINDS[kind], P(*a), len(d), self._stream(stream)))
+
     def release_array(self, handle: int) -> None:
         """Drop the graphs, the surface object and the event bindings that refer to a CUDA array (meao_release_array; synchronises
         the device).  Required before the array is freed or re-registered: a new array may come back with the same handle."""

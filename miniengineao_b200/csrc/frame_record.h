@@ -419,6 +419,15 @@ struct FrameIO {
     void *ao = nullptr;                 // the final upsample's AO at the pitches of vp (nullptr: tight); nullptr: the result buffer
     const ViewPitch *vp = nullptr;
     const LayerView *views = nullptr;   // layer l reads and writes the rectangles and slices of views[l] (launch_entry_views)
+    const struct BatchIO *batch = nullptr;  // layer l reads and writes its own resources (launch_entry_batch)
+};
+
+// A batch (meao_render_arrays_batch / meao_render_batch): the kernel-parameter tables of its first and last launch.  arrays: layer l
+// reads depth.e[l] and writes ao.e[l]; otherwise layer l reads and writes its own buffers, ptr.e[l].
+struct BatchIO {
+    bool arrays = false;
+    BatchArrays depth{}, ao{};
+    BatchPointers ptr{};
 };
 
 // Launches schedule entry l of a frame on stream s.  force_tile: render_tile_variant's force.
@@ -461,6 +470,30 @@ inline cudaError_t launch_entry_views(const FrameState &f, const FrameLaunch &l,
     a.out_vec_ok = a.out_pitch % 8 == 0;
     return launch_blur_upsample_lin_views(f.maps.low_ups[1], ao_map, &f.maps.hq_ups[1], f.tma_ok, a, lo_ao2, f.occ_pitch[1], d, f.layers,
                                           f.sm_count, io.views, s);
+}
+
+// launch_entry for a batch (FrameIO.batch): its prepare and its final upsample are the batch kernels, every other launch is launch_entry's.
+// A CUDA-array batch, or a pointer batch recorded fused (io.low_only and io.fused: the prepare reads the even rows, the final upsample
+// linearises every pixel).  Perspective and whole frames only (meao_api.cu refuses an orthographic projection and a row band).  Apart
+// from launch_entry so that a recorder that never renders a batch does not link the batch kernels.
+inline cudaError_t launch_entry_batch(const FrameState &f, const FrameLaunch &l, const FrameIO &io, int force_tile, cudaStream_t s)
+{
+    const bool final_level = l.stage == kStageUpsample && l.level == 1;
+    if (!io.batch || (l.stage != kStagePrepare && !final_level)) return launch_entry(f, l, io, force_tile, s);
+    if (f.plan.orthographic || io.aio || io.views || (!io.batch->arrays && !(io.low_only && io.fused))) return cudaErrorInvalidValue;
+    if (l.stage == kStagePrepare) {
+        const PrepareArgs a = prepare_args(f, io.depth);
+        if (io.batch->arrays) return launch_prepare_depth_array_batch(a, io.batch->depth, f.layers, s, f.layer_zb);
+        return launch_prepare_depth_batch(a, io.batch->ptr, f.layers, s, f.layer_zb);
+    }
+    const UpsampleArgs a = upsample_args(f, 1, nullptr, nullptr);
+    const uint8_t *lo_ao2 = upsample_lo_ao2(f, 1);
+    const CUtensorMap &ao_map = upsample_ao_map(f, 1);
+    if (io.batch->arrays)
+        return launch_blur_upsample_array_batch(f.maps.low_ups[1], ao_map, &f.maps.hq_ups[1], f.tma_ok, a, lo_ao2, f.occ_pitch[1], f.layers,
+                                                f.sm_count, io.batch->ao, s);
+    return launch_blur_upsample_lin_batch(f.maps.low_ups[1], ao_map, &f.maps.hq_ups[1], f.tma_ok, a, lo_ao2, f.occ_pitch[1], io.depth, f.layers,
+                                          f.sm_count, io.batch->ptr, s);
 }
 
 // launch_entry for a frame under an orthographic projection (Plan.orthographic): the launches whose arithmetic depends on the projection

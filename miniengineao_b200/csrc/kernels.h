@@ -272,6 +272,35 @@ cudaError_t launch_blur_upsample_lin_views(const CUtensorMap &lo_depth_map, cons
                                            const UpsampleArgs &a, const uint8_t *lo_ao2, int lo_a2pitch, const DepthIn &din, int layers,
                                            int sm_count, const LayerView *views, cudaStream_t s);
 
+// ---- batches (meao_render_arrays_batch / meao_render_batch): layer l of a layered frame reads and writes resources of its own ---------
+// The first and the last kernel of the frame in a form that takes each layer's depth and AO from entry l of a table passed BY VALUE as a
+// __grid_constant__ kernel parameter (read at blockIdx.z; the upsample: at its tile's layer).  A parameter rather than an arena table
+// (LayerView): the list is baked into the context's graphs and the caller's captures, so there is no stream-ordered table write, and a
+// replay can never read another frame's list.  BatchArrays is 4 KB and BatchPointers 6 KB: over the classic 4 KB parameter limit, inside
+// the 32,764 bytes CUDA >= 12.1 allows on sm_70+.  The caller has checked every entry (meao_api.cu check_batch_*); only layers < `layers`
+// are read.  Separate kernels and translation units (*_batch.cu, build.py BATCH_SOURCES), so the existing kernels keep their code.
+constexpr int kMaxBatch = 256;                                  // include/meao.h MEAO_MAX_BATCH
+struct BatchSurf { cudaSurfaceObject_t surf; int kind; };       // a 2-D array (kSurf2D) or a layered array of depth 1 (kSurfLayered, layer 0)
+struct BatchArrays { BatchSurf e[kMaxBatch]; };
+// one layer of a pointer batch: its depth (rows depth_pitch ELEMENTS apart) and its AO (rows ao_pitch BYTES apart).  The kernels test
+// each base and pitch for the vector loads and stores themselves: a misaligned layer takes the element-wise path for its own pixels.
+struct BatchPtr { const void *depth; uint8_t *ao; int depth_pitch; int ao_pitch; };
+struct BatchPointers { BatchPtr e[kMaxBatch]; };
+static_assert(sizeof(BatchArrays) == 4096 && sizeof(BatchPointers) == 6144, "the batch tables' parameter sizes");
+// CUDA arrays: prepare (f32 / D16) and the final upsample, frame pixel (x, y) at texel (x, y) of layer l's arrays
+cudaError_t launch_prepare_depth_array_batch(const PrepareArgs &a, const BatchArrays &depth, int layers, cudaStream_t s,
+                                             const struct LayerZ *layer_zb = nullptr);
+cudaError_t launch_blur_upsample_array_batch(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map,
+                                             bool use_tma, const UpsampleArgs &a, const uint8_t *lo_ao2, int lo_a2pitch, int layers, int sm_count,
+                                             const BatchArrays &ao, cudaStream_t s);
+// The fused pointer frame: the low-only prepare and the fused final upsample.  a.depth / din.depth, their pitches and a.out are unused:
+// each layer's come from its entry.
+cudaError_t launch_prepare_depth_batch(const PrepareArgs &a, const BatchPointers &io, int layers, cudaStream_t s,
+                                       const struct LayerZ *layer_zb = nullptr);
+cudaError_t launch_blur_upsample_lin_batch(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
+                                           const UpsampleArgs &a, const uint8_t *lo_ao2, int lo_a2pitch, const DepthIn &din, int layers,
+                                           int sm_count, const BatchPointers &io, cudaStream_t s);
+
 // ---- orthographic projection (meao_set_projection): the launches whose arithmetic depends on the projection --------------------------
 // The prepare of raw depth (an affine linearisation, depth_in.cuh), every render (a sampling sphere of constant size: RenderArgs /
 // LayerRender inv_thickness carries it_i and neg_front is not read, render_ao_kernel.inc) and the fused final upsample of raw depth.  Same
@@ -395,6 +424,13 @@ extern const KernelUnit kPrepareDepthOrthoUnit, kPrepareDepthOrthoLayeredUnit, k
 #ifndef MEAO_EMULATE
 inline const KernelUnit *const kOrthoKernelUnits[] = {&kPrepareDepthOrthoUnit, &kPrepareDepthOrthoLayeredUnit, &kPrepareDepthArrayOrthoUnit,
                                                       &kRenderAoOrthoUnit, &kRenderAoOrthoLayeredUnit, &kBlurUpsampleLinOrthoUnit};
+#endif
+// The batch units (build.py BATCH_SOURCES), loaded eagerly like the others.  The emulator builds them into a library of their own
+// (tests/emu/batch.py), so the emulator's unit list above stays the SOURCES one.
+extern const KernelUnit kPrepareDepthArrayBatchUnit, kBlurUpsampleArrayBatchUnit, kPrepareDepthBatchUnit, kBlurUpsampleLinBatchUnit;
+#ifndef MEAO_EMULATE
+inline const KernelUnit *const kBatchKernelUnits[] = {&kPrepareDepthArrayBatchUnit, &kBlurUpsampleArrayBatchUnit, &kPrepareDepthBatchUnit,
+                                                      &kBlurUpsampleLinBatchUnit};
 #endif
 
 // ---- halo pack / unpack: row blocks of pitched buffers <-> contiguous staging, one launch ------

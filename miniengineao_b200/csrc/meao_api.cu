@@ -17,6 +17,7 @@
 #include <cmath>
 #include <functional>
 #include <map>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <tuple>
@@ -135,12 +136,17 @@ struct MeaoCtx : SizeState {
     // same pointers with other pitches is another graph, never a replay that reads the wrong rows.
     // size: the frame size and camera table slot the graph was captured at (launch_cached fills it in) -- a reserved context keeps the
     // graphs of every size it has visited, and a size re-planned into another slot never replays a graph that reads the old slot.
-    struct GraphKey { const void *p[4]; int kind; int64_t pitch[4] = {0, 0, 0, 0}; int size[3] = {0, 0, 0}; bool operator<(const GraphKey &o) const {
+    // list / list_hash: a batch's whole list (kBatchArrayGraphKind+: the depth arrays, then the AO arrays; kBatchGraphKind+: depth, depth
+    // row pitch, AO, AO row pitch per layer), compared by its hash first and in full on a tie, so a graph replays only its own list.
+    struct GraphKey { const void *p[4]; int kind; int64_t pitch[4] = {0, 0, 0, 0}; int size[3] = {0, 0, 0}; uint64_t list_hash = 0;
+        std::vector<uintptr_t> list = {};
+        bool operator<(const GraphKey &o) const {
         for (int i = 0; i < 4; i++) if (p[i] != o.p[i]) return p[i] < o.p[i];
         if (kind != o.kind) return kind < o.kind;
         for (int i = 0; i < 4; i++) if (pitch[i] != o.pitch[i]) return pitch[i] < o.pitch[i];
         for (int i = 0; i < 3; i++) if (size[i] != o.size[i]) return size[i] < o.size[i];
-        return false; } };
+        if (list_hash != o.list_hash) return list_hash < o.list_hash;
+        return list < o.list; } };
     // launches: the kernels its capture recorded; gen: the plan_gen of the constants it launches with
     struct GraphEntry { cudaGraphExec_t exec; uint64_t last_use; int launches; uint64_t gen; };
     std::map<GraphKey, GraphEntry> graphs;
@@ -660,9 +666,10 @@ int forced_render_tile()
 int record_launch(MeaoCtx *c, const FrameLaunch &l, const FrameIO &io, cudaStream_t s)
 {
     static const char *nvtx[4] = {"meao::prepare_depth", "meao::render_ao", "meao::render_ao_wide", "meao::blur_upsample"};
-    if (l.stage == kStageUpsample && l.level == 1) c->last_out = io.aio ? const_cast<void *>(io.aio->ao_array) : io.ao;
+    if (l.stage == kStageUpsample && l.level == 1 && !io.batch) c->last_out = io.aio ? const_cast<void *>(io.aio->ao_array) : io.ao;
     NvtxRange nv(nvtx[l.stage]);
-    CUDA_TRY(c, c->plan.orthographic ? launch_entry_ortho(*c, l, io, forced_render_tile(), s) : launch_entry_views(*c, l, io, forced_render_tile(), s));
+    if (io.batch) CUDA_TRY(c, launch_entry_batch(*c, l, io, forced_render_tile(), s));
+    else CUDA_TRY(c, c->plan.orthographic ? launch_entry_ortho(*c, l, io, forced_render_tile(), s) : launch_entry_views(*c, l, io, forced_render_tile(), s));
     c->launches++;
     return 0;
 }
@@ -783,8 +790,9 @@ std::mutex g_event_mutex;
 // each time the event runs; exact: meao_bind_event_arrays (W x H arrays).  Otherwise a pointer frame at the pitches `pitch`, or, with
 // tight (meao_bind_event), at the tight pitches of the context when the event runs -- a meao_resize between binding and rendering keeps
 // meaning what it meant before.
+// batch (meao_bind_event_arrays_batch): copies of the lists, depth arrays then AO arrays (depth / out unused).
 struct EventBinding { MeaoCtx *ctx; const void *depth; int kind; void *out; void *stream; bool arrays; bool tight; ViewPitch pitch;
-                      int org[4] = {0, 0, 0, 0}; bool exact = false; };
+                      int org[4] = {0, 0, 0, 0}; bool exact = false; std::vector<const void *> batch = {}; };
 std::map<int, EventBinding> g_events;
 
 }  // namespace
@@ -862,6 +870,7 @@ int meao_create(const MeaoDeviceCfg *cfg, MeaoCtx **out)
             for (const KernelUnit *u : kKernelUnits) u->walk(&pe);
             for (const KernelUnit *u : kViewKernelUnits) u->walk(&pe);
             for (const KernelUnit *u : kOrthoKernelUnits) u->walk(&pe);
+            for (const KernelUnit *u : kBatchKernelUnits) u->walk(&pe);
             if (pe != cudaSuccess) { cudaGetLastError(); meao_destroy(c); return fail(nullptr, MEAO_ERR_CUDA, "loading the kernels failed: %s", cudaGetErrorString(pe)); }
             preloaded[dev] = true;
         }
@@ -1739,6 +1748,15 @@ int meao_render_pitched(MeaoCtx *c, const void *depth, int64_t depth_row_pitch, 
 // ---- CUDA arrays (include/meao.h "CUDA arrays") ------------------------------------------------------------------------
 namespace {
 constexpr int kArrayGraphKind = 400;        // GraphKey.kind of an array frame: 400 + depth kind
+// GraphKey.kind of a batch over CUDA arrays / over device buffers (meao_render_arrays_batch / meao_render_batch): + depth kind
+constexpr int kBatchArrayGraphKind = 500, kBatchGraphKind = 600;
+
+// The graph of `k` launches with `array`: an array frame's p[0] / p[1], or an entry of an array batch's list
+bool graph_names_array(const MeaoCtx::GraphKey &k, const void *array)
+{
+    if (k.kind >= kBatchArrayGraphKind && k.kind < kBatchGraphKind) return std::count(k.list.begin(), k.list.end(), (uintptr_t)array) != 0;
+    return k.kind >= kArrayGraphKind && k.kind < kBatchArrayGraphKind && (k.p[0] == array || k.p[1] == array);
+}
 
 // What a cudaArray_t is, checked against the context on the host before anything is launched.  role: "depth" or "ao", the prefix of
 // the fields named in a refusal (<role>_array, <role>_x, <role>_y).  elem_bits / is_float: the one channel the role needs.  exact: the
@@ -1932,17 +1950,19 @@ int meao_release_array(MeaoCtx *c, const void *array)
     {   // a plugin event bound to the array would re-create its surface after the array is freed
         std::lock_guard<std::mutex> g(g_event_mutex);
         for (auto it = g_events.begin(); it != g_events.end();) {
-            if (it->second.ctx == c && it->second.arrays && (it->second.depth == array || it->second.out == array)) it = g_events.erase(it); else ++it;
+            const EventBinding &b = it->second;
+            const bool names = b.arrays && (b.depth == array || b.out == array || std::count(b.batch.begin(), b.batch.end(), array));
+            if (b.ctx == c && names) it = g_events.erase(it); else ++it;
         }
     }
     bool used = c->surfaces.count(array) != 0;
-    for (auto &kv : c->graphs) used |= kv.first.kind >= kArrayGraphKind && (kv.first.p[0] == array || kv.first.p[1] == array);
+    for (auto &kv : c->graphs) used |= graph_names_array(kv.first, array);
     if (!used) return MEAO_OK;
     c->frame_gen++;
     CUDA_TRY(c, cudaSetDevice(c->device));
     CUDA_TRY(c, cudaDeviceSynchronize());       // frames that use the array may be in flight on any stream
     for (auto it = c->graphs.begin(); it != c->graphs.end();) {
-        if (it->first.kind >= kArrayGraphKind && (it->first.p[0] == array || it->first.p[1] == array)) {
+        if (graph_names_array(it->first, array)) {
             cudaGraphExecDestroy(it->second.exec);
             it = c->graphs.erase(it);
         } else ++it;
@@ -1952,6 +1972,184 @@ int meao_release_array(MeaoCtx *c, const void *array)
     auto s = c->surfaces.find(array);
     if (s != c->surfaces.end()) { cudaDestroySurfaceObject(s->second); c->surfaces.erase(s); }
     return MEAO_OK;
+}
+
+// ---- batches (include/meao.h "Batches") ------------------------------------------------------------------------------------
+namespace {
+static_assert(MEAO_MAX_BATCH == kMaxBatch, "include/meao.h states the batch bound");
+
+// a refusal about one entry: the message names its layer first
+int layer_fail(MeaoCtx *c, int rc, int l)
+{
+    c->error = "layer " + std::to_string(l) + ": " + c->error;
+    return rc;
+}
+
+// The checks of a batch before its entries: the count, the depth kind and the forms a batch does not combine with.
+int check_batch(MeaoCtx *c, int count, int kind, bool arrays)
+{
+    if (count < 1 || count > MEAO_MAX_BATCH)
+        return fail(c, MEAO_ERR_INVALID, "count %d: a batch holds 1 .. MEAO_MAX_BATCH (%d) layers", count, MEAO_MAX_BATCH);
+    if (count != c->layers)
+        return fail(c, MEAO_ERR_INVALID, "count %d differs from the context's layer count %d (meao_set_layers)", count, c->layers);
+    if (kind < MEAO_DEPTH_RAW_F32 || kind > MEAO_DEPTH_RAW_D24S8) return fail(c, MEAO_ERR_INVALID, "bad depth kind %d", kind);
+    if (arrays && kind == MEAO_DEPTH_RAW_D24S8) return fail(c, MEAO_ERR_UNSUPPORTED, "depth_kind RAW_D24S8: CUDA arrays have no depth-stencil format");
+    if (!c->views.empty())
+        return fail(c, MEAO_ERR_INVALID, "a layer-viewport table is set (meao_set_layer_viewports): a batch places every layer in resources of "
+                                         "its own; clear the table first");
+    if (c->projection != MEAO_PROJECTION_PERSPECTIVE)
+        return fail(c, MEAO_ERR_UNSUPPORTED, "batches are perspective-only: this context has an orthographic projection (meao_set_projection)");
+    if (c->band0 != 0 || c->band1 != c->H) return fail(c, MEAO_ERR_UNSUPPORTED, "batches need a whole-frame context (no row band)");
+    return 0;
+}
+
+// One array of an array batch: check_array's format and flag tests, a 2-D array or a layered array of depth 1, at least W x H.
+int check_batch_array(MeaoCtx *c, int l, const void *arr, const char *role, bool d16, int *surf_kind)
+{
+    if (!arr) return fail(c, MEAO_ERR_INVALID, "layer %d: %s_arrays[%d] is NULL", l, role, l);
+    const bool depth = role[0] == 'd';
+    cudaExtent e{};
+    int n = 0;
+    const int rc = check_array(c, arr, role, depth ? (d16 ? 16 : 32) : 8, depth && !d16, 0, 0, false, surf_kind, &e, &n);
+    if (rc) return layer_fail(c, rc, l);
+    if (*surf_kind == kSurfCube || n != 1)
+        return fail(c, MEAO_ERR_INVALID, "layer %d: %s_arrays[%d] has %d layers: a batch entry is a 2-D array or a layered array of depth 1",
+                    l, role, l, n);
+    if (e.width < (size_t)c->W || e.height < (size_t)c->H)
+        return fail(c, MEAO_ERR_INVALID, "layer %d: %s_arrays[%d]: extent %zux%zu is smaller than the context's %dx%d", l, role, l, e.width,
+                    e.height, c->W, c->H);
+    return 0;
+}
+
+// Every check of an array batch after check_batch; on success `io` holds each layer's surfaces (made on first use).  capturing: the
+// frame records into a caller's capture, where no surface object can be made.
+int prepare_batch_arrays(MeaoCtx *c, const void *const *depth_arrays, int kind, const void *const *ao_arrays, int count, bool capturing,
+                         BatchIO *io)
+{
+    if (!depth_arrays || !ao_arrays) return fail(c, MEAO_ERR_INVALID, "depth_arrays / ao_arrays is NULL");
+    const bool d16 = kind == MEAO_DEPTH_RAW_D16_UNORM;
+    int rc;
+    for (int l = 0; l < count; l++) {
+        if ((rc = check_batch_array(c, l, depth_arrays[l], "depth", d16, &io->depth.e[l].kind))) return rc;
+        if ((rc = check_batch_array(c, l, ao_arrays[l], "ao", d16, &io->ao.e[l].kind))) return rc;
+    }
+    // no two layers write one AO array: sorted handles, so O(L log L)
+    std::vector<std::pair<const void *, int>> ao(count);
+    for (int l = 0; l < count; l++) ao[l] = {ao_arrays[l], l};
+    std::sort(ao.begin(), ao.end());
+    for (int i = 1; i < count; i++)
+        if (ao[i].first == ao[i - 1].first)
+            return fail(c, MEAO_ERR_INVALID, "layer %d: ao_arrays[%d] is layer %d's AO array too", ao[i].second, ao[i].second, ao[i - 1].second);
+    if (capturing)      // a surface object is made on an array's first frame, which therefore cannot be recorded into a capture
+        for (int l = 0; l < count; l++)
+            if (!c->surfaces.count(depth_arrays[l]) || !c->surfaces.count(ao_arrays[l]))
+                return fail(c, MEAO_ERR_INVALID, "layer %d: cannot record into the stream's capture: an array this context has not rendered with "
+                                                 "needs a surface object first; issue one frame with these arrays outside the capture first", l);
+    for (int l = 0; l < count; l++) {
+        if ((rc = surface_of(c, depth_arrays[l], &io->depth.e[l].surf))) return rc;
+        if ((rc = surface_of(c, ao_arrays[l], &io->ao.e[l].surf))) return rc;
+    }
+    io->arrays = true;
+    return 0;
+}
+
+// Every check of a pointer batch after check_batch: per layer those of meao_render_pitched (pitch bounds and multiples, the depth's
+// alignment to its element); no two AO extents intersect, and no AO extent intersects any depth extent (depth entries may repeat).  An
+// extent runs from a layer's first byte to its last, (H - 1) x row pitch + W x element size.  The AO extents are sorted and then
+// disjoint, so their ends are sorted too: a depth extent meets one exactly when the last AO extent that starts before its end ends after
+// its start.  O(L log L).  On success `io` holds each layer's bases and pitches (rows in elements for the depth).
+int prepare_batch_pointers(MeaoCtx *c, const void *const *depth, const int64_t *depth_row_pitch, int kind, void *const *ao,
+                           const int64_t *ao_row_pitch, int count, BatchIO *io)
+{
+    if (!depth || !depth_row_pitch || !ao || !ao_row_pitch) return fail(c, MEAO_ERR_INVALID, "depth / depth_row_pitch / ao / ao_row_pitch is NULL");
+    const int64_t es = depth_esize(kind), W = c->W, H = c->H;
+    struct Extent { __int128 lo, hi; int l; bool operator<(const Extent &o) const { return lo < o.lo; } };
+    std::vector<Extent> dx(count), ax(count);
+    for (int l = 0; l < count; l++) {
+        if (!depth[l]) return fail(c, MEAO_ERR_INVALID, "layer %d: depth[%d] is NULL", l, l);
+        if (!ao[l]) return fail(c, MEAO_ERR_INVALID, "layer %d: ao[%d] is NULL", l, l);
+        const int64_t dr = depth_row_pitch[l] ? depth_row_pitch[l] : W * es, ar = ao_row_pitch[l] ? ao_row_pitch[l] : W;
+        if (dr < 0 || dr > INT32_MAX || dr < W * es || dr % es)
+            return fail(c, MEAO_ERR_INVALID, "layer %d: depth_row_pitch[%d] = %lld: must be at least width x %lld = %lld bytes, at most INT32_MAX "
+                        "and a multiple of %lld", l, l, (long long)depth_row_pitch[l], (long long)es, (long long)(W * es), (long long)es);
+        if (ar < 0 || ar > INT32_MAX || ar < W)
+            return fail(c, MEAO_ERR_INVALID, "layer %d: ao_row_pitch[%d] = %lld: must be at least the width %lld and at most INT32_MAX", l, l,
+                        (long long)ao_row_pitch[l], (long long)W);
+        if ((uintptr_t)depth[l] % es)
+            return fail(c, MEAO_ERR_INVALID, "layer %d: depth[%d] %p is not aligned to its %lld-byte element", l, l, depth[l], (long long)es);
+        io->ptr.e[l] = BatchPtr{depth[l], (uint8_t *)ao[l], (int)(dr / es), (int)ar};
+        const __int128 d0 = (__int128)(uintptr_t)depth[l], a0 = (__int128)(uintptr_t)ao[l];
+        dx[l] = Extent{d0, d0 + (__int128)(H - 1) * dr + W * es, l};
+        ax[l] = Extent{a0, a0 + (__int128)(H - 1) * ar + W, l};
+    }
+    std::sort(ax.begin(), ax.end());
+    for (int i = 1; i < count; i++)
+        if (ax[i].lo < ax[i - 1].hi)
+            return fail(c, MEAO_ERR_INVALID, "layer %d: the byte extent of ao[%d] intersects layer %d's AO extent", ax[i].l, ax[i].l, ax[i - 1].l);
+    for (const Extent &d : dx) {
+        auto it = std::lower_bound(ax.begin(), ax.end(), Extent{d.hi, 0, 0});     // the first AO extent that starts at or after d's end
+        if (it != ax.begin() && std::prev(it)->hi > d.lo)
+            return fail(c, MEAO_ERR_INVALID, "layer %d: the byte extent of ao[%d] intersects layer %d's depth extent (depth[%d])", std::prev(it)->l,
+                        std::prev(it)->l, d.l, d.l);
+    }
+    io->arrays = false;
+    return 0;
+}
+
+// FNV-1a over a batch's list (GraphKey.list_hash)
+uint64_t list_hash(const std::vector<uintptr_t> &v)
+{
+    uint64_t h = 1469598103934665603ull;
+    for (uintptr_t w : v)
+        for (int b = 0; b < 8; b++) { h ^= (w >> (8 * b)) & 0xffu; h *= 1099511628211ull; }
+    return h;
+}
+
+// A checked batch on a context that frame_ready has prepared: the frame graph of meao_render_arrays / meao_render with its first and last
+// node reading and writing each layer's own resources.  The list is a kernel parameter of those two nodes, so it is baked into the graph
+// (GraphKey.list) and into a caller's capture.
+int render_batch(MeaoCtx *c, const BatchIO &io, int kind, std::vector<uintptr_t> list, void *last_out, cudaStream_t s, bool capturing)
+{
+    NvtxRange nv("meao::frame_batch");
+    MeaoCtx::GraphKey key{{nullptr, nullptr, nullptr, nullptr}, (io.arrays ? kBatchArrayGraphKind : kBatchGraphKind) + kind};
+    key.list_hash = list_hash(list);
+    key.list = std::move(list);
+    c->last_kind = kind; c->last_out = last_out;
+    return launch_cached(c, key, s, capturing, [&](cudaStream_t cs, int pdl) {
+        FrameIO fio = frame_io(c, nullptr, kind, nullptr, !io.arrays);      // pointers: the fused frame (low-only prepare)
+        fio.batch = &io;
+        return record_frame_dag(c, fio, cs, 0, pdl);
+    });
+}
+}  // namespace
+
+int meao_render_arrays_batch(MeaoCtx *c, const void *const *depth_arrays, int32_t kind, void *const *ao_arrays, int32_t count, void *stream)
+{
+    bool capturing;
+    int rc = frame_ready(c, (cudaStream_t)stream, &capturing); if (rc) return rc;
+    if ((rc = check_batch(c, count, kind, true))) return rc;
+    std::unique_ptr<BatchIO> io(new BatchIO);
+    if ((rc = prepare_batch_arrays(c, depth_arrays, kind, ao_arrays, count, capturing, io.get()))) return rc;
+    std::vector<uintptr_t> list(2 * (size_t)count);
+    for (int l = 0; l < count; l++) { list[l] = (uintptr_t)depth_arrays[l]; list[count + l] = (uintptr_t)ao_arrays[l]; }
+    return render_batch(c, *io, kind, std::move(list), ao_arrays[0], (cudaStream_t)stream, capturing);
+}
+
+int meao_render_batch(MeaoCtx *c, const void *const *depth, const int64_t *depth_row_pitch, int32_t kind, void *const *ao,
+                      const int64_t *ao_row_pitch, int32_t count, void *stream)
+{
+    bool capturing;
+    int rc = frame_ready(c, (cudaStream_t)stream, &capturing); if (rc) return rc;
+    if ((rc = check_batch(c, count, kind, false))) return rc;
+    std::unique_ptr<BatchIO> io(new BatchIO);
+    if ((rc = prepare_batch_pointers(c, depth, depth_row_pitch, kind, ao, ao_row_pitch, count, io.get()))) return rc;
+    std::vector<uintptr_t> list(4 * (size_t)count);
+    for (int l = 0; l < count; l++) {
+        const BatchPtr &e = io->ptr.e[l];
+        list[4 * l] = (uintptr_t)e.depth; list[4 * l + 1] = (uintptr_t)e.depth_pitch;
+        list[4 * l + 2] = (uintptr_t)e.ao; list[4 * l + 3] = (uintptr_t)e.ao_pitch;
+    }
+    return render_batch(c, *io, kind, std::move(list), ao[0], (cudaStream_t)stream, capturing);
 }
 
 int meao_render_host_async(MeaoCtx *c, const void *depth_host, int32_t kind, uint8_t *ao_host, int32_t slot)
@@ -2267,6 +2465,27 @@ int meao_bind_event_arrays_at(MeaoCtx *c, int32_t event_id, const void *depth_ar
     return bind_event_arrays(c, event_id, depth_array, depth_x, depth_y, kind, ao_array, ao_x, ao_y, false, stream);
 }
 
+int meao_bind_event_arrays_batch(MeaoCtx *c, int32_t event_id, const void *const *depth_arrays, int32_t kind, void *const *ao_arrays,
+                                 int32_t count, void *stream)
+{
+    if (!c) return MEAO_ERR_INVALID;
+    if (!depth_arrays && !ao_arrays) {
+        std::lock_guard<std::mutex> g(g_event_mutex);
+        g_events.erase(event_id);
+        return MEAO_OK;
+    }
+    // checked now: the plugin event cannot report an error.  The surfaces are made now too, so the event may run inside a capture
+    int rc = ensure_ready(c); if (rc) return rc;
+    if ((rc = check_batch(c, count, kind, true))) return rc;
+    std::unique_ptr<BatchIO> io(new BatchIO);
+    if ((rc = prepare_batch_arrays(c, depth_arrays, kind, ao_arrays, count, false, io.get()))) return rc;
+    std::vector<const void *> list(depth_arrays, depth_arrays + count);
+    list.insert(list.end(), ao_arrays, ao_arrays + count);
+    std::lock_guard<std::mutex> g(g_event_mutex);
+    g_events[event_id] = EventBinding{c, nullptr, kind, nullptr, stream, true, false, ViewPitch{}, {0, 0, 0, 0}, true, std::move(list)};
+    return MEAO_OK;
+}
+
 void meao_render_event(int event_id)
 {
     EventBinding b;
@@ -2276,7 +2495,10 @@ void meao_render_event(int event_id)
         if (it == g_events.end()) return;
         b = it->second;
     }
-    if (b.arrays) render_arrays(b.ctx, b.depth, b.org[0], b.org[1], b.kind, b.out, b.org[2], b.org[3], b.exact, b.stream);
+    if (!b.batch.empty()) {
+        const size_t n = b.batch.size() / 2;
+        meao_render_arrays_batch(b.ctx, b.batch.data(), b.kind, const_cast<void *const *>(b.batch.data() + n), (int32_t)n, b.stream);
+    } else if (b.arrays) render_arrays(b.ctx, b.depth, b.org[0], b.org[1], b.kind, b.out, b.org[2], b.org[3], b.exact, b.stream);
     else if (b.tight) meao_render(b.ctx, b.depth, b.kind, b.out, b.stream);      // meao_render_pitched at the tight pitches of now
     else meao_render_pitched(b.ctx, b.depth, b.pitch.depth_row, b.pitch.depth_layer, b.kind, b.out, b.pitch.ao_row, b.pitch.ao_layer, b.stream);
 }
