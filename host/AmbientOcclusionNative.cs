@@ -71,6 +71,9 @@ namespace MiniEngineAO
         [DllImport(Lib)] public static extern int meao_reserve(IntPtr ctx, int maxWidth, int maxHeight);
         [DllImport(Lib)] public static extern int meao_reservation(IntPtr ctx, out MeaoReservation r);
         [DllImport(Lib)] public static extern int meao_set_layers(IntPtr ctx, int layers);   // layered frames: L views per frame, [L][H][W] buffers
+        // lay the intermediates out once for the most layers; a layer change up to it then allocates and synchronises nothing (0 clears)
+        [DllImport(Lib)] public static extern int meao_reserve_layers(IntPtr ctx, int maxLayers);
+        [DllImport(Lib)] public static extern int meao_layer_reservation(IntPtr ctx);
         // one camera per layer (split-screen viewports, mirrors, batches from several cameras); null with count 0 clears the table
         [DllImport(Lib)] public static extern int meao_set_layer_cameras(IntPtr ctx, [In] MeaoCamera[] cameras, int count);
         [DllImport(Lib)] public static extern int meao_get_layer_cameras(IntPtr ctx, [Out] MeaoCamera[] cameras, int capacity);
@@ -166,6 +169,12 @@ namespace MiniEngineAO
         // (meao_reserve); a size change inside it then costs no allocation, device synchronise, graph teardown or event rebind.
         Vector2Int _maxResolution;
         public Vector2Int MaxResolution { get { return _maxResolution; } set { _maxResolution = value; } }
+        // Dynamic view counts (split-screen players joining and leaving, visible cube faces): the most Layers the component will have
+        // (zero: none).  Reserved once (meao_reserve_layers); a change of Layers up to it then costs no allocation, device synchronise
+        // or graph teardown.
+        int _maxLayers;
+        public int MaxLayers { get { return _maxLayers; } set { _maxLayers = value; } }
+        int _reservedLayers, _contextLayers = 1;               // what meao_reserve_layers / meao_set_layers were last given
         // An engine that records the plugin's frame into a CUDA graph of its own (meao_render on a stream it captures) replays that
         // graph only while this equals the value read right after the capture, and captures again when it changes (include/meao.h).
         public long FrameGeneration { get { return _ctx == IntPtr.Zero ? -1 : MeaoNative.meao_frame_generation(_ctx); } }
@@ -235,8 +244,8 @@ namespace MiniEngineAO
                 single_scale = 0                                                             // BASELINE configs[0] plumbing mode; the component never selects it
             };
             rebuild |= MeaoNative.meao_set_variants(_ctx, ref variants) == 1;
-            var layered = MeaoNative.meao_set_layers(_ctx, _layers);
-            MeaoNative.Check(_ctx, layered);
+            rebuild |= ReserveLayers();                                                      // before meao_set_layers
+            var layered = SetLayers(_layers);
             rebuild |= layered == 1;
             rebuild |= SetLayerCameras() == 1;                                               // after meao_set_layers, which clears the table
             var viewports = _layerViewports == null ? MeaoNative.meao_set_layer_viewports(_ctx, null, 0)
@@ -271,6 +280,27 @@ namespace MiniEngineAO
             }
             MeaoNative.Check(_ctx, MeaoNative.meao_reserve(_ctx, w, h));
             _reservedW = w; _reservedH = h;
+            return true;
+        }
+
+        int SetLayers(int layers)
+        {
+            var rc = MeaoNative.meao_set_layers(_ctx, layers);
+            MeaoNative.Check(_ctx, rc);
+            _contextLayers = layers;
+            return rc;
+        }
+
+        // Hands MaxLayers to meao_reserve_layers; true if the arena was re-allocated.  When the context has more layers than the new
+        // reservation, it first takes Layers (meao_reserve_layers refuses a reservation below the current count).
+        bool ReserveLayers()
+        {
+            var want = _maxLayers > 0 ? _maxLayers : 0;
+            if (want != 0 && _layers > want) throw new InvalidOperationException("Layers " + _layers + " lies above MaxLayers " + want);
+            if (want == _reservedLayers) return false;
+            if (want != 0 && _contextLayers > want) SetLayers(_layers);
+            MeaoNative.Check(_ctx, MeaoNative.meao_reserve_layers(_ctx, want));
+            _reservedLayers = want;
             return true;
         }
 

@@ -43,7 +43,9 @@ extern "C" {
                               *      viewport of shared CUDA arrays: split-screen, side-by-side stereo, cube atlases; additive)
                               *    + MeaoProjection, meao_set_projection / meao_get_projection (orthographic cameras; additive)
                               *    + MEAO_MAX_BATCH, meao_render_arrays_batch / meao_render_batch / meao_bind_event_arrays_batch (each
-                              *      layer with its own depth and AO resources: several cameras, each with its own targets; additive) */
+                              *      layer with its own depth and AO resources: several cameras, each with its own targets; additive)
+                              *    + meao_reserve_layers / meao_layer_reservation (dynamic view counts: a layer change inside the
+                              *      reservation is host bookkeeping; additive) */
 
 typedef struct MeaoCtx MeaoCtx;
 
@@ -150,8 +152,8 @@ int meao_abi_version(void);
  * arguments (cudaGraphExecUpdate) at its next launch.  Under the ordering contract (meao_reserve) frame n sees the constants set
  * before it was issued, and frame n-1, still in flight, keeps its own.  A host may therefore animate the camera and the
  * parameters every frame.
- * STRUCTURAL INPUTS re-plan with a device synchronise and drop the captured graphs: MeaoVariants, meao_set_layers, a resize without
- * a reservation, meao_reserve, row bands, a change of the cameras' reversed_z (it selects kernel instantiations; it is a
+ * STRUCTURAL INPUTS re-plan with a device synchronise and drop the captured graphs: MeaoVariants, meao_set_layers without a layer
+ * reservation, a resize without a reservation, meao_reserve, row bands, a change of the cameras' reversed_z (it selects kernel instantiations; it is a
  * platform property) and meao_set_projection.
  * A refused camera, table or parameter block leaves the context exactly as it was. */
 /* replaces: the property setters AO.cs:22-66 (CheckPropertiesChanged, AO.cs:104-113): returns 1 if a value changed, 0 if not. */
@@ -210,7 +212,8 @@ int meao_resize(MeaoCtx *ctx, int32_t width, int32_t height);
  *     MEAO_ERR_NOMEM leaves the previous reservation and arena in place.
  *   - meao_resize on a reserved context returns 1 when the size changed, as always; a size outside the reservation is refused with
  *     MEAO_ERR_INVALID and changes nothing -- a dynamic-resolution host never gets a silent re-allocation.
- *   - meao_set_layers re-allocates at the reservation x the new layer count.  A change of MeaoVariants or of the cameras' reversed_z
+ *   - meao_set_layers re-allocates at the reservation x the new layer count, unless the count lies inside a layer reservation
+ *     (meao_reserve_layers).  A change of MeaoVariants or of the cameras' reversed_z
  *     re-plans with a device synchronise, as without a reservation, and forgets the other planned sizes; the arena stays.  A change
  *     of a frame constant (MeaoParams, a camera's planes and field of view, the layer-camera table) keeps every planned size: a size
  *     parked with older constants is planned again on the host when it is swapped back in, and its graphs are re-targeted at their
@@ -226,6 +229,31 @@ int meao_resize(MeaoCtx *ctx, int32_t width, int32_t height);
 #define MEAO_SIZE_SLOTS 8
 #define MEAO_MAX_GRAPHS_HELD 72
 int meao_reserve(MeaoCtx *ctx, int32_t max_width, int32_t max_height);
+/* ---- dynamic view counts -----------------------------------------------------------------------------------------------------
+ * meao_reserve_layers lays the intermediates out for max_layers layers (at the size reservation, or without one at the current size),
+ * so that meao_set_layers to any count in 1..max_layers is host bookkeeping: no allocation, free or memset, no stream or device
+ * synchronise, no graph destruction -- for hosts whose view count changes at run time (split-screen players joining and leaving,
+ * mirrors and portals coming into view, the visible faces of a cube map, the short last batch of an epoch).
+ *   - Returns 1 when the reservation changed (the arena is re-allocated once, with a synchronise, like meao_reserve), 0 when the same
+ *     one is set again; 0 clears it (the arena is then re-allocated at the current count).  max_layers must be in 1..65535 and not
+ *     below the current layer count, else MEAO_ERR_INVALID naming the field, and nothing changes; MEAO_ERR_NOMEM leaves the previous
+ *     reservation and arena in place.  Works on plan-only contexts (device < 0): the reservation is recorded, nothing is allocated.
+ *   - MeaoReservation.arena_bytes reports the arena laid out for max_layers; arena_bytes_needed is the current (W, H, L)'s layout.
+ *   - meao_set_layers(L), 1 <= L <= max_layers, still returns 1 when L changed, moves meao_frame_generation and clears the
+ *     layer-camera and layer-viewport tables, but allocates, frees, memsets, synchronises and destroys nothing.  An L above the
+ *     reservation is refused with MEAO_ERR_INVALID and changes nothing: a host never gets a silent re-allocation.
+ *   - Planned (W, H, L) triples share the MEAO_SIZE_SLOTS slots of meao_reserve, least recently used out: a return to a recently used
+ *     one is a plain graph replay; a new one is planned on the host and its camera tables are written in stream order by its first
+ *     frame (which is therefore refused inside a caller's capture, with the "issue one frame outside the capture first" message).
+ *   - Setting a layer-viewport table where there was none, or clearing one, is a frame constant too on such a context: no re-plan, no
+ *     synchronise; the next frame writes the table on its own stream.
+ *   - MeaoVariants, a change of reversed_z and meao_set_projection stay structural: they re-plan with a device synchronise and forget
+ *     the other planned (W, H, L); the arena stays.
+ *   - Row bands and a layer reservation exclude each other (MEAO_ERR_UNSUPPORTED both ways, before anything changes).
+ *   - After a layer change meao_get_buffer and meao_debug_view describe L layers; their contents are unspecified until the first frame
+ *     at that L (a reserved arena holds whatever earlier frames left). */
+int meao_reserve_layers(MeaoCtx *ctx, int32_t max_layers);
+int meao_layer_reservation(const MeaoCtx *ctx);   /* the reserved maximum layer count, 0 = none; MEAO_ERR_INVALID for a NULL context */
 typedef struct {
     int32_t width, height;              /* the reservation; 0 x 0 = none */
     int64_t arena_bytes;                /* bytes of the arena (plan-only contexts: what it would allocate) */
@@ -246,7 +274,7 @@ int meao_reservation(const MeaoCtx *ctx, MeaoReservation *out);
  * (one layered launch is one kernel); meao_algorithmic_bytes scales by L.
  * A plan input like meao_resize: default 1 (every entry point behaves as without layers); returns 1 if the value changed, 0 if
  * not.  A change re-allocates the intermediates, drops the captured graphs, resets the row band to the whole frame and drops the
- * neighbour connections.  layers must be in 1..65535 (the layer is a grid dimension of the layered kernels), else
+ * neighbour connections -- except inside a layer reservation (meao_reserve_layers), where it is host bookkeeping.  layers must be in 1..65535 (the layer is a grid dimension of the layered kernels), else
  * MEAO_ERR_INVALID; MEAO_ERR_NOMEM if the intermediates do not fit (the context keeps its previous layer count).
  * Row bands and layers exclude each other: with layers > 1, meao_set_row_band, the halo calls (meao_halo_*, meao_render_band_*,
  * meao_band_phase_a / _b) and the native exchange (meao_band_export / _connect / _step / _step_host) return MEAO_ERR_UNSUPPORTED.
@@ -280,7 +308,8 @@ int meao_get_layer_cameras(const MeaoCtx *ctx, MeaoCamera *out, int32_t capacity
  * layer count clears the table.
  * A frame constant: changing the entries of a set table returns 1 and the next frame takes the new table without a re-plan, a device
  * synchronise or a graph instantiation; setting the same table again returns 0.  Setting a table where there was none, or clearing
- * one, switches kernels: it returns 1 and re-plans like a structural change.  meao_frame_generation moves with every change.  A frame
+ * one, switches kernels: it returns 1 and re-plans like a structural change (inside a layer reservation, meao_reserve_layers, it is a
+ * frame constant as well).  meao_frame_generation moves with every change.  A frame
  * whose new table is not written yet is refused inside a caller's capture, like new camera tables.  Works on plan-only contexts.
  * Checked at every frame, against the current W x H (a reserved context may change size under a set table).  CUDA arrays: every
  * rectangle fits its array (x + W <= width, y + H <= height) and every slice is below the array's layer count (1 for a 2-D array, n for a layered one,

@@ -76,6 +76,8 @@ SIGNATURES = {
     "meao_resize": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
     "meao_reserve": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
     "meao_reservation": (C.c_int, [C.c_void_p, C.POINTER(MeaoReservation)]),
+    "meao_reserve_layers": (C.c_int, [C.c_void_p, C.c_int32]),
+    "meao_layer_reservation": (C.c_int, [C.c_void_p]),
     "meao_set_layers": (C.c_int, [C.c_void_p, C.c_int32]),
     "meao_set_layer_cameras": (C.c_int, [C.c_void_p, C.POINTER(MeaoCamera), C.c_int32]),
     "meao_get_layer_cameras": (C.c_int, [C.c_void_p, C.POINTER(MeaoCamera), C.c_int32]),

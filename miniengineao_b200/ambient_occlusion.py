@@ -97,6 +97,11 @@ class AmbientOcclusion:
         # change inside it costs no allocation, device synchronise or graph teardown; None = every size change re-allocates
         self.maxResolution: tuple[int, int] | None = None
         self._reserved = (0, 0)             # what meao_reserve was last given (doubled width under single-pass stereo)
+        # dynamic view counts: the most layers the context will have, reserved once (meao_reserve_layers) so that a change of `layers`
+        # up to it costs no allocation, device synchronise or graph teardown; None = every layer change re-allocates
+        self.maxLayers: int | None = None
+        self._reservedLayers = 0            # what meao_reserve_layers was last given
+        self._contextLayers = 1             # what meao_set_layers was last given
         self._band = None                   # (row0, row1) after set_row_band; reset by every re-allocation
         self._drawCountPerFrame = 0         # AO.cs:289: used to detect single-pass stereo
         self._stereo = False                # singlePassStereoEnabled as latched by the last LateUpdate
@@ -166,12 +171,15 @@ class AmbientOcclusion:
         v = N.MeaoVariants(int(stereo), int(self.sampleExhaustively), int(self.highQualityMask), int(self.singleScale))
         rebuild |= self._check(self._lib.meao_set_variants(self._ctx, C.byref(v))) == 1
         width = cam.pixelWidth * (2 if stereo else 1)                                                # AO.cs:338-341, 501-504
-        layered = self._check(self._lib.meao_set_layers(self._ctx, int(self.layers))) == 1           # re-allocates like a resize
+        reallocated = self._apply_layer_reservation()
+        layered = self._set_layers(int(self.layers))
+        reallocated |= layered and not self._reservedLayers     # inside a layer reservation a layer change allocates nothing
+        rebuild |= layered
         rebuild |= self._apply_layer_cameras()
         rebuild |= self._apply_layer_viewports()
         if cam.orthographic:
             rebuild |= self._check(self._lib.meao_set_projection(self._ctx, N.MEAO_PROJECTION_ORTHOGRAPHIC)) == 1
-        reallocated = layered | self._apply_reservation(width, cam.pixelHeight, stereo)
+        reallocated |= self._apply_reservation(width, cam.pixelHeight, stereo)
         resized = self._check(self._lib.meao_resize(self._ctx, width, cam.pixelHeight)) == 1          # CheckBaseDimensions
         reallocated |= resized and self._reserved == (0, 0)       # inside a reservation a resize allocates nothing
         resized |= reallocated
@@ -198,6 +206,26 @@ class AmbientOcclusion:
             self._check(self._lib.meao_resize(self._ctx, width, height))
         self._check(self._lib.meao_reserve(self._ctx, *want))
         self._reserved = want
+        return True
+
+    def _set_layers(self, layers: int) -> bool:
+        changed = self._check(self._lib.meao_set_layers(self._ctx, layers)) == 1
+        self._contextLayers = layers
+        return changed
+
+    def _apply_layer_reservation(self) -> bool:
+        """Hands maxLayers to meao_reserve_layers before the frame's meao_set_layers; True if the arena was re-allocated.  When the
+        context has more layers than the new reservation, it first takes the frame's layer count, so that meao_reserve_layers never
+        sees a reservation below the current count."""
+        want = 0 if self.maxLayers is None else int(self.maxLayers)
+        if want and int(self.layers) > want:
+            raise ValueError(f"layers {int(self.layers)} lies above maxLayers {want}")
+        if want == self._reservedLayers:
+            return False
+        if want and self._contextLayers > want:
+            self._set_layers(int(self.layers))
+        self._check(self._lib.meao_reserve_layers(self._ctx, want))
+        self._reservedLayers = want
         return True
 
     def reservation(self) -> dict:

@@ -6,7 +6,10 @@
 // persistent upsample grids, kSizeSlots per-layer camera table slots, the layer-viewport table, LinearDepth, the AO result, LowDepth / Occlusion / Combined /
 // HighQuality of levels 1..4, and the two host-staging slots.  Every entry starts on a 256-byte boundary; rows start on 128-byte
 // boundaries (pitches below).  Every entry's size is monotone in W and H, so the entries of a W' x H' frame with W' <= W and H' <= H
-// lie inside the arena of W x H, each at an offset no larger than the W x H one (dynamic resolution, meao_reserve).
+// lie inside the arena of W x H, each at an offset no larger than the W x H one (dynamic resolution, meao_reserve).  Every entry is
+// monotone in L as well, and the camera table slots and the layer-viewport table are laid out for table_layers >= L layers: a context
+// with a layer reservation (meao_reserve_layers) passes its maximum, so every (W, H, L) inside it finds the tables at the same offsets
+// and its images inside the arena of (Wmax, Hmax, Lmax).
 #ifndef MEAO_ARENA_LAYOUT_H
 #define MEAO_ARENA_LAYOUT_H
 
@@ -33,7 +36,7 @@ struct ArenaLayout {
 
 inline int layout_align_up(int x, int a) { return (x + a - 1) / a * a; }
 
-inline ArenaLayout arena_layout(int W, int H, int L)
+inline ArenaLayout arena_layout(int W, int H, int L, int table_layers)
 {
     ArenaLayout a{};
     for (int l = 0; l < 7; l++) {
@@ -44,16 +47,16 @@ inline ArenaLayout arena_layout(int W, int H, int L)
     a.lin_pitch = layout_align_up(a.lw[0], 64);
     a.result_pitch = layout_align_up(a.lw[0], 128);
     // every image: L views of the same pitch, back to back ([L][h][pitch], kernels.h "layered frames")
-    const size_t n = (size_t)L;
+    const size_t n = (size_t)L, nt = (size_t)(table_layers > L ? table_layers : L);
     size_t off = 0;
     auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 255) / 256 * 256; return o; };
     take(sizeof(BandFlags));
     a.ctr = take(8 * sizeof(unsigned int));
-    const size_t zb_bytes = (n * sizeof(LayerZ) + 255) / 256 * 256, ren_bytes = 8 * n * sizeof(LayerRender);
+    const size_t zb_bytes = (nt * sizeof(LayerZ) + 255) / 256 * 256, ren_bytes = 8 * nt * sizeof(LayerRender);
     a.table_ren = zb_bytes;
     a.table_stride = zb_bytes + (ren_bytes + 255) / 256 * 256;
     a.table0 = take(kSizeSlots * a.table_stride);
-    a.views = take(n * sizeof(LayerView));
+    a.views = take(nt * sizeof(LayerView));
     a.lin = take(n * a.lin_pitch * a.lh[0] * 2);
     a.result = take(n * a.result_pitch * a.lh[0]);
     for (int k = 1; k <= 4; k++) {
@@ -68,6 +71,8 @@ inline ArenaLayout arena_layout(int W, int H, int L)
     a.bytes = off;
     return a;
 }
+
+inline ArenaLayout arena_layout(int W, int H, int L) { return arena_layout(W, H, L, L); }
 
 }  // namespace meao
 

@@ -47,9 +47,10 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap *, CUtensorMapDataType, cuuint32
                                     const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
                                     CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-// Everything of a context that depends on the frame size: what the recorders read (frame_record.h FrameState) plus the band's
-// neighbours and row ranges and the state of the per-layer camera table slot.  A reserved context (meao_reserve) keeps one of these
-// per recently used size (MeaoCtx::size_slots) and swaps it in on a resize to that size, so a return to a planned size is host bookkeeping only.
+// Everything of a context that depends on the frame size and the layer count: what the recorders read (frame_record.h FrameState)
+// plus the band's neighbours and row ranges and the state of the per-layer camera table slot.  A reserved context (meao_reserve,
+// meao_reserve_layers) keeps one of these per recently used (W, H, L) (MeaoCtx::size_slots) and swaps it in on a resize or a layer
+// change to it, so a return to a planned (W, H, L) is host bookkeeping only.
 struct SizeState : FrameState {
     int prev0 = -1, next1 = -1;             // the neighbour bands' extents (meao_set_row_band)
     Range need_low[5];                      // rows of LowDepth<k> required by this band
@@ -96,10 +97,11 @@ struct MeaoCtx : SizeState {
     // meao_frame_generation: bumped by every change a frame recorded into a caller's graph depends on (include/meao.h)
     int64_t frame_gen = 0;
 
-    // meao_reserve: the arena is laid out for res_w x res_h (0 x 0: for the current size) and every size inside it keeps its plan
-    int res_w = 0, res_h = 0;
+    // meao_reserve: the arena is laid out for res_w x res_h (0 x 0: for the current size) and every size inside it keeps its plan;
+    // meao_reserve_layers: and for res_layers layers (0: the current count), with every layer count up to it keeping its plan too
+    int res_w = 0, res_h = 0, res_layers = 0;
     struct SizeSlot { bool valid = false; uint64_t last_use = 0; SizeState s; };
-    SizeSlot size_slots[kSizeSlots];        // slot i: the parked state of a planned size whose camera tables live in arena slot i
+    SizeSlot size_slots[kSizeSlots];        // slot i: the parked state of a planned (W, H, L) whose camera tables live in arena slot i
     uint64_t size_clock = 0;
     int64_t arena_allocations = 0, graph_instantiations = 0;
 
@@ -134,17 +136,22 @@ struct MeaoCtx : SizeState {
     // cudaArray_t handles, so a pointer equal to a handle value never finds an array frame's graph, nor the reverse).
     // pitch: the byte pitches of a pointer frame's depth and AO views (meao_render_pitched; 0 for the other kinds) -- a frame at the
     // same pointers with other pitches is another graph, never a replay that reads the wrong rows.
-    // size: the frame size and camera table slot the graph was captured at (launch_cached fills it in) -- a reserved context keeps the
-    // graphs of every size it has visited, and a size re-planned into another slot never replays a graph that reads the old slot.
+    // size: the frame size, camera table slot and layer count the graph was captured at (launch_cached fills it in) -- a reserved
+    // context keeps the graphs of every (W, H, L) it has visited, a size re-planned into another slot never replays a graph that reads
+    // the old slot, and a slot re-used by another layer count never replays a graph launched with the other count's grid.
+    // table: the layer-viewport table an array frame reads (nullptr: none; a pointer frame carries it in p[2]), so that on a context
+    // whose table may come and go without a re-plan (meao_reserve_layers) a frame never replays a graph recorded with the other choice.
     // list / list_hash: a batch's whole list (kBatchArrayGraphKind+: the depth arrays, then the AO arrays; kBatchGraphKind+: depth, depth
     // row pitch, AO, AO row pitch per layer), compared by its hash first and in full on a tie, so a graph replays only its own list.
-    struct GraphKey { const void *p[4]; int kind; int64_t pitch[4] = {0, 0, 0, 0}; int size[3] = {0, 0, 0}; uint64_t list_hash = 0;
+    struct GraphKey { const void *p[4]; int kind; int64_t pitch[4] = {0, 0, 0, 0}; int size[4] = {0, 0, 0, 0}; uint64_t list_hash = 0;
         std::vector<uintptr_t> list = {};
+        const void *table = nullptr;
         bool operator<(const GraphKey &o) const {
         for (int i = 0; i < 4; i++) if (p[i] != o.p[i]) return p[i] < o.p[i];
         if (kind != o.kind) return kind < o.kind;
         for (int i = 0; i < 4; i++) if (pitch[i] != o.pitch[i]) return pitch[i] < o.pitch[i];
-        for (int i = 0; i < 3; i++) if (size[i] != o.size[i]) return size[i] < o.size[i];
+        for (int i = 0; i < 4; i++) if (size[i] != o.size[i]) return size[i] < o.size[i];
+        if (table != o.table) return table < o.table;
         if (list_hash != o.list_hash) return list_hash < o.list_hash;
         return list < o.list; } };
     // launches: the kernels its capture recorded; gen: the plan_gen of the constants it launches with
@@ -186,6 +193,9 @@ int refuse_layered(MeaoCtx *c, const char *what)
 // Row bands and reservations exclude each other too: every arena of one frame size must have one layout (DESIGN.md 4).
 int refuse_reserved(MeaoCtx *c, const char *what)
 {
+    if (c->res_w <= 0)
+        return fail(c, MEAO_ERR_UNSUPPORTED, "%s: row bands need an unreserved context (this one reserves %d layers, meao_reserve_layers)", what,
+                    c->res_layers);
     return fail(c, MEAO_ERR_UNSUPPORTED, "%s: row bands need an unreserved context (this one reserves %dx%d, meao_reserve)", what, c->res_w, c->res_h);
 }
 // Row bands and an orthographic projection exclude each other too: the band paths have no orthographic kernels.
@@ -195,7 +205,7 @@ int refuse_ortho_band(MeaoCtx *c, const char *what)
                 "(meao_set_projection)", what);
 }
 #define BAND_GUARD(c, what) do { if ((c) && (c)->layers > 1) return refuse_layered((c), (what)); \
-    if ((c) && (c)->res_w > 0) return refuse_reserved((c), (what)); \
+    if ((c) && ((c)->res_w > 0 || (c)->res_layers > 0)) return refuse_reserved((c), (what)); \
     if ((c) && (c)->projection != MEAO_PROJECTION_PERSPECTIVE) return refuse_ortho_band((c), (what)); } while (0)
 #define CUDA_TRY(c, expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) \
     return fail((c), MEAO_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); } while (0)
@@ -434,14 +444,17 @@ int setup_band(MeaoCtx *c)
 // The size the arena is laid out for: the reservation, or the current size
 inline int arena_w(const MeaoCtx *c) { return c->res_w > 0 ? c->res_w : c->W; }
 inline int arena_h(const MeaoCtx *c) { return c->res_w > 0 ? c->res_h : c->H; }
+// The layer count the arena is laid out for: the layer reservation, or the current count
+inline int arena_layers(const MeaoCtx *c) { return c->res_layers > 0 ? c->res_layers : c->layers; }
 
-// Places the buffers of the current size (c->W x c->H) in the arena, where a fresh context of that size has them, with its camera
-// tables in slot `slot`; encodes the TMA maps and resets the band to the whole frame.  Host work only: no allocation, no CUDA call.
+// Places the buffers of the current size and layer count (c->W x c->H x c->layers) in the arena, where a fresh context of that size has
+// them (with a layer reservation: the tables where one of the reserved count has them), with its camera tables in slot `slot`; encodes
+// the TMA maps and resets the band to the whole frame.  Host work only: no allocation, no CUDA call.
 int place_size(MeaoCtx *c, int slot)
 {
     c->band0 = 0; c->band1 = c->H; c->prev0 = -1; c->next1 = -1;
     c->slot = slot;
-    place_frame(*c, arena_layout(c->W, c->H, c->layers), (char *)c->arena, slot);
+    place_frame(*c, arena_layout(c->W, c->H, c->layers, arena_layers(c)), (char *)c->arena, slot);
     if (!c->arena) return setup_band(c);
     c->tma_ok = c->encode && encode_maps(*c, [c](CUtensorMap &m, const MapSpec &sp) {
         return make_map(c, &m, sp.elem == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT8, sp.elem, sp.base, sp.w, sp.h,
@@ -451,12 +464,12 @@ int place_size(MeaoCtx *c, int slot)
     return setup_band(c);
 }
 
-// A new arena for arena_w x arena_h at the layer count, laid out by arena_layout; the current size (if any) is placed in it and
+// A new arena for arena_w x arena_h x arena_layers, laid out by arena_layout; the current size (if any) is placed in it and
 // re-planned by the next ensure_ready.  keep_old: allocate before freeing the old arena, so that MEAO_ERR_NOMEM leaves the context as
 // it was (meao_reserve); otherwise the old arena goes first, as a resize always did.
 int allocate(MeaoCtx *c, bool keep_old = false)
 {
-    const ArenaLayout a = arena_layout(arena_w(c), arena_h(c), c->layers);
+    const ArenaLayout a = arena_layout(arena_w(c), arena_h(c), arena_layers(c));
     if (!c->plan_only) {
         if (!keep_old) free_buffers(c);
         void *arena = nullptr;
@@ -495,13 +508,14 @@ void refresh_constants(MeaoCtx *c)
     c->table_pending = !c->plan_only;
 }
 
-// Reserved contexts: make w x h the current size without touching the device.  The current size is parked in its slot; a size parked
-// earlier is swapped back in as it was (plan, maps, camera tables); a new size takes a free slot or the least recently used one, and
-// is planned on the host -- its camera tables are written by its first frame, on that frame's stream (write_tables).
+// Reserved contexts: make w x h x layers the current size and layer count without touching the device.  The current one is parked in
+// its slot; a (W, H, L) parked earlier is swapped back in as it was (plan, maps, camera tables); a new one takes a free slot or the
+// least recently used one, and is planned on the host -- its camera tables are written by its first frame, on that frame's stream
+// (write_tables).
 // HAZARD: a parked size keeps the constants it was parked with.  Frame constants may have changed since, so a size swapped back in
 // re-plans its constants here (refresh_constants) before any frame or getter can read them, and its graphs re-target at their first
 // replay; it must never replay with the constants it was parked with.
-int switch_size(MeaoCtx *c, int w, int h)
+int switch_size(MeaoCtx *c, int w, int h, int layers)
 {
     c->frame_gen++;
     SizeState &cur = *c;
@@ -509,7 +523,7 @@ int switch_size(MeaoCtx *c, int w, int h)
     int slot = -1;
     for (int i = 0; i < kSizeSlots; i++) {
         MeaoCtx::SizeSlot &s = c->size_slots[i];
-        if (s.valid && s.s.W == w && s.s.H == h) {
+        if (s.valid && s.s.W == w && s.s.H == h && s.s.layers == layers) {
             cur = s.s;
             s.last_use = ++c->size_clock;
             refresh_constants(c);
@@ -517,7 +531,7 @@ int switch_size(MeaoCtx *c, int w, int h)
         }
         if (slot < 0 || (c->size_slots[slot].valid && (!s.valid || s.last_use < c->size_slots[slot].last_use))) slot = i;
     }
-    c->W = w; c->H = h;
+    c->W = w; c->H = h; c->layers = layers;
     int rc = place_size(c, slot);
     if (rc) return rc;
     if (!c->plan_dirty) {                           // else ensure_ready re-plans (and drops every other slot)
@@ -1034,7 +1048,9 @@ int meao_set_layer_viewports(MeaoCtx *c, const MeaoLayerViewport *views, int32_t
         if (c->views.empty()) return 0;
         c->views.clear();
         c->views_pending = false;
-        c->plan_dirty = true;               // back to the array kernels without a table: a structural change
+        // back to the kernels without a table: a structural change, except under a layer reservation, whose table offset is one for
+        // every (W, H, L) and whose graph keys carry the table a frame reads
+        if (!c->res_layers) c->plan_dirty = true;
         c->frame_gen++;
         return 1;
     }
@@ -1047,7 +1063,7 @@ int meao_set_layer_viewports(MeaoCtx *c, const MeaoLayerViewport *views, int32_t
             if (view_field(views[l], i) < 0)
                 return fail(c, MEAO_ERR_INVALID, "layer %d: %s = %d is negative", l, kViewField[i], view_field(views[l], i));
     if ((int)c->views.size() == count && memcmp(c->views.data(), views, (size_t)count * sizeof(MeaoLayerViewport)) == 0) return 0;
-    if (c->views.empty()) c->plan_dirty = true;     // the table kernels replace the array kernels: a structural change
+    if (c->views.empty() && !c->res_layers) c->plan_dirty = true;   // the table kernels replace the array kernels: a structural change
     else c->views_pending = !c->plan_only;          // a frame constant: written by the next frame on its stream
     c->views.assign(views, views + count);
     for (int i = 0; i < 6; i++) {
@@ -1088,7 +1104,7 @@ int meao_resize(MeaoCtx *c, int32_t w, int32_t h)
         return fail(c, MEAO_ERR_INVALID, "size %dx%d lies outside the reservation %dx%d (meao_reserve)", w, h, c->res_w, c->res_h);
     if (w == c->W && h == c->H && (c->arena || c->plan_only)) return 0;       // RTHandle.CheckBaseDimensions, AO.cs:145-148
     if (c->res_w > 0 && (c->arena || c->plan_only)) {
-        const int rc = switch_size(c, w, h);        // no allocation, no synchronise, the other sizes' graphs stay
+        const int rc = switch_size(c, w, h, c->layers);     // no allocation, no synchronise, the other sizes' graphs stay
         return rc ? rc : 1;
     }
     if (!c->plan_only) {
@@ -1130,7 +1146,7 @@ int meao_reservation(const MeaoCtx *c, MeaoReservation *out)
     if (!c || !out) return MEAO_ERR_INVALID;
     memset(out, 0, sizeof *out);
     out->width = c->res_w; out->height = c->res_h;
-    if (arena_w(c) > 0) out->arena_bytes = c->plan_only ? (int64_t)arena_layout(arena_w(c), arena_h(c), c->layers).bytes : (int64_t)c->arena_bytes;
+    if (arena_w(c) > 0) out->arena_bytes = c->plan_only ? (int64_t)arena_layout(arena_w(c), arena_h(c), arena_layers(c)).bytes : (int64_t)c->arena_bytes;
     if (c->W > 0) out->arena_bytes_needed = (int64_t)arena_layout(c->W, c->H, c->layers).bytes;
     out->arena_allocations = c->arena_allocations;
     out->graphs_held = (int64_t)(c->graphs.size() + c->retired.size());
@@ -1138,12 +1154,34 @@ int meao_reservation(const MeaoCtx *c, MeaoReservation *out)
     return MEAO_OK;
 }
 
+// meao_set_layers inside a layer reservation: host bookkeeping.  The tables are cleared -- the layer cameras as a camera change
+// (note_camera_change), the viewport table as meao_set_layer_viewports clears it -- and the new count is swapped in like a size
+// (switch_size); the arena, the graphs and every other planned (W, H, L) stay.
+static int switch_layers(MeaoCtx *c, int layers)
+{
+    c->frame_gen++;
+    if (!c->layer_cams.empty()) {
+        const int old_z = ctx_reversed_z(c);
+        c->layer_cams.clear();
+        note_camera_change(c, old_z, c->camera.reversed_z);
+    }
+    c->views.clear();
+    c->views_pending = false;
+    c->views_checked.clear();
+    if (c->W <= 0) { c->layers = layers; return 1; }    // placed by the first meao_resize
+    const int rc = switch_size(c, c->W, c->H, layers);
+    return rc ? rc : 1;
+}
+
 int meao_set_layers(MeaoCtx *c, int32_t layers)
 {
     if (!c) return MEAO_ERR_INVALID;
     if (layers < 1 || layers > kMaxLayers)
         return fail(c, MEAO_ERR_INVALID, "layers %d not in 1..%d (the layer is a grid dimension of the layered kernels)", layers, kMaxLayers);
+    if (c->res_layers > 0 && layers > c->res_layers)    // never a silent re-allocation for a host that reserved its layer count
+        return fail(c, MEAO_ERR_INVALID, "layers %d lies above the layer reservation %d (meao_reserve_layers)", layers, c->res_layers);
     if (layers == c->layers) return 0;
+    if (c->res_layers > 0) return switch_layers(c, layers);
     const int old = c->layers;
     c->frame_gen++;
     std::vector<MeaoCamera> old_cams;
@@ -1172,6 +1210,30 @@ int meao_set_layers(MeaoCtx *c, int32_t layers)
     }
     return 1;
 }
+
+int meao_reserve_layers(MeaoCtx *c, int32_t max_layers)
+{
+    if (!c) return MEAO_ERR_INVALID;
+    const bool clear = max_layers == 0;
+    if (!clear && (max_layers < 1 || max_layers > kMaxLayers))
+        return fail(c, MEAO_ERR_INVALID, "bad max_layers %d (in 1..%d, or 0 to clear)", max_layers, kMaxLayers);
+    if (c->W > 0 && (c->band0 != 0 || c->band1 != c->H || c->prev0 >= 0 || c->next1 >= 0))
+        return fail(c, MEAO_ERR_UNSUPPORTED, "meao_reserve_layers: this context has a row band (meao_set_row_band); row bands need an unreserved context");
+    if (!clear && max_layers < c->layers)
+        return fail(c, MEAO_ERR_INVALID, "max_layers %d is below the current layer count %d", max_layers, c->layers);
+    if (max_layers == c->res_layers) return 0;
+    const int old = c->res_layers;
+    c->res_layers = max_layers;
+    if (c->plan_only) { c->frame_gen++; return 1; }     // recorded; nothing to allocate
+    CUDA_TRY(c, cudaSetDevice(c->device));
+    CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+    if (arena_w(c) <= 0) { c->frame_gen++; return 1; }  // no size yet: laid out by the first meao_resize
+    const int rc = allocate(c, true);               // like meao_reserve: the old arena stays until the new one exists
+    if (rc) { c->res_layers = old; return rc; }
+    return 1;
+}
+
+int meao_layer_reservation(const MeaoCtx *c) { return c ? c->res_layers : MEAO_ERR_INVALID; }
 
 int meao_set_row_band(MeaoCtx *c, int32_t row0, int32_t row1, int32_t prev_row0, int32_t next_row1)
 {
@@ -1375,7 +1437,7 @@ static int launch_cached(MeaoCtx *c, const MeaoCtx::GraphKey &key_in, cudaStream
     if (c->flags & MEAO_FLAG_NO_GRAPH) return record(s, 0);
     if (capturing) return record(s, c->pdl_level >= 0 ? c->pdl_level : 0);
     MeaoCtx::GraphKey key = key_in;
-    key.size[0] = c->W; key.size[1] = c->H; key.size[2] = c->slot;
+    key.size[0] = c->W; key.size[1] = c->H; key.size[2] = c->slot; key.size[3] = c->layers;
     auto it = c->graphs.find(key);
     bool retiring = false;
     if (it == c->graphs.end() || it->second.gen != c->plan_gen) {
@@ -1920,7 +1982,8 @@ int render_arrays(MeaoCtx *c, const void *depth_array, int dx, int dy, int kind,
     if ((rc = prepare_arrays(c, depth_array, dx, dy, kind, ao_array, ax, ay, exact, &io))) return rc;
     // the frame graph of meao_render with its first and last node reading / writing the arrays
     NvtxRange nv("meao::frame_arrays");
-    const MeaoCtx::GraphKey key{{depth_array, ao_array, origin_key(dx, dy), origin_key(ax, ay)}, kArrayGraphKind + kind};
+    MeaoCtx::GraphKey key{{depth_array, ao_array, origin_key(dx, dy), origin_key(ax, ay)}, kArrayGraphKind + kind};
+    key.table = c->views.empty() ? nullptr : c->layer_views;
     c->last_kind = kind; c->last_out = ao_array;
     return launch_cached(c, key, (cudaStream_t)stream, capturing, [&](cudaStream_t cs, int pdl) {
         FrameIO fio = frame_io(c, nullptr, kind, nullptr, false);
