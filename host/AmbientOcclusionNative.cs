@@ -116,6 +116,10 @@ namespace MiniEngineAO
         // an orthographic camera 1 / projectionMatrix[0,0] is the view volume's half-width, and LINEAR_F32 depth must be eye depth / far
         [DllImport(Lib)] public static extern int meao_set_projection(IntPtr ctx, int projection);
         [DllImport(Lib)] public static extern int meao_get_projection(IntPtr ctx);
+        // one projection per layer (an editor's quad view, a bird's-eye-view camera beside perspective sensors): count = meao_set_layers,
+        // null with count 0 clears the table, which then decides each layer's projection alone (a structural input)
+        [DllImport(Lib)] public static extern int meao_set_layer_projections(IntPtr ctx, [In] int[] projections, int count);
+        [DllImport(Lib)] public static extern int meao_get_layer_projections(IntPtr ctx, [Out] int[] projections, int capacity);
 
         public static void Check(IntPtr ctx, int rc)
         {
@@ -159,6 +163,10 @@ namespace MiniEngineAO
         // renders with this component's camera.  Each must have this camera's pixel size; Length must equal Layers.
         Camera[] _layerCameras;
         public Camera[] LayerCameras { get { return _layerCameras; } set { _layerCameras = value; } }
+        // Perspective and orthographic layers in one frame: true hands each LayerCameras[i].orthographic to the plugin as that layer's
+        // projection (meao_set_layer_projections) instead of requiring it to match this camera's.
+        bool _perLayerProjection;
+        public bool PerLayerProjection { get { return _perLayerProjection; } set { _perLayerProjection = value; } }
         // Where each layer lives in the depth and AO targets (split-screen players in one texture, a side-by-side stereo pair, cube faces
         // in a 2-D atlas); null: every layer at the origin of its own slice.  Length must equal Layers.  Honoured by the frames of
         // meao_render, meao_render_pitched and meao_render_arrays and the events bound to them; the host-buffer calls, the stage calls,
@@ -248,10 +256,14 @@ namespace MiniEngineAO
             var layered = SetLayers(_layers);
             rebuild |= layered == 1;
             rebuild |= SetLayerCameras() == 1;                                               // after meao_set_layers, which clears the table
+            // an orthographic layer excludes a layer-viewport table: the projection table is cleared before the viewports and set after them
+            var perLayer = _perLayerProjection && _layerCameras != null;
+            if (!perLayer) rebuild |= SetLayerProjections(false) == 1;
             var viewports = _layerViewports == null ? MeaoNative.meao_set_layer_viewports(_ctx, null, 0)
                                                     : MeaoNative.meao_set_layer_viewports(_ctx, _layerViewports, _layerViewports.Length);
             MeaoNative.Check(_ctx, viewports);
             rebuild |= viewports == 1;                                                       // after meao_set_layers too
+            if (perLayer) rebuild |= SetLayerProjections(true) == 1;
             if (_camera.orthographic) rebuild |= SetProjection(1) == 1;
             var width = _camera.pixelWidth * (stereo ? 2 : 1);
             rebuild |= Reserve(width, _camera.pixelHeight, stereo);                          // before meao_resize, doubled like the width
@@ -322,8 +334,8 @@ namespace MiniEngineAO
                 var c = _layerCameras[i];
                 if (c.pixelWidth != _camera.pixelWidth || c.pixelHeight != _camera.pixelHeight)
                     throw new ArgumentException("LayerCameras[" + i + "] has another pixel size than the camera");
-                if (c.orthographic != _camera.orthographic)
-                    throw new ArgumentException("LayerCameras[" + i + "] has another projection than the camera (one per context)");
+                if (!_perLayerProjection && c.orthographic != _camera.orthographic)
+                    throw new ArgumentException("LayerCameras[" + i + "] has another projection than the camera (set PerLayerProjection to mix them)");
                 cams[i] = new MeaoNative.MeaoCamera
                 {
                     near_clip = c.nearClipPlane, far_clip = c.farClipPlane,
@@ -332,6 +344,22 @@ namespace MiniEngineAO
                 };
             }
             var rc = MeaoNative.meao_set_layer_cameras(_ctx, cams, cams.Length);
+            MeaoNative.Check(_ctx, rc);
+            return rc;
+        }
+
+        // Hands the projections of LayerCameras to the plugin (set), or clears the table (!set); returns 1 if it changed (a re-plan), 0 if
+        // not, so this runs every frame.
+        int SetLayerProjections(bool set)
+        {
+            int rc;
+            if (!set) rc = MeaoNative.meao_set_layer_projections(_ctx, null, 0);
+            else
+            {
+                var projections = new int[_layerCameras.Length];
+                for (int i = 0; i < projections.Length; i++) projections[i] = _layerCameras[i].orthographic ? 1 : 0;
+                rc = MeaoNative.meao_set_layer_projections(_ctx, projections, projections.Length);
+            }
             MeaoNative.Check(_ctx, rc);
             return rc;
         }

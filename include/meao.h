@@ -45,7 +45,9 @@ extern "C" {
                               *    + MEAO_MAX_BATCH, meao_render_arrays_batch / meao_render_batch / meao_bind_event_arrays_batch (each
                               *      layer with its own depth and AO resources: several cameras, each with its own targets; additive)
                               *    + meao_reserve_layers / meao_layer_reservation (dynamic view counts: a layer change inside the
-                              *      reservation is host bookkeeping; additive) */
+                              *      reservation is host bookkeeping; additive)
+                              *    + meao_set_layer_projections / meao_get_layer_projections (perspective and orthographic layers in one
+                              *      layered frame; additive) */
 
 typedef struct MeaoCtx MeaoCtx;
 
@@ -168,7 +170,8 @@ int meao_get_variants(const MeaoCtx *ctx, MeaoVariants *out);
 int meao_set_camera(MeaoCtx *ctx, const MeaoCamera *camera);
 
 /* ---- projection ----------------------------------------------------------------------------------
- * The projection model of the context's cameras, one for all layers (a batch that mixes projections needs two contexts).
+ * The projection model of the context's cameras, one for all layers; a layered frame whose layers differ sets a projection per layer
+ * with meao_set_layer_projections below.
  * PERSPECTIVE (the default) is what the reference does.  ORTHOGRAPHIC (isometric and top-down views, CAD viewers, editor views):
  *   - raw depth is affine in eye depth: with r = near_clip / far_clip, lin = fma(1 - r, d, r), reversed Z lin = fma(r - 1, d, 1) -- eye
  *     depth / far_clip, LinearDepth's convention; d == 1 (reversed: d == 0) is sky, 1e5, as for perspective.  meao_zbuffer_params
@@ -193,6 +196,37 @@ typedef enum {
 } MeaoProjection;
 int meao_set_projection(MeaoCtx *ctx, int32_t projection);
 int meao_get_projection(const MeaoCtx *ctx);     /* MeaoProjection, or MEAO_ERR_INVALID for a NULL context */
+/* ---- per-layer projections ------------------------------------------------------------------------
+ * One MeaoProjection per layer of a layered frame (meao_set_layers): an editor's perspective pane beside its top, front and side
+ * orthographic panes, a bird's-eye-view camera beside perspective sensor cameras, an isometric view beside a perspective one -- in one
+ * frame, one set of intermediates and one graph instead of a context per projection.
+ *   - count must equal the layer count; projections == NULL with count == 0 clears the table.  Every entry must be
+ *     MEAO_PROJECTION_PERSPECTIVE or MEAO_PROJECTION_ORTHOGRAPHIC.  A refusal returns MEAO_ERR_INVALID, names the layer and the field in
+ *     meao_last_error and changes nothing.
+ *   - While a table is set it alone decides each layer's projection.  meao_set_projection still records the context's projection, which
+ *     takes effect again when the table is cleared (as meao_set_camera relates to meao_set_layer_cameras).  A change of the layer count
+ *     clears the table, as it clears the layer-camera and layer-viewport tables.
+ *   - A layer's projection decides how its camera (the table's or the context's) is read, exactly as meao_set_projection describes for a
+ *     whole context: under ORTHOGRAPHIC tan_half_fov_h is the view volume's half-width and MEAO_DEPTH_LINEAR_F32 input is eye depth /
+ *     far_clip.  meao_zbuffer_params_layer and meao_render_constants_layer return each layer's constants for its own projection, and the
+ *     layer's atlas padding follows it.  Every layer of a frame equals a single-layer frame of its depth with that projection and camera.
+ *   - A set returns 1 if the table changed, 0 if not.  A change is a structural input like meao_set_projection: it re-plans with a device
+ *     synchronise, drops the captured graphs and moves meao_frame_generation.  Inside a layer reservation (meao_reserve_layers) the clearing
+ *     done by meao_set_layers stays host bookkeeping like the other tables': no synchronise, allocation or graph destruction.  Setting
+ *     the table again for the new count is a change, hence structural: a host that changes the layer count of a frame that keeps mixing
+ *     projections pays one re-plan with a device synchronise per count change, even inside the reservation.
+ *   - A table with an ORTHOGRAPHIC entry carries the restrictions of an orthographic context, each refused with MEAO_ERR_UNSUPPORTED
+ *     before anything changes, in either order: a layer-viewport table, batches (meao_render_arrays_batch, meao_render_batch and their
+ *     event) and row bands.  The context-level refusals of meao_set_projection stay as they are.
+ *   - Every other frame form of a layered context takes the table: pointers, pitched views, host buffers, CUDA arrays and their _at
+ *     viewports, the bound events, MEAO_FLAG_NO_GRAPH, recording into a caller's capture, reservations, per-layer cameras, every
+ *     MeaoVariants and both Z directions.  Plan-only contexts accept the table.
+ *   - A table whose layers are all alike records the frame of a context with that projection; one that mixes both runs layered kernels
+ *     that pick each layer's projection per CTA (DESIGN.md 2.17).
+ * The getter follows meao_get_layer_cameras: it returns the entry count (0: no table), or MEAO_ERR_INVALID if the table does not fit in
+ * capacity. */
+int meao_set_layer_projections(MeaoCtx *ctx, const int32_t *projections, int32_t count);
+int meao_get_layer_projections(const MeaoCtx *ctx, int32_t *out, int32_t capacity);
 /* replaces: RTHandle.SetBaseDimensions + AllocateNow + the rebuild it triggers (AO.cs:338-341, 501-506).
  * Allocates the intermediates for width x height.  Returns 1 if dimensions changed, 0 if not.
  * A size change RESETS the row band to the whole frame and drops the neighbour connections (meao_set_row_band,

@@ -88,6 +88,10 @@ class AmbientOcclusion:
         # one Camera per layer (meao_set_layer_cameras): split-screen viewports, mirrors, batches from several cameras; None = every
         # layer uses `camera`.  Each entry must match the main camera's pixelWidth, pixelHeight, usesReversedZBuffer and orthographic.
         self.layerCameras: list[Camera] | None = None
+        # perspective and orthographic layers in one frame (meao_set_layer_projections): True hands each layerCameras[i].orthographic to
+        # the context as that layer's projection -- an editor's quad view, a bird's-eye-view camera beside perspective sensor cameras --
+        # instead of requiring it to match the main camera's
+        self.perLayerProjection = False
         # where each layer lives in the caller's depth and AO (meao_set_layer_viewports): one (depth_x, depth_y, depth_slice, ao_x,
         # ao_y, ao_slice) per layer -- split-screen players in one texture, a side-by-side stereo pair, cube faces in a 2-D atlas.  Honoured
         # by render (and its plugin event), the pitched frames and render_arrays (not with origins); render_host, the stage calls, the
@@ -176,7 +180,15 @@ class AmbientOcclusion:
         reallocated |= layered and not self._reservedLayers     # inside a layer reservation a layer change allocates nothing
         rebuild |= layered
         rebuild |= self._apply_layer_cameras()
+        # an orthographic layer excludes a layer-viewport table: the projection table is cleared before the viewports are applied and set
+        # after them
+        projections = self._layer_projections()
+        if projections is None:
+            rebuild |= self._check(self._lib.meao_set_layer_projections(self._ctx, None, 0)) == 1
         rebuild |= self._apply_layer_viewports()
+        if projections is not None:
+            arr = (C.c_int32 * len(projections))(*projections)
+            rebuild |= self._check(self._lib.meao_set_layer_projections(self._ctx, arr, len(projections))) == 1
         if cam.orthographic:
             rebuild |= self._check(self._lib.meao_set_projection(self._ctx, N.MEAO_PROJECTION_ORTHOGRAPHIC)) == 1
         reallocated |= self._apply_reservation(width, cam.pixelHeight, stereo)
@@ -242,7 +254,7 @@ class AmbientOcclusion:
             return self._check(self._lib.meao_set_layer_cameras(self._ctx, None, 0)) == 1
         main = self._camera
         for i, c in enumerate(cams):
-            for f in ("pixelWidth", "pixelHeight", "usesReversedZBuffer", "orthographic"):
+            for f in ("pixelWidth", "pixelHeight", "usesReversedZBuffer") + (() if self.perLayerProjection else ("orthographic",)):
                 if getattr(c, f) != getattr(main, f):
                     raise ValueError(f"layerCameras[{i}].{f} = {getattr(c, f)!r} differs from the camera's {getattr(main, f)!r}")
         if len(cams) != int(self.layers):
@@ -250,6 +262,12 @@ class AmbientOcclusion:
         arr = (N.MeaoCamera * len(cams))(*[N.MeaoCamera(c.nearClipPlane, c.farClipPlane, 1.0 / c.projection00, int(c.usesReversedZBuffer))
                                            for c in cams])
         return self._check(self._lib.meao_set_layer_cameras(self._ctx, arr, len(cams))) == 1
+
+    def _layer_projections(self) -> list[int] | None:
+        """The projection table perLayerProjection asks for (one MeaoProjection per layerCameras entry), or None for none."""
+        if not self.perLayerProjection or self.layerCameras is None:
+            return None
+        return [N.MEAO_PROJECTION_ORTHOGRAPHIC if c.orthographic else N.MEAO_PROJECTION_PERSPECTIVE for c in self.layerCameras]
 
     def _apply_layer_viewports(self) -> bool:
         """Hands layerViewports to meao_set_layer_viewports (after meao_set_layers, which clears the table); True if a value changed."""

@@ -26,7 +26,11 @@ ORTHO_SOURCES = ["prepare_depth_ortho.cu", "prepare_depth_ortho_layered.cu", "pr
 # The batch kernels (meao_render_arrays_batch / meao_render_batch: each layer with its own depth and AO): compiled into libmeao.so with
 # SOURCES; the CPU emulator builds them into a library of their own (tests/emu/batch.py), and tests/test_batch_units.py audits them.
 BATCH_SOURCES = ["prepare_depth_array_batch.cu", "blur_upsample_array_batch.cu", "prepare_depth_batch.cu", "blur_upsample_lin_batch.cu"]
-HEADERS = ["common.cuh", "kernels.h", "prepare_depth_kernel.inc", "render_ao_kernel.inc", "blur_upsample_device.inc", "blur_upsample_kernel.inc",
+# The per-layer projection kernels (meao_set_layer_projections: a layered frame whose layers mix both projections): compiled into
+# libmeao.so with SOURCES, each a textual include of an existing kernel body under MEAO_ORTHO 2, so the other kernels keep their code; the
+# CPU emulator builds them into a library of their own (tests/emu/mixed.py), and tests/test_layer_projections_units.py audits them.
+MIXED_SOURCES = ["prepare_depth_mixed_layered.cu", "prepare_depth_array_mixed.cu", "render_ao_mixed_layered.cu", "blur_upsample_lin_mixed.cu"]
+HEADERS = ["common.cuh", "kernels.h", "prepare_depth_kernel.inc", "render_ao_kernel.inc", "render_ao_groups.inc", "render_ao_sample.inc", "blur_upsample_device.inc", "blur_upsample_kernel.inc",
            "blur_upsample_layer_args.inc", "blur_upsample_lin_device.inc", "surface_io.cuh", "depth_in.cuh", "arena_layout.h", "frame_record.h",
            os.path.join("..", "..", "include", "meao.h")]
 
@@ -52,7 +56,7 @@ def is_stale() -> bool:
     if not os.path.exists(LIB):
         return True
     t = os.path.getmtime(LIB)
-    deps = [os.path.join(CSRC, f) for f in SOURCES + VIEW_SOURCES + ORTHO_SOURCES + BATCH_SOURCES + HEADERS] + [os.path.abspath(__file__)]
+    deps = [os.path.join(CSRC, f) for f in SOURCES + VIEW_SOURCES + ORTHO_SOURCES + BATCH_SOURCES + MIXED_SOURCES + HEADERS] + [os.path.abspath(__file__)]
     return any(os.path.getmtime(d) > t for d in deps)
 
 
@@ -60,7 +64,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     if not force and not is_stale():
         return LIB
     extra = os.environ.get("MEAO_NVCC_DEFS", "").split()      # tuning experiments, e.g. "-DMEAO_REN_MINB=12"
-    cmd = [_nvcc()] + NVCC_FLAGS + extra + ["-o", LIB] + [os.path.join(CSRC, f) for f in SOURCES + VIEW_SOURCES + ORTHO_SOURCES + BATCH_SOURCES]
+    cmd = [_nvcc()] + NVCC_FLAGS + extra + ["-o", LIB] + [os.path.join(CSRC, f) for f in SOURCES + VIEW_SOURCES + ORTHO_SOURCES + BATCH_SOURCES + MIXED_SOURCES]
     proc = subprocess.run(cmd, capture_output=True, text=True)
     if verbose or proc.returncode != 0:
         sys.stderr.write(proc.stdout + proc.stderr)

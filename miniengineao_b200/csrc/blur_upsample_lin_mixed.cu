@@ -1,0 +1,69 @@
+// blur_upsample_lin_mixed.cu -- blur_upsample_lin_ortho.cu's layered kernels (the fused final upsample that linearises the caller's raw
+// depth) for a frame whose layers mix both projections (meao_set_layer_projections): the same bodies with MEAO_ORTHO 2, so each tile
+// reads its layer's bit of the LayerProjections parameter once and linearises with depth_in.cuh's perspective or affine linearize8.  The
+// upsample itself works on the stored linear depth and does not depend on the projection; linear ingest stays with blur_upsample_lin.cu's
+// kernels.  A mixed frame has two layers or more, so only the layered forms exist.  A translation unit of its own (build.py MIXED_SOURCES).
+#include <cstdlib>
+
+#include "common.cuh"
+#include "kernels.h"
+
+namespace meao {
+
+namespace {
+
+#define MEAO_ORTHO 2
+#include "blur_upsample_device.inc"
+#include "blur_upsample_layer_args.inc"
+#include "depth_in.cuh"
+
+#include "blur_upsample_lin_device.inc"
+
+#define MEAO_UPS_LIN 1
+#define MEAO_UPS_LAYERED 1
+#define MEAO_UPS_PREMIN 0
+#include "blur_upsample_kernel.inc"
+#undef MEAO_UPS_PREMIN
+#define MEAO_UPS_PREMIN 1
+#include "blur_upsample_kernel.inc"
+#undef MEAO_UPS_PREMIN
+#undef MEAO_UPS_LAYERED
+#undef MEAO_UPS_LIN
+#undef MEAO_ORTHO
+
+const struct {      // [depth_format_slot]
+    Kernel<CUtensorMap, CUtensorMap, UpsampleArgs, int, int, DepthIn, LayerProjections> plain[kDepthFormatSlots];
+    Kernel<CUtensorMap, CUtensorMap, CUtensorMap, UpsamplePreminArgs, int, int, DepthIn, LayerProjections> premin[kDepthFormatSlots];
+} kKernels = {MEAO_LIN_SLOTS(blur_upsample_lin_mixed_kernel), MEAO_LIN_SLOTS(blur_upsample_premin_lin_mixed_kernel)};
+
+}  // namespace
+
+cudaError_t launch_blur_upsample_lin_mixed(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
+                                           const UpsampleArgs &a_in, const uint8_t *lo_ao2, int lo_a2pitch, const DepthIn &din_in, int layers,
+                                           int sm_count, const LayerProjections &proj, cudaStream_t s)
+{
+    if (!din_in.raw)
+        return launch_blur_upsample_lin(lo_depth_map, lo_ao_map, lo_ao2_map, use_tma, a_in, lo_ao2, lo_a2pitch, din_in, layers, sm_count, s);
+    if (a_in.row1 <= a_in.row0) return cudaSuccess;
+    if (layers < 2 || layers > kMaxLayers || !din_in.layer_zb) return cudaErrorInvalidValue;
+    if (!a_in.hi_is_half || a_in.hi_ao || (lo_ao2 && !lo_ao2_map)) return cudaErrorInvalidValue;      // the final level only
+    UpsampleArgs a = a_in;
+    dim3 grid;
+    if (!ups_tile_grid(a, layers, sm_count, &grid)) return cudaErrorInvalidValue;
+    const int t = use_tma ? 1 : 0;
+    DepthIn din = din_in;           // zero pitches: the tight values
+    if (!din.depth_pitch) din.depth_pitch = a.hiw;
+    if (!din.depth_layer_pitch) din.depth_layer_pitch = (long long)din.depth_pitch * a.hih;
+    if (!din.ao_layer_pitch) din.ao_layer_pitch = (long long)a.hih * a.out_pitch;
+    const int k = depth_format_slot(din.in_format);
+    const UpsamplePreminArgs pa{a, lo_ao2, lo_a2pitch};
+    if (!lo_ao2) MEAO_LAUNCH((kKernels.plain[k]), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, a, t, layers, din, proj);
+    else         MEAO_LAUNCH((kKernels.premin[k]), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, *lo_ao2_map, pa, t, layers, din, proj);
+    return cudaGetLastError();
+}
+
+const KernelUnit kBlurUpsampleLinMixedUnit = {"blur_upsample_lin_mixed.cu", [](cudaError_t *load) {
+    return walk_kernels(load, kKernels.plain, kKernels.premin);
+}};
+
+}  // namespace meao

@@ -2,7 +2,13 @@
 // stages that read it: prepare_depth (prepare_depth_kernel.inc) and the final upsample of a whole frame (blur_upsample_lin.cu),
 // which linearises its own pixels and writes LinearDepth itself.  Included inside an anonymous namespace.
 
-#if !MEAO_ORTHO
+#if MEAO_ORTHO == 2
+// MEAO_ORTHO 2 (the *_mixed kernels, meao_set_layer_projections): both linearisations below, under the names of their projection; the
+// linearize8 at the end picks one per call from a CTA-uniform flag
+#define linearize linearize_persp
+#define linearize8 linearize8_persp
+#endif
+#if MEAO_ORTHO != 1
 template <bool RAW, bool REVERSED>
 __device__ __forceinline__ float linearize(float depth, float zbx, float zby)
 {
@@ -49,7 +55,14 @@ __device__ __forceinline__ void linearize8(const float (&v)[8], float zbx, float
         for (int e = 0; e < 8; e++) d[e] = linearize<RAW, REVERSED>(v[e], zbx, zby);
     }
 }
-#else
+#endif
+#if MEAO_ORTHO == 2
+#undef linearize8
+#undef linearize
+#define linearize linearize_ortho
+#define linearize8 linearize8_ortho
+#endif
+#if MEAO_ORTHO
 // An orthographic projection (MEAO_ORTHO: the *_ortho kernels, meao_set_projection) stores depth that is affine in eye depth, so the
 // linear depth is one fused multiply-add: zb = {1 - n/f, n/f} (reversed: {n/f - 1, 1}) gives eye depth / far, LinearDepth's
 // convention.  The sky rule of DS1:41-44 is the perspective one.  No reciprocal, so no range test.
@@ -82,6 +95,18 @@ __device__ __forceinline__ void linearize8(const float (&v)[8], float zbx, float
         if (REVERSED) { if (v[e] == 0.0f) d[e] = 1e5f; }
         else          { if (v[e] == 1.0f) d[e] = 1e5f; }
     }
+}
+#endif
+#if MEAO_ORTHO == 2
+#undef linearize8
+#undef linearize
+// A layer's linearisation by its projection: `ortho` is uniform across the CTA (one layer's, read once), so each call runs one of the
+// two loops above as its twin kernel does
+template <bool RAW, bool REVERSED>
+__device__ __forceinline__ void linearize8(const float (&v)[8], float zbx, float zby, float (&d)[8], bool ortho)
+{
+    if (ortho) linearize8_ortho<RAW, REVERSED>(v, zbx, zby, d);
+    else linearize8_persp<RAW, REVERSED>(v, zbx, zby, d);
 }
 #endif
 

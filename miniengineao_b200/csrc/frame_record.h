@@ -35,7 +35,7 @@ struct Plan {
     // the plan inputs the recorders read besides the constants: the variants and the cameras' Z direction
     MeaoVariants variants;
     int reversed_z;
-    int orthographic;                       // MEAO_PROJECTION_ORTHOGRAPHIC: launch_entry_ortho's kernels
+    int orthographic;                       // every layer MEAO_PROJECTION_ORTHOGRAPHIC: launch_entry_ortho's kernels
 };
 
 // The camera-dependent part of the plan, for one camera: ZBufferParams, both inv_thickness tables of every level and the atlas
@@ -84,7 +84,31 @@ struct FrameState {
 
     Plan plan;
     std::vector<CamConsts> layer_consts;    // the plan's camera constants of every layer (all alike without a layer-camera table)
+    // the layers' projections when they mix both (meao_set_layer_projections): bit l of word l / 32 set = layer l orthographic, the
+    // kernels.h LayerProjections table of launch_entry_mixed; empty when every layer has the same projection (Plan.orthographic).
+    // proj_key: 0 for an all-perspective frame, else a hash of the layers' projections (the graph cache keeps frames of other kernels apart)
+    std::vector<uint32_t> layer_ortho;
+    uint64_t proj_key = 0;
 };
+
+// The layers' projections of a plan: Plan.orthographic, FrameState::layer_ortho and proj_key from ortho(l), layer l orthographic
+template <class F> inline void plan_projections(FrameState &f, F &&ortho)
+{
+    const int L = f.layers;
+    std::vector<uint32_t> bits((size_t)(L + 31) / 32, 0u);
+    int n = 0;
+    for (int l = 0; l < L; l++)
+        if (ortho(l)) { bits[l >> 5] |= 1u << (l & 31); n++; }
+    f.plan.orthographic = n == L;
+    f.proj_key = 0;
+    if (n) {
+        uint64_t h = 1469598103934665603ull;                // FNV-1a over the words
+        for (uint32_t w : bits) { h ^= w; h *= 1099511628211ull; }
+        f.proj_key = h | 1;
+    }
+    if (n > 0 && n < L) f.layer_ortho.swap(bits);
+    else f.layer_ortho.clear();
+}
 
 inline float host_f16_round(float x) { return __half2float(__float2half_rn(x)); }
 
@@ -522,6 +546,33 @@ inline cudaError_t launch_entry_ortho(const FrameState &f, const FrameLaunch &l,
                                               f.sm_count, s);
     }
     return launch_entry(f, l, io, force_tile, s);
+}
+
+// launch_entry for a layered frame whose layers mix both projections (FrameState::layer_ortho): the launches whose arithmetic depends on
+// the projection -- the prepare of raw depth, every render and the fused final upsample of raw depth -- are the mixed kernels (kernels.h),
+// which take the layers' projections as a parameter; every other launch is launch_entry's.  No layer-viewport table, batch or row band
+// goes with an orthographic layer (meao_set_layer_projections).  Apart from launch_entry so that a recorder that never sets a projection
+// table does not link the mixed kernels.
+inline cudaError_t launch_entry_mixed(const FrameState &f, const FrameLaunch &l, const FrameIO &io, int force_tile, cudaStream_t s)
+{
+    if (f.layer_ortho.empty() || f.layers < 2 || io.views || io.batch) return cudaErrorInvalidValue;
+    const bool render = l.stage == kStageRender || l.stage == kStageRenderWide;
+    if (!render && l.stage != kStagePrepare && !(l.level == 1 && io.fused)) return launch_entry(f, l, io, force_tile, s);
+    LayerProjections proj{};
+    for (size_t i = 0; i < f.layer_ortho.size(); i++) proj.ortho[i] = f.layer_ortho[i];
+    if (l.stage == kStagePrepare) {
+        const PrepareArgs a = prepare_args(f, io.depth);
+        if (io.aio)
+            return launch_prepare_depth_array_mixed(a, io.aio->depth, io.aio->depth_surf, io.aio->depth_x, io.aio->depth_y, f.layers, s, f.layer_zb, proj);
+        return launch_prepare_depth_mixed_layered(a, f.layers, s, io.low_only, f.layer_zb, proj);
+    }
+    if (render) {
+        const RenderArgs a = render_args(f, l.level, io.kind, l.stage == kStageRenderWide, force_tile);
+        return launch_render_ao_mixed_layered(render_map(f, a, l.level), f.tma_ok, a, f.layers, s, render_layer_cams(f, a, l.level),
+                                              io.kind != MEAO_DEPTH_LINEAR_F32 ? 1 : 0, proj);
+    }
+    return launch_blur_upsample_lin_mixed(f.maps.low_ups[1], upsample_ao_map(f, 1), &f.maps.hq_ups[1], f.tma_ok, upsample_args(f, 1, io.ao, io.vp),
+                                          upsample_lo_ao2(f, 1), f.occ_pitch[1], io.depth, f.layers, f.sm_count, proj, s);
 }
 
 // ---- the debug buffers (meao_get_buffer, meao_set_buffer, meao_debug_view) ---------------------------------------------------

@@ -319,6 +319,27 @@ cudaError_t launch_blur_upsample_lin_ortho(const CUtensorMap &lo_depth_map, cons
                                            const UpsampleArgs &a, const uint8_t *lo_ao2, int lo_a2pitch, const DepthIn &din, int layers,
                                            int sm_count, cudaStream_t s);
 
+// ---- per-layer projections (meao_set_layer_projections): a layered frame whose layers mix both projections ---------------------------
+// The same three launches in a form that reads each layer's projection from bit l of a table passed BY VALUE as a __grid_constant__
+// kernel parameter, once per CTA (prepare and render: layer blockIdx.z; the fused upsample: its tile's layer), and runs the perspective or
+// the orthographic body of its twin (*_ortho*.cu) under that CTA-uniform branch.  The table is a structural input, so the context's
+// graphs carry it baked in; the arena (LayerZ / LayerRender, whose entries are computed with each layer's projection) keeps its layout.
+// 8 KB: one bit for each of kMaxLayers layers.  Only frames with at least one layer of each projection launch these (frame_record.h
+// launch_entry_mixed).  Separate kernels and translation units (*_mixed*.cu, build.py MIXED_SOURCES), so the existing kernels keep their
+// code.  Layered frames only (layers >= 1, layer_zb and layer_cam set); linear ingest goes to the perspective launchers.
+struct LayerProjections { uint32_t ortho[(kMaxLayers + 31) / 32]; };
+static_assert(sizeof(LayerProjections) == 8192, "the projection table's parameter size");
+__host__ __device__ inline bool layer_is_ortho(const LayerProjections &p, int l) { return ((p.ortho[l >> 5] >> (l & 31)) & 1u) != 0; }
+cudaError_t launch_prepare_depth_mixed_layered(const PrepareArgs &a, int layers, cudaStream_t s, bool low_only, const struct LayerZ *layer_zb,
+                                               const LayerProjections &proj);
+cudaError_t launch_prepare_depth_array_mixed(const PrepareArgs &a, cudaSurfaceObject_t depth, int surf_kind, int depth_x, int depth_y, int layers,
+                                             cudaStream_t s, const struct LayerZ *layer_zb, const LayerProjections &proj);
+cudaError_t launch_render_ao_mixed_layered(const CUtensorMap &low_map, bool use_tma, const RenderArgs &a, int layers, cudaStream_t s,
+                                           const struct LayerRender *layer_cam, int layer_pad, const LayerProjections &proj);
+cudaError_t launch_blur_upsample_lin_mixed(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
+                                           const UpsampleArgs &a, const uint8_t *lo_ao2, int lo_a2pitch, const DepthIn &din, int layers,
+                                           int sm_count, const LayerProjections &proj, cudaStream_t s);
+
 // ---- debug: synthesise a TiledDepth<k> view (reference layout [16][sh][sw], f16 bits) ----------
 cudaError_t launch_synth_tiled(const float *low, int lw, int lh, int lpitch, int sw, int sh, float pad,
                                __half *out, cudaStream_t s);
@@ -431,6 +452,13 @@ extern const KernelUnit kPrepareDepthArrayBatchUnit, kBlurUpsampleArrayBatchUnit
 #ifndef MEAO_EMULATE
 inline const KernelUnit *const kBatchKernelUnits[] = {&kPrepareDepthArrayBatchUnit, &kBlurUpsampleArrayBatchUnit, &kPrepareDepthBatchUnit,
                                                       &kBlurUpsampleLinBatchUnit};
+#endif
+// The per-layer projection units (build.py MIXED_SOURCES), loaded eagerly like the others.  The emulator builds them into a library of
+// their own (tests/emu/mixed.py), so the emulator's unit list above stays the SOURCES one.
+extern const KernelUnit kPrepareDepthMixedLayeredUnit, kPrepareDepthArrayMixedUnit, kRenderAoMixedLayeredUnit, kBlurUpsampleLinMixedUnit;
+#ifndef MEAO_EMULATE
+inline const KernelUnit *const kMixedKernelUnits[] = {&kPrepareDepthMixedLayeredUnit, &kPrepareDepthArrayMixedUnit, &kRenderAoMixedLayeredUnit,
+                                                      &kBlurUpsampleLinMixedUnit};
 #endif
 
 // ---- halo pack / unpack: row blocks of pitched buffers <-> contiguous staging, one launch ------

@@ -90,6 +90,11 @@ struct MeaoCtx : SizeState {
     std::vector<std::pair<int, int>> views_checked;
     MeaoVariants variants = {0, 0, 0, 0};
     int projection = MEAO_PROJECTION_PERSPECTIVE;  // meao_set_projection (a structural input: it selects the orthographic kernels)
+    // meao_set_layer_projections: one MeaoProjection per layer, or empty (every layer has `projection`).  A structural input like the
+    // context's projection: a table that mixes both selects the mixed kernels (frame_record.h launch_entry_mixed).  layer_proj_ortho: its
+    // orthographic entries.
+    std::vector<int32_t> layer_proj;
+    int layer_proj_ortho = 0;
     bool plan_dirty = true;                 // a structural input changed: the next frame re-plans (replan)
     // Frame constants (include/meao.h): bumped by every change of MeaoParams or of a camera that keeps the Z direction.  A size whose
     // plan_gen is older re-plans its constants on the host (refresh_constants); a graph captured at an older one re-targets (launch_cached).
@@ -146,9 +151,11 @@ struct MeaoCtx : SizeState {
     struct GraphKey { const void *p[4]; int kind; int64_t pitch[4] = {0, 0, 0, 0}; int size[4] = {0, 0, 0, 0}; uint64_t list_hash = 0;
         std::vector<uintptr_t> list = {};
         const void *table = nullptr;
+        uint64_t proj = 0;                  // FrameState::proj_key: the layers' projections the graph was recorded with
         bool operator<(const GraphKey &o) const {
         for (int i = 0; i < 4; i++) if (p[i] != o.p[i]) return p[i] < o.p[i];
         if (kind != o.kind) return kind < o.kind;
+        if (proj != o.proj) return proj < o.proj;
         for (int i = 0; i < 4; i++) if (pitch[i] != o.pitch[i]) return pitch[i] < o.pitch[i];
         for (int i = 0; i < 4; i++) if (size[i] != o.size[i]) return size[i] < o.size[i];
         if (table != o.table) return table < o.table;
@@ -204,9 +211,16 @@ int refuse_ortho_band(MeaoCtx *c, const char *what)
     return fail(c, MEAO_ERR_UNSUPPORTED, "%s: row bands and the halo exchange are not supported under an orthographic projection "
                 "(meao_set_projection)", what);
 }
+// An orthographic layer of a projection table (meao_set_layer_projections) carries the same restriction.
+int refuse_ortho_layer_band(MeaoCtx *c, const char *what)
+{
+    return fail(c, MEAO_ERR_UNSUPPORTED, "%s: row bands and the halo exchange are not supported with an orthographic layer "
+                "(meao_set_layer_projections)", what);
+}
 #define BAND_GUARD(c, what) do { if ((c) && (c)->layers > 1) return refuse_layered((c), (what)); \
     if ((c) && ((c)->res_w > 0 || (c)->res_layers > 0)) return refuse_reserved((c), (what)); \
-    if ((c) && (c)->projection != MEAO_PROJECTION_PERSPECTIVE) return refuse_ortho_band((c), (what)); } while (0)
+    if ((c) && (c)->projection != MEAO_PROJECTION_PERSPECTIVE) return refuse_ortho_band((c), (what)); \
+    if ((c) && (c)->layer_proj_ortho > 0) return refuse_ortho_layer_band((c), (what)); } while (0)
 #define CUDA_TRY(c, expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) \
     return fail((c), MEAO_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); } while (0)
 
@@ -225,6 +239,9 @@ void sample_thickness(float t[12])
     t[10] = mathf_sqrt(1 - 0.4f * 0.4f - 0.8f * 0.8f);  t[11] = mathf_sqrt(1 - 0.6f * 0.6f - 0.6f * 0.6f);
 }
 
+// The projection of layer l: its entry of the projection table while one is set, else the context's (meao_set_layer_projections)
+inline int layer_projection(const MeaoCtx *c, int l) { return c->layer_proj.empty() ? c->projection : c->layer_proj[l]; }
+
 // Z direction of the context's cameras (meao_set_layer_cameras requires one for all layers)
 inline int ctx_reversed_z(const MeaoCtx *c) { return c->layer_cams.empty() ? c->camera.reversed_z : c->layer_cams[0].reversed_z; }
 
@@ -240,10 +257,11 @@ void note_camera_change(MeaoCtx *c, int old_reversed_z, int new_reversed_z)
 // The camera-dependent constants of camera `cam` (the part of build_plan that reads the camera).
 // Under an orthographic projection (include/meao.h meao_set_projection) ZBufferParams holds the affine linearisation {1 - n/f, n/f}
 // (reversed: {n/f - 1, 1}), the inv_thickness tables hold it_i = (far / ThicknessMultiplier) / SampleThickness[i] -- a sphere of constant
-// size, in units of LinearDepth (eye depth / far) -- and the padding value is the linearisation of raw depth 0.
-void camera_consts(const MeaoCtx *c, const MeaoCamera &cam, CamConsts &p)
+// size, in units of LinearDepth (eye depth / far) -- and the padding value is the linearisation of raw depth 0.  `projection`: that of
+// the camera's layer (layer_projection).
+void camera_consts(const MeaoCtx *c, const MeaoCamera &cam, int projection, CamConsts &p)
 {
-    const bool ortho = c->projection == MEAO_PROJECTION_ORTHOGRAPHIC;
+    const bool ortho = projection == MEAO_PROJECTION_ORTHOGRAPHIC;
     if (!ortho) {
         // AO.cs:561-568
         const float fpn = cam.far_clip / cam.near_clip;
@@ -285,17 +303,15 @@ void camera_consts(const MeaoCtx *c, const MeaoCamera &cam, CamConsts &p)
 void build_plan(MeaoCtx *c)
 {
     Plan &p = c->plan;
-    // every layer's camera constants: one entry per distinct camera computed, copied to the layers that share it
+    // every layer's camera constants, with its camera and its projection: one entry per run of layers that share both computed, copied to
+    // the others of the run
     const int L = c->layers;
     c->layer_consts.resize(L);
-    if (c->layer_cams.empty()) {
-        camera_consts(c, c->camera, c->layer_consts[0]);
-        for (int l = 1; l < L; l++) c->layer_consts[l] = c->layer_consts[0];
-    } else {
-        for (int l = 0; l < L; l++) {
-            if (l > 0 && memcmp(&c->layer_cams[l], &c->layer_cams[l - 1], sizeof(MeaoCamera)) == 0) c->layer_consts[l] = c->layer_consts[l - 1];
-            else camera_consts(c, c->layer_cams[l], c->layer_consts[l]);
-        }
+    auto cam = [c](int l) -> const MeaoCamera & { return c->layer_cams.empty() ? c->camera : c->layer_cams[l]; };
+    for (int l = 0; l < L; l++) {
+        if (l > 0 && layer_projection(c, l) == layer_projection(c, l - 1) && memcmp(&cam(l), &cam(l - 1), sizeof(MeaoCamera)) == 0)
+            c->layer_consts[l] = c->layer_consts[l - 1];
+        else camera_consts(c, cam(l), layer_projection(c, l), c->layer_consts[l]);
     }
     // the Plan's own camera constants: the first layer's
     const CamConsts &cc = c->layer_consts[0];
@@ -303,7 +319,7 @@ void build_plan(MeaoCtx *c)
     p.zb[2] = p.zb[3] = 0;
     p.variants = c->variants;
     p.reversed_z = ctx_reversed_z(c);
-    p.orthographic = c->projection == MEAO_PROJECTION_ORTHOGRAPHIC;
+    plan_projections(*c, [c](int l) { return layer_projection(c, l) == MEAO_PROJECTION_ORTHOGRAPHIC; });
     memcpy(p.inv_thickness, cc.inv_thickness, sizeof p.inv_thickness);
     memcpy(p.inv_thickness_wide, cc.inv_thickness_wide, sizeof p.inv_thickness_wide);
     memcpy(p.pad, cc.pad, sizeof p.pad);
@@ -683,6 +699,7 @@ int record_launch(MeaoCtx *c, const FrameLaunch &l, const FrameIO &io, cudaStrea
     if (l.stage == kStageUpsample && l.level == 1 && !io.batch) c->last_out = io.aio ? const_cast<void *>(io.aio->ao_array) : io.ao;
     NvtxRange nv(nvtx[l.stage]);
     if (io.batch) CUDA_TRY(c, launch_entry_batch(*c, l, io, forced_render_tile(), s));
+    else if (!c->layer_ortho.empty()) CUDA_TRY(c, launch_entry_mixed(*c, l, io, forced_render_tile(), s));
     else CUDA_TRY(c, c->plan.orthographic ? launch_entry_ortho(*c, l, io, forced_render_tile(), s) : launch_entry_views(*c, l, io, forced_render_tile(), s));
     c->launches++;
     return 0;
@@ -885,6 +902,7 @@ int meao_create(const MeaoDeviceCfg *cfg, MeaoCtx **out)
             for (const KernelUnit *u : kViewKernelUnits) u->walk(&pe);
             for (const KernelUnit *u : kOrthoKernelUnits) u->walk(&pe);
             for (const KernelUnit *u : kBatchKernelUnits) u->walk(&pe);
+            for (const KernelUnit *u : kMixedKernelUnits) u->walk(&pe);
             if (pe != cudaSuccess) { cudaGetLastError(); meao_destroy(c); return fail(nullptr, MEAO_ERR_CUDA, "loading the kernels failed: %s", cudaGetErrorString(pe)); }
             preloaded[dev] = true;
         }
@@ -996,6 +1014,52 @@ int meao_set_projection(MeaoCtx *c, int32_t projection)
 
 int meao_get_projection(const MeaoCtx *c) { return c ? c->projection : MEAO_ERR_INVALID; }
 
+int meao_set_layer_projections(MeaoCtx *c, const int32_t *projections, int32_t count)
+{
+    if (!c) return MEAO_ERR_INVALID;
+    if (!projections && count == 0) {
+        if (c->layer_proj.empty()) return 0;
+        c->layer_proj.clear();
+        c->layer_proj_ortho = 0;
+        c->plan_dirty = true;       // the context's projection again: re-plan + drop the captured graphs (ensure_ready)
+        c->frame_gen++;
+        return 1;
+    }
+    if (!projections) return fail(c, MEAO_ERR_INVALID, "projections is NULL with count %d (NULL clears the table only with count 0)", count);
+    if (count != c->layers) return fail(c, MEAO_ERR_INVALID, "count %d differs from the context's %d layers (meao_set_layers)", count, c->layers);
+    int ortho = 0;
+    for (int l = 0; l < count; l++) {
+        if (projections[l] != MEAO_PROJECTION_PERSPECTIVE && projections[l] != MEAO_PROJECTION_ORTHOGRAPHIC)
+            return fail(c, MEAO_ERR_INVALID, "layer %d: projection %d is neither MEAO_PROJECTION_PERSPECTIVE (0) nor MEAO_PROJECTION_ORTHOGRAPHIC (1)",
+                        l, projections[l]);
+        if (projections[l] == MEAO_PROJECTION_ORTHOGRAPHIC) ortho++;
+    }
+    if (ortho) {        // an orthographic layer carries the restrictions of an orthographic context (meao_set_projection)
+        const int l = (int)(std::find(projections, projections + count, (int32_t)MEAO_PROJECTION_ORTHOGRAPHIC) - projections);
+        if (!c->views.empty())
+            return fail(c, MEAO_ERR_UNSUPPORTED, "layer %d: projection: an orthographic layer is not supported with a layer-viewport table "
+                        "(meao_set_layer_viewports)", l);
+        if ((c->W > 0 && (c->band0 != 0 || c->band1 != c->H)) || c->peer_base[0] || c->peer_base[1])
+            return fail(c, MEAO_ERR_UNSUPPORTED, "layer %d: projection: an orthographic layer is not supported with a row band or a neighbour "
+                        "connection (meao_set_row_band, meao_band_connect)", l);
+    }
+    if ((int)c->layer_proj.size() == count && std::equal(projections, projections + count, c->layer_proj.begin())) return 0;
+    c->layer_proj.assign(projections, projections + count);
+    c->layer_proj_ortho = ortho;
+    c->plan_dirty = true;           // other kernels and other constants: re-plan + drop the captured graphs (ensure_ready)
+    c->frame_gen++;
+    return 1;
+}
+
+int meao_get_layer_projections(const MeaoCtx *c, int32_t *out, int32_t capacity)
+{
+    if (!c) return MEAO_ERR_INVALID;
+    const int n = (int)c->layer_proj.size();
+    if (n && (!out || capacity < n)) return MEAO_ERR_INVALID;
+    if (n) std::copy(c->layer_proj.begin(), c->layer_proj.end(), out);
+    return n;
+}
+
 int meao_set_layer_cameras(MeaoCtx *c, const MeaoCamera *cams, int32_t count)
 {
     if (!c) return MEAO_ERR_INVALID;
@@ -1057,6 +1121,8 @@ int meao_set_layer_viewports(MeaoCtx *c, const MeaoLayerViewport *views, int32_t
     if (!views) return fail(c, MEAO_ERR_INVALID, "views is NULL with count %d (NULL clears the table only with count 0)", count);
     if (c->projection != MEAO_PROJECTION_PERSPECTIVE)
         return fail(c, MEAO_ERR_UNSUPPORTED, "a layer-viewport table is not supported under an orthographic projection (meao_set_projection)");
+    if (c->layer_proj_ortho > 0)
+        return fail(c, MEAO_ERR_UNSUPPORTED, "a layer-viewport table is not supported with an orthographic layer (meao_set_layer_projections)");
     if (count != c->layers) return fail(c, MEAO_ERR_INVALID, "count %d differs from the context's %d layers (meao_set_layers)", count, c->layers);
     for (int l = 0; l < count; l++)
         for (int i = 0; i < 6; i++)
@@ -1165,6 +1231,13 @@ static int switch_layers(MeaoCtx *c, int layers)
         c->layer_cams.clear();
         note_camera_change(c, old_z, c->camera.reversed_z);
     }
+    if (!c->layer_proj.empty()) {
+        // the projection table too, as host bookkeeping: every planned (W, H, L) plans its constants and projections again when it is
+        // next swapped in (refresh_constants), and the graph keys carry the projections a frame was recorded with (GraphKey::proj)
+        c->layer_proj.clear();
+        c->layer_proj_ortho = 0;
+        c->consts_gen++;
+    }
     c->views.clear();
     c->views_pending = false;
     c->views_checked.clear();
@@ -1188,6 +1261,10 @@ int meao_set_layers(MeaoCtx *c, int32_t layers)
     old_cams.swap(c->layer_cams);                   // a table has one camera per layer: a new layer count clears it
     std::vector<MeaoLayerViewport> old_views;       // and so does a viewport table
     old_views.swap(c->views);
+    std::vector<int32_t> old_proj;                  // and a projection table
+    old_proj.swap(c->layer_proj);
+    const int old_proj_ortho = c->layer_proj_ortho;
+    c->layer_proj_ortho = 0;
     const bool old_views_pending = c->views_pending;
     c->views_pending = false;
     c->layers = layers;
@@ -1204,6 +1281,8 @@ int meao_set_layers(MeaoCtx *c, int32_t layers)
         c->layer_cams.swap(old_cams);
         c->views.swap(old_views);
         c->views_pending = old_views_pending;
+        c->layer_proj.swap(old_proj);
+        c->layer_proj_ortho = old_proj_ortho;
         if (allocate(c)) { c->W = c->H = 0; }        // the previous arena could not be restored either: the context needs meao_resize
         c->error = err;
         return rc;
@@ -1438,6 +1517,7 @@ static int launch_cached(MeaoCtx *c, const MeaoCtx::GraphKey &key_in, cudaStream
     if (capturing) return record(s, c->pdl_level >= 0 ? c->pdl_level : 0);
     MeaoCtx::GraphKey key = key_in;
     key.size[0] = c->W; key.size[1] = c->H; key.size[2] = c->slot; key.size[3] = c->layers;
+    key.proj = c->proj_key;
     auto it = c->graphs.find(key);
     bool retiring = false;
     if (it == c->graphs.end() || it->second.gen != c->plan_gen) {
@@ -2062,6 +2142,8 @@ int check_batch(MeaoCtx *c, int count, int kind, bool arrays)
                                          "its own; clear the table first");
     if (c->projection != MEAO_PROJECTION_PERSPECTIVE)
         return fail(c, MEAO_ERR_UNSUPPORTED, "batches are perspective-only: this context has an orthographic projection (meao_set_projection)");
+    if (c->layer_proj_ortho > 0)
+        return fail(c, MEAO_ERR_UNSUPPORTED, "batches are perspective-only: this context has an orthographic layer (meao_set_layer_projections)");
     if (c->band0 != 0 || c->band1 != c->H) return fail(c, MEAO_ERR_UNSUPPORTED, "batches need a whole-frame context (no row band)");
     return 0;
 }
