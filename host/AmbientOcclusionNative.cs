@@ -120,6 +120,10 @@ namespace MiniEngineAO
         // null with count 0 clears the table, which then decides each layer's projection alone (a structural input)
         [DllImport(Lib)] public static extern int meao_set_layer_projections(IntPtr ctx, [In] int[] projections, int count);
         [DllImport(Lib)] public static extern int meao_get_layer_projections(IntPtr ctx, [Out] int[] projections, int capacity);
+        // Cameras read from device memory at every launch and graph replay (meao_bind_device_cameras).  Declarations only: a Unity host has
+        // no CUDA buffer of its own to hand over; a native plugin or an interop host that keeps its cameras on the GPU passes its pointer.
+        [DllImport(Lib)] public static extern int meao_bind_device_cameras(IntPtr ctx, IntPtr camerasDev, int capacity);
+        [DllImport(Lib)] public static extern int meao_device_camera_status(IntPtr ctx, [Out] int[] out4);
 
         public static void Check(IntPtr ctx, int rc)
         {

@@ -47,7 +47,9 @@ extern "C" {
                               *    + meao_reserve_layers / meao_layer_reservation (dynamic view counts: a layer change inside the
                               *      reservation is host bookkeeping; additive)
                               *    + meao_set_layer_projections / meao_get_layer_projections (perspective and orthographic layers in one
-                              *      layered frame; additive) */
+                              *      layered frame; additive)
+                              *    + meao_bind_device_cameras / meao_device_camera_status (cameras read from device memory at every
+                              *      launch and graph replay; additive) */
 
 typedef struct MeaoCtx MeaoCtx;
 
@@ -227,6 +229,39 @@ int meao_get_projection(const MeaoCtx *ctx);     /* MeaoProjection, or MEAO_ERR_
  * capacity. */
 int meao_set_layer_projections(MeaoCtx *ctx, const int32_t *projections, int32_t count);
 int meao_get_layer_projections(const MeaoCtx *ctx, int32_t *out, int32_t capacity);
+/* Cameras from device memory: a frame recorded into a graph (the context's own or a caller's capture, torch.cuda.graph) follows a moving
+ * camera without a capture or an instantiation per camera change, and a camera that already lives on the GPU (a pose network's output,
+ * a GPU-side camera animation) is never copied to the host.
+ *   - cameras_dev: device memory of the context's device holding `capacity` cameras of 3 floats each, {near_clip, far_clip,
+ *     tan_half_fov_h}, each with the meaning of MeaoCamera under its layer's projection.  A contiguous [n, 3] float32 CUDA tensor fits.
+ *     Layer l of every frame uses entry l.  A frame with more layers than capacity is refused with MEAO_ERR_INVALID and launches nothing,
+ *     so one buffer of max_layers cameras serves every layer count of a reservation (meao_reserve_layers).
+ *   - cameras_dev == NULL with capacity == 0 unbinds.  capacity must be in 1..65535.  Returns 1 when the binding changed, 0 when the same
+ *     one is set again.  Binding, unbinding and a new pointer or capacity are structural inputs: a re-plan with a device synchronise, the
+ *     captured graphs dropped, meao_frame_generation moved.  Plan-only contexts record the binding and allocate nothing.
+ *   - The buffer's CONTENTS are not tracked: they are read by the frame's first kernel, in stream order, at every launch and every replay.
+ *     Writing new cameras moves no generation and needs no capture.  The host-buffer calls (meao_render_host, _async) run on the context's
+ *     own streams, so the buffer must be complete before such a call is made.  The caller keeps the buffer alive while it is bound.
+ *   - While a buffer is bound it alone decides every layer's near and far planes and field of view.  meao_set_camera and
+ *     meao_set_layer_cameras still record their values, which apply again once the buffer is unbound; a change that keeps the Z direction
+ *     neither moves meao_frame_generation nor marks tables pending, so it never makes a recording into a caller's capture refuse.
+ *     reversed_z and the projections (meao_set_projection, meao_set_layer_projections) stay structural, host-side inputs.
+ *   - The constant getters (meao_zbuffer_params, meao_render_constants and their _layer forms) keep describing the HOST cameras.
+ *   - Every frame form runs the derivation first: pointers, pitched views, host buffers, CUDA arrays and _at, layer-viewport tables,
+ *     batches, orthographic and mixed projection tables, the bound events, MEAO_FLAG_NO_GRAPH and recording into a caller's capture.
+ *     meao_stage_downsample runs it too, and the later stage calls use the tables it derived.  meao_kernels_per_frame counts it (+1).  A
+ *     single-layer frame takes the layered kernels with one layer, which read the derived tables; each layer is bit-identical to a frame
+ *     of a context whose host cameras are the buffer's.
+ *   - Refused with MEAO_ERR_UNSUPPORTED before anything changes, in either order: row bands and their halo and exchange calls; and while
+ *     bound, meao_debug_view of the TiledDepth ids 6-9, whose atlas padding is a host value.  meao_get_buffer of ids 6-9 reads each
+ *     layer's padding back from the derived tables.
+ * meao_device_camera_status: {frames that met an invalid camera since the bind, the lowest such layer of the latest of them, its field (1
+ * near_clip, 2 far_clip, 3 tan_half_fov_h), 0}.  An entry is invalid when it fails meao_set_camera's tests (!(near > 0), !(far > near),
+ * !(tan_half_fov_h > 0); NaN fails): its layer's tables are not written, so its AO is unspecified, and every other layer is exact.  A
+ * stream-less read like meao_band_status, without a device synchronise; all zeros on a plan-only context; MEAO_ERR_INVALID when nothing
+ * is bound. */
+int meao_bind_device_cameras(MeaoCtx *ctx, const float *cameras_dev, int32_t capacity);
+int meao_device_camera_status(const MeaoCtx *ctx, int32_t out4[4]);
 /* replaces: RTHandle.SetBaseDimensions + AllocateNow + the rebuild it triggers (AO.cs:338-341, 501-506).
  * Allocates the intermediates for width x height.  Returns 1 if dimensions changed, 0 if not.
  * A size change RESETS the row band to the whole frame and drops the neighbour connections (meao_set_row_band,

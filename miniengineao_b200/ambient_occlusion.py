@@ -105,6 +105,14 @@ class AmbientOcclusion:
         # up to it costs no allocation, device synchronise or graph teardown; None = every layer change re-allocates
         self.maxLayers: int | None = None
         self._reservedLayers = 0            # what meao_reserve_layers was last given
+        # cameras that live on the GPU (meao_bind_device_cameras): a contiguous CUDA float32 tensor [n >= layers, 3] of (near_clip,
+        # far_clip, tan_half_fov_h) per layer, read by every frame at launch and at every graph replay -- write new cameras into it (a torch
+        # op inside a captured graph, a pose network's output) and a recorded frame follows them without a re-capture.  While one is set
+        # it decides every layer's planes and field of view; the cameras' Z direction and projection still come from `camera` and
+        # layerCameras.  None = the host cameras
+        self.deviceCameras = None
+        self._boundCameras = (0, 0)         # (data_ptr, n) meao_bind_device_cameras was last given
+        self._boundCameraTensor = None      # a reference that keeps the bound buffer alive
         self._contextLayers = 1             # what meao_set_layers was last given
         self._band = None                   # (row0, row1) after set_row_band; reset by every re-allocation
         self._drawCountPerFrame = 0         # AO.cs:289: used to detect single-pass stereo
@@ -191,6 +199,7 @@ class AmbientOcclusion:
             rebuild |= self._check(self._lib.meao_set_layer_projections(self._ctx, arr, len(projections))) == 1
         if cam.orthographic:
             rebuild |= self._check(self._lib.meao_set_projection(self._ctx, N.MEAO_PROJECTION_ORTHOGRAPHIC)) == 1
+        rebuild |= self._apply_device_cameras()
         reallocated |= self._apply_reservation(width, cam.pixelHeight, stereo)
         resized = self._check(self._lib.meao_resize(self._ctx, width, cam.pixelHeight)) == 1          # CheckBaseDimensions
         reallocated |= resized and self._reserved == (0, 0)       # inside a reservation a resize allocates nothing
@@ -268,6 +277,31 @@ class AmbientOcclusion:
         if not self.perLayerProjection or self.layerCameras is None:
             return None
         return [N.MEAO_PROJECTION_ORTHOGRAPHIC if c.orthographic else N.MEAO_PROJECTION_PERSPECTIVE for c in self.layerCameras]
+
+    def _apply_device_cameras(self) -> bool:
+        """Hands deviceCameras to meao_bind_device_cameras when its data_ptr or length changed; True if the binding changed."""
+        t = self.deviceCameras
+        if t is None:
+            want = (0, 0)
+        else:
+            if not getattr(t, "is_cuda", False) or str(t.dtype) != "torch.float32" or t.dim() != 2 or t.shape[1] != 3 or not t.is_contiguous():
+                raise ValueError("deviceCameras must be a contiguous CUDA float32 tensor of shape [n, 3]")
+            if t.shape[0] < int(self.layers):
+                raise ValueError(f"deviceCameras has {t.shape[0]} cameras for {int(self.layers)} layers")
+            want = (t.data_ptr(), int(t.shape[0]))
+        if want == self._boundCameras:
+            self._boundCameraTensor = t
+            return False
+        changed = self._check(self._lib.meao_bind_device_cameras(self._ctx, C.c_void_p(want[0] or None), want[1])) == 1
+        self._boundCameras, self._boundCameraTensor = want, t
+        return changed
+
+    def deviceCameraStatus(self) -> tuple[int, int, int]:
+        """meao_device_camera_status: (frames that met an invalid camera since the bind, the lowest such layer of the latest of them,
+        its field: 1 near_clip, 2 far_clip, 3 tan_half_fov_h).  Reads without a device synchronise."""
+        out = (C.c_int32 * 4)()
+        self._check(self._lib.meao_device_camera_status(self._ctx, out))
+        return int(out[0]), int(out[1]), int(out[2])
 
     def _apply_layer_viewports(self) -> bool:
         """Hands layerViewports to meao_set_layer_viewports (after meao_set_layers, which clears the table); True if a value changed."""

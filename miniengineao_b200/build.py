@@ -30,6 +30,10 @@ BATCH_SOURCES = ["prepare_depth_array_batch.cu", "blur_upsample_array_batch.cu",
 # libmeao.so with SOURCES, each a textual include of an existing kernel body under MEAO_ORTHO 2, so the other kernels keep their code; the
 # CPU emulator builds them into a library of their own (tests/emu/mixed.py), and tests/test_layer_projections_units.py audits them.
 MIXED_SOURCES = ["prepare_depth_mixed_layered.cu", "prepare_depth_array_mixed.cu", "render_ao_mixed_layered.cu", "blur_upsample_lin_mixed.cu"]
+# The device-camera kernel (meao_bind_device_cameras: the per-layer camera tables derived on the device at the head of every frame):
+# compiled into libmeao.so with SOURCES; tests/test_device_cameras_units.py audits it, and the CPU emulator builds it into a library of its
+# own (tests/emu/device_cameras.py).
+CAMERA_SOURCES = ["camera_tables.cu"]
 HEADERS = ["common.cuh", "kernels.h", "prepare_depth_kernel.inc", "render_ao_kernel.inc", "render_ao_groups.inc", "render_ao_sample.inc", "blur_upsample_device.inc", "blur_upsample_kernel.inc",
            "blur_upsample_layer_args.inc", "blur_upsample_lin_device.inc", "surface_io.cuh", "depth_in.cuh", "arena_layout.h", "frame_record.h",
            os.path.join("..", "..", "include", "meao.h")]
@@ -56,7 +60,7 @@ def is_stale() -> bool:
     if not os.path.exists(LIB):
         return True
     t = os.path.getmtime(LIB)
-    deps = [os.path.join(CSRC, f) for f in SOURCES + VIEW_SOURCES + ORTHO_SOURCES + BATCH_SOURCES + MIXED_SOURCES + HEADERS] + [os.path.abspath(__file__)]
+    deps = [os.path.join(CSRC, f) for f in SOURCES + VIEW_SOURCES + ORTHO_SOURCES + BATCH_SOURCES + MIXED_SOURCES + CAMERA_SOURCES + HEADERS] + [os.path.abspath(__file__)]
     return any(os.path.getmtime(d) > t for d in deps)
 
 
@@ -64,7 +68,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     if not force and not is_stale():
         return LIB
     extra = os.environ.get("MEAO_NVCC_DEFS", "").split()      # tuning experiments, e.g. "-DMEAO_REN_MINB=12"
-    cmd = [_nvcc()] + NVCC_FLAGS + extra + ["-o", LIB] + [os.path.join(CSRC, f) for f in SOURCES + VIEW_SOURCES + ORTHO_SOURCES + BATCH_SOURCES + MIXED_SOURCES]
+    cmd = [_nvcc()] + NVCC_FLAGS + extra + ["-o", LIB] + [os.path.join(CSRC, f) for f in SOURCES + VIEW_SOURCES + ORTHO_SOURCES + BATCH_SOURCES + MIXED_SOURCES + CAMERA_SOURCES]
     proc = subprocess.run(cmd, capture_output=True, text=True)
     if verbose or proc.returncode != 0:
         sys.stderr.write(proc.stdout + proc.stderr)

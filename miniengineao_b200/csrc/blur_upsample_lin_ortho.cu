@@ -56,10 +56,10 @@ const struct {      // [depth_format_slot]
 
 cudaError_t launch_blur_upsample_lin_ortho(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
                                            const UpsampleArgs &a_in, const uint8_t *lo_ao2, int lo_a2pitch, const DepthIn &din_in, int layers,
-                                           int sm_count, cudaStream_t s)
+                                           int sm_count, cudaStream_t s, bool layered)
 {
     if (!din_in.raw)
-        return launch_blur_upsample_lin(lo_depth_map, lo_ao_map, lo_ao2_map, use_tma, a_in, lo_ao2, lo_a2pitch, din_in, layers, sm_count, s);
+        return launch_blur_upsample_lin(lo_depth_map, lo_ao_map, lo_ao2_map, use_tma, a_in, lo_ao2, lo_a2pitch, din_in, layers, sm_count, s, layered);
     if (a_in.row1 <= a_in.row0) return cudaSuccess;
     if (layers < 1 || layers > kMaxLayers) return cudaErrorInvalidValue;
     if (!a_in.hi_is_half || a_in.hi_ao || (lo_ao2 && !lo_ao2_map)) return cudaErrorInvalidValue;      // the final level only
@@ -73,7 +73,7 @@ cudaError_t launch_blur_upsample_lin_ortho(const CUtensorMap &lo_depth_map, cons
     if (!din.ao_layer_pitch) din.ao_layer_pitch = (long long)a.hih * a.out_pitch;
     const int k = depth_format_slot(din.in_format);
     const UpsamplePreminArgs pa{a, lo_ao2, lo_a2pitch};
-    if (layers == 1) {
+    if (layers == 1 && !layered) {
         if (!lo_ao2) MEAO_LAUNCH((kKernels.plain[k]), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, a, t, din);
         else         MEAO_LAUNCH((kKernels.premin[k]), grid, kThreads, 0, s, lo_depth_map, lo_ao_map, *lo_ao2_map, pa, t, din);
     } else {

@@ -270,11 +270,12 @@ inline PrepareArgs prepare_args(const FrameState &f, const DepthIn &d)
 }
 
 // aio: read the depth from a CUDA array instead of a.depth.  low_only: LowDepth1..4 only -- the frame's final upsample is launched
-// with the same depth (launch_upsample's `fused`) and writes LinearDepth itself.
-inline cudaError_t launch_prepare(const FrameState &f, const PrepareArgs &a, const ArrayIO *aio, bool low_only, cudaStream_t s)
+// with the same depth (launch_upsample's `fused`) and writes LinearDepth itself.  layered: the layered kernel at layers == 1 too, which
+// reads the camera table (a device camera buffer is bound: FrameIO.cams)
+inline cudaError_t launch_prepare(const FrameState &f, const PrepareArgs &a, const ArrayIO *aio, bool low_only, cudaStream_t s, bool layered = false)
 {
     if (aio) return launch_prepare_depth_array(a, aio->depth, aio->depth_surf, aio->depth_x, aio->depth_y, f.layers, s, f.layer_zb);
-    if (f.layers > 1) return launch_prepare_depth_layered(a, f.layers, s, low_only, f.layer_zb);
+    if (f.layers > 1 || layered) return launch_prepare_depth_layered(a, f.layers, s, low_only, f.layer_zb);
     return launch_prepare_depth(a, s, low_only);
 }
 
@@ -318,11 +319,12 @@ inline const LayerRender *render_layer_cams(const FrameState &f, const RenderArg
     return f.layer_ren ? f.layer_ren + (size_t)(2 * (k - 1) + a.wide) * f.layers : nullptr;
 }
 
-// The render launch of level k with the map of a.tile_h; a layered frame takes its layers' camera table entries
-inline cudaError_t launch_render(const FrameState &f, const RenderArgs &a, int k, int kind, cudaStream_t s)
+// The render launch of level k with the map of a.tile_h; a layered frame (and, with `layered`, a single layer) takes its layers'
+// camera table entries
+inline cudaError_t launch_render(const FrameState &f, const RenderArgs &a, int k, int kind, cudaStream_t s, bool layered = false)
 {
     const CUtensorMap &map = render_map(f, a, k);
-    if (f.layers == 1) return launch_render_ao(map, f.tma_ok, a, s);
+    if (f.layers == 1 && !layered) return launch_render_ao(map, f.tma_ok, a, s);
     return launch_render_ao_layered(map, f.tma_ok, a, f.layers, s, render_layer_cams(f, a, k), kind != MEAO_DEPTH_LINEAR_F32 ? 1 : 0);
 }
 
@@ -364,14 +366,16 @@ inline const CUtensorMap &upsample_ao_map(const FrameState &f, int lo)
 }
 inline const uint8_t *upsample_lo_ao2(const FrameState &f, int lo) { return hq_level(f, lo) ? f.hq[lo] : nullptr; }
 
-inline cudaError_t launch_upsample(const FrameState &f, int lo, const UpsampleArgs &a, const ArrayIO *aio, const DepthIn *fused, cudaStream_t s)
+// layered: a fused final upsample reads the camera table at layers == 1 too.
+inline cudaError_t launch_upsample(const FrameState &f, int lo, const UpsampleArgs &a, const ArrayIO *aio, const DepthIn *fused, cudaStream_t s,
+                                   bool layered = false)
 {
     const bool final_level = lo == 1;
     const uint8_t *lo_ao2 = upsample_lo_ao2(f, lo);
     const CUtensorMap &ao_map = upsample_ao_map(f, lo);
     const CUtensorMap &dm = f.maps.low_ups[lo], *hm = &f.maps.hq_ups[lo];
     if (fused && final_level)
-        return launch_blur_upsample_lin(dm, ao_map, hm, f.tma_ok, a, lo_ao2, f.occ_pitch[lo], *fused, f.layers, f.sm_count, s);
+        return launch_blur_upsample_lin(dm, ao_map, hm, f.tma_ok, a, lo_ao2, f.occ_pitch[lo], *fused, f.layers, f.sm_count, s, layered);
     if (aio && final_level)
         return launch_blur_upsample_array(dm, ao_map, hm, f.tma_ok, a, lo_ao2, f.occ_pitch[lo], f.layers, f.sm_count, aio->ao, aio->ao_surf,
                                           aio->ao_x, aio->ao_y, s);
@@ -380,7 +384,8 @@ inline cudaError_t launch_upsample(const FrameState &f, int lo, const UpsampleAr
 }
 
 // ---- the frame schedule: which kernels a frame launches, in what order, on which stream and after which other launch ----------
-enum FrameStage { kStagePrepare, kStageRender, kStageRenderWide, kStageUpsample };
+// kStageCamera: the camera tables derived from a bound device camera buffer (launch_camera_tables), ahead of the prepare
+enum FrameStage { kStagePrepare, kStageRender, kStageRenderWide, kStageUpsample, kStageCamera };
 // PDL (DESIGN.md 2.5): a launch whose only predecessor is the launch before it on its stream carries the programmatic-dependent-launch
 // attribute from PDL level 1 on; one that also waits for another branch, from level 2; the first launch of a branch never.
 enum PdlClass { kPdlNever = 0, kPdlFrom1 = 1, kPdlFrom2 = 2 };
@@ -399,7 +404,9 @@ inline bool pdl_on(const FrameLaunch &l, int pdl_level) { return l.pdl != kPdlNe
 // high_quality_mask levels, upsamples k..1.  The branches make it a DAG: the four render levels are independent (SURVEY.md 3.2), a
 // level's wide render rides on its branch, the coarse upsample chain 4->3->2 only needs Occlusion2..4, and only the last two upsamples
 // wait for the big level-1 render.  single_scale (BASELINE.json configs[0]): prepare, render 1 and the final-style upsample on Occlusion1.
-inline std::vector<FrameLaunch> frame_schedule(const MeaoVariants &v)
+// device_cameras (meao_bind_device_cameras): the camera stage first, on the caller's stream; every other launch follows it through the
+// prepare.
+inline std::vector<FrameLaunch> frame_schedule(const MeaoVariants &v, bool device_cameras = false)
 {
     const int kmax = v.single_scale ? 1 : 4;
     std::vector<FrameLaunch> s;
@@ -408,8 +415,10 @@ inline std::vector<FrameLaunch> frame_schedule(const MeaoVariants &v)
         last[branch] = (int)s.size();
         s.push_back(FrameLaunch{stage, level, branch, wait, pdl});
     };
+    if (device_cameras) add(kStageCamera, 0, 0, -1, kPdlNever);
+    const int prep = (int)s.size();
     add(kStagePrepare, 0, 0, -1, kPdlNever);
-    for (int k = 1; k <= kmax; k++) add(kStageRender, k, k - 1, k == 1 ? -1 : 0, k == 1 ? kPdlFrom1 : kPdlNever);
+    for (int k = 1; k <= kmax; k++) add(kStageRender, k, k - 1, k == 1 ? -1 : prep, k == 1 ? kPdlFrom1 : kPdlNever);
     for (int k = 1; k <= kmax; k++)
         if ((v.high_quality_mask >> (k - 1)) & 1) add(kStageRenderWide, k, k - 1, -1, kPdlFrom1);
     if (kmax == 4) {
@@ -427,6 +436,7 @@ inline std::string launch_name(const FrameLaunch &l)
     const std::string k = std::to_string(l.level);
     switch (l.stage) {
         case kStagePrepare: return "prepare_depth";
+        case kStageCamera: return "camera_tables";
         case kStageRender: return "render_ao L" + k;
         case kStageRenderWide: return "render_ao_wide L" + k;
         default: return "blur_upsample L" + k + "->L" + std::to_string(l.level - 1);
@@ -444,7 +454,45 @@ struct FrameIO {
     const ViewPitch *vp = nullptr;
     const LayerView *views = nullptr;   // layer l reads and writes the rectangles and slices of views[l] (launch_entry_views)
     const struct BatchIO *batch = nullptr;  // layer l reads and writes its own resources (launch_entry_batch)
+    // a bound device camera buffer (meao_bind_device_cameras): the schedule's camera stage derives the tables from it, and every launch
+    // that reads a camera takes the layered kernel at layers == 1 too, so that it reads the tables rather than its argument block
+    const struct DeviceCameras *cams = nullptr;
 };
+
+// A bound device camera buffer: cams[l] = {near_clip, far_clip, tan_half_fov_h} of layer l, the kernel's status words (kernels.h
+// CameraTableArgs) and SampleThickness in table order (meao_api.cu sample_thickness).
+struct DeviceCameras {
+    const float *cams = nullptr;
+    uint32_t *status = nullptr;
+    float thick[12] = {0};
+};
+
+// The camera stage's arguments: the tables of the frame's slot, and what camera_consts / layer_render read besides the camera
+inline CameraTableArgs camera_args(const FrameState &f, const DeviceCameras &dc)
+{
+    const bool exh = f.plan.variants.sample_exhaustively != 0;
+    const int *idx = exh ? kIdxExh : kIdxChecker;
+    CameraTableArgs a{};
+    a.cams = dc.cams; a.zb = f.layer_zb; a.ren = f.layer_ren; a.status = dc.status;
+    a.layers = f.layers;
+    for (int l = 0; l < 7; l++) a.lw[l] = f.lw[l];
+    a.stereo = f.plan.variants.single_pass_stereo != 0;
+    a.reversed_z = f.plan.reversed_z != 0;
+    a.ortho = f.plan.orthographic != 0;
+    a.n = exh ? 12 : 7;
+    for (int i = 0; i < a.n; i++) a.thick[i] = dc.thick[idx[i]];
+    return a;
+}
+
+// The camera stage of a frame (kStageCamera): with the layers' projections as a kernel parameter when they mix both.  Apart from
+// launch_entry so that a recorder that never binds a camera buffer does not link the camera kernels.
+inline cudaError_t launch_cameras(const FrameState &f, const DeviceCameras &dc, cudaStream_t s)
+{
+    if (f.layer_ortho.empty()) return launch_camera_tables(camera_args(f, dc), nullptr, s);
+    LayerProjections proj{};
+    for (size_t i = 0; i < f.layer_ortho.size(); i++) proj.ortho[i] = f.layer_ortho[i];
+    return launch_camera_tables(camera_args(f, dc), &proj, s);
+}
 
 // A batch (meao_render_arrays_batch / meao_render_batch): the kernel-parameter tables of its first and last launch.  arrays: layer l
 // reads depth.e[l] and writes ao.e[l]; otherwise layer l reads and writes its own buffers, ptr.e[l].
@@ -458,14 +506,16 @@ struct BatchIO {
 inline cudaError_t launch_entry(const FrameState &f, const FrameLaunch &l, const FrameIO &io, int force_tile, cudaStream_t s)
 {
     const bool final_level = l.stage == kStageUpsample && l.level == 1;
+    const bool layered = io.cams != nullptr;
     switch (l.stage) {
-        case kStagePrepare: return launch_prepare(f, prepare_args(f, io.depth), io.aio, io.low_only, s);
+        case kStageCamera: return cudaErrorInvalidValue;       // launch_cameras, apart so that a recorder without the stage does not link it
+        case kStagePrepare: return launch_prepare(f, prepare_args(f, io.depth), io.aio, io.low_only, s, layered);
         case kStageRender:
         case kStageRenderWide:
-            return launch_render(f, render_args(f, l.level, io.kind, l.stage == kStageRenderWide, force_tile), l.level, io.kind, s);
+            return launch_render(f, render_args(f, l.level, io.kind, l.stage == kStageRenderWide, force_tile), l.level, io.kind, s, layered);
         default:
             return launch_upsample(f, l.level, upsample_args(f, l.level, final_level ? io.ao : nullptr, final_level ? io.vp : nullptr),
-                                   io.aio, io.fused ? &io.depth : nullptr, s);
+                                   io.aio, io.fused ? &io.depth : nullptr, s, layered);
     }
 }
 
@@ -527,23 +577,24 @@ inline cudaError_t launch_entry_batch(const FrameState &f, const FrameLaunch &l,
 inline cudaError_t launch_entry_ortho(const FrameState &f, const FrameLaunch &l, const FrameIO &io, int force_tile, cudaStream_t s)
 {
     if (!f.plan.orthographic || io.views) return cudaErrorInvalidValue;
+    const bool layered = f.layers > 1 || io.cams;
     if (l.stage == kStagePrepare) {
         const PrepareArgs a = prepare_args(f, io.depth);
         if (io.aio) return launch_prepare_depth_array_ortho(a, io.aio->depth, io.aio->depth_surf, io.aio->depth_x, io.aio->depth_y, f.layers, s, f.layer_zb);
-        if (f.layers > 1) return launch_prepare_depth_ortho_layered(a, f.layers, s, io.low_only, f.layer_zb);
+        if (layered) return launch_prepare_depth_ortho_layered(a, f.layers, s, io.low_only, f.layer_zb);
         return launch_prepare_depth_ortho(a, s, io.low_only);
     }
     if (l.stage == kStageRender || l.stage == kStageRenderWide) {
         const RenderArgs a = render_args(f, l.level, io.kind, l.stage == kStageRenderWide, force_tile);
         const CUtensorMap &map = render_map(f, a, l.level);
-        if (f.layers == 1) return launch_render_ao_ortho(map, f.tma_ok, a, s);
+        if (!layered) return launch_render_ao_ortho(map, f.tma_ok, a, s);
         return launch_render_ao_ortho_layered(map, f.tma_ok, a, f.layers, s, render_layer_cams(f, a, l.level),
                                               io.kind != MEAO_DEPTH_LINEAR_F32 ? 1 : 0);
     }
     if (l.level == 1 && io.fused) {
         return launch_blur_upsample_lin_ortho(f.maps.low_ups[1], upsample_ao_map(f, 1), &f.maps.hq_ups[1], f.tma_ok,
                                               upsample_args(f, 1, io.ao, io.vp), upsample_lo_ao2(f, 1), f.occ_pitch[1], io.depth, f.layers,
-                                              f.sm_count, s);
+                                              f.sm_count, s, layered);
     }
     return launch_entry(f, l, io, force_tile, s);
 }
@@ -596,11 +647,13 @@ inline bool buffer_ref(const FrameState &f, int id, BufferRef &b)
 }
 
 // TiledDepth<k> of layer l in the reference layout (16 slices of lw[k + 2] x lh[k + 2] f16) into out, synthesised from LowDepth<k> with
-// the layer's atlas padding for depth kind `kind`
-inline cudaError_t launch_tiled_atlas(const FrameState &f, int k, int l, int kind, __half *out, cudaStream_t s)
+// the layer's atlas padding for depth kind `kind`.  table_pad: the raw-ingest padding value of the layer's camera table entry, read back
+// from the device (a bound device camera buffer derived it); nullptr: the plan's.
+inline cudaError_t launch_tiled_atlas(const FrameState &f, int k, int l, int kind, __half *out, cudaStream_t s, const float *table_pad = nullptr)
 {
+    const float pad = table_pad ? (kind != MEAO_DEPTH_LINEAR_F32 ? *table_pad : 0.0f) : layer_pad(f, l, k, kind);
     return launch_synth_tiled(f.low[k] + (size_t)l * f.lh[k] * f.low_pitch[k], f.lw[k], f.lh[k], f.low_pitch[k], f.lw[k + 2], f.lh[k + 2],
-                              layer_pad(f, l, k, kind), out, s);
+                              pad, out, s);
 }
 
 // The debug view of layer l of buffer `id` into the W x H R8 image at out: TiledDepth<k> through Blit.shader pass 4 (AO.cs:810-814)

@@ -206,7 +206,8 @@ struct DepthIn {
 };
 cudaError_t launch_blur_upsample_lin(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
                                      const UpsampleArgs &a, const uint8_t *lo_ao2, int lo_a2pitch, const DepthIn &din, int layers, int sm_count,
-                                     cudaStream_t s);
+                                     cudaStream_t s, bool layered = false);
+// layered: the layered kernels at layers == 1 too, which read the layer's ZBufferParams from din.layer_zb (meao_bind_device_cameras)
 // blur_upsample_lin<IN>: depth_format_slot(DepthIn.in_format).  The plain / premin and single-image / layered kernels take other
 // parameters: the unit lists each apart, in this order.
 #define MEAO_LIN_SLOTS(K) {K<IN_F32>, K<IN_D16>, K<IN_D24S8>}
@@ -317,7 +318,7 @@ cudaError_t launch_render_ao_ortho_layered(const CUtensorMap &low_map, bool use_
                                            const struct LayerRender *layer_cam = nullptr, int layer_pad = 0);
 cudaError_t launch_blur_upsample_lin_ortho(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
                                            const UpsampleArgs &a, const uint8_t *lo_ao2, int lo_a2pitch, const DepthIn &din, int layers,
-                                           int sm_count, cudaStream_t s);
+                                           int sm_count, cudaStream_t s, bool layered = false);
 
 // ---- per-layer projections (meao_set_layer_projections): a layered frame whose layers mix both projections ---------------------------
 // The same three launches in a form that reads each layer's projection from bit l of a table passed BY VALUE as a __grid_constant__
@@ -339,6 +340,29 @@ cudaError_t launch_render_ao_mixed_layered(const CUtensorMap &low_map, bool use_
 cudaError_t launch_blur_upsample_lin_mixed(const CUtensorMap &lo_depth_map, const CUtensorMap &lo_ao_map, const CUtensorMap *lo_ao2_map, bool use_tma,
                                            const UpsampleArgs &a, const uint8_t *lo_ao2, int lo_a2pitch, const DepthIn &din, int layers,
                                            int sm_count, const LayerProjections &proj, cudaStream_t s);
+
+// ---- device cameras (meao_bind_device_cameras): the camera tables derived on the device, at the head of every frame --------------
+// Layer l's LayerZ entry and its eight LayerRender rows from camera entry l of a device buffer ({near_clip, far_clip, tan_half_fov_h}
+// per layer), with the host planner's arithmetic (camera_tables.cu).  The buffer's contents are read at every launch and every graph
+// replay, so a recorded frame follows the cameras it holds.  status: words {frames that met an invalid camera, its lowest invalid
+// layer, that layer's field (1 near_clip, 2 far_clip, 3 tan_half_fov_h), 0, per launch: the complement of the lowest invalid layer x 4
+// + field (0: none), per launch: the CTAs finished}, all zero at bind time; the last CTA of a launch resets the per-launch two.
+struct CameraTableArgs {
+    const float *cams;      // [layers][3]
+    LayerZ *zb;             // the slot's tables (FrameState::layer_zb / layer_ren)
+    LayerRender *ren;
+    uint32_t *status;       // kCameraStatusWords words
+    int layers;
+    int lw[7];              // the level widths (lw[1..6] are read)
+    int stereo;             // MeaoVariants.single_pass_stereo
+    int reversed_z;
+    int ortho;              // every layer orthographic (no projection table passed)
+    int n;                  // the render stage's sample count: 7 (checker) or 12 (exhaustive)
+    float thick[12];        // SampleThickness in the render stage's call order (frame_record.h kIdxChecker / kIdxExh)
+};
+constexpr int kCameraStatusWords = 6;
+// proj: the layers' projections of a frame that mixes both (nullptr: a.ortho for every layer)
+cudaError_t launch_camera_tables(const CameraTableArgs &a, const LayerProjections *proj, cudaStream_t s);
 
 // ---- debug: synthesise a TiledDepth<k> view (reference layout [16][sh][sw], f16 bits) ----------
 cudaError_t launch_synth_tiled(const float *low, int lw, int lh, int lpitch, int sw, int sh, float pad,
@@ -459,6 +483,11 @@ extern const KernelUnit kPrepareDepthMixedLayeredUnit, kPrepareDepthArrayMixedUn
 #ifndef MEAO_EMULATE
 inline const KernelUnit *const kMixedKernelUnits[] = {&kPrepareDepthMixedLayeredUnit, &kPrepareDepthArrayMixedUnit, &kRenderAoMixedLayeredUnit,
                                                       &kBlurUpsampleLinMixedUnit};
+#endif
+// The device-camera unit (build.py CAMERA_SOURCES), loaded eagerly like the others and kept out of the emulator's unit list the same way.
+extern const KernelUnit kCameraTablesUnit;
+#ifndef MEAO_EMULATE
+inline const KernelUnit *const kCameraKernelUnits[] = {&kCameraTablesUnit};
 #endif
 
 // ---- halo pack / unpack: row blocks of pitched buffers <-> contiguous staging, one launch ------

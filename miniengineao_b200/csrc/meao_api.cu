@@ -59,6 +59,9 @@ struct SizeState : FrameState {
     int slot = 0;                           // the arena slot of this size's camera tables (FrameState::layer_zb / layer_ren)
     bool table_pending = false;             // the slot's tables are not written yet: the next frame writes them on its own stream
     uint64_t plan_gen = 0;                  // the frame-constant generation (MeaoCtx::consts_gen) this size's plan was built at
+    // a host camera changed while a device camera buffer was bound (note_camera_change): the change moved no generation, so this
+    // size's layer_consts still hold the older host cameras, which the constant getters describe -- they plan it again first
+    bool host_cams_stale = false;
 };
 
 }  // namespace
@@ -95,6 +98,11 @@ struct MeaoCtx : SizeState {
     // orthographic entries.
     std::vector<int32_t> layer_proj;
     int layer_proj_ortho = 0;
+    // meao_bind_device_cameras: the bound buffer (cams.cams, nullptr: none) and its capacity in cameras.  A structural input: the frames
+    // run the camera stage (frame_record.h frame_schedule) and take the layered kernels at every layer count.  cams.status: the kernel's
+    // status words, a small allocation of their own made at bind time (nullptr on a plan-only context).
+    DeviceCameras cams;
+    int cams_capacity = 0;
     bool plan_dirty = true;                 // a structural input changed: the next frame re-plans (replan)
     // Frame constants (include/meao.h): bumped by every change of MeaoParams or of a camera that keeps the Z direction.  A size whose
     // plan_gen is older re-plans its constants on the host (refresh_constants); a graph captured at an older one re-targets (launch_cached).
@@ -152,10 +160,12 @@ struct MeaoCtx : SizeState {
         std::vector<uintptr_t> list = {};
         const void *table = nullptr;
         uint64_t proj = 0;                  // FrameState::proj_key: the layers' projections the graph was recorded with
+        const void *cams = nullptr;         // the device camera buffer the graph's camera stage reads (nullptr: none)
         bool operator<(const GraphKey &o) const {
         for (int i = 0; i < 4; i++) if (p[i] != o.p[i]) return p[i] < o.p[i];
         if (kind != o.kind) return kind < o.kind;
         if (proj != o.proj) return proj < o.proj;
+        if (cams != o.cams) return cams < o.cams;
         for (int i = 0; i < 4; i++) if (pitch[i] != o.pitch[i]) return pitch[i] < o.pitch[i];
         for (int i = 0; i < 4; i++) if (size[i] != o.size[i]) return size[i] < o.size[i];
         if (table != o.table) return table < o.table;
@@ -217,10 +227,17 @@ int refuse_ortho_layer_band(MeaoCtx *c, const char *what)
     return fail(c, MEAO_ERR_UNSUPPORTED, "%s: row bands and the halo exchange are not supported with an orthographic layer "
                 "(meao_set_layer_projections)", what);
 }
+// And a bound device camera buffer too: the band paths run the single-image kernels, which read the camera from their arguments.
+int refuse_device_cameras_band(MeaoCtx *c, const char *what)
+{
+    return fail(c, MEAO_ERR_UNSUPPORTED, "%s: row bands and the halo exchange are not supported while a device camera buffer is bound "
+                "(meao_bind_device_cameras)", what);
+}
 #define BAND_GUARD(c, what) do { if ((c) && (c)->layers > 1) return refuse_layered((c), (what)); \
     if ((c) && ((c)->res_w > 0 || (c)->res_layers > 0)) return refuse_reserved((c), (what)); \
     if ((c) && (c)->projection != MEAO_PROJECTION_PERSPECTIVE) return refuse_ortho_band((c), (what)); \
-    if ((c) && (c)->layer_proj_ortho > 0) return refuse_ortho_layer_band((c), (what)); } while (0)
+    if ((c) && (c)->layer_proj_ortho > 0) return refuse_ortho_layer_band((c), (what)); \
+    if ((c) && (c)->cams.cams) return refuse_device_cameras_band((c), (what)); } while (0)
 #define CUDA_TRY(c, expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) \
     return fail((c), MEAO_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); } while (0)
 
@@ -246,9 +263,15 @@ inline int layer_projection(const MeaoCtx *c, int l) { return c->layer_proj.empt
 inline int ctx_reversed_z(const MeaoCtx *c) { return c->layer_cams.empty() ? c->camera.reversed_z : c->layer_cams[0].reversed_z; }
 
 // A change of the cameras in effect.  Their near and far planes and fields of view are frame constants; their Z direction selects
-// kernel instantiations (prepare_slot), so a change of it re-plans like any structural input.
+// kernel instantiations (prepare_slot), so a change of it re-plans like any structural input.  While a device camera buffer is bound the
+// planes and fields of view are the buffer's: a host change that keeps the Z direction is only recorded, for after the unbind.
 void note_camera_change(MeaoCtx *c, int old_reversed_z, int new_reversed_z)
 {
+    if (c->cams.cams && old_reversed_z == new_reversed_z) {
+        c->host_cams_stale = true;
+        for (auto &slot : c->size_slots) slot.s.host_cams_stale = true;
+        return;
+    }
     c->frame_gen++;
     if (old_reversed_z != new_reversed_z) c->plan_dirty = true;
     else c->consts_gen++;
@@ -357,6 +380,7 @@ void build_plan(MeaoCtx *c)
     }
     c->plan_dirty = false;
     c->plan_gen = c->consts_gen;
+    c->host_cams_stale = false;
 }
 
 // Caller must have made c->device current (ensure_ready / meao_resize / meao_destroy do).
@@ -588,6 +612,9 @@ int write_tables(MeaoCtx *c, cudaStream_t s)
         c->views_pending = false;
     }
     if (!c->table_pending) return 0;
+    // a bound device camera buffer: every frame's camera stage derives the tables, and the later calls of a staged frame read the ones
+    // meao_stage_downsample derived -- the host cameras' tables must not land over them
+    if (c->cams.cams) { c->table_pending = false; return 0; }
     std::vector<LayerZ> zb;
     std::vector<LayerRender> ren;
     camera_tables(*c, zb, ren);
@@ -675,6 +702,9 @@ int ensure_ready(MeaoCtx *c, cudaStream_t s = nullptr, bool *capturing = nullptr
 // stage call, so that each sees the tables of the constants set before it was issued.  *capturing (optional): s is being captured.
 int frame_ready(MeaoCtx *c, cudaStream_t s, bool *capturing = nullptr)
 {
+    if (c && c->cams.cams && c->layers > c->cams_capacity)
+        return fail(c, MEAO_ERR_INVALID, "the frame has %d layers and the bound device camera buffer holds %d cameras (meao_bind_device_cameras)",
+                    c->layers, c->cams_capacity);
     bool cap = false;
     int rc = ensure_ready(c, s, capturing ? capturing : &cap);
     return rc ? rc : write_tables(c, s);
@@ -695,10 +725,11 @@ int forced_render_tile()
 // goes through record_downsample, which checks the depth kind first.
 int record_launch(MeaoCtx *c, const FrameLaunch &l, const FrameIO &io, cudaStream_t s)
 {
-    static const char *nvtx[4] = {"meao::prepare_depth", "meao::render_ao", "meao::render_ao_wide", "meao::blur_upsample"};
+    static const char *nvtx[5] = {"meao::prepare_depth", "meao::render_ao", "meao::render_ao_wide", "meao::blur_upsample", "meao::camera_tables"};
     if (l.stage == kStageUpsample && l.level == 1 && !io.batch) c->last_out = io.aio ? const_cast<void *>(io.aio->ao_array) : io.ao;
     NvtxRange nv(nvtx[l.stage]);
-    if (io.batch) CUDA_TRY(c, launch_entry_batch(*c, l, io, forced_render_tile(), s));
+    if (l.stage == kStageCamera) CUDA_TRY(c, io.cams ? launch_cameras(*c, *io.cams, s) : cudaErrorInvalidValue);
+    else if (io.batch) CUDA_TRY(c, launch_entry_batch(*c, l, io, forced_render_tile(), s));
     else if (!c->layer_ortho.empty()) CUDA_TRY(c, launch_entry_mixed(*c, l, io, forced_render_tile(), s));
     else CUDA_TRY(c, c->plan.orthographic ? launch_entry_ortho(*c, l, io, forced_render_tile(), s) : launch_entry_views(*c, l, io, forced_render_tile(), s));
     c->launches++;
@@ -711,6 +742,7 @@ FrameIO frame_io(MeaoCtx *c, const void *depth, int kind, void *ao_out, bool fus
 {
     FrameIO io;
     io.kind = kind; io.depth = depth_in(*c, depth, kind, vp); io.low_only = io.fused = fused; io.ao = ao_out; io.vp = vp;
+    io.cams = c->cams.cams ? &c->cams : nullptr;
     return io;
 }
 
@@ -735,6 +767,12 @@ int record_downsample(MeaoCtx *c, const void *depth, int kind, cudaStream_t s, b
     io.low_only = low_only;
     return record_downsample(c, io, s);
 }
+// The camera stage alone (a bound device camera buffer), ahead of a stage call's prepare and of the AO regeneration
+int record_cameras(MeaoCtx *c, cudaStream_t s)
+{
+    if (!c->cams.cams) return 0;
+    return record_launch(c, FrameLaunch{kStageCamera, 0, 0, -1, kPdlNever}, frame_io(c, nullptr, c->last_kind, nullptr, false), s);
+}
 // PushRenderCommands, AO.cs:660-748.  wide = false: the call AmbientOcclusion.cs makes (tiled source, kernel main_interleaved);
 // wide = true: the same recorder for the non-tiled source LowDepth<k> (kernel main) -> HighQuality<k>.
 int record_render(MeaoCtx *c, int k, int kind, cudaStream_t s, bool wide = false)
@@ -758,7 +796,7 @@ struct PdlScope { bool prev; explicit PdlScope(bool on) : prev(g_launch_pdl) { g
 // resources that the neighbour band's kernels may need: see DESIGN.md 4), so the first launch goes without PDL.
 int record_frame_dag(MeaoCtx *c, const FrameIO &io, cudaStream_t s, size_t first, int pdl, bool after_exchange = false)
 {
-    const std::vector<FrameLaunch> sched = frame_schedule(c->plan.variants);
+    const std::vector<FrameLaunch> sched = frame_schedule(c->plan.variants, c->cams.cams != nullptr);
     const cudaStream_t st[4] = {s, c->branch[0], c->branch[1], c->branch[2]};
     std::vector<int> ev(sched.size(), -1);          // the event (of c->ev) recorded after launch i, if one waits for it: at most 4
     int nev = 0;
@@ -783,7 +821,7 @@ int record_frame_dag(MeaoCtx *c, const FrameIO &io, cudaStream_t s, size_t first
 // pair around every launch (meao_profile_frame), each launched profile_repeats times.
 int record_frame(MeaoCtx *c, const FrameIO &io, cudaStream_t s, size_t first, bool profile)
 {
-    const std::vector<FrameLaunch> sched = frame_schedule(c->plan.variants);
+    const std::vector<FrameLaunch> sched = frame_schedule(c->plan.variants, c->cams.cams != nullptr);
     std::vector<cudaEvent_t> ev;
     auto mark = [&]() { if (profile) { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, s); ev.push_back(e); } };
     const int reps = profile ? c->profile_repeats : 1;         // every kernel is idempotent (out of place), so repeating it is harmless
@@ -811,7 +849,8 @@ int own_ao(MeaoCtx *c, int id, cudaStream_t s)
 {
     if (id != MEAO_BUF_AMBIENT_OCCLUSION || !c->last_out) return 0;
     const int64_t before = c->launches;
-    const int rc = record_upsample(c, 1, nullptr, s);
+    int rc = record_cameras(c, s);
+    if (!rc) rc = record_upsample(c, 1, nullptr, s);
     c->launches = before;
     return rc;
 }
@@ -903,6 +942,7 @@ int meao_create(const MeaoDeviceCfg *cfg, MeaoCtx **out)
             for (const KernelUnit *u : kOrthoKernelUnits) u->walk(&pe);
             for (const KernelUnit *u : kBatchKernelUnits) u->walk(&pe);
             for (const KernelUnit *u : kMixedKernelUnits) u->walk(&pe);
+            for (const KernelUnit *u : kCameraKernelUnits) u->walk(&pe);
             if (pe != cudaSuccess) { cudaGetLastError(); meao_destroy(c); return fail(nullptr, MEAO_ERR_CUDA, "loading the kernels failed: %s", cudaGetErrorString(pe)); }
             preloaded[dev] = true;
         }
@@ -936,6 +976,7 @@ void meao_destroy(MeaoCtx *c)
     for (auto e : c->slot_done) if (e) cudaEventDestroy(e);
     if (c->compute_done) cudaEventDestroy(c->compute_done);
     if (c->host_error) cudaFreeHost(c->host_error);
+    if (c->cams.status) cudaFree(c->cams.status);
     delete c;
 }
 
@@ -1518,6 +1559,7 @@ static int launch_cached(MeaoCtx *c, const MeaoCtx::GraphKey &key_in, cudaStream
     MeaoCtx::GraphKey key = key_in;
     key.size[0] = c->W; key.size[1] = c->H; key.size[2] = c->slot; key.size[3] = c->layers;
     key.proj = c->proj_key;
+    key.cams = c->cams.cams;
     auto it = c->graphs.find(key);
     bool retiring = false;
     if (it == c->graphs.end() || it->second.gen != c->plan_gen) {
@@ -2300,6 +2342,7 @@ int meao_render_batch(MeaoCtx *c, const void *const *depth, const int64_t *depth
 int meao_render_host_async(MeaoCtx *c, const void *depth_host, int32_t kind, uint8_t *ao_host, int32_t slot)
 {
     int rc = ensure_ready(c); if (rc) return rc;
+    if (c->cams.cams && c->layers > c->cams_capacity) return frame_ready(c, c->stream);     // refused before the staging copy
     if (!depth_host || !ao_host) return fail(c, MEAO_ERR_INVALID, "depth / ao_out is NULL");
     if (slot != 0 && slot != 1) return fail(c, MEAO_ERR_INVALID, "slot must be 0 or 1");
     const size_t rows = (size_t)(c->band1 - c->band0) * c->layers;      // layered: L images of H rows (no band)
@@ -2356,6 +2399,8 @@ int meao_stage_downsample(MeaoCtx *c, const void *depth, int32_t kind, void *str
 {
     int rc = frame_ready(c, (cudaStream_t)stream); if (rc) return rc;
     if (!depth) return fail(c, MEAO_ERR_INVALID, "depth is NULL");
+    if (kind < MEAO_DEPTH_RAW_F32 || kind > MEAO_DEPTH_RAW_D24S8) return fail(c, MEAO_ERR_INVALID, "bad depth kind %d", kind);
+    if ((rc = record_cameras(c, (cudaStream_t)stream))) return rc;      // the later stage calls read the tables it derives
     return record_downsample(c, depth, kind, (cudaStream_t)stream);
 }
 
@@ -2398,11 +2443,19 @@ int meao_get_buffer(MeaoCtx *c, int32_t id, void *host_out, size_t host_bytes)
     if (host_bytes < need) return fail(c, MEAO_ERR_INVALID, "buffer %d needs %zu bytes, got %zu", id, need, host_bytes);
     CUDA_TRY(c, cudaDeviceSynchronize());     // debug path: frames may be in flight on any caller stream
     if (b.slices == 16) {
+        const int k = b.level - 2;
+        // a bound device camera buffer: each layer's padding value is the one its last frame derived, read back from the table slot
+        std::vector<float> pads;
+        if (c->cams.cams) {
+            pads.resize(c->layers);
+            CUDA_TRY(c, cudaMemcpy2D(pads.data(), sizeof(float), &c->layer_ren[(size_t)2 * (k - 1) * c->layers].pad, sizeof(LayerRender),
+                                     sizeof(float), c->layers, cudaMemcpyDeviceToHost));
+        }
         __half *tmp = nullptr;
         CUDA_TRY(c, cudaMalloc(&tmp, need));
         cudaError_t e = cudaSuccess;
         for (int l = 0; l < c->layers && e == cudaSuccess; l++)
-            e = launch_tiled_atlas(*c, b.level - 2, l, c->last_kind, (__half *)((char *)tmp + l * one), c->stream);
+            e = launch_tiled_atlas(*c, k, l, c->last_kind, (__half *)((char *)tmp + l * one), c->stream, pads.empty() ? nullptr : &pads[l]);
         if (e == cudaSuccess) e = cudaMemcpyAsync(host_out, tmp, need, cudaMemcpyDeviceToHost, c->stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
         cudaFree(tmp);
@@ -2421,6 +2474,9 @@ int meao_debug_view(MeaoCtx *c, int32_t id, void *out, void *stream)
     BufferRef b;
     if (!out || !buffer_ref(*c, id, b)) return fail(c, MEAO_ERR_INVALID, "bad buffer id %d / out is NULL", id);
     if (c->band0 != 0 || c->band1 != c->H) return fail(c, MEAO_ERR_UNSUPPORTED, "debug views need a whole-frame context (no row band)");
+    if (b.slices == 16 && c->cams.cams)
+        return fail(c, MEAO_ERR_UNSUPPORTED, "debug view %d: the TiledDepth views take the atlas padding from the host cameras, and a device "
+                                             "camera buffer is bound (meao_bind_device_cameras); meao_get_buffer reads them", id);
     cudaStream_t s = (cudaStream_t)stream;
     if ((rc = own_ao(c, id, s))) return rc;
     for (int l = 0; l < c->layers; l++) {                           // layered: L images, each from its own layer of the source
@@ -2452,6 +2508,9 @@ static int plan_only(MeaoCtx *c)
     if (!c || c->W <= 0) return MEAO_ERR_INVALID;
     if (c->plan_dirty) replan(c);           // the captured graphs are dropped by the next ensure_ready, on c->device
     refresh_constants(c);                   // the tables are written by the next frame, on its stream
+    // a host camera changed while a device camera buffer is bound, without moving the generation: the getters describe the host
+    // cameras, so the plan takes them now (the frames derive their tables on the device and never read these)
+    if (c->host_cams_stale) build_plan(c);
     return 0;
 }
 
@@ -2650,12 +2709,73 @@ void meao_render_event(int event_id)
 
 MeaoRenderEventFunc meao_get_render_event_func(void) { return meao_render_event; }
 
+int meao_bind_device_cameras(MeaoCtx *c, const float *cameras_dev, int32_t capacity)
+{
+    if (!c) return MEAO_ERR_INVALID;
+    if (!c->plan_only && in_open_capture(c))
+        return fail(c, MEAO_ERR_UNSUPPORTED, "meao_bind_device_cameras synchronises the device: not while a capture that holds a frame of this context is open");
+    if (!cameras_dev && capacity == 0) {
+        if (!c->cams.cams) return 0;
+        if (!c->plan_only) {
+            CUDA_TRY(c, cudaSetDevice(c->device));
+            CUDA_TRY(c, cudaDeviceSynchronize());       // frames in flight may still write the status words
+            CUDA_TRY(c, cudaFree(c->cams.status));
+        }
+        c->cams = DeviceCameras{};
+        c->cams_capacity = 0;
+        c->plan_dirty = true;           // the host cameras and the single-image kernels again: re-plan + drop the captured graphs
+        c->frame_gen++;
+        return 1;
+    }
+    if (!cameras_dev) return fail(c, MEAO_ERR_INVALID, "cameras_dev is NULL with capacity %d (NULL unbinds only with capacity 0)", capacity);
+    if (capacity < 1 || capacity > kMaxLayers) return fail(c, MEAO_ERR_INVALID, "capacity %d not in 1..%d", capacity, kMaxLayers);
+    if ((uintptr_t)cameras_dev % alignof(float)) return fail(c, MEAO_ERR_INVALID, "cameras_dev %p is not aligned to a float", (const void *)cameras_dev);
+    if ((c->W > 0 && (c->band0 != 0 || c->band1 != c->H)) || c->peer_base[0] || c->peer_base[1])
+        return fail(c, MEAO_ERR_UNSUPPORTED, "a device camera buffer is not supported with a row band or a neighbour connection "
+                                             "(meao_set_row_band, meao_band_connect)");
+    if (cameras_dev == c->cams.cams && capacity == c->cams_capacity) return 0;
+    if (!c->plan_only) {
+        CUDA_TRY(c, cudaSetDevice(c->device));
+        cudaPointerAttributes at{};
+        if (cudaPointerGetAttributes(&at, cameras_dev) != cudaSuccess || (at.type != cudaMemoryTypeDevice && at.type != cudaMemoryTypeManaged) ||
+            at.device != c->device) {
+            cudaGetLastError();
+            return fail(c, MEAO_ERR_INVALID, "cameras_dev %p is not device memory of device %d", (const void *)cameras_dev, c->device);
+        }
+        CUDA_TRY(c, cudaDeviceSynchronize());           // frames in flight may still read the old buffer and write the status words
+        if (!c->cams.status) CUDA_TRY(c, cudaMalloc(&c->cams.status, kCameraStatusWords * sizeof(uint32_t)));
+        CUDA_TRY(c, cudaMemset(c->cams.status, 0, kCameraStatusWords * sizeof(uint32_t)));     // kernels.h CameraTableArgs
+    }
+    sample_thickness(c->cams.thick);
+    c->cams.cams = cameras_dev;
+    c->cams_capacity = capacity;
+    c->plan_dirty = true;               // the camera stage and the layered kernels at every layer count: re-plan + drop the captured graphs
+    c->frame_gen++;
+    return 1;
+}
+
+int meao_device_camera_status(const MeaoCtx *cc, int32_t out4[4])
+{
+    MeaoCtx *c = const_cast<MeaoCtx *>(cc);
+    if (!c || !out4) return MEAO_ERR_INVALID;
+    if (!c->cams.cams) return fail(c, MEAO_ERR_INVALID, "no device camera buffer is bound (meao_bind_device_cameras)");
+    uint32_t w[4] = {0, 0, 0, 0};
+    if (c->cams.status) {
+        CUDA_TRY(c, cudaSetDevice(c->device));
+        // a dedicated non-blocking stream, like meao_band_status: never waits for (or delays) the frames in flight
+        CUDA_TRY(c, cudaMemcpyAsync(w, c->cams.status, sizeof w, cudaMemcpyDeviceToHost, c->slot_stream[1]));
+        CUDA_TRY(c, cudaStreamSynchronize(c->slot_stream[1]));
+    }
+    out4[0] = (int32_t)w[0]; out4[1] = (int32_t)w[1]; out4[2] = (int32_t)w[2]; out4[3] = 0;
+    return MEAO_OK;
+}
+
 int64_t meao_launch_count(const MeaoCtx *c) { return c ? c->launches : 0; }
 int64_t meao_frame_generation(const MeaoCtx *c) { return c ? c->frame_gen : MEAO_ERR_INVALID; }
 int meao_pdl_level(const MeaoCtx *c) { return c ? c->pdl_level : -1; }
 int meao_kernels_per_frame(const MeaoCtx *c)
 {
-    return (int)frame_schedule(c ? c->variants : MeaoVariants{}).size();        // as set: the plan may not be rebuilt yet
+    return (int)frame_schedule(c ? c->variants : MeaoVariants{}, c && c->cams.cams).size();     // as set: the plan may not be rebuilt yet
 }
 
 int64_t meao_algorithmic_bytes(const MeaoCtx *c, int32_t stage)
