@@ -64,11 +64,12 @@ void syncthreads();
 void *dynamic_smem();
 [[noreturn]] void unsupported(const char *what);
 extern long long tma_box_loads;      // number of emulated cp.async.bulk.tensor loads so far (tests assert the TMA branch really ran)
-// The launch ledger: per kernel launched since the last reset, its address relative to the library's load base, its launch count
-// and the TMA box loads issued during its launches.  The emulated MEAO_LAUNCH (kernels.h) reports each kernel through note_launch
+// The launch ledger: per kernel launched since the last reset, its address relative to the library's load base, its launch count,
+// the TMA box loads issued during its launches and the CTAs of their grids (a persistent upsample grid is one wave of CTAs whatever
+// its tile count; any other grid has one CTA per tile).  The emulated MEAO_LAUNCH (kernels.h) reports each kernel through note_launch
 // just before its launch.  ledger_read fills up to cap entries and returns the number of kernels.
 void ledger_reset();
-int ledger_read(unsigned long long *offset, long long *launches, long long *tma_loads, int cap);
+int ledger_read(unsigned long long *offset, long long *launches, long long *tma_loads, long long *ctas, int cap);
 }
 inline void __syncthreads() { meao_emu::syncthreads(); }
 

@@ -75,7 +75,7 @@ def lib() -> C.CDLL:
         l.frame_cams_tables.argtypes = [P, P, P]
         l.frame_cams_clobber.argtypes = [P, I]
         l.frame_cams_derive.argtypes = [P, P, P]
-        l.frame_cams_run.argtypes = [P, P, P, P, I, I, P]
+        l.frame_cams_run.argtypes = [P, P, P, P, I, I, P, I]
         l.frame_cams_tiled.argtypes = [P, I, I, I, P]
         l.frame_cams_kernel_unit.argtypes = [C.c_char_p]
         _lib = l
@@ -123,16 +123,17 @@ def derive(f: emu.Frame, cams: np.ndarray, status: np.ndarray) -> None:
     assert rc == 0, f"the camera launch failed ({rc})"
 
 
-def run(f: emu.Frame, cams: np.ndarray, status: np.ndarray, depth: np.ndarray, *, fused: bool = True) -> None:
+def run(f: emu.Frame, cams: np.ndarray, status: np.ndarray, depth: np.ndarray, *, fused: bool = True, ren_tile: int = -1) -> None:
     """A whole bound frame (the camera stage, then the schedule with the layered kernels at every layer count).  fused: meao_render's
-    frame, AO into a tight array of the caller's (f.buffer(17)); otherwise the stage API's frame.  depth [H, W] or [layers, H, W]."""
+    frame, AO into a tight array of the caller's (f.buffer(17)); otherwise the stage API's frame.  depth [H, W] or [layers, H, W].
+    ren_tile: -1 the planner's rule; 0 / 1 / 2 force 64x32 / 64x16 / 64x8 render tiles."""
     c = np.ascontiguousarray(cams, np.float32)
     d = emu._aligned(np.ascontiguousarray(depth))
     assert d.shape == f._shape(d)
     ao = emu._aligned(np.zeros((f.layers, f.H, f.W), np.uint8)) if fused else None
     f._ao, f._keep = ao, (c, d, ao)
     rc = lib().frame_cams_run(f._h, c.ctypes.data, status.ctypes.data, d.ctypes.data, f._kind(d), int(fused),
-                              None if ao is None else ao.ctypes.data)
+                              None if ao is None else ao.ctypes.data, ren_tile)
     assert rc == 0, f"a launch failed ({rc})"
 
 
@@ -152,3 +153,23 @@ def kernel_unit() -> tuple:
     name = C.create_string_buffer(32)
     n = lib().frame_cams_kernel_unit(name)
     return name.value.decode(), n
+
+
+_symbols: dict | None = None
+
+
+def _kernel_symbols() -> dict:
+    global _symbols
+    if _symbols is None:
+        _symbols = emu.library_symbols(lib()._name)
+    return _symbols
+
+
+def kernels() -> set:
+    """The name of every kernel this library builds (camera_tables_kernel, camera_tables_mixed_kernel)."""
+    return set(_kernel_symbols().values())
+
+
+def ledger() -> dict:
+    """This library's kernels in the emulator's launch ledger since its last reset: {name: (launches, TMA box loads, CTAs)}."""
+    return emu.unit_ledger(_kernel_symbols())

@@ -55,7 +55,7 @@ def lib() -> C.CDLL:
         l.frame_kernel_units.argtypes = [P, P, I]
         l.frame_tma_box_loads.restype = LL
         l.frame_surface_accesses.restype = LL
-        l.frame_ledger_read.argtypes = [P, P, P, I]
+        l.frame_ledger_read.argtypes = [P, P, P, P, I]
         _lib = l
     return _lib
 
@@ -335,14 +335,38 @@ def ledger_reset() -> None:
     lib().frame_ledger_reset()
 
 
+def _ledger() -> dict:
+    """{library-relative kernel address: (launches, TMA box loads issued during them, CTAs of their grids)} since ledger_reset()."""
+    cap = 256
+    off, n_launch, n_tma, n_cta = (C.c_ulonglong * cap)(), (C.c_longlong * cap)(), (C.c_longlong * cap)(), (C.c_longlong * cap)()
+    n = lib().frame_ledger_read(off, n_launch, n_tma, n_cta, cap)
+    assert 0 <= n <= cap
+    return {off[i]: (n_launch[i], n_tma[i], n_cta[i]) for i in range(n)}
+
+
 def kernel_ledger() -> dict:
     """The kernels launched since ledger_reset() in this process: {name: (launches, TMA box loads issued during them)}."""
-    cap = 256
-    off, n_launch, n_tma = (C.c_ulonglong * cap)(), (C.c_longlong * cap)(), (C.c_longlong * cap)()
-    n = lib().frame_ledger_read(off, n_launch, n_tma, cap)
-    assert 0 <= n <= cap
     names = _kernel_symbols()
-    return {names.get(off[i], hex(off[i])): (n_launch[i], n_tma[i]) for i in range(n)}
+    return {names.get(off, hex(off)): e[:2] for off, e in _ledger().items()}
+
+
+def library_symbols(path: str) -> dict:
+    """library-relative address -> 'name<template args>' of every kernel of the library at `path` (one nm run)."""
+    out = subprocess.run(["nm", "-C", "--defined-only", path], capture_output=True, text=True, check=True).stdout
+    syms = {}
+    for line in out.splitlines():
+        parts = line.split(" ", 2)
+        m = _KERNEL.fullmatch(parts[2]) if len(parts) == 3 and parts[1] in "tT" else None
+        if m:
+            syms[int(parts[0], 16)] = m.group(1)
+    return syms
+
+
+def unit_ledger(names: dict) -> dict:
+    """The ledger entries of one library's kernels (`names`: its library_symbols): {name: (launches, TMA box loads, CTAs)}.  The
+    ledger keys a kernel by its address relative to its own library, so the libraries' kernels must not share an offset
+    (tests/test_unit_matrix_emulated.py checks that they do not)."""
+    return {names[off]: e for off, e in _ledger().items() if off in names}
 
 
 def composite(ao: np.ndarray, color: np.ndarray, *, rgb: bool, alpha: bool, one_minus: bool) -> np.ndarray:

@@ -21,9 +21,11 @@ ucontext_t g_sched;
 int g_current = -1;
 const std::function<void()> *g_body = nullptr;
 alignas(128) unsigned char g_dynamic_smem[64 * 1024];
-// the launch ledger: kernel address relative to its library's load base -> {launches, TMA box loads issued during them}.  The kernels
-// live in anonymous namespaces and have no dynamic symbols, so the test suite names them from the library's symbol table (nm).
-std::map<uintptr_t, std::pair<long long, long long>> g_ledger;
+// the launch ledger: kernel address relative to its library's load base -> its launches, the TMA box loads issued during them and the
+// CTAs of their grids.  The kernels live in anonymous namespaces and have no dynamic symbols, so the test suite names them from the
+// library's symbol table (nm).
+struct LedgerEntry { long long launches, tma, ctas; };
+std::map<uintptr_t, LedgerEntry> g_ledger;
 uintptr_t g_next_kernel = 0;         // note_launch's kernel, the next launch's (0: none reported)
 
 void trampoline()
@@ -97,19 +99,20 @@ void launch(dim3 grid, dim3 block, size_t dynamic_smem_bytes, const std::functio
     g_body = nullptr;
     g_current = -1;
     if (kernel) {
-        auto &e = g_ledger[kernel];
-        e.first++;
-        e.second += tma_box_loads - tma0;
+        LedgerEntry &e = g_ledger[kernel];
+        e.launches++;
+        e.tma += tma_box_loads - tma0;
+        e.ctas += (long long)grid.x * grid.y * grid.z;
     }
 }
 
 void ledger_reset() { g_ledger.clear(); }
 
-int ledger_read(unsigned long long *offset, long long *launches, long long *tma_loads, int cap)
+int ledger_read(unsigned long long *offset, long long *launches, long long *tma_loads, long long *ctas, int cap)
 {
     int n = 0;
     for (const auto &kv : g_ledger) {
-        if (n < cap) { offset[n] = kv.first; launches[n] = kv.second.first; tma_loads[n] = kv.second.second; }
+        if (n < cap) { offset[n] = kv.first; launches[n] = kv.second.launches; tma_loads[n] = kv.second.tma; ctas[n] = kv.second.ctas; }
         n++;
     }
     return n;

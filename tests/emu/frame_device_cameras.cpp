@@ -105,8 +105,9 @@ int frame_cams_derive(void *h, const float *cams, uint32_t *status)
 
 // One whole bound frame: the schedule with the camera stage first (frame_schedule(variants, true)), every other launch through the
 // launcher libmeao picks for the plan (launch_entry_mixed, launch_entry_ortho or launch_entry) with FrameIO.cams set.  fused and ao as
-// frame_mixed.cpp frame_run_mixed.  Returns the first launch error (a cudaError_t), 0 when every launch was made.
-int frame_cams_run(void *h, const float *cams, uint32_t *status, const void *depth, int kind, int fused, void *ao)
+// frame_mixed.cpp frame_run_mixed.  ren_tile: render_tile_variant's force (-1: the planner's rule).  Returns the first launch error (a
+// cudaError_t), 0 when every launch was made.
+int frame_cams_run(void *h, const float *cams, uint32_t *status, const void *depth, int kind, int fused, void *ao, int ren_tile)
 {
     FrameState &f = *static_cast<FrameState *>(h);
     whole_frame(f);
@@ -118,9 +119,9 @@ int frame_cams_run(void *h, const float *cams, uint32_t *status, const void *dep
     for (const FrameLaunch &l : frame_schedule(f.plan.variants, true)) {
         cudaError_t e;
         if (l.stage == kStageCamera) e = launch_cameras(f, dc, nullptr);
-        else if (!f.layer_ortho.empty()) e = launch_entry_mixed(f, l, io, -1, nullptr);
-        else if (f.plan.orthographic) e = launch_entry_ortho(f, l, io, -1, nullptr);
-        else e = launch_entry(f, l, io, -1, nullptr);
+        else if (!f.layer_ortho.empty()) e = launch_entry_mixed(f, l, io, ren_tile, nullptr);
+        else if (f.plan.orthographic) e = launch_entry_ortho(f, l, io, ren_tile, nullptr);
+        else e = launch_entry(f, l, io, ren_tile, nullptr);
         if (e != cudaSuccess) return (int)e;
     }
     return 0;

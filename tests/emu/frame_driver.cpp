@@ -340,11 +340,11 @@ int frame_kernel_units(char *names, int *counts, int cap)
 long long frame_tma_box_loads() { return meao_emu::tma_box_loads; }
 long long frame_surface_accesses() { return meao_emu::surface_accesses; }
 
-// the launch ledger (cuda_emu.h): which kernels ran since the reset, how often, and with how many TMA box loads
+// the launch ledger (cuda_emu.h): which kernels ran since the reset, how often, with how many TMA box loads and over how many CTAs
 void frame_ledger_reset() { meao_emu::ledger_reset(); }
-int frame_ledger_read(unsigned long long *offset, long long *launches, long long *tma_loads, int cap)
+int frame_ledger_read(unsigned long long *offset, long long *launches, long long *tma_loads, long long *ctas, int cap)
 {
-    return meao_emu::ledger_read(offset, launches, tma_loads, cap);
+    return meao_emu::ledger_read(offset, launches, tma_loads, ctas, cap);
 }
 
 // aborts (on purpose) with the emulated TMA's alignment complaint: an f32 box starting at x = 3

@@ -79,6 +79,13 @@ def lib() -> C.CDLL:
     return _lib
 
 
+def _note_kind(frame: emu.Frame, dtype) -> None:
+    """The emulator's driver pads its tiled debug views by the ingest kind of the last prepare it ran (as libmeao does by the last
+    frame's): one low-only prepare of a zero depth of this kind tells it.  The table frame then rewrites every intermediate."""
+    zero = np.zeros((frame.layers, frame.H, frame.W), dtype)
+    emu.lib().frame_prepare_low(frame._h, zero.ctypes.data, frame._kind(zero))
+
+
 def run_arrays_views(frame: emu.Frame, depth: np.ndarray, ao: np.ndarray, views, depth_shape: str = "2d", ao_shape: str | None = None) -> None:
     """A layered CUDA-array frame on `frame` with the layer-viewport table `views` (one (depth_x, depth_y, depth_slice, ao_x, ao_y,
     ao_slice) per layer).  depth: the whole emulated depth array [slices, h, w] (float32 / uint16 D16 codes); ao: the whole AO array
@@ -87,6 +94,7 @@ def run_arrays_views(frame: emu.Frame, depth: np.ndarray, ao: np.ndarray, views,
     assert len(views) == frame.layers
     ao_shape = ao_shape or depth_shape
     table = np.ascontiguousarray(np.asarray(views, np.int32).reshape(frame.layers, 6))
+    _note_kind(frame, depth.dtype)
     lib().frame_run_arrays_views(frame._h, depth.ctypes.data, frame._kind(depth), emu.SHAPES[depth_shape], depth.shape[2], depth.shape[1],
                                  depth.shape[0], depth.strides[1], ao.ctypes.data, emu.SHAPES[ao_shape], ao.shape[2], ao.shape[1],
                                  ao.shape[0], ao.strides[1], table.ctypes.data)
@@ -98,6 +106,7 @@ def run_pitched_views(frame: emu.Frame, depth: np.ndarray, depth_pitches, ao: np
     assert depth.flags.c_contiguous and ao.flags.c_contiguous and ao.dtype == np.uint8
     table = np.ascontiguousarray(np.asarray(views, np.int32).reshape(frame.layers, 6))
     frame._keep = (depth, ao, table)
+    _note_kind(frame, depth.dtype)
     lib().frame_run_pitched_views(frame._h, depth.ctypes.data, frame._kind(depth), depth_pitches[0], depth_pitches[1], ao.ctypes.data,
                                   ao_pitches[0], ao_pitches[1], table.ctypes.data)
 
@@ -117,7 +126,7 @@ def _kernel_symbols() -> dict:
     """library-relative address -> 'name<template args>' of every kernel this library builds (one nm run, cached)"""
     global _symbols
     if _symbols is None:
-        out = subprocess.run(["nm", "-C", "--defined-only", _build(build_emu.LIB)], capture_output=True, text=True, check=True).stdout
+        out = subprocess.run(["nm", "-C", "--defined-only", lib()._name], capture_output=True, text=True, check=True).stdout
         _symbols = {}
         for line in out.splitlines():
             parts = line.split(" ", 2)
@@ -137,3 +146,8 @@ def launched() -> set:
     kernel's address relative to its own library, and names only libmeao_emu.so's; the others are named here."""
     names = _kernel_symbols()
     return {names[int(k, 16)] for k in emu.kernel_ledger() if k.startswith("0x") and int(k, 16) in names}
+
+
+def ledger() -> dict:
+    """launched() with each kernel's ledger entry: {name: (launches, TMA box loads issued during them, CTAs of their grids)}."""
+    return emu.unit_ledger(_kernel_symbols())

@@ -145,7 +145,7 @@ def _kernel_symbols() -> dict:
     """library-relative address -> 'name<template args>' of every kernel this library builds (one nm run, cached)"""
     global _symbols
     if _symbols is None:
-        out = subprocess.run(["nm", "-C", "--defined-only", _build(build_emu.LIB)], capture_output=True, text=True, check=True).stdout
+        out = subprocess.run(["nm", "-C", "--defined-only", lib()._name], capture_output=True, text=True, check=True).stdout
         _symbols = {}
         for line in out.splitlines():
             parts = line.split(" ", 2)
@@ -165,3 +165,8 @@ def launched() -> set:
     kernel's address relative to its own library, and names only libmeao_emu.so's; the others are named here."""
     names = _kernel_symbols()
     return {names[int(k, 16)] for k in emu.kernel_ledger() if k.startswith("0x") and int(k, 16) in names}
+
+
+def ledger() -> dict:
+    """launched() with each kernel's ledger entry: {name: (launches, TMA box loads issued during them, CTAs of their grids)}."""
+    return emu.unit_ledger(_kernel_symbols())

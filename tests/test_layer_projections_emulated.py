@@ -1,28 +1,21 @@
-"""CPU tests of the per-layer projection kernels (build.py MIXED_SOURCES) in the emulator (tests/emu/mixed.py): a case matrix of whole
-layered frames whose layers mix both projections -- stage and fused pointer frames and CUDA arrays, tables [P, O] and [O, P, O, O] with
-per-layer cameras, every depth kind and Z direction, plain and premin final upsamples, exhaustive sampling, the high-quality levels and
-every render tile height -- each layer bit-exact on every buffer (ids 1-21) to the perspective oracle or the orthographic oracle
-(tests/ortho_oracle.py), by its projection, and each case launching exactly the mixed kernels its fields name; together the cases launch
-every mixed kernel built.  Hostile depth and the extreme cameras of tests/hostile_cases.py on a mixed table are held to the oracles the
-same way."""
+"""CPU tests of the per-layer projection kernels (build.py MIXED_SOURCES) in the emulator (tests/emu/mixed.py): which tables are mixed,
+and hostile depth and the extreme cameras of tests/hostile_cases.py on a mixed table, each layer held on every buffer to the
+perspective oracle or the orthographic oracle (tests/ortho_oracle.py), by its projection.  The case matrix that launches every mixed
+kernel is tests/unit_matrix.py's, run by test_unit_matrix_emulated.py."""
 import ctypes as C
-import itertools
 
 import numpy as np
 import pytest
 
 import harness
 import hostile_cases as HC
+import unit_matrix as um
 from emu import emu, mixed
 from miniengineao_b200 import Camera
 from miniengineao_b200 import _native as N
 from ortho_oracle import OrthoOracle
 
 P, O = N.MEAO_PROJECTION_PERSPECTIVE, N.MEAO_PROJECTION_ORTHOGRAPHIC
-IN = {"f32": 0, "d16": 1, "d24s8": 2}
-KIND_CODE = {"f32": 0, "linear": 1, "d16": 2, "d24s8": 3}           # MEAO_DEPTH_*
-TILE_H = (32, 16, 8)
-TABLES = {2: [P, O], 4: [O, P, O, O]}
 # (near, far, size): the orthographic half-height (orthographicSize), or the perspective vertical field of view in degrees
 LAYER_CAMS = ((0.5, 80.0, 6.0), (1.0, 300.0, 55.0), (0.1, 20.0, 2.0), (0.3, 150.0, 9.0))
 
@@ -48,104 +41,8 @@ def oracle(cam, linear, **kw):
     return harness.oracle(cam.pixelWidth, cam.pixelHeight, camera=cam, linear=linear, **kw)
 
 
-def _b(v):
-    return "true" if v else "false"
-
-
-def expected(c) -> set:
-    """The mixed kernels case `c` launches, written from its fields: the raw prepare (linear ingest keeps the perspective kernel), the
-    render of every level (wide ones for the hq levels) at the forced tile height, and the fused final upsample of raw depth (premin when
-    level 1 is a high-quality level)."""
-    out = set()
-    raw = c["kind"] != "linear"
-    if raw:
-        if c["form"] == "arrays":
-            out.add(f"prepare_depth_array_mixed_kernel<true, {_b(c['rz'])}, {IN[c['kind']]}>")
-        else:
-            base = "prepare_depth_low_mixed_layered" if c["form"] == "fused" else "prepare_depth_mixed_layered"
-            out.add(f"{base}_kernel<true, {_b(c['rz'])}, {IN[c['kind']]}>")
-    th = TILE_H[c["tile"]]
-    for k in range(1, 5):
-        out.add(f"render_ao_mixed_layered_kernel<0, {_b(c['exh'])}, {th}>")
-        if (c["hq"] >> (k - 1)) & 1:
-            out.add(f"render_ao_mixed_layered_kernel<1, {_b(c['exh'])}, {th}>")
-    if raw and c["form"] == "fused":
-        pre = "premin_" if c["hq"] & 1 else ""
-        out.add(f"blur_upsample_{pre}lin_mixed_kernel<{IN[c['kind']]}, false, true>")
-    return out
-
-
-def _cases():
-    cases = []
-    kinds = list(itertools.product(("f32", "d16", "d24s8", "linear"), (True, False)))
-    for L in (2, 4):
-        for form, exh, hq in (("fused", False, 0), ("stage", True, 15), ("fused", False, 1)):
-            for i, (kind, rz) in enumerate(kinds):
-                cases.append(dict(form=form, L=L, kind=kind, rz=rz, exh=exh, hq=hq, tile=i % 3))
-        for i, (kind, rz) in enumerate(itertools.product(("f32", "d16", "linear"), (True, False))):
-            cases.append(dict(form="arrays", L=L, kind=kind, rz=rz, exh=i % 2 == 1, hq=2 if i < 3 else 0, tile=i % 3))
-    return cases
-
-
-CASES = _cases()
-
-
-def _depth(W, H, L, kind, rz, seed):
-    if kind == "linear":
-        d = harness.contrasting_layers(W, H, L, seed=seed)
-        return d, d
-    r = harness.frames(W, H, L, seed=seed, reversed_z=rz)
-    return harness.ingest(r, kind)
-
-
-@pytest.fixture(scope="module")
-def launched_all():
-    return set()
-
-
-@pytest.mark.parametrize("c", CASES, ids=lambda c: "-".join(f"{k}{v}" for k, v in c.items()))
-def test_case_matrix(c, launched_all):
-    W, H = (150, 70) if c["L"] == 2 else (120, 56)
-    table = TABLES[c["L"]]
-    cams = [camera(W, H, table[l], c["rz"], *LAYER_CAMS[l]) for l in range(c["L"])]
-    plan = plan_context(cams, table, sample_exhaustively=c["exh"], high_quality_mask=c["hq"])
-    f = mixed.frame(plan, table, linear=c["kind"] == "linear")
-    assert mixed.is_mixed(f)
-    d, seen = _depth(W, H, c["L"], c["kind"], c["rz"], seed=c["tile"] + 3 * c["L"])
-    emu.ledger_reset()
-    if c["form"] == "arrays":
-        ao = mixed.run_arrays(f, d, "layered", ren_tile=c["tile"])
-    else:
-        mixed.run(f, d, fused=c["form"] == "fused", ren_tile=c["tile"])
-    got = mixed.launched()
-    assert got == expected(c), (sorted(got ^ expected(c)))
-    launched_all |= got
-    kind = KIND_CODE[c["kind"]]
-    ids = [b for b in harness.buffer_ids(c["hq"]) if not (c["form"] == "arrays" and b == 17)]     # an array frame's AO is the array
-    for l, cam in enumerate(cams):
-        orc = oracle(cam, c["kind"] == "linear", sample_exhaustively=c["exh"], high_quality_mask=c["hq"])
-        orc.run(seen[l])
-        harness.compare_buffers(lambda bid: mixed.buffer(f, bid, l, kind), orc, f"{c} layer {l} ({'O' if cam.orthographic else 'P'})", ids)
-        if c["form"] == "arrays":
-            assert (ao[l] == orc.codes(17)).all(), l
-
-
-def expected_union():
-    u = set()
-    for c in CASES:
-        u |= expected(c)
-    return u
-
-
-def test_cases_launch_every_mixed_kernel(launched_all):
-    if len(launched_all) < len(expected_union()):
-        pytest.skip("the case matrix did not run in this session")
-    assert launched_all == mixed.kernels()
-    assert len(mixed.kernels()) == 34
-
-
 def test_matrix_names_every_kernel_built():
-    assert expected_union() == mixed.kernels()
+    assert set().union(*(um.expected_kernels(c) for c in um.CASES if c.unit == "mixed")) == mixed.kernels()
 
 
 def test_emulator_units_match_libmeao_tables():

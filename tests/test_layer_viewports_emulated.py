@@ -6,8 +6,9 @@ other CPU tests use).  Every array case compares each layer's AO rectangle with 
 tests/emu/frame_views.cpp) of that rectangle and that layer's camera, checks that every AO byte outside the rectangles keeps its
 sentinel, and that the frame makes exactly one surface access per depth texel and per AO byte of its rectangles.  The pointer cases
 (meao_render_pitched) compare each layer with the single-layer fused frame of a tight copy, in every depth format, with one layer
-whose base misses the vector alignment.  Also here: the
-plan-only contract of the table (set, get, clear, refusals, the layer-count reset, meao_frame_generation)."""
+whose base misses the vector alignment.  Also here: the plan-only contract of the table (set, get, clear, refusals, the layer-count
+reset, meao_frame_generation).  The slot cases that launch every table kernel are tests/unit_matrix.py's, run by
+test_unit_matrix_emulated.py."""
 import ctypes as C
 
 import numpy as np
@@ -160,43 +161,6 @@ def test_pitched_quadrants_and_slices(hq):
     table = [(0, 0, 0, 0, 0, 1), (W, 0, 0, W, 0, 1), (3, 1, 1, 1, H + 2, 0), (W + 1, H, 0, 0, 0, 0)]
     _pitched_frame(W, H, table, "raw_f32", depth_row=drow, depth_slice=dsl, ao_row=arow, ao_slice=asl, slices=2, seed=6,
                    high_quality_mask=hq)
-
-
-# ---- every kernel of the table units, by the launch ledger -----------------------------------------------------------------------
-# (io, depth kind, reversed Z, high_quality_mask): together they select every slot of the four units' tables -- the five prepare forms
-# of an array, the seven of a pointer (D24S8 too), both Z directions, and the plain and premin final level of every depth format
-SLOT_CASES = [("arrays", "linear_f32", True, 0), ("arrays", "raw_f32", True, 1), ("arrays", "raw_f32", False, 0),
-              ("arrays", "d16", True, 0), ("arrays", "d16", False, 1),
-              ("pitched", "linear_f32", True, 0), ("pitched", "raw_f32", True, 1), ("pitched", "raw_f32", False, 0),
-              ("pitched", "d16", True, 0), ("pitched", "d16", False, 1), ("pitched", "d24s8", True, 1), ("pitched", "d24s8", False, 0)]
-
-
-def _slot_case(io, kind, reversed_z, hq):
-    W, H = 40, 24
-    table = [(0, 0, 0, 0, 0, 0), (W, 0, 0, W, 0, 0)]
-    if io == "arrays":
-        _table_frame(W, H, table, kind, depth_shape="2d", depth_ext=(1, H, 2 * W), ao_shape="2d", ao_ext=(1, H, 2 * W), seed=7,
-                     reversed_z=reversed_z, high_quality_mask=hq)
-    else:
-        _pitched_frame(W, H, table, kind, depth_row=2 * W, depth_slice=2 * W * H, ao_row=2 * W, ao_slice=2 * W * H, slices=1, seed=7,
-                       reversed_z=reversed_z, high_quality_mask=hq)
-
-
-@pytest.mark.parametrize("io,kind,reversed_z,hq", SLOT_CASES)
-def test_slot_case_matches_the_single_layer_frames(io, kind, reversed_z, hq):
-    _slot_case(io, kind, reversed_z, hq)
-
-
-def test_the_slot_cases_launch_every_table_kernel():
-    """The launch ledger of the cases above holds every kernel the table units build, and nothing else of theirs"""
-    built = layer_views.kernels()
-    assert len(built) == 20, sorted(built)
-    ran = set()
-    for c in SLOT_CASES:
-        emu.ledger_reset()
-        _slot_case(*c)
-        ran |= layer_views.launched()
-    assert ran == built, sorted(built - ran)
 
 
 # ---- the table on plan-only contexts ---------------------------------------------------------------------------------------
