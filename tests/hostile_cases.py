@@ -159,9 +159,11 @@ def camera(name: str, W: int, H: int, reversed_z: bool):
 
 # ---- parameters ---------------------------------------------------------------------------------------------------------------
 # upsample_tolerance -16.55 / -16.56 put 10^x on either side of 2^-55; 0 and +20 (10^20 >= 2^60) on either side of the top;
-# noise_filter_tolerance 15.65 / 15.66 put noise_filter_strength on either side of 2^-52
+# noise_filter_tolerance 15.65 / 15.66 put noise_filter_strength on either side of 2^-52; -37 (10^-37, still a normal float) makes the
+# weight sum of a flat neighbourhood 16 / tol = 1.6e38, whose reciprocal is subnormal: a fast division there flushes it to zero
 PARAMS = [
     dict(upsample_tolerance=-16.55), dict(upsample_tolerance=-16.56), dict(upsample_tolerance=0.0), dict(upsample_tolerance=20.0),
+    dict(upsample_tolerance=-37.0),
     dict(noise_filter_tolerance=15.65), dict(noise_filter_tolerance=15.66),
     dict(blur_tolerance=1.0), dict(blur_tolerance=-30.0),
     dict(thickness_modifier=1e-6), dict(thickness_modifier=1e6), dict(intensity=100.0),

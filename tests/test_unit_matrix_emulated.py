@@ -7,11 +7,17 @@ intermediate, ids 1-21.  In the TMA-fed cases every render and upsample kernel t
 the interior tiles ran too.  In the tile-loop cases (MEAO_UPS_PERSIST_MIN_WAVES tiny) the final upsample's grid must be the one wave
 of the persistent loop, not one CTA per tile: the emulator runs its CTAs in turn, so the first walks every tile of every layer and the
 last re-arms the counters for the next of the three frames.  The matrix as a whole names all 140 kernels of the five units, feeds
-every render and upsample kernel among them TMA boxes and runs every final upsample kernel through the tile loop."""
+every render and upsample kernel among them TMA boxes and runs every final upsample kernel through the tile loop.
+
+The hostile cases run the same way on the depth of tests/hostile_cases.py, with the NaN rule documented there for the float buffers.
+A case with tolerance overrides first checks that its plan lands on the side of upsample_fast_div_ok it was chosen for.  Their share
+of the matrix must reach all 140 kernels, meet both sides of fast_div_ok in every unit's final upsample, and run hostile depth through
+the tile loop of every unit and target form that has one."""
 import numpy as np
 import pytest
 
 import harness
+import hostile_cases as HC
 import unit_matrix as um  # noqa: E402  (tests/ is on sys.path via conftest)
 from emu import batch, emu, layer_views, mixed, ortho
 from emu import device_cameras as DC
@@ -33,7 +39,7 @@ def _ledger() -> dict:
 def _render_plan(c):
     cams = c.cameras()
     plan = harness.context(cams[0], layers=c.layers, layer_cameras=cams if c.layers > 1 else None, sample_exhaustively=c.exhaustive,
-                           high_quality_mask=c.hq)
+                           high_quality_mask=c.hq, **dict(c.params))
     if c.unit == "mixed" or (c.unit == "camera" and c.layers > 1):
         plan.perLayerProjection = True
         plan.LateUpdate()
@@ -47,7 +53,14 @@ def _check_layers(c, cams, seen, get, ao=None, tag=""):
         ref = orc.run(seen[l])
         if ao is not None:
             assert np.array_equal(ao[l], ref), f"{tag} layer {l}: the AO differs from the oracle"
-        harness.compare_buffers(lambda bid: get(bid, l), orc, f"{tag} layer {l} ({'O' if cam.orthographic else 'P'})", c.buffer_ids())
+        harness.compare_buffers(lambda bid: get(bid, l), orc, f"{tag} layer {l} ({'O' if cam.orthographic else 'P'})", c.buffer_ids(),
+                                nan_equal=c.hostile)
+
+
+def _check_fast_div_side(c, plan):
+    """A tolerance case tests nothing unless its plan's final upsample levels fall on the side of fast_div_ok it was chosen for."""
+    if c.fast_div_side is not None:
+        assert HC.fast_div_sides(plan) == {c.fast_div_side}, f"{c.id}: the plan is not on the {c.fast_div_side} side of fast_div_ok"
 
 
 # ---- orthographic, mixed and bound-camera frames ------------------------------------------------------------------------------------
@@ -62,9 +75,11 @@ def _render_unit(c):
     else:
         host = [type(cam)(cam.pixelWidth, cam.pixelHeight, nearClipPlane=1.0, farClipPlane=500.0, usesReversedZBuffer=c.reversed_z,
                           **(dict(orthographic=True, orthographicSize=2.0) if cam.orthographic else dict(fieldOfView=70.0))) for cam in cams]
-        plan = harness.context(host[0], layers=c.layers, layer_cameras=host, high_quality_mask=c.hq, sample_exhaustively=c.exhaustive)
+        plan = harness.context(host[0], layers=c.layers, layer_cameras=host, high_quality_mask=c.hq, sample_exhaustively=c.exhaustive,
+                               **dict(c.params))
         plan.perLayerProjection = True
         f = DC.frame(plan, list(c.table), linear=c.linear)
+    _check_fast_div_side(c, plan)
     emu.ledger_reset()
     for n in range(c.frames):
         d, seen = um.depth(c, n)
@@ -180,7 +195,9 @@ TARGET_FRAMES = {("batch", "arrays"): _batch_arrays_frame, ("batch", "pointers")
 def _target_unit(c):
     W, H = c.size
     cams = c.cameras()
-    f = Frame(harness.context(W, H, layers=c.layers, layer_cameras=cams, reversed_z=c.reversed_z, high_quality_mask=c.hq), linear=c.linear)
+    plan = harness.context(W, H, layers=c.layers, layer_cameras=cams, reversed_z=c.reversed_z, high_quality_mask=c.hq, **dict(c.params))
+    _check_fast_div_side(c, plan)
+    f = Frame(plan, linear=c.linear)
     emu.ledger_reset()
     for n in range(c.frames):
         seen, ao = TARGET_FRAMES[(c.unit, c.form)](c, f, cams, n)
@@ -241,3 +258,31 @@ def test_the_libraries_kernels_have_distinct_offsets():
     would be credited to both."""
     tables = [set(m._kernel_symbols()) for m in LIBS.values()] + [set(emu._kernel_symbols())]
     assert sum(map(len, tables)) == len(set().union(*tables))
+
+
+# ---- the hostile cases as a whole ---------------------------------------------------------------------------------------------------
+def test_the_hostile_cases_name_every_kernel_of_the_five_units():
+    hostile = set().union(*(um.expected_kernels(c) for c in um.CASES if c.hostile))
+    assert hostile == _named() and len(hostile) == 140, sorted(_named() - hostile)
+
+
+def test_every_units_final_upsample_meets_both_sides_of_fast_div_ok():
+    sides = {}
+    for c in um.CASES:
+        if c.unit != "camera" and any(k.startswith("blur_upsample") for k in um.expected_kernels(c)):
+            plan = harness.context(*c.size, reversed_z=c.reversed_z, high_quality_mask=c.hq, **dict(c.params))
+            got = HC.fast_div_sides(plan)
+            assert c.fast_div_side is None or got == {c.fast_div_side}, c.id
+            sides.setdefault(c.unit, set()).update(got)
+            if c.fast_div_side is not None:
+                sides.setdefault((c.unit, "premin"), set()).update(got if c.hq & 1 else ())
+    for u in ("ortho", "mixed", "batch", "views"):
+        assert sides[u] == {True, False}, f"{u}: the final upsample meets only the {sides[u]} side of fast_div_ok"
+        assert sides[(u, "premin")] == {True, False}, f"{u}: no premin tolerance case on each side of fast_div_ok"
+
+
+def test_every_unit_and_target_form_with_a_tile_loop_has_a_hostile_loop_case():
+    loops = {(c.unit, c.form) for c in um.CASES if c.persist}
+    hostile = {(c.unit, c.form, c.kind) for c in um.CASES if c.persist and c.hostile}
+    for unit, form in loops:
+        assert {(unit, form, k) for k in ("f32", "d16")} <= hostile, f"{unit} {form}: no hostile tile-loop case in f32 and in D16"

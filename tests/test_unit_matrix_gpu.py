@@ -10,11 +10,18 @@ loop's atomics and barriers with CTAs really in flight together.  A fresh contex
 MEAO_UPS_PERSIST_MIN_WAVES are read when a frame is recorded and a cached graph would keep another case's choice.  The tile-loop cases
 run three frames through one context (half of them replaying a recorded graph), so the counters the last CTA re-arms are used again.
 Last, one frame per unit at a size where the planner chooses the tile loop itself: a 4K orthographic frame, three 1080p layers of
-mixed projections, and three 1080p batch layers as tensors and as CUDA arrays."""
+mixed projections, and three 1080p batch layers as tensors and as CUDA arrays; and the 4K orthographic and 1080p batch frames again on
+hostile depth.
+
+The hostile cases are where a fast-path guard that admits a bad operand shows: the emulator models MUFU.RCP as the correctly rounded
+reciprocal, the H100's is an approximation, and its NaNs are canonical.  They compare their float buffers with the NaN rule of
+tests/hostile_cases.py; a case with tolerance overrides first checks that its context lands on the side of upsample_fast_div_ok it
+was chosen for."""
 import numpy as np
 import pytest
 
 import harness
+import hostile_cases as HC
 import unit_matrix as um  # noqa: E402  (tests/ is on sys.path via conftest)
 from gpu_harness import Array, rt, torch_cuda  # noqa: E402,F401  (the fixtures)
 from miniengineao_b200 import Camera
@@ -36,7 +43,7 @@ def _tensor(torch, a):
 
 def _context(torch, c, use_graph=True):
     cams = c.cameras()
-    kw = dict(device=0, layers=c.layers, sample_exhaustively=c.exhaustive, high_quality_mask=c.hq, use_graph=use_graph)
+    kw = dict(device=0, layers=c.layers, sample_exhaustively=c.exhaustive, high_quality_mask=c.hq, use_graph=use_graph, **dict(c.params))
     if c.unit == "camera":
         # the host cameras are other ones: a bound frame must read the buffer's
         host = [Camera(k.pixelWidth, k.pixelHeight, nearClipPlane=1.0, farClipPlane=500.0, usesReversedZBuffer=c.reversed_z,
@@ -192,6 +199,8 @@ def _run(torch, rt, c, use_graph=True, frames=None, buffers=True):
     W, H = c.size
     ao, cams = _context(torch, c, use_graph)
     try:
+        if c.fast_div_side is not None:
+            assert HC.fast_div_sides(ao) == {c.fast_div_side}, f"{c.id}: the context is not on the {c.fast_div_side} side of fast_div_ok"
         for n in range(frames or c.frames):
             depth, seen = um.depth(c, n)
             run = TARGETS.get((c.unit, c.form)) or FRAMES[c.form]
@@ -204,7 +213,8 @@ def _run(torch, rt, c, use_graph=True, frames=None, buffers=True):
                 bad = int((got[l] != want).sum())
                 assert bad == 0, f"{c.id} frame {n}: the AO of layer {l} differs from the oracle in {bad} pixels"
                 assert int(got[l].astype(np.uint64).sum()) == int(want.astype(np.uint64).sum())
-                harness.compare_buffers(lambda bid: bufs[bid][l] if c.layers > 1 else bufs[bid], ref, f"{c.id} frame {n} layer {l}", ids)
+                harness.compare_buffers(lambda bid: bufs[bid][l] if c.layers > 1 else bufs[bid], ref, f"{c.id} frame {n} layer {l}", ids,
+                                        nan_equal=c.hostile)
     finally:
         ao.close()
 
@@ -223,7 +233,9 @@ def test_case_matches_the_oracle(torch_cuda, rt, case, monkeypatch):
 NATURAL = [um.Case("ortho", "fused", 1, (um.O,), "f32", size=(3840, 2160)),
            um.Case("mixed", "fused", 3, (um.P, um.O, um.P), "d16", size=(1920, 1080)),
            um.Case("batch", "pointers", 3, (um.P,) * 3, "f32", size=(1920, 1080)),
-           um.Case("batch", "arrays", 3, (um.P,) * 3, "d16", hq=1, size=(1920, 1080))]
+           um.Case("batch", "arrays", 3, (um.P,) * 3, "d16", hq=1, size=(1920, 1080)),
+           um.Case("ortho", "fused", 1, (um.O,), "f32", size=(3840, 2160), hostile=True),
+           um.Case("batch", "pointers", 3, (um.P,) * 3, "f32", size=(1920, 1080), hostile=True)]
 
 
 @pytest.mark.parametrize("case", NATURAL, ids=lambda c: c.id.replace("-tile8", ""))

@@ -18,16 +18,26 @@ Three kinds of case:
   tiny, so a CTA walks tiles of different layers and the last CTA's counter re-arm is used by the next frame.  Their layers differ:
   per-layer cameras, mixed projections, targets of their own pitch or misaligned base, viewports at other origins and slices.
 
+And their hostile twins (hostile): the same frames on the depth of tests/hostile_cases.py, each layer salted for its own layer's
+camera, so the fast-path guards of every kernel meet zeros, subnormals, infinities, NaNs and the raw depths where the linearisation's
+denominator crosses zero: a twin of every slot case, of the TMA-fed render cases and of a few tile-loop cases (whose second frame also
+carries a solid hostile block of whole final-level tiles in one layer), the extreme cameras (camera: on layer 0 of a one-layer case,
+on the middle layer of a layered one) and the tolerances either side of upsample_fast_div_ok and far below it (params).  A hostile
+case compares its float buffers with harness.n_diff(nan_equal=True), the rule of tests/hostile_cases.py; AO codes stay exact.
+
 Every case forces the render tile height (kernels.h kRenderTileHs, MEAO_REN_TILE), so the render kernel a case launches does not
 depend on the SM count of the device."""
 from __future__ import annotations
 
-from dataclasses import dataclass
+from dataclasses import dataclass, replace
+
+import numpy as np
 
 from miniengineao_b200 import Camera
 from miniengineao_b200 import _native as N
 
 import harness  # noqa: E402  (tests/ is on sys.path via conftest)
+import hostile_cases as HC  # noqa: E402
 
 P, O = N.MEAO_PROJECTION_PERSPECTIVE, N.MEAO_PROJECTION_ORTHOGRAPHIC
 TILE_H = (32, 16, 8)                # forced render tile variant 0 / 1 / 2
@@ -44,6 +54,16 @@ UNITS = ("ortho", "mixed", "batch", "views", "camera")
 ORTHO_CAMS = ((0.5, 80.0, 6.0), (1.0, 300.0, 25.0), (0.1, 20.0, 2.0))
 MIXED_CAMS = ((0.5, 80.0, 6.0), (1.0, 300.0, 55.0), (0.1, 20.0, 2.0), (0.3, 150.0, 9.0))
 PERSP_CAMS = ((0.3, 100.0, 60.0), (0.1, 1000.0, 90.0), (0.5, 50.0, 40.0))
+HOSTILE_FED = (203, 97)             # ragged: W % 8 == 3, no level a multiple of 4, 16 or 64
+# name -> (near, far, tan_half_fov_h): hostile_cases.CAMERAS with 5 for the default camera's tangent (an orthographic layer's half-width),
+# and a half-width small enough that it_i of the orthographic coarse levels overflows to inf
+HOSTILE_CAMERAS = {name: (n, f, 5.0 if t is None else t) for name, (n, f, t) in HC.CAMERAS.items()}
+HOSTILE_CAMERAS["it_overflows"] = (1.0, 1e30, 1e-10)
+# the MeaoParams overrides of hostile_cases.PARAMS either side of upsample_fast_div_ok -> the side their plan must land on
+FAST_DIV_SIDE = {("upsample_tolerance", -16.55): True, ("upsample_tolerance", -16.56): False, ("upsample_tolerance", 0.0): True,
+                 ("upsample_tolerance", 20.0): False, ("noise_filter_tolerance", 15.65): True, ("noise_filter_tolerance", 15.66): False,
+                 ("upsample_tolerance", -37.0): False}
+SOLID_BLOCK = (slice(32, 96), slice(64, 192))       # 2 x 2 final-level tiles (64 x 32 outputs) of a tile-loop case's layer 0, frame 1
 
 
 @dataclass(frozen=True)
@@ -60,6 +80,9 @@ class Case:
     tile: int = 2                   # forced render tile variant (TILE_H)
     size: tuple = (150, 70)
     persist: bool = False           # the persistent upsample tile loop on every level, FRAMES_PER_LOOP_CASE frames
+    hostile: bool = False           # the depth of tests/hostile_cases.py
+    camera: str = ""                # a HOSTILE_CAMERAS entry on layer 0 (one layer) or the middle layer (layered); the others keep theirs
+    params: tuple = ()              # sorted (name, value) MeaoParams overrides (harness.PARAMS names)
 
     @property
     def id(self) -> str:
@@ -72,6 +95,11 @@ class Case:
         parts += [f"tile{TILE_H[self.tile]}", "x".join(map(str, self.size))]
         if self.persist:
             parts.append("loop")
+        if self.hostile:
+            parts.append("hostile")
+        if self.camera:
+            parts.append(self.camera)
+        parts += [f"{k}={v}" for k, v in self.params]
         return "-".join(parts)
 
     @property
@@ -91,29 +119,52 @@ class Case:
         own_ao = self.unit in ("ortho", "mixed", "camera") and self.form != "arrays"
         return [b for b in harness.buffer_ids(self.hq) if own_ao or b != 17]
 
+    @property
+    def fast_div_side(self):
+        """The side of upsample_fast_div_ok the case's tolerances are chosen for (None: no tolerance override)."""
+        sides = {FAST_DIV_SIDE[p] for p in self.params if p in FAST_DIV_SIDE}
+        assert len(sides) <= 1, self.id
+        return sides.pop() if sides else None
+
     def cameras(self) -> list:
         W, H = self.size
         rz = self.reversed_z
         if self.unit == "ortho":
-            return [Camera(W, H, nearClipPlane=n, farClipPlane=f, usesReversedZBuffer=rz, orthographic=True, orthographicSize=s)
-                    for n, f, s in ORTHO_CAMS[:self.layers]]
-        if self.unit in ("mixed", "camera"):
+            out = [Camera(W, H, nearClipPlane=n, farClipPlane=f, usesReversedZBuffer=rz, orthographic=True, orthographicSize=s)
+                   for n, f, s in ORTHO_CAMS[:self.layers]]
+        elif self.unit in ("mixed", "camera"):
             out = []
             for l, p in enumerate(self.table):
                 n, f, s = MIXED_CAMS[l]
                 out.append(Camera(W, H, nearClipPlane=n, farClipPlane=f, usesReversedZBuffer=rz, orthographic=True, orthographicSize=s)
                            if p == O else Camera(W, H, nearClipPlane=n, farClipPlane=f, usesReversedZBuffer=rz, fieldOfView=s))
-            return out
-        return [Camera(W, H, nearClipPlane=n, farClipPlane=f, fieldOfView=v, usesReversedZBuffer=rz) for n, f, v in PERSP_CAMS[:self.layers]]
+        else:
+            out = [Camera(W, H, nearClipPlane=n, farClipPlane=f, fieldOfView=v, usesReversedZBuffer=rz)
+                   for n, f, v in PERSP_CAMS[:self.layers]]
+        if self.camera:
+            m = 0 if self.layers == 1 else self.layers // 2
+            out[m] = hostile_camera(self.camera, W, H, rz, out[m].orthographic)
+        return out
 
 
-def _ortho(form, L, kind, rz, exh=False, hq=0, tile=2, size=None, persist=False):
-    return Case("ortho", form, L, (O,) * L, kind, rz, exh, hq, tile, size or ((300, 136) if L == 1 else (150, 70)), persist)
+def hostile_camera(name: str, W: int, H: int, rz: bool, orthographic: bool) -> Camera:
+    """HOSTILE_CAMERAS[name] as an orthographic camera (its planes, its tangent as the half-width) or a perspective one
+    (hostile_cases.camera(), or the field of view of the tangent for the cameras hostile_cases has no entry for)."""
+    near, far, t = HOSTILE_CAMERAS[name]
+    if orthographic:
+        return Camera(W, H, nearClipPlane=near, farClipPlane=far, usesReversedZBuffer=rz, orthographic=True, orthographicSize=t / (W / H))
+    if name in HC.CAMERAS:
+        return HC.camera(name, W, H, rz)
+    return Camera(W, H, nearClipPlane=near, farClipPlane=far, usesReversedZBuffer=rz, fieldOfView=HC.fov_for_tan_half_h(t, W, H))
 
 
-def _mixed(form, table, kind, rz, exh=False, hq=0, tile=2, size=None, persist=False):
+def _ortho(form, L, kind, rz, exh=False, hq=0, tile=2, size=None, persist=False, **hostile):
+    return Case("ortho", form, L, (O,) * L, kind, rz, exh, hq, tile, size or ((300, 136) if L == 1 else (150, 70)), persist, **hostile)
+
+
+def _mixed(form, table, kind, rz, exh=False, hq=0, tile=2, size=None, persist=False, **hostile):
     return Case("mixed", form, len(table), tuple(table), kind, rz, exh, hq, tile, size or ((150, 70) if len(table) == 2 else (120, 56)),
-                persist)
+                persist, **hostile)
 
 
 def _cases() -> list:
@@ -155,6 +206,48 @@ def _cases() -> list:
     # ---- device camera tables: a bound camera buffer on an orthographic and on a mixed table
     out.append(Case("camera", "fused", 2, (O, O), "f32", True, hq=1, tile=1, size=(97, 61)))
     out.append(Case("camera", "fused", 3, (P, O, P), "d24s8", False, tile=0, size=LOOP_FED))
+    return out + _hostile_cases(out)
+
+
+def _hostile_cases(ordinary: list) -> list:
+    out = []
+    # ---- hostile twins: every slot case and bound-camera case, every TMA-fed render case, and a tile-loop case of each unit and target
+    # form in f32 and in D16
+    out += [replace(c, hostile=True) for c in ordinary if not c.persist]
+    loops = [c for c in ordinary if c.persist and c.unit != "camera"]
+    for unit, form in dict.fromkeys((c.unit, c.form) for c in loops):
+        for kind in ("f32", "d16"):
+            mine = [c for c in loops if (c.unit, c.form, c.kind) == (unit, form, kind)]
+            out.append(replace(mine[0] if kind == "d16" else mine[-1], hostile=True))   # ortho: one layer in D16, two in f32
+    # ---- the extreme cameras: raw depth through the stage and the fused frame in both Z directions, D16 / D24S8 under the far / near
+    # ratio of 1e7, linear depth under the cameras of extreme tangent; a layered case puts the camera on its middle layer, so the mixed
+    # cases take both orders of a [P, O] table for the camera to meet both projections
+    HF = HOSTILE_FED
+    for i, name in enumerate(HOSTILE_CAMERAS):
+        for rz in (True, False):
+            for form in ("stage", "fused"):
+                out.append(_ortho(form, 1, "f32", rz, hq=9, tile=i % 3, size=HF, hostile=True, camera=name))
+                out += [_mixed(form, t, "f32", rz, hq=9, tile=i % 3, size=HF, hostile=True, camera=name) for t in ((P, O), (O, P))]
+    for kind in ("d16", "d24s8"):
+        for rz in (True, False):
+            out.append(_ortho("fused", 1, kind, rz, size=HF, hostile=True, camera="far_near_1e7"))
+            out += [_mixed("fused", t, kind, rz, size=HF, hostile=True, camera="far_near_1e7") for t in ((P, O), (O, P))]
+    for name in ("tan_half_fov_1em6", "tan_half_fov_1e6", "it_overflows"):
+        out.append(_ortho("fused", 1, "linear", True, exh=True, size=HF, hostile=True, camera=name))
+        out += [_mixed("fused", t, "linear", True, exh=True, size=HF, hostile=True, camera=name) for t in ((P, O), (O, P))]
+    # batches and viewports: every extreme camera on the middle layer, through both target forms
+    for i, name in enumerate(HC.CAMERAS):
+        kind, rz = ("f32", "d16", "linear", "f32", "d16")[i], i % 2 == 0
+        for unit, L, size in (("batch", 3, (61, 37)), ("views", 2, (40, 24))):
+            out += [Case(unit, form, L, (P,) * L, kind, rz, size=size, hostile=True, camera=name)
+                    for form in (("pointers", "arrays") if unit == "batch" else ("pitched", "arrays"))]
+    # ---- the tolerances either side of upsample_fast_div_ok through the fused final level of each unit; one pair of each unit premin
+    for u, make in enumerate((lambda kind, rz, hq, j, **kw: _ortho("fused", 1 + j % 2, kind, rz, hq=hq, tile=j % 3, **kw),
+                              lambda kind, rz, hq, j, **kw: _mixed("fused", (P, O), kind, rz, hq=hq, tile=j % 3, **kw),
+                              lambda kind, rz, hq, j, **kw: Case("batch", "pointers", 3, (P,) * 3, kind, rz, hq=hq, size=(61, 37), **kw),
+                              lambda kind, rz, hq, j, **kw: Case("views", "pitched", 2, (P,) * 2, kind, rz, hq=hq, size=(40, 24), **kw))):
+        for j, p in enumerate(FAST_DIV_SIDE):
+            out.append(make(("f32", "d16", "d24s8")[(j + u) % 3], j % 2 == 0, int(j // 2 == u % 3), j, hostile=True, params=(p,)))
     return out
 
 
@@ -211,6 +304,8 @@ def upsample_kernel(c: Case) -> str:
 def depth(c: Case, frame: int = 0):
     """(the depth of every layer in the case's ingest format [layers, H, W], the float32 the oracle sees); each frame of a tile-loop
     case its own."""
+    if c.hostile:
+        return _hostile_depth(c, frame)
     W, H = c.size
     if c.unit in ("ortho", "mixed", "camera"):
         seed = c.tile + 3 * c.layers + 101 * frame
@@ -225,9 +320,40 @@ def depth(c: Case, frame: int = 0):
     return harness.ingest(harness.raw(lin, reversed_z=c.reversed_z), c.kind)
 
 
+def _hostile_depth(c: Case, frame: int):
+    """Hostile depth of every layer, raw f32 salted with the values where its own layer's linearisation crosses zero (the zbuffer params
+    of that layer's camera, orthographic or perspective); a seed of its own per layer and frame.  Frame 1 (the second frame of a
+    tile-loop case) also fills SOLID_BLOCK of layer 0 with one value -- NaN, +inf, -inf, or the sky code of a UNORM format -- so whole
+    tiles of one layer are hostile while the next layer's are not: a CTA that carries a box, a border or a count from one tile to the
+    next shows."""
+    W, H = c.size
+    ds, seen = [], []
+    for l, cam in enumerate(c.cameras()):
+        seed = 7 * l + 101 * frame + 3 * c.layers + c.tile + 13 * KIND_CODE[c.kind]
+        if c.kind == "linear":
+            d = s = HC.hostile_linear(W, H, seed=seed)
+        elif c.kind == "f32":
+            d = s = HC.hostile_raw(W, H, harness.context(cam).zbuffer_params(), c.reversed_z, seed=seed)
+        else:
+            d, s = HC.hostile_unorm(W, H, 16 if c.kind == "d16" else 24, c.reversed_z, seed=seed)
+        ds.append(d)
+        seen.append(s)
+    d, seen = np.stack(ds), np.stack(seen)
+    if frame == 1:
+        if c.kind in ("f32", "linear"):
+            d[(0,) + SOLID_BLOCK] = seen[(0,) + SOLID_BLOCK] = (np.nan, np.inf, -np.inf)[(c.hq + c.layers + c.reversed_z) % 3]
+        else:
+            full = (1 << (16 if c.kind == "d16" else 24)) - 1
+            code = 0 if c.reversed_z else full                                  # the sky of the Z direction
+            blk = d[(0,) + SOLID_BLOCK]
+            d[(0,) + SOLID_BLOCK] = (blk & ~np.array(full, blk.dtype)) | np.array(code, blk.dtype)
+            seen[(0,) + SOLID_BLOCK] = np.float32(code) * np.float32(1.0 / full)
+    return d, seen
+
+
 def oracle(c: Case, cam, threads=4):
     """The oracle of one layer of case `c` with camera `cam`: the orthographic one for an orthographic camera, else the perspective one."""
-    kw = dict(sample_exhaustively=c.exhaustive, high_quality_mask=c.hq)
+    kw = dict(sample_exhaustively=c.exhaustive, high_quality_mask=c.hq, **dict(c.params))
     if cam.orthographic:
         from ortho_oracle import OrthoOracle
         return OrthoOracle(cam.pixelWidth, cam.pixelHeight, near=cam.nearClipPlane, far=cam.farClipPlane,
