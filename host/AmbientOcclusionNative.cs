@@ -58,6 +58,7 @@ namespace MiniEngineAO
         [DllImport(Lib)] public static extern IntPtr meao_last_error(IntPtr ctx);
         [DllImport(Lib)] public static extern int meao_set_params(IntPtr ctx, ref MeaoParams p);
         [DllImport(Lib)] public static extern int meao_set_variants(IntPtr ctx, ref MeaoVariants v);
+        [DllImport(Lib)] public static extern int meao_set_hierarchy_depth(IntPtr ctx, int levels);
         [DllImport(Lib)] public static extern int meao_set_camera(IntPtr ctx, ref MeaoCamera c);
         [DllImport(Lib)] public static extern int meao_resize(IntPtr ctx, int width, int height);
         // Dynamic resolution: what meao_reservation reports (meao.h MeaoReservation)
@@ -159,6 +160,10 @@ namespace MiniEngineAO
         // ---- not in the reference inspector: the shader variants Render.compute / Upsample.compute ship but AO.cs never selects ----
         [SerializeField] bool _sampleExhaustively;             // Render.compute:144-159, AmbientOcclusion.cs:709-715 (FIXME there)
         [SerializeField, Range(0, 15)] int _highQualityMask;   // bit k-1: Render kernel "main" on level k + Upsample "main_premin*"
+        // The levels of the AO pyramid a frame renders and upsamples (upstream MiniEngine's "Hierarchy Depth"): 4 is the reference's
+        // frame; fewer cost less and drop the coarsest, large-scale darkening.  A change re-plans the plugin (a device synchronise).
+        [SerializeField, Range(1, 4)] int _hierarchyDepth = 4;
+        public int HierarchyDepth { get { return _hierarchyDepth; } set { _hierarchyDepth = value; } }
         // Layered frames (meao_set_layers): views per frame, rendered together -- 2 for the eye slices of a texture-array (instanced)
         // stereo target, 6 for cube-map faces.  The depth and AO buffers the interop layer maps then hold Layers images each.
         [SerializeField, Range(1, 65535)] int _layers = 1;
@@ -256,6 +261,9 @@ namespace MiniEngineAO
                 single_scale = 0                                                             // BASELINE configs[0] plumbing mode; the component never selects it
             };
             rebuild |= MeaoNative.meao_set_variants(_ctx, ref variants) == 1;
+            var depthChanged = MeaoNative.meao_set_hierarchy_depth(_ctx, _hierarchyDepth);              // a structural input, like the variants
+            MeaoNative.Check(_ctx, depthChanged);
+            rebuild |= depthChanged == 1;
             rebuild |= ReserveLayers();                                                      // before meao_set_layers
             var layered = SetLayers(_layers);
             rebuild |= layered == 1;

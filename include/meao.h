@@ -49,7 +49,9 @@ extern "C" {
                               *    + meao_set_layer_projections / meao_get_layer_projections (perspective and orthographic layers in one
                               *      layered frame; additive)
                               *    + meao_bind_device_cameras / meao_device_camera_status (cameras read from device memory at every
-                              *      launch and graph replay; additive) */
+                              *      launch and graph replay; additive)
+                              *    + meao_set_hierarchy_depth / meao_get_hierarchy_depth (render and upsample only the finest 1-4 levels;
+                              *      additive, MeaoVariants unchanged) */
 
 typedef struct MeaoCtx MeaoCtx;
 
@@ -135,7 +137,8 @@ typedef struct {
                                      only, 15 = every level (the quality ladder of the upstream MiniEngine sample, which is not vendored). */
     int32_t single_scale;         /* BASELINE.json configs[0] "single-scale AO": the frame is Downsample1 -> Render level 1 -> the FINAL-style
                                      Upsample (kernel "main", AO.cs:531's dispatch with LoResAO1 = Occlusion1 instead of Combined1): three of
-                                     the ten dispatches of AO.cs:511-531, no coarser level contributes.  Requires high_quality_mask == 0. */
+                                     the ten dispatches of AO.cs:511-531, no coarser level contributes.  Requires high_quality_mask == 0.
+                                     It is the frame of hierarchy depth 1 (meao_set_hierarchy_depth): while set, the depth in effect is 1. */
 } MeaoVariants;
 
 /* ---- lifetime ------------------------------------------------------------------------------ */
@@ -156,7 +159,7 @@ int meao_abi_version(void);
  * arguments (cudaGraphExecUpdate) at its next launch.  Under the ordering contract (meao_reserve) frame n sees the constants set
  * before it was issued, and frame n-1, still in flight, keeps its own.  A host may therefore animate the camera and the
  * parameters every frame.
- * STRUCTURAL INPUTS re-plan with a device synchronise and drop the captured graphs: MeaoVariants, meao_set_layers without a layer
+ * STRUCTURAL INPUTS re-plan with a device synchronise and drop the captured graphs: MeaoVariants, meao_set_hierarchy_depth, meao_set_layers without a layer
  * reservation, a resize without a reservation, meao_reserve, row bands, a change of the cameras' reversed_z (it selects kernel instantiations; it is a
  * platform property) and meao_set_projection.
  * A refused camera, table or parameter block leaves the context exactly as it was. */
@@ -167,6 +170,30 @@ void meao_default_params(MeaoParams *out);          /* AO.cs:20-68 defaults */
 /* Selects the undispatched shader variants above (a structural input); returns 1 if a value changed, 0 if not. */
 int meao_set_variants(MeaoCtx *ctx, const MeaoVariants *variants);
 int meao_get_variants(const MeaoCtx *ctx, MeaoVariants *out);
+/* ---- hierarchy depth: how many levels of the AO pyramid a frame renders and upsamples (upstream MiniEngine's "Hierarchy Depth").
+ * levels = n in 1..4, default 4 (the reference's frame).  A frame of depth n:
+ *   - prepares as at depth 4: LowDepth1..4 (and LinearDepth) are always written;
+ *   - renders levels 1..n, and the wide render of every high_quality_mask bit k <= n.  Mask bits above n launch nothing: they are kept,
+ *     not refused, so that meao_set_variants and this setter may be called in either order;
+ *   - runs n upsamples, lo levels n, n-1, ..., 1.  The first reads Occlusion<n> (and HighQuality<n> when bit n is set) where the depth-4
+ *     frame's lo-level-4 upsample reads Occlusion4; every later one reads the Combined<lo> the one before wrote.  At n = 1 the first
+ *     upsample is the final one, on Occlusion1: the single_scale frame.  With single_scale = 0 and n = 1 a high_quality_mask bit 0 is
+ *     allowed (the premin final upsample on Occlusion1 and HighQuality1).
+ * The depth in effect is MeaoVariants.single_scale ? 1 : levels; meao_get_hierarchy_depth returns `levels` as set.
+ * The kernels are the depth-4 frame's: fewer levels, fewer launches.  meao_kernels_per_frame = 1 + n + (mask bits <= n) + n (+1 with
+ * a bound device camera buffer), meao_algorithmic_bytes counts the renders and upsamples of levels 1..n, and meao_profile_frame lists
+ * the launches of the schedule.  The stage API refuses meao_stage_upsample(lo_level > n) with MEAO_ERR_INVALID; lo_level = n reads
+ * Occlusion<n>.  meao_stage_render is unchanged.
+ * The debug buffers of stages a frame of depth n does not run -- Occlusion<k> and HighQuality<k> for k > n, Combined<k> for k >= n --
+ * have unspecified contents; reading them is not refused.
+ * Every frame form, reservation, capture and row band takes it; a band's halo rows are those of the depth-4 frame.
+ * A structural input, like MeaoVariants: a change re-plans behind a device synchronise, drops the captured graphs and moves
+ * meao_frame_generation, so a host that toggles it every frame pays a re-plan per toggle.  Under a size or layer reservation the arena
+ * stays; the other planned (W, H, L) are forgotten.  Plan-only contexts accept it.
+ * Returns 1 on a change, 0 for the value already set; any value outside 1..4 returns MEAO_ERR_INVALID, names the field in
+ * meao_last_error and changes nothing. */
+int meao_set_hierarchy_depth(MeaoCtx *ctx, int32_t levels);
+int meao_get_hierarchy_depth(const MeaoCtx *ctx);
 /* replaces: CalculateZBufferParams / CalculateTanHalfFovHeight inputs (AO.cs:561-573).  A frame constant, except reversed_z;
  * returns MEAO_OK. */
 int meao_set_camera(MeaoCtx *ctx, const MeaoCamera *camera);
@@ -739,7 +766,8 @@ int64_t meao_launch_count(const MeaoCtx *ctx);       /* kernels launched (or rep
  * kernels whose only predecessor is the kernel before them in their stream, 2 = also where a cross-branch event joins.  The runtime
  * decides what it accepts at the first capture; env MEAO_PDL=0|1|2 caps it. */
 int meao_pdl_level(const MeaoCtx *ctx);
-int meao_kernels_per_frame(const MeaoCtx *ctx);      /* kernel nodes in one frame: 9 + one per bit of high_quality_mask (3 with single_scale) */
+int meao_kernels_per_frame(const MeaoCtx *ctx);      /* kernel nodes in one frame: 9 + one per bit of high_quality_mask (3 with single_scale);
+                                                       at hierarchy depth n, 1 + 2 n + the mask bits <= n (+1 with device cameras) */
 /* Algorithmic bytes of the reference data-flow (SURVEY.md 8d): stage 0 = whole frame, 1 = Downsample1,
  * 2 = Downsample2, 3 = Render x4, 4 = Upsample x4, 5 = final Upsample (L1->L0) only. */
 int64_t meao_algorithmic_bytes(const MeaoCtx *ctx, int32_t stage);

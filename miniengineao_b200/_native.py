@@ -72,6 +72,8 @@ SIGNATURES = {
     "meao_default_params": (None, [C.POINTER(MeaoParams)]),
     "meao_set_variants": (C.c_int, [C.c_void_p, C.POINTER(MeaoVariants)]),
     "meao_get_variants": (C.c_int, [C.c_void_p, C.POINTER(MeaoVariants)]),
+    "meao_set_hierarchy_depth": (C.c_int, [C.c_void_p, C.c_int32]),
+    "meao_get_hierarchy_depth": (C.c_int, [C.c_void_p]),
     "meao_set_camera": (C.c_int, [C.c_void_p, C.POINTER(MeaoCamera)]),
     "meao_resize": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
     "meao_reserve": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),

@@ -84,6 +84,10 @@ class AmbientOcclusion:
         self.sampleExhaustively = False     # Render.compute:144-159
         self.highQualityMask = 0            # bit k-1: Render.compute kernel "main" on level k + Upsample main_premin*
         self.singleScale = False            # BASELINE.json configs[0]: Downsample1 -> Render level 1 -> final-style Upsample only
+        # the levels of the AO pyramid a frame renders and upsamples (meao_set_hierarchy_depth, upstream MiniEngine's "Hierarchy Depth"):
+        # 1..4, 4 = the reference's frame.  Fewer levels cost less and drop the coarsest, large-scale darkening.  A structural input: a
+        # change re-plans (a device synchronise and new graphs), so it is a setting, not something to toggle every frame
+        self.hierarchyDepth = 4
         self.layers = 1                     # views per frame (meao_set_layers): texture-array stereo 2, cube faces 6, frame batches
         # one Camera per layer (meao_set_layer_cameras): split-screen viewports, mirrors, batches from several cameras; None = every
         # layer uses `camera`.  Each entry must match the main camera's pixelWidth, pixelHeight, usesReversedZBuffer and orthographic.
@@ -182,6 +186,7 @@ class AmbientOcclusion:
         stereo = self._stereo
         v = N.MeaoVariants(int(stereo), int(self.sampleExhaustively), int(self.highQualityMask), int(self.singleScale))
         rebuild |= self._check(self._lib.meao_set_variants(self._ctx, C.byref(v))) == 1
+        rebuild |= self._check(self._lib.meao_set_hierarchy_depth(self._ctx, int(self.hierarchyDepth))) == 1
         width = cam.pixelWidth * (2 if stereo else 1)                                                # AO.cs:338-341, 501-504
         reallocated = self._apply_layer_reservation()
         layered = self._set_layers(int(self.layers))

@@ -18,6 +18,18 @@ namespace meao {
 
 struct Range { int lo, hi; };   // [lo, hi)
 
+// The plan's variants: MeaoVariants as set (meao_set_variants) and the hierarchy depth as set (meao_set_hierarchy_depth, 1..4).
+// Together they decide the levels a frame runs (effective_depth), so they travel as one value.
+struct PlanVariants : MeaoVariants {
+    int levels = 4;
+    PlanVariants() : MeaoVariants{0, 0, 0, 0} {}
+    PlanVariants(const MeaoVariants &v, int levels_ = 4) : MeaoVariants(v), levels(levels_) {}
+};
+
+// The levels 1..n a frame renders and upsamples; the first upsample reads Occlusion<n>.  single_scale (BASELINE.json configs[0]) is
+// n = 1.  The one place the depth in effect is derived: the schedule, the upsample wiring and the launch counts all read it.
+inline int effective_depth(const PlanVariants &v) { return v.single_scale ? 1 : v.levels; }
+
 struct Plan {
     // Render (per level 1..4) -- AO.cs:660-734
     float inv_thickness[5][12];
@@ -32,8 +44,8 @@ struct Plan {
     float inv_low[5][2], inv_high[5][2];
     float noise_filter_strength[5], step_size[5], blur_tolerance[5], upsample_tolerance[5];
     float zb[4];
-    // the plan inputs the recorders read besides the constants: the variants and the cameras' Z direction
-    MeaoVariants variants;
+    // the plan inputs the recorders read besides the constants: the variants with the hierarchy depth, and the cameras' Z direction
+    PlanVariants variants;
     int reversed_z;
     int orthographic;                       // every layer MEAO_PROJECTION_ORTHOGRAPHIC: launch_entry_ortho's kernels
 };
@@ -52,9 +64,9 @@ struct FrameMaps {
     CUtensorMap low_ren[kRenderTileVariants][5];    // LowDepth<k> with the render box of tile height kRenderTileHs[t]
     CUtensorMap low_wide[kRenderTileVariants][5];   // LowDepth<k> with the wide-render box
     CUtensorMap low_ups[5];                 // LowDepth<k> with the upsample depth box
-    CUtensorMap ao_ups[5];                  // lo AO of upsample lo level k (Occlusion4 / Combined k)
+    CUtensorMap comb_ups[4];                // Combined<k> (k = 1..3) as LoResAO1 of upsample lo level k below the frame's depth
+    CUtensorMap occ_ups[5];                 // Occlusion<k> as LoResAO1 of upsample lo level k = the frame's depth (its first upsample)
     CUtensorMap hq_ups[5];                  // HighQuality<k> as LoResAO2 of upsample lo level k
-    CUtensorMap occ1_ups;                   // Occlusion1 as LoResAO1 of the final upsample (MeaoVariants.single_scale)
 };
 
 // What the recorders read: the geometry and rows of one frame size, where its buffers are, its maps, its plan and its camera tables.
@@ -150,10 +162,10 @@ template <class Enc> bool encode_maps(FrameState &f, Enc &&enc)
             ok &= enc(m.low_wide[t][k], MapSpec{f.low[k], 4, f.lw[k], mh, f.low_pitch[k], kRenderWideBoxW, render_box_h(kRenderTileHs[t], true)});
         }
         ok &= enc(m.low_ups[k], MapSpec{f.low[k], 4, f.lw[k], mh, f.low_pitch[k], kUpsDepthBoxW, kUpsDepthBoxH});
-        ok &= enc(m.ao_ups[k], MapSpec{(k == 4) ? f.occ[4] : f.comb[k], 1, f.lw[k], mh, f.occ_pitch[k], kUpsAoBoxW, kUpsAoBoxH});
+        if (k <= 3) ok &= enc(m.comb_ups[k], MapSpec{f.comb[k], 1, f.lw[k], mh, f.occ_pitch[k], kUpsAoBoxW, kUpsAoBoxH});
+        ok &= enc(m.occ_ups[k], MapSpec{f.occ[k], 1, f.lw[k], mh, f.occ_pitch[k], kUpsAoBoxW, kUpsAoBoxH});
         ok &= enc(m.hq_ups[k], MapSpec{f.hq[k], 1, f.lw[k], mh, f.occ_pitch[k], kUpsAoBoxW, kUpsAoBoxH});
     }
-    ok &= enc(m.occ1_ups, MapSpec{f.occ[1], 1, f.lw[1], f.layers * f.lh[1], f.occ_pitch[1], kUpsAoBoxW, kUpsAoBoxH});
     return ok;
 }
 
@@ -329,14 +341,14 @@ inline cudaError_t launch_render(const FrameState &f, const RenderArgs &a, int k
 }
 
 // PushUpsampleCommands with the wiring of AO.cs:528-531, lo level `lo`.  ao_out (final level only): the caller's AO at the pitches
-// of vp (nullptr: tight), its first row band0; nullptr: the context's result buffer.
+// of vp (nullptr: tight), its first row band0; nullptr: the context's result buffer.  The frame's first upsample (lo = effective_depth)
+// reads Occlusion<lo> as LoResAO1, since no coarser level contributes; every later one the Combined<lo> the one before wrote.
 inline UpsampleArgs upsample_args(const FrameState &f, int lo, void *ao_out, const ViewPitch *vp)
 {
     const int hi = lo - 1;
-    const bool single = f.plan.variants.single_scale != 0 && lo == 1;     // LoResAO1 = Occlusion1: no coarser level contributes
     UpsampleArgs a{};
     a.lo_depth = f.low[lo]; a.low = f.lw[lo]; a.loh = f.lh[lo]; a.lo_dpitch = f.low_pitch[lo];
-    a.lo_ao = single ? f.occ[1] : (lo == 4) ? f.occ[4] : f.comb[lo]; a.lo_apitch = f.occ_pitch[lo];
+    a.lo_ao = lo == effective_depth(f.plan.variants) ? f.occ[lo] : f.comb[lo]; a.lo_apitch = f.occ_pitch[lo];
     if (hi == 0) { a.hi_depth = f.lin; a.hi_is_half = 1; a.hi_dpitch = f.lin_pitch; a.hi_ao = nullptr; a.hi_apitch = 0; }
     else { a.hi_depth = f.low[hi]; a.hi_is_half = 0; a.hi_dpitch = f.low_pitch[hi]; a.hi_ao = f.occ[hi]; a.hi_apitch = f.occ_pitch[hi]; }
     if (hi == 0) {
@@ -362,7 +374,7 @@ inline UpsampleArgs upsample_args(const FrameState &f, int lo, void *ao_out, con
 // main / main_blendout)
 inline const CUtensorMap &upsample_ao_map(const FrameState &f, int lo)
 {
-    return (f.plan.variants.single_scale != 0 && lo == 1) ? f.maps.occ1_ups : f.maps.ao_ups[lo];
+    return lo == effective_depth(f.plan.variants) ? f.maps.occ_ups[lo] : f.maps.comb_ups[lo];
 }
 inline const uint8_t *upsample_lo_ao2(const FrameState &f, int lo) { return hq_level(f, lo) ? f.hq[lo] : nullptr; }
 
@@ -400,15 +412,16 @@ struct FrameLaunch {
 
 inline bool pdl_on(const FrameLaunch &l, int pdl_level) { return l.pdl != kPdlNever && pdl_level >= l.pdl; }
 
-// The launches of one frame in serial order (RebuildCommandBuffers, AO.cs:511-531): prepare, render 1..k, the wide renders of the
-// high_quality_mask levels, upsamples k..1.  The branches make it a DAG: the four render levels are independent (SURVEY.md 3.2), a
-// level's wide render rides on its branch, the coarse upsample chain 4->3->2 only needs Occlusion2..4, and only the last two upsamples
-// wait for the big level-1 render.  single_scale (BASELINE.json configs[0]): prepare, render 1 and the final-style upsample on Occlusion1.
+// The launches of one frame of depth n in serial order (RebuildCommandBuffers, AO.cs:511-531): prepare, render 1..n, the wide renders
+// of the high_quality_mask levels up to n, upsamples n..1.  The branches make it a DAG: the render levels are independent (SURVEY.md
+// 3.2), a level's wide render rides on its branch, the coarse upsample chain n->..->2 runs on level n's branch and only needs
+// Occlusion2..n, and only the last two upsamples wait for the big level-1 render.  The first upsample reads Occlusion<n> (and
+// HighQuality<n>); at n = 1 it is the final upsample, on the caller's stream behind render 1.  Mask bits above n launch nothing.
 // device_cameras (meao_bind_device_cameras): the camera stage first, on the caller's stream; every other launch follows it through the
 // prepare.
-inline std::vector<FrameLaunch> frame_schedule(const MeaoVariants &v, bool device_cameras = false)
+inline std::vector<FrameLaunch> frame_schedule(const PlanVariants &v, bool device_cameras = false)
 {
-    const int kmax = v.single_scale ? 1 : 4;
+    const int hq_mask = v.high_quality_mask, n = effective_depth(v);
     std::vector<FrameLaunch> s;
     int last[4] = {0, 0, 0, 0};             // the last launch on each branch so far
     auto add = [&](int stage, int level, int branch, int wait, int pdl) {
@@ -418,14 +431,12 @@ inline std::vector<FrameLaunch> frame_schedule(const MeaoVariants &v, bool devic
     if (device_cameras) add(kStageCamera, 0, 0, -1, kPdlNever);
     const int prep = (int)s.size();
     add(kStagePrepare, 0, 0, -1, kPdlNever);
-    for (int k = 1; k <= kmax; k++) add(kStageRender, k, k - 1, k == 1 ? -1 : prep, k == 1 ? kPdlFrom1 : kPdlNever);
-    for (int k = 1; k <= kmax; k++)
-        if ((v.high_quality_mask >> (k - 1)) & 1) add(kStageRenderWide, k, k - 1, -1, kPdlFrom1);
-    if (kmax == 4) {
-        add(kStageUpsample, 4, 3, last[2], kPdlFrom2);
-        add(kStageUpsample, 3, 3, last[1], kPdlFrom2);
-        add(kStageUpsample, 2, 0, last[3], kPdlFrom2);
-    }
+    for (int k = 1; k <= n; k++) add(kStageRender, k, k - 1, k == 1 ? -1 : prep, k == 1 ? kPdlFrom1 : kPdlNever);
+    for (int k = 1; k <= n; k++)
+        if ((hq_mask >> (k - 1)) & 1) add(kStageRenderWide, k, k - 1, -1, kPdlFrom1);
+    // lo >= 3 on level n's branch, waiting for Occlusion<lo - 1>; lo = 2 on the caller's stream (Occlusion1), waiting for the chain
+    for (int lo = n; lo >= 3; lo--) add(kStageUpsample, lo, n - 1, last[lo - 2], kPdlFrom2);
+    if (n >= 2) add(kStageUpsample, 2, 0, last[n - 1], kPdlFrom2);
     add(kStageUpsample, 1, 0, -1, kPdlFrom1);
     return s;
 }

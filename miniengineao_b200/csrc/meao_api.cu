@@ -92,6 +92,7 @@ struct MeaoCtx : SizeState {
     int views_last[2][2] = {{0, 0}, {0, 0}};
     std::vector<std::pair<int, int>> views_checked;
     MeaoVariants variants = {0, 0, 0, 0};
+    int hierarchy_depth = 4;                // meao_set_hierarchy_depth (a structural input: the schedule's levels, frame_record.h effective_depth)
     int projection = MEAO_PROJECTION_PERSPECTIVE;  // meao_set_projection (a structural input: it selects the orthographic kernels)
     // meao_set_layer_projections: one MeaoProjection per layer, or empty (every layer has `projection`).  A structural input like the
     // context's projection: a table that mixes both selects the mixed kernels (frame_record.h launch_entry_mixed).  layer_proj_ortho: its
@@ -340,7 +341,7 @@ void build_plan(MeaoCtx *c)
     const CamConsts &cc = c->layer_consts[0];
     p.zb[0] = cc.zb[0]; p.zb[1] = cc.zb[1];
     p.zb[2] = p.zb[3] = 0;
-    p.variants = c->variants;
+    p.variants = PlanVariants(c->variants, c->hierarchy_depth);
     p.reversed_z = ctx_reversed_z(c);
     plan_projections(*c, [c](int l) { return layer_projection(c, l) == MEAO_PROJECTION_ORTHOGRAPHIC; });
     memcpy(p.inv_thickness, cc.inv_thickness, sizeof p.inv_thickness);
@@ -1020,6 +1021,19 @@ int meao_get_variants(const MeaoCtx *c, MeaoVariants *out)
     *out = c->variants;
     return MEAO_OK;
 }
+
+int meao_set_hierarchy_depth(MeaoCtx *c, int32_t levels)
+{
+    if (!c) return MEAO_ERR_INVALID;
+    if (levels < 1 || levels > 4) return fail(c, MEAO_ERR_INVALID, "hierarchy depth (levels) %d not in 1..4", levels);
+    if (levels == c->hierarchy_depth) return 0;
+    c->hierarchy_depth = levels;
+    c->plan_dirty = true;           // another schedule: re-plan + drop the captured graphs (ensure_ready)
+    c->frame_gen++;
+    return 1;
+}
+
+int meao_get_hierarchy_depth(const MeaoCtx *c) { return c ? c->hierarchy_depth : MEAO_ERR_INVALID; }
 
 int meao_set_camera(MeaoCtx *c, const MeaoCamera *cam)
 {
@@ -2422,6 +2436,9 @@ int meao_stage_upsample(MeaoCtx *c, int32_t lo_level, void *ao_out, void *stream
 {
     int rc = frame_ready(c, (cudaStream_t)stream); if (rc) return rc;
     if (lo_level < 1 || lo_level > 4) return fail(c, MEAO_ERR_INVALID, "upsample lo level %d not in 1..4", lo_level);
+    if (lo_level > effective_depth(c->plan.variants))
+        return fail(c, MEAO_ERR_INVALID, "upsample lo level %d is above the frame's hierarchy depth %d (meao_set_hierarchy_depth, single_scale)",
+                    lo_level, effective_depth(c->plan.variants));
     return record_upsample(c, lo_level, lo_level == 1 ? ao_out : nullptr, (cudaStream_t)stream);
 }
 
@@ -2775,19 +2792,22 @@ int64_t meao_frame_generation(const MeaoCtx *c) { return c ? c->frame_gen : MEAO
 int meao_pdl_level(const MeaoCtx *c) { return c ? c->pdl_level : -1; }
 int meao_kernels_per_frame(const MeaoCtx *c)
 {
-    return (int)frame_schedule(c ? c->variants : MeaoVariants{}, c && c->cams.cams).size();     // as set: the plan may not be rebuilt yet
+    if (!c) return (int)frame_schedule(PlanVariants()).size();
+    return (int)frame_schedule(PlanVariants(c->variants, c->hierarchy_depth), c->cams.cams != nullptr).size();     // as set: the plan may not be rebuilt yet
 }
 
 int64_t meao_algorithmic_bytes(const MeaoCtx *c, int32_t stage)
 {
     if (!c || c->W <= 0) return MEAO_ERR_INVALID;
     auto px = [&](int l) { return (int64_t)c->lw[l] * c->lh[l] * c->layers; };      // every layer moves the same bytes
-    // SURVEY.md 8(d): every buffer of the reference data-flow read once per consuming stage, written once
+    // SURVEY.md 8(d): every buffer of the reference data-flow read once per consuming stage, written once; the renders and upsamples of
+    // the levels the frame runs (its hierarchy depth, as set)
+    const int n = effective_depth(PlanVariants(c->variants, c->hierarchy_depth));
     const int64_t ds1 = 6 * px(0) + 4 * px(1) + 4 * px(2) + 32 * px(3) + 32 * px(4);
     const int64_t ds2 = 4 * px(2) + 4 * px(3) + 4 * px(4) + 32 * px(5) + 32 * px(6);
     int64_t ren = 0, ups = 0, ups_final = 0;
-    for (int k = 1; k <= 4; k++) ren += 32 * px(k + 2) + px(k);
-    for (int lo = 4; lo >= 1; lo--) {
+    for (int k = 1; k <= n; k++) ren += 32 * px(k + 2) + px(k);
+    for (int lo = n; lo >= 1; lo--) {
         const int hi = lo - 1;
         const int64_t b = 5 * px(lo) + (hi == 0 ? 2 : 5) * px(hi) + px(hi);
         ups += b;
