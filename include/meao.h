@@ -723,7 +723,8 @@ MeaoRenderEventFunc meao_get_render_event_func(void);
 
 /* ---- frames inside a caller's graph ------------------------------------------------------------------------------------------
  * When the stream an entry point is given is being captured (cudaStreamBeginCapture in any mode, torch.cuda.graph, the graph trees of
- * torch.compile(mode="reduce-overhead")), the call records its kernel launches straight into that capture: the caller's graph then
+ * torch.compile(mode="reduce-overhead"), which reach a frame through the torch.library operator meao::ambient_occlusion of
+ * miniengineao_b200/torch_ops.py), the call records its kernel launches straight into that capture: the caller's graph then
  * holds the frame, and every replay of it runs the frame.  No graph of the context is captured, instantiated or launched, and the
  * graph cache is neither used nor changed.  A graph-path frame forks to the context's own streams and joins back inside the caller's
  * capture (cross-stream dependencies of the caller's graph); a MEAO_FLAG_NO_GRAPH frame records its launches serially.  The launches
