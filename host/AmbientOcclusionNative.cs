@@ -125,6 +125,10 @@ namespace MiniEngineAO
         // no CUDA buffer of its own to hand over; a native plugin or an interop host that keeps its cameras on the GPU passes its pointer.
         [DllImport(Lib)] public static extern int meao_bind_device_cameras(IntPtr ctx, IntPtr camerasDev, int capacity);
         [DllImport(Lib)] public static extern int meao_device_camera_status(IntPtr ctx, [Out] int[] out4);
+        // Thickness modifier and intensity read from device memory at every launch and graph replay (meao_bind_device_params).
+        // Declarations only, like the device cameras: a native plugin or an interop host that animates them on the GPU passes its pointer.
+        [DllImport(Lib)] public static extern int meao_bind_device_params(IntPtr ctx, IntPtr paramsDev);
+        [DllImport(Lib)] public static extern int meao_device_param_status(IntPtr ctx, [Out] int[] out4);
 
         public static void Check(IntPtr ctx, int rc)
         {

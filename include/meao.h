@@ -51,7 +51,9 @@ extern "C" {
                               *    + meao_bind_device_cameras / meao_device_camera_status (cameras read from device memory at every
                               *      launch and graph replay; additive)
                               *    + meao_set_hierarchy_depth / meao_get_hierarchy_depth (render and upsample only the finest 1-4 levels;
-                              *      additive, MeaoVariants unchanged) */
+                              *      additive, MeaoVariants unchanged)
+                              *    + meao_bind_device_params / meao_device_param_status (thickness_modifier and intensity read from
+                              *      device memory at every launch and graph replay; additive) */
 
 typedef struct MeaoCtx MeaoCtx;
 
@@ -289,6 +291,39 @@ int meao_get_layer_projections(const MeaoCtx *ctx, int32_t *out, int32_t capacit
  * is bound. */
 int meao_bind_device_cameras(MeaoCtx *ctx, const float *cameras_dev, int32_t capacity);
 int meao_device_camera_status(const MeaoCtx *ctx, int32_t out4[4]);
+/* Thickness and intensity from device memory: a frame recorded into a graph (the context's own or a caller's capture, torch.cuda.graph,
+ * the torch operator under torch.compile) follows an AO fade, a quality slider or a tuning loop without a capture or an instantiation per
+ * change.
+ *   - params_dev: device memory of the context's device holding 2 floats, {thickness_modifier, intensity}, with the meaning of the
+ *     MeaoParams fields.  A contiguous float32 CUDA tensor of shape [2] fits.  It must be 4-byte aligned (else MEAO_ERR_INVALID, nothing
+ *     changes).
+ *   - params_dev == NULL unbinds.  Returns 1 when the binding changed, 0 when the same pointer is bound again.  Binding, unbinding and a
+ *     new pointer are structural inputs: a re-plan with a device synchronise, the captured graphs dropped, meao_frame_generation moved.
+ *     Plan-only contexts record the binding and allocate nothing.
+ *   - The buffer's CONTENTS are not tracked: a stage ahead of the renders reads them, in stream order, at every launch and every replay,
+ *     and derives the renders' reject_fadeoff (-1 / thickness_modifier, bit for bit the host's) and intensity.  Writing new values moves no
+ *     generation and needs no capture.  The host-buffer calls (meao_render_host, _async) run on the context's own streams, so the buffer
+ *     must be complete before such a call is made.  The caller keeps the buffer alive while it is bound.
+ *   - A block is valid when it passes meao_set_params's test, thickness_modifier > 0 (NaN fails); intensity is taken as the host takes it.
+ *     An invalid block leaves the derived values as they were -- the last valid block's, or the host parameters at bind time -- so the
+ *     frame's AO is that of a host-parameter frame with those values.
+ *   - While a buffer is bound it alone decides thickness_modifier and intensity.  meao_set_params still records them, and they apply
+ *     again once the buffer is unbound: a change of those two fields alone returns 1 but moves no meao_frame_generation and marks nothing
+ *     pending.  A change of a tolerance (or of debug) behaves as without a binding: the three tolerances stay host frame constants.
+ *     meao_render_constants and its _layer and _wide forms keep describing the HOST values.
+ *   - Every frame form runs the stage: pointers, pitched views, host buffers, CUDA arrays and _at, layer-viewport tables, both batch
+ *     calls, orthographic and mixed projections, device cameras (both may be bound), the bound events, MEAO_FLAG_NO_GRAPH, recording into a
+ *     caller's capture, both reservations and every hierarchy depth.  meao_stage_downsample runs it too, and the later meao_stage_render /
+ *     _render_wide use the values it derived.  A single-layer frame takes the layered render kernels with one layer; every frame is
+ *     bit-identical to a frame of a context whose host parameters are the buffer's.  meao_kernels_per_frame counts the stage (+1), and
+ *     meao_profile_frame names it "render_params".
+ *   - Refused with MEAO_ERR_UNSUPPORTED before anything changes, in either order: row bands and their halo and exchange calls.
+ * meao_device_param_status: {frames that met an invalid block since the bind, the field of the latest (1 thickness_modifier), 0, 0}.  The
+ * count is of the stage's launches: a frame launches it once, and meao_profile_frame, which launches every kernel profile_repeats times
+ * (meao_set_profile_repeats), adds profile_repeats for a profiled frame that meets an invalid block.  A stream-less read like
+ * meao_device_camera_status, without a device synchronise; all zeros on a plan-only context; MEAO_ERR_INVALID when nothing is bound. */
+int meao_bind_device_params(MeaoCtx *ctx, const float *params_dev);
+int meao_device_param_status(const MeaoCtx *ctx, int32_t out4[4]);
 /* replaces: RTHandle.SetBaseDimensions + AllocateNow + the rebuild it triggers (AO.cs:338-341, 501-506).
  * Allocates the intermediates for width x height.  Returns 1 if dimensions changed, 0 if not.
  * A size change RESETS the row band to the whole frame and drops the neighbour connections (meao_set_row_band,
@@ -768,7 +803,8 @@ int64_t meao_launch_count(const MeaoCtx *ctx);       /* kernels launched (or rep
  * decides what it accepts at the first capture; env MEAO_PDL=0|1|2 caps it. */
 int meao_pdl_level(const MeaoCtx *ctx);
 int meao_kernels_per_frame(const MeaoCtx *ctx);      /* kernel nodes in one frame: 9 + one per bit of high_quality_mask (3 with single_scale);
-                                                       at hierarchy depth n, 1 + 2 n + the mask bits <= n (+1 with device cameras) */
+                                                       at hierarchy depth n, 1 + 2 n + the mask bits <= n (+1 with device cameras,
+                                                       +1 with device parameters) */
 /* Algorithmic bytes of the reference data-flow (SURVEY.md 8d): stage 0 = whole frame, 1 = Downsample1,
  * 2 = Downsample2, 3 = Render x4, 4 = Upsample x4, 5 = final Upsample (L1->L0) only. */
 int64_t meao_algorithmic_bytes(const MeaoCtx *ctx, int32_t stage);

@@ -151,6 +151,8 @@ SIGNATURES = {
     "meao_get_layer_projections": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32]),
     "meao_bind_device_cameras": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),
     "meao_device_camera_status": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),
+    "meao_bind_device_params": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "meao_device_param_status": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),
     "meao_pdl_level": (C.c_int, [C.c_void_p]),
     "meao_kernels_per_frame": (C.c_int, [C.c_void_p]),
     "meao_algorithmic_bytes": (C.c_int64, [C.c_void_p, C.c_int32]),

@@ -117,6 +117,13 @@ class AmbientOcclusion:
         self.deviceCameras = None
         self._boundCameras = (0, 0)         # (data_ptr, n) meao_bind_device_cameras was last given
         self._boundCameraTensor = None      # a reference that keeps the bound buffer alive
+        # thickness and intensity that live on the GPU (meao_bind_device_params): a contiguous CUDA float32 tensor [2] of
+        # (thicknessModifier, intensity), read by every frame at launch and at every graph replay -- write new values into it (a fade inside
+        # a captured graph, a tuning loop) and a recorded frame follows them without a re-capture.  While one is set it decides both; the
+        # tolerances still come from the properties.  None = thicknessModifier and intensity
+        self.deviceParams = None
+        self._boundParams = 0               # the data_ptr meao_bind_device_params was last given
+        self._boundParamTensor = None       # a reference that keeps the bound buffer alive
         self._contextLayers = 1             # what meao_set_layers was last given
         self._band = None                   # (row0, row1) after set_row_band; reset by every re-allocation
         self._drawCountPerFrame = 0         # AO.cs:289: used to detect single-pass stereo
@@ -205,6 +212,7 @@ class AmbientOcclusion:
         if cam.orthographic:
             rebuild |= self._check(self._lib.meao_set_projection(self._ctx, N.MEAO_PROJECTION_ORTHOGRAPHIC)) == 1
         rebuild |= self._apply_device_cameras()
+        rebuild |= self._apply_device_params()
         reallocated |= self._apply_reservation(width, cam.pixelHeight, stereo)
         resized = self._check(self._lib.meao_resize(self._ctx, width, cam.pixelHeight)) == 1          # CheckBaseDimensions
         reallocated |= resized and self._reserved == (0, 0)       # inside a reservation a resize allocates nothing
@@ -307,6 +315,29 @@ class AmbientOcclusion:
         out = (C.c_int32 * 4)()
         self._check(self._lib.meao_device_camera_status(self._ctx, out))
         return int(out[0]), int(out[1]), int(out[2])
+
+    def _apply_device_params(self) -> bool:
+        """Hands deviceParams to meao_bind_device_params when its data_ptr changed; True if the binding changed."""
+        t = self.deviceParams
+        if t is None:
+            want = 0
+        else:
+            if not getattr(t, "is_cuda", False) or str(t.dtype) != "torch.float32" or tuple(t.shape) != (2,) or not t.is_contiguous():
+                raise ValueError("deviceParams must be a contiguous CUDA float32 tensor of shape [2]")
+            want = t.data_ptr()
+        if want == self._boundParams:
+            self._boundParamTensor = t
+            return False
+        changed = self._check(self._lib.meao_bind_device_params(self._ctx, C.c_void_p(want or None))) == 1
+        self._boundParams, self._boundParamTensor = want, t
+        return changed
+
+    def deviceParamStatus(self) -> tuple[int, int]:
+        """meao_device_param_status: (frames that met an invalid block since the bind, the field of the latest: 1 thickness_modifier).
+        Reads without a device synchronise."""
+        out = (C.c_int32 * 4)()
+        self._check(self._lib.meao_device_param_status(self._ctx, out))
+        return int(out[0]), int(out[1])
 
     def _apply_layer_viewports(self) -> bool:
         """Hands layerViewports to meao_set_layer_viewports (after meao_set_layers, which clears the table); True if a value changed."""

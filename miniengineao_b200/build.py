@@ -34,6 +34,11 @@ MIXED_SOURCES = ["prepare_depth_mixed_layered.cu", "prepare_depth_array_mixed.cu
 # compiled into libmeao.so with SOURCES; tests/test_device_cameras_units.py audits it, and the CPU emulator builds it into a library of its
 # own (tests/emu/device_cameras.py).
 CAMERA_SOURCES = ["camera_tables.cu"]
+# The device-parameter kernels (meao_bind_device_params: reject_fadeoff and intensity derived on the device ahead of the renders, and the
+# layered render kernels that read them): compiled into libmeao.so with SOURCES, the renders each a textual include of an existing kernel
+# body under MEAO_DEVICE_PARAMS, so the other kernels keep their code; tests/test_device_params_units.py audits them, and the CPU emulator
+# builds them into a library of their own (tests/emu/device_params.py).
+PARAM_SOURCES = ["render_params.cu", "render_ao_params_layered.cu", "render_ao_ortho_params_layered.cu", "render_ao_mixed_params_layered.cu"]
 HEADERS = ["common.cuh", "kernels.h", "prepare_depth_kernel.inc", "render_ao_kernel.inc", "render_ao_groups.inc", "render_ao_sample.inc", "blur_upsample_device.inc", "blur_upsample_kernel.inc",
            "blur_upsample_layer_args.inc", "blur_upsample_lin_device.inc", "surface_io.cuh", "depth_in.cuh", "arena_layout.h", "frame_record.h",
            os.path.join("..", "..", "include", "meao.h")]
@@ -60,7 +65,7 @@ def is_stale() -> bool:
     if not os.path.exists(LIB):
         return True
     t = os.path.getmtime(LIB)
-    deps = [os.path.join(CSRC, f) for f in SOURCES + VIEW_SOURCES + ORTHO_SOURCES + BATCH_SOURCES + MIXED_SOURCES + CAMERA_SOURCES + HEADERS] + [os.path.abspath(__file__)]
+    deps = [os.path.join(CSRC, f) for f in SOURCES + VIEW_SOURCES + ORTHO_SOURCES + BATCH_SOURCES + MIXED_SOURCES + CAMERA_SOURCES + PARAM_SOURCES + HEADERS] + [os.path.abspath(__file__)]
     return any(os.path.getmtime(d) > t for d in deps)
 
 
@@ -68,7 +73,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     if not force and not is_stale():
         return LIB
     extra = os.environ.get("MEAO_NVCC_DEFS", "").split()      # tuning experiments, e.g. "-DMEAO_REN_MINB=12"
-    cmd = [_nvcc()] + NVCC_FLAGS + extra + ["-o", LIB] + [os.path.join(CSRC, f) for f in SOURCES + VIEW_SOURCES + ORTHO_SOURCES + BATCH_SOURCES + MIXED_SOURCES + CAMERA_SOURCES]
+    cmd = [_nvcc()] + NVCC_FLAGS + extra + ["-o", LIB] + [os.path.join(CSRC, f) for f in SOURCES + VIEW_SOURCES + ORTHO_SOURCES + BATCH_SOURCES + MIXED_SOURCES + CAMERA_SOURCES + PARAM_SOURCES]
     proc = subprocess.run(cmd, capture_output=True, text=True)
     if verbose or proc.returncode != 0:
         sys.stderr.write(proc.stdout + proc.stderr)

@@ -396,8 +396,9 @@ inline cudaError_t launch_upsample(const FrameState &f, int lo, const UpsampleAr
 }
 
 // ---- the frame schedule: which kernels a frame launches, in what order, on which stream and after which other launch ----------
-// kStageCamera: the camera tables derived from a bound device camera buffer (launch_camera_tables), ahead of the prepare
-enum FrameStage { kStagePrepare, kStageRender, kStageRenderWide, kStageUpsample, kStageCamera };
+// kStageCamera: the camera tables derived from a bound device camera buffer (launch_camera_tables), ahead of the prepare.
+// kStageParams: reject_fadeoff and intensity derived from a bound device parameter buffer (launch_render_params), ahead of the prepare.
+enum FrameStage { kStagePrepare, kStageRender, kStageRenderWide, kStageUpsample, kStageCamera, kStageParams };
 // PDL (DESIGN.md 2.5): a launch whose only predecessor is the launch before it on its stream carries the programmatic-dependent-launch
 // attribute from PDL level 1 on; one that also waits for another branch, from level 2; the first launch of a branch never.
 enum PdlClass { kPdlNever = 0, kPdlFrom1 = 1, kPdlFrom2 = 2 };
@@ -418,8 +419,9 @@ inline bool pdl_on(const FrameLaunch &l, int pdl_level) { return l.pdl != kPdlNe
 // Occlusion2..n, and only the last two upsamples wait for the big level-1 render.  The first upsample reads Occlusion<n> (and
 // HighQuality<n>); at n = 1 it is the final upsample, on the caller's stream behind render 1.  Mask bits above n launch nothing.
 // device_cameras (meao_bind_device_cameras): the camera stage first, on the caller's stream; every other launch follows it through the
-// prepare.
-inline std::vector<FrameLaunch> frame_schedule(const PlanVariants &v, bool device_cameras = false)
+// prepare.  device_params (meao_bind_device_params): the parameter stage next, on the caller's stream and without PDL, so every render
+// follows it through the prepare as well; it sits on the frame's critical path, ahead of a prepare that waits for it in full.
+inline std::vector<FrameLaunch> frame_schedule(const PlanVariants &v, bool device_cameras = false, bool device_params = false)
 {
     const int hq_mask = v.high_quality_mask, n = effective_depth(v);
     std::vector<FrameLaunch> s;
@@ -429,6 +431,7 @@ inline std::vector<FrameLaunch> frame_schedule(const PlanVariants &v, bool devic
         s.push_back(FrameLaunch{stage, level, branch, wait, pdl});
     };
     if (device_cameras) add(kStageCamera, 0, 0, -1, kPdlNever);
+    if (device_params) add(kStageParams, 0, 0, -1, kPdlNever);
     const int prep = (int)s.size();
     add(kStagePrepare, 0, 0, -1, kPdlNever);
     for (int k = 1; k <= n; k++) add(kStageRender, k, k - 1, k == 1 ? -1 : prep, k == 1 ? kPdlFrom1 : kPdlNever);
@@ -448,6 +451,7 @@ inline std::string launch_name(const FrameLaunch &l)
     switch (l.stage) {
         case kStagePrepare: return "prepare_depth";
         case kStageCamera: return "camera_tables";
+        case kStageParams: return "render_params";
         case kStageRender: return "render_ao L" + k;
         case kStageRenderWide: return "render_ao_wide L" + k;
         default: return "blur_upsample L" + k + "->L" + std::to_string(l.level - 1);
@@ -468,6 +472,9 @@ struct FrameIO {
     // a bound device camera buffer (meao_bind_device_cameras): the schedule's camera stage derives the tables from it, and every launch
     // that reads a camera takes the layered kernel at layers == 1 too, so that it reads the tables rather than its argument block
     const struct DeviceCameras *cams = nullptr;
+    // a bound device parameter buffer (meao_bind_device_params): the schedule's parameter stage derives the slot from it, and every render
+    // takes the *_params_layered kernel, at layers == 1 too (launch_render_params_entry)
+    const RenderParamArgs *params = nullptr;
 };
 
 // A bound device camera buffer: cams[l] = {near_clip, far_clip, tan_half_fov_h} of layer l, the kernel's status words (kernels.h
@@ -503,6 +510,26 @@ inline cudaError_t launch_cameras(const FrameState &f, const DeviceCameras &dc, 
     LayerProjections proj{};
     for (size_t i = 0; i < f.layer_ortho.size(); i++) proj.ortho[i] = f.layer_ortho[i];
     return launch_camera_tables(camera_args(f, dc), &proj, s);
+}
+
+// A render of a frame with a bound device parameter buffer (FrameIO.params): the kernel for the plan's projections that reads reject_fadeoff
+// and intensity from the derived slot.  The layers' camera table entries as the layered launch takes them (launch_render,
+// launch_entry_ortho, launch_entry_mixed); a single layer without device cameras reads its argument block, as the single-image kernels
+// do.  Apart from launch_entry so that a recorder that never binds a parameter buffer does not link these kernels.
+inline cudaError_t launch_render_params_entry(const FrameState &f, const FrameLaunch &l, const FrameIO &io, int force_tile, cudaStream_t s)
+{
+    if (!io.params || (l.stage != kStageRender && l.stage != kStageRenderWide)) return cudaErrorInvalidValue;
+    const RenderArgs a = render_args(f, l.level, io.kind, l.stage == kStageRenderWide, force_tile);
+    const CUtensorMap &map = render_map(f, a, l.level);
+    const LayerRender *cam = f.layers > 1 || io.cams ? render_layer_cams(f, a, l.level) : nullptr;
+    const int pad = io.kind != MEAO_DEPTH_LINEAR_F32 ? 1 : 0;
+    if (!f.layer_ortho.empty()) {
+        LayerProjections proj{};
+        for (size_t i = 0; i < f.layer_ortho.size(); i++) proj.ortho[i] = f.layer_ortho[i];
+        return launch_render_ao_mixed_params_layered(map, f.tma_ok, a, f.layers, s, cam, pad, io.params->derived, proj);
+    }
+    if (f.plan.orthographic) return launch_render_ao_ortho_params_layered(map, f.tma_ok, a, f.layers, s, cam, pad, io.params->derived);
+    return launch_render_ao_params_layered(map, f.tma_ok, a, f.layers, s, cam, pad, io.params->derived);
 }
 
 // A batch (meao_render_arrays_batch / meao_render_batch): the kernel-parameter tables of its first and last launch.  arrays: layer l

@@ -364,6 +364,29 @@ constexpr int kCameraStatusWords = 6;
 // proj: the layers' projections of a frame that mixes both (nullptr: a.ortho for every layer)
 cudaError_t launch_camera_tables(const CameraTableArgs &a, const LayerProjections *proj, cudaStream_t s);
 
+// ---- device parameters (meao_bind_device_params): the render stage's reject_fadeoff and intensity derived on the device ----------------
+// {reject_fadeoff, intensity} from a device buffer {thickness_modifier, intensity}, with the host planner's arithmetic (render_params.cu),
+// ahead of the renders of every frame.  The buffer's contents are read at every launch and every graph replay.  derived: the context's
+// slot of two floats, which the *_params_layered render kernels read; an invalid block (!(thickness_modifier > 0)) leaves it as it was.
+// status: words {launches of the stage that met an invalid block, the field of the latest (1 thickness_modifier)}, zero at bind time.  A
+// frame launches the stage once; meao_profile_frame launches each kernel profile_repeats times, and each of those launches counts.
+struct RenderParamArgs {
+    const float *params;    // {thickness_modifier, intensity}
+    float *derived;         // {reject_fadeoff, intensity}
+    uint32_t *status;       // kParamStatusWords words
+};
+constexpr int kParamStatusWords = 2;
+cudaError_t launch_render_params(const RenderParamArgs &a, cudaStream_t s);
+// render_ao_layered.cu's, render_ao_ortho_layered.cu's and render_ao_mixed_layered.cu's launches with the kernels that read reject_fadeoff
+// and intensity from `derived` instead of their argument block (render_ao_kernel.inc MEAO_DEVICE_PARAMS)
+cudaError_t launch_render_ao_params_layered(const CUtensorMap &low_map, bool use_tma, const RenderArgs &a, int layers, cudaStream_t s,
+                                            const struct LayerRender *layer_cam, int layer_pad, const float *derived);
+cudaError_t launch_render_ao_ortho_params_layered(const CUtensorMap &low_map, bool use_tma, const RenderArgs &a, int layers, cudaStream_t s,
+                                                  const struct LayerRender *layer_cam, int layer_pad, const float *derived);
+cudaError_t launch_render_ao_mixed_params_layered(const CUtensorMap &low_map, bool use_tma, const RenderArgs &a, int layers, cudaStream_t s,
+                                                  const struct LayerRender *layer_cam, int layer_pad, const float *derived,
+                                                  const LayerProjections &proj);
+
 // ---- debug: synthesise a TiledDepth<k> view (reference layout [16][sh][sw], f16 bits) ----------
 cudaError_t launch_synth_tiled(const float *low, int lw, int lh, int lpitch, int sw, int sh, float pad,
                                __half *out, cudaStream_t s);
@@ -488,6 +511,12 @@ inline const KernelUnit *const kMixedKernelUnits[] = {&kPrepareDepthMixedLayered
 extern const KernelUnit kCameraTablesUnit;
 #ifndef MEAO_EMULATE
 inline const KernelUnit *const kCameraKernelUnits[] = {&kCameraTablesUnit};
+#endif
+// The device-parameter units (build.py PARAM_SOURCES), loaded eagerly like the others and kept out of the emulator's unit list the same way.
+extern const KernelUnit kRenderParamsUnit, kRenderAoParamsLayeredUnit, kRenderAoOrthoParamsLayeredUnit, kRenderAoMixedParamsLayeredUnit;
+#ifndef MEAO_EMULATE
+inline const KernelUnit *const kParamKernelUnits[] = {&kRenderParamsUnit, &kRenderAoParamsLayeredUnit, &kRenderAoOrthoParamsLayeredUnit,
+                                                      &kRenderAoMixedParamsLayeredUnit};
 #endif
 
 // ---- halo pack / unpack: row blocks of pitched buffers <-> contiguous staging, one launch ------

@@ -59,9 +59,10 @@ struct SizeState : FrameState {
     int slot = 0;                           // the arena slot of this size's camera tables (FrameState::layer_zb / layer_ren)
     bool table_pending = false;             // the slot's tables are not written yet: the next frame writes them on its own stream
     uint64_t plan_gen = 0;                  // the frame-constant generation (MeaoCtx::consts_gen) this size's plan was built at
-    // a host camera changed while a device camera buffer was bound (note_camera_change): the change moved no generation, so this
-    // size's layer_consts still hold the older host cameras, which the constant getters describe -- they plan it again first
-    bool host_cams_stale = false;
+    // a host camera changed while a device camera buffer was bound (note_camera_change), or a host thickness_modifier / intensity while a
+    // device parameter buffer was (meao_set_params): the change moved no generation, so this size's plan still holds the older host
+    // values, which the constant getters describe -- they plan it again first
+    bool host_consts_stale = false;
 };
 
 }  // namespace
@@ -104,6 +105,10 @@ struct MeaoCtx : SizeState {
     // status words, a small allocation of their own made at bind time (nullptr on a plan-only context).
     DeviceCameras cams;
     int cams_capacity = 0;
+    // meao_bind_device_params: the bound buffer (dev_params.params, nullptr: none).  A structural input: the frames run the parameter
+    // stage (frame_record.h frame_schedule) and take the *_params_layered renders at every layer count.  dev_params.derived / .status: the
+    // derived slot and the kernel's status words, one small allocation made at bind time (nullptr on a plan-only context).
+    RenderParamArgs dev_params{};
     bool plan_dirty = true;                 // a structural input changed: the next frame re-plans (replan)
     // Frame constants (include/meao.h): bumped by every change of MeaoParams or of a camera that keeps the Z direction.  A size whose
     // plan_gen is older re-plans its constants on the host (refresh_constants); a graph captured at an older one re-targets (launch_cached).
@@ -162,11 +167,13 @@ struct MeaoCtx : SizeState {
         const void *table = nullptr;
         uint64_t proj = 0;                  // FrameState::proj_key: the layers' projections the graph was recorded with
         const void *cams = nullptr;         // the device camera buffer the graph's camera stage reads (nullptr: none)
+        const void *params = nullptr;       // the device parameter buffer the graph's parameter stage reads (nullptr: none)
         bool operator<(const GraphKey &o) const {
         for (int i = 0; i < 4; i++) if (p[i] != o.p[i]) return p[i] < o.p[i];
         if (kind != o.kind) return kind < o.kind;
         if (proj != o.proj) return proj < o.proj;
         if (cams != o.cams) return cams < o.cams;
+        if (params != o.params) return params < o.params;
         for (int i = 0; i < 4; i++) if (pitch[i] != o.pitch[i]) return pitch[i] < o.pitch[i];
         for (int i = 0; i < 4; i++) if (size[i] != o.size[i]) return size[i] < o.size[i];
         if (table != o.table) return table < o.table;
@@ -234,11 +241,19 @@ int refuse_device_cameras_band(MeaoCtx *c, const char *what)
     return fail(c, MEAO_ERR_UNSUPPORTED, "%s: row bands and the halo exchange are not supported while a device camera buffer is bound "
                 "(meao_bind_device_cameras)", what);
 }
+// And a bound device parameter buffer: the band paths run the single-image kernels, which read reject_fadeoff and intensity from their
+// arguments.
+int refuse_device_params_band(MeaoCtx *c, const char *what)
+{
+    return fail(c, MEAO_ERR_UNSUPPORTED, "%s: row bands and the halo exchange are not supported while a device parameter buffer is bound "
+                "(meao_bind_device_params)", what);
+}
 #define BAND_GUARD(c, what) do { if ((c) && (c)->layers > 1) return refuse_layered((c), (what)); \
     if ((c) && ((c)->res_w > 0 || (c)->res_layers > 0)) return refuse_reserved((c), (what)); \
     if ((c) && (c)->projection != MEAO_PROJECTION_PERSPECTIVE) return refuse_ortho_band((c), (what)); \
     if ((c) && (c)->layer_proj_ortho > 0) return refuse_ortho_layer_band((c), (what)); \
-    if ((c) && (c)->cams.cams) return refuse_device_cameras_band((c), (what)); } while (0)
+    if ((c) && (c)->cams.cams) return refuse_device_cameras_band((c), (what)); \
+    if ((c) && (c)->dev_params.params) return refuse_device_params_band((c), (what)); } while (0)
 #define CUDA_TRY(c, expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) \
     return fail((c), MEAO_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); } while (0)
 
@@ -269,8 +284,8 @@ inline int ctx_reversed_z(const MeaoCtx *c) { return c->layer_cams.empty() ? c->
 void note_camera_change(MeaoCtx *c, int old_reversed_z, int new_reversed_z)
 {
     if (c->cams.cams && old_reversed_z == new_reversed_z) {
-        c->host_cams_stale = true;
-        for (auto &slot : c->size_slots) slot.s.host_cams_stale = true;
+        c->host_consts_stale = true;
+        for (auto &slot : c->size_slots) slot.s.host_consts_stale = true;
         return;
     }
     c->frame_gen++;
@@ -381,7 +396,7 @@ void build_plan(MeaoCtx *c)
     }
     c->plan_dirty = false;
     c->plan_gen = c->consts_gen;
-    c->host_cams_stale = false;
+    c->host_consts_stale = false;
 }
 
 // Caller must have made c->device current (ensure_ready / meao_resize / meao_destroy do).
@@ -726,10 +741,14 @@ int forced_render_tile()
 // goes through record_downsample, which checks the depth kind first.
 int record_launch(MeaoCtx *c, const FrameLaunch &l, const FrameIO &io, cudaStream_t s)
 {
-    static const char *nvtx[5] = {"meao::prepare_depth", "meao::render_ao", "meao::render_ao_wide", "meao::blur_upsample", "meao::camera_tables"};
+    static const char *nvtx[6] = {"meao::prepare_depth", "meao::render_ao", "meao::render_ao_wide", "meao::blur_upsample", "meao::camera_tables",
+                                  "meao::render_params"};
     if (l.stage == kStageUpsample && l.level == 1 && !io.batch) c->last_out = io.aio ? const_cast<void *>(io.aio->ao_array) : io.ao;
     NvtxRange nv(nvtx[l.stage]);
+    const bool render = l.stage == kStageRender || l.stage == kStageRenderWide;
     if (l.stage == kStageCamera) CUDA_TRY(c, io.cams ? launch_cameras(*c, *io.cams, s) : cudaErrorInvalidValue);
+    else if (l.stage == kStageParams) CUDA_TRY(c, io.params ? launch_render_params(*io.params, s) : cudaErrorInvalidValue);
+    else if (io.params && render) CUDA_TRY(c, launch_render_params_entry(*c, l, io, forced_render_tile(), s));
     else if (io.batch) CUDA_TRY(c, launch_entry_batch(*c, l, io, forced_render_tile(), s));
     else if (!c->layer_ortho.empty()) CUDA_TRY(c, launch_entry_mixed(*c, l, io, forced_render_tile(), s));
     else CUDA_TRY(c, c->plan.orthographic ? launch_entry_ortho(*c, l, io, forced_render_tile(), s) : launch_entry_views(*c, l, io, forced_render_tile(), s));
@@ -744,6 +763,7 @@ FrameIO frame_io(MeaoCtx *c, const void *depth, int kind, void *ao_out, bool fus
     FrameIO io;
     io.kind = kind; io.depth = depth_in(*c, depth, kind, vp); io.low_only = io.fused = fused; io.ao = ao_out; io.vp = vp;
     io.cams = c->cams.cams ? &c->cams : nullptr;
+    io.params = c->dev_params.params ? &c->dev_params : nullptr;
     return io;
 }
 
@@ -774,6 +794,12 @@ int record_cameras(MeaoCtx *c, cudaStream_t s)
     if (!c->cams.cams) return 0;
     return record_launch(c, FrameLaunch{kStageCamera, 0, 0, -1, kPdlNever}, frame_io(c, nullptr, c->last_kind, nullptr, false), s);
 }
+// The parameter stage alone (a bound device parameter buffer), ahead of a stage call's prepare
+int record_params(MeaoCtx *c, cudaStream_t s)
+{
+    if (!c->dev_params.params) return 0;
+    return record_launch(c, FrameLaunch{kStageParams, 0, 0, -1, kPdlNever}, frame_io(c, nullptr, c->last_kind, nullptr, false), s);
+}
 // PushRenderCommands, AO.cs:660-748.  wide = false: the call AmbientOcclusion.cs makes (tiled source, kernel main_interleaved);
 // wide = true: the same recorder for the non-tiled source LowDepth<k> (kernel main) -> HighQuality<k>.
 int record_render(MeaoCtx *c, int k, int kind, cudaStream_t s, bool wide = false)
@@ -797,7 +823,7 @@ struct PdlScope { bool prev; explicit PdlScope(bool on) : prev(g_launch_pdl) { g
 // resources that the neighbour band's kernels may need: see DESIGN.md 4), so the first launch goes without PDL.
 int record_frame_dag(MeaoCtx *c, const FrameIO &io, cudaStream_t s, size_t first, int pdl, bool after_exchange = false)
 {
-    const std::vector<FrameLaunch> sched = frame_schedule(c->plan.variants, c->cams.cams != nullptr);
+    const std::vector<FrameLaunch> sched = frame_schedule(c->plan.variants, c->cams.cams != nullptr, c->dev_params.params != nullptr);
     const cudaStream_t st[4] = {s, c->branch[0], c->branch[1], c->branch[2]};
     std::vector<int> ev(sched.size(), -1);          // the event (of c->ev) recorded after launch i, if one waits for it: at most 4
     int nev = 0;
@@ -822,7 +848,7 @@ int record_frame_dag(MeaoCtx *c, const FrameIO &io, cudaStream_t s, size_t first
 // pair around every launch (meao_profile_frame), each launched profile_repeats times.
 int record_frame(MeaoCtx *c, const FrameIO &io, cudaStream_t s, size_t first, bool profile)
 {
-    const std::vector<FrameLaunch> sched = frame_schedule(c->plan.variants, c->cams.cams != nullptr);
+    const std::vector<FrameLaunch> sched = frame_schedule(c->plan.variants, c->cams.cams != nullptr, c->dev_params.params != nullptr);
     std::vector<cudaEvent_t> ev;
     auto mark = [&]() { if (profile) { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, s); ev.push_back(e); } };
     const int reps = profile ? c->profile_repeats : 1;         // every kernel is idempotent (out of place), so repeating it is harmless
@@ -944,6 +970,7 @@ int meao_create(const MeaoDeviceCfg *cfg, MeaoCtx **out)
             for (const KernelUnit *u : kBatchKernelUnits) u->walk(&pe);
             for (const KernelUnit *u : kMixedKernelUnits) u->walk(&pe);
             for (const KernelUnit *u : kCameraKernelUnits) u->walk(&pe);
+            for (const KernelUnit *u : kParamKernelUnits) u->walk(&pe);
             if (pe != cudaSuccess) { cudaGetLastError(); meao_destroy(c); return fail(nullptr, MEAO_ERR_CUDA, "loading the kernels failed: %s", cudaGetErrorString(pe)); }
             preloaded[dev] = true;
         }
@@ -978,6 +1005,7 @@ void meao_destroy(MeaoCtx *c)
     if (c->compute_done) cudaEventDestroy(c->compute_done);
     if (c->host_error) cudaFreeHost(c->host_error);
     if (c->cams.status) cudaFree(c->cams.status);
+    if (c->dev_params.derived) cudaFree(c->dev_params.derived);
     delete c;
 }
 
@@ -991,8 +1019,16 @@ int meao_set_params(MeaoCtx *c, const MeaoParams *p)
                    c->params.upsample_tolerance != p->upsample_tolerance || c->params.thickness_modifier != p->thickness_modifier ||
                    c->params.intensity != p->intensity || c->params.debug != p->debug;
     if (!(p->thickness_modifier > 0.0f)) return fail(c, MEAO_ERR_INVALID, "thickness_modifier must be > 0");
+    // a bound device parameter buffer decides thickness_modifier and intensity: a change of those two alone is only recorded, for after the
+    // unbind, and the constant getters plan the host values again first
+    const bool render_only = c->dev_params.params && c->params.noise_filter_tolerance == p->noise_filter_tolerance &&
+                             c->params.blur_tolerance == p->blur_tolerance && c->params.upsample_tolerance == p->upsample_tolerance &&
+                             c->params.debug == p->debug;
     c->params = *p;
-    if (changed) { c->consts_gen++; c->frame_gen++; }   // frame constants: the next frame takes them without a re-plan
+    if (changed && render_only) {
+        c->host_consts_stale = true;
+        for (auto &slot : c->size_slots) slot.s.host_consts_stale = true;
+    } else if (changed) { c->consts_gen++; c->frame_gen++; }   // frame constants: the next frame takes them without a re-plan
     return changed ? 1 : 0;
 }
 
@@ -1574,6 +1610,7 @@ static int launch_cached(MeaoCtx *c, const MeaoCtx::GraphKey &key_in, cudaStream
     key.size[0] = c->W; key.size[1] = c->H; key.size[2] = c->slot; key.size[3] = c->layers;
     key.proj = c->proj_key;
     key.cams = c->cams.cams;
+    key.params = c->dev_params.params;
     auto it = c->graphs.find(key);
     bool retiring = false;
     if (it == c->graphs.end() || it->second.gen != c->plan_gen) {
@@ -2415,6 +2452,7 @@ int meao_stage_downsample(MeaoCtx *c, const void *depth, int32_t kind, void *str
     if (!depth) return fail(c, MEAO_ERR_INVALID, "depth is NULL");
     if (kind < MEAO_DEPTH_RAW_F32 || kind > MEAO_DEPTH_RAW_D24S8) return fail(c, MEAO_ERR_INVALID, "bad depth kind %d", kind);
     if ((rc = record_cameras(c, (cudaStream_t)stream))) return rc;      // the later stage calls read the tables it derives
+    if ((rc = record_params(c, (cudaStream_t)stream))) return rc;       // and the slot it derives
     return record_downsample(c, depth, kind, (cudaStream_t)stream);
 }
 
@@ -2525,9 +2563,10 @@ static int plan_only(MeaoCtx *c)
     if (!c || c->W <= 0) return MEAO_ERR_INVALID;
     if (c->plan_dirty) replan(c);           // the captured graphs are dropped by the next ensure_ready, on c->device
     refresh_constants(c);                   // the tables are written by the next frame, on its stream
-    // a host camera changed while a device camera buffer is bound, without moving the generation: the getters describe the host
-    // cameras, so the plan takes them now (the frames derive their tables on the device and never read these)
-    if (c->host_cams_stale) build_plan(c);
+    // a host camera changed while a device camera buffer is bound, or a host thickness_modifier / intensity while a device parameter
+    // buffer is, without moving the generation: the getters describe the host values, so the plan takes them now (the frames derive
+    // theirs on the device and never read these)
+    if (c->host_consts_stale) build_plan(c);
     return 0;
 }
 
@@ -2787,13 +2826,76 @@ int meao_device_camera_status(const MeaoCtx *cc, int32_t out4[4])
     return MEAO_OK;
 }
 
+int meao_bind_device_params(MeaoCtx *c, const float *params_dev)
+{
+    if (!c) return MEAO_ERR_INVALID;
+    if ((uintptr_t)params_dev % alignof(float)) return fail(c, MEAO_ERR_INVALID, "params_dev %p is not aligned to a float", (const void *)params_dev);
+    if (!c->plan_only && in_open_capture(c))
+        return fail(c, MEAO_ERR_UNSUPPORTED, "meao_bind_device_params synchronises the device: not while a capture that holds a frame of this context is open");
+    if (!params_dev) {
+        if (!c->dev_params.params) return 0;
+        if (!c->plan_only) {
+            CUDA_TRY(c, cudaSetDevice(c->device));
+            CUDA_TRY(c, cudaDeviceSynchronize());       // frames in flight may still write the slot and the status words
+            CUDA_TRY(c, cudaFree(c->dev_params.derived));
+        }
+        c->dev_params = RenderParamArgs{};
+        c->plan_dirty = true;           // the host parameters and the renders of the plan again: re-plan + drop the captured graphs
+        c->frame_gen++;
+        return 1;
+    }
+    if ((c->W > 0 && (c->band0 != 0 || c->band1 != c->H)) || c->peer_base[0] || c->peer_base[1])
+        return fail(c, MEAO_ERR_UNSUPPORTED, "a device parameter buffer is not supported with a row band or a neighbour connection "
+                                             "(meao_set_row_band, meao_band_connect)");
+    if (params_dev == c->dev_params.params) return 0;
+    if (!c->plan_only) {
+        CUDA_TRY(c, cudaSetDevice(c->device));
+        cudaPointerAttributes at{};
+        if (cudaPointerGetAttributes(&at, params_dev) != cudaSuccess || (at.type != cudaMemoryTypeDevice && at.type != cudaMemoryTypeManaged) ||
+            at.device != c->device) {
+            cudaGetLastError();
+            return fail(c, MEAO_ERR_INVALID, "params_dev %p is not device memory of device %d", (const void *)params_dev, c->device);
+        }
+        CUDA_TRY(c, cudaDeviceSynchronize());           // frames in flight may still read the old buffer and write the slot
+        if (!c->dev_params.derived) {
+            void *mem = nullptr;
+            CUDA_TRY(c, cudaMalloc(&mem, 2 * sizeof(float) + kParamStatusWords * sizeof(uint32_t)));
+            c->dev_params.derived = static_cast<float *>(mem);
+            c->dev_params.status = reinterpret_cast<uint32_t *>(c->dev_params.derived + 2);
+        }
+        // the slot starts at the host parameters (build_plan's arithmetic), which an invalid first block leaves in place; the status at zero
+        struct { float derived[2]; uint32_t status[kParamStatusWords]; } init = {{-1 / c->params.thickness_modifier, c->params.intensity}, {0, 0}};
+        CUDA_TRY(c, cudaMemcpy(c->dev_params.derived, &init, sizeof init, cudaMemcpyHostToDevice));
+    }
+    c->dev_params.params = params_dev;
+    c->plan_dirty = true;               // the parameter stage and the *_params_layered renders: re-plan + drop the captured graphs
+    c->frame_gen++;
+    return 1;
+}
+
+int meao_device_param_status(const MeaoCtx *cc, int32_t out4[4])
+{
+    MeaoCtx *c = const_cast<MeaoCtx *>(cc);
+    if (!c || !out4) return MEAO_ERR_INVALID;
+    if (!c->dev_params.params) return fail(c, MEAO_ERR_INVALID, "no device parameter buffer is bound (meao_bind_device_params)");
+    uint32_t w[kParamStatusWords] = {0, 0};
+    if (c->dev_params.status) {
+        CUDA_TRY(c, cudaSetDevice(c->device));
+        // a dedicated non-blocking stream, like meao_device_camera_status: never waits for (or delays) the frames in flight
+        CUDA_TRY(c, cudaMemcpyAsync(w, c->dev_params.status, sizeof w, cudaMemcpyDeviceToHost, c->slot_stream[1]));
+        CUDA_TRY(c, cudaStreamSynchronize(c->slot_stream[1]));
+    }
+    out4[0] = (int32_t)w[0]; out4[1] = (int32_t)w[1]; out4[2] = 0; out4[3] = 0;
+    return MEAO_OK;
+}
+
 int64_t meao_launch_count(const MeaoCtx *c) { return c ? c->launches : 0; }
 int64_t meao_frame_generation(const MeaoCtx *c) { return c ? c->frame_gen : MEAO_ERR_INVALID; }
 int meao_pdl_level(const MeaoCtx *c) { return c ? c->pdl_level : -1; }
 int meao_kernels_per_frame(const MeaoCtx *c)
 {
     if (!c) return (int)frame_schedule(PlanVariants()).size();
-    return (int)frame_schedule(PlanVariants(c->variants, c->hierarchy_depth), c->cams.cams != nullptr).size();     // as set: the plan may not be rebuilt yet
+    return (int)frame_schedule(PlanVariants(c->variants, c->hierarchy_depth), c->cams.cams != nullptr, c->dev_params.params != nullptr).size();     // as set: the plan may not be rebuilt yet
 }
 
 int64_t meao_algorithmic_bytes(const MeaoCtx *c, int32_t stage)

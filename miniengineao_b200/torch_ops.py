@@ -5,7 +5,8 @@ CUDA graph (include/meao.h, "frames inside a caller's graph").
 
 The operators run on AmbientOcclusion instances: `render` / `render_batch` on torch's current stream of the depth's device, the depth
 read in place through its strides (meao_render_pitched) and a new contiguous uint8 AO.  Nothing is copied or converted; the only other
-device work is the copy of a `cameras` tensor into the context's bound camera buffer.
+device work is the copy of a `cameras` tensor into the context's bound camera buffer, and of a `render_params` tensor into its bound
+parameter buffer.
 
 Cameras, chosen by the caller's input:
   - `cameras`, a CUDA float32 tensor [L, 3] of (near_clip, far_clip, tan_half_fov_h) per layer: a camera that may move every call.  The
@@ -22,6 +23,11 @@ the frame form, device, L, H, W, kind, the MeaoParams floats, reversed_z, the pr
 MeaoVariants fields, the hierarchy depth and the host camera.  A new value of any of these gets a new context, and no context is ever
 handed a new value.  The parameters are floats of the operator's schema, which Dynamo specialises on: a new intensity is a new compiled
 graph and a new context, not a per-frame knob.  Nothing is evicted; release_contexts() drops them all.
+
+Thickness and intensity that change every call: `render_params`, a CUDA float32 tensor [2] of (thickness_modifier, intensity), the
+operators' last argument.  The context binds a buffer of its own once (meao_bind_device_params) and every call copies `render_params`
+into it on the stream, as for `cameras`, so a fade runs in one compiled graph and one context.  The key then holds "device" in place of
+those two floats, and the schema floats thickness_modifier and intensity are ignored.
 
 A context is created and settled by a frame issued outside any stream capture.  torch.cuda.graph's documented warm-up and the graph
 trees' warm-up run every call eagerly first; a first call for a key inside a capture raises.  After its first frame each context's
@@ -119,11 +125,16 @@ def _f32(x: float) -> float:
 
 def context_key(form: str, device: int, layers: int, height: int, width: int, kind: str, cameras_on_device: bool,
                 camera: Optional[Sequence[float]], params: Sequence[float], reversed_z: bool, projection: int,
-                layer_projections: Optional[Sequence[int]], variants: Sequence[int], hierarchy_depth: int) -> tuple:
+                layer_projections: Optional[Sequence[int]], variants: Sequence[int], hierarchy_depth: int,
+                params_on_device: bool = False) -> tuple:
     """The cache key of a context: form ("frame" or "batch"), device ordinal, L, H, W, kind, the five MeaoParams floats, reversed_z, the
     projection and projection table, the MeaoVariants fields (single_pass_stereo, sample_exhaustively, high_quality_mask, single_scale),
-    the hierarchy depth, and the host camera (None: cameras from the bound device buffer)."""
-    return (form, int(device), int(layers), int(height), int(width), kind, tuple(_f32(p) for p in params), bool(reversed_z),
+    the hierarchy depth, and the host camera (None: cameras from the bound device buffer).  params_on_device: thickness_modifier and
+    intensity come from the bound device parameter buffer, and the key holds "device" in place of those two floats."""
+    params = tuple(_f32(p) for p in params)
+    if params_on_device:
+        params = params[:3] + ("device", "device")
+    return (form, int(device), int(layers), int(height), int(width), kind, params, bool(reversed_z),
             int(projection), None if layer_projections is None else tuple(int(p) for p in layer_projections),
             tuple(int(v) for v in variants), int(hierarchy_depth),
             "device" if cameras_on_device else tuple(_f32(c) for c in camera))
@@ -145,7 +156,8 @@ class _HostCamera(Camera):
 def _outside_graph_pools(alloc):
     """alloc() on a helper thread.  The graph trees of torch.compile route every allocation of the calling thread to their private pool
     while they warm up or record a function, and check that nothing but the function's outputs stays alive there; a context's camera
-    buffer, made by the first call for its key (a warm-up), outlives every graph, so it comes from the ordinary pool."""
+    buffer (or parameter buffer), made by the first call for its key (a warm-up), outlives every graph, so it comes from the ordinary
+    pool."""
     out = []
     t = threading.Thread(target=lambda: out.append(alloc()))
     t.start()
@@ -156,7 +168,8 @@ def _outside_graph_pools(alloc):
 
 
 class _Context:
-    """One AmbientOcclusion configured once from its key, its bound camera buffer and the generation recorded after its first frame."""
+    """One AmbientOcclusion configured once from its key, its bound camera and parameter buffers and the generation recorded after its
+    first frame."""
 
     def __init__(self, key: tuple):
         form, device, L, H, W, kind, params, reversed_z, projection, table, variants, depth, camera = key
@@ -164,6 +177,9 @@ class _Context:
         near, far, tan = (0.3, 100.0, 1.0) if camera == "device" else camera      # a valid host camera under device ones
         cam = _HostCamera(W // 2 if stereo else W, H, near, far, tan, reversed_z, bool(stereo))
         ao = AmbientOcclusion(cam, device=device)
+        params_on_device = params[3] == "device"
+        if params_on_device:
+            params = params[:3] + (1.0, 1.0)        # valid host values under device ones
         (ao.noiseFilterTolerance, ao.blurTolerance, ao.upsampleTolerance, ao.thicknessModifier, ao.intensity) = params
         ao.sampleExhaustively, ao.highQualityMask, ao.singleScale, ao.hierarchyDepth = bool(exhaustive), hq, bool(single_scale), depth
         ao.layers = L
@@ -179,6 +195,10 @@ class _Context:
         if camera == "device" and device >= 0:
             self.cameras = _outside_graph_pools(lambda: torch.empty((L, 3), dtype=torch.float32, device=f"cuda:{device}"))
             ao.deviceCameras = self.cameras
+        self.params = None
+        if params_on_device and device >= 0:
+            self.params = _outside_graph_pools(lambda: torch.tensor(params[3:], dtype=torch.float32, device=f"cuda:{device}"))
+            ao.deviceParams = self.params
         self.key, self.ao, self.form, self.kind, self.stereo = key, ao, form, kind, bool(stereo)
         self.generation = None
         self._settle()
@@ -189,13 +209,15 @@ class _Context:
             self.ao.OnPreRender()       # one draw of both eyes: single-pass stereo (AO.cs:352-355)
         self.ao.LateUpdate()
 
-    def frame(self, depths: Sequence[torch.Tensor], cameras: Optional[torch.Tensor]):
+    def frame(self, depths: Sequence[torch.Tensor], cameras: Optional[torch.Tensor], render_params: Optional[torch.Tensor] = None):
         """Issues the frame on torch's current stream and returns the new AO: a tensor, or a list for a batch."""
         capturing = torch.cuda.is_current_stream_capturing()
         if self.generation is None and capturing:
             raise RuntimeError(_WARM_UP)
         if cameras is not None:
             self.cameras.copy_(cameras)
+        if render_params is not None:
+            self.params.copy_(render_params)
         if self.stereo:
             self.ao.OnPreRender()
         linear = self.kind == "linear_f32"
@@ -232,16 +254,16 @@ def _context(key: tuple) -> _Context:
 
 
 def contexts() -> dict:
-    """The cached contexts, key -> AmbientOcclusion (context_key), for introspection: reservation(), deviceCameraStatus(),
+    """The cached contexts, key -> AmbientOcclusion (context_key), for introspection: reservation(), deviceCameraStatus(), deviceParamStatus(),
     kernels_per_frame.  Changing one of them makes its recorded frames stale and the next call raise."""
     return {k: c.ao for k, c in _CONTEXTS.items()}
 
 
 def release_contexts() -> None:
-    """Destroys every cached context and its camera buffer (after a device synchronise).  The caller's error: calling this while a
+    """Destroys every cached context and its camera and parameter buffers (after a device synchronise).  The caller's error: calling this while a
     stream capture is open, or while a CUDA graph that holds a frame of one of them is still alive (a torch.cuda.CUDAGraph, or a
     function compiled with mode="reduce-overhead" that has run the operator) -- those graphs would read and write freed memory."""
-    if any(c.cameras is not None for c in _CONTEXTS.values()):
+    if any(c.cameras is not None or c.params is not None for c in _CONTEXTS.values()):
         torch.cuda.synchronize()
     for c in _CONTEXTS.values():
         c.ao.close()
@@ -249,10 +271,19 @@ def release_contexts() -> None:
 
 
 # ---- the operators ----------------------------------------------------------------------------------------------------------------
-def _key_of(form, depth, layers, kind, cameras, camera, params, reversed_z, projection, layer_projections, variants, hierarchy_depth):
+def _key_of(form, depth, layers, kind, cameras, camera, params, reversed_z, projection, layer_projections, variants, hierarchy_depth,
+            render_params):
     return context_key(form, depth.device.index if depth.device.index is not None else torch.cuda.current_device(), layers,
                        depth.shape[-2], depth.shape[-1], kind, cameras is not None, camera, params, reversed_z, projection,
-                       layer_projections, variants, hierarchy_depth)
+                       layer_projections, variants, hierarchy_depth, render_params is not None)
+
+
+def _check_render_params(render_params: Optional[torch.Tensor], device: torch.device) -> None:
+    """render_params: None, or a float32 tensor [2] of (thickness_modifier, intensity) on the depth's device."""
+    if render_params is not None and (render_params.device != device or render_params.dtype != torch.float32
+                                      or tuple(render_params.shape) != (2,)):
+        raise ValueError(f"render_params must be a float32 tensor [2] of (thickness_modifier, intensity) on {device} (got "
+                         f"{str(render_params.dtype).replace('torch.', '')} {tuple(render_params.shape)} on {render_params.device})")
 
 
 @torch.library.custom_op("meao::ambient_occlusion", mutates_args=())
@@ -260,14 +291,17 @@ def _ambient_occlusion(depth: torch.Tensor, cameras: Optional[torch.Tensor], cam
                        noise_filter_tolerance: float = 0.0, blur_tolerance: float = -4.6, upsample_tolerance: float = -12.0,
                        thickness_modifier: float = 1.0, intensity: float = 1.0, reversed_z: bool = True, projection: int = 0,
                        layer_projections: Optional[List[int]] = None, single_pass_stereo: bool = False, sample_exhaustively: bool = False,
-                       high_quality_mask: int = 0, single_scale: bool = False, hierarchy_depth: int = 4) -> torch.Tensor:
+                       high_quality_mask: int = 0, single_scale: bool = False, hierarchy_depth: int = 4,
+                       render_params: Optional[torch.Tensor] = None) -> torch.Tensor:
     L = _frame_layers(depth)
     _check_inputs([depth], L, cameras, camera, kind, projection, layer_projections, single_pass_stereo, high_quality_mask, hierarchy_depth,
                   batch=False)
+    _check_render_params(render_params, depth.device)
     key = _key_of("frame", depth, L, kind, cameras, camera,
                   (noise_filter_tolerance, blur_tolerance, upsample_tolerance, thickness_modifier, intensity), reversed_z, projection,
-                  layer_projections, (single_pass_stereo, sample_exhaustively, high_quality_mask, single_scale), hierarchy_depth)
-    return _context(key).frame([depth], cameras)
+                  layer_projections, (single_pass_stereo, sample_exhaustively, high_quality_mask, single_scale), hierarchy_depth,
+                  render_params)
+    return _context(key).frame([depth], cameras, render_params)
 
 
 def _frame_layers(depth: torch.Tensor) -> int:
@@ -279,10 +313,11 @@ def _frame_layers(depth: torch.Tensor) -> int:
 @_ambient_occlusion.register_fake
 def _(depth, cameras, camera, kind, noise_filter_tolerance=0.0, blur_tolerance=-4.6, upsample_tolerance=-12.0, thickness_modifier=1.0,
       intensity=1.0, reversed_z=True, projection=0, layer_projections=None, single_pass_stereo=False, sample_exhaustively=False,
-      high_quality_mask=0, single_scale=False, hierarchy_depth=4):
+      high_quality_mask=0, single_scale=False, hierarchy_depth=4, render_params=None):
     L = _frame_layers(depth)
     _check_inputs([depth], L, cameras, camera, kind, projection, layer_projections, single_pass_stereo, high_quality_mask, hierarchy_depth,
                   batch=False)
+    _check_render_params(render_params, depth.device)
     return torch.empty(depth.shape, dtype=torch.uint8, device=depth.device)
 
 
@@ -292,14 +327,16 @@ def _ambient_occlusion_batch(depths: List[torch.Tensor], cameras: Optional[torch
                              thickness_modifier: float = 1.0, intensity: float = 1.0, reversed_z: bool = True, projection: int = 0,
                              layer_projections: Optional[List[int]] = None, single_pass_stereo: bool = False,
                              sample_exhaustively: bool = False, high_quality_mask: int = 0, single_scale: bool = False,
-                             hierarchy_depth: int = 4) -> List[torch.Tensor]:
+                             hierarchy_depth: int = 4, render_params: Optional[torch.Tensor] = None) -> List[torch.Tensor]:
     _check_batch(depths)
     _check_inputs(depths, len(depths), cameras, camera, kind, projection, layer_projections, single_pass_stereo, high_quality_mask,
                   hierarchy_depth, batch=True)
+    _check_render_params(render_params, depths[0].device)
     key = _key_of("batch", depths[0], len(depths), kind, cameras, camera,
                   (noise_filter_tolerance, blur_tolerance, upsample_tolerance, thickness_modifier, intensity), reversed_z, projection,
-                  layer_projections, (single_pass_stereo, sample_exhaustively, high_quality_mask, single_scale), hierarchy_depth)
-    return _context(key).frame(depths, cameras)
+                  layer_projections, (single_pass_stereo, sample_exhaustively, high_quality_mask, single_scale), hierarchy_depth,
+                  render_params)
+    return _context(key).frame(depths, cameras, render_params)
 
 
 def _check_batch(depths) -> None:
@@ -313,10 +350,11 @@ def _check_batch(depths) -> None:
 @_ambient_occlusion_batch.register_fake
 def _(depths, cameras, camera, kind, noise_filter_tolerance=0.0, blur_tolerance=-4.6, upsample_tolerance=-12.0, thickness_modifier=1.0,
       intensity=1.0, reversed_z=True, projection=0, layer_projections=None, single_pass_stereo=False, sample_exhaustively=False,
-      high_quality_mask=0, single_scale=False, hierarchy_depth=4):
+      high_quality_mask=0, single_scale=False, hierarchy_depth=4, render_params=None):
     _check_batch(depths)
     _check_inputs(depths, len(depths), cameras, camera, kind, projection, layer_projections, single_pass_stereo, high_quality_mask,
                   hierarchy_depth, batch=True)
+    _check_render_params(render_params, depths[0].device)
     return [torch.empty(d.shape, dtype=torch.uint8, device=d.device) for d in depths]
 
 
@@ -347,17 +385,18 @@ def ambient_occlusion(depth: torch.Tensor, cameras: Optional[torch.Tensor] = Non
                       upsample_tolerance: float = -12.0, thickness_modifier: float = 1.0, intensity: float = 1.0, reversed_z: bool = True,
                       projection: Union[Projection, Sequence[Projection]] = "perspective", single_pass_stereo: bool = False,
                       sample_exhaustively: bool = False, high_quality_mask: int = 0, single_scale: bool = False,
-                      hierarchy_depth: int = 4) -> torch.Tensor:
+                      hierarchy_depth: int = 4, render_params: Optional[torch.Tensor] = None) -> torch.Tensor:
     """The AO of one frame (meao::ambient_occlusion): depth [H, W] or [L, H, W] on a CUDA device, of `kind` "raw_f32" / "linear_f32"
     (float32), "d16" (uint16 D16_UNORM codes) or "d24s8" (int32 / uint32 D24_UNORM_S8_UINT words), read in place through its strides
     (last stride 1).  Returns a new contiguous uint8 tensor of the same shape.  Give `cameras` (CUDA float32 [L, 3] of near_clip,
     far_clip, tan_half_fov_h; may change every call) or `camera` (one such triple, fixed).  projection: "perspective", "orthographic",
     or a list with one per layer.  The other keywords are the MeaoParams floats, the Z direction, the MeaoVariants fields and the
-    hierarchy depth, with the library's defaults.  See the module docstring for how contexts are cached."""
+    hierarchy depth, with the library's defaults.  render_params: a CUDA float32 tensor [2] of (thickness_modifier, intensity) that may
+    change every call; the two keywords are then ignored.  See the module docstring for how contexts are cached."""
     proj, table = _projection_args(projection)
     return torch.ops.meao.ambient_occlusion(depth, cameras, _camera_arg(camera), kind, noise_filter_tolerance, blur_tolerance,
                                             upsample_tolerance, thickness_modifier, intensity, reversed_z, proj, table, single_pass_stereo,
-                                            sample_exhaustively, high_quality_mask, single_scale, hierarchy_depth)
+                                            sample_exhaustively, high_quality_mask, single_scale, hierarchy_depth, render_params)
 
 
 def ambient_occlusion_batch(depths: Sequence[torch.Tensor], cameras: Optional[torch.Tensor] = None,
@@ -366,7 +405,7 @@ def ambient_occlusion_batch(depths: Sequence[torch.Tensor], cameras: Optional[to
                             intensity: float = 1.0, reversed_z: bool = True,
                             projection: Union[Projection, Sequence[Projection]] = "perspective", single_pass_stereo: bool = False,
                             sample_exhaustively: bool = False, high_quality_mask: int = 0, single_scale: bool = False,
-                            hierarchy_depth: int = 4) -> List[torch.Tensor]:
+                            hierarchy_depth: int = 4, render_params: Optional[torch.Tensor] = None) -> List[torch.Tensor]:
     """The AO of a list of [H, W] depths, one layer each, in one layered frame (meao::ambient_occlusion_batch, meao_render_batch): each
     with its own row stride, all of one size, dtype and device; 1..MEAO_MAX_BATCH of them.  Returns one new uint8 [H, W] tensor per
     depth.  The other arguments as ambient_occlusion, with L = len(depths); a per-layer projection list may not hold an orthographic
@@ -375,4 +414,4 @@ def ambient_occlusion_batch(depths: Sequence[torch.Tensor], cameras: Optional[to
     return torch.ops.meao.ambient_occlusion_batch(list(depths), cameras, _camera_arg(camera), kind, noise_filter_tolerance,
                                                   blur_tolerance, upsample_tolerance, thickness_modifier, intensity, reversed_z, proj, table,
                                                   single_pass_stereo, sample_exhaustively, high_quality_mask, single_scale,
-                                                  hierarchy_depth)
+                                                  hierarchy_depth, render_params)
